@@ -1,5 +1,5 @@
 """adaptive_voice_conversion_b200 -- the AdaIN-VC (arXiv 1904.05742) forward/backward hot
-path as hand-written sm_100a CUDA behind the reference's own Python API.
+path as hand-written sm_90a (H100) CUDA behind the reference's own Python API.
 
 Public surface (mirrors the reference repo's modules):
     model.AE, solver.Solver, inference.Inferencer, utils.cc

@@ -9,20 +9,20 @@ import ctypes as C
 import os
 
 _PKG = os.path.dirname(os.path.abspath(__file__))
-# engine.py: fused speaker dense stack / batched AdaIN affine layers (csrc/dense_fused.cu); ON since
-# the B200 validation run (42 513 -> 45 462 seg/s); AVC_FUSED_DENSE=0 = one launch per nn.Linear
+# engine.py: fused speaker dense stack / batched AdaIN affine layers (csrc/dense_fused.cu);
+# AVC_FUSED_DENSE=0 = one launch per nn.Linear
 DEFAULT_FUSED_DENSE = True
-# engine.py: conv weight gradients accumulated in place with vector atomics + ONE flush launch per
-# backward pass (csrc/wgrad_tc.cu, ATOMIC).  ON since the round-2 B200 validation (tests green, 45 649 ->
-# 49 658 seg/s); AVC_WGRAD_ACC=0 = per-slice partials + deterministic reduction
-DEFAULT_WGRAD_ACC = True
+# engine.py: AVC_WGRAD_ACC=1 accumulates conv weight gradients in place with vector atomics + ONE flush launch per
+# backward pass (csrc/wgrad_tc.cu, ATOMIC); off by default: the atomics' summation order varies from run to run, and
+# Adam turns that rounding noise into different trajectories.  Default = per-slice partials + deterministic reduction
+DEFAULT_WGRAD_ACC = False
 # engine.py: reflect-padding / residual adjoint inside the data-gradient conv's epilogue (AVC_F_FOLD, 30
-# avc_fold_add_fwd launches fewer per step).  ON since the round-2 validation (tests green, +0.5 %)
+# avc_fold_add_fwd launches fewer per step)
 DEFAULT_FOLD_FUSED = True
 # engine.py: the data-gradient conv of a block also runs the UPSTREAM block's InstanceNorm / AdaIN / ReLU backward in
 # its epilogue (AVC_F_NORMBWD, persistent kernel): 27 avc_norm_bwd launches and their dy/dc round trips fewer per step.
-# Validated on the B200 (tests/test_gpu_normbwd_fused.py, all model tests green) but SLOWER (47 853 vs 49 697 seg/s):
-# the conv kernel is bound by its 8 epilogue warps, the stand-alone avc_norm_bwd runs at full occupancy -> opt-in
+# Correct (tests/test_gpu_normbwd_fused.py) but it lengthens the conv kernel's epilogue while the stand-alone
+# avc_norm_bwd runs at full occupancy -> opt-in
 DEFAULT_NORM_BWD_FUSED = False
 LIB_PATH = os.environ.get("AVC_LIB", os.path.join(_PKG, "libavc_b200.so"))
 
@@ -52,6 +52,7 @@ class ConvDesc(C.Structure):
         ("dy", _fp), ("dy_bstride", C.c_int64),
         ("dc", _fp), ("dcond", _fp), ("dcond_bstride", C.c_int64), ("dbias", _fp),
         ("w_tc", _fp), ("flags", C.c_int32), ("out_tstride", C.c_int32), ("out_toff", C.c_int32), ("out_T", C.c_int32),
+        ("dbias_part", _fp),
     ]
 
 
@@ -103,6 +104,7 @@ class DenseStackDesc(C.Structure):
 
 
 LINEAR_BATCH_MAX = 16
+VAE_PARTIALS = 2112   # AVC_VAE_PARTIALS
 
 
 class LinearBatchDesc(C.Structure):
@@ -154,7 +156,7 @@ PROTOTYPES = {
     "avc_linear_batch_dw": (_i, [C.POINTER(LinearBatchDesc), _p]),
     "avc_reparam_fwd": (_i, [_p, _p, _p, _p, _p, _p, _i, _i, _i, _p]),
     "avc_reparam_bwd": (_i, [_p, _p, _p, _p, _p, _p, _p, _i, _i, _i, _p]),
-    "avc_vae_loss": (_i, [_p, _p, _i64, _p, _p, _i64, _p, _p, _p, _p, _p, _p]),
+    "avc_vae_loss": (_i, [_p, _p, _i64, _p, _p, _i64, _p, _p, _p, _p, _p, _p, _p]),
     "avc_sqnorm": (_i, [_p, _i64, _p, _p, _p]),
     "avc_adam_step": (_i, [_p, _p, _p, _p, _p, _i64, _p, _p, _p, _p]),
     "avc_fill_zero": (_i, [_p, _i64, _p]),

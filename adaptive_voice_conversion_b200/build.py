@@ -1,11 +1,11 @@
-"""Build libavc_b200.so (sm_100a) in-tree with nvcc.
+"""Build libavc_b200.so (sm_90a, H100) in-tree with nvcc.
 
     python -m adaptive_voice_conversion_b200.build [--force] [--verbose]
 
 Every .cu under csrc/ is compiled to an object file (in parallel) with
-``-gencode arch=compute_100a,code=sm_100a -lineinfo -O3`` and linked into
+``-gencode arch=compute_90a,code=sm_90a -lineinfo -O3`` and linked into
 ``adaptive_voice_conversion_b200/libavc_b200.so``.  nvcc cross-compiles, so this works in
-the GPU-less authoring container; the .so travels to the GPU box with the tree.
+a machine without a GPU.
 
 Safe under ``torchrun``: the build takes an exclusive file lock (the other ranks wait, then find the
 stamp up to date) and every output is written to a temporary name and renamed into place, so no
@@ -30,7 +30,7 @@ LIB = os.path.join(PKG, "libavc_b200.so")
 VARIANTS = {  # name -> (library, object dir, extra nvcc flags)
     "default": (LIB, OBJ, []),
 }
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 FLAGS = ["-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC"]
 
 

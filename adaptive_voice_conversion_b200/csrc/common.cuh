@@ -1,4 +1,4 @@
-// Shared device/host helpers for libavc_b200 (sm_100a only).
+// Shared device/host helpers for libavc_b200 (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -6,8 +6,8 @@
 
 #include "../../include/avc_b200.h"
 
-#if defined(__CUDA_ARCH__) && (__CUDA_ARCH__ < 1000)
-#error "libavc_b200 is written for sm_100a (B200) only"
+#if defined(__CUDA_ARCH__) && (__CUDA_ARCH__ != 900)
+#error "libavc_b200 is written for sm_90a (H100) only"
 #endif
 
 namespace avc {

@@ -1,4 +1,4 @@
-// Fused ConvBlock forward, fp32 FFMA path (exact-fp32 twin of the tcgen05 path).
+// Fused ConvBlock forward, fp32 FFMA path (exact-fp32 twin of the tensor-core path).
 //
 //   reflect/zero pad -> Conv1d(K, stride) -> [pixel shuffle] -> [InstanceNorm over T]
 //   -> [AdaIN gamma/beta] -> [ReLU] -> [+ residual (same | avg-pool2 | nearest-up2)] -> [* mask]

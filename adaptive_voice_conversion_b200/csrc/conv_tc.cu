@@ -1,21 +1,23 @@
-// Fused ConvBlock forward on the 5th-gen tensor cores (tcgen05, TF32 inputs / fp32 accumulate).
+// Fused ConvBlock forward on the tensor cores (wgmma m64nNk8 tf32, fp32 accumulate), one tile per CTA.
 //
 // Same contract as conv_simt.cu (reflect/zero pad -> Conv1d -> [pixel shuffle] ->
 // [InstanceNorm] -> [AdaIN] -> [ReLU] -> [+residual] -> [*mask]); replaces the same reference
 // ops (model.py:21-32, 52-59, 77-83, 237-250, 309-320, 354-369) and, with the DGRAD pack and
-// zero padding, autograd's conv data gradient.
+// zero padding, autograd's conv data gradient.  The persistent kernel (conv_tc2.cu) runs every
+// shape it plans; this one takes the rest up to TC_MAX_COLS columns per CTA.
 //
 // Formulation (no im2col): per sample, D[co][t] = sum_tap sum_ci W_tap[co][ci] * X[ci][t+tap].
 //   * A operand = weights of one tap, K-major [ci/4][co][4] (no swizzle): 128 co rows x 16 ci.
 //   * B operand = the input tile in its HBM layout [ci/4][row][4] staged ONCE per 16-channel
 //     slab; the taps are the same tile at descriptor start + tap*16 bytes (row shift), so one
 //     staged tile feeds all K taps.  Reflect / zero halos are patched in shared memory.
-//   * D = 128 lanes (co) x Npad columns (time) per sample in TMEM; G samples per CTA share every
-//     weight stage.  Epilogue: thread <-> lane <-> output channel, so the InstanceNorm
-//     statistics of a (sample, channel) are a per-thread reduction over TMEM columns.
+//   * D = 128 rows (co) x npad columns (time) per sample, in the registers of two consumer
+//     warpgroups (64 rows each); after the main loop they are written to a shared-memory image
+//     over the stage ring, and the epilogue reads it with thread <-> row <-> output channel, so the
+//     InstanceNorm statistics of a (sample, channel) are a per-thread reduction over its row.
 // Pipeline: warp 0 = bulk-copy (TMA) producer, warps 1+3 = halo patch + round-to-nearest TF32
 // of the staged inputs (the tensor core truncates; rounding here keeps the path unbiased),
-// warp 2 = MMA issuer; all four warps run the epilogue (one TMEM lane quarter each).
+// warps 4-11 = the two wgmma warpgroups; all 16 warps run the epilogue.
 #include "common.cuh"
 #include "tc_common.cuh"
 
@@ -28,10 +30,11 @@ int conv_block_tc2_launch(const avc_conv_desc* d, int* status, void* stream);  /
 constexpr int TC_SLAB = 16;          // input channels per pipeline stage (2 MMA K-steps)
 constexpr int TC_WTAP_BYTES = 8192;  // one tap of one slab: 4 chunks x 128 co x 16 B
 constexpr int TC_MAX_STAGES = 4;
+constexpr int TC_MAX_COLS = 128;   // accumulator columns of a CTA (G samples x npad): 64 registers per consumer thread
 
 struct TcArgs {
   avc_conv_desc d;
-  int G, npad, rows, nslab, nstage, ncols;  // samples/CTA, padded cols/sample, smem rows/sample, Cin/16, ring depth, TMEM cols
+  int G, npad, rows, nslab, nstage;  // samples/CTA, padded cols/sample, smem rows/sample, Cin/16, ring depth
   uint32_t stage_bytes, w_bytes;
   int* status;
   long long* dbg;  // optional: per-CTA phase timestamps (tools/diag_phases.py)
@@ -60,49 +63,76 @@ __device__ __forceinline__ void quad_transpose(float& a0, float& a1, float& a2, 
   }
 }
 
-// All MMAs of one 16-channel slab: 2 k-steps x nsamp samples x K taps; taps j = 0..K-1 of one
-// (k-step, sample) accumulate into the same TMEM columns.  Called by the whole (converged) issuer
-// warp with warp-uniform arguments.
-template <int KT>
-__device__ __forceinline__ void issue_slab(uint32_t tb, uint32_t a_lo0, uint32_t b_lo0, uint32_t ks_b, uint32_t d_hi, uint32_t idesc,
-                                           uint32_t slab, int nsamp, int rows, int npad, int K) {
-  const int n = KT ? KT : K;
+// Main loop of one consumer warpgroup (accumulator rows 64 wg .. 64 wg + 63): per 16-channel slab, 2 k-steps x nsamp
+// samples x K taps of wgmma m64nNk8 (N = npad), taps j = 0..K-1 of one (k-step, sample) accumulating into the same
+// registers; sample g owns acc[g * N / 2, (g + 1) * N / 2).  Then the accumulators go to the shared-memory image
+// img[row][col] (row pitch `pitch` floats, col = g * npad + time column) that the epilogue reads.
+template <int N>
+__device__ __forceinline__ bool tc_mainloop(const TcArgs& a, uint32_t smem0, uint64_t* bar_ready, uint64_t* bar_empty, int nsamp, int wg,
+                                            int wt, float* img, int pitch) {
+  constexpr int GMAX = TC_MAX_COLS / N;
+  float acc[GMAX * N / 2];
+  const int K = a.d.K;
+  const uint32_t x_chunk_bytes = (uint32_t)(a.G * a.rows) * 16u;
+  const uint32_t ks_b = 2u * (x_chunk_bytes >> 4);
+  const uint32_t d_hi = tc::sdesc_hi(128);
+  for (int i = 0; i < a.nslab; ++i) {
+    const int s = i % a.nstage;
+    const uint32_t ph = (uint32_t)(i / a.nstage) & 1u;
+    if (!__all_sync(0xffffffffu, tc::mbar_wait(&bar_ready[s], ph, a.status, 3))) return false;
+    const uint32_t sw = smem0 + (uint32_t)s * a.stage_bytes;
+    const uint32_t a_lo0 = tc::sdesc_lo(sw + (uint32_t)wg * 1024u, 2048), b_lo0 = tc::sdesc_lo(sw + a.w_bytes, x_chunk_bytes);
+    tc::wgmma_fence();
 #pragma unroll
-  for (int ks = 0; ks < 2; ++ks) {
-    const uint64_t a_ks = tc::sdesc64(a_lo0 + (uint32_t)ks * (4096 >> 4), d_hi);
-    uint64_t b_g = tc::sdesc64(b_lo0 + (uint32_t)ks * ks_b, d_hi);
-    uint32_t dcol = tb;
-#pragma unroll 2
-    for (int g = 0; g < nsamp; ++g) {
-      uint64_t a_desc = a_ks, b_desc = b_g;
+    for (int ks = 0; ks < 2; ++ks) {
 #pragma unroll
-      for (int j = 0; j < n; ++j) {
-        tc::mma_tf32_elect(dcol, a_desc, b_desc, idesc, (slab | (uint32_t)ks | (uint32_t)j) ? 1u : 0u);
-        a_desc += (uint64_t)(TC_WTAP_BYTES >> 4);
-        b_desc += 1u;
+      for (int g = 0; g < GMAX; ++g) {
+        if (g >= nsamp) break;
+        uint64_t a_desc = tc::sdesc64(a_lo0 + (uint32_t)ks * (4096 >> 4), d_hi);
+        uint64_t b_desc = tc::sdesc64(b_lo0 + (uint32_t)ks * ks_b + (uint32_t)(g * a.rows), d_hi);
+        for (int j = 0; j < K; ++j) {
+          tc::wgmma_tf32<N>(acc + g * (N / 2), a_desc, b_desc, ((uint32_t)i | (uint32_t)ks | (uint32_t)j) ? 1u : 0u);
+          a_desc += (uint64_t)(TC_WTAP_BYTES >> 4);
+          b_desc += 1u;
+        }
       }
-      b_g += (uint32_t)rows;
-      dcol += (uint32_t)npad;
     }
+    tc::wgmma_commit();
+    tc::wgmma_wait<0>();
+    tc::acc_fence(acc, GMAX * N / 2);
+    if (wt == 0) tc::mbar_arrive(&bar_empty[s]);
   }
+  // the image overwrites the stage ring: both warpgroups must be done reading it
+  asm volatile("bar.sync 2, 256;" ::: "memory");
+#pragma unroll
+  for (int g = 0; g < GMAX; ++g) {
+    if (g >= nsamp) break;
+#pragma unroll
+    for (int r = 0; r < N / 2; ++r)
+      img[(size_t)(64 * wg + tc::wg_acc_row(wt, r)) * pitch + g * a.npad + tc::wg_acc_col(wt, r)] = acc[g * (N / 2) + r];
+  }
+  return true;
 }
 
-// UI (uniform issue): warp index via lane-0 broadcast + election inside the MMA asm, see issue_slab.
-// UI = false is the round-1 issue loop (ELECT + VOTEU per MMA), kept selectable with AVC_TC_ISSUE=legacy.
+// 16 consecutive accumulator columns of one row of the shared-memory image
+__device__ __forceinline__ void img_ld16(const float* p, float (&v)[16]) {
+#pragma unroll
+  for (int i = 0; i < 16; ++i) v[i] = p[i];
+}
+
+// UI: warp index via lane-0 broadcast (AVC_TC_ISSUE=legacy: plain tid >> 5).
 // FOLD (AVC_F_FOLD, plain stride-1 data-gradient convs): the epilogue applies the adjoint of the forward
 // conv's reflect padding and of its residual branch itself (what avc_fold_add_fwd does in a second pass).
 template <bool UI, bool FOLD>
 __global__ void __launch_bounds__(512, 1) conv_block_tc_kernel(const TcArgs a) {
   extern __shared__ __align__(1024) uint8_t smem[];
-  __shared__ uint64_t bar_full[TC_MAX_STAGES], bar_ready[TC_MAX_STAGES], bar_empty[TC_MAX_STAGES], bar_done;
-  __shared__ uint32_t tmem_slot;
+  __shared__ uint64_t bar_full[TC_MAX_STAGES], bar_ready[TC_MAX_STAGES], bar_empty[TC_MAX_STAGES];
   __shared__ float2 ep_stat[4][128];  // partial InstanceNorm sums of the 4 epilogue warp groups
   const avc_conv_desc& d = a.d;
   const int tid = threadIdx.x, warp = UI ? tc::warp_idx_sync() : (tid >> 5), lane = tid & 31;
   const int b0 = blockIdx.x * a.G;
   const int mtile = blockIdx.y;
   const int nsamp = min(a.G, d.B - b0);
-  const int K = d.K;
   const int xrows = a.G * a.rows;                 // rows of one chunk plane in a stage
   const uint32_t x_chunk_bytes = (uint32_t)xrows * 16u;
 
@@ -110,16 +140,13 @@ __global__ void __launch_bounds__(512, 1) conv_block_tc_kernel(const TcArgs a) {
     for (int s = 0; s < a.nstage; ++s) {
       tc::mbar_init(&bar_full[s], 1);
       tc::mbar_init(&bar_ready[s], 64);
-      tc::mbar_init(&bar_empty[s], 1);
+      tc::mbar_init(&bar_empty[s], 2);
     }
-    tc::mbar_init(&bar_done, 1);
     tc::fence_mbar_init();
   }
-  if (warp == 0) tc::tmem_alloc(&tmem_slot, (uint32_t)a.ncols);
-  tc::tc_fence_before();
   __syncthreads();
-  tc::tc_fence_after();
-  const uint32_t tbase = tmem_slot;
+  float* img = reinterpret_cast<float*>(smem);   // accumulator image, written over the stage ring after the main loop
+  const int pitch = a.G * a.npad + 1;
   bool ok = true;
   long long tm0 = 0, tm1 = 0, tm2 = 0, dbg_acc0 = 0, dbg_acc1 = 0;
   if (a.dbg && tid == 64) tm0 = clock64();
@@ -148,55 +175,17 @@ __global__ void __launch_bounds__(512, 1) conv_block_tc_kernel(const TcArgs a) {
             tc::bulk_g2s(sx + (size_t)q * x_chunk_bytes + ((size_t)g * a.rows + d.pad_left) * 16,
                          d.in + (size_t)(b0 + g) * d.in_bstride + ((size_t)(i * 4 + q) * d.Tin) * 4, (uint32_t)d.Tin * 16u, &bar_full[s]);
     }
-  } else if (warp == 2) {
-    // MMA issuer.  The WHOLE warp runs this loop converged with warp-uniform values, and one
-    // elected lane executes each tcgen05 instruction: descriptors then live in uniform registers.
-    // (Issuing from inside `if (lane == 0)` made ptxas wrap every UTCHMMA in an ELECT + 5x
-    // R2UR.BROADCAST waterfall: measured 144 cycles per MMA.)
-    const uint32_t idesc = tc::make_idesc_tf32(128, a.npad, 0, 0);
-    const uint32_t d_hi = tc::sdesc_hi(128);
-    const uint32_t tb = __shfl_sync(0xffffffffu, tbase, 0);
+  } else if (warp >= 4 && warp < 12) {
+    // two consumer warpgroups: wgmma main loop, accumulators -> shared-memory image
+    const int wg = (warp - 4) >> 2, wt = tid & 127;
     const uint32_t smem0 = tc::smem_u32(smem);
-    for (int i = 0; i < a.nslab; ++i) {
-      const int s = i % a.nstage;
-      const uint32_t ph = (uint32_t)(i / a.nstage) & 1u;
-      const long long w0 = a.dbg ? clock64() : 0;
-      ok = __all_sync(0xffffffffu, tc::mbar_wait(&bar_ready[s], ph, a.status, 3));
-      const long long w1 = a.dbg ? clock64() : 0;
-      dbg_acc0 += w1 - w0;
-      if (!ok) break;
-      tc::tc_fence_after();
-      const uint32_t sw = smem0 + (uint32_t)s * a.stage_bytes;
-      const uint32_t sx = sw + a.w_bytes;
-      const uint32_t a_lo0 = tc::sdesc_lo(sw, 2048), b_lo0 = tc::sdesc_lo(sx, x_chunk_bytes);
-      const uint32_t ks_b = 2u * (x_chunk_bytes >> 4);
-      if constexpr (UI) {
-        // loop order ks -> sample -> tap: the tap loop only advances two loop-carried 64-bit descriptors
-        // (weights: next tap block; input: one row down), ~6 uniform instructions per MMA
-        if (K == 5) issue_slab<5>(tb, a_lo0, b_lo0, ks_b, d_hi, idesc, (uint32_t)i, nsamp, a.rows, a.npad, 5);
-        else issue_slab<0>(tb, a_lo0, b_lo0, ks_b, d_hi, idesc, (uint32_t)i, nsamp, a.rows, a.npad, K);
-      } else {
-        for (int j = 0; j < K; ++j) {
-  #pragma unroll
-          for (int ks = 0; ks < 2; ++ks) {
-            const uint32_t a_lo = a_lo0 + (uint32_t)j * (TC_WTAP_BYTES >> 4) + (uint32_t)ks * (4096 >> 4);
-            uint32_t b_lo = b_lo0 + (uint32_t)ks * ks_b + (uint32_t)j;
-            uint32_t dcol = tb;
-            const uint32_t acc = (i | j | ks) ? 1u : 0u;
-            for (int g = 0; g < nsamp; ++g) {
-              if (tc::elect_one()) tc::mma_tf32_lohi(dcol, a_lo, d_hi, b_lo, d_hi, idesc, acc);
-              b_lo += (uint32_t)a.rows;
-              dcol += (uint32_t)a.npad;
-            }
-          }
-        }
-      }
-      __syncwarp();
-      if (tc::elect_one()) tc::mma_commit(&bar_empty[s]);
-      if (a.dbg) dbg_acc1 += clock64() - w1;
+    switch (a.npad) {
+#define TC_CASE(n) \
+  case n: ok = tc_mainloop<n>(a, smem0, bar_ready, bar_empty, nsamp, wg, wt, img, pitch); break;
+      TC_CASE(16) TC_CASE(32) TC_CASE(48) TC_CASE(64) TC_CASE(80) TC_CASE(96) TC_CASE(112) TC_CASE(128)
+#undef TC_CASE
+      default: ok = false;
     }
-    __syncwarp();
-    if (ok && tc::elect_one()) tc::mma_commit(&bar_done);
   } else if (warp == 1 || warp == 3) {
     // warps 1 and 3: round staged inputs to TF32 (RN) and patch the halo rows
     const int ptid = (warp == 1 ? 0 : 32) + lane;  // 0..63
@@ -246,14 +235,12 @@ __global__ void __launch_bounds__(512, 1) conv_block_tc_kernel(const TcArgs a) {
 
   // ------------------------------------------------------------------ epilogue (all warps)
   __syncwarp();
-  ok = tc::mbar_wait(&bar_done, 0, a.status, 5) && ok;
-  ok = __syncthreads_and(ok) != 0;  // block-uniform: the TMEM loads below are .sync.aligned
-  tc::tc_fence_after();
+  ok = __syncthreads_and(ok) != 0;  // the accumulator image is complete
   if (a.dbg && tid == 64) tm1 = clock64();
-  // 16 epilogue warps = 4 groups x 4 TMEM lane quarters.  A group takes one (sample, column part):
+  // 16 epilogue warps = 4 groups x 4 row quarters.  A group takes one (sample, column part):
   // with fewer than 4 samples per CTA the columns of a sample are split between groups and the
   // InstanceNorm partial sums are merged through shared memory.
-  const int etid = tid & 127, ewarp = warp & 3, egrp = warp >> 2;
+  const int etid = tid & 127, egrp = warp >> 2;
   const int co = mtile * 128 + etid;  // conv output row of this thread
   const bool co_ok = co < d.Cout;
   if (ok) {
@@ -266,11 +253,11 @@ __global__ void __launch_bounds__(512, 1) conv_block_tc_kernel(const TcArgs a) {
     const int r4 = lane & 3;             // position inside the 4-lane quad (= channel within an A4 chunk)
     const int cq = (mtile * 128 + (etid & ~3)) >> 2;  // A4 chunk of the quad's 4 conv rows
     const bool q_ok = (mtile * 128 + (etid & ~3)) < d.Cout;
-    const uint32_t lane_addr = tbase + ((uint32_t)(ewarp * 32) << 16);
+    const float* lane_addr = img + (size_t)etid * pitch;   // this thread's accumulator row
     // stride 2: the MMAs compute every input position; only even columns are conv outputs
     const int sshift = d.stride == 2 ? 1 : 0, smask = sshift;
     const int ots = d.out_tstride > 0 ? d.out_tstride : 1, oto = d.out_toff;  // out time index = t*ots + oto
-    const int ncol = d.stride == 2 ? min(a.npad, 2 * d.Tout) : d.Tout;  // TMEM columns that matter
+    const int ncol = d.stride == 2 ? min(a.npad, 2 * d.Tout) : d.Tout;  // accumulator columns that matter
     const int nsplit = nsamp >= 3 ? 1 : (nsamp == 2 ? 2 : 4);
     const int items = nsamp * nsplit, nchunk = a.npad >> 4;
     for (int it0 = 0; it0 < items; it0 += 4) {
@@ -284,7 +271,7 @@ __global__ void __launch_bounds__(512, 1) conv_block_tc_kernel(const TcArgs a) {
         float s1 = 0.f, s2 = 0.f;
         for (int c0 = cbeg; c0 < cend; c0 += 16) {
           float v[16];
-          tc::tmem_ld16(lane_addr + (uint32_t)(g * a.npad + c0), v);
+          img_ld16(lane_addr + (uint32_t)(g * a.npad + c0), v);
 #pragma unroll
           for (int i = 0; i < 16; ++i)
             if (c0 + i < ncol && ((c0 + i) & smask) == 0) {
@@ -319,19 +306,19 @@ __global__ void __launch_bounds__(512, 1) conv_block_tc_kernel(const TcArgs a) {
       if constexpr (FOLD) {
         // D holds Tout = T + pl + pr columns of the zero-padded transposed conv (dxp); the input gradient
         // is dx[t] = D[t+pl] + D[pl-t] (1 <= t <= pl) + D[2(T-1)-t+pl] (that column >= pl+T) + residual
-        // adjoint.  All mirrored columns belong to this thread's own TMEM lane.
+        // adjoint.  All mirrored columns belong to this thread's own row.
         const int fpl = (d.flags >> 8) & 0xff, fpr = (d.flags >> 16) & 0xff;
         const int Tf = d.Tout - fpl - fpr;
-        const uint32_t col0 = lane_addr + (uint32_t)(g * a.npad);
+        const float* col0 = lane_addr + g * a.npad;
         float Le[4], Re[4];
         {
           float v0[16], v1[16], v2[16];
-          tc::tmem_ld16(col0, v0);
+          img_ld16(col0, v0);
           Le[0] = v0[0]; Le[1] = v0[1]; Le[2] = v0[2]; Le[3] = v0[3];
           const int rc0 = ((fpl + Tf) >> 4) << 4, ro = fpl + Tf - rc0;   // chunk and offset of column pl+T
-          tc::tmem_ld16(col0 + (uint32_t)rc0, v1);
+          img_ld16(col0 + (uint32_t)rc0, v1);
           if (rc0 + 16 < a.npad) {
-            tc::tmem_ld16(col0 + (uint32_t)(rc0 + 16), v2);
+            img_ld16(col0 + (uint32_t)(rc0 + 16), v2);
           } else {
 #pragma unroll
             for (int i = 0; i < 16; ++i) v2[i] = 0.f;
@@ -352,7 +339,7 @@ __global__ void __launch_bounds__(512, 1) conv_block_tc_kernel(const TcArgs a) {
         const int ur = Tf - 2 + fpl;   // column that receives Re[0]; Re[e] goes to column ur - e
         for (int c0 = cbeg; c0 < cend; c0 += 16) {
           float v[16];
-          tc::tmem_ld16(col0 + (uint32_t)c0, v);
+          img_ld16(col0 + (uint32_t)c0, v);
           if (c0 == 0) {   // left halo: source column e -> target column 2*pl - e (2*pl <= 8 < 16)
 #pragma unroll
             for (int i = 0; i < 16; ++i)
@@ -412,11 +399,11 @@ __global__ void __launch_bounds__(512, 1) conv_block_tc_kernel(const TcArgs a) {
       const float* maskp = d.mask ? d.mask + (size_t)b * d.mask_bstride + ((size_t)(cn >> 2) * Tn) * 4 + (cn & 3) : nullptr;
       for (int c0 = cbeg; c0 < cend; c0 += 16) {
         float v[16];
-        tc::tmem_ld16(lane_addr + (uint32_t)(g * a.npad + c0), v);
+        img_ld16(lane_addr + (uint32_t)(g * a.npad + c0), v);
 #pragma unroll
         for (int i4 = 0; i4 < 16; i4 += 4) {
           float x0 = v[i4] + bias, x1 = v[i4 + 1] + bias, x2 = v[i4 + 2] + bias, x3 = v[i4 + 3] + bias;
-          const int tc_ = c0 + i4 + r4;  // after the quad transpose this lane owns TMEM column tc_ for 4 channels
+          const int tc_ = c0 + i4 + r4;  // after the quad transpose this lane owns column tc_ for 4 channels
           const bool t_ok = tc_ < ncol && (tc_ & smask) == 0;
           const int t = tc_ >> sshift;   // conv output time step
           if (cbase) {
@@ -485,9 +472,6 @@ __global__ void __launch_bounds__(512, 1) conv_block_tc_kernel(const TcArgs a) {
     long long* o = a.dbg + (size_t)(blockIdx.y * gridDim.x + blockIdx.x) * 12;
     o[0] = tm0; o[1] = tm1; o[2] = tm2; o[3] = 0;
   }
-  tc::tc_fence_before();
-  __syncthreads();
-  if (warp == 0) tc::tmem_dealloc(tbase, (uint32_t)a.ncols);
 }
 
 // nn.Conv1d weight [Cout][Cin][K] -> per (m-tile, 16-channel slab) blocks
@@ -588,7 +572,7 @@ extern "C" int avc_pack_conv_weight_tc(const float* w, float* packed, int Cout, 
   const int co_total = mode == AVC_PACK_FWD ? Cout : Cin, ci_total = mode == AVC_PACK_FWD ? Cin : Cout;
   const int64_t n = avc_tc_packed_floats(co_total, ci_total, K);
   int blocks = (int)cdiv64(n, 256);
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > 132 * 8) blocks = 132 * 8;
   AVC_LAUNCH(pack_weight_tc_kernel, blocks, 256, 0, (cudaStream_t)stream, w, packed, Cout, Cin, K, mode, co_total, ci_total);
   AVC_CHECK_LAUNCH("pack_conv_weight_tc");
   return AVC_OK;
@@ -624,7 +608,7 @@ extern "C" int avc_conv_block_tc(const avc_conv_desc* d, int* status, void* stre
   }
   AVC_REQUIRE(!normbwd, AVC_ERR_UNSUPPORTED, "avc_conv_block_tc: AVC_F_NORMBWD needs the persistent kernel and a one-tile shape (Tout <= 144, Cout <= 128)");
   const int ncols_full = d->stride == 2 ? 2 * d->Tout - 1 : d->Tout;  // stride 2: full-resolution columns 0 .. 2(Tout-1)
-  AVC_REQUIRE(ncols_full <= 256, AVC_ERR_UNSUPPORTED, "avc_conv_block_tc: more than 256 columns per sample");
+  AVC_REQUIRE(ncols_full <= TC_MAX_COLS, AVC_ERR_UNSUPPORTED, "avc_conv_block_tc: more than %d columns per sample", TC_MAX_COLS);
   AVC_REQUIRE(!d->res || d->res_mode != AVC_RES_NONE, AVC_ERR_INVALID, "avc_conv_block_tc: res without res_mode");
   TcArgs a;
   a.d = *d;
@@ -637,9 +621,9 @@ extern "C" int avc_conv_block_tc(const avc_conv_desc* d, int* status, void* stre
   a.nslab = d->Cin / TC_SLAB;
   a.w_bytes = (uint32_t)d->K * TC_WTAP_BYTES;
   const int mtiles = cdiv(d->Cout, 128);
-  int G = cdiv(d->B * mtiles, 148);
-  const int gmax_tmem = 512 / a.npad;
-  if (G > gmax_tmem) G = gmax_tmem;
+  int G = cdiv(d->B * mtiles, 132);
+  const int gmax_acc = TC_MAX_COLS / a.npad;
+  if (G > gmax_acc) G = gmax_acc;
   if (G < 1) G = 1;
   const int smem_max = 220 * 1024;
   auto stage_bytes = [&](int g) { return (uint32_t)(a.w_bytes + 4 * g * a.rows * 16); };
@@ -650,10 +634,8 @@ extern "C" int avc_conv_block_tc(const avc_conv_desc* d, int* status, void* stre
   a.nstage = smem_max / (int)a.stage_bytes;
   if (a.nstage > TC_MAX_STAGES) a.nstage = TC_MAX_STAGES;
   if (a.nstage > a.nslab) a.nstage = a.nslab;
-  int ncols = 32;
-  while (ncols < G * a.npad) ncols <<= 1;
-  a.ncols = ncols;
-  const int smem = a.nstage * (int)a.stage_bytes;
+  const int img_bytes = 128 * (G * a.npad + 1) * 4;
+  const int smem = a.nstage * (int)a.stage_bytes > img_bytes ? a.nstage * (int)a.stage_bytes : img_bytes;
   static int attr_smem = 0;
   if (smem > attr_smem) {
     cudaError_t e = cudaFuncSetAttribute(conv_block_tc_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_max);

@@ -1,46 +1,31 @@
-// Fused ConvBlock on the 5th-gen tensor cores, persistent / warp-specialised edition
-// (tcgen05 kind::tf32, fp32 accumulation in TMEM).  Same contract as conv_tc.cu / conv_simt.cu:
+// Fused ConvBlock on the tensor cores, persistent / warp-specialised edition (wgmma m64nNk8 tf32,
+// fp32 accumulation in registers).  Same contract as conv_tc.cu / conv_simt.cu:
 //   reflect|zero pad -> Conv1d -> [pixel shuffle] -> [InstanceNorm] -> [AdaIN] -> [ReLU] -> [+residual] -> [*mask]
 // (model.py:21-32, 52-59, 77-83, 237-250, 309-320, 354-369) and, with the DGRAD weight pack and zero
 // padding, autograd's conv data gradient incl. the adjoint of the reflect padding / residual branch
-// (AVC_F_FOLD).  What changed against conv_tc.cu (round 1), following its own phase counters:
+// (AVC_F_FOLD).
 //
 //   * PERSISTENT CTAs (one per SM) walk a static tile list; a tile = G samples x 128 output channels.
-//   * TWO TMEM ACCUMULATORS (2 x 256 columns): the epilogue of tile i overlaps the main loop of tile
-//     i+1.  Roles: warp 0 bulk-copy (TMA) producer, warp 1 MMA issuer, warp 2 TMEM allocator, warps 4-7
-//     halo patch / TF32 rounding of the staged input, warps 8-15 epilogue.  Five mbarrier pipelines:
-//     full / ready / empty per shared-memory stage, acc_full / acc_empty per accumulator.
+//   * Roles: warp 0 bulk-copy (TMA) producer, warps 1-3 halo patch / TF32 rounding of the staged input,
+//     warps 4-11 two consumer warpgroups (output rows 0-63 / 64-127) that issue the wgmma main loop into
+//     their register accumulators and then run the epilogue.  mbarrier pipelines per shared-memory stage:
+//     full (weights) / fullx (input rows) / ready (patched) / empty (read by both warpgroups' MMAs).
 //   * STACKED SAMPLES: the G samples of a tile lie one after another in the staged row space at a
-//     pitch of R = (rows one sample needs) and ONE MMA of N <= 256 columns per (k-step, tap) covers all
+//     pitch of R = (rows one sample needs) and ONE MMA of N <= T2_MAX_N columns per (k-step, tap) covers all
 //     of them (columns between two samples are garbage and never read): the small-T layers issue
 //     2K MMAs per 16-channel slab instead of 2K*G.
-//   * EPILOGUE THROUGH SHARED MEMORY: one TMEM pass (thread = output channel = TMEM lane) adds the bias,
-//     accumulates the InstanceNorm sums and drops the raw conv row into an A4-layout tile in shared
-//     memory with conflict-free scalar stores (chunk pitch == 1 mod 8 sixteen-byte units); the
-//     accumulator is released right there.  A second pass (thread = one 16-byte A4 unit, lanes along
-//     time) normalises / AdaIN / ReLU / residual / mask / rounds and writes `c` and `out` with fully
-//     coalesced 16-byte stores -- no cross-lane transposes, and the reflect-padding adjoint of the
-//     data-gradient variant becomes three shared-memory reads.
+//   * EPILOGUE THROUGH SHARED MEMORY: pass 0 adds the bias and drops the accumulator registers (wgmma
+//     fragment layout) into an A4-layout tile in shared memory (chunk pitch == 1 mod 8 sixteen-byte units:
+//     conflict-free); the InstanceNorm sums are one sweep over that tile.  A second pass (thread = one
+//     16-byte A4 unit, lanes along time) normalises / AdaIN / ReLU / residual / mask / rounds and writes `c`
+//     and `out` with fully coalesced 16-byte stores; the reflect-padding adjoint of the data-gradient
+//     variant becomes three shared-memory reads.
 //   * Halo rows come straight from global memory (no dependence on the bulk copy), so long samples
 //     can be TIME-TILED (T > 144 columns: inference) for blocks without InstanceNorm.
 //   * STAGE GRANULARITY: a stage is `hs` HALF-SLABS of 8 input channels (one MMA K-step each).  Default hs = 2 (one
-//     16-channel slab of the weight pack, one contiguous bulk copy) for K >= 2 and hs = 4 for the 1x1 layers (a
-//     1104-channel in_conv makes 35 barrier round trips per tile instead of 69: 62.5 -> 60.5 us).  hs = 1 (K x 4 KB
-//     of weights per stage fetched by ONE 4-D tensor-map copy out of the [slab][tap][chunk] pack, 6 stages in flight
-//     instead of 3 for the k = 5 layers) is implemented and correct but SLOWER (AVC_T2_HS=1: 26.6 vs 23.4 us at
-//     T = 128, 48.6k vs 52.0k seg/s; K bulk copies of 4 KB instead of the tensor-map copy: 27.6 us): every stage
-//     iteration costs ~450-600 cycles of barrier round trips whatever it carries, and hs = 1 doubles their number.
-//     Depth does matter at equal stage size: capping the k = 5 layers at 2 stages (AVC_T2_NSTAGE=2) costs 4.1 us at
-//     T = 128 (23.9 -> 28.0), i.e. the main loop runs at ~(3 K cycles ring latency) / (stages in flight); the 70 KB
-//     epilogue tile is what keeps the k = 5 layers at 3 stages of 49 KB.
-//   * WHAT BOUNDS IT (tools/diag_ablate.py, profiles/r2_conv_ablation.txt): removing the MMAs, the copies or the store
-//     pass from the T = 128 block saves 3.3 / 2.5 / 5.8 us of 23.4 -- the parts ADD UP instead of overlapping.  A
-//     kind::tf32 SS-MMA of N = 128 fetches (128 + 128) x 32 B of operands in its 64 cycles = the whole 128 B/clk of
-//     the SM's shared memory, so while the tensor pipe runs, the copy engine's writes, the TMEM->tile pass and the
-//     store pass's reads wait (and vice versa): 1.17 MB of shared-memory traffic per sample = 9.2 K cycles, twice
-//     per CTA, plus ~10 us of launch + pipeline skeleton.  Spinning instead of suspending on the barriers, 1-D bulk
-//     copies instead of the tensor-map copy for the input rows, a 132-row plane pitch for the 1x1 layers and four
-//     independent patch warps were each measured and change nothing (<= 2 %).
+//     16-channel slab of the weight pack, one contiguous bulk copy) for K >= 2 and hs = 4 for the 1x1 layers (fewer
+//     barrier round trips per tile); hs = 1 (K x 4 KB of weights per stage fetched by ONE 4-D tensor-map copy out of
+//     the [slab][tap][chunk] pack) is selectable with AVC_T2_HS=1.  AVC_T2_NSTAGE caps the pipeline depth.
 #include <stdlib.h>
 
 #include "common.cuh"
@@ -57,18 +42,22 @@ constexpr int T2_WTAP_BYTES = 8192;  // one tap of one slab: 4 chunks x 128 co x
 constexpr int T2_HALF_BYTES = 4096;  // one tap of one half-slab (8 channels): 2 chunks x 128 co x 16 B
 constexpr int T2_MAX_STAGES = 8;
 constexpr int T2_MAX_G = 8;
+constexpr int T2_MAX_N = 160;       // accumulator columns: N / 2 registers per consumer thread
 constexpr int T2_SMEM_MAX = 226 * 1024;  // 227 KB per block minus the static shared memory (barriers)
 
 struct Tc2Args {
   avc_conv_desc d;
   int G;        // samples per tile
-  int R;        // row pitch between the stacked samples of a tile (= TMEM column pitch)
-  int N;        // MMA N: multiple of 16, <= 256
+  int R;        // row pitch between the stacked samples of a tile (= accumulator column pitch)
+  int N;        // MMA N: multiple of 16, <= T2_MAX_N
   int srows;    // rows of one 4-channel plane of a stage (>= N + K - 1)
   int nslab, nstage;
   int hs;       // half-slabs (8 input channels = one MMA K-step) per pipeline stage: 1, or an even number
   int nhalf;    // half-slabs per tile (2 * nslab)
   int nst;      // pipeline stages per tile = ceil(nhalf / hs); the last one may hold fewer half-slabs
+  int nchunk;   // column chunks of N accumulator columns per tile (> 1 only for a folded sample of more than 144
+                // columns: the main loop runs once per chunk over the same staged rows)
+  int N_last;   // accumulator columns of the last chunk
   int TT, ntt;  // output time steps per tile, time tiles per sample
   int Ts;       // columns one sample stages for the second pass (TT, or Tout for AVC_F_FOLD)
   int P;        // chunk pitch of the staged tile in 16-byte units (== 1 mod 8)
@@ -78,7 +67,7 @@ struct Tc2Args {
   int patch;    // 1: the patch warps sit between the bulk copy and the MMAs (halo rows and/or TF32 rounding)
   int variant;  // bit 0: `c` rows leave through bulk (TMA) stores; bit 1: `out` rows too (written back in place)
                 // ABLATION bits (timing probes only, results are WRONG; tools/diag_ablate.py): 16 weight copies shrunk to
-                // 1 KB, 32 no store pass, 64 no MMAs, 128 no TMEM pass, 256 no input-row copies; 2048: one patch warp
+                // 1 KB, 32 no store pass, 64 no MMAs, 128 no accumulator pass, 256 no input-row copies; 2048: one patch warp
                 // owns every stage (results stay correct)
   int* status;
   long long* dbg;
@@ -138,14 +127,104 @@ __device__ __forceinline__ TileCoord t2_decode(const Tc2Args& a, int tile) {
 // rows / samples outside the tensor arrive as zeros (that IS the zero padding of the data-gradient convs).
 // tmw (hs == 1 only): the weight pack as a 4-D tensor (256 floats, 2 halves of a [co][4] row, 4 chunks, slab*K+tap): the box
 // (256, 2, 2, K) is one half-slab -- [tap][2 chunks][co][4] -- in one copy-engine instruction.
-__global__ void __launch_bounds__(512, 1) conv_block_tc2_kernel(const Tc2Args a, const __grid_constant__ CUtensorMap tmx,
+// Main loop of one tile for one consumer warpgroup (rows 64 wg .. 64 wg + 63 of the 128-row m-tile): every stage is
+// K taps x (half-slabs) wgmma m64nNk8 into the register accumulator `acc`; the stage is released to the producer
+// once this warpgroup's MMAs have read it (bar_empty counts one arrival per warpgroup).
+template <int N>
+__device__ __forceinline__ bool t2_mainloop(const Tc2Args& a, uint32_t smem0, uint64_t* bar_full, uint64_t* bar_fullx, uint64_t* bar_ready,
+                                            uint64_t* bar_empty, int& s, uint32_t& ph, float* acc, int wg, int wt, int col0) {
+  const int K = a.d.K;
+  const uint32_t d_hi = tc::sdesc_hi(128);
+  const uint32_t ks_b = 2u * (a.x_chunk_bytes >> 4);                       // B operand: next half-slab = 2 chunk planes on
+  const uint32_t tap_a = (a.hs == 1 ? T2_HALF_BYTES : T2_WTAP_BYTES) >> 4;   // A operand: next tap
+  const uint32_t slab_a = (uint32_t)K * (T2_WTAP_BYTES >> 4);                // A operand: next slab (hs > 1)
+  for (int i = 0; i < a.nst; ++i) {
+    const bool ok = __all_sync(0xffffffffu, tc::mbar_wait(a.patch ? &bar_ready[s] : &bar_fullx[s], ph, a.status, 3) &&
+                                                tc::mbar_wait(&bar_full[s], ph, a.status, 3));
+    if (!ok) return false;
+    const uint32_t sw = smem0 + (uint32_t)s * a.stage_bytes;
+    // rows 64 wg.. of the A operand: 64 rows x 16 B further inside every 4-channel chunk
+    // B operand: the chunk's first column = staged row col0 (16 B per row)
+    const uint32_t a_lo0 = tc::sdesc_lo(sw + (uint32_t)wg * 1024u, 2048),
+                   b_lo0 = tc::sdesc_lo(sw + a.w_bytes, a.x_chunk_bytes) + (uint32_t)col0;
+    const int nh = min(a.hs, a.nhalf - i * a.hs);
+    tc::wgmma_fence();
+    for (int e = 0; e < nh; ++e) {   // half-slab e of the stage: one K-step of 8 input channels per tap
+      if (a.variant & 64) break;
+      const uint32_t a_off = a.hs == 1 ? 0u : (uint32_t)(e >> 1) * slab_a + (uint32_t)(e & 1) * (T2_HALF_BYTES >> 4);
+      uint64_t a_desc = tc::sdesc64(a_lo0 + a_off, d_hi);
+      uint64_t b_desc = tc::sdesc64(b_lo0 + (uint32_t)e * ks_b, d_hi);
+      if (K == 5) {
+#pragma unroll
+        for (int j = 0; j < 5; ++j) {
+          tc::wgmma_tf32<N>(acc, a_desc, b_desc, ((uint32_t)i | (uint32_t)e | (uint32_t)j) ? 1u : 0u);
+          a_desc += (uint64_t)tap_a;
+          b_desc += 1u;
+        }
+      } else {
+        for (int j = 0; j < K; ++j) {
+          tc::wgmma_tf32<N>(acc, a_desc, b_desc, ((uint32_t)i | (uint32_t)e | (uint32_t)j) ? 1u : 0u);
+          a_desc += (uint64_t)tap_a;
+          b_desc += 1u;
+        }
+      }
+    }
+    tc::wgmma_commit();
+    tc::wgmma_wait<0>();
+    tc::acc_fence(acc, N / 2);
+    if (wt == 0) tc::mbar_arrive(&bar_empty[s]);
+    if (++s == a.nstage) { s = 0; ph ^= 1u; }
+  }
+  return true;
+}
+
+// Pass 0 of the epilogue, straight from the accumulator registers: + bias, raw conv rows of every stacked sample into
+// the staged A4 tile (chunk pitch P == 1 mod 8 sixteen-byte units: the four lanes of a quad and the eight row groups of
+// a warp hit 32 different banks).
+template <int N>
+__device__ __forceinline__ void t2_acc_to_tile(const Tc2Args& a, const TileCoord& c, const float* acc, float* stile, int wg, int wt,
+                                               int col0) {
+  const int sshift = a.d.stride == 2 ? 1 : 0;
+  const int ncol = (c.tw - 1) * a.d.stride + 1;  // accumulator columns of one sample that hold outputs
+  const int r0 = 64 * wg + tc::wg_acc_row(wt, 0);
+  const int co0 = c.mtile * 128 + r0, co1 = co0 + 8;
+  const float bias0 = (a.d.bias && co0 < a.d.Cout) ? __ldg(a.d.bias + co0) : 0.f;
+  const float bias1 = (a.d.bias && co1 < a.d.Cout) ? __ldg(a.d.bias + co1) : 0.f;
+  float* srow0 = stile + ((size_t)(r0 >> 2) * a.P) * 4 + (r0 & 3);
+  float* srow1 = stile + ((size_t)((r0 + 8) >> 2) * a.P) * 4 + ((r0 + 8) & 3);
+  int g = 0, gbase = 0;   // stacked sample of the column and its first column; columns grow with the register index
+#pragma unroll
+  for (int j = 0; j < N / 8; ++j) {
+#pragma unroll
+    for (int k = 0; k < 2; ++k) {
+      const int col = col0 + tc::wg_acc_col(wt, 4 * j + k);
+      while (col >= gbase + a.R) { gbase += a.R; ++g; }
+      const int tl = col - gbase;
+      if (g < c.nsamp && tl < ncol && (tl & sshift) == 0) {
+        const size_t off = (size_t)(g * a.Ts + (tl >> sshift)) * 4;
+        srow0[off] = acc[4 * j + k] + bias0;
+        srow1[off] = acc[4 * j + 2 + k] + bias1;
+      }
+    }
+  }
+}
+
+// MMAs and pass 0 of one tile, instantiated for every accumulator width N (a multiple of 16, <= T2_MAX_N)
+template <int N>
+__device__ __forceinline__ bool t2_tile(const Tc2Args& a, const TileCoord& c, uint32_t smem0, uint64_t* bar_full, uint64_t* bar_fullx,
+                                     uint64_t* bar_ready, uint64_t* bar_empty, int& s, uint32_t& ph, float* stile, int wg, int wt, int col0) {
+  float acc[N / 2];
+  if (!t2_mainloop<N>(a, smem0, bar_full, bar_fullx, bar_ready, bar_empty, s, ph, acc, wg, wt, col0)) return false;
+  if (!(a.variant & 128)) t2_acc_to_tile<N>(a, c, acc, stile, wg, wt, col0);
+  return true;
+}
+
+__global__ void __launch_bounds__(384, 1) conv_block_tc2_kernel(const Tc2Args a, const __grid_constant__ CUtensorMap tmx,
                                                                 const __grid_constant__ CUtensorMap tmw) {
   extern __shared__ __align__(1024) uint8_t smem[];
   // per stage: full = weights landed, fullx = input rows landed (they are small and issued first, so the patch step
   // runs while the 5x larger weight copy is still in flight), ready = patched, empty = consumed by the MMAs
-  __shared__ uint64_t bar_full[T2_MAX_STAGES], bar_fullx[T2_MAX_STAGES], bar_ready[T2_MAX_STAGES], bar_empty[T2_MAX_STAGES], bar_accf[2],
-      bar_acce[2];
-  __shared__ uint32_t tmem_slot;
+  __shared__ uint64_t bar_full[T2_MAX_STAGES], bar_fullx[T2_MAX_STAGES], bar_ready[T2_MAX_STAGES], bar_empty[T2_MAX_STAGES];
   const avc_conv_desc& d = a.d;
   const int tid = threadIdx.x, warp = tc::warp_idx_sync(), lane = tid & 31;
   const int K = d.K, S = d.stride;
@@ -155,19 +234,11 @@ __global__ void __launch_bounds__(512, 1) conv_block_tc2_kernel(const Tc2Args a,
       tc::mbar_init(&bar_full[s], 1);
       tc::mbar_init(&bar_fullx[s], 1);
       tc::mbar_init(&bar_ready[s], 1);
-      tc::mbar_init(&bar_empty[s], 1);
-    }
-    for (int b = 0; b < 2; ++b) {
-      tc::mbar_init(&bar_accf[b], 1);
-      tc::mbar_init(&bar_acce[b], 256);
+      tc::mbar_init(&bar_empty[s], 2);
     }
     tc::fence_mbar_init();
   }
-  if (warp == 2) tc::tmem_alloc(&tmem_slot, 512u);
-  tc::tc_fence_before();
   __syncthreads();
-  tc::tc_fence_after();
-  const uint32_t tbase = tmem_slot;
   long long tm0 = 0;
   if (a.dbg && tid == 0) tm0 = clock64();
 
@@ -192,7 +263,8 @@ __global__ void __launch_bounds__(512, 1) conv_block_tc2_kernel(const Tc2Args a,
         }
       }
       __syncwarp();
-      for (int i = 0; i < a.nst; ++i) {
+      for (int ii = 0; ii < a.nst * a.nchunk; ++ii) {   // every column chunk streams the same stages again
+        const int i = ii % a.nst;
         const long long w0 = a.dbg ? clock64() : 0;
         if (!first_round) ok = __all_sync(0xffffffffu, tc::mbar_wait(&bar_empty[s], ph ^ 1u, a.status, 2));
         if (a.dbg) dbg0 += clock64() - w0;
@@ -227,77 +299,8 @@ __global__ void __launch_bounds__(512, 1) conv_block_tc2_kernel(const Tc2Args a,
       }
     }
     if (a.dbg && lane == 0) a.dbg[(size_t)blockIdx.x * 16 + 2] = dbg0;
-  } else if (warp == 1) {
-    // ================================================================ MMA issuer
-    // The WHOLE warp runs converged with warp-uniform values and one elected lane executes each tcgen05
-    // instruction (descriptors stay in uniform registers, see conv_tc.cu).
-    const uint32_t idesc = tc::make_idesc_tf32(128, a.N, 0, 0);
-    const uint32_t d_hi = tc::sdesc_hi(128);
-    const uint32_t tb = __shfl_sync(0xffffffffu, tbase, 0);
-    const uint32_t smem0 = tc::smem_u32(smem);
-    const uint32_t ks_b = 2u * (a.x_chunk_bytes >> 4);                       // B operand: next half-slab = 2 chunk planes on
-    const uint32_t tap_a = (a.hs == 1 ? T2_HALF_BYTES : T2_WTAP_BYTES) >> 4;   // A operand: next tap
-    const uint32_t slab_a = (uint32_t)K * (T2_WTAP_BYTES >> 4);                // A operand: next slab (hs > 1)
-    int s = 0;
-    uint32_t ph = 0;
-    bool ok = true;
-    int tl = 0;
-    long long dbg0 = 0, dbg1 = 0, dbg2 = 0;
-    for (int tile = blockIdx.x; tile < a.ntiles && ok; tile += gridDim.x, ++tl) {
-      const uint32_t buf = (uint32_t)tl & 1u;
-      const long long wa = a.dbg ? clock64() : 0;
-      if (tl >= 2) ok = __all_sync(0xffffffffu, tc::mbar_wait(&bar_acce[buf], (uint32_t)((tl >> 1) - 1) & 1u, a.status, 6));
-      if (a.dbg) dbg1 += clock64() - wa;
-      if (!ok) break;
-      tc::tc_fence_after();
-      const uint32_t dcol = tb + buf * 256u;
-      for (int i = 0; i < a.nst; ++i) {
-        const long long w0 = a.dbg ? clock64() : 0;
-        ok = __all_sync(0xffffffffu, tc::mbar_wait(a.patch ? &bar_ready[s] : &bar_fullx[s], ph, a.status, 3) &&
-                                         tc::mbar_wait(&bar_full[s], ph, a.status, 3));
-        const long long w1 = a.dbg ? clock64() : 0;
-        dbg0 += w1 - w0;
-        if (!ok) break;
-        tc::tc_fence_after();
-        const uint32_t sw = smem0 + (uint32_t)s * a.stage_bytes;
-        const uint32_t a_lo0 = tc::sdesc_lo(sw, 2048), b_lo0 = tc::sdesc_lo(sw + a.w_bytes, a.x_chunk_bytes);
-        const int nh = min(a.hs, a.nhalf - i * a.hs);
-        for (int e = 0; e < nh; ++e) {   // half-slab e of the stage: one K-step of 8 input channels per tap
-          if (a.variant & 64) break;
-          const uint32_t a_off = a.hs == 1 ? 0u : (uint32_t)(e >> 1) * slab_a + (uint32_t)(e & 1) * (T2_HALF_BYTES >> 4);
-          uint64_t a_desc = tc::sdesc64(a_lo0 + a_off, d_hi);
-          uint64_t b_desc = tc::sdesc64(b_lo0 + (uint32_t)e * ks_b, d_hi);
-          if (K == 5) {
-#pragma unroll
-            for (int j = 0; j < 5; ++j) {
-              tc::mma_tf32_elect(dcol, a_desc, b_desc, idesc, ((uint32_t)i | (uint32_t)e | (uint32_t)j) ? 1u : 0u);
-              a_desc += (uint64_t)tap_a;
-              b_desc += 1u;
-            }
-          } else {
-            for (int j = 0; j < K; ++j) {
-              tc::mma_tf32_elect(dcol, a_desc, b_desc, idesc, ((uint32_t)i | (uint32_t)e | (uint32_t)j) ? 1u : 0u);
-              a_desc += (uint64_t)tap_a;
-              b_desc += 1u;
-            }
-          }
-        }
-        __syncwarp();
-        if (tc::elect_one()) tc::mma_commit(&bar_empty[s]);
-        __syncwarp();
-        if (a.dbg) dbg2 += clock64() - w1;
-        if (++s == a.nstage) { s = 0; ph ^= 1u; }
-      }
-      if (!ok) break;
-      if (tc::elect_one()) tc::mma_commit(&bar_accf[buf]);
-      __syncwarp();
-    }
-    if (a.dbg && lane == 0) {
-      long long* o = a.dbg + (size_t)blockIdx.x * 16;
-      o[5] = dbg0; o[6] = dbg1; o[7] = dbg2;
-    }
-  } else if (warp >= 4 && warp < 8) {
-    // ================================================================ patch warps (4 warps, ROUND ROBIN over the stages)
+  } else if (warp < 4) {
+    // ================================================================ patch warps (3 warps, ROUND ROBIN over the stages)
     // (a) reflect padding: the copy engine delivered zeros for the rows outside the sample; they are overwritten
     //     with their mirror rows, taken from the staged rows of the same sample (from global memory only when a
     //     time-tiled sample's mirror row lies outside the tile);
@@ -306,17 +309,16 @@ __global__ void __launch_bounds__(512, 1) conv_block_tc2_kernel(const Tc2Args a,
     //     that the tensor core's truncation is exact.
     // a.patch == 0 (zero padding or K = 1, pre-rounded input): these warps idle, the MMAs wait on the copies directly.
     // One patch step is a dependent chain (barrier wake-up, shared-memory load, store, proxy fence, arrive) of
-    // ~400-1000 cycles whatever the stage holds, and with ONE owner of all stages it was the serial resource of the
-    // whole pipeline (tools/diag_ablate.py: the empty pipeline cost ~740 cycles per stage, 2x the stages = 2x the
-    // time).  Warp w therefore owns the shared-memory STAGES s % npw == w outright (wait, round, mirror, fence, ONE
-    // arrive): up to four patch steps are in flight and none of them synchronises with another warp.  Ownership goes
+    // ~400-1000 cycles whatever the stage holds, and with ONE owner of all stages it is the serial resource of the
+    // whole pipeline.  Warp w therefore owns the shared-memory STAGES s % npw == w outright (wait, round, mirror, fence, ONE
+    // arrive): up to three patch steps are in flight and none of them synchronises with another warp.  Ownership goes
     // by stage, not by iteration: every phase of a stage's barrier is then seen by the same warp in order (a warp
     // that skipped a phase could run a whole ring revolution ahead, and a parity wait on a barrier that is still one
     // phase behind returns immediately -- the false positive every mbarrier pipeline has to exclude).
-    const int pw = warp - 4;
+    const int pw = warp - 1;
     const bool rnd = !(d.flags & AVC_F_IN_TF32);
     const bool refl = d.pad_mode == AVC_PAD_REFLECT;
-    const int npw = (a.variant & 2048) ? 1 : min(4, a.nstage);   // probe bit 2048: a single patch warp owns every stage (the previous structure)
+    const int npw = (a.variant & 2048) ? 1 : min(3, a.nstage);   // probe bit 2048: a single patch warp owns every stage (the previous structure)
     int s = 0;
     uint32_t ph = 0;
     bool ok = true;
@@ -351,7 +353,8 @@ __global__ void __launch_bounds__(512, 1) conv_block_tc2_kernel(const Tc2Args a,
           else if (p >= 0) h_glob[j] = p;
         }
       }
-      for (int i = 0; i < a.nst && ok; ++i) {
+      for (int ii = 0; ii < a.nst * a.nchunk && ok; ++ii) {
+        const int i = ii % a.nst;
         if (s % npw == pw) {
           const long long w0 = a.dbg ? clock64() : 0;
           ok = tc::mbar_wait(&bar_fullx[s], ph, a.status, 4);
@@ -408,15 +411,19 @@ __global__ void __launch_bounds__(512, 1) conv_block_tc2_kernel(const Tc2Args a,
         if (++s == a.nstage) { s = 0; ph ^= 1u; }
       }
     }
-    if (a.dbg && tid == 128) {
+    if (a.dbg && tid == 32) {
       long long* o = a.dbg + (size_t)blockIdx.x * 16;
       o[3] = dbg0; o[4] = dbg1;
     }
-  } else if (warp >= 8) {
-    // ================================================================ epilogue (256 threads)
-    const int etid = tid - 256, ewarp = warp - 8;
-    const int quarter = warp & 3, half = ewarp >> 2;  // TMEM lane quarter of this warp; column half
-    const int col_l = quarter * 32 + lane;            // conv output row inside the 128-row tile
+  } else {
+    // ================================================================ MMA + epilogue (two warpgroups, 256 threads)
+    const int etid = tid - 128, ewarp = warp - 4;
+    const int wg = ewarp >> 2, wt = etid & 127;      // warpgroup: accumulator rows 64 wg .. 64 wg + 63
+    const int quarter = ewarp & 3, half = ewarp >> 2;
+    const int col_l = quarter * 32 + lane;            // conv output row of the per-channel parameter pass
+    const uint32_t smem0 = tc::smem_u32(smem);
+    int s = 0;
+    uint32_t ph = 0;
     float* stile = reinterpret_cast<float*>(smem + a.off_tile);
     float* par = reinterpret_cast<float*>(smem + a.off_par);          // [3][G][128]: mean, scale, shift
     float2* stat = reinterpret_cast<float2*>(smem + a.off_stat);      // [2][G][128] partial (sum, sum sq)
@@ -426,7 +433,6 @@ __global__ void __launch_bounds__(512, 1) conv_block_tc2_kernel(const Tc2Args a,
     const int Tn = shuf ? d.Tout * 2 : d.Tout;                        // normalised length of a whole sample
     const int out_T = d.out_T > 0 ? d.out_T : Tn;
     const int ots = d.out_tstride > 0 ? d.out_tstride : 1, oto = d.out_toff;
-    const int sshift = S == 2 ? 1 : 0, smask = sshift;
     const bool fold = (d.flags & AVC_F_FOLD) != 0;
     // AVC_F_NORMBWD (with AVC_F_FOLD): norm / relu / eps / cond / save_c / stats / dc / dcond / dbias describe the UPSTREAM
     // block whose output gradient this data-gradient conv produces; its InstanceNorm/AdaIN/ReLU backward runs here
@@ -441,63 +447,40 @@ __global__ void __launch_bounds__(512, 1) conv_block_tc2_kernel(const Tc2Args a,
     long long dbg0 = 0, dbg1 = 0, dbg2 = 0, dbg3 = 0, dbg4 = 0, dbg5 = 0;
     for (int tile = blockIdx.x; tile < a.ntiles; tile += gridDim.x, ++tl) {
       const TileCoord c = t2_decode(a, tile);
-      const uint32_t buf = (uint32_t)tl & 1u;
       long long e3b = 0;
       const long long e0 = a.dbg ? clock64() : 0;
-      ok = tc::mbar_wait(&bar_accf[buf], (uint32_t)(tl >> 1) & 1u, a.status, 5) && ok;
-      tc::tc_fence_after();
+      // ---------------- main loop, then pass 0: accumulators (+bias) -> staged A4 tile
+      for (int ch = 0; ch < a.nchunk; ++ch) {
+        bool mok = false;
+        const int col0 = ch * a.N;
+        switch (ch + 1 == a.nchunk ? a.N_last : a.N) {
+#define T2_CASE(n) \
+  case n: mok = t2_tile<n>(a, c, smem0, bar_full, bar_fullx, bar_ready, bar_empty, s, ph, stile, wg, wt, col0); break;
+          T2_CASE(16) T2_CASE(32) T2_CASE(48) T2_CASE(64) T2_CASE(80) T2_CASE(96) T2_CASE(112) T2_CASE(128) T2_CASE(144) T2_CASE(160)
+#undef T2_CASE
+        }
+        ok = ok && mok;
+      }
       const long long e1 = a.dbg ? clock64() : 0;
       const int co = c.mtile * 128 + col_l;
       const bool co_ok = co < d.Cout;
-      const float bias = (d.bias && co_ok) ? __ldg(d.bias + co) : 0.f;
-      const int ncol = (c.tw - 1) * S + 1;  // TMEM columns of one sample that hold outputs
-      const int nch = (ncol + 15) >> 4;
-      const uint32_t lane_addr = tbase + ((uint32_t)(quarter * 32) << 16) + buf * 256u;
-      // ---------------- pass 0: TMEM -> (+bias, InstanceNorm sums) -> staged A4 tile
-      if (ok && !(a.variant & 128)) {
-        float* srow = stile + ((size_t)(col_l >> 2) * P) * 4 + (col_l & 3);
-        for (int g = 0; g < c.nsamp; ++g) {
+      t2_bar_sync(2, 256);
+      // ---------------- InstanceNorm sums of every (sample, row) over the staged tile
+      if (ok && fwd_norm) {
+        for (int e = etid; e < c.nsamp * 128; e += 256) {
+          const int g = e >> 7, r = e & 127;
+          const float* src = stile + ((size_t)(r >> 2) * P + g * Ts) * 4 + (r & 3);
           float s1 = 0.f, s2 = 0.f;
-          float* sdst = srow + (size_t)(g * Ts) * 4;
-          for (int j = half; j < nch; j += 4) {   // this warp's chunks j, j+2, ...: two loads in flight per wait
-            float v[32];
-            const bool two = j + 2 < nch;
-            tc::tmem_ld16_nowait(lane_addr + (uint32_t)(g * a.R + 16 * j), v);
-            if (two) tc::tmem_ld16_nowait(lane_addr + (uint32_t)(g * a.R + 16 * (j + 2)), v + 16);
-            tc::tmem_ld_wait();
-#pragma unroll
-            for (int k = 0; k < 2; ++k) {
-              if (k == 1 && !two) break;
-              const int cbase = 16 * (j + 2 * k);
-              if (S == 1 && cbase + 16 <= ncol) {   // whole chunk valid, stride 1: no per-column predicates
-                float* sd = sdst + (size_t)cbase * 4;
-#pragma unroll
-                for (int i = 0; i < 16; ++i) {
-                  const float x = v[16 * k + i] + bias;
-                  s1 += x;
-                  s2 = fmaf(x, x, s2);
-                  sd[i * 4] = x;
-                }
-              } else {
-#pragma unroll
-                for (int i = 0; i < 16; ++i) {
-                  const int col = cbase + i;
-                  if (col < ncol && (col & smask) == 0) {
-                    const float x = v[16 * k + i] + bias;
-                    s1 += x;
-                    s2 = fmaf(x, x, s2);
-                    sdst[(size_t)(col >> sshift) * 4] = x;
-                  }
-                }
-              }
-            }
+          for (int t = 0; t < c.tw; ++t) {
+            const float x = src[(size_t)t * 4];
+            s1 += x;
+            s2 = fmaf(x, x, s2);
           }
-          if (fwd_norm) stat[(half * a.G + g) * 128 + col_l] = make_float2(s1, s2);
+          stat[(0 * a.G + g) * 128 + r] = make_float2(s1, s2);
+          stat[(1 * a.G + g) * 128 + r] = make_float2(0.f, 0.f);
         }
       }
       if (a.variant & 3) tc::fence_proxy_async_smem();   // the staged rows will be read by bulk (async-proxy) stores
-      tc::tc_fence_before();
-      tc::mbar_arrive(&bar_acce[buf]);  // the accumulator is free: the MMA warp may start tile tl+2 into it
       const long long e2 = a.dbg ? clock64() : 0;
       t2_bar_sync(2, 256);
       // ---------------- per (sample, channel) parameters: mean, scale = rstd*gamma, shift = beta
@@ -809,7 +792,7 @@ __global__ void __launch_bounds__(512, 1) conv_block_tc2_kernel(const Tc2Args a,
           }
           if (bulk_c || bulk_y) {
             tc::bulk_commit();
-            tc::bulk_wait_read_all();   // the staged tile is rewritten by the next tile's TMEM pass
+            tc::bulk_wait_read_all();   // the staged tile is rewritten by the next tile's accumulator pass
           }
         }
       }
@@ -827,13 +810,11 @@ __global__ void __launch_bounds__(512, 1) conv_block_tc2_kernel(const Tc2Args a,
       o[8] = dbg0; o[9] = dbg1; o[10] = dbg2; o[11] = dbg3; o[12] = tl; o[13] = dbg4; o[14] = dbg5;
     }
   }
-  tc::tc_fence_before();
   __syncthreads();
   if (a.dbg && tid == 0) {
     long long* o = a.dbg + (size_t)blockIdx.x * 16;
     o[0] = tm0; o[1] = clock64();
   }
-  if (warp == 2) tc::tmem_dealloc(tbase, 512u);
 }
 
 // ------------------------------------------------------------------ host side: tile plan
@@ -843,7 +824,7 @@ static int t2_num_sms() {
     int dev = 0;
     cudaDeviceProp p;
     if (cudaGetDevice(&dev) == cudaSuccess && cudaGetDeviceProperties(&p, dev) == cudaSuccess) n = p.multiProcessorCount;
-    if (n <= 0) n = 148;
+    if (n <= 0) n = 132;
   }
   return n;
 }
@@ -861,7 +842,10 @@ int t2_plan(const avc_conv_desc* d, Tc2Args& a) {
   if (d->pad_mode == AVC_PAD_REFLECT && d->Tin <= d->pad_left) return AVC_ERR_UNSUPPORTED;   // no mirror row to copy
   if ((d->flags & AVC_F_NORMBWD) && (!fold || d->Cout > 128 || !d->save_c || !d->dc || (d->norm && !d->stats))) return AVC_ERR_UNSUPPORTED;
   if (d->in_bstride % 4 != 0 || ((uintptr_t)d->in & 15u)) return AVC_ERR_UNSUPPORTED;        // tensor-map strides are multiples of 16 bytes
-  if (ncol_full <= 144) {
+  // a folded data-gradient sample of up to 256 staged rows (one tensor-map box) stays one tile: its columns are
+  // accumulated in chunks of 128
+  const bool chunked = ncol_full > 144 && fold && ncol_full + K - 1 <= 256;
+  if (ncol_full <= 144 || chunked) {
     a.TT = d->Tout;
     a.ntt = 1;
   } else {
@@ -878,9 +862,10 @@ int t2_plan(const avc_conv_desc* d, Tc2Args& a) {
   double best = 1e30;
   const int gmax = a.ntt > 1 ? 1 : T2_MAX_G;
   for (int G = 1; G <= gmax && G <= d->B; ++G) {
+    if (chunked) { bestG = 1; break; }
     if (G * a.Ts > 144) break;
     const int span = (G - 1) * a.R;
-    if (span + (ncol + 15) / 16 * 16 > 256) break;
+    if (span + (ncol + 15) / 16 * 16 > T2_MAX_N) break;
     const int N = (span + ncol + 15) / 16 * 16;
     const int ntiles = cdiv(d->B, G) * a.ntt * a.mtiles;
     const double mma = (double)a.nhalf * K * (N / 2 > 40 ? N / 2 : 40);
@@ -890,6 +875,13 @@ int t2_plan(const avc_conv_desc* d, Tc2Args& a) {
   if (bestG == 0) return AVC_ERR_UNSUPPORTED;
   a.G = bestG;
   a.N = ((a.G - 1) * a.R + ncol + 15) / 16 * 16;
+  a.nchunk = 1;
+  a.N_last = a.N;
+  if (chunked) {
+    a.N = 128;
+    a.nchunk = cdiv(ncol, 128);
+    a.N_last = (ncol - (a.nchunk - 1) * 128 + 15) / 16 * 16;
+  }
   a.srows = a.G * a.R;   // one plane of the tensor-copy box: [G samples][R rows] of 16 bytes
   a.x_chunk_bytes = (uint32_t)a.srows * 16u;
   a.ngroups = cdiv(d->B, a.G);
@@ -1001,7 +993,7 @@ int conv_block_tc2_launch(const avc_conv_desc* d, int* status, void* stream) {
     attr_done = true;
   }
   const int grid = a.ntiles < t2_num_sms() ? a.ntiles : t2_num_sms();
-  AVC_LAUNCH(conv_block_tc2_kernel, grid, 512, smem, (cudaStream_t)stream, a, tmx, tmw);
+  AVC_LAUNCH(conv_block_tc2_kernel, grid, 384, smem, (cudaStream_t)stream, a, tmx, tmw);
   AVC_CHECK_LAUNCH("conv_block_tc2");
   return AVC_OK;
 }

@@ -239,7 +239,8 @@ __global__ void __launch_bounds__(256) norm_bwd_kernel(const avc_conv_desc d) {
         const float s = warp_sum(db[sx][c]);
         if (lane == 0) {
           const int co = SHUF ? 2 * (qn * 4 + c) + sx : qn * 4 + c;
-          atomicAdd(d.dbias + co, s);
+          if (d.dbias_part) d.dbias_part[(int64_t)b * d.Cout + co] = s;   // partial of sample b
+          else atomicAdd(d.dbias + co, s);
         }
       }
   }
@@ -342,7 +343,8 @@ __global__ void __launch_bounds__(256) norm_bwd_cached_kernel(const avc_conv_des
       float s = 0.f;
 #pragma unroll
       for (int w = 0; w < 8; ++w) s += db_sh[w][threadIdx.x];
-      atomicAdd(d.dbias + qn * 4 + threadIdx.x, s);
+      if (d.dbias_part) d.dbias_part[(int64_t)(blockIdx.x - qn * bgroups) * d.Cout + qn * 4 + threadIdx.x] = s;   // partial of the sample group
+      else atomicAdd(d.dbias + qn * 4 + threadIdx.x, s);
     }
   }
 }
@@ -388,30 +390,40 @@ __global__ void __launch_bounds__(256) fold_add_kernel(const avc_fold_desc d) {
   }
 }
 
-// grid (C/4 chunks, batch slices): block-reduce a slice of (b, t), one atomicAdd per channel
+// dbias[c] += sum over the nslices rows of part[slice][C], in slice order
+__global__ void __launch_bounds__(256) partial_sum_kernel(const float* __restrict__ part, int nslices, int C, float* __restrict__ dbias) {
+  const int c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= C) return;
+  float s = 0.f;
+  for (int i = 0; i < nslices; ++i) s += part[(int64_t)i * C + c];
+  dbias[c] += s;
+}
+
+// grid (C/4 chunks): one block reduces all (b, t) of its 4 channels in a fixed order and adds the result to dbias --
+// no atomics, so the bias gradient is the same on every run
 // dbias_tab != null: channel group g = c / group_c accumulates into dbias_tab[g][c % group_c] (several layers whose dc
 // rows lie side by side in one tensor: the conv bank)
-__global__ void __launch_bounds__(256) bias_grad_kernel(const float* __restrict__ dc, int64_t bstride, float* __restrict__ dbias,
-                                                        int B, int C, int T, int bps, float* const* __restrict__ dbias_tab, int group_c) {
+__global__ void __launch_bounds__(1024) bias_grad_kernel(const float* __restrict__ dc, int64_t bstride, float* __restrict__ dbias,
+                                                         int B, int C, int T, float* const* __restrict__ dbias_tab, int group_c) {
   const int q = blockIdx.x;
   if (dbias_tab) dbias = dbias_tab[(q * 4) / group_c] - ((q * 4) / group_c) * group_c;
-  const int b0 = blockIdx.y * bps, b1 = min(B, b0 + bps);
   float4 s = zero4();
-  const int64_t n = (int64_t)(b1 - b0) * T;
-  for (int64_t i = threadIdx.x; i < n; i += blockDim.x) {
-    const int b = b0 + (int)(i / T), t = (int)(i % T);
-    const float4 v = ldg4(dc + (int64_t)b * bstride + ((int64_t)q * T + t) * 4);
-    s.x += v.x; s.y += v.y; s.z += v.z; s.w += v.w;
+  const int rows = blockDim.x / T;   // thread = (sample row, time step); the threads past rows * T idle
+  if ((int)threadIdx.x < rows * T) {
+    for (int b = threadIdx.x / T; b < B; b += rows) {
+      const float4 v = ldg4(dc + (int64_t)b * bstride + ((int64_t)q * T + threadIdx.x % T) * 4);
+      s.x += v.x; s.y += v.y; s.z += v.z; s.w += v.w;
+    }
   }
   s = warp_sum4(s);
-  __shared__ float4 part[8];
+  __shared__ float4 part[32];
   if ((threadIdx.x & 31) == 0) part[threadIdx.x >> 5] = s;
   __syncthreads();
   if (threadIdx.x == 0) {
     float4 r = zero4();
-    for (int w = 0; w < 8; ++w) { r.x += part[w].x; r.y += part[w].y; r.z += part[w].z; r.w += part[w].w; }
-    atomicAdd(dbias + q * 4 + 0, r.x); atomicAdd(dbias + q * 4 + 1, r.y);
-    atomicAdd(dbias + q * 4 + 2, r.z); atomicAdd(dbias + q * 4 + 3, r.w);
+    for (int w = 0; w < (int)(blockDim.x >> 5); ++w) { r.x += part[w].x; r.y += part[w].y; r.z += part[w].z; r.w += part[w].w; }
+    dbias[q * 4 + 0] += r.x; dbias[q * 4 + 1] += r.y;
+    dbias[q * 4 + 2] += r.z; dbias[q * 4 + 3] += r.w;
   }
 }
 
@@ -442,10 +454,16 @@ extern "C" int avc_norm_bwd(const avc_conv_desc* d, void* stream) {
   const int Cn = d->shuffle ? d->Cout / 2 : d->Cout;
   const int64_t warps = (int64_t)d->B * (Cn / 4);
   const int blocks = (int)cdiv64(warps * 32, 256);
+  const bool cached = !d->shuffle && d->Tout <= 128;
   if (d->shuffle) AVC_LAUNCH(norm_bwd_kernel<true>, blocks, 256, 0, (cudaStream_t)stream, *d);
-  else if (d->Tout <= 128) AVC_LAUNCH(norm_bwd_cached_kernel, (Cn / 4) * ((d->B + 7) / 8), 256, 0, (cudaStream_t)stream, *d);
+  else if (cached) AVC_LAUNCH(norm_bwd_cached_kernel, (Cn / 4) * ((d->B + 7) / 8), 256, 0, (cudaStream_t)stream, *d);
   else AVC_LAUNCH(norm_bwd_kernel<false>, blocks, 256, 0, (cudaStream_t)stream, *d);
   AVC_CHECK_LAUNCH("norm_bwd");
+  if (d->dbias && d->dbias_part) {   // partials: one row per sample, or per group of 8 samples (cached kernel)
+    const int nslices = cached ? (d->B + 7) / 8 : d->B;
+    AVC_LAUNCH(partial_sum_kernel, cdiv(d->Cout, 256), 256, 0, (cudaStream_t)stream, d->dbias_part, nslices, d->Cout, d->dbias);
+    AVC_CHECK_LAUNCH("norm_bwd_dbias");
+  }
   return AVC_OK;
 }
 
@@ -465,12 +483,8 @@ extern "C" int avc_fold_add_fwd(const avc_fold_desc* d, void* stream) {
 
 extern "C" int avc_bias_grad(const float* dc, int64_t bstride, float* dbias, int B, int C, int T, void* stream) {
   AVC_REQUIRE(dc && dbias && B > 0 && C > 0 && C % 4 == 0 && T > 0, AVC_ERR_INVALID, "avc_bias_grad: bad argument");
-  int slices = cdiv(148 * 4, C / 4);
-  if (slices > B) slices = B;
-  if (slices < 1) slices = 1;
-  const int bps = cdiv(B, slices);
-  dim3 grid(C / 4, cdiv(B, bps));
-  AVC_LAUNCH(bias_grad_kernel, grid, 256, 0, (cudaStream_t)stream, dc, bstride, dbias, B, C, T, bps, (float* const*)nullptr, 0);
+  AVC_REQUIRE(T <= 1024, AVC_ERR_UNSUPPORTED, "avc_bias_grad: T=%d > 1024", T);
+  AVC_LAUNCH(bias_grad_kernel, C / 4, 1024, 0, (cudaStream_t)stream, dc, bstride, dbias, B, C, T, (float* const*)nullptr, 0);
   AVC_CHECK_LAUNCH("bias_grad");
   return AVC_OK;
 }
@@ -478,12 +492,8 @@ extern "C" int avc_bias_grad(const float* dc, int64_t bstride, float* dbias, int
 extern "C" int avc_bias_grad_groups(const float* dc, int64_t bstride, float* const* dbias_tab_dev, int group_c, int B, int C, int T, void* stream) {
   AVC_REQUIRE(dc && dbias_tab_dev && B > 0 && C > 0 && C % 4 == 0 && T > 0 && group_c > 0 && group_c % 4 == 0 && C % group_c == 0, AVC_ERR_INVALID,
               "avc_bias_grad_groups: bad argument");
-  int slices = cdiv(148 * 4, C / 4);
-  if (slices > B) slices = B;
-  if (slices < 1) slices = 1;
-  const int bps = cdiv(B, slices);
-  dim3 grid(C / 4, cdiv(B, bps));
-  AVC_LAUNCH(bias_grad_kernel, grid, 256, 0, (cudaStream_t)stream, dc, bstride, (float*)nullptr, B, C, T, bps, dbias_tab_dev, group_c);
+  AVC_REQUIRE(T <= 1024, AVC_ERR_UNSUPPORTED, "avc_bias_grad_groups: T=%d > 1024", T);
+  AVC_LAUNCH(bias_grad_kernel, C / 4, 1024, 0, (cudaStream_t)stream, dc, bstride, (float*)nullptr, B, C, T, dbias_tab_dev, group_c);
   AVC_CHECK_LAUNCH("bias_grad_groups");
   return AVC_OK;
 }

@@ -7,9 +7,8 @@
 
 #include "common.cuh"
 
-// defaults of the runtime options (avc_set_option).  Both are ON since the B200 validation run of
-// tools/validate_opts.sh (profiles/r1_opts_validation.md): 56 tcgen05 / model parity tests green,
-// 39 856 -> 42 513 seg/s.  AVC_TC_ISSUE=legacy / AVC_WGRAD_REDUCE=v1 select the round-1 kernels.
+// defaults of the runtime options (avc_set_option).  AVC_TC_ISSUE=legacy / AVC_WGRAD_REDUCE=v1 select the
+// round-1 variants.
 #ifndef AVC_DEFAULT_TC_UNIFORM_ISSUE
 #define AVC_DEFAULT_TC_UNIFORM_ISSUE 1
 #endif
@@ -280,7 +279,7 @@ __device__ __forceinline__ float block_sum_256(float v, float* sh) {
 
 __global__ void __launch_bounds__(256) vae_loss_kernel(const float* __restrict__ dec, const float* __restrict__ x, int64_t n_rec,
                                                        const float* __restrict__ mu, const float* __restrict__ ls, int64_t n_lat,
-                                                       const float* __restrict__ hp, float* __restrict__ sums,
+                                                       const float* __restrict__ hp, float* __restrict__ part,
                                                        float* __restrict__ ddec, float* __restrict__ dmu, float* __restrict__ dls) {
   __shared__ float sh[8];
   const float lrec = hp[0], lkl = hp[1];
@@ -302,9 +301,17 @@ __global__ void __launch_bounds__(256) vae_loss_kernel(const float* __restrict__
   const float r = block_sum_256(s_rec, sh);
   const float k = block_sum_256(s_kl, sh);
   if (threadIdx.x == 0) {
-    atomicAdd(sums + 0, r);
-    atomicAdd(sums + 1, k);
+    part[2 * blockIdx.x + 0] = r;
+    part[2 * blockIdx.x + 1] = k;
   }
+}
+
+// sums[j] = the nb block partials part[2 i + j] added in block order
+__global__ void vae_sums_kernel(const float* __restrict__ part, int nb, float* __restrict__ sums) {
+  if (threadIdx.x >= 2) return;
+  float s = 0.f;
+  for (int i = 0; i < nb; ++i) s += part[2 * i + threadIdx.x];
+  sums[threadIdx.x] = s;
 }
 
 // ------------------------------------------------------------------ grad norm + Adam
@@ -360,7 +367,7 @@ __global__ void __launch_bounds__(256) adam_kernel(float* __restrict__ p, const 
 
 static int ew_blocks(int64_t n) {
   int64_t b = cdiv64(n, 256);
-  if (b > 148 * 8) b = 148 * 8;
+  if (b > 132 * 8) b = 132 * 8;   // AVC_VAE_PARTIALS = 2 x this
   if (b < 1) b = 1;
   return (int)b;
 }
@@ -419,7 +426,7 @@ using namespace avc;
 
 extern "C" const char* avc_last_error(void) { return g_err; }
 extern "C" const char* avc_build_info(void) {
-  return "libavc_b200 sm_100a (compute_100a) fp32-ffma + tcgen05 paths";
+  return "libavc_b200 sm_90a (compute_90a) fp32-ffma + wgmma paths";
 }
 extern "C" int64_t avc_launch_count(void) { return (int64_t)g_launches.load(); }
 
@@ -508,15 +515,13 @@ extern "C" int avc_reparam_bwd(const float* dz4, const float* ls4, const float* 
 }
 
 extern "C" int avc_vae_loss(const float* dec, const float* x, int64_t n_rec, const float* mu, const float* ls, int64_t n_lat,
-                            const float* hp, float* sums, float* ddec, float* dmu, float* dls, void* stream) {
-  AVC_REQUIRE(dec && x && mu && ls && hp && sums && n_rec > 0 && n_lat > 0, AVC_ERR_INVALID, "avc_vae_loss: bad argument");
-  cudaError_t e = cudaMemsetAsync(sums, 0, 2 * sizeof(float), (cudaStream_t)stream);
-  if (e != cudaSuccess) {
-    set_error("avc_vae_loss: memset: %s", cudaGetErrorString(e));
-    return AVC_ERR_CUDA;
-  }
-  AVC_LAUNCH(vae_loss_kernel, ew_blocks(n_rec), 256, 0, (cudaStream_t)stream, dec, x, n_rec, mu, ls, n_lat, hp, sums, ddec, dmu, dls);
+                            const float* hp, float* sums, float* part, float* ddec, float* dmu, float* dls, void* stream) {
+  AVC_REQUIRE(dec && x && mu && ls && hp && sums && part && n_rec > 0 && n_lat > 0, AVC_ERR_INVALID, "avc_vae_loss: bad argument");
+  const int nb = ew_blocks(n_rec);
+  AVC_LAUNCH(vae_loss_kernel, nb, 256, 0, (cudaStream_t)stream, dec, x, n_rec, mu, ls, n_lat, hp, part, ddec, dmu, dls);
   AVC_CHECK_LAUNCH("vae_loss");
+  AVC_LAUNCH(vae_sums_kernel, 1, 32, 0, (cudaStream_t)stream, part, nb, sums);
+  AVC_CHECK_LAUNCH("vae_sums");
   return AVC_OK;
 }
 

@@ -1,7 +1,7 @@
-// tcgen05 self-test: D[128][N] = sum over `nk` K=8 steps of A_k (128x8) * B_k (Nx8)^T with
-// tf32 inputs / fp32 accumulation, operands given as raw shared-memory images plus the
-// descriptor strides.  tests/test_gpu_tc.py uses it to pin the descriptor conventions the
-// conv kernels rely on (no-swizzle core-matrix layout, row-offset tap shifts, MN-major).
+// wgmma self-test: D[128][N] = sum over `nk` K=8 steps of A_k (128x8) * B_k (Nx8)^T with tf32 inputs / fp32
+// accumulation, operands given as raw shared-memory images plus the descriptor strides.  tests/test_gpu_tc.py uses it
+// to pin the descriptor conventions the conv kernels rely on (no-swizzle K-major core-matrix layout, row-offset tap
+// shifts).  Two warpgroups: rows 0-63 and 64-127 (the A descriptor of the second starts 8 core-matrix groups further).
 #include "common.cuh"
 #include "tc_common.cuh"
 
@@ -11,64 +11,54 @@ struct ProbeArgs {
   const float* a_img;
   const float* b_img;
   int a_bytes, b_bytes;
-  uint32_t a_lbo, a_sbo, b_lbo, b_sbo, a_kstep, b_kstep, a_off, b_off, a_layout, b_layout;
+  uint32_t a_lbo, a_sbo, b_lbo, b_sbo, a_kstep, b_kstep, a_off, b_off;
   int nk, N, reps, ld_shift;
-  uint32_t idesc;
   float* D;
   int* status;
 };
 
-__global__ void __launch_bounds__(128) tc_probe_kernel(const ProbeArgs a) {
+template <int N>
+__device__ __forceinline__ void probe_run(const ProbeArgs& a, uint32_t sa, uint32_t sb, int wg, int wt) {
+  float acc[N / 2];
+  tc::wgmma_fence();
+  for (int r = 0; r < a.reps; ++r)
+    for (int k = 0; k < a.nk; ++k) {
+      const uint64_t ad = tc::make_sdesc(sa + a.a_off + k * a.a_kstep + (uint32_t)wg * 8u * a.a_sbo, a.a_lbo, a.a_sbo);
+      const uint64_t bd = tc::make_sdesc(sb + a.b_off + k * a.b_kstep, a.b_lbo, a.b_sbo);
+      tc::wgmma_tf32<N>(acc, ad, bd, (k > 0 || r > 0) ? 1u : 0u);
+    }
+  tc::wgmma_commit();
+  tc::wgmma_wait<0>();
+  tc::acc_fence(acc, N / 2);
+  // ld_shift: columns before it stay untouched (pins that the caller's column window is honoured)
+#pragma unroll
+  for (int i = 0; i < N / 2; ++i) {
+    const int row = 64 * wg + tc::wg_acc_row(wt, i), col = tc::wg_acc_col(wt, i);
+    if (col >= a.ld_shift) a.D[(size_t)row * N + col] = acc[i];
+  }
+}
+
+__global__ void __launch_bounds__(256) tc_probe_kernel(const ProbeArgs a) {
   extern __shared__ __align__(1024) uint8_t smem[];
-  __shared__ uint64_t bar;
-  __shared__ uint32_t tmem_slot;
-  const int tid = threadIdx.x, warp = tid >> 5;
+  const int tid = threadIdx.x, wg = tid >> 7, wt = tid & 127;
   uint8_t* sa = smem;
   uint8_t* sb = smem + ((a.a_bytes + 1023) / 1024) * 1024;
-  for (int i = tid; i < a.a_bytes / 16; i += 128) reinterpret_cast<float4*>(sa)[i] = reinterpret_cast<const float4*>(a.a_img)[i];
-  for (int i = tid; i < a.b_bytes / 16; i += 128) reinterpret_cast<float4*>(sb)[i] = reinterpret_cast<const float4*>(a.b_img)[i];
+  for (int i = tid; i < a.a_bytes / 16; i += 256) reinterpret_cast<float4*>(sa)[i] = reinterpret_cast<const float4*>(a.a_img)[i];
+  for (int i = tid; i < a.b_bytes / 16; i += 256) reinterpret_cast<float4*>(sb)[i] = reinterpret_cast<const float4*>(a.b_img)[i];
   tc::fence_proxy_async_smem();
-  if (tid == 0) {
-    tc::mbar_init(&bar, 1);
-    tc::fence_mbar_init();
-  }
-  uint32_t ncols = 32;
-  while ((int)ncols < a.N) ncols <<= 1;
-  if (warp == 0) tc::tmem_alloc(&tmem_slot, ncols);
-  tc::tc_fence_before();
   __syncthreads();
-  tc::tc_fence_after();
-  const uint32_t tbase = tmem_slot;
-  long long t0 = 0;
+  const long long t0 = clock64();
+  switch (a.N) {
+#define PROBE_CASE(n) \
+  case n: probe_run<n>(a, tc::smem_u32(sa), tc::smem_u32(sb), wg, wt); break;
+    PROBE_CASE(16) PROBE_CASE(32) PROBE_CASE(48) PROBE_CASE(64) PROBE_CASE(80) PROBE_CASE(96) PROBE_CASE(112) PROBE_CASE(128)
+    PROBE_CASE(144) PROBE_CASE(160) PROBE_CASE(176) PROBE_CASE(192) PROBE_CASE(208) PROBE_CASE(224) PROBE_CASE(240) PROBE_CASE(256)
+#undef PROBE_CASE
+  }
   if (tid == 0) {
-    t0 = clock64();
-    for (int r = 0; r < a.reps; ++r)
-      for (int k = 0; k < a.nk; ++k) {
-        const uint64_t ad = tc::make_sdesc(tc::smem_u32(sa) + a.a_off + k * a.a_kstep, a.a_lbo, a.a_sbo, a.a_layout);
-        const uint64_t bd = tc::make_sdesc(tc::smem_u32(sb) + a.b_off + k * a.b_kstep, a.b_lbo, a.b_sbo, a.b_layout);
-        tc::mma_tf32(tbase, ad, bd, a.idesc, (k > 0 || r > 0) ? 1u : 0u);
-      }
-    tc::mma_commit(&bar);
+    a.status[0] = 0;
+    a.status[1] = (int)(clock64() - t0);  // cycles: issue of the first MMA -> all complete (warpgroup 0)
   }
-  const bool ok = tc::mbar_wait(&bar, 0, a.status, 1);
-  if (tid == 0) a.status[1] = (int)(clock64() - t0);  // cycles: issue of the first MMA -> all complete
-  tc::tc_fence_after();
-  if (ok) {
-    // ld_shift != 0: the 16-column loads start at column ld_shift + 16 j (NOT a multiple of 16) -- pins that
-    // tcgen05.ld accepts any start column (the conv epilogue reads samples stacked at an arbitrary pitch)
-    const int sh = a.ld_shift;
-    for (int c0 = 0; c0 + sh + 16 <= (int)ncols || c0 == 0; c0 += 16) {
-      if (c0 + sh >= a.N) break;
-      float v[16];
-      tc::tmem_ld16(tbase + ((uint32_t)(warp * 32) << 16) + (uint32_t)(c0 + sh), v);
-#pragma unroll
-      for (int i = 0; i < 16; ++i)
-        if (c0 + sh + i < a.N) a.D[(size_t)tid * a.N + c0 + sh + i] = v[i];
-    }
-  }
-  tc::tc_fence_before();
-  __syncthreads();
-  if (warp == 0) tc::tmem_dealloc(tbase, ncols);
 }
 
 // Store-path probe: every CTA writes `bytes` to its own region of `dst`; mode 0 = coalesced STG.128 from registers,
@@ -124,17 +114,19 @@ extern "C" int avc_tc_probe_gemm(const float* a_img, int a_bytes, const float* b
   AVC_REQUIRE(a_img && b_img && strides && D && status, AVC_ERR_INVALID, "avc_tc_probe_gemm: null argument");
   AVC_REQUIRE(a_bytes % 16 == 0 && b_bytes % 16 == 0 && N % 16 == 0 && N >= 16 && N <= 256 && nk >= 1, AVC_ERR_INVALID,
               "avc_tc_probe_gemm: bad sizes");
+  // tf32 wgmma reads K-major operands only, and the kernels use the no-swizzle layout
+  AVC_REQUIRE(a_mn == 0 && b_mn == 0 && strides[8] == 0 && strides[9] == 0, AVC_ERR_UNSUPPORTED,
+              "avc_tc_probe_gemm: tf32 operands must be K-major without swizzle");
   ProbeArgs a;
   a.a_img = a_img; a.b_img = b_img; a.a_bytes = a_bytes; a.b_bytes = b_bytes;
   a.a_lbo = strides[0]; a.a_sbo = strides[1]; a.b_lbo = strides[2]; a.b_sbo = strides[3];
   a.a_kstep = strides[4]; a.b_kstep = strides[5]; a.a_off = strides[6]; a.b_off = strides[7];
-  a.a_layout = strides[8]; a.b_layout = strides[9];
-  a.nk = nk; a.N = N; a.reps = reps < 1 ? 1 : reps; a.ld_shift = g_probe_ld_shift; a.idesc = tc::make_idesc_tf32(128, N, a_mn, b_mn); a.D = D; a.status = status;
+  a.nk = nk; a.N = N; a.reps = reps < 1 ? 1 : reps; a.ld_shift = g_probe_ld_shift; a.D = D; a.status = status;
   const int smem = ((a_bytes + 1023) / 1024) * 1024 + b_bytes + 1024;
   AVC_REQUIRE(smem <= 200 * 1024, AVC_ERR_INVALID, "avc_tc_probe_gemm: images too large");
   cudaError_t e = cudaFuncSetAttribute(tc_probe_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
   if (e != cudaSuccess) { set_error("avc_tc_probe_gemm: %s", cudaGetErrorString(e)); return AVC_ERR_CUDA; }
-  tc_probe_kernel<<<1, 128, smem, (cudaStream_t)stream>>>(a);
+  tc_probe_kernel<<<1, 256, smem, (cudaStream_t)stream>>>(a);
   AVC_CHECK_LAUNCH("tc_probe");
   return AVC_OK;
 }

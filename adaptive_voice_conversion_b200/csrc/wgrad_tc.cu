@@ -1,31 +1,29 @@
-// Conv weight gradient on the tcgen05 tensor cores (TF32 in, fp32 accumulate in TMEM):
+// Conv weight gradient on the tensor cores (mma.sync m16n8k8, TF32 in, fp32 accumulate in registers):
 //   dW[co][ci][j] += sum_{b,t} dc[b][co][t] * xpad[b][ci][t + j]        (stride 1)
 // (autograd of pad_layer + nn.Conv1d w.r.t. the weight, model.py:21-32 under solver.py:90).
 //
-// GEMM view: M = co (128 per CTA), N = ci (64 per CTA), reduction K = time rows of a batch
-// slice.  Both operands are MN-major: the A4 activation layout [c/4][t][4] already keeps 4
-// channels of one time step in a 16-byte unit, so staging is a plain LDG.128 -> STS.128 of
-// units into the tensor core's MN-major TF32 layout (UMMA layout code 1, "SW128_32B"):
+// GEMM view: M = co (128 per CTA), N = taps x ci (WT_NT ci per CTA), reduction K = time rows of a batch
+// slice.  The A4 activation layout [c/4][t][4] keeps 4 channels of one time step in a 16-byte unit,
+// so staging is a plain cp.async of units into an XOR-swizzled MN-major tile:
 //     byte(c, row) = (c/32)*LBO + row*128 + ((((c%32)/8) ^ (row%4)) * 32) + (c%8)*4
-// measured on B200 with tools/diag_mn4.py / diag_mn5.py (the XOR is keyed on the absolute
-// shared-memory row, so a descriptor start shifted by whole rows addresses shifted rows).
-// The K taps are therefore K descriptor starts (row shifts) into ONE staged input tile whose
-// reflect padding is resolved while staging; tap j accumulates into TMEM columns [j*N, (j+1)*N).
+// (conflict-free 16-byte stores).  tf32 wgmma reads K-major operands only, so the MMAs are warp-level:
+// every warp owns 16 co rows and loads its fragments from the staged tile with 32-bit shared loads.
+// The K taps are row shifts into ONE staged input tile whose reflect padding is resolved while staging.
 // Each CTA owns (co tile, ci tile, batch slice); partial sums go to a scratch buffer
-// [slice][tap][ci/4][co][4] with coalesced 16-byte stores and are reduced into the canonical
-// nn.Conv1d gradient layout by wgrad_tc_reduce_kernel (deterministic, no atomics).
+// [slice][tap][ci/4][co][4] and are reduced into the canonical nn.Conv1d gradient layout by
+// wgrad_tc_reduce_kernel (deterministic, no atomics), or added in place (ATOMIC, see below).
 #include "common.cuh"
 #include "tc_common.cuh"
 
 namespace avc {
 
-constexpr int WT_NT = 64;  // ci columns per CTA
+constexpr int WT_NT = 32;  // ci columns per CTA (K x 32 accumulator columns: <= 128 registers per thread)
 
 struct WgTcArgs {
   avc_wgrad_desc d;
   float* scratch;
   long long* dbg;   // optional per-CTA phase cycle counters (avc_wgrad_tc_set_debug)
-  int nslices, tiles_per_slice, G, RA, RX, ntpad, ncols_tmem, coutp, TX, H;  // H: rows of one parity block (stride 2)
+  int nslices, tiles_per_slice, G, RA, RX, ntpad, coutp, TX, H;  // H: rows of one parity block (stride 2)
   uint32_t buf_bytes, x_off;
   int* status;
 };
@@ -48,406 +46,166 @@ __device__ __forceinline__ uint32_t mn_unit_off(int q, int row, uint32_t atom_by
   return (uint32_t)(q >> 3) * atom_bytes + (uint32_t)row * 128u + (uint32_t)((((q & 7) >> 1) ^ (row & 3)) << 5) + (uint32_t)((q & 1) << 4);
 }
 
-// UI (uniform issue): see conv_tc.cu; UI = false is the round-1 issue loop.
-// ATOMIC: the epilogue adds the CTA's partial straight into ONE accumulation buffer per layer
-// ([tap][ci/4][co][4], vector red.global.add.v4.f32) instead of writing a per-slice partial: no
-// scratch round trip and no per-layer reduction launch (avc_wgrad_acc_flush unpacks every layer at
-// the end of the backward pass); the price is a run-to-run summation order.
-template <bool UI, bool ATOMIC>
-__global__ void __launch_bounds__(128, 1) conv_wgrad_tc_kernel(const WgTcArgs a) {
-  extern __shared__ __align__(1024) uint8_t smem[];
-  __shared__ uint64_t bar_free[2], bar_done;
-  __shared__ uint32_t tmem_slot;
-  const avc_wgrad_desc& d = a.d;
-  const int tid = threadIdx.x, warp = UI ? tc::warp_idx_sync() : (tid >> 5);
-  const int ci0 = blockIdx.x * WT_NT, co0 = blockIdx.y * 128, sl = blockIdx.z;
-  const int K = d.K, T = d.Tout, TX = a.TX;  // padded input positions per sample
-  const int S = d.stride, H = a.H;
-  const int tile0 = sl * a.tiles_per_slice;
-  const int ntiles_all = cdiv(d.B, a.G);
-  const int tile1 = min(ntiles_all, tile0 + a.tiles_per_slice);
+// one m16n8k8 TF32 tensor-core MMA (operands are fp32 bit patterns; the tensor core reads their TF32 part)
+__device__ __forceinline__ void mma_tf32_16x8x8(float* c, uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint32_t b0, uint32_t b1) {
+  asm volatile("mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, {%0, %1, %2, %3};"
+               : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
+               : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "r"(b0), "r"(b1));
+}
+__device__ __forceinline__ uint32_t lds_u32(const uint8_t* p) { return *reinterpret_cast<const uint32_t*>(p); }
 
-  if (tid == 0) {
-    tc::mbar_init(&bar_free[0], 1);
-    tc::mbar_init(&bar_free[1], 1);
-    tc::mbar_init(&bar_done, 1);
-    tc::fence_mbar_init();
-  }
-  if (warp == 0) tc::tmem_alloc(&tmem_slot, (uint32_t)a.ncols_tmem);
-  tc::tc_fence_before();
-  __syncthreads();
-  tc::tc_fence_after();
-  const uint32_t tbase = __shfl_sync(0xffffffffu, tmem_slot, 0);
+// Accumulator of one warp: co rows 16 warp + lane / 4 (+ 8) of the 128-row tile, n8 tile nt = 4 tap + (ci / 8) of the
+// WT_NT = 32 ci columns; acc[4 nt + {0, 1}] = columns 8 (nt % 4) + 2 (lane % 4) + {0, 1}, acc[4 nt + {2, 3}] the row + 8.
+constexpr int WG_NT_MAX = 4 * 8;   // n8 tiles for K <= 8
+
+// All MMAs of one staged tile (nsamp samples, reduction over their time rows) for the warp's 16 co rows.
+__device__ __forceinline__ void wgrad_mma_tile(const WgTcArgs& a, const uint8_t* sA, const uint8_t* sX, int nsamp, float* acc, int warp,
+                                               int lane) {
+  const int K = a.d.K, T = a.d.Tout, S = a.d.stride, H = a.H, TX = a.TX;
   const uint32_t atomA = (uint32_t)a.RA * 128u, atomX = (uint32_t)a.RX * 128u;
-  const uint32_t idesc = tc::make_idesc_tf32(128, a.ntpad, 1, 1);
-  const int nq_x = a.ntpad >> 2;  // 16-byte units per row of the x operand
-  bool ok = true;
-  const uint32_t smem_base = tc::smem_u32(smem);
-  long long t_begin = 0, c_stage = 0, c_free = 0, c_issue = 0;
-  if (a.dbg) t_begin = clock64();
-
-  for (int tile = tile0; tile < tile1; ++tile) {
-    const int it = tile - tile0;
-    const int buf = it & 1;
-    const long long q0 = a.dbg ? clock64() : 0;
-    if (it >= 2) ok = tc::mbar_wait(&bar_free[buf], (uint32_t)((it >> 1) - 1) & 1u, a.status, 6) && ok;
-    const long long q1 = a.dbg ? clock64() : 0;
-    uint8_t* sA = smem + (size_t)buf * a.buf_bytes;
-    uint8_t* sX = sA + a.x_off;
-    const int b0 = tile * a.G;
-    const int nsamp = min(a.G, d.B - b0);
-    // ---- stage dc: [4 atoms of 32 co][G*T rows][128 B]; cp.async keeps ~50 16-byte copies per
-    // thread in flight (the tensor core truncates fp32 -> tf32; a uniform ~1e-3 shrink of dW).
-    // Row -> (sample, time) is decomposed once per row and reused for all channel chunks.
-    for (int r = tid; r < nsamp * T; r += 128) {
-      const int g = r / T, t = r - g * T;
-      const float* src = d.dc + (size_t)(b0 + g) * d.dc_bstride + (size_t)t * 4;
-#pragma unroll 8
-      for (int q = 0; q < 32; ++q) {
-        const int co = co0 + 4 * q;
-        const bool cv = co < d.Cout;
-        cp_async16(sA + mn_unit_off(q, r, atomA), src + (size_t)((cv ? co : 0) >> 2) * T * 4, cv);
-      }
-    }
-    // ---- stage x with the reflect padding resolved: [ntpad/32 atoms][G*(T+K-1) rows][128 B]
-    for (int r0 = tid; r0 < nsamp * TX; r0 += 128) {
-      const int g = r0 / TX, u = r0 - g * TX;
-      // stride 2: even and odd padded positions go to separate row blocks, so tap j addresses
-      // rows (j&1)*H + t + (j>>1) -- contiguous in t
-      const int r = S == 1 ? r0 : g * 2 * H + (u & 1) * H + (u >> 1);
-      const int p = src_pos(u - d.pad_left, d.Tin, AVC_PAD_REFLECT, 1);
-      const float* src = d.x + (size_t)(b0 + g) * d.x_bstride + (size_t)(p >= 0 ? p : 0) * 4;
-#pragma unroll 8
-      for (int q = 0; q < nq_x; ++q) {
-        const int ci = ci0 + 4 * q;
-        const bool v = ci < d.Cin && p >= 0;
-        cp_async16(sX + mn_unit_off(q, r, atomX), src + (size_t)((v ? ci : 0) >> 2) * d.Tin * 4, v);
-      }
-    }
-    asm volatile("cp.async.commit_group;" ::: "memory");
-    asm volatile("cp.async.wait_group 0;" ::: "memory");
-    tc::fence_proxy_async_smem();
-    ok = __syncthreads_and(ok) != 0;  // also makes `ok` block-uniform for the issue loop below
-    const long long q2 = a.dbg ? clock64() : 0;
-    c_free += q1 - q0;
-    c_stage += q2 - q1;
-    if (warp == 0) {  // warp-converged issue loop, one elected lane per instruction (uniform descriptors)
-      if (__all_sync(0xffffffffu, ok)) {
-        if constexpr (UI) {
-          tc::tc_fence_after();
-          // everything the MMAs consume is re-derived from lane-0 broadcasts: ptxas then proves the
-          // values warp-uniform and keeps the whole issue loop on the uniform datapath
-          const int it_u = __shfl_sync(0xffffffffu, it, 0), nsamp_u = __shfl_sync(0xffffffffu, nsamp, 0);
-          const uint32_t tb_u = __shfl_sync(0xffffffffu, tbase, 0);
-          const uint32_t sbase = __shfl_sync(0xffffffffu, smem_base, 0) + (uint32_t)(it_u & 1) * a.buf_bytes;
-          const uint32_t a_lo0 = tc::sdesc_lo(sbase, atomA), b_lo0 = tc::sdesc_lo(sbase + a.x_off, atomX);
-          const uint32_t hi = tc::sdesc_hi(512, 1);
-          const int nks = T >> 3;
-          for (int g = 0; g < nsamp_u; ++g) {
-            // loop-carried 64-bit descriptors: one k-step = 8 rows = 64 descriptor units on both operands
-            uint64_t a_desc = tc::sdesc64(a_lo0 + (uint32_t)(g * T) * 8u, hi);
-            uint64_t b_ks = tc::sdesc64(b_lo0 + (uint32_t)(S == 1 ? g * TX : g * 2 * H) * 8u, hi);
-            for (int ks = 0; ks < nks; ++ks) {
-              const uint32_t acc = (it_u | g | ks) ? 1u : 0u;
-              uint32_t dcol = tb_u;
-              if (S == 1) {
-                uint64_t b_desc = b_ks;
-                if (K == 5) {
-  #pragma unroll
-                  for (int j = 0; j < 5; ++j) {
-                    tc::mma_tf32_elect(dcol, a_desc, b_desc, idesc, acc);
-                    b_desc += 8u;
-                    dcol += (uint32_t)a.ntpad;
-                  }
-                } else {
-                  for (int j = 0; j < K; ++j) {
-                    tc::mma_tf32_elect(dcol, a_desc, b_desc, idesc, acc);
-                    b_desc += 8u;
-                    dcol += (uint32_t)a.ntpad;
-                  }
-                }
-              } else {
-                for (int j = 0; j < K; ++j) {
-                  tc::mma_tf32_elect(dcol, a_desc, b_ks + (uint32_t)((j & 1) * H + (j >> 1)) * 8u, idesc, acc);
-                  dcol += (uint32_t)a.ntpad;
-                }
-              }
-              a_desc += 64u;
-              b_ks += 64u;
-            }
-          }
-        } else {
-          tc::tc_fence_after();
-          const uint32_t sbase = smem_base + (uint32_t)buf * a.buf_bytes;
-          const uint32_t a_lo0 = tc::sdesc_lo(sbase, atomA), b_lo0 = tc::sdesc_lo(sbase + a.x_off, atomX);
-          const uint32_t hi = tc::sdesc_hi(512, 1);
-          for (int g = 0; g < nsamp; ++g)
-            for (int ks = 0; ks < T / 8; ++ks) {
-              const uint32_t a_lo = a_lo0 + (uint32_t)(g * T + 8 * ks) * 8u;         // rows * 128 B >> 4
-              const uint32_t b_base = b_lo0 + (uint32_t)((S == 1 ? g * TX : g * 2 * H) + 8 * ks) * 8u;
-              uint32_t dcol = tbase;
-              const uint32_t acc = (it == 0 && g == 0 && ks == 0) ? 0u : 1u;
-              if (S == 1) {
-                uint32_t b_lo = b_base;
-                for (int j = 0; j < K; ++j) {
-                  if (tc::elect_one()) tc::mma_tf32_lohi(dcol, a_lo, hi, b_lo, hi, idesc, acc);
-                  b_lo += 8u;
-                  dcol += (uint32_t)a.ntpad;
-                }
-              } else {
-                for (int j = 0; j < K; ++j) {
-                  const uint32_t b_lo = b_base + (uint32_t)((j & 1) * H + (j >> 1)) * 8u;
-                  if (tc::elect_one()) tc::mma_tf32_lohi(dcol, a_lo, hi, b_lo, hi, idesc, acc);
-                  dcol += (uint32_t)a.ntpad;
-                }
-              }
-            }
-        }
-        __syncwarp();
-        if (tc::elect_one()) tc::mma_commit(&bar_free[buf]);
-      }
-      if (a.dbg) c_issue += clock64() - q2;
-    }
-  }
-  if (warp == 0) {
-    __syncwarp();
-    if (tc::elect_one()) tc::mma_commit(&bar_done);
-  }
-  const long long q3 = a.dbg ? clock64() : 0;
-  ok = tc::mbar_wait(&bar_done, 0, a.status, 7) && ok;
-  ok = __syncthreads_and(ok) != 0;
-  tc::tc_fence_after();
-  const long long q4 = a.dbg ? clock64() : 0;
-  if (ok && tile1 > tile0) {
-    // partial dW of this slice: scratch[sl][tap][ci/4][co][4]
-    const int co = co0 + tid;
-    const uint32_t lane_addr = tbase + ((uint32_t)(warp * 32) << 16);
-    for (int j = 0; j < K; ++j) {
-      float* sbase = a.scratch + (((size_t)(ATOMIC ? 0 : sl) * K + j) * (size_t)(d.Cin >> 2)) * (size_t)a.coutp * 4;
-      for (int c0 = 0; c0 < a.ntpad; c0 += 16) {
-        float v[16];
-        tc::tmem_ld16(lane_addr + (uint32_t)(j * a.ntpad + c0), v);
+  const int gid = lane >> 2, tig = lane & 3;
+  const int m0 = warp * 16 + gid, m1 = m0 + 8;
+  const uint8_t* pA0 = sA + ((m0 & 3) << 2);
+  const uint8_t* pA1 = sA + ((m1 & 3) << 2);
+  for (int g = 0; g < nsamp; ++g) {
+    for (int ks = 0; ks < T / 8; ++ks) {
+      const int r0 = g * T + 8 * ks + tig;
+      const uint32_t a0 = lds_u32(pA0 + mn_unit_off(m0 >> 2, r0, atomA)), a1 = lds_u32(pA1 + mn_unit_off(m1 >> 2, r0, atomA));
+      const uint32_t a2 = lds_u32(pA0 + mn_unit_off(m0 >> 2, r0 + 4, atomA)), a3 = lds_u32(pA1 + mn_unit_off(m1 >> 2, r0 + 4, atomA));
 #pragma unroll
-        for (int i4 = 0; i4 < 16; i4 += 4) {
-          const int ci = ci0 + c0 + i4;
-          if (ci < d.Cin) {
-            float* p = sbase + ((size_t)(ci >> 2) * a.coutp + co) * 4;
-            if constexpr (ATOMIC)
-              asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(p), "f"(v[i4]), "f"(v[i4 + 1]), "f"(v[i4 + 2]), "f"(v[i4 + 3]) : "memory");
-            else
-              st4(p, make_float4(v[i4], v[i4 + 1], v[i4 + 2], v[i4 + 3]));
-          }
+      for (int nt = 0; nt < WG_NT_MAX; ++nt) {
+        if (nt < 4 * K) {
+          const int j = nt >> 2, n = (nt & 3) * 8 + gid;
+          // tap j reads padded input position t + j (stride 1), or parity block j & 1, row t + j / 2 (stride 2)
+          const int xr = (S == 1 ? g * TX + j : g * 2 * H + (j & 1) * H + (j >> 1)) + 8 * ks + tig;
+          const uint8_t* pX = sX + ((n & 3) << 2);
+          const uint32_t b0 = lds_u32(pX + mn_unit_off(n >> 2, xr, atomX)), b1 = lds_u32(pX + mn_unit_off(n >> 2, xr + 4, atomX));
+          mma_tf32_16x8x8(acc + 4 * nt, a0, a1, a2, a3, b0, b1);
         }
       }
     }
   }
-  tc::tc_fence_before();
-  __syncthreads();
-  if (a.dbg && tid == 0) {
-    long long* o = a.dbg + ((size_t)(blockIdx.z * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x) * 8;
-    const long long q5 = clock64();
-    o[0] = t_begin; o[1] = q5; o[2] = c_stage; o[3] = c_free; o[4] = c_issue; o[5] = q4 - q3; o[6] = q5 - q4; o[7] = tile1 - tile0;
-  }
-  if (warp == 0) tc::tmem_dealloc(tbase, (uint32_t)a.ncols_tmem);
 }
 
-// ---------------------------------------------------------------------------------------------------------------
-// Round-2 variant ("wgrad_split"): 8 staging / epilogue warps + a dedicated MMA warp, so that staging tile i+1 runs
-// under the MMAs of tile i (the kernel above issues from staging warp 0, whose blocking issue loop serialises the two:
-// 17.3 K staging + 16.6 K issue of a 43 K-cycle CTA, tools/diag_wgrad.py).  Pipelines: full[2] (256 staging arrivals),
-// free[2] (tcgen05.commit), done.  (Staging the operands with swizzled tensor-map TMA copies instead was tried and
-// dropped: CU_TENSOR_MAP_SWIZZLE_128B* needs 128-byte inner rows, the A4 layout has 16-byte ones.)
-constexpr int WS_STAGE_THREADS = 256;
-constexpr int WS_THREADS = WS_STAGE_THREADS + 32;
-
+// partial dW of this CTA: scratch[sl][tap][ci/4][co][4] (ATOMIC: added into the layer's accumulation buffer)
 template <bool ATOMIC>
-__global__ void __launch_bounds__(WS_THREADS, 1) conv_wgrad_split_kernel(const WgTcArgs a) {
-  extern __shared__ __align__(1024) uint8_t smem[];
-  __shared__ uint64_t bar_full[2], bar_free[2], bar_done;
-  __shared__ uint32_t tmem_slot;
+__device__ __forceinline__ void wgrad_store(const WgTcArgs& a, const float* acc, int warp, int lane) {
   const avc_wgrad_desc& d = a.d;
-  const int tid = threadIdx.x, warp = tc::warp_idx_sync(), lane = tid & 31;
   const int ci0 = blockIdx.x * WT_NT, co0 = blockIdx.y * 128, sl = blockIdx.z;
-  const int K = d.K, T = d.Tout, TX = a.TX;
-  const int S = d.stride, H = a.H;
-  const int tile0 = sl * a.tiles_per_slice;
-  const int tile1 = min(cdiv(d.B, a.G), tile0 + a.tiles_per_slice);
-  if (tid == 0) {
-    tc::mbar_init(&bar_full[0], WS_STAGE_THREADS);
-    tc::mbar_init(&bar_full[1], WS_STAGE_THREADS);
-    tc::mbar_init(&bar_free[0], 1);
-    tc::mbar_init(&bar_free[1], 1);
-    tc::mbar_init(&bar_done, 1);
-    tc::fence_mbar_init();
-  }
-  if (warp == 8) tc::tmem_alloc(&tmem_slot, (uint32_t)a.ncols_tmem);
-  tc::tc_fence_before();
-  __syncthreads();
-  tc::tc_fence_after();
-  const uint32_t tbase = tmem_slot;
-  const uint32_t atomA = (uint32_t)a.RA * 128u, atomX = (uint32_t)a.RX * 128u;
-  const int nq_x = a.ntpad >> 2;
-  long long t_begin = 0, c_stage = 0, c_free = 0, c_issue = 0, q3 = 0, q4 = 0;
-  if (a.dbg) t_begin = clock64();
-  bool ok = true;
-
-  if (warp < 8) {
-    // ============================================================ staging warps: one tile of copies at a time; the
-    // tile is handed to the MMA warp as soon as its copies have landed, BEFORE waiting for the next free buffer
-    for (int tile = tile0; tile < tile1 && ok; ++tile) {
-      const int it = tile - tile0;
-      const int buf = it & 1;
-      const long long q0 = a.dbg ? clock64() : 0;
-      if (it >= 2) ok = tc::mbar_wait(&bar_free[buf], (uint32_t)((it >> 1) - 1) & 1u, a.status, 6);
-      const long long q1 = a.dbg ? clock64() : 0;
-      if (!ok) break;
-      uint8_t* sA = smem + (size_t)buf * a.buf_bytes;
-      uint8_t* sX = sA + a.x_off;
-      const int b0 = tile * a.G;
-      const int nsamp = min(a.G, d.B - b0);
-      // Unit -> lane mapping: a warp writes 4 rows x the 8 units of one 128-byte atom row = four whole bank sweeps.
-      // (One row per lane, as in the round-1 kernel, puts 32 lanes on 4 bank groups: an 8-way conflict that made the
-      // shared-memory side of every cp.async 8x slower -- staging was 6.5 K cycles per tile against 1.5 K of issue.)
-      // Each thread walks rows r_lo, r_lo + 16 (dc: + 8), ... with (g, t) kept incrementally: no division per unit.
-      // Unit -> lane mapping: a warp writes 4 rows x the 8 units of one 128-byte atom row = four whole bank sweeps, and
-      // each thread walks rows r_lo, r_lo + 8 (x: + 16), ... with (g, t) kept incrementally: no division per unit.
-      // (Measured alternatives, tools/diag_wgrad.py: one row per lane as in round 1 -- same time; LDG.128 -> registers
-      // -> STS.128 with eight loads in flight -- 40 % slower.  The ~6.5 K cycles per 97 KB tile are not the bank mapping.)
-      {
-        // dc: 4 atoms x 8 units per row; 256 threads = 8 warps = (2 row groups of 4 rows) x 4 atoms
-        const int q = ((tid >> 5) & 3) * 8 + (tid & 7), r_lo = ((tid >> 7) << 2) + ((tid >> 3) & 3);
-        const int co = co0 + 4 * q;
-        const bool cv = co < d.Cout;
-        const float* colsrc = d.dc + (size_t)((cv ? co : 0) >> 2) * T * 4;
-        int g = r_lo / T, t = r_lo - g * T;
-        for (int r = r_lo; r < nsamp * T; r += 8) {
-          cp_async16(sA + mn_unit_off(q, r, atomA), colsrc + (size_t)(b0 + g) * d.dc_bstride + (size_t)t * 4, cv);
-          t += 8;
-          while (t >= T) { t -= T; ++g; }
-        }
-      }
-      {
-        // x: ntpad/32 atoms x 8 units per row; a warp = 4 rows of one atom, the 8 warps cover natom atoms x (8/natom) row groups
-        const int natom = nq_x >> 3, wpa = 8 / natom;             // warps per atom
-        const int w = tid >> 5, atom = w % natom, rg = w / natom;  // row group of this warp
-        const int q = atom * 8 + (tid & 7), r_lo = (rg << 2) + ((tid >> 3) & 3), rstep = wpa << 2;
-        const int ci = ci0 + 4 * q;
-        const bool civ = ci < d.Cin;
-        const float* colsrc = d.x + (size_t)((civ ? ci : 0) >> 2) * d.Tin * 4;
-        int g = r_lo / TX, u = r_lo - g * TX;
-        for (int r0 = r_lo; r0 < nsamp * TX; r0 += rstep) {
-          const int r = S == 1 ? r0 : g * 2 * H + (u & 1) * H + (u >> 1);
-          const int p = src_pos(u - d.pad_left, d.Tin, AVC_PAD_REFLECT, 1);
-          const bool v = civ && p >= 0;
-          cp_async16(sX + mn_unit_off(q, r, atomX), colsrc + (size_t)(b0 + g) * d.x_bstride + (size_t)(p >= 0 ? p : 0) * 4, v);
-          u += rstep;
-          while (u >= TX) { u -= TX; ++g; }
-        }
-      }
-      asm volatile("cp.async.commit_group;" ::: "memory");
-      asm volatile("cp.async.wait_group 0;" ::: "memory");
-      tc::fence_proxy_async_smem();
-      tc::mbar_arrive(&bar_full[buf]);
-      if (a.dbg) {
-        const long long q2 = clock64();
-        c_free += q1 - q0;
-        c_stage += q2 - q1;
-      }
-    }
-  } else {
-    // ============================================================ MMA issuer (warp 8), uniform datapath.
-    // ALL TAPS IN ONE MMA: for a 32-channel block of x, tap j is the same swizzled atom one row (128 B) further, so
-    // a B descriptor with LBO = 128 B addresses the K taps as K consecutive 32-column atoms: one MMA of N = 32 K
-    // columns per k-step and channel block (stride 2: the even and the odd taps form two such groups) instead of K
-    // MMAs of N = 64 -- the dc operand is read once per k-step instead of K times (the MMAs here are bound by
-    // shared-memory operand traffic), 2 instead of 5 instructions per k-step.
-    const int NT = K * 32;                 // TMEM columns of one 32-channel block
-    const int natom = a.ntpad >> 5;
-    const int ne = (K + 1) >> 1, no = K >> 1;
-    const uint32_t idesc_all = tc::make_idesc_tf32(128, NT, 1, 1);
-    const uint32_t idesc_e = tc::make_idesc_tf32(128, 32 * ne, 1, 1), idesc_o = tc::make_idesc_tf32(128, no ? 32 * no : 32, 1, 1);
-    const uint32_t tb_u = __shfl_sync(0xffffffffu, tbase, 0);
-    const uint32_t smem_base = __shfl_sync(0xffffffffu, tc::smem_u32(smem), 0);
-    const uint32_t hi = tc::sdesc_hi(512, 1);
-    const int nks = T >> 3;
-    for (int tile = tile0; tile < tile1 && ok; ++tile) {
-      const int it_u = tile - tile0;
-      const int nsamp_u = min(a.G, d.B - tile * a.G);
-      ok = __all_sync(0xffffffffu, tc::mbar_wait(&bar_full[it_u & 1], (uint32_t)(it_u >> 1) & 1u, a.status, 8));
-      if (!ok) break;
-      tc::tc_fence_after();
-      const long long q2 = a.dbg ? clock64() : 0;
-      const uint32_t sbase = smem_base + (uint32_t)(it_u & 1) * a.buf_bytes;
-      const uint32_t a_lo0 = tc::sdesc_lo(sbase, atomA);
-      for (int g = 0; g < nsamp_u; ++g) {
-        uint64_t a_desc = tc::sdesc64(a_lo0 + (uint32_t)(g * T) * 8u, hi);
-        const uint32_t xrow0 = (uint32_t)(S == 1 ? g * TX : g * 2 * H) * 8u;   // in 16-byte descriptor units
-        for (int ks = 0; ks < nks; ++ks) {
-          const uint32_t acc = (it_u | g | ks) ? 1u : 0u;
-          for (int cb = 0; cb < natom; ++cb) {
-            const uint32_t b_lo = tc::sdesc_lo(sbase + a.x_off + (uint32_t)cb * atomX, 128u) + xrow0 + (uint32_t)ks * 64u;
-            const uint32_t dcol = tb_u + (uint32_t)(cb * NT);
-            if (S == 1) {
-              tc::mma_tf32_elect(dcol, a_desc, tc::sdesc64(b_lo, hi), idesc_all, acc);
-            } else {
-              tc::mma_tf32_elect(dcol, a_desc, tc::sdesc64(b_lo, hi), idesc_e, acc);
-              if (no) tc::mma_tf32_elect(dcol + (uint32_t)(32 * ne), a_desc, tc::sdesc64(b_lo + (uint32_t)H * 8u, hi), idesc_o, acc);
-            }
-          }
-          a_desc += 64u;
-        }
-      }
-      __syncwarp();
-      if (tc::elect_one()) tc::mma_commit(&bar_free[it_u & 1]);
-      __syncwarp();
-      if (a.dbg) c_issue += clock64() - q2;
-    }
-    __syncwarp();
-    if (tc::elect_one()) tc::mma_commit(&bar_done);
-  }
-  if (a.dbg) q3 = clock64();
-  ok = tc::mbar_wait(&bar_done, 0, a.status, 7) && ok;
-  ok = __syncthreads_and(ok) != 0;
-  tc::tc_fence_after();
-  if (a.dbg) q4 = clock64();
-  if (ok && tile1 > tile0 && warp < 8) {
-    // TMEM column of (32-channel block cb, tap j, channel c) = cb * 32 K + slot(j) * 32 + c, slot(j) = j (stride 1) or the
-    // even taps first (stride 2); 8 warps: lane quarter = warp & 3, the 16-column chunks are split between its two warps
-    const int quarter = warp & 3, half = warp >> 2;
-    const int co = co0 + quarter * 32 + lane;
-    const uint32_t lane_addr = tbase + ((uint32_t)(quarter * 32) << 16);
-    const int nch = a.ntpad >> 4;
-    const int NT = K * 32, ne = (K + 1) >> 1;
-    for (int j = 0; j < K; ++j) {
-      const int slot = S == 1 ? j : ((j & 1) ? ne + (j >> 1) : (j >> 1));
-      float* sbase = a.scratch + (((size_t)(ATOMIC ? 0 : sl) * K + j) * (size_t)(d.Cin >> 2)) * (size_t)a.coutp * 4;
-      for (int ch = half; ch < nch; ch += 2) {
-        const int c0 = ch << 4;
-        float v[16];
-        tc::tmem_ld16(lane_addr + (uint32_t)((c0 >> 5) * NT + slot * 32 + (c0 & 31)), v);
+  const int gid = lane >> 2, tig = lane & 3;
 #pragma unroll
-        for (int i4 = 0; i4 < 16; i4 += 4) {
-          const int ci = ci0 + c0 + i4;
-          if (ci < d.Cin) {
-            float* p = sbase + ((size_t)(ci >> 2) * a.coutp + co) * 4;
-            if constexpr (ATOMIC)
-              asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(p), "f"(v[i4]), "f"(v[i4 + 1]), "f"(v[i4 + 2]), "f"(v[i4 + 3]) : "memory");
-            else
-              st4(p, make_float4(v[i4], v[i4 + 1], v[i4 + 2], v[i4 + 3]));
-          }
+  for (int nt = 0; nt < WG_NT_MAX; ++nt) {
+    if (nt < 4 * d.K) {
+      const int j = nt >> 2, ci = ci0 + (nt & 3) * 8 + 2 * tig;
+      if (ci < d.Cin) {
+        float* sbase = a.scratch + (((size_t)(ATOMIC ? 0 : sl) * d.K + j) * (size_t)(d.Cin >> 2)) * (size_t)a.coutp * 4;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int co = co0 + warp * 16 + gid + 8 * h;
+          float* p = sbase + ((size_t)(ci >> 2) * a.coutp + co) * 4 + (ci & 3);
+          const float v0 = acc[4 * nt + 2 * h], v1 = acc[4 * nt + 2 * h + 1];
+          if constexpr (ATOMIC)
+            asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(p), "f"(v0), "f"(v1) : "memory");
+          else
+            *reinterpret_cast<float2*>(p) = make_float2(v0, v1);
         }
       }
     }
   }
-  tc::tc_fence_before();
-  __syncthreads();
-  if (a.dbg && (tid == 0 || tid == WS_STAGE_THREADS)) {
-    long long* o = a.dbg + ((size_t)(blockIdx.z * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x) * 8;
-    const long long q5 = clock64();
-    if (tid == 0) { o[0] = t_begin; o[1] = q5; o[2] = c_stage; o[3] = c_free; o[5] = q4 - q3; o[6] = q5 - q4; o[7] = tile1 - tile0; }
-    else o[4] = c_issue;
+}
+
+constexpr int WG_THREADS = 256;   // 8 warps: staging, then 16 co rows of MMAs each
+
+// Stage one tile of operands with cp.async: dc as [4 atoms of 32 co][G*T rows][128 B], x with the reflect padding resolved
+// as [ntpad/32 atoms][G*(T+K-1) rows][128 B] (stride 2: even and odd padded positions in separate row blocks, so tap j
+// addresses rows (j&1)*H + t + (j>>1) -- contiguous in t).  A warp writes 4 rows x the 8 units of one 128-byte atom row
+// (four whole bank sweeps); each thread walks its rows with (g, t) kept incrementally.
+__device__ __forceinline__ void wgrad_stage(const WgTcArgs& a, uint8_t* sA, uint8_t* sX, int b0, int nsamp, int tid) {
+  const avc_wgrad_desc& d = a.d;
+  const int ci0 = blockIdx.x * WT_NT, co0 = blockIdx.y * 128;
+  const int T = d.Tout, TX = a.TX, S = d.stride, H = a.H;
+  const uint32_t atomA = (uint32_t)a.RA * 128u, atomX = (uint32_t)a.RX * 128u;
+  {
+    const int q = ((tid >> 5) & 3) * 8 + (tid & 7), r_lo = ((tid >> 7) << 2) + ((tid >> 3) & 3);
+    const int co = co0 + 4 * q;
+    const bool cv = co < d.Cout;
+    const float* colsrc = d.dc + (size_t)((cv ? co : 0) >> 2) * T * 4;
+    int g = r_lo / T, t = r_lo - g * T;
+    for (int r = r_lo; r < nsamp * T; r += 8) {
+      cp_async16(sA + mn_unit_off(q, r, atomA), colsrc + (size_t)(b0 + g) * d.dc_bstride + (size_t)t * 4, cv);
+      t += 8;
+      while (t >= T) { t -= T; ++g; }
+    }
   }
-  if (warp == 8) tc::tmem_dealloc(tbase, (uint32_t)a.ncols_tmem);
+  {
+    const int nq_x = a.ntpad >> 2;
+    const int natom = nq_x >> 3, wpa = 8 / natom;             // warps per atom
+    const int w = tid >> 5, atom = w % natom, rg = w / natom;  // row group of this warp
+    const int q = atom * 8 + (tid & 7), r_lo = (rg << 2) + ((tid >> 3) & 3), rstep = wpa << 2;
+    const int ci = ci0 + 4 * q;
+    const bool civ = ci < d.Cin;
+    const float* colsrc = d.x + (size_t)((civ ? ci : 0) >> 2) * d.Tin * 4;
+    int g = r_lo / TX, u = r_lo - g * TX;
+    for (int r0 = r_lo; r0 < nsamp * TX; r0 += rstep) {
+      const int r = S == 1 ? r0 : g * 2 * H + (u & 1) * H + (u >> 1);
+      const int p = src_pos(u - d.pad_left, d.Tin, AVC_PAD_REFLECT, 1);
+      const bool v = civ && p >= 0;
+      cp_async16(sX + mn_unit_off(q, r, atomX), colsrc + (size_t)(b0 + g) * d.x_bstride + (size_t)(p >= 0 ? p : 0) * 4, v);
+      u += rstep;
+      while (u >= TX) { u -= TX; ++g; }
+    }
+  }
+  asm volatile("cp.async.commit_group;" ::: "memory");
+}
+
+// Weight gradient, one tile at a time: stage (all warps), then MMAs (all warps).  UI is kept for the option that
+// selects it and has no effect on this architecture.
+template <bool UI, bool ATOMIC>
+__global__ void __launch_bounds__(WG_THREADS, 1) conv_wgrad_tc_kernel(const WgTcArgs a) {
+  extern __shared__ __align__(1024) uint8_t smem[];
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int tile0 = blockIdx.z * a.tiles_per_slice;
+  const int tile1 = min(cdiv(a.d.B, a.G), tile0 + a.tiles_per_slice);
+  float acc[4 * WG_NT_MAX];
+#pragma unroll
+  for (int i = 0; i < 4 * WG_NT_MAX; ++i) acc[i] = 0.f;
+  for (int tile = tile0; tile < tile1; ++tile) {
+    const int nsamp = min(a.G, a.d.B - tile * a.G);
+    wgrad_stage(a, smem, smem + a.x_off, tile * a.G, nsamp, tid);
+    asm volatile("cp.async.wait_group 0;" ::: "memory");
+    __syncthreads();
+    wgrad_mma_tile(a, smem, smem + a.x_off, nsamp, acc, warp, lane);
+    __syncthreads();
+  }
+  if (tile1 > tile0) wgrad_store<ATOMIC>(a, acc, warp, lane);
+}
+
+// "wgrad_split": the copies of tile i+1 are in flight (cp.async, second buffer) while the MMAs of tile i run.
+template <bool ATOMIC>
+__global__ void __launch_bounds__(WG_THREADS, 1) conv_wgrad_split_kernel(const WgTcArgs a) {
+  extern __shared__ __align__(1024) uint8_t smem[];
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int tile0 = blockIdx.z * a.tiles_per_slice;
+  const int tile1 = min(cdiv(a.d.B, a.G), tile0 + a.tiles_per_slice);
+  float acc[4 * WG_NT_MAX];
+#pragma unroll
+  for (int i = 0; i < 4 * WG_NT_MAX; ++i) acc[i] = 0.f;
+  if (tile1 > tile0) wgrad_stage(a, smem, smem + a.x_off, tile0 * a.G, min(a.G, a.d.B - tile0 * a.G), tid);
+  for (int tile = tile0; tile < tile1; ++tile) {
+    const int it = tile - tile0;
+    uint8_t* sA = smem + (size_t)(it & 1) * a.buf_bytes;
+    if (tile + 1 < tile1) {
+      uint8_t* sN = smem + (size_t)((it + 1) & 1) * a.buf_bytes;
+      wgrad_stage(a, sN, sN + a.x_off, (tile + 1) * a.G, min(a.G, a.d.B - (tile + 1) * a.G), tid);
+      asm volatile("cp.async.wait_group 1;" ::: "memory");
+    } else {
+      asm volatile("cp.async.wait_group 0;" ::: "memory");
+    }
+    __syncthreads();
+    wgrad_mma_tile(a, sA, sA + a.x_off, min(a.G, a.d.B - tile * a.G), acc, warp, lane);
+    __syncthreads();   // the buffer is restaged two tiles later
+  }
+  if (tile1 > tile0) wgrad_store<ATOMIC>(a, acc, warp, lane);
 }
 
 // dW[co][ci][j] += sum over slices of scratch[sl][j][ci/4][co][ci%4]
@@ -544,14 +302,11 @@ static int wgrad_tc_plan(const avc_wgrad_desc* d, WgTcArgs& a) {
   a.RX = d->stride == 1 ? (a.G * a.TX + 7) / 8 * 8 : a.G * 2 * a.H;
   a.ntpad = WT_NT;
   a.coutp = cdiv(d->Cout, 128) * 128;
-  int ncols = 32;
-  while (ncols < K * a.ntpad) ncols <<= 1;
-  a.ncols_tmem = ncols;
   a.x_off = (uint32_t)(4 * a.RA * 128 + 1023) / 1024 * 1024;
   a.buf_bytes = (a.x_off + (uint32_t)((a.ntpad / 32) * a.RX * 128) + 1023) / 1024 * 1024;
   const int ntiles = cdiv(d->B, a.G);
   const int cta_per_slice = cdiv(d->Cin, WT_NT) * cdiv(d->Cout, 128);
-  int nsl = 148 / cta_per_slice;
+  int nsl = 132 / cta_per_slice;
   if (nsl < 1) nsl = 1;
   if (nsl > ntiles) nsl = ntiles;
   a.tiles_per_slice = cdiv(ntiles, nsl);
@@ -610,12 +365,12 @@ static int wgrad_tc_launch(const avc_wgrad_desc* d, float* scratch, int* status,
       }
       attr2 = true;
     }
-    if (accumulate) AVC_LAUNCH(conv_wgrad_split_kernel<true>, grid, WS_THREADS, smem, (cudaStream_t)stream, a);
-    else AVC_LAUNCH(conv_wgrad_split_kernel<false>, grid, WS_THREADS, smem, (cudaStream_t)stream, a);
+    if (accumulate) AVC_LAUNCH(conv_wgrad_split_kernel<true>, grid, WG_THREADS, smem, (cudaStream_t)stream, a);
+    else AVC_LAUNCH(conv_wgrad_split_kernel<false>, grid, WG_THREADS, smem, (cudaStream_t)stream, a);
   } else {
     void (*kern)(const WgTcArgs) = opt_tc_uniform_issue() ? conv_wgrad_tc_kernel<true, false> : conv_wgrad_tc_kernel<false, false>;
     if (accumulate) kern = conv_wgrad_tc_kernel<true, true>;
-    AVC_LAUNCH(kern, grid, 128, smem, (cudaStream_t)stream, a);
+    AVC_LAUNCH(kern, grid, WG_THREADS, smem, (cudaStream_t)stream, a);
   }
   AVC_CHECK_LAUNCH(who);
   if (accumulate) return AVC_OK;

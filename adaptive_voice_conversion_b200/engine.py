@@ -1,4 +1,4 @@
-"""Host-side sequencing of the sm_100a kernels for the AdaIN-VC stacks.
+"""Host-side sequencing of the sm_90a kernels for the AdaIN-VC stacks.
 
 This is the layer between the reference-shaped Python API (model.AE, solver.Solver) and
 the C ABI (include/avc_b200.h).  It mirrors, launch by launch, what the reference's
@@ -65,11 +65,11 @@ class Engine:
         self.cfg = config
         self.dev = torch.device(device)
         if self.dev.type != "cuda":
-            raise L.AvcError("adaptive_voice_conversion_b200 runs on CUDA (sm_100a) only; there is no CPU path")
+            raise L.AvcError("adaptive_voice_conversion_b200 runs on CUDA (sm_90a) only; there is no CPU path")
         self.lib = L.load()
         self.packed: Dict[str, Dict[str, torch.Tensor]] = {}
         self.debug = None  # optional callback(name, stage, obj) for tools/diag_*.py
-        # "tf32": conv blocks / data gradients on the tcgen05 tensor cores (TF32 inputs rounded
+        # "tf32": conv blocks / data gradients on the tensor cores (TF32 inputs rounded
         # to nearest, fp32 accumulate); "fp32": the exact FFMA kernels.  AVC_PRECISION overrides.
         self.precision = os.environ.get("AVC_PRECISION", "tf32")
         if self.precision not in ("tf32", "fp32"):
@@ -129,10 +129,10 @@ class Engine:
         return torch.empty(shape, dtype=torch.float32, device=self.dev)
 
     def check_tc_status(self):
-        """Synchronises; raises if a tcgen05 pipeline barrier ever timed out."""
+        """Synchronises; raises if a tensor-core pipeline barrier ever timed out."""
         code = int(self.tc_status.item())
         if code != 0:
-            raise L.AvcError(f"tcgen05 conv pipeline barrier timed out (code {code})")
+            raise L.AvcError(f"tensor-core conv pipeline barrier timed out (code {code})")
 
     def zeros(self, *shape):
         t = self.empty(*shape)
@@ -312,12 +312,13 @@ class Engine:
             out = A4.empty(B, Cn, Tn, self.dev)
         assert (out.C, out.T) == (Cn, Tn)
         need_c = train and (norm or relu)
-        # tcgen05 path: one tile per sample up to 256 columns (fused block).  Longer samples (inference) are
-        # time-tiled by the persistent kernel: fused when the block has no whole-sample statistics, otherwise
-        # as a plain conv whose raw output avc_norm_apply_fwd finishes (shuffle / InstanceNorm / AdaIN / residual)
+        # tensor-core path: one tile per sample up to 144 columns (fused block; the accumulator of a tile lives in
+        # registers).  Longer samples (inference) are time-tiled by the persistent kernel: fused when the block has
+        # no whole-sample statistics, otherwise as a plain conv whose raw output avc_norm_apply_fwd finishes
+        # (shuffle / InstanceNorm / AdaIN / residual)
         tc_ok = (self.precision == "tf32" and not self.fwd_fp32 and Cin % 16 == 0 and not (stride == 2 and shuffle)
                  and "fwd_tc" in self.packed[name])
-        use_tc = tc_ok and (Tout * stride <= 256 or (self.tc_conv_v2 and not norm and not shuffle))
+        use_tc = tc_ok and (Tout * stride <= 144 or (self.tc_conv_v2 and not norm and not shuffle))
         tc_split = tc_ok and not use_tc and self.tc_conv_v2 and norm
         fused = use_tc or (not tc_split and ((not norm) or (Tout <= 128) or (Tout <= 256 and K in (1, 5))))
         c = A4.empty(B, Cout, Tout, self.dev) if (need_c or not fused) else None
@@ -517,6 +518,11 @@ class Engine:
             # per-channel mean); autograd returns ~1e-9 rounding noise there, we leave the zeroed buffer untouched
             # (not with pixel shuffle: there two conv rows with different biases share one normalised channel)
             d.dc, d.dbias = dc.ptr, (None if (rec["norm"] and not rec["shuffle"]) else gb.data_ptr())
+            if d.dbias:
+                # per-block partial sums reduced in a fixed order: atomics would make the gradient (and every later
+                # step) vary from run to run
+                part = self.empty(B * Cout)
+                d.dbias_part = part.data_ptr()
             if self.precision == "tf32":
                 d.flags = L.F_ROUND_OUT
                 dc.tf32 = True
@@ -564,8 +570,9 @@ class Engine:
                 self._ck(self.lib.avc_conv_block_tc(C.byref(d), self.tc_status.data_ptr(), st), f"conv_dgrad_tc_s2[{name}]")
         elif (self.precision == "tf32" and stride == 1 and Cout % 16 == 0 and Lp <= 256 and "dgrad_tc" in self.packed[name]):
             d.w_tc = self.packed[name]["dgrad_tc"].data_ptr()
-            if self.fold_fused and not direct and xin.T >= 2 * rec["pl"] + 1 and xin.T >= rec["pr"] + 2:
-                # the data-gradient conv folds the reflect halo and the residual adjoint in its own epilogue
+            if self.fold_fused and not direct and Lp + K - 1 <= 256 and xin.T >= 2 * rec["pl"] + 1 and xin.T >= rec["pr"] + 2:
+                # the data-gradient conv folds the reflect halo and the residual adjoint in its own epilogue (one tile
+                # of the persistent kernel per sample: its staged rows are one tensor-map box of at most 256)
                 d.out, d.out_bstride, d.out_T = dx.ptr, dx.bstride, xin.T
                 d.flags = int(d.flags) | L.F_FOLD | (rec["pl"] << 8) | (rec["pr"] << 16)
                 if dres is not None:

@@ -1,6 +1,6 @@
 """Inferencer with the reference's surface (inference.py:24-93).
 
-The model call (``AE.inference``) is the B200 path.  The wav <-> mel DSP of the reference
+The model call (``AE.inference``) is the H100 path.  The wav <-> mel DSP of the reference
 (librosa STFT / Griffin-Lim in preprocess/tacotron/utils.py) is out of scope (SURVEY.md
 section 2 rows 8, 12) and its dependencies are not in this image: ``inference_from_path``
 uses a caller-supplied ``vocoder`` object with ``get_spectrograms(path)`` /

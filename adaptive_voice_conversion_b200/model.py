@@ -1,4 +1,4 @@
-"""Reference-shaped model API on top of the sm_100a kernels.
+"""Reference-shaped model API on top of the sm_90a kernels.
 
 Drop-in for the reference's ``model.py`` classes used by its Solver / Inferencer
 (model.py:209-395 of jjery2243542/adaptive_voice_conversion):
@@ -94,7 +94,7 @@ class Decoder(_ParamStack):
 
 def _check_input(x: torch.Tensor, what: str) -> torch.Tensor:
     if not x.is_cuda:
-        raise L.AvcError(f"{what}: tensor is on {x.device}; this implementation has no CPU path (move it to a B200)")
+        raise L.AvcError(f"{what}: tensor is on {x.device}; this implementation has no CPU path (move it to an H100)")
     if x.dtype != torch.float32 or x.dim() != 3:
         raise L.AvcError(f"{what}: expected float32 [B, C, T], got {x.dtype} {tuple(x.shape)}")
     return x.contiguous()
@@ -194,7 +194,7 @@ class _DecoderFn(_StackFn):
 
 
 class AE(nn.Module):
-    """The auto-encoder of the reference (model.py:373-395), B200-native."""
+    """The auto-encoder of the reference (model.py:373-395), H100-native."""
 
     def __init__(self, config: dict):
         super().__init__()

@@ -2,7 +2,7 @@
 ``train(n)``, ``ae_step(data, lambda_kl) -> {'loss_rec','loss_kl','grad_norm'}``,
 ``save_model`` / ``load_model`` / ``save_config`` / ``build_model`` / ``get_data_loaders``.
 
-What changed underneath: the model is the B200-native ``AE``; one optimizer step is
+What changed underneath: the model is the H100-native ``AE``; one optimizer step is
 ``FusedTrainer.step`` (hand-written forward+backward kernels, a single NCCL all-reduce of
 the flat gradient when launched with torchrun, fused clip+Adam(amsgrad)); checkpoints stay
 ``<path>.ckpt`` (model state_dict) + ``<path>.opt`` (torch.optim.Adam state_dict format),

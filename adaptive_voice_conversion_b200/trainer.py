@@ -40,9 +40,10 @@ class FusedTrainer:
         self.pg = process_group
         self.world = opt.world_size
         # one 16-byte report block so that reading a step's scalars is ONE device->host copy:
-        # [sum|dec-x|, sum KL terms, sum g^2, tcgen05 status word]
+        # [sum|dec-x|, sum KL terms, sum g^2, tensor-core pipeline status word]
         self.report = torch.zeros(4, dtype=torch.float32, device=self.dev)
         self.sums = self.report[0:2]
+        self.loss_part = torch.empty(L.VAE_PARTIALS, dtype=torch.float32, device=self.dev)   # avc_vae_loss block partials
         opt.sqnorm = self.report[2:3]
         self.eng.tc_status = self.report[3:4].view(torch.int32)
         self.n_rec = 1
@@ -101,7 +102,7 @@ class FusedTrainer:
         ddec, dmu, dls = torch.empty_like(dec), torch.empty_like(mu), torch.empty_like(ls)
         self.n_rec, self.n_lat = dec.numel(), mu.numel()
         L.check(self.lib.avc_vae_loss(dec.data_ptr(), x.data_ptr(), dec.numel(), mu.data_ptr(), ls.data_ptr(), mu.numel(),
-                                      self.opt.hp.data_ptr(), self.sums.data_ptr(), ddec.data_ptr(), dmu.data_ptr(),
+                                      self.opt.hp.data_ptr(), self.sums.data_ptr(), self.loss_part.data_ptr(), ddec.data_ptr(), dmu.data_ptr(),
                                       dls.data_ptr(), eng.stream), "vae_loss")
         ddec4 = A4.empty(dec4.B, dec4.C, dec4.T, self.dev)
         eng.pack_a4(ddec, ddec4)
@@ -230,8 +231,8 @@ class FusedTrainer:
     def _decode_report(self, r):
         import struct
         status = struct.unpack("<i", struct.pack("<f", r[3]))[0]
-        if status != 0:              # a tcgen05 pipeline barrier time-out must not go unnoticed
-            raise L.AvcError(f"tcgen05 conv pipeline barrier timed out (code {status})")
+        if status != 0:              # a tensor-core pipeline barrier time-out must not go unnoticed
+            raise L.AvcError(f"tensor-core conv pipeline barrier timed out (code {status})")
         return r[0] / self.n_rec, 0.5 * r[1] / self.n_lat, (r[2] ** 0.5) / self.world
 
     def losses(self):

@@ -1,4 +1,4 @@
-"""cc / Logger / infinite_iter of the reference's utils.py (utils.py:8-35), B200 edition.
+"""cc / Logger / infinite_iter of the reference's utils.py (utils.py:8-35), H100 edition.
 
 ``cc`` moves to the local rank's CUDA device and refuses to fall back to the CPU.  The
 tensorboardX writer is optional (it is not installed in this image): without it the
@@ -13,7 +13,7 @@ import torch
 
 def local_device() -> torch.device:
     if not torch.cuda.is_available():
-        raise RuntimeError("adaptive_voice_conversion_b200 needs a CUDA device (B200); there is no CPU fallback")
+        raise RuntimeError("adaptive_voice_conversion_b200 needs a CUDA device (H100); there is no CPU fallback")
     return torch.device("cuda", int(os.environ.get("LOCAL_RANK", "0")))
 
 

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- headline measurement of the AdaIN-VC hot path on B200.
+"""bench.py -- headline measurement of the AdaIN-VC hot path on H100.
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference] [--c-in 80] [--batch 256]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 ... bench.py --gpus N ...
@@ -55,7 +55,9 @@ def parse():
     ap.add_argument("--no-graph", action="store_true")
     ap.add_argument("--skip-cpu", action="store_true", help="skip the cpu_baseline leg")
     ap.add_argument("--skip-extras", action="store_true", help="skip the extra configurations (fp32 path, c_in=512, inference) of the N=1 line")
-    ap.add_argument("--windows", type=int, default=3, help="timed windows of --steps steps each; the median window is reported")
+    ap.add_argument("--windows", type=int, default=1, help="timed windows of --steps steps each; the median window is reported")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last timed step computed (losses, updated parameters) as DIR/<name>.npy")
     ap.add_argument("--e2e-api", choices=["ae_step", "run_steps"], default="run_steps",
                     help="public call timed by the e2e arm: Solver.run_steps (the loop body of Solver.train: pinned host batch "
                          "copied per step, losses read per step, copy/read pipelined one step deep; default), or Solver.ae_step "
@@ -216,7 +218,7 @@ def dominant_kernel_roofline(dev, batch):
     P = {"r.weight": w, "r.bias": torch.zeros(Cc, device=dev)}
     eng.conv_names = lambda: ["r"]
     eng.pack_weights(P, need_dgrad=False)
-    nbuf = 10  # 10 x 16.8 MB inputs > 126 MB L2
+    nbuf = 10  # 10 x 16.8 MB inputs > 50 MB L2
     xs = [A4.empty(batch, Cc, T, dev) for _ in range(nbuf)]
     for a in xs:
         a.t.normal_()
@@ -260,28 +262,18 @@ def dominant_kernel_roofline(dev, batch):
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    peak_tf = float(peaks.get("bf16_tflops", 1590.0))
-    peak_hbm = float(peaks.get("hbm_gbs", 6650.0))
+    peak_tf = float(peaks.get("bf16_tflops", 989.0))
+    peak_hbm = float(peaks.get("hbm_gbs", 3350.0))
     src = ("measured (MEASURED_PEAKS.json: hbm_gbs copy bandwidth; bf16_tflops burst for the tensor keys)" if peaks
-           else "fallback 6.65 TB/s / 1.59 PFLOP/s (B200_PROFILING.md)")
+           else "H100 SXM data sheet (700 W): 3.35 TB/s HBM3, 989 TFLOP/s dense BF16")
     tf = flops / (avg_ms * 1e-3) / 1e12
     gbs = alg_bytes / (avg_ms * 1e-3) / 1e9
-    traffic, traffic_src = None, None   # dram__bytes_read.sum + dram__bytes_write.sum per launch, from the committed ncu --set full capture
-    if eng.precision == "tf32":
-        for name in ("r2_ncu_full_conv_block_tc.json", "r1_ncu_full_conv_block_tc.json"):
-            try:
-                m = json.load(open(os.path.join(ROOT, "profiles", name)))
-                scale = {"byte": 1, "Kbyte": 1e3, "Mbyte": 1e6, "Gbyte": 1e9}
-                traffic = sum(float(m[k][0]) * scale[m[k][1]] for k in ("dram__bytes_read.sum", "dram__bytes_write.sum"))
-                traffic_src = "profiles/" + name
-                break
-            except Exception:
-                continue
+    traffic, traffic_src = None, None   # DRAM bytes per launch: not measured (no hardware-counter capture)
     # Governing roofline: at the TF32 tensor rate (half the bf16 rate) this block needs ~4.7 us of tensor time
     # but ~7.7 us of HBM time for its algorithmic bytes (x in once, c and y out once, weights) -> HBM-bound.
     return {"bound": "hbm", "achieved": gbs, "peak": peak_hbm, "unit": "GB/s", "frac": gbs / peak_hbm, "traffic": traffic,
             "traffic_source": traffic_src,
-            "kernel": ("conv_block_tc2_kernel (persistent tcgen05 TF32: fused reflect-pad conv k5 128->128 + InstanceNorm + ReLU, saves c)" if eng.precision == "tf32"
+            "kernel": ("conv_block_tc2_kernel (persistent wgmma TF32: fused reflect-pad conv k5 128->128 + InstanceNorm + ReLU, saves c)" if eng.precision == "tf32"
                        else "conv_block_fwd_kernel<5,1,128,128> (same block, fp32 FFMA path)"),
             "shape": f"B={batch}, 128->128, k=5, T={T}",
             "avg_launch_ms": avg_ms, "avg_launch_ms_prerounded_input": avg_ms_pre,
@@ -295,6 +287,16 @@ def dominant_kernel_roofline(dev, batch):
 
 
 # ----------------------------------------------------------------------------- main arm
+def dump_outputs(out_dir, tr):
+    """What the last timed training step hands its caller: the step's losses (L1 reconstruction, KL, gradient norm)
+    and the parameters Adam left behind, concatenated in state_dict order (float32, ~20 MB at c_in=80)."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "losses.npy"), np.asarray(tr.losses(), dtype=np.float64))
+    params = torch.cat([p.detach().reshape(-1) for p in tr.P.values()]).float().cpu().numpy()
+    np.save(os.path.join(out_dir, "params.npy"), params)
+
+
 def run_b200(args):
     import types
     from adaptive_voice_conversion_b200 import _lib as L
@@ -309,6 +311,7 @@ def run_b200(args):
     if world > 1:
         torch.distributed.init_process_group("nccl", device_id=dev)
     L.load(build_if_missing=False)
+    torch.manual_seed(0)   # weights and the reparameterisation noise: the same inputs on every run
 
     cfg = config_for(args.c_in, args.batch)
     sargs = types.SimpleNamespace(data_dir="synthetic", train_set="", train_index_file="", logdir="/tmp/avc_log", load_model=False,
@@ -365,6 +368,8 @@ def run_b200(args):
 
     with ClockSampler(local) as clk:
         win, _ = timed_windows(run_resident)
+        if args.dump_outputs and rank == 0:
+            dump_outputs(args.dump_outputs, tr)
         # ---- end-to-end arm through the public API, host batches
         if args.e2e_api == "run_steps":
             solver.run_steps(2, lambda_of=lambda it: 1.0)
@@ -383,11 +388,11 @@ def run_b200(args):
         line = {
             "metric": METRIC, "value": value, "unit": UNIT, "n_gpus": world, "steps": K, "warmup": W, "ms_per_step": ms / K,
             "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
-            # arithmetic type of the conv path: tcgen05 kind::tf32 (TF32 operands, fp32 accumulate) or exact fp32 FFMA
+            # arithmetic type of the conv path: tensor-core TF32 (TF32 operands, fp32 accumulate) or exact fp32 FFMA
             "dtype": "tf32" if precision == "tf32" else "f32",
             "data": "synthetic N(0,1) segments, random-init weights",
             "config": workload_config(args, world),   # identical on the reference arm
-            "run": {"executed_on": "B200", "cuda_graph": not args.no_graph,
+            "run": {"executed_on": torch.cuda.get_device_name(dev), "cuda_graph": not args.no_graph,
                     "streams": ("3 (speaker-encoder branch beside the content-encoder branch, forward and backward; the decoder's weight "
                                 "gradients on a third, lower-priority stream)") if os.environ.get("AVC_OVERLAP", "1") == "1" else "1"},
             "timing": {"windows": NWIN, "steps_per_window": K, "reported": "median window",

@@ -1,5 +1,5 @@
 /*
- * avc_b200.h -- C ABI of libavc_b200.so: the sm_100a kernels behind the AdaIN-VC hot path.
+ * avc_b200.h -- C ABI of libavc_b200.so: the sm_90a (H100) kernels behind the AdaIN-VC hot path.
  *
  * The reference (jjery2243542/adaptive_voice_conversion) has no FFI: its hot path is the
  * Python class surface model.AE / solver.Solver / inference.Inferencer on top of stock
@@ -103,24 +103,27 @@ typedef struct avc_conv_desc {
   float* dc;    /* dense A4 [B][Cout/4][Tout][4], grad w.r.t. the raw conv output */
   float* dcond; /* [B][2*Cn] (dbeta | dgamma) rows, dcond_bstride apart; or null */
   int64_t dcond_bstride;
-  float* dbias; /* [Cout], accumulated with atomics; or null */
+  float* dbias; /* [Cout] (+=); or null */
   /* ---- tensor-core path (avc_conv_block_tc) ---- */
   const float* w_tc; /* weights packed by avc_pack_conv_weight_tc; or null */
   int32_t flags;     /* AVC_F_* */
   int32_t out_tstride, out_toff, out_T; /* avc_conv_block_tc: out time index = t*out_tstride + out_toff inside an out
                                           tensor of out_T time steps (0, 0, 0 = dense: index t of Tn) */
+  float* dbias_part; /* avc_norm_bwd with dbias: scratch of B x Cout floats for per-block partial sums, reduced into
+                        dbias in a fixed order (the same result on every run); null = per-block atomics */
 } avc_conv_desc;
 
 /* Fused block forward.  norm=1 needs the whole Tn of a sample inside one CTA tile:
  * supported for Tout <= 256, otherwise AVC_ERR_UNSUPPORTED -- run it with norm=0, relu=0,
  * res=null, save_c=out-of-conv and follow with avc_norm_apply_fwd. */
 int avc_conv_block_fwd(const avc_conv_desc* d, void* stream);
-/* The same fused block on the tcgen05 tensor cores (TF32 inputs rounded to nearest, fp32
- * accumulation in TMEM).  Covers stride 1, in_ups 1, Cin % 16 == 0, Tout <= 256; otherwise
+/* The same fused block on the tensor cores (wgmma, TF32 inputs rounded to nearest, fp32
+ * accumulation).  Covers stride 1|2, in_ups 1, Cin % 16 == 0; whole samples up to 144 columns, folded
+ * (AVC_F_FOLD) ones up to 256 staged rows (longer ones time-tiled without InstanceNorm / fold / pixel shuffle); otherwise
  * AVC_ERR_UNSUPPORTED (use avc_conv_block_fwd).  Reads d->w_tc instead of d->w_packed.
  * status: device int, set non-zero if an internal pipeline barrier timed out. */
 int avc_conv_block_tc(const avc_conv_desc* d, int* status, void* stream);
-/* nn.Conv1d weight [Cout][Cin][K] -> tcgen05 operand blocks (TF32-rounded), AVC_PACK_FWD or
+/* nn.Conv1d weight [Cout][Cin][K] -> tensor-core operand blocks (TF32-rounded), AVC_PACK_FWD or
  * AVC_PACK_DGRAD; avc_tc_packed_floats gives the buffer size for a conv with co_total output
  * and ci_total input channels (FWD: Cout, Cin; DGRAD: Cin, Cout). */
 int avc_pack_conv_weight_tc(const float* w, float* packed, int Cout, int Cin, int K, int mode, void* stream);
@@ -130,16 +133,15 @@ int64_t avc_tc_packed_floats(int co_total, int ci_total, int K);
 void avc_tc_set_debug(void* dev_buffer);
 /* Same for the persistent kernel: 16 int64 per CTA: [0] start [1] end clock; wait / work cycle sums of the roles:
  * [2] producer wait-empty, [3] patch wait-full [4] patch work, [5] MMA wait-ready [6] wait-accumulator [7] issue,
- * [8] epilogue wait-accumulator [9] TMEM pass [10] parameters [11] c rows [13] out rows [14] end barrier, [12] tiles done. */
+ * [8] epilogue wait-accumulator [9] accumulator pass [10] parameters [11] c rows [13] out rows [14] end barrier, [12] tiles done. */
 void avc_tc2_set_debug(void* dev_buffer);
-/* Weight-gradient kernel: 8 int64 per CTA: [0] start [1] end clock, cycle sums [2] staging [3] wait for a free buffer
- * [4] MMA issue [5] wait for the last MMAs [6] epilogue, [7] tiles. */
+/* Weight-gradient kernels: kept for ABI compatibility; they record no phase counters. */
 void avc_wgrad_tc_set_debug(void* dev_buffer);
 /* Store path of the persistent kernel's second pass (default from AVC_T2_VARIANT): bit 0 = `c` rows through bulk
  * (TMA) stores, bit 1 = `out` rows written back in place and bulk-stored. */
 void avc_tc2_set_variant(int v);
 /* Runtime options (process-wide; each also has an environment default read on first use):
- *   "tc_uniform_issue"  (AVC_TC_ISSUE=uniform|legacy)   tcgen05 issue loops on the uniform datapath
+ *   "tc_uniform_issue"  (AVC_TC_ISSUE=uniform|legacy)   warp index of the round-1 conv kernel via lane-0 broadcast
  *   "wgrad_reduce_v2"   (AVC_WGRAD_REDUCE=v2|v1)        unrolled partial-sum reduction of conv_wgrad_tc
  *   "tc_conv_v2"        (AVC_TC_CONV=v2|v1)             persistent, epilogue-overlapped conv block kernel (default on)
  *   "wgrad_split"       (AVC_WGRAD_KERNEL=split|r1)     weight gradient with a dedicated MMA warp, all taps in one MMA (default on)
@@ -178,7 +180,7 @@ typedef struct avc_wgrad_desc {
   float* dw; /* [Cout][Cin][K] */
 } avc_wgrad_desc;
 int avc_conv_wgrad(const avc_wgrad_desc* d, void* stream);
-/* The same gradient on the tcgen05 tensor cores (TF32 operands rounded to nearest, fp32
+/* The same gradient on the tensor cores (mma.sync TF32, fp32
  * accumulate; deterministic two-stage reduction through `scratch`).  Supported for stride 1,
  * Tout % 8 == 0, Tout <= 128: avc_wgrad_tc_scratch_floats returns the scratch size in floats,
  * or -1 when the shape must use avc_conv_wgrad.  status as in avc_conv_block_tc. */
@@ -222,7 +224,8 @@ int avc_pack_conv_weight(const float* w, float* packed, int Cout, int Cin, int K
 int avc_pack_a4(const float* planar, float* a4, int64_t a4_bstride, int B, int C, int T, int round_tf32, void* stream);
 int avc_unpack_a4(const float* a4, int64_t a4_bstride, float* planar, int B, int C, int T, void* stream);
 
-/* sum over (b, t) of an A4 tensor -> out[C] (+=): bias gradient of a conv without epilogue. */
+/* sum over (b, t) of an A4 tensor -> out[C] (+=): bias gradient of a conv.  Fixed summation order (no atomics):
+ * the same result on every run; T <= 1024. */
 int avc_bias_grad(const float* dc, int64_t bstride, float* dbias, int B, int C, int T, void* stream);
 /* The same for a tensor whose C channels are `C / group_c` layers side by side (the conv-bank gradient): channel c adds
  * into dbias_tab_dev[c / group_c][c % group_c]; dbias_tab_dev is a DEVICE array of C / group_c pointers.  One launch
@@ -311,10 +314,12 @@ int avc_reparam_bwd(const float* dz4, const float* ls4, const float* eps, const 
                     const float* dls_ext, float* dmu4, float* dls4, int B, int C, int T, void* stream);
 
 /* Losses of Solver.ae_step (solver.py:84-88) with their gradients in one pass.
- * hp (device): [0]=lambda_rec [1]=lambda_kl.  sums (device, zeroed by the call):
- * [0]=sum|dec-x| [1]=sum(exp(ls)+mu^2-1-ls).  d* receive d(lambda_rec*L1 + lambda_kl*KL). */
+ * hp (device): [0]=lambda_rec [1]=lambda_kl.  sums (device, overwritten by the call):
+ * [0]=sum|dec-x| [1]=sum(exp(ls)+mu^2-1-ls).  d* receive d(lambda_rec*L1 + lambda_kl*KL).
+ * part (device, AVC_VAE_PARTIALS floats): per-block partial sums, added in a fixed order (the same sums on every run). */
+#define AVC_VAE_PARTIALS 2112
 int avc_vae_loss(const float* dec, const float* x, int64_t n_rec, const float* mu, const float* ls,
-                 int64_t n_lat, const float* hp, float* sums, float* ddec, float* dmu, float* dls,
+                 int64_t n_lat, const float* hp, float* sums, float* part, float* ddec, float* dmu, float* dls,
                  void* stream);
 
 /* clip_grad_norm_ + Adam(amsgrad, L2 weight decay) over flat fp32 buffers
@@ -329,23 +334,24 @@ int avc_adam_step(float* p, const float* g, float* m, float* v, float* vmax, int
 
 int avc_fill_zero(void* ptr, int64_t bytes, void* stream);
 
-/* tcgen05 self-test (one CTA): D[128][N] = sum_k A_k * B_k^T over nk K=8 tf32 steps, the
+/* wgmma self-test (one CTA): D[128][N] = sum_k A_k * B_k^T over nk K=8 tf32 steps, the
  * operands given as raw shared-memory images; strides[10] = {a_lbo, a_sbo, b_lbo, b_sbo,
- * a_kstep, b_kstep, a_off, b_off (bytes), a_layout, b_layout (UMMA swizzle code, 0 = none)}; a_mn/b_mn = 1 for MN-major operands; the nk steps
- * are issued `reps` times (accumulating) for timing.  status (device int[2]): [0] non-zero if
- * the completion barrier timed out, [1] SM cycles from first MMA issue to completion.  Used by the tests to
- * pin the UMMA descriptor conventions the conv kernels rely on. */
+ * a_kstep, b_kstep, a_off, b_off (bytes), a_layout, b_layout (must be 0: no swizzle)}; a_mn/b_mn must be 0
+ * (tf32 wgmma reads K-major operands only: AVC_ERR_UNSUPPORTED otherwise); the nk steps
+ * are issued `reps` times (accumulating) for timing.  status (device int[2]): [0] 0,
+ * [1] SM cycles from first MMA issue to completion.  Used by the tests to
+ * pin the descriptor conventions the conv kernels rely on. */
 int avc_tc_probe_gemm(const float* a_img, int a_bytes, const float* b_img, int b_bytes, const uint32_t* strides,
                       int nk, int N, int a_mn, int b_mn, int reps, float* D, int* status, void* stream);
-/* Read-back variant of the self-test: the accumulator is read with 16-column tcgen05.ld's starting at
- * column `shift` + 16 j (any shift >= 0; columns below `shift` are left untouched in D). */
+/* Read-back variant of the self-test: only columns >= `shift` are written (columns below `shift` are left
+ * untouched in D). */
 void avc_tc_probe_set_ld_shift(int shift);
 /* Store-path probe (diagnostic): `ctas` CTAs of 256 threads each write bytes_per_cta (multiple of 4096) to their own
  * region of dst; mode 0 = STG.128, 1 = 2 KB bulk (TMA) stores from shared memory, 2 = half each; cycles[cta] = span. */
 int avc_probe_store(float* dst, long long bytes_per_cta, int ctas, int mode, long long* cycles, void* stream);
 
 const char* avc_last_error(void);
-/* "sm_100a" build tag, number of kernels launched so far by this process (for bench.py's
+/* "sm_90a" build tag, number of kernels launched so far by this process (for bench.py's
  * gpu_launches claim). */
 const char* avc_build_info(void);
 int64_t avc_launch_count(void);

@@ -31,7 +31,7 @@ OPTIONS = [
 
 
 def parse_args(argv=None):
-    parser = ArgumentParser(description="AdaIN-VC training on B200")
+    parser = ArgumentParser(description="AdaIN-VC training on H100")
     for flags, default, kind in OPTIONS:
         parser.add_argument(*flags, default=default, type=kind)
     for switch in ("--load_model", "--load_opt"):

@@ -11,7 +11,7 @@ GOLDEN = os.path.join(ROOT, "tests", "golden")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on an H100 with -m gpu)")
     # the CPU oracle is the slow part of the GPU suite; oneDNN on a 128-thread host is much
     # slower oversubscribed than with a moderate thread count
     import torch

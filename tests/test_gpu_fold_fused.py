@@ -1,6 +1,6 @@
 """GPU: the data-gradient conv with the reflect-padding / residual adjoint folded into its epilogue
 (AVC_F_FOLD, csrc/conv_tc.cu) against the two-pass path (conv + avc_fold_add_fwd) and autograd.
-Default path since the round-2 B200 validation."""
+Default path."""
 import math
 import os
 

@@ -23,7 +23,7 @@ def relerr(a, b):
 def eng():
     from adaptive_voice_conversion_b200.engine import Engine
     e = Engine(orc.default_config(80), torch.device("cuda", 0))
-    e.precision = "fp32"   # this file pins the exact-fp32 FFMA kernels; tests/test_gpu_tc_conv.py covers tcgen05
+    e.precision = "fp32"   # this file pins the exact-fp32 FFMA kernels; tests/test_gpu_tc_conv.py covers the tensor-core kernels
     return e
 
 
@@ -250,7 +250,8 @@ def test_reparam_and_loss(eng):
     dg, xg, mg, lg = dec.cuda(), x.cuda(), mu.cuda(), ls.cuda()
     ddec, dmu, dls = torch.empty_like(dg), torch.empty_like(mg), torch.empty_like(lg)
     L.check(eng.lib.avc_vae_loss(dg.data_ptr(), xg.data_ptr(), dg.numel(), mg.data_ptr(), lg.data_ptr(), mg.numel(),
-                                 hp.data_ptr(), sums.data_ptr(), ddec.data_ptr(), dmu.data_ptr(), dls.data_ptr(), eng.stream), "loss")
+                                 hp.data_ptr(), sums.data_ptr(), eng.empty(L.VAE_PARTIALS).data_ptr(), ddec.data_ptr(), dmu.data_ptr(),
+                                 dls.data_ptr(), eng.stream), "loss")
     s = sums.cpu()
     assert abs(float(s[0]) / dec.numel() - float(l1)) / float(l1) < 1e-5
     assert abs(0.5 * float(s[1]) / mu.numel() - float(kl)) / float(kl) < 1e-5

@@ -1,4 +1,4 @@
-"""GPU: tcgen05 descriptor conventions (avc_tc_probe_gemm) -- the foundation of the tensor-core
+"""GPU: wgmma descriptor conventions (avc_tc_probe_gemm) -- the foundation of the tensor-core
 conv kernels.  TF32 inputs (10-bit mantissa, truncated by the tensor core), fp32 accumulate:
 tolerance 2e-3 of max."""
 import ctypes as C
@@ -29,7 +29,7 @@ def run_probe(a_img, b_img, strides, nk, N, a_mn=0, b_mn=0, reps=1, want_cycles=
     L.check(lib.avc_tc_probe_gemm(a.data_ptr(), a.numel() * 4, b.data_ptr(), b.numel() * 4, st, nk, N, a_mn, b_mn, reps,
                                   D.data_ptr(), status.data_ptr(), torch.cuda.current_stream().cuda_stream), "probe")
     torch.cuda.synchronize()
-    assert int(status[0]) == 0, "tcgen05 completion barrier timed out"
+    assert int(status[0]) == 0, "probe reported a failure"
     if want_cycles:
         return D.cpu(), int(status[1])
     return D.cpu()
@@ -60,8 +60,8 @@ def test_row_offset_is_a_tap_shift():
         assert rel(D, A @ Bfull[j:j + N].t()) < 2e-3, (j, rel(D, A @ Bfull[j:j + N].t()))
 
 
-@pytest.mark.xfail(reason="MN-major tf32 operands with the no-swizzle layout return zeros on B200 in every LBO/SBO "
-                          "variant tried (tools/diag_tc.py); the weight-gradient kernel stays on the FFMA path until resolved", strict=False)
+@pytest.mark.xfail(reason="tf32 wgmma reads K-major operands only: the probe rejects MN-major ones (the weight gradient "
+                          "kernels load their MN-major fragments with warp-level MMAs instead)", strict=False)
 def test_mn_major_gemm():
     """Both operands MN-major (the weight-gradient form: reduction over time rows):
     D[m][n] = sum_k At[k][m] * Bt[k][n] with images [m/4][k][4]."""
@@ -79,8 +79,8 @@ def test_mn_major_gemm():
 
 @pytest.mark.parametrize("shift", [1, 4, 20, 36, 132])
 def test_tmem_load_at_any_start_column(shift):
-    """tcgen05.ld 32x32b.x16 accepts a start column that is not a multiple of 16: the persistent conv kernel
-    stacks samples in TMEM at a pitch of T+K-1 columns and reads every sample from its own first column."""
+    """The probe writes the accumulator from column `shift` on (any start column, not a multiple of 16): the
+    persistent conv kernel stacks samples at a pitch of T+K-1 columns and reads every sample from its own first column."""
     from adaptive_voice_conversion_b200 import _lib as L
     N, K = 256, 16
     g = torch.Generator().manual_seed(shift)

@@ -1,4 +1,4 @@
-"""GPU: the tcgen05 (TF32) fused conv block and its data-gradient use against the CPU oracle.
+"""GPU: the tensor-core (TF32) fused conv block and its data-gradient use against the CPU oracle.
 TF32 inputs are rounded to nearest (10-bit mantissa): tolerance 3e-3 of the tensor max for a
 single block (fp32 path: 2e-4, tests/test_gpu_kernels.py)."""
 import math
@@ -37,7 +37,7 @@ CASES = [
     (2, 128, 128, 5, 37, 0, 1, 0, 1, 1),      # odd length
     (2, 128, 128, 5, 200, 0, 1, 0, 1, 1),     # N = 208 columns
     (2, 128, 128, 5, 256, 0, 1, 1, 1, 1),
-    # persistent kernel (conv_tc2.cu): more tiles than SMs (both TMEM accumulators, barrier phases wrap)
+    # persistent kernel (conv_tc2.cu): more tiles than SMs (stage barrier phases wrap)
     (301, 128, 128, 5, 128, 0, 1, 0, 1, 1),
     (601, 128, 128, 5, 64, 0, 1, 1, 1, 1),    # 2 samples per tile, odd tail
     (450, 128, 256, 5, 32, 1, 1, 1, 1, 3),    # stacked samples + pixel shuffle, two M tiles
@@ -144,7 +144,7 @@ def test_tc_dgrad_linear(eng, B, Cin, Cout, K, T):
 @pytest.mark.parametrize("B,Cin,Cout,K,T", [(5, 128, 128, 5, 128), (37, 128, 128, 5, 16), (9, 128, 256, 5, 32), (3, 80, 128, 8, 128),
                                              (3, 80, 128, 1, 128), (2, 1104, 128, 1, 128), (3, 128, 80, 1, 64), (300, 128, 128, 5, 16)])
 def test_tc_wgrad(eng, B, Cin, Cout, K, T):
-    """Weight gradient on tcgen05 (MN-major operands staged from the A4 layout) vs autograd."""
+    """Weight gradient on the tensor cores (MN-major operands staged from the A4 layout) vs autograd."""
     import ctypes as C
     from adaptive_voice_conversion_b200 import _lib as L
     x = rnd((B, Cin, T), 1)
@@ -166,7 +166,7 @@ def test_tc_wgrad(eng, B, Cin, Cout, K, T):
 @pytest.mark.parametrize("B,C_,T", [(5, 128, 128), (19, 128, 32), (3, 128, 64)])
 def test_tc_stride2_backward_linear(eng, B, C_, T):
     """Stride-2 conv (encoder second convs): data gradient as two tap-parity convs and the weight
-    gradient with parity-split staging, both on tcgen05, vs autograd of the plain conv."""
+    gradient with parity-split staging, both on the tensor cores, vs autograd of the plain conv."""
     K = 5
     x = rnd((B, C_, T), 1).requires_grad_(True)
     w = (rnd((C_, C_, K), 2) / math.sqrt(C_ * K)).requires_grad_(True)

@@ -1,6 +1,6 @@
 """GPU: conv weight gradients accumulated in place (vector atomics + one flush launch,
 csrc/wgrad_tc.cu ATOMIC / avc_wgrad_acc_flush) against the two-stage deterministic path and
-against autograd.  Default path since the round-2 B200 validation."""
+against autograd.  Default path."""
 import math
 import os
 

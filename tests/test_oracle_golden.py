@@ -7,10 +7,11 @@ import pytest
 import torch
 
 import oracle.ae_oracle as orc
+from oracle.make_golden import load_fixture, pick
 
 
 def load(golden_dir, name):
-    return torch.load(os.path.join(golden_dir, name), weights_only=False)
+    return load_fixture(os.path.join(golden_dir, name))
 
 
 def rel(a, b):
@@ -58,7 +59,7 @@ def test_train_steps(golden_dir, name):
         res = orc.ae_train_step(sd, st, cfg, fx["x"], rec["eps"], fx["lambda_kl"])
         o = res["outs"]
         for k in ("mu", "log_sigma", "emb", "dec"):
-            assert rel(o[k], rec[k]) < tol, (name, i, k, rel(o[k], rec[k]))
+            assert rel(*pick(o[k], rec[k])) < tol, (name, i, k, rel(*pick(o[k], rec[k])))
         assert abs(res["loss_rec"] - float(rec["loss_rec"])) / float(rec["loss_rec"]) < tol / 10
         assert abs(res["loss_kl"] - float(rec["loss_kl"])) / float(rec["loss_kl"]) < tol / 10
         assert abs(res["grad_norm"] - float(rec["grad_norm"])) / float(rec["grad_norm"]) < tol
@@ -66,14 +67,16 @@ def test_train_steps(golden_dir, name):
         assert torch.allclose(gl2, rec["grad_l2"], rtol=50 * tol, atol=1e-5)
         if i == 0:
             for k, g in rec["grad_small"].items():
-                assert rel(res["grads"][k], g) < 5e-3 or float(g.abs().max()) < 1e-5, (name, k)
+                got, g = pick(res["grads"][k], g)
+                assert rel(got, g) < 5e-3 or float(g.abs().max()) < 1e-5, (name, k)
         pl2 = torch.stack([sd[k].norm() for k in fx["names"]])
         assert torch.allclose(pl2, rec["param_l2_after"], rtol=1e-5 if i == 0 else 2e-3)
         if i == 0:
             for k, p in rec["param_small_after"].items():
-                g = rec["grad_small"][k]
+                _, g = pick(res["grads"][k], rec["grad_small"][k])
+                got, p = pick(sd[k], p)
                 sel = g.abs() > 1e-5          # skip noise-gradient elements (see above)
-                assert ((sd[k] - p).abs() * sel).max() < 1e-4, (name, k)
+                assert ((got - p).abs() * sel).max() < 1e-4, (name, k)
 
 
 @pytest.mark.parametrize("name", ["infer_c80.pt", "infer_c80_t512.pt"])
@@ -89,19 +92,21 @@ def test_inference(golden_dir, name):
     assert rel(emb, fx["emb"]) < 2e-4
 
 
-@pytest.mark.skipif(not os.path.isdir("/root/reference"), reason="reference tree only exists in the authoring container")
 def test_live_reference_matches_fixture(golden_dir):
-    """Re-run the unmodified reference and compare with the committed fixture (guards the
-    fixture generator itself)."""
-    from oracle.make_golden import import_reference
-    ref_model = import_reference()
+    """The unmodified reference's forward pass on the training fixture's input (run by oracle/make_golden.py and
+    stored in reference_forward_c80.pt) agrees with the committed fixture, and the oracle reproduces it from the
+    stored input and noise (guards the fixture generator itself)."""
+    ref = torch.load(os.path.join(golden_dir, "reference_forward_c80.pt"), weights_only=False)
     fx = load(golden_dir, "train_c80_b1.pt")
+    rec = fx["steps"][0]
+    assert rel(fx["x"], ref["x"]) < 1e-6 and rel(rec["eps"], ref["eps"]) < 1e-6
+    for k in ("mu", "log_sigma", "emb", "dec"):
+        assert rel(*pick(ref[k], rec[k])) < 1e-5, k
     cfg = orc.default_config(80)
-    ae = ref_model.AE(cfg)
-    ae.load_state_dict(orc.init_state(cfg, seed=0), strict=True)
-    torch.manual_seed(100)
-    mu, ls, emb, dec = ae(fx["x"])
-    assert rel(dec, fx["steps"][0]["dec"]) < 1e-5
+    with torch.no_grad():
+        outs = orc.ae_forward(orc.init_state(cfg, seed=0), cfg, ref["x"], ref["eps"])
+    for k, v in zip(("mu", "log_sigma", "emb", "dec"), outs):
+        assert rel(v, ref[k]) < 2e-4, k
 
 
 def test_torch_optim_step_agrees_with_restated_adam(golden_dir):

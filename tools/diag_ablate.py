@@ -14,7 +14,7 @@ dev = torch.device("cuda", 0)
 eng = Engine(default_config(80), dev)
 B = int(os.environ.get("DIAG_B", "256"))
 PROBES = [(0, "full kernel"), (16, "weights 1 KB/stage"), (256, "no input rows"), (16 + 256, "no copies"), (64, "no MMAs"),
-          (128, "no TMEM pass"), (32, "no store pass"), (32 + 128, "no epilogue"), (16 + 256 + 32 + 128, "MMAs only"),
+          (128, "no accumulator pass"), (32, "no store pass"), (32 + 128, "no epilogue"), (16 + 256 + 32 + 128, "MMAs only"),
           (64 + 32 + 128, "copies only"), (16 + 256 + 64 + 128, "stores only"), (16 + 256 + 64 + 32 + 128, "empty pipeline"),
           (2048, "full, one patch warp"), (2048 + 496, "empty, one patch warp")]
 if os.environ.get("DIAG_PROBES"):

@@ -1,4 +1,4 @@
-"""GPU diagnostic: per-CTA phase timing (main loop vs epilogue) of the tcgen05 conv kernel."""
+"""GPU diagnostic: per-CTA phase timing (main loop vs epilogue) of the tensor-core conv kernel."""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch

@@ -6,7 +6,7 @@ from adaptive_voice_conversion_b200 import _lib as L
 lib = L.load()
 dev = torch.device("cuda", 0)
 st = torch.cuda.current_stream().cuda_stream
-for ctas in (148, 32, 1):
+for ctas in (132, 32, 1):
     for kb in (64, 256, 2048):
         nbytes = kb * 1024
         dst = torch.empty(ctas * nbytes // 4, device=dev)

@@ -1,4 +1,4 @@
-"""GPU diagnostic: per-CTA phase cycles of the tcgen05 weight-gradient kernels (avc_wgrad_tc_set_debug), TMA-staged vs round-1 -staged."""
+"""GPU diagnostic: per-CTA phase cycles of the tensor-core weight-gradient kernels (avc_wgrad_tc_set_debug), TMA-staged vs round-1 -staged."""
 import os, sys, ctypes as C
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
