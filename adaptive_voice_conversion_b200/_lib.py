@@ -124,12 +124,7 @@ PROTOTYPES = {
     "avc_conv_block_tc": (_i, [C.POINTER(ConvDesc), _p, _p]),
     "avc_pack_conv_weight_tc": (_i, [_p, _p, _i, _i, _i, _i, _p]),
     "avc_tc_packed_floats": (_i64, [_i, _i, _i]),
-    "avc_tc_set_debug": (None, [_p]),
     "avc_tc2_set_debug": (None, [_p]),
-    "avc_tc2_set_variant": (None, [_i]),
-    "avc_wgrad_tc_set_debug": (None, [_p]),
-    "avc_set_option": (_i, [C.c_char_p, _i]),
-    "avc_get_option": (_i, [C.c_char_p]),
     "avc_pack_conv_weights_batch": (_i, [_p, _i, _i64, _p]),
     "avc_norm_apply_fwd": (_i, [C.POINTER(ConvDesc), _p]),
     "avc_norm_bwd": (_i, [C.POINTER(ConvDesc), _p]),
@@ -208,12 +203,3 @@ def check(rc: int, what: str = ""):
 
 def launch_count() -> int:
     return int(load().avc_launch_count())
-
-
-def set_option(name: str, value: bool):
-    """Process-wide runtime option of the library (include/avc_b200.h: avc_set_option)."""
-    check(load().avc_set_option(name.encode(), int(bool(value))), f"set_option[{name}]")
-
-
-def get_option(name: str) -> int:
-    return int(load().avc_get_option(name.encode()))

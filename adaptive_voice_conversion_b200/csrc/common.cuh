@@ -16,9 +16,6 @@ namespace avc {
 
 void set_error(const char* fmt, ...);
 void count_launch(int n = 1);
-int opt_tc_uniform_issue();  // runtime options, see avc_set_option
-int opt_wgrad_reduce_v2();
-int opt_wgrad_split();
 
 #define AVC_REQUIRE(cond, code, ...) \
   do {                               \

@@ -1,5 +1,5 @@
 // Fused ConvBlock on the tensor cores, persistent / warp-specialised edition (wgmma m64nNk8 tf32,
-// fp32 accumulation in registers).  Same contract as conv_tc.cu / conv_simt.cu:
+// fp32 accumulation in registers), launched by avc_conv_block_tc (conv_tc.cu).  Same contract as conv_simt.cu:
 //   reflect|zero pad -> Conv1d -> [pixel shuffle] -> [InstanceNorm] -> [AdaIN] -> [ReLU] -> [+residual] -> [*mask]
 // (model.py:21-32, 52-59, 77-83, 237-250, 309-320, 354-369) and, with the DGRAD weight pack and zero
 // padding, autograd's conv data gradient incl. the adjoint of the reflect padding / residual branch
@@ -25,17 +25,12 @@
 //   * STAGE GRANULARITY: a stage is `hs` HALF-SLABS of 8 input channels (one MMA K-step each).  Default hs = 2 (one
 //     16-channel slab of the weight pack, one contiguous bulk copy) for K >= 2 and hs = 4 for the 1x1 layers (fewer
 //     barrier round trips per tile); hs = 1 (K x 4 KB of weights per stage fetched by ONE 4-D tensor-map copy out of
-//     the [slab][tap][chunk] pack) is selectable with AVC_T2_HS=1.  AVC_T2_NSTAGE caps the pipeline depth.
-#include <stdlib.h>
-
+//     the [slab][tap][chunk] pack) when fewer than three one-slab stages fit (e.g. K = 8 on time-tiled long inputs).
 #include "common.cuh"
 #include "tc_common.cuh"
 #include "tmap.cuh"
 
 namespace avc {
-
-int validate_conv_desc(const avc_conv_desc* d, const char* who);
-int opt_tc_conv_v2();
 
 constexpr int T2_SLAB = 16;          // input channels per weight-pack slab (2 MMA K-steps)
 constexpr int T2_WTAP_BYTES = 8192;  // one tap of one slab: 4 chunks x 128 co x 16 B
@@ -65,10 +60,6 @@ struct Tc2Args {
   uint32_t stage_bytes, w_bytes, x_chunk_bytes;
   uint32_t off_tile, off_par, off_stat;  // byte offsets inside dynamic shared memory
   int patch;    // 1: the patch warps sit between the bulk copy and the MMAs (halo rows and/or TF32 rounding)
-  int variant;  // bit 0: `c` rows leave through bulk (TMA) stores; bit 1: `out` rows too (written back in place)
-                // ABLATION bits (timing probes only, results are WRONG; tools/diag_ablate.py): 16 weight copies shrunk to
-                // 1 KB, 32 no store pass, 64 no MMAs, 128 no accumulator pass, 256 no input-row copies; 2048: one patch warp
-                // owns every stage (results stay correct)
   int* status;
   long long* dbg;
 };
@@ -150,7 +141,6 @@ __device__ __forceinline__ bool t2_mainloop(const Tc2Args& a, uint32_t smem0, ui
     const int nh = min(a.hs, a.nhalf - i * a.hs);
     tc::wgmma_fence();
     for (int e = 0; e < nh; ++e) {   // half-slab e of the stage: one K-step of 8 input channels per tap
-      if (a.variant & 64) break;
       const uint32_t a_off = a.hs == 1 ? 0u : (uint32_t)(e >> 1) * slab_a + (uint32_t)(e & 1) * (T2_HALF_BYTES >> 4);
       uint64_t a_desc = tc::sdesc64(a_lo0 + a_off, d_hi);
       uint64_t b_desc = tc::sdesc64(b_lo0 + (uint32_t)e * ks_b, d_hi);
@@ -215,7 +205,7 @@ __device__ __forceinline__ bool t2_tile(const Tc2Args& a, const TileCoord& c, ui
                                      uint64_t* bar_ready, uint64_t* bar_empty, int& s, uint32_t& ph, float* stile, int wg, int wt, int col0) {
   float acc[N / 2];
   if (!t2_mainloop<N>(a, smem0, bar_full, bar_fullx, bar_ready, bar_empty, s, ph, acc, wg, wt, col0)) return false;
-  if (!(a.variant & 128)) t2_acc_to_tile<N>(a, c, acc, stile, wg, wt, col0);
+  t2_acc_to_tile<N>(a, c, acc, stile, wg, wt, col0);
   return true;
 }
 
@@ -253,16 +243,6 @@ __global__ void __launch_bounds__(384, 1) conv_block_tc2_kernel(const Tc2Args a,
       const TileCoord c = t2_decode(a, tile);
       const float* wsrc = d.w_tc + (size_t)c.mtile * a.nslab * ((size_t)K * (T2_WTAP_BYTES / 4));
       const int tstart = c.t0 * S - d.pad_left;   // first input position of the staged rows (may be negative)
-      // warm L2 with the NEXT tile's input rows (they usually come from HBM: a saved activation, or an input the L2
-      // no longer holds), so that the latency-sensitive stage copies of that tile hit L2 like the weights do
-      if (tile + (int)gridDim.x < a.ntiles && (a.variant & 8)) {   // opt-in: measured slower (the prefetches occupy the copy engine), AVC_T2_VARIANT bit 3
-        const TileCoord cn = t2_decode(a, tile + gridDim.x);
-        if (cn.b0 != c.b0 || cn.t0 != c.t0) {   // (another m-tile of the same samples reads the same rows)
-          const int tsn = cn.t0 * S - d.pad_left;
-          for (int i = lane; i < a.nst; i += 32) tc::tensor_prefetch_l2_4d(&tmx, 0, tsn, cn.b0, i * 2 * a.hs);
-        }
-      }
-      __syncwarp();
       for (int ii = 0; ii < a.nst * a.nchunk; ++ii) {   // every column chunk streams the same stages again
         const int i = ii % a.nst;
         const long long w0 = a.dbg ? clock64() : 0;
@@ -272,24 +252,14 @@ __global__ void __launch_bounds__(384, 1) conv_block_tc2_kernel(const Tc2Args a,
         uint8_t* sw = smem + (size_t)s * a.stage_bytes;
         const int h0 = i * a.hs, nh = min(a.hs, a.nhalf - h0);   // half-slabs [h0, h0 + nh) of the tile
         if (tc::elect_one()) {
-          if (a.variant & 256) tc::mbar_arrive(&bar_fullx[s]);
-          else {
-            // the box always has 2*hs chunk planes; planes past Cin/4 (short last stage) arrive as zeros and are not used
-            tc::mbar_arrive_expect_tx(&bar_fullx[s], 2u * (uint32_t)a.hs * a.x_chunk_bytes);
-            tc::tensor_g2s_4d(sw + a.w_bytes, &tmx, 0, tstart, c.b0, h0 * 2, &bar_fullx[s]);
-          }
+          // the box always has 2*hs chunk planes; planes past Cin/4 (short last stage) arrive as zeros and are not used
+          tc::mbar_arrive_expect_tx(&bar_fullx[s], 2u * (uint32_t)a.hs * a.x_chunk_bytes);
+          tc::tensor_g2s_4d(sw + a.w_bytes, &tmx, 0, tstart, c.b0, h0 * 2, &bar_fullx[s]);
           if (a.hs == 1) {
-            const uint32_t wb = (uint32_t)K * T2_HALF_BYTES;
-            if (a.variant & 16) {
-              tc::mbar_arrive_expect_tx(&bar_full[s], 1024u);
-              tc::bulk_g2s(sw, wsrc, 1024u, &bar_full[s]);
-            } else {
-              tc::mbar_arrive_expect_tx(&bar_full[s], wb);
-              tc::tensor_g2s_4d(sw, &tmw, 0, 0, (h0 & 1) * 2, (c.mtile * a.nslab + (h0 >> 1)) * K, &bar_full[s]);
-            }
+            tc::mbar_arrive_expect_tx(&bar_full[s], (uint32_t)K * T2_HALF_BYTES);
+            tc::tensor_g2s_4d(sw, &tmw, 0, 0, (h0 & 1) * 2, (c.mtile * a.nslab + (h0 >> 1)) * K, &bar_full[s]);
           } else {
-            const uint32_t wfull = (uint32_t)(nh >> 1) * (uint32_t)K * T2_WTAP_BYTES;   // whole slabs, contiguous in the pack
-            const uint32_t wb = (a.variant & 16) ? 1024u : wfull;
+            const uint32_t wb = (uint32_t)(nh >> 1) * (uint32_t)K * T2_WTAP_BYTES;   // whole slabs, contiguous in the pack
             tc::mbar_arrive_expect_tx(&bar_full[s], wb);
             tc::bulk_g2s(sw, wsrc + (size_t)(h0 >> 1) * ((size_t)K * (T2_WTAP_BYTES / 4)), wb, &bar_full[s]);
           }
@@ -318,7 +288,7 @@ __global__ void __launch_bounds__(384, 1) conv_block_tc2_kernel(const Tc2Args a,
     const int pw = warp - 1;
     const bool rnd = !(d.flags & AVC_F_IN_TF32);
     const bool refl = d.pad_mode == AVC_PAD_REFLECT;
-    const int npw = (a.variant & 2048) ? 1 : min(3, a.nstage);   // probe bit 2048: a single patch warp owns every stage (the previous structure)
+    const int npw = min(3, a.nstage);
     int s = 0;
     uint32_t ph = 0;
     bool ok = true;
@@ -480,7 +450,6 @@ __global__ void __launch_bounds__(384, 1) conv_block_tc2_kernel(const Tc2Args a,
           stat[(1 * a.G + g) * 128 + r] = make_float2(0.f, 0.f);
         }
       }
-      if (a.variant & 3) tc::fence_proxy_async_smem();   // the staged rows will be read by bulk (async-proxy) stores
       const long long e2 = a.dbg ? clock64() : 0;
       t2_bar_sync(2, 256);
       // ---------------- per (sample, channel) parameters: mean, scale = rstd*gamma, shift = beta
@@ -516,7 +485,7 @@ __global__ void __launch_bounds__(384, 1) conv_block_tc2_kernel(const Tc2Args a,
       t2_bar_sync(2, 256);
       const long long e3 = a.dbg ? clock64() : 0;
       // ---------------- pass B: staged tile -> c / out, thread = one 16-byte A4 unit, lanes along time
-      if (ok && !(a.variant & 32)) {
+      if (ok) {
         const int nq = min(32, (d.Cout - c.mtile * 128) >> 2);  // valid 4-row chunks of this tile
         const float4* st4p = reinterpret_cast<const float4*>(stile);
         const float4* par4 = reinterpret_cast<const float4*>(par);
@@ -639,7 +608,7 @@ __global__ void __launch_bounds__(384, 1) conv_block_tc2_kernel(const Tc2Args a,
               }
             }
           }
-        } else if (!shuf && !d.mask && ots == 1 && (a.variant & 3) == 0) {
+        } else if (!shuf && !d.mask && ots == 1) {
           // Common case (every block without pixel shuffle / mask): `c` and `out` in ONE sweep over the staged tile.
           // Per-sample base pointers, per-row pointer = base + row * stride, four time steps per lane in flight:
           // the per-row 64-bit address arithmetic of the generic loops below was a ~300-cycle dependent chain in
@@ -701,22 +670,12 @@ __global__ void __launch_bounds__(384, 1) conv_block_tc2_kernel(const Tc2Args a,
           }
           if (a.dbg) e3b = clock64();
         } else {
-          const bool bulk_c = (a.variant & 1) != 0;
-          const bool bulk_y = (a.variant & 2) != 0 && !shuf && ots == 1;
           if (d.save_c) {  // raw conv (+bias) rows in conv layout, kept for the backward pass
             for (RowIter ri = t2_rows(ewarp, lane, c.tw, nq); ri.row < c.nsamp * nq; t2_next(ri)) {
               const int g = ri.g, cql = ri.cql;
               const float4* sr = st4p + (size_t)cql * P + g * Ts;
               float* cb = d.save_c + (((size_t)(c.b0 + g) * (d.Cout >> 2) + (c.mtile * 32 + cql)) * d.Tout + c.t0) * 4;
-              if (bulk_c) {   // one bulk (TMA) store per row: the copy engine moves it, no LSU traffic
-                if (ri.tl0 == 0) tc::bulk_s2g(cb, sr, (uint32_t)c.tw * 16u);
-              } else {
-                for (int t = ri.tl0; t < c.tw; t += ri.tstep) st4(cb + (size_t)t * 4, sr[t]);
-              }
-            }
-            if (bulk_c) {
-              tc::bulk_commit();
-              if (bulk_y) tc::bulk_wait_read_all();   // the rows are about to be overwritten in place
+              for (int t = ri.tl0; t < c.tw; t += ri.tstep) st4(cb + (size_t)t * 4, sr[t]);
             }
             __syncwarp();
           }
@@ -781,18 +740,8 @@ __global__ void __launch_bounds__(384, 1) conv_block_tc2_kernel(const Tc2Args a,
                 o.x = m.x > 0.f ? o.x : 0.f; o.y = m.y > 0.f ? o.y : 0.f; o.z = m.z > 0.f ? o.z : 0.f; o.w = m.w > 0.f ? o.w : 0.f;
               }
               if (rnd_out) o = t2_round4(o);
-              if (bulk_y) const_cast<float4*>(srA)[tl_] = o;   // in place: this warp owns the row
-              else st4(ob + (size_t)(t * ots + oto) * 4, o);
+              st4(ob + (size_t)(t * ots + oto) * 4, o);
             }
-            if (bulk_y) {
-              tc::fence_proxy_async_smem();
-              __syncwarp();
-              if (ri.tl0 == 0) tc::bulk_s2g(ob + (size_t)(to0 + oto) * 4, srA, (uint32_t)two * 16u);
-            }
-          }
-          if (bulk_c || bulk_y) {
-            tc::bulk_commit();
-            tc::bulk_wait_read_all();   // the staged tile is rewritten by the next tile's accumulator pass
           }
         }
       }
@@ -829,7 +778,7 @@ static int t2_num_sms() {
   return n;
 }
 
-// returns AVC_OK and fills a, or AVC_ERR_UNSUPPORTED (caller falls back to the round-1 kernel / FFMA path)
+// returns AVC_OK and fills a, or AVC_ERR_UNSUPPORTED with the reason (the shape needs avc_conv_block_fwd)
 int t2_plan(const avc_conv_desc* d, Tc2Args& a) {
   const int K = d->K, S = d->stride;
   const bool fold = (d->flags & AVC_F_FOLD) != 0;
@@ -839,9 +788,12 @@ int t2_plan(const avc_conv_desc* d, Tc2Args& a) {
   a.nhalf = 2 * a.nslab;
   a.mtiles = cdiv(d->Cout, 128);
   const int ncol_full = (d->Tout - 1) * S + 1;
-  if (d->pad_mode == AVC_PAD_REFLECT && d->Tin <= d->pad_left) return AVC_ERR_UNSUPPORTED;   // no mirror row to copy
-  if ((d->flags & AVC_F_NORMBWD) && (!fold || d->Cout > 128 || !d->save_c || !d->dc || (d->norm && !d->stats))) return AVC_ERR_UNSUPPORTED;
-  if (d->in_bstride % 4 != 0 || ((uintptr_t)d->in & 15u)) return AVC_ERR_UNSUPPORTED;        // tensor-map strides are multiples of 16 bytes
+  AVC_REQUIRE(d->pad_mode != AVC_PAD_REFLECT || d->Tin > d->pad_left, AVC_ERR_UNSUPPORTED,
+              "avc_conv_block_tc: reflect padding %d needs more than %d input steps", d->pad_left, d->Tin);
+  AVC_REQUIRE(!(d->flags & AVC_F_NORMBWD) || (fold && d->Cout <= 128 && d->save_c && d->dc && (!d->norm || d->stats)), AVC_ERR_UNSUPPORTED,
+              "avc_conv_block_tc: AVC_F_NORMBWD needs AVC_F_FOLD, Cout <= 128, save_c, dc and (with norm) stats");
+  AVC_REQUIRE(d->in_bstride % 4 == 0 && ((uintptr_t)d->in & 15u) == 0, AVC_ERR_UNSUPPORTED,   // tensor-map operands
+              "avc_conv_block_tc: input address and batch stride must be multiples of 16 bytes");
   // a folded data-gradient sample of up to 256 staged rows (one tensor-map box) stays one tile: its columns are
   // accumulated in chunks of 128
   const bool chunked = ncol_full > 144 && fold && ncol_full + K - 1 <= 256;
@@ -849,7 +801,9 @@ int t2_plan(const avc_conv_desc* d, Tc2Args& a) {
     a.TT = d->Tout;
     a.ntt = 1;
   } else {
-    if (d->norm || fold || d->shuffle) return AVC_ERR_UNSUPPORTED;  // whole-sample statistics / fold need one tile per sample
+    AVC_REQUIRE(!d->norm && !fold && !d->shuffle, AVC_ERR_UNSUPPORTED,   // whole-sample statistics / fold need one tile per sample
+                "avc_conv_block_tc: %d columns per sample need time tiles, which InstanceNorm, AVC_F_FOLD and pixel shuffle do not allow",
+                ncol_full);
     a.TT = S == 2 ? 64 : 128;
     a.ntt = cdiv(d->Tout, a.TT);
   }
@@ -872,7 +826,8 @@ int t2_plan(const avc_conv_desc* d, Tc2Args& a) {
     const double cost = (double)cdiv(ntiles, sms) * (3000.0 + mma);
     if (cost <= best) { best = cost; bestG = G; }
   }
-  if (bestG == 0) return AVC_ERR_UNSUPPORTED;
+  AVC_REQUIRE(bestG > 0, AVC_ERR_UNSUPPORTED, "avc_conv_block_tc: no tile of %d columns per sample fits %d accumulator columns", ncol,
+              T2_MAX_N);
   a.G = bestG;
   a.N = ((a.G - 1) * a.R + ncol + 15) / 16 * 16;
   a.nchunk = 1;
@@ -894,13 +849,7 @@ int t2_plan(const avc_conv_desc* d, Tc2Args& a) {
   const uint32_t tail = tile_bytes + par_bytes + stat_bytes;
   // Half-slabs per stage (see the header): one slab for K >= 2; the 1x1 layers have tiny half-slabs and want fewer
   // barrier round trips (hs = 4, falling back to one slab per stage when the tile leaves no room for three such stages).
-  static int hs_env = -1;
-  if (hs_env < 0) {
-    const char* e = getenv("AVC_T2_HS");
-    hs_env = e ? atoi(e) : 0;
-  }
   int hs = K >= 2 ? 2 : 4;
-  if (hs_env > 0) hs = hs_env == 1 ? 1 : (hs_env + 1) / 2 * 2;
   if (hs > a.nhalf) hs = a.nhalf;
   int nstage = 0;
   for (;; hs = hs > 2 ? hs - 2 : 1) {
@@ -913,15 +862,7 @@ int t2_plan(const avc_conv_desc* d, Tc2Args& a) {
     if (nstage >= 3 || hs == 1) break;
   }
   if (nstage > T2_MAX_STAGES) nstage = T2_MAX_STAGES;
-  {
-    static int cap = -1;   // probe: AVC_T2_NSTAGE caps the pipeline depth (how does the main loop scale with stages in flight?)
-    if (cap < 0) {
-      const char* e = getenv("AVC_T2_NSTAGE");
-      cap = e ? atoi(e) : 0;
-    }
-    if (cap >= 2 && nstage > cap) nstage = cap;
-  }
-  if (nstage < 2) return AVC_ERR_UNSUPPORTED;
+  AVC_REQUIRE(nstage >= 2, AVC_ERR_UNSUPPORTED, "avc_conv_block_tc: two pipeline stages do not fit shared memory");
   a.nst = cdiv(a.nhalf, a.hs);
   a.nstage = nstage;
   a.off_tile = (uint32_t)nstage * a.stage_bytes;
@@ -931,14 +872,6 @@ int t2_plan(const avc_conv_desc* d, Tc2Args& a) {
 }
 
 static long long* g_tc2_dbg = nullptr;
-static int g_tc2_variant = -1;
-static int t2_variant() {
-  if (g_tc2_variant < 0) {
-    const char* e = getenv("AVC_T2_VARIANT");
-    g_tc2_variant = e ? atoi(e) : 0;
-  }
-  return g_tc2_variant;
-}
 
 int conv_block_tc2_launch(const avc_conv_desc* d, int* status, void* stream) {
   Tc2Args a;
@@ -947,7 +880,6 @@ int conv_block_tc2_launch(const avc_conv_desc* d, int* status, void* stream) {
   a.status = status;
   a.dbg = g_tc2_dbg;
   a.patch = (!(d->flags & AVC_F_IN_TF32) || (d->pad_mode == AVC_PAD_REFLECT && d->K > 1)) ? 1 : 0;
-  a.variant = t2_variant();
   CUtensorMap tmx, tmw;
   {
     PFN_tmap_encode enc = tmap_encode_fn();
@@ -968,7 +900,7 @@ int conv_block_tc2_launch(const avc_conv_desc* d, int* status, void* stream) {
     }
     tmw = tmx;   // unused unless hs == 1
     if (a.hs == 1) {
-      if ((uintptr_t)d->w_tc & 15u) return AVC_ERR_UNSUPPORTED;
+      AVC_REQUIRE(((uintptr_t)d->w_tc & 15u) == 0, AVC_ERR_UNSUPPORTED, "avc_conv_block_tc: w_tc must be 16-byte aligned");
       // the weight pack [mtile][slab][tap][chunk 4][co 128][4] as rows of 2 KB, each split into two 1 KB halves (a box
       // dimension holds at most 256 elements): (256 floats, half, chunk, slab*K + tap)
       const cuuint64_t wdim[4] = {256, 2, 4, (cuuint64_t)a.mtiles * (cuuint64_t)a.nslab * (cuuint64_t)d->K};
@@ -1001,4 +933,3 @@ int conv_block_tc2_launch(const avc_conv_desc* d, int* status, void* stream) {
 }  // namespace avc
 
 extern "C" void avc_tc2_set_debug(void* dev_buffer) { avc::g_tc2_dbg = (long long*)dev_buffer; }
-extern "C" void avc_tc2_set_variant(int v) { avc::g_tc2_variant = v; }

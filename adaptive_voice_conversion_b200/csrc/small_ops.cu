@@ -1,20 +1,9 @@
 // Layout converters, the small dense layers of the speaker encoder / AdaIN affine heads,
 // the VAE reparameterisation, the losses, and the fused clip + Adam(amsgrad) update.
 #include <stdarg.h>
-#include <stdlib.h>
-#include <string.h>
 #include <atomic>
 
 #include "common.cuh"
-
-// defaults of the runtime options (avc_set_option).  AVC_TC_ISSUE=legacy / AVC_WGRAD_REDUCE=v1 select the
-// round-1 variants.
-#ifndef AVC_DEFAULT_TC_UNIFORM_ISSUE
-#define AVC_DEFAULT_TC_UNIFORM_ISSUE 1
-#endif
-#ifndef AVC_DEFAULT_WGRAD_REDUCE_V2
-#define AVC_DEFAULT_WGRAD_REDUCE_V2 1
-#endif
 
 namespace avc {
 
@@ -373,54 +362,6 @@ static int ew_blocks(int64_t n) {
 }
 
 }  // namespace avc
-
-namespace avc {
-// ---- runtime options: -1 = not read yet (environment default on first use)
-struct Option {
-  const char* name;
-  const char* env;
-  const char* on;   // environment value that enables
-  const char* off;  // environment value that disables
-  int dflt;
-  int value;
-};
-static Option g_opts[] = {
-    {"tc_uniform_issue", "AVC_TC_ISSUE", "uniform", "legacy", AVC_DEFAULT_TC_UNIFORM_ISSUE, -1},
-    {"wgrad_reduce_v2", "AVC_WGRAD_REDUCE", "v2", "v1", AVC_DEFAULT_WGRAD_REDUCE_V2, -1},
-    {"tc_conv_v2", "AVC_TC_CONV", "v2", "v1", 1, -1},   // persistent conv block kernel (conv_tc2.cu); v1 = conv_tc.cu
-    {"wgrad_split", "AVC_WGRAD_KERNEL", "split", "r1", 1, -1},   // weight gradient with a dedicated MMA warp (conv_wgrad_split_kernel)
-};
-static int opt_value(int i) {
-  Option& o = g_opts[i];
-  if (o.value < 0) {
-    const char* e = getenv(o.env);
-    o.value = o.dflt;
-    if (e && !strcmp(e, o.on)) o.value = 1;
-    if (e && !strcmp(e, o.off)) o.value = 0;
-  }
-  return o.value;
-}
-int opt_tc_uniform_issue() { return opt_value(0); }
-int opt_wgrad_reduce_v2() { return opt_value(1); }
-int opt_tc_conv_v2() { return opt_value(2); }
-int opt_wgrad_split() { return opt_value(3); }
-}  // namespace avc
-extern "C" int avc_set_option(const char* name, int value) {
-  if (name)
-    for (auto& o : avc::g_opts)
-      if (!strcmp(o.name, name)) {
-        o.value = value ? 1 : 0;
-        return AVC_OK;
-      }
-  avc::set_error("avc_set_option: unknown option '%s'", name ? name : "(null)");
-  return AVC_ERR_INVALID;
-}
-extern "C" int avc_get_option(const char* name) {
-  if (name)
-    for (int i = 0; i < (int)(sizeof(avc::g_opts) / sizeof(avc::g_opts[0])); ++i)
-      if (!strcmp(avc::g_opts[i].name, name)) return avc::opt_value(i);
-  return -1;
-}
 
 using namespace avc;
 

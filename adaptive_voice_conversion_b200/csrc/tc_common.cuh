@@ -68,19 +68,11 @@ __device__ __forceinline__ void tensor_g2s_4d(void* smem_dst, const void* tmap, 
       "l"(reinterpret_cast<uint64_t>(tmap)), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(smem_u32(bar))
       : "memory");
 }
-// the same box fetched into L2 only (no shared-memory destination, no completion): warms the NEXT tile's rows
-__device__ __forceinline__ void tensor_prefetch_l2_4d(const void* tmap, int c0, int c1, int c2, int c3) {
-  asm volatile("cp.async.bulk.prefetch.tensor.4d.L2.global.tile [%0, {%1, %2, %3, %4}];" ::"l"(reinterpret_cast<uint64_t>(tmap)), "r"(c0),
-               "r"(c1), "r"(c2), "r"(c3)
-               : "memory");
-}
 __device__ __forceinline__ void bulk_s2g(void* gdst, const void* smem_src, uint32_t bytes) {
   asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(gdst), "r"(smem_u32(smem_src)), "r"(bytes) : "memory");
 }
 __device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 __device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
-// all bulk stores committed by this thread have finished READING their shared-memory source
-__device__ __forceinline__ void bulk_wait_read_all() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
 
 // ---- wgmma (one warpgroup = 4 consecutive warps, the first a multiple of 4)
 // No-swizzle descriptor words: the issuing warpgroup keeps (lo, hi) and advances the start address with a

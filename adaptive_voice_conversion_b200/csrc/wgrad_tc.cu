@@ -22,7 +22,6 @@ constexpr int WT_NT = 32;  // ci columns per CTA (K x 32 accumulator columns: <=
 struct WgTcArgs {
   avc_wgrad_desc d;
   float* scratch;
-  long long* dbg;   // optional per-CTA phase cycle counters (avc_wgrad_tc_set_debug)
   int nslices, tiles_per_slice, G, RA, RX, ntpad, coutp, TX, H;  // H: rows of one parity block (stride 2)
   uint32_t buf_bytes, x_off;
   int* status;
@@ -158,29 +157,8 @@ __device__ __forceinline__ void wgrad_stage(const WgTcArgs& a, uint8_t* sA, uint
   asm volatile("cp.async.commit_group;" ::: "memory");
 }
 
-// Weight gradient, one tile at a time: stage (all warps), then MMAs (all warps).  UI is kept for the option that
-// selects it and has no effect on this architecture.
-template <bool UI, bool ATOMIC>
-__global__ void __launch_bounds__(WG_THREADS, 1) conv_wgrad_tc_kernel(const WgTcArgs a) {
-  extern __shared__ __align__(1024) uint8_t smem[];
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int tile0 = blockIdx.z * a.tiles_per_slice;
-  const int tile1 = min(cdiv(a.d.B, a.G), tile0 + a.tiles_per_slice);
-  float acc[4 * WG_NT_MAX];
-#pragma unroll
-  for (int i = 0; i < 4 * WG_NT_MAX; ++i) acc[i] = 0.f;
-  for (int tile = tile0; tile < tile1; ++tile) {
-    const int nsamp = min(a.G, a.d.B - tile * a.G);
-    wgrad_stage(a, smem, smem + a.x_off, tile * a.G, nsamp, tid);
-    asm volatile("cp.async.wait_group 0;" ::: "memory");
-    __syncthreads();
-    wgrad_mma_tile(a, smem, smem + a.x_off, nsamp, acc, warp, lane);
-    __syncthreads();
-  }
-  if (tile1 > tile0) wgrad_store<ATOMIC>(a, acc, warp, lane);
-}
-
-// "wgrad_split": the copies of tile i+1 are in flight (cp.async, second buffer) while the MMAs of tile i run.
+// Weight gradient of one (ci tile, co tile, batch slice): the copies of tile i+1 are in flight (cp.async, second
+// buffer) while the MMAs of tile i run.
 template <bool ATOMIC>
 __global__ void __launch_bounds__(WG_THREADS, 1) conv_wgrad_split_kernel(const WgTcArgs a) {
   extern __shared__ __align__(1024) uint8_t smem[];
@@ -209,8 +187,8 @@ __global__ void __launch_bounds__(WG_THREADS, 1) conv_wgrad_split_kernel(const W
 }
 
 // dW[co][ci][j] += sum over slices of scratch[sl][j][ci/4][co][ci%4]
-// block (32, 8): x = output float4 (coalesced 512 B per warp), y = slice group
-template <bool V2>
+// block (32, 8): x = output float4 (coalesced 512 B per warp), y = slice group; four independent 16-byte loads in
+// flight per thread (the partials sit in L2)
 __global__ void __launch_bounds__(256) wgrad_tc_reduce_kernel(const float* __restrict__ scratch, float* __restrict__ dw, int Cout, int Cin,
                                                               int K, int coutp, int nslices) {
   __shared__ float4 part[8][32];
@@ -220,17 +198,15 @@ __global__ void __launch_bounds__(256) wgrad_tc_reduce_kernel(const float* __res
   float4 s = zero4();
   if (i < n) {
     int sl = threadIdx.y;
-    if (V2) {  // four independent 16-byte loads in flight per thread (the partials sit in L2)
-      float4 s1 = zero4();
-      const float* p = scratch + i * 4;
-      for (; sl + 24 < nslices; sl += 32) {
-        const float4 v0 = ldg4(p + (sl + 0) * slice_stride), v1 = ldg4(p + (sl + 8) * slice_stride);
-        const float4 v2 = ldg4(p + (sl + 16) * slice_stride), v3 = ldg4(p + (sl + 24) * slice_stride);
-        s.x += v0.x + v2.x; s.y += v0.y + v2.y; s.z += v0.z + v2.z; s.w += v0.w + v2.w;
-        s1.x += v1.x + v3.x; s1.y += v1.y + v3.y; s1.z += v1.z + v3.z; s1.w += v1.w + v3.w;
-      }
-      s.x += s1.x; s.y += s1.y; s.z += s1.z; s.w += s1.w;
+    float4 s1 = zero4();
+    const float* p = scratch + i * 4;
+    for (; sl + 24 < nslices; sl += 32) {
+      const float4 v0 = ldg4(p + (sl + 0) * slice_stride), v1 = ldg4(p + (sl + 8) * slice_stride);
+      const float4 v2 = ldg4(p + (sl + 16) * slice_stride), v3 = ldg4(p + (sl + 24) * slice_stride);
+      s.x += v0.x + v2.x; s.y += v0.y + v2.y; s.z += v0.z + v2.z; s.w += v0.w + v2.w;
+      s1.x += v1.x + v3.x; s1.y += v1.y + v3.y; s1.z += v1.z + v3.z; s1.w += v1.w + v3.w;
     }
+    s.x += s1.x; s.y += s1.y; s.z += s1.z; s.w += s1.w;
     for (; sl < nslices; sl += 8) {
       const float4 v = ldg4(scratch + sl * slice_stride + i * 4);
       s.x += v.x; s.y += v.y; s.z += v.z; s.w += v.w;
@@ -330,7 +306,6 @@ extern "C" int64_t avc_wgrad_tc_scratch_floats(const avc_wgrad_desc* d) {
   return (int64_t)a.nslices * d->K * d->Cin * a.coutp;
 }
 
-static long long* g_wg_dbg = nullptr;
 static int wgrad_tc_launch(const avc_wgrad_desc* d, float* scratch, int* status, void* stream, bool accumulate, const char* who) {
   AVC_REQUIRE(d && d->x && d->dc && scratch && status && (accumulate || d->dw), AVC_ERR_INVALID, "%s: null argument", who);
   AVC_REQUIRE(d->B > 0 && d->Cin > 0 && d->Cout > 0 && d->Tin > 0 && d->Tout > 0, AVC_ERR_INVALID, "%s: bad shape", who);
@@ -339,14 +314,12 @@ static int wgrad_tc_launch(const avc_wgrad_desc* d, float* scratch, int* status,
   wgrad_tc_plan(d, a);
   a.scratch = scratch;
   a.status = status;
-  a.dbg = g_wg_dbg;
   const int smem = 2 * (int)a.buf_bytes;
   AVC_REQUIRE(smem <= 224 * 1024, AVC_ERR_UNSUPPORTED, "%s: tile does not fit shared memory", who);
   static bool attr_done = false;
   if (!attr_done) {
-    cudaError_t e = cudaFuncSetAttribute(conv_wgrad_tc_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 224 * 1024);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(conv_wgrad_tc_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 224 * 1024);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(conv_wgrad_tc_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 224 * 1024);
+    cudaError_t e = cudaFuncSetAttribute(conv_wgrad_split_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 224 * 1024);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(conv_wgrad_split_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 224 * 1024);
     if (e != cudaSuccess) {
       set_error("%s: cudaFuncSetAttribute: %s", who, cudaGetErrorString(e));
       return AVC_ERR_CUDA;
@@ -354,31 +327,12 @@ static int wgrad_tc_launch(const avc_wgrad_desc* d, float* scratch, int* status,
     attr_done = true;
   }
   dim3 grid(cdiv(d->Cin, WT_NT), cdiv(d->Cout, 128), a.nslices);
-  if (opt_wgrad_split()) {   // "wgrad_split": dedicated MMA warp
-    static bool attr2 = false;
-    if (!attr2) {
-      cudaError_t e = cudaFuncSetAttribute(conv_wgrad_split_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 224 * 1024);
-      if (e == cudaSuccess) e = cudaFuncSetAttribute(conv_wgrad_split_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 224 * 1024);
-      if (e != cudaSuccess) {
-        set_error("%s: cudaFuncSetAttribute: %s", who, cudaGetErrorString(e));
-        return AVC_ERR_CUDA;
-      }
-      attr2 = true;
-    }
-    if (accumulate) AVC_LAUNCH(conv_wgrad_split_kernel<true>, grid, WG_THREADS, smem, (cudaStream_t)stream, a);
-    else AVC_LAUNCH(conv_wgrad_split_kernel<false>, grid, WG_THREADS, smem, (cudaStream_t)stream, a);
-  } else {
-    void (*kern)(const WgTcArgs) = opt_tc_uniform_issue() ? conv_wgrad_tc_kernel<true, false> : conv_wgrad_tc_kernel<false, false>;
-    if (accumulate) kern = conv_wgrad_tc_kernel<true, true>;
-    AVC_LAUNCH(kern, grid, WG_THREADS, smem, (cudaStream_t)stream, a);
-  }
+  if (accumulate) AVC_LAUNCH(conv_wgrad_split_kernel<true>, grid, WG_THREADS, smem, (cudaStream_t)stream, a);
+  else AVC_LAUNCH(conv_wgrad_split_kernel<false>, grid, WG_THREADS, smem, (cudaStream_t)stream, a);
   AVC_CHECK_LAUNCH(who);
   if (accumulate) return AVC_OK;
   const int64_t n = (int64_t)d->K * (d->Cin / 4) * a.coutp;
-  if (opt_wgrad_reduce_v2())
-    AVC_LAUNCH(wgrad_tc_reduce_kernel<true>, (int)cdiv64(n, 32), dim3(32, 8), 0, (cudaStream_t)stream, scratch, d->dw, d->Cout, d->Cin, d->K, a.coutp, a.nslices);
-  else
-    AVC_LAUNCH(wgrad_tc_reduce_kernel<false>, (int)cdiv64(n, 32), dim3(32, 8), 0, (cudaStream_t)stream, scratch, d->dw, d->Cout, d->Cin, d->K, a.coutp, a.nslices);
+  AVC_LAUNCH(wgrad_tc_reduce_kernel, (int)cdiv64(n, 32), dim3(32, 8), 0, (cudaStream_t)stream, scratch, d->dw, d->Cout, d->Cin, d->K, a.coutp, a.nslices);
   AVC_CHECK_LAUNCH("wgrad_tc_reduce");
   return AVC_OK;
 }
@@ -406,5 +360,3 @@ extern "C" int avc_wgrad_acc_flush(const avc_wgrad_acc_item* items_dev, int n_it
   AVC_CHECK_LAUNCH("wgrad_acc_flush");
   return AVC_OK;
 }
-
-extern "C" void avc_wgrad_tc_set_debug(void* dev_buffer) { g_wg_dbg = (long long*)dev_buffer; }

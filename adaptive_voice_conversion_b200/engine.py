@@ -107,7 +107,6 @@ class Engine:
         self._wg_acc = None
         self.wgrad_stream = None     # set by FusedTrainer around a step: weight gradients fork onto this stream
         self._wg_keep = []
-        self.tc_conv_v2 = bool(self.lib.avc_get_option(b"tc_conv_v2"))
         # the data-gradient conv of a block also runs the upstream block's norm backward (AVC_F_NORMBWD); off = one
         # avc_norm_bwd launch per block
         self.norm_bwd_fused = os.environ.get("AVC_NORM_BWD_FUSED", "1" if L.DEFAULT_NORM_BWD_FUSED else "0") == "1"
@@ -318,8 +317,8 @@ class Engine:
         # (shuffle / InstanceNorm / AdaIN / residual)
         tc_ok = (self.precision == "tf32" and not self.fwd_fp32 and Cin % 16 == 0 and not (stride == 2 and shuffle)
                  and "fwd_tc" in self.packed[name])
-        use_tc = tc_ok and (Tout * stride <= 144 or (self.tc_conv_v2 and not norm and not shuffle))
-        tc_split = tc_ok and not use_tc and self.tc_conv_v2 and norm
+        use_tc = tc_ok and (Tout * stride <= 144 or (not norm and not shuffle))
+        tc_split = tc_ok and not use_tc and norm
         fused = use_tc or (not tc_split and ((not norm) or (Tout <= 128) or (Tout <= 256 and K in (1, 5))))
         c = A4.empty(B, Cout, Tout, self.dev) if (need_c or not fused) else None
         stats = self.empty(B, Cn, 2) if norm else None
@@ -474,7 +473,7 @@ class Engine:
     def _can_fuse_norm_bwd(self, rec, up, Cdx) -> bool:
         """May the data-gradient conv of `rec` run the InstanceNorm/AdaIN/ReLU backward of the upstream block `up`
         in its own epilogue (AVC_F_NORMBWD)?  Needs the persistent kernel's fold path and matching shapes."""
-        if not (self.norm_bwd_fused and self.fold_fused and self.tc_conv_v2 and self.precision == "tf32") or up is None:
+        if not (self.norm_bwd_fused and self.fold_fused and self.precision == "tf32") or up is None:
             return False
         xin, K, pl, pr = rec["xin"], rec["K"], rec["pl"], rec["pr"]
         Lp = xin.T + pl + pr

@@ -128,26 +128,11 @@ int avc_conv_block_tc(const avc_conv_desc* d, int* status, void* stream);
  * and ci_total input channels (FWD: Cout, Cin; DGRAD: Cin, Cout). */
 int avc_pack_conv_weight_tc(const float* w, float* packed, int Cout, int Cin, int K, int mode, void* stream);
 int64_t avc_tc_packed_floats(int co_total, int ci_total, int K);
-/* Diagnostics: device buffer of 4 int64 per CTA receiving clock64 at kernel start / main loop
- * done / epilogue done for subsequent avc_conv_block_tc launches (null disables). */
-void avc_tc_set_debug(void* dev_buffer);
-/* Same for the persistent kernel: 16 int64 per CTA: [0] start [1] end clock; wait / work cycle sums of the roles:
+/* Diagnostics: device buffer of 16 int64 per CTA receiving phase counters of subsequent avc_conv_block_tc launches
+ * (null disables): [0] start [1] end clock; wait / work cycle sums of the roles:
  * [2] producer wait-empty, [3] patch wait-full [4] patch work, [5] MMA wait-ready [6] wait-accumulator [7] issue,
  * [8] epilogue wait-accumulator [9] accumulator pass [10] parameters [11] c rows [13] out rows [14] end barrier, [12] tiles done. */
 void avc_tc2_set_debug(void* dev_buffer);
-/* Weight-gradient kernels: kept for ABI compatibility; they record no phase counters. */
-void avc_wgrad_tc_set_debug(void* dev_buffer);
-/* Store path of the persistent kernel's second pass (default from AVC_T2_VARIANT): bit 0 = `c` rows through bulk
- * (TMA) stores, bit 1 = `out` rows written back in place and bulk-stored. */
-void avc_tc2_set_variant(int v);
-/* Runtime options (process-wide; each also has an environment default read on first use):
- *   "tc_uniform_issue"  (AVC_TC_ISSUE=uniform|legacy)   warp index of the round-1 conv kernel via lane-0 broadcast
- *   "wgrad_reduce_v2"   (AVC_WGRAD_REDUCE=v2|v1)        unrolled partial-sum reduction of conv_wgrad_tc
- *   "tc_conv_v2"        (AVC_TC_CONV=v2|v1)             persistent, epilogue-overlapped conv block kernel (default on)
- *   "wgrad_split"       (AVC_WGRAD_KERNEL=split|r1)     weight gradient with a dedicated MMA warp, all taps in one MMA (default on)
- * avc_set_option returns AVC_ERR_INVALID for an unknown name; avc_get_option returns -1. */
-int avc_set_option(const char* name, int value);
-int avc_get_option(const char* name);
 /* Every re-pack of a model in one launch: a DEVICE-resident table of items (null destinations
  * are skipped); max_elems = the largest destination element count in the table. */
 typedef struct avc_pack_item {
@@ -181,8 +166,8 @@ typedef struct avc_wgrad_desc {
 } avc_wgrad_desc;
 int avc_conv_wgrad(const avc_wgrad_desc* d, void* stream);
 /* The same gradient on the tensor cores (mma.sync TF32, fp32
- * accumulate; deterministic two-stage reduction through `scratch`).  Supported for stride 1,
- * Tout % 8 == 0, Tout <= 128: avc_wgrad_tc_scratch_floats returns the scratch size in floats,
+ * accumulate; deterministic two-stage reduction through `scratch`).  Supported for Tout % 8 == 0 with
+ * stride 1 and Tout <= 128 or stride 2 and Tout <= 64: avc_wgrad_tc_scratch_floats returns the scratch size in floats,
  * or -1 when the shape must use avc_conv_wgrad.  status as in avc_conv_block_tc. */
 int64_t avc_wgrad_tc_scratch_floats(const avc_wgrad_desc* d);
 int avc_conv_wgrad_tc(const avc_wgrad_desc* d, float* scratch, int* status, void* stream);

@@ -1,5 +1,5 @@
 """GPU: the data-gradient conv with the reflect-padding / residual adjoint folded into its epilogue
-(AVC_F_FOLD, csrc/conv_tc.cu) against the two-pass path (conv + avc_fold_add_fwd) and autograd.
+(AVC_F_FOLD, csrc/conv_tc2.cu) against the two-pass path (conv + avc_fold_add_fwd) and autograd.
 Default path."""
 import math
 import os

@@ -158,20 +158,6 @@ def test_decoder_accumulators_can_be_flushed_early(rig):
     assert seen == [(0, 58)]
 
 
-def test_runtime_options_roundtrip():
-    from adaptive_voice_conversion_b200 import _lib as L
-    for name in ("tc_uniform_issue", "wgrad_reduce_v2"):
-        v = L.get_option(name)
-        assert v in (0, 1)
-        L.set_option(name, not v)
-        assert L.get_option(name) == (0 if v else 1)
-        L.set_option(name, bool(v))
-        assert L.get_option(name) == v
-    assert L.get_option("no_such_option") == -1
-    with pytest.raises(L.AvcError):
-        L.set_option("no_such_option", True)
-
-
 def test_fused_fold_drops_the_fold_launches(rig):
     e, P, G = rig
     e.lib.calls.clear()

@@ -7,7 +7,6 @@ from adaptive_voice_conversion_b200.config import default_config
 dev = torch.device("cuda", 0)
 eng = Engine(default_config(80), dev)
 B = int(os.environ.get("DIAG_B", "256"))
-VARS0 = int(os.environ.get("DIAG_VARIANTS", "0,1,3").split(",")[0])
 for (Cin, Cout, K, T, kw, tag) in [(128, 128, 5, 128, dict(norm=True, relu=True), "conv5 T128 IN"), (128, 128, 5, 128, dict(), "conv5 T128 plain"),
                                    (1104, 128, 1, 128, dict(norm=True, relu=True), "in_conv"), (128, 128, 5, 64, dict(norm=True, relu=True), "conv5 T64"),
                                    (128, 128, 5, 16, dict(norm=True, relu=True), "conv5 T16"), (80, 128, 8, 128, dict(relu=True), "bank k8")]:
@@ -25,37 +24,17 @@ for (Cin, Cout, K, T, kw, tag) in [(128, 128, 5, 128, dict(norm=True, relu=True)
     for _ in range(10):
         eng.conv(P, "r", x, train=train, **kw)
     e1.record(); torch.cuda.synchronize()
-    from adaptive_voice_conversion_b200 import _lib as L
-    L.set_option("tc_conv_v2", False)
-    try:
-        for _ in range(3):
-            eng.conv(P, "r", x, train=train, **kw)
-        torch.cuda.synchronize()
-        f0, f1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        f0.record()
-        for _ in range(10):
-            eng.conv(P, "r", x, train=train, **kw)
-        f1.record(); torch.cuda.synchronize()
-        v1_us = f0.elapsed_time(f1) * 100
-    except Exception as e:
-        v1_us = float("nan")
-    L.set_option("tc_conv_v2", True)
-    for variant in [int(v) for v in os.environ.get("DIAG_VARIANTS", "0,1,3").split(",")]:
-        eng.lib.avc_tc2_set_variant(variant)
-        for _ in range(2):
-            eng.conv(P, "r", x, train=train, **kw)
-        dbg = torch.zeros(16 * 256, dtype=torch.int64, device=dev)
-        eng.lib.avc_tc2_set_debug(dbg.data_ptr())
-        eng.conv(P, "r", x, train=train, **kw)
-        torch.cuda.synchronize()
-        eng.lib.avc_tc2_set_debug(None)
-        t = dbg.view(-1, 16).cpu()
-        t = t[t[:, 0] != 0]
-        f = lambda i: float(t[:, i].float().mean())
-        life = (t[:, 1] - t[:, 0]).float()
-        if variant == VARS0:
-            print(f"{tag:18s} round-1 kernel {v1_us:6.1f} us/launch incl. python (hot L2)  CTAs {len(t)}  tiles/CTA {f(12):.2f}")
-        print(f"  variant {variant}: CTA life mean {life.mean():7.0f} max {life.max():7.0f} cyc = {life.max() / 1965:5.1f} us | producer wait-empty {f(2):6.0f} | patch wait-full {f(3):6.0f} work {f(4):6.0f}"
-              f" | mma wait-ready {f(5):6.0f} wait-acc {f(6):5.0f} issue {f(7):6.0f} | epi wait-acc {f(8):6.0f} tmem {f(9):5.0f} params {f(10):5.0f} c-rows {f(11):5.0f} out-rows {f(13):5.0f} end-bar {f(14):5.0f}", flush=True)
-    eng.lib.avc_tc2_set_variant(0)
+    us = e0.elapsed_time(e1) * 100
+    dbg = torch.zeros(16 * 256, dtype=torch.int64, device=dev)
+    eng.lib.avc_tc2_set_debug(dbg.data_ptr())
+    eng.conv(P, "r", x, train=train, **kw)
+    torch.cuda.synchronize()
+    eng.lib.avc_tc2_set_debug(None)
+    t = dbg.view(-1, 16).cpu()
+    t = t[t[:, 0] != 0]
+    f = lambda i: float(t[:, i].float().mean())
+    life = (t[:, 1] - t[:, 0]).float()
+    print(f"{tag:18s} {us:6.1f} us/launch incl. python (hot L2)  CTAs {len(t)}  tiles/CTA {f(12):.2f}")
+    print(f"  CTA life mean {life.mean():7.0f} max {life.max():7.0f} cyc = {life.max() / 1965:5.1f} us | producer wait-empty {f(2):6.0f} | patch wait-full {f(3):6.0f} work {f(4):6.0f}"
+          f" | mma wait-ready {f(5):6.0f} wait-acc {f(6):5.0f} issue {f(7):6.0f} | epi wait-acc {f(8):6.0f} acc-pass {f(9):5.0f} params {f(10):5.0f} c-rows {f(11):5.0f} out-rows {f(13):5.0f} end-bar {f(14):5.0f}", flush=True)
 eng.check_tc_status()

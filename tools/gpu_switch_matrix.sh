@@ -1,6 +1,5 @@
 #!/bin/bash
-# the documented runtime switches still work on the final tree: conv-level tests under the stage-granularity / pipeline
-# probes, model + DP tests under the stream switches
+# the documented runtime switches still work on the final tree: model + DP tests under the stream and fusion switches
 set -u
 O=gpurun_out; mkdir -p $O
 run() { # name, env..., -- pytest args
@@ -9,8 +8,6 @@ run() { # name, env..., -- pytest args
   while [ "$1" != "--" ]; do envs+=("$1"); shift; done; shift
   env "${envs[@]}" timeout 200 python -m pytest -q -x -m gpu -p no:cacheprovider "$@" > $O/sw_$name.out 2>&1; echo "$name rc=$? $(tail -1 $O/sw_$name.out)"
 }
-run hs1 AVC_T2_HS=1 -- tests/test_gpu_tc_conv.py tests/test_gpu_fold_fused.py tests/test_gpu_normbwd_fused.py
-run nstage2 AVC_T2_NSTAGE=2 -- tests/test_gpu_tc_conv.py
 run overlap0 AVC_OVERLAP=0 AVC_INFER_GRAPH=0 -- tests/test_gpu_model.py tests/test_gpu_dp.py
 run wgstream1 AVC_WGRAD_STREAM=1 -- tests/test_gpu_model.py tests/test_gpu_dp.py tests/test_gpu_properties.py
 run wgstream0 AVC_WGRAD_STREAM=0 -- tests/test_gpu_model.py -k "solver or graph"
