@@ -8,7 +8,8 @@
 //   * PERSISTENT CTAs (one per SM) walk a static tile list; a tile = G samples x 128 output channels.
 //   * Roles: warp 0 bulk-copy (TMA) producer, warps 1-3 halo patch / TF32 rounding of the staged input,
 //     warps 4-11 two consumer warpgroups (output rows 0-63 / 64-127) that issue the wgmma main loop into
-//     their register accumulators and then run the epilogue.  mbarrier pipelines per shared-memory stage:
+//     their register accumulators and then run the epilogue (setmaxnreg moves registers from warps 0-3 to the
+//     consumers; one kernel instance per accumulator width).  mbarrier pipelines per shared-memory stage:
 //     full (weights) / fullx (input rows) / ready (patched) / empty (read by both warpgroups' MMAs).
 //   * STACKED SAMPLES: the G samples of a tile lie one after another in the staged row space at a
 //     pitch of R = (rows one sample needs) and ONE MMA of N <= T2_MAX_N columns per (k-step, tap) covers all
@@ -118,9 +119,24 @@ __device__ __forceinline__ TileCoord t2_decode(const Tc2Args& a, int tile) {
 // rows / samples outside the tensor arrive as zeros (that IS the zero padding of the data-gradient convs).
 // tmw (hs == 1 only): the weight pack as a 4-D tensor (256 floats, 2 halves of a [co][4] row, 4 chunks, slab*K+tap): the box
 // (256, 2, 2, K) is one half-slab -- [tap][2 chunks][co][4] -- in one copy-engine instruction.
+// The KT taps of one half-slab: KT wgmma back to back behind one fence, one basic block (ptxas adds no fences of its own
+// between them).  `first` == 0 only for the first half-slab of a chunk: its first MMA overwrites the accumulator.
+template <int N, int KT>
+__device__ __forceinline__ void t2_taps(float* acc, uint64_t a_desc, uint64_t b_desc, uint32_t tap_a, uint32_t first) {
+  tc::wgmma_fence();
+#pragma unroll
+  for (int j = 0; j < KT; ++j) {
+    tc::wgmma_tf32<N>(acc, a_desc, b_desc, (first | (uint32_t)j) ? 1u : 0u);
+    a_desc += (uint64_t)tap_a;
+    b_desc += 1u;
+  }
+}
+
 // Main loop of one tile for one consumer warpgroup (rows 64 wg .. 64 wg + 63 of the 128-row m-tile): every stage is
-// K taps x (half-slabs) wgmma m64nNk8 into the register accumulator `acc`; the stage is released to the producer
-// once this warpgroup's MMAs have read it (bar_empty counts one arrival per warpgroup).
+// K taps x (half-slabs) wgmma m64nNk8 into the register accumulator `acc`, issued back to back as one commit group.
+// The MMAs of stage i are issued while those of stage i-1 may still run: wait_group 1 after the commit retires stage
+// i-1, which is then released to the producer (bar_empty counts one arrival per warpgroup); the last stage of the
+// chunk is retired and released by wait_group 0 before the accumulator is read.
 template <int N>
 __device__ __forceinline__ bool t2_mainloop(const Tc2Args& a, uint32_t smem0, uint64_t* bar_full, uint64_t* bar_fullx, uint64_t* bar_ready,
                                             uint64_t* bar_empty, int& s, uint32_t& ph, float* acc, int wg, int wt, int col0) {
@@ -129,10 +145,15 @@ __device__ __forceinline__ bool t2_mainloop(const Tc2Args& a, uint32_t smem0, ui
   const uint32_t ks_b = 2u * (a.x_chunk_bytes >> 4);                       // B operand: next half-slab = 2 chunk planes on
   const uint32_t tap_a = (a.hs == 1 ? T2_HALF_BYTES : T2_WTAP_BYTES) >> 4;   // A operand: next tap
   const uint32_t slab_a = (uint32_t)K * (T2_WTAP_BYTES >> 4);                // A operand: next slab (hs > 1)
+  int s_prev = -1;   // stage whose MMAs may still be in flight
+  tc::acc_fence(acc, N / 2);
   for (int i = 0; i < a.nst; ++i) {
     const bool ok = __all_sync(0xffffffffu, tc::mbar_wait(a.patch ? &bar_ready[s] : &bar_fullx[s], ph, a.status, 3) &&
                                                 tc::mbar_wait(&bar_full[s], ph, a.status, 3));
-    if (!ok) return false;
+    if (!ok) {
+      tc::wgmma_wait<0>();
+      return false;
+    }
     const uint32_t sw = smem0 + (uint32_t)s * a.stage_bytes;
     // rows 64 wg.. of the A operand: 64 rows x 16 B further inside every 4-channel chunk
     // B operand: the chunk's first column = staged row col0 (16 B per row)
@@ -142,29 +163,33 @@ __device__ __forceinline__ bool t2_mainloop(const Tc2Args& a, uint32_t smem0, ui
     tc::wgmma_fence();
     for (int e = 0; e < nh; ++e) {   // half-slab e of the stage: one K-step of 8 input channels per tap
       const uint32_t a_off = a.hs == 1 ? 0u : (uint32_t)(e >> 1) * slab_a + (uint32_t)(e & 1) * (T2_HALF_BYTES >> 4);
-      uint64_t a_desc = tc::sdesc64(a_lo0 + a_off, d_hi);
-      uint64_t b_desc = tc::sdesc64(b_lo0 + (uint32_t)e * ks_b, d_hi);
-      if (K == 5) {
-#pragma unroll
-        for (int j = 0; j < 5; ++j) {
-          tc::wgmma_tf32<N>(acc, a_desc, b_desc, ((uint32_t)i | (uint32_t)e | (uint32_t)j) ? 1u : 0u);
-          a_desc += (uint64_t)tap_a;
-          b_desc += 1u;
-        }
-      } else {
-        for (int j = 0; j < K; ++j) {
-          tc::wgmma_tf32<N>(acc, a_desc, b_desc, ((uint32_t)i | (uint32_t)e | (uint32_t)j) ? 1u : 0u);
-          a_desc += (uint64_t)tap_a;
-          b_desc += 1u;
-        }
+      const uint64_t a_desc = tc::sdesc64(a_lo0 + a_off, d_hi);
+      const uint64_t b_desc = tc::sdesc64(b_lo0 + (uint32_t)e * ks_b, d_hi);
+      const uint32_t first = (uint32_t)i | (uint32_t)e;
+      switch (K) {
+        case 1: t2_taps<N, 1>(acc, a_desc, b_desc, tap_a, first); break;
+        case 2: t2_taps<N, 2>(acc, a_desc, b_desc, tap_a, first); break;
+        case 3: t2_taps<N, 3>(acc, a_desc, b_desc, tap_a, first); break;
+        case 4: t2_taps<N, 4>(acc, a_desc, b_desc, tap_a, first); break;
+        case 5: t2_taps<N, 5>(acc, a_desc, b_desc, tap_a, first); break;
+        case 6: t2_taps<N, 6>(acc, a_desc, b_desc, tap_a, first); break;
+        case 7: t2_taps<N, 7>(acc, a_desc, b_desc, tap_a, first); break;
+        case 8: t2_taps<N, 8>(acc, a_desc, b_desc, tap_a, first); break;
+        default:
+          for (int j = 0; j < K; ++j) t2_taps<N, 1>(acc, a_desc + (uint64_t)j * tap_a, b_desc + (uint64_t)j, tap_a, first | (uint32_t)j);
       }
     }
+    tc::wgmma_fence();   // the commit follows a join of the tap paths: ptxas closes the group with an empty MMA
     tc::wgmma_commit();
-    tc::wgmma_wait<0>();
+    tc::wgmma_wait<1>();
     tc::acc_fence(acc, N / 2);
-    if (wt == 0) tc::mbar_arrive(&bar_empty[s]);
+    if (s_prev >= 0 && wt == 0) tc::mbar_arrive(&bar_empty[s_prev]);
+    s_prev = s;
     if (++s == a.nstage) { s = 0; ph ^= 1u; }
   }
+  tc::wgmma_wait<0>();
+  tc::acc_fence(acc, N / 2);
+  if (wt == 0) tc::mbar_arrive(&bar_empty[s_prev]);   // nst >= 1
   return true;
 }
 
@@ -199,18 +224,35 @@ __device__ __forceinline__ void t2_acc_to_tile(const Tc2Args& a, const TileCoord
   }
 }
 
-// MMAs and pass 0 of one tile, instantiated for every accumulator width N (a multiple of 16, <= T2_MAX_N)
+// MMAs and pass 0 of one column chunk of a tile, accumulator width N (a multiple of 16, <= T2_MAX_N)
 template <int N>
 __device__ __forceinline__ bool t2_tile(const Tc2Args& a, const TileCoord& c, uint32_t smem0, uint64_t* bar_full, uint64_t* bar_fullx,
                                      uint64_t* bar_ready, uint64_t* bar_empty, int& s, uint32_t& ph, float* stile, int wg, int wt, int col0) {
+  // Defined before the first MMA (which ignores it: scale-d = 0): an undefined "+f" operand would keep the registers of
+  // the previous chunk live, and with two widths in one kernel both accumulators would be.
   float acc[N / 2];
+#pragma unroll
+  for (int j = 0; j < N / 2; ++j) acc[j] = 0.f;
   if (!t2_mainloop<N>(a, smem0, bar_full, bar_fullx, bar_ready, bar_empty, s, ph, acc, wg, wt, col0)) return false;
   t2_acc_to_tile<N>(a, c, acc, stile, wg, wt, col0);
   return true;
 }
 
-__global__ void __launch_bounds__(384, 1) conv_block_tc2_kernel(const Tc2Args a, const __grid_constant__ CUtensorMap tmx,
-                                                                const __grid_constant__ CUtensorMap tmw) {
+// Register budget per thread after the role split (setmaxnreg): warpgroup 0 (bulk copy + patch warps) gives registers
+// back, the two consumer warpgroups take them.  The block is launched with the __launch_bounds__ cap of 168 per
+// thread; the split must not ask for more than that allocation.
+constexpr int T2_THREADS = 384;
+constexpr int T2_REGS_LAUNCH = 168;
+constexpr int T2_REGS_PRODUCER = 56;
+constexpr int T2_REGS_CONSUMER = 224;
+static_assert(128 * T2_REGS_PRODUCER + 256 * T2_REGS_CONSUMER <= T2_THREADS * T2_REGS_LAUNCH, "setmaxnreg budget exceeds the launch allocation");
+
+// One instance per accumulator width: N columns per MMA, NL for the last column chunk (NL == N unless a folded sample
+// is accumulated in chunks of N = 128, see t2_plan).  Instantiating the width keeps ONE accumulator array live in the
+// consumer and lets its N / 2 registers stay in place across the asynchronous MMAs.
+template <int N, int NL>
+__global__ void __launch_bounds__(T2_THREADS, 1) conv_block_tc2_kernel(const Tc2Args a, const __grid_constant__ CUtensorMap tmx,
+                                                                       const __grid_constant__ CUtensorMap tmw) {
   extern __shared__ __align__(1024) uint8_t smem[];
   // per stage: full = weights landed, fullx = input rows landed (they are small and issued first, so the patch step
   // runs while the 5x larger weight copy is still in flight), ready = patched, empty = consumed by the MMAs
@@ -229,163 +271,167 @@ __global__ void __launch_bounds__(384, 1) conv_block_tc2_kernel(const Tc2Args a,
     tc::fence_mbar_init();
   }
   __syncthreads();
-  long long tm0 = 0;
-  if (a.dbg && tid == 0) tm0 = clock64();
+  // CTA start time goes out at once: a value live across the register split would be spilled
+  if (a.dbg && tid == 0) a.dbg[(size_t)blockIdx.x * 16] = clock64();
 
-  if (warp == 0) {
-    // ================================================================ bulk-copy producer
-    int s = 0;
-    uint32_t ph = 0;
-    bool ok = true;
-    bool first_round = true;
-    long long dbg0 = 0;
-    for (int tile = blockIdx.x; tile < a.ntiles && ok; tile += gridDim.x) {
-      const TileCoord c = t2_decode(a, tile);
-      const float* wsrc = d.w_tc + (size_t)c.mtile * a.nslab * ((size_t)K * (T2_WTAP_BYTES / 4));
-      const int tstart = c.t0 * S - d.pad_left;   // first input position of the staged rows (may be negative)
-      for (int ii = 0; ii < a.nst * a.nchunk; ++ii) {   // every column chunk streams the same stages again
-        const int i = ii % a.nst;
-        const long long w0 = a.dbg ? clock64() : 0;
-        if (!first_round) ok = __all_sync(0xffffffffu, tc::mbar_wait(&bar_empty[s], ph ^ 1u, a.status, 2));
-        if (a.dbg) dbg0 += clock64() - w0;
-        if (!ok) break;
-        uint8_t* sw = smem + (size_t)s * a.stage_bytes;
-        const int h0 = i * a.hs, nh = min(a.hs, a.nhalf - h0);   // half-slabs [h0, h0 + nh) of the tile
-        if (tc::elect_one()) {
-          // the box always has 2*hs chunk planes; planes past Cin/4 (short last stage) arrive as zeros and are not used
-          tc::mbar_arrive_expect_tx(&bar_fullx[s], 2u * (uint32_t)a.hs * a.x_chunk_bytes);
-          tc::tensor_g2s_4d(sw + a.w_bytes, &tmx, 0, tstart, c.b0, h0 * 2, &bar_fullx[s]);
-          if (a.hs == 1) {
-            tc::mbar_arrive_expect_tx(&bar_full[s], (uint32_t)K * T2_HALF_BYTES);
-            tc::tensor_g2s_4d(sw, &tmw, 0, 0, (h0 & 1) * 2, (c.mtile * a.nslab + (h0 >> 1)) * K, &bar_full[s]);
-          } else {
-            const uint32_t wb = (uint32_t)(nh >> 1) * (uint32_t)K * T2_WTAP_BYTES;   // whole slabs, contiguous in the pack
-            tc::mbar_arrive_expect_tx(&bar_full[s], wb);
-            tc::bulk_g2s(sw, wsrc + (size_t)(h0 >> 1) * ((size_t)K * (T2_WTAP_BYTES / 4)), wb, &bar_full[s]);
-          }
-        }
-        __syncwarp();
-        if (++s == a.nstage) { s = 0; ph ^= 1u; first_round = false; }
-      }
-    }
-    if (a.dbg && lane == 0) a.dbg[(size_t)blockIdx.x * 16 + 2] = dbg0;
-  } else if (warp < 4) {
-    // ================================================================ patch warps (3 warps, ROUND ROBIN over the stages)
-    // (a) reflect padding: the copy engine delivered zeros for the rows outside the sample; they are overwritten
-    //     with their mirror rows, taken from the staged rows of the same sample (from global memory only when a
-    //     time-tiled sample's mirror row lies outside the tile);
-    // (b) TF32 rounding, when the producer of the input did not round it (AVC_F_IN_TF32 unset: the residual
-    //     stream stays full fp32 like the reference's activations): every row is rounded to nearest in place, so
-    //     that the tensor core's truncation is exact.
-    // a.patch == 0 (zero padding or K = 1, pre-rounded input): these warps idle, the MMAs wait on the copies directly.
-    // One patch step is a dependent chain (barrier wake-up, shared-memory load, store, proxy fence, arrive) of
-    // ~400-1000 cycles whatever the stage holds, and with ONE owner of all stages it is the serial resource of the
-    // whole pipeline.  Warp w therefore owns the shared-memory STAGES s % npw == w outright (wait, round, mirror, fence, ONE
-    // arrive): up to three patch steps are in flight and none of them synchronises with another warp.  Ownership goes
-    // by stage, not by iteration: every phase of a stage's barrier is then seen by the same warp in order (a warp
-    // that skipped a phase could run a whole ring revolution ahead, and a parity wait on a barrier that is still one
-    // phase behind returns immediately -- the false positive every mbarrier pipeline has to exclude).
-    const int pw = warp - 1;
-    const bool rnd = !(d.flags & AVC_F_IN_TF32);
-    const bool refl = d.pad_mode == AVC_PAD_REFLECT;
-    const int npw = min(3, a.nstage);
-    int s = 0;
-    uint32_t ph = 0;
-    bool ok = true;
-    long long dbg0 = 0, dbg1 = 0;
-    for (int tile = blockIdx.x; a.patch && pw < npw && tile < a.ntiles && ok; tile += gridDim.x) {
-      const TileCoord c = t2_decode(a, tile);
-      const int pbeg = c.t0 * S - d.pad_left;
-      const int nr = (c.tw - 1) * S + K;  // rows one sample needs
-      const int p_lo = max(0, pbeg), p_hi = min(d.Tin, pbeg + a.R);   // input positions present in the staged rows
-      const int ncopy = max(0, min(p_hi, pbeg + nr) - p_lo), r_lo = p_lo - pbeg;
-      const int nh = refl ? nr - ncopy : 0;
-      // The halo assignment of a lane is the same for every stage of the tile: resolve it ONCE (the index arithmetic
-      // -- runtime divisions and the mirror position -- was a ~600-cycle dependent chain in front of every stage).
-      // Entry e = lane + 32 j (j < 4) is (sample g, halo row h, plane q); more than 128 entries use the generic loop.
-      const int npl = 2 * a.hs;                  // 4-channel planes of a stage
-      const int nent = c.nsamp * nh * npl;
-      int h_dst[4], h_src[4], h_glob[4], h_q[4], h_g[4];   // float4 offsets inside the stage's x region; global source
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        const int e = lane + 32 * j;
-        h_dst[j] = h_src[j] = h_glob[j] = -1;
-        h_q[j] = h_g[j] = 0;
-        if (e < nent) {
-          const int q = e % npl, r = e / npl;
-          const int g = r / nh, h = r - g * nh;
-          const int u = h < r_lo ? h : h + ncopy;
-          const int p = src_pos(pbeg + u, d.Tin, AVC_PAD_REFLECT, 1);
-          h_dst[j] = q * a.srows + g * a.R + u;
-          h_q[j] = q;
-          h_g[j] = g;
-          if (p >= p_lo && p < p_hi) h_src[j] = q * a.srows + g * a.R + (p - pbeg);
-          else if (p >= 0) h_glob[j] = p;
-        }
-      }
-      for (int ii = 0; ii < a.nst * a.nchunk && ok; ++ii) {
-        const int i = ii % a.nst;
-        if (s % npw == pw) {
+  if (warp < 4) {
+    tc::setmaxnreg_dec<T2_REGS_PRODUCER>();   // all four warps, also patch warps that idle (a.patch == 0)
+    if (warp == 0) {
+      // ================================================================ bulk-copy producer
+      int s = 0;
+      uint32_t ph = 0;
+      bool ok = true;
+      bool first_round = true;
+      long long dbg0 = 0;
+      for (int tile = blockIdx.x; tile < a.ntiles && ok; tile += gridDim.x) {
+        const TileCoord c = t2_decode(a, tile);
+        const float* wsrc = d.w_tc + (size_t)c.mtile * a.nslab * ((size_t)K * (T2_WTAP_BYTES / 4));
+        const int tstart = c.t0 * S - d.pad_left;   // first input position of the staged rows (may be negative)
+        for (int ii = 0; ii < a.nst * a.nchunk; ++ii) {   // every column chunk streams the same stages again
+          const int i = ii % a.nst;
           const long long w0 = a.dbg ? clock64() : 0;
-          ok = tc::mbar_wait(&bar_fullx[s], ph, a.status, 4);
-          const long long w1 = a.dbg ? clock64() : 0;
-          dbg0 += w1 - w0;
+          if (!first_round) ok = __all_sync(0xffffffffu, tc::mbar_wait(&bar_empty[s], ph ^ 1u, a.status, 2));
+          if (a.dbg) dbg0 += clock64() - w0;
           if (!ok) break;
-          float4* sx = reinterpret_cast<float4*>(smem + (size_t)s * a.stage_bytes + a.w_bytes);
-          bool wrote = false;
-          if (rnd) {
-            // every row of every plane (halo / gap rows included: rounding them again is harmless): the planes are
-            // contiguous, so the sweep is a linear, conflict-free walk with no index arithmetic; 4 loads in flight
-            const int nf4 = npl * a.srows;
-            int e = lane;
-            for (; e + 96 < nf4; e += 128) {
-              const float4 v0 = sx[e], v1 = sx[e + 32], v2 = sx[e + 64], v3 = sx[e + 96];
-              sx[e] = t2_round4(v0); sx[e + 32] = t2_round4(v1); sx[e + 64] = t2_round4(v2); sx[e + 96] = t2_round4(v3);
+          uint8_t* sw = smem + (size_t)s * a.stage_bytes;
+          const int h0 = i * a.hs, nh = min(a.hs, a.nhalf - h0);   // half-slabs [h0, h0 + nh) of the tile
+          if (tc::elect_one()) {
+            // the box always has 2*hs chunk planes; planes past Cin/4 (short last stage) arrive as zeros and are not used
+            tc::mbar_arrive_expect_tx(&bar_fullx[s], 2u * (uint32_t)a.hs * a.x_chunk_bytes);
+            tc::tensor_g2s_4d(sw + a.w_bytes, &tmx, 0, tstart, c.b0, h0 * 2, &bar_fullx[s]);
+            if (a.hs == 1) {
+              tc::mbar_arrive_expect_tx(&bar_full[s], (uint32_t)K * T2_HALF_BYTES);
+              tc::tensor_g2s_4d(sw, &tmw, 0, 0, (h0 & 1) * 2, (c.mtile * a.nslab + (h0 >> 1)) * K, &bar_full[s]);
+            } else {
+              const uint32_t wb = (uint32_t)(nh >> 1) * (uint32_t)K * T2_WTAP_BYTES;   // whole slabs, contiguous in the pack
+              tc::mbar_arrive_expect_tx(&bar_full[s], wb);
+              tc::bulk_g2s(sw, wsrc + (size_t)(h0 >> 1) * ((size_t)K * (T2_WTAP_BYTES / 4)), wb, &bar_full[s]);
             }
-            for (; e < nf4; e += 32) sx[e] = t2_round4(sx[e]);
-            wrote = true;
-            if (nh > 0) __syncwarp();   // the reflect rows below copy ROUNDED rows
           }
+          __syncwarp();
+          if (++s == a.nstage) { s = 0; ph ^= 1u; first_round = false; }
+        }
+      }
+      if (a.dbg && lane == 0) a.dbg[(size_t)blockIdx.x * 16 + 2] = dbg0;
+    } else {
+      // ================================================================ patch warps (3 warps, ROUND ROBIN over the stages)
+      // (a) reflect padding: the copy engine delivered zeros for the rows outside the sample; they are overwritten
+      //     with their mirror rows, taken from the staged rows of the same sample (from global memory only when a
+      //     time-tiled sample's mirror row lies outside the tile);
+      // (b) TF32 rounding, when the producer of the input did not round it (AVC_F_IN_TF32 unset: the residual
+      //     stream stays full fp32 like the reference's activations): every row is rounded to nearest in place, so
+      //     that the tensor core's truncation is exact.
+      // a.patch == 0 (zero padding or K = 1, pre-rounded input): these warps idle, the MMAs wait on the copies directly.
+      // One patch step is a dependent chain (barrier wake-up, shared-memory load, store, proxy fence, arrive) of
+      // ~400-1000 cycles whatever the stage holds, and with ONE owner of all stages it is the serial resource of the
+      // whole pipeline.  Warp w therefore owns the shared-memory STAGES s % npw == w outright (wait, round, mirror, fence, ONE
+      // arrive): up to three patch steps are in flight and none of them synchronises with another warp.  Ownership goes
+      // by stage, not by iteration: every phase of a stage's barrier is then seen by the same warp in order (a warp
+      // that skipped a phase could run a whole ring revolution ahead, and a parity wait on a barrier that is still one
+      // phase behind returns immediately -- the false positive every mbarrier pipeline has to exclude).
+      const int pw = warp - 1;
+      const bool rnd = !(d.flags & AVC_F_IN_TF32);
+      const bool refl = d.pad_mode == AVC_PAD_REFLECT;
+      const int npw = min(3, a.nstage);
+      int s = 0;
+      uint32_t ph = 0;
+      bool ok = true;
+      long long dbg0 = 0, dbg1 = 0;
+      for (int tile = blockIdx.x; a.patch && pw < npw && tile < a.ntiles && ok; tile += gridDim.x) {
+        const TileCoord c = t2_decode(a, tile);
+        const int pbeg = c.t0 * S - d.pad_left;
+        const int nr = (c.tw - 1) * S + K;  // rows one sample needs
+        const int p_lo = max(0, pbeg), p_hi = min(d.Tin, pbeg + a.R);   // input positions present in the staged rows
+        const int ncopy = max(0, min(p_hi, pbeg + nr) - p_lo), r_lo = p_lo - pbeg;
+        const int nh = refl ? nr - ncopy : 0;
+        // The halo assignment of a lane is the same for every stage of the tile: resolve it ONCE (the index arithmetic
+        // -- runtime divisions and the mirror position -- was a ~600-cycle dependent chain in front of every stage).
+        // Entry e = lane + 32 j (j < 4) is (sample g, halo row h, plane q); more than 128 entries use the generic loop.
+        const int npl = 2 * a.hs;                  // 4-channel planes of a stage
+        const int nent = c.nsamp * nh * npl;
+        int h_dst[4], h_src[4], h_glob[4], h_q[4], h_g[4];   // float4 offsets inside the stage's x region; global source
 #pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            if (h_dst[j] >= 0) {
-              float4 v = zero4();
-              if (h_src[j] >= 0) v = sx[h_src[j]];
-              else if (h_glob[j] >= 0 && (i * npl + h_q[j]) * 4 < d.Cin) {
-                v = ldg4(d.in + (size_t)(c.b0 + h_g[j]) * d.in_bstride + ((size_t)(i * npl + h_q[j]) * d.Tin + h_glob[j]) * 4);
-                if (rnd) v = t2_round4(v);
-              }
-              sx[h_dst[j]] = v;
-              wrote = true;
-            }
-          }
-          for (int e = lane + 128; e < nent; e += 32) {   // more than 128 halo entries (large K x G): generic path
+        for (int j = 0; j < 4; ++j) {
+          const int e = lane + 32 * j;
+          h_dst[j] = h_src[j] = h_glob[j] = -1;
+          h_q[j] = h_g[j] = 0;
+          if (e < nent) {
             const int q = e % npl, r = e / npl;
             const int g = r / nh, h = r - g * nh;
             const int u = h < r_lo ? h : h + ncopy;
             const int p = src_pos(pbeg + u, d.Tin, AVC_PAD_REFLECT, 1);
-            float4 v = zero4();
-            if (p >= p_lo && p < p_hi) v = sx[(size_t)q * a.srows + g * a.R + (p - pbeg)];
-            else if (p >= 0 && (i * npl + q) * 4 < d.Cin) {
-              v = ldg4(d.in + (size_t)(c.b0 + g) * d.in_bstride + ((size_t)(i * npl + q) * d.Tin + p) * 4);
-              if (rnd) v = t2_round4(v);
-            }
-            sx[(size_t)q * a.srows + g * a.R + u] = v;
-            wrote = true;
+            h_dst[j] = q * a.srows + g * a.R + u;
+            h_q[j] = q;
+            h_g[j] = g;
+            if (p >= p_lo && p < p_hi) h_src[j] = q * a.srows + g * a.R + (p - pbeg);
+            else if (p >= 0) h_glob[j] = p;
           }
-          if (wrote) tc::fence_proxy_async_smem();   // only writers pay for the proxy fence
-          __syncwarp();
-          if (lane == 0) tc::mbar_arrive(&bar_ready[s]);
-          if (a.dbg) dbg1 += clock64() - w1;
         }
-        if (++s == a.nstage) { s = 0; ph ^= 1u; }
+        for (int ii = 0; ii < a.nst * a.nchunk && ok; ++ii) {
+          const int i = ii % a.nst;
+          if (s % npw == pw) {
+            const long long w0 = a.dbg ? clock64() : 0;
+            ok = tc::mbar_wait(&bar_fullx[s], ph, a.status, 4);
+            const long long w1 = a.dbg ? clock64() : 0;
+            dbg0 += w1 - w0;
+            if (!ok) break;
+            float4* sx = reinterpret_cast<float4*>(smem + (size_t)s * a.stage_bytes + a.w_bytes);
+            bool wrote = false;
+            if (rnd) {
+              // every row of every plane (halo / gap rows included: rounding them again is harmless): the planes are
+              // contiguous, so the sweep is a linear, conflict-free walk with no index arithmetic; 4 loads in flight
+              const int nf4 = npl * a.srows;
+              int e = lane;
+              for (; e + 96 < nf4; e += 128) {
+                const float4 v0 = sx[e], v1 = sx[e + 32], v2 = sx[e + 64], v3 = sx[e + 96];
+                sx[e] = t2_round4(v0); sx[e + 32] = t2_round4(v1); sx[e + 64] = t2_round4(v2); sx[e + 96] = t2_round4(v3);
+              }
+              for (; e < nf4; e += 32) sx[e] = t2_round4(sx[e]);
+              wrote = true;
+              if (nh > 0) __syncwarp();   // the reflect rows below copy ROUNDED rows
+            }
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+              if (h_dst[j] >= 0) {
+                float4 v = zero4();
+                if (h_src[j] >= 0) v = sx[h_src[j]];
+                else if (h_glob[j] >= 0 && (i * npl + h_q[j]) * 4 < d.Cin) {
+                  v = ldg4(d.in + (size_t)(c.b0 + h_g[j]) * d.in_bstride + ((size_t)(i * npl + h_q[j]) * d.Tin + h_glob[j]) * 4);
+                  if (rnd) v = t2_round4(v);
+                }
+                sx[h_dst[j]] = v;
+                wrote = true;
+              }
+            }
+            for (int e = lane + 128; e < nent; e += 32) {   // more than 128 halo entries (large K x G): generic path
+              const int q = e % npl, r = e / npl;
+              const int g = r / nh, h = r - g * nh;
+              const int u = h < r_lo ? h : h + ncopy;
+              const int p = src_pos(pbeg + u, d.Tin, AVC_PAD_REFLECT, 1);
+              float4 v = zero4();
+              if (p >= p_lo && p < p_hi) v = sx[(size_t)q * a.srows + g * a.R + (p - pbeg)];
+              else if (p >= 0 && (i * npl + q) * 4 < d.Cin) {
+                v = ldg4(d.in + (size_t)(c.b0 + g) * d.in_bstride + ((size_t)(i * npl + q) * d.Tin + p) * 4);
+                if (rnd) v = t2_round4(v);
+              }
+              sx[(size_t)q * a.srows + g * a.R + u] = v;
+              wrote = true;
+            }
+            if (wrote) tc::fence_proxy_async_smem();   // only writers pay for the proxy fence
+            __syncwarp();
+            if (lane == 0) tc::mbar_arrive(&bar_ready[s]);
+            if (a.dbg) dbg1 += clock64() - w1;
+          }
+          if (++s == a.nstage) { s = 0; ph ^= 1u; }
+        }
+      }
+      if (a.dbg && tid == 32) {
+        long long* o = a.dbg + (size_t)blockIdx.x * 16;
+        o[3] = dbg0; o[4] = dbg1;
       }
     }
-    if (a.dbg && tid == 32) {
-      long long* o = a.dbg + (size_t)blockIdx.x * 16;
-      o[3] = dbg0; o[4] = dbg1;
-    }
   } else {
+    tc::setmaxnreg_inc<T2_REGS_CONSUMER>();
     // ================================================================ MMA + epilogue (two warpgroups, 256 threads)
     const int etid = tid - 128, ewarp = warp - 4;
     const int wg = ewarp >> 2, wt = etid & 127;      // warpgroup: accumulator rows 64 wg .. 64 wg + 63
@@ -421,14 +467,10 @@ __global__ void __launch_bounds__(384, 1) conv_block_tc2_kernel(const Tc2Args a,
       const long long e0 = a.dbg ? clock64() : 0;
       // ---------------- main loop, then pass 0: accumulators (+bias) -> staged A4 tile
       for (int ch = 0; ch < a.nchunk; ++ch) {
-        bool mok = false;
-        const int col0 = ch * a.N;
-        switch (ch + 1 == a.nchunk ? a.N_last : a.N) {
-#define T2_CASE(n) \
-  case n: mok = t2_tile<n>(a, c, smem0, bar_full, bar_fullx, bar_ready, bar_empty, s, ph, stile, wg, wt, col0); break;
-          T2_CASE(16) T2_CASE(32) T2_CASE(48) T2_CASE(64) T2_CASE(80) T2_CASE(96) T2_CASE(112) T2_CASE(128) T2_CASE(144) T2_CASE(160)
-#undef T2_CASE
-        }
+        const int col0 = ch * N;
+        const bool mok = (NL != N && ch + 1 == a.nchunk)
+                             ? t2_tile<NL>(a, c, smem0, bar_full, bar_fullx, bar_ready, bar_empty, s, ph, stile, wg, wt, col0)
+                             : t2_tile<N>(a, c, smem0, bar_full, bar_fullx, bar_ready, bar_empty, s, ph, stile, wg, wt, col0);
         ok = ok && mok;
       }
       const long long e1 = a.dbg ? clock64() : 0;
@@ -760,10 +802,7 @@ __global__ void __launch_bounds__(384, 1) conv_block_tc2_kernel(const Tc2Args a,
     }
   }
   __syncthreads();
-  if (a.dbg && tid == 0) {
-    long long* o = a.dbg + (size_t)blockIdx.x * 16;
-    o[0] = tm0; o[1] = clock64();
-  }
+  if (a.dbg && tid == 0) a.dbg[(size_t)blockIdx.x * 16 + 1] = clock64();
 }
 
 // ------------------------------------------------------------------ host side: tile plan
@@ -833,6 +872,8 @@ int t2_plan(const avc_conv_desc* d, Tc2Args& a) {
   a.nchunk = 1;
   a.N_last = a.N;
   if (chunked) {
+    // the last chunk keeps its own width (a kernel instance with both widths): at the full 128 columns its MMAs would
+    // read up to 111 rows past the staged sample, beyond the 32-row slack of the stage
     a.N = 128;
     a.nchunk = cdiv(ncol, 128);
     a.N_last = (ncol - (a.nchunk - 1) * 128 + 15) / 16 * 16;
@@ -872,6 +913,42 @@ int t2_plan(const avc_conv_desc* d, Tc2Args& a) {
 }
 
 static long long* g_tc2_dbg = nullptr;
+
+template <int N, int NL>
+static int t2_launch(const Tc2Args& a, const CUtensorMap& tmx, const CUtensorMap& tmw, int grid, int smem, cudaStream_t stream) {
+  auto kern = conv_block_tc2_kernel<N, NL>;
+  static bool attr_done = false;
+  if (!attr_done) {
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, T2_SMEM_MAX);
+    if (e != cudaSuccess) {
+      set_error("avc_conv_block_tc: cudaFuncSetAttribute: %s", cudaGetErrorString(e));
+      return AVC_ERR_CUDA;
+    }
+    attr_done = true;
+  }
+  AVC_LAUNCH(kern, grid, T2_THREADS, smem, stream, a, tmx, tmw);
+  AVC_CHECK_LAUNCH("conv_block_tc2");
+  return AVC_OK;
+}
+
+// the instance for the plan's accumulator widths: N in 16..T2_MAX_N, or N = 128 with a last chunk of 32..128 columns
+static int t2_dispatch(const Tc2Args& a, const CUtensorMap& tmx, const CUtensorMap& tmw, int grid, int smem, cudaStream_t stream) {
+#define T2_CASE(n, nl) \
+  case nl: return t2_launch<n, nl>(a, tmx, tmw, grid, smem, stream);
+  if (a.nchunk == 1) {
+    switch (a.N) {
+      T2_CASE(16, 16) T2_CASE(32, 32) T2_CASE(48, 48) T2_CASE(64, 64) T2_CASE(80, 80)
+      T2_CASE(96, 96) T2_CASE(112, 112) T2_CASE(128, 128) T2_CASE(144, 144) T2_CASE(160, 160)
+    }
+  } else if (a.N == 128) {
+    switch (a.N_last) {
+      T2_CASE(128, 32) T2_CASE(128, 48) T2_CASE(128, 64) T2_CASE(128, 80) T2_CASE(128, 96) T2_CASE(128, 112) T2_CASE(128, 128)
+    }
+  }
+#undef T2_CASE
+  set_error("avc_conv_block_tc: no kernel instance for N=%d (%d chunks, last %d)", a.N, a.nchunk, a.N_last);
+  return AVC_ERR_UNSUPPORTED;
+}
 
 int conv_block_tc2_launch(const avc_conv_desc* d, int* status, void* stream) {
   Tc2Args a;
@@ -915,19 +992,8 @@ int conv_block_tc2_launch(const avc_conv_desc* d, int* status, void* stream) {
     }
   }
   const int smem = (int)(a.off_stat + 2u * (uint32_t)a.G * 128u * 8u);
-  static bool attr_done = false;
-  if (!attr_done) {
-    cudaError_t e = cudaFuncSetAttribute(conv_block_tc2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, T2_SMEM_MAX);
-    if (e != cudaSuccess) {
-      set_error("avc_conv_block_tc: cudaFuncSetAttribute: %s", cudaGetErrorString(e));
-      return AVC_ERR_CUDA;
-    }
-    attr_done = true;
-  }
   const int grid = a.ntiles < t2_num_sms() ? a.ntiles : t2_num_sms();
-  AVC_LAUNCH(conv_block_tc2_kernel, grid, 384, smem, (cudaStream_t)stream, a, tmx, tmw);
-  AVC_CHECK_LAUNCH("conv_block_tc2");
-  return AVC_OK;
+  return t2_dispatch(a, tmx, tmw, grid, smem, (cudaStream_t)stream);
 }
 
 }  // namespace avc

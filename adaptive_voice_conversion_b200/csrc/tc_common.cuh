@@ -88,6 +88,14 @@ __host__ __device__ __forceinline__ uint64_t make_sdesc(uint32_t smem_addr, uint
 // warp index as a value ptxas can prove warp-uniform: role branches on it are uniform branches
 __device__ __forceinline__ int warp_idx_sync() { return __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0); }
 
+// ---- per-warpgroup register budget: all four warps of a warpgroup execute the SAME instruction.  The block starts with
+// the kernel's register count per thread; dec returns registers to the pool, inc waits until the pool can grant them,
+// so the budgets of all warpgroups must fit the block's allocation (count a multiple of 8 in [24, 256]).
+template <int R>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
+
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 template <int N>
