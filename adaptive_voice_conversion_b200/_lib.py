@@ -56,6 +56,13 @@ class ConvDesc(C.Structure):
     ]
 
 
+class TcPlan(C.Structure):
+    """avc_tc_plan: the tile plan of avc_conv_block_tc for one descriptor (avc_conv_block_tc_plan)."""
+    _fields_ = [(n, C.c_int32) for n in (
+        "G", "N", "N_last", "nchunk", "R", "srows", "hs", "nstage", "nst", "ntt", "TT", "Ts", "P", "mtiles", "ntiles", "patch",
+        "stage_bytes", "smem_bytes", "smem_max", "instance")]
+
+
 class WgradDesc(C.Structure):
     _fields_ = [
         ("B", C.c_int32), ("Cin", C.c_int32), ("Cout", C.c_int32), ("K", C.c_int32),
@@ -122,6 +129,7 @@ _i, _i64, _p = C.c_int, C.c_int64, C.c_void_p
 PROTOTYPES = {
     "avc_conv_block_fwd": (_i, [C.POINTER(ConvDesc), _p]),
     "avc_conv_block_tc": (_i, [C.POINTER(ConvDesc), _p, _p]),
+    "avc_conv_block_tc_plan": (_i, [C.POINTER(ConvDesc), _i, C.POINTER(TcPlan)]),
     "avc_pack_conv_weight_tc": (_i, [_p, _p, _i, _i, _i, _i, _p]),
     "avc_tc_packed_floats": (_i64, [_i, _i, _i]),
     "avc_tc2_set_debug": (None, [_p]),

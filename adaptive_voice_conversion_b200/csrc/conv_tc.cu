@@ -10,6 +10,7 @@ namespace avc {
 
 int validate_conv_desc(const avc_conv_desc* d, const char* who);
 int conv_block_tc2_launch(const avc_conv_desc* d, int* status, void* stream);  // conv_tc2.cu
+int conv_block_tc2_plan(const avc_conv_desc* d, int num_sms, avc_tc_plan* out);
 
 constexpr int TC_SLAB = 16;  // input channels per weight-pack slab (2 MMA K-steps)
 
@@ -123,11 +124,12 @@ extern "C" int avc_pack_conv_weight_tc(const float* w, float* packed, int Cout, 
   return AVC_OK;
 }
 
-extern "C" int avc_conv_block_tc(const avc_conv_desc* d, int* status, void* stream) {
+// the argument checks of avc_conv_block_tc (all but the status pointer), shared with the plan query
+static int check_conv_tc(const avc_conv_desc* d) {
   int rc = validate_conv_desc(d, "avc_conv_block_tc");
   if (rc != AVC_OK) return rc;
   const bool normbwd = (d->flags & AVC_F_NORMBWD) != 0;
-  AVC_REQUIRE(d->in && d->w_tc && (d->out || normbwd) && status, AVC_ERR_INVALID, "avc_conv_block_tc: null in/w_tc/out/status");
+  AVC_REQUIRE(d->in && d->w_tc && (d->out || normbwd), AVC_ERR_INVALID, "avc_conv_block_tc: null in/w_tc/out");
   AVC_REQUIRE(!normbwd || ((d->flags & AVC_F_FOLD) && d->save_c && d->dc && (!d->norm || d->stats) && (!d->cond || d->dcond) && !d->shuffle),
               AVC_ERR_INVALID, "avc_conv_block_tc: AVC_F_NORMBWD needs AVC_F_FOLD and the upstream block's save_c / stats / dc (dcond with cond)");
   AVC_REQUIRE((d->stride == 1 || d->stride == 2) && d->in_ups == 1, AVC_ERR_UNSUPPORTED, "avc_conv_block_tc: stride must be 1 or 2, in_ups 1");
@@ -144,5 +146,19 @@ extern "C" int avc_conv_block_tc(const avc_conv_desc* d, int* status, void* stre
   }
   AVC_REQUIRE(d->Cin % TC_SLAB == 0, AVC_ERR_UNSUPPORTED, "avc_conv_block_tc: Cin %% 16 != 0");
   AVC_REQUIRE(!d->res || d->res_mode != AVC_RES_NONE, AVC_ERR_INVALID, "avc_conv_block_tc: res without res_mode");
+  return AVC_OK;
+}
+
+extern "C" int avc_conv_block_tc(const avc_conv_desc* d, int* status, void* stream) {
+  const int rc = check_conv_tc(d);
+  if (rc != AVC_OK) return rc;
+  AVC_REQUIRE(status, AVC_ERR_INVALID, "avc_conv_block_tc: null status");
   return conv_block_tc2_launch(d, status, stream);
+}
+
+extern "C" int avc_conv_block_tc_plan(const avc_conv_desc* d, int num_sms, avc_tc_plan* out) {
+  AVC_REQUIRE(out, AVC_ERR_INVALID, "avc_conv_block_tc_plan: null out");
+  const int rc = check_conv_tc(d);
+  if (rc != AVC_OK) return rc;
+  return conv_block_tc2_plan(d, num_sms, out);
 }

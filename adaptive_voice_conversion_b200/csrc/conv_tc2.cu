@@ -817,8 +817,9 @@ static int t2_num_sms() {
   return n;
 }
 
-// returns AVC_OK and fills a, or AVC_ERR_UNSUPPORTED with the reason (the shape needs avc_conv_block_fwd)
-int t2_plan(const avc_conv_desc* d, Tc2Args& a) {
+// returns AVC_OK and fills a, or AVC_ERR_UNSUPPORTED with the reason (the shape needs avc_conv_block_fwd).  sms: SMs of the
+// device the kernel runs on (one persistent CTA each), which set the samples per tile.
+int t2_plan(const avc_conv_desc* d, int sms, Tc2Args& a) {
   const int K = d->K, S = d->stride;
   const bool fold = (d->flags & AVC_F_FOLD) != 0;
   a.d = *d;
@@ -850,7 +851,6 @@ int t2_plan(const avc_conv_desc* d, Tc2Args& a) {
   const int ncol = (a.TT - 1) * S + 1;
   a.R = ncol + K - 1;
   // samples per tile: minimise rounds x (fixed + MMA time); an N-column MMA costs ~max(40, N/2) cycles
-  const int sms = t2_num_sms();
   int bestG = 0;
   double best = 1e30;
   const int gmax = a.ntt > 1 ? 1 : T2_MAX_G;
@@ -909,8 +909,12 @@ int t2_plan(const avc_conv_desc* d, Tc2Args& a) {
   a.off_tile = (uint32_t)nstage * a.stage_bytes;
   a.off_par = a.off_tile + tile_bytes;
   a.off_stat = a.off_par + par_bytes;
+  a.patch = (!(d->flags & AVC_F_IN_TF32) || (d->pad_mode == AVC_PAD_REFLECT && K > 1)) ? 1 : 0;
   return AVC_OK;
 }
+
+// dynamic shared memory of a plan: the stages, the staged epilogue tile, the parameter and statistics arrays
+static uint32_t t2_smem_bytes(const Tc2Args& a) { return a.off_stat + 2u * (uint32_t)a.G * 128u * 8u; }
 
 static long long* g_tc2_dbg = nullptr;
 
@@ -931,32 +935,45 @@ static int t2_launch(const Tc2Args& a, const CUtensorMap& tmx, const CUtensorMap
   return AVC_OK;
 }
 
-// the instance for the plan's accumulator widths: N in 16..T2_MAX_N, or N = 128 with a last chunk of 32..128 columns
-static int t2_dispatch(const Tc2Args& a, const CUtensorMap& tmx, const CUtensorMap& tmw, int grid, int smem, cudaStream_t stream) {
-#define T2_CASE(n, nl) \
-  case nl: return t2_launch<n, nl>(a, tmx, tmw, grid, smem, stream);
-  if (a.nchunk == 1) {
-    switch (a.N) {
-      T2_CASE(16, 16) T2_CASE(32, 32) T2_CASE(48, 48) T2_CASE(64, 64) T2_CASE(80, 80)
-      T2_CASE(96, 96) T2_CASE(112, 112) T2_CASE(128, 128) T2_CASE(144, 144) T2_CASE(160, 160)
-    }
-  } else if (a.N == 128) {
-    switch (a.N_last) {
-      T2_CASE(128, 32) T2_CASE(128, 48) T2_CASE(128, 64) T2_CASE(128, 80) T2_CASE(128, 96) T2_CASE(128, 112) T2_CASE(128, 128)
-    }
-  }
-#undef T2_CASE
+// Kernel instances (N, NL): every accumulator width N in 16..T2_MAX_N, and N = 128 with a last column chunk of NL = 32..112
+// columns (a chunked sample whose last chunk is 128 wide runs <128, 128>).  The launch and the plan query both find the
+// instance of a plan in this table (t2_instance).
+struct T2Inst {
+  int n, nl;
+};
+constexpr T2Inst T2_INSTANCES[] = {{16, 16},  {32, 32},  {48, 48},  {64, 64},  {80, 80},  {96, 96},  {112, 112}, {128, 128},
+                                   {144, 144}, {160, 160}, {128, 32}, {128, 48}, {128, 64}, {128, 80}, {128, 96}, {128, 112}};
+constexpr int T2_NINST = (int)(sizeof(T2_INSTANCES) / sizeof(T2_INSTANCES[0]));
+
+// index into T2_INSTANCES of the instance that runs plan a, or -1
+static int t2_instance(const Tc2Args& a) {
+  const int nl = a.nchunk == 1 ? a.N : a.N_last;
+  for (int i = 0; i < T2_NINST; ++i)
+    if (T2_INSTANCES[i].n == a.N && T2_INSTANCES[i].nl == nl) return i;
+  return -1;
+}
+
+static int t2_no_instance(const Tc2Args& a) {
   set_error("avc_conv_block_tc: no kernel instance for N=%d (%d chunks, last %d)", a.N, a.nchunk, a.N_last);
   return AVC_ERR_UNSUPPORTED;
 }
 
+template <int I>
+static int t2_launch_instance(int inst, const Tc2Args& a, const CUtensorMap& tmx, const CUtensorMap& tmw, int grid, int smem, cudaStream_t stream) {
+  if constexpr (I < T2_NINST) {
+    if (inst == I) return t2_launch<T2_INSTANCES[I].n, T2_INSTANCES[I].nl>(a, tmx, tmw, grid, smem, stream);
+    return t2_launch_instance<I + 1>(inst, a, tmx, tmw, grid, smem, stream);
+  } else {
+    return t2_no_instance(a);
+  }
+}
+
 int conv_block_tc2_launch(const avc_conv_desc* d, int* status, void* stream) {
   Tc2Args a;
-  const int rc = t2_plan(d, a);
+  const int rc = t2_plan(d, t2_num_sms(), a);
   if (rc != AVC_OK) return rc;
   a.status = status;
   a.dbg = g_tc2_dbg;
-  a.patch = (!(d->flags & AVC_F_IN_TF32) || (d->pad_mode == AVC_PAD_REFLECT && d->K > 1)) ? 1 : 0;
   CUtensorMap tmx, tmw;
   {
     PFN_tmap_encode enc = tmap_encode_fn();
@@ -991,9 +1008,23 @@ int conv_block_tc2_launch(const avc_conv_desc* d, int* status, void* stream) {
       }
     }
   }
-  const int smem = (int)(a.off_stat + 2u * (uint32_t)a.G * 128u * 8u);
   const int grid = a.ntiles < t2_num_sms() ? a.ntiles : t2_num_sms();
-  return t2_dispatch(a, tmx, tmw, grid, smem, (cudaStream_t)stream);
+  return t2_launch_instance<0>(t2_instance(a), a, tmx, tmw, grid, (int)t2_smem_bytes(a), (cudaStream_t)stream);
+}
+
+// host only: the plan avc_conv_block_tc would run d with on a device of num_sms SMs (<= 0: the current device)
+int conv_block_tc2_plan(const avc_conv_desc* d, int num_sms, avc_tc_plan* out) {
+  Tc2Args a;
+  const int rc = t2_plan(d, num_sms > 0 ? num_sms : t2_num_sms(), a);
+  if (rc != AVC_OK) return rc;
+  *out = avc_tc_plan{};
+  out->G = a.G; out->N = a.N; out->N_last = a.N_last; out->nchunk = a.nchunk;
+  out->R = a.R; out->srows = a.srows; out->hs = a.hs; out->nstage = a.nstage; out->nst = a.nst;
+  out->ntt = a.ntt; out->TT = a.TT; out->Ts = a.Ts; out->P = a.P;
+  out->mtiles = a.mtiles; out->ntiles = a.ntiles; out->patch = a.patch;
+  out->stage_bytes = (int)a.stage_bytes; out->smem_bytes = (int)t2_smem_bytes(a); out->smem_max = T2_SMEM_MAX;
+  out->instance = t2_instance(a);
+  return out->instance >= 0 ? AVC_OK : t2_no_instance(a);
 }
 
 }  // namespace avc

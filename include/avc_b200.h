@@ -123,6 +123,26 @@ int avc_conv_block_fwd(const avc_conv_desc* d, void* stream);
  * AVC_ERR_UNSUPPORTED (use avc_conv_block_fwd).  Reads d->w_tc instead of d->w_packed.
  * status: device int, set non-zero if an internal pipeline barrier timed out. */
 int avc_conv_block_tc(const avc_conv_desc* d, int* status, void* stream);
+/* The tile plan avc_conv_block_tc runs a descriptor with.  Host only: launches nothing, reads no pointer; runs the same
+ * argument checks and returns AVC_ERR_UNSUPPORTED (with the message of avc_last_error()) where the launch would; `out` is
+ * filled when the plan exists, also when no kernel instance has its widths (instance = -1, AVC_ERR_UNSUPPORTED).
+ * num_sms: SMs of the device the kernel would run on; <= 0 = the current device. */
+typedef struct avc_tc_plan {
+  int32_t G;          /* samples per tile (stacked along the accumulator columns R rows apart) */
+  int32_t N, N_last;  /* accumulator columns of a column chunk, of the last chunk */
+  int32_t nchunk;     /* column chunks per tile (> 1: folded sample of more than 144 columns) */
+  int32_t R, srows;   /* staged rows per sample, per 4-channel plane of a stage (G * R) */
+  int32_t hs;         /* half-slabs (8 input channels) per pipeline stage */
+  int32_t nstage;     /* shared-memory stages of the ring */
+  int32_t nst;        /* pipeline stages per tile (and column chunk) */
+  int32_t ntt, TT;    /* time tiles per sample, output steps per time tile */
+  int32_t Ts, P;      /* columns one sample stages for the epilogue; chunk pitch of that tile in 16-byte units */
+  int32_t mtiles, ntiles;  /* 128-channel output tiles; tiles in all */
+  int32_t patch;      /* 1: the patch warps round / mirror the staged input */
+  int32_t stage_bytes, smem_bytes, smem_max;  /* one stage, dynamic shared memory of the launch, its limit */
+  int32_t instance;   /* index of the kernel instance for (N, N_last), or -1 */
+} avc_tc_plan;
+int avc_conv_block_tc_plan(const avc_conv_desc* d, int num_sms, avc_tc_plan* out);
 /* nn.Conv1d weight [Cout][Cin][K] -> tensor-core operand blocks (TF32-rounded), AVC_PACK_FWD or
  * AVC_PACK_DGRAD; avc_tc_packed_floats gives the buffer size for a conv with co_total output
  * and ci_total input channels (FWD: Cout, Cin; DGRAD: Cin, Cout). */
