@@ -124,6 +124,29 @@ class LinearBatchDesc(C.Structure):
     ]
 
 
+STFT_MAG, STFT_COMPLEX, STFT_PROJECT = 0, 1, 2
+MEL_TO_MAG, MAG_TO_MEL = 0, 1
+
+
+class AudioSeg(C.Structure):
+    _fields_ = [("sample_off", C.c_int64), ("n_samples", C.c_int32), ("frame_off", C.c_int32), ("n_frames", C.c_int32),
+                ("reserved", C.c_int32)]
+
+
+class AudioDesc(C.Structure):
+    _fields_ = [
+        ("n_fft", C.c_int32), ("hop", C.c_int32), ("win", C.c_int32), ("n_seg", C.c_int32),
+        ("n_frames", C.c_int32), ("n_samples", C.c_int32), ("mode", C.c_int32), ("n_iter", C.c_int32),
+        ("preemph", C.c_float), ("max_db", C.c_float), ("ref_db", C.c_float), ("reserved", C.c_int32),
+        ("segs", _fp), ("y", _fp), ("mag", _fp), ("X", _fp), ("frames", _fp), ("mag_out", _fp), ("mag_db", _fp),
+    ]
+
+
+class MelDesc(C.Structure):
+    _fields_ = [("rows", C.c_int32), ("n_mels", C.c_int32), ("n_bins", C.c_int32), ("dir", C.c_int32),
+                ("max_db", C.c_float), ("ref_db", C.c_float), ("in_", _fp), ("mat", _fp), ("out", _fp)]
+
+
 # name -> (restype, argtypes); the single source of truth for tests/test_cabi_symbols.py
 _i, _i64, _p = C.c_int, C.c_int64, C.c_void_p
 PROTOTYPES = {
@@ -163,6 +186,12 @@ PROTOTYPES = {
     "avc_sqnorm": (_i, [_p, _i64, _p, _p, _p]),
     "avc_adam_step": (_i, [_p, _p, _p, _p, _p, _i64, _p, _p, _p, _p]),
     "avc_fill_zero": (_i, [_p, _i64, _p]),
+    "avc_stft": (_i, [C.POINTER(AudioDesc), _p]),
+    "avc_istft": (_i, [C.POINTER(AudioDesc), _p]),
+    "avc_griffin_lim": (_i, [C.POINTER(AudioDesc), _p]),
+    "avc_frame_power": (_i, [C.POINTER(AudioDesc), _p, _p]),
+    "avc_deemphasis": (_i, [C.POINTER(AudioDesc), C.c_float, _p]),
+    "avc_mel_project": (_i, [C.POINTER(MelDesc), _p]),
     "avc_tc_probe_gemm": (_i, [_p, _i, _p, _i, C.POINTER(C.c_uint32), _i, _i, _i, _i, _i, _p, _p, _p]),
     "avc_tc_probe_set_ld_shift": (None, [_i]),
     "avc_probe_store": (_i, [_p, C.c_longlong, _i, _i, _p, _p]),

@@ -1,10 +1,9 @@
 """Inferencer with the reference's surface (inference.py:24-93).
 
-The model call (``AE.inference``) is the H100 path.  The wav <-> mel DSP of the reference
-(librosa STFT / Griffin-Lim in preprocess/tacotron/utils.py) is out of scope (SURVEY.md
-section 2 rows 8, 12) and its dependencies are not in this image: ``inference_from_path``
-uses a caller-supplied ``vocoder`` object with ``get_spectrograms(path)`` /
-``melspectrogram2wav(mel)`` and raises a clear error without one.  ``inference_batch`` is
+The model call (``AE.inference``) is the H100 path.  ``inference_from_path`` uses a
+caller-supplied ``vocoder`` object with ``get_spectrograms(path)`` / ``melspectrogram2wav(mel)``
+(``vocoder.Vocoder``, the reference's librosa STFT / Griffin-Lim DSP on the GPU) and raises a
+clear error without one.  ``inference_batch`` is
 the batched entry point BASELINE config 5 measures.
 """
 from __future__ import annotations
@@ -129,7 +128,7 @@ class Inferencer(object):
     def inference_from_path(self):
         if self.vocoder is None:
             raise RuntimeError("inference_from_path needs a vocoder with get_spectrograms/melspectrogram2wav "
-                               "(the reference's librosa/Griffin-Lim DSP is outside this hot-path build)")
+                               "(e.g. adaptive_voice_conversion_b200.vocoder.Vocoder)")
         src_mel, _ = self.vocoder.get_spectrograms(self.args.source)
         tar_mel, _ = self.vocoder.get_spectrograms(self.args.target)
         dev = local_device()

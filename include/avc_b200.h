@@ -339,6 +339,78 @@ int avc_adam_step(float* p, const float* g, float* m, float* v, float* vmax, int
 
 int avc_fill_zero(void* ptr, int64_t bytes, void* stream);
 
+/* ---- Vocoder DSP (csrc/audio.cu): the reference's librosa STFT / Griffin-Lim path
+ * (preprocess/tacotron/utils.py get_spectrograms, melspectrogram2wav), fp32.
+ *
+ * Every call takes a ragged batch: a DEVICE table of utterances, sorted by both frame_off and sample_off.  Frame f
+ * of utterance u lives in row segs[u].frame_off + f of the frame-major buffers; its signal is the n_samples floats
+ * at y + sample_off.  An STFT of a signal of n_samples gives 1 + n_samples / hop frames and needs
+ * n_samples >= n_fft/2 + 1 (one reflection); an iSTFT of n_frames gives hop * (n_frames - 1) samples.  No call uses
+ * atomics: an utterance gets the same bits in any batch.  Supported: n_fft = 2048, even win <= n_fft, 0 < hop <= win
+ * (AVC_ERR_UNSUPPORTED otherwise).  The window is the periodic Hann of length win centred in n_fft. */
+typedef struct avc_audio_seg {
+  int64_t sample_off;          /* first sample of the utterance in y */
+  int32_t n_samples;
+  int32_t frame_off, n_frames; /* first row and row count in the frame-major buffers */
+  int32_t reserved;
+} avc_audio_seg;
+
+#define AVC_STFT_MAG 0     /* mag_out = |X| and / or mag_db = clip((20 log10(max(1e-5,|X|)) - ref_db + max_db) / max_db, 1e-8, 1) */
+#define AVC_STFT_COMPLEX 1 /* X = the half spectrum */
+#define AVC_STFT_PROJECT 2 /* X = mag * E / max(1e-8, |E|), E the half spectrum: one Griffin-Lim projection */
+
+typedef struct avc_audio_desc {
+  int32_t n_fft, hop, win;
+  int32_t n_seg;     /* entries of segs */
+  int32_t n_frames;  /* rows of the frame-major buffers (sum of segs[].n_frames) */
+  int32_t n_samples; /* floats of y the table spans (iSTFT output grid) */
+  int32_t mode;      /* avc_stft: AVC_STFT_* */
+  int32_t n_iter;    /* avc_griffin_lim */
+  float preemph;     /* avc_stft: y'[n] = y[n] - preemph * y[n-1] applied on the fly (0: none) */
+  float max_db, ref_db; /* avc_stft MAG with mag_db */
+  int32_t reserved;
+  const avc_audio_seg* segs; /* DEVICE table */
+  float* y;          /* signal: avc_stft / avc_frame_power input, avc_istft / avc_griffin_lim output, avc_deemphasis in place */
+  const float* mag;  /* [n_frames][n_fft/2+1]: target magnitude S of PROJECT / avc_griffin_lim; avc_istft input when X is null */
+  float* X;          /* [n_frames][n_fft/2+1] complex (re, im): avc_stft COMPLEX / PROJECT output, avc_istft input,
+                        avc_griffin_lim workspace */
+  float* frames;     /* [n_frames][win] workspace of avc_istft / avc_griffin_lim: windowed inverse frames */
+  float* mag_out;    /* avc_stft MAG: [n_frames][n_fft/2+1] or null */
+  float* mag_db;     /* avc_stft MAG: [n_frames][n_fft/2+1] or null */
+} avc_audio_desc;
+
+/* STFT (center, reflect padding) of every utterance: one launch. */
+int avc_stft(const avc_audio_desc* d, void* stream);
+/* iSTFT: irfft x window per frame into `frames`, then a gather overlap-add divided by the exact window sum-square
+ * (where it exceeds FLT_MIN) with n_fft/2 cut from each end, into y.  X null: the spectrum is mag with zero phase.
+ * Two launches. */
+int avc_istft(const avc_audio_desc* d, void* stream);
+/* Griffin-Lim: X = mag (zero phase); n_iter x { X = mag * E / max(1e-8, |E|), E = stft(istft(X)) }; y = istft(X).
+ * 3 n_iter + 2 launches (iSTFT frames, overlap-add, projecting STFT per iteration). */
+int avc_griffin_lim(const avc_audio_desc* d, void* stream);
+/* power[frame] = mean of y^2 over frames of n_fft samples hop apart, reflect-padded by n_fft/2 (librosa's trim
+ * statistic): segs frame_off / n_frames count these frames, 1 + n_samples / hop per utterance.  Any even n_fft. */
+int avc_frame_power(const avc_audio_desc* d, float* power, void* stream);
+/* y[n] = y[n] + coef * y[n-1] over each utterance in place (scipy.signal.lfilter([1], [1, -coef])): an exact chunked
+ * scan, one CTA per utterance.  Reads segs, n_seg, y. */
+int avc_deemphasis(const avc_audio_desc* d, float coef, void* stream);
+
+/* Mel projections of the concatenated frames of a ragged batch (rows are independent).
+ *   AVC_MEL_TO_MAG: out[rows][n_bins] = A x mat, A = 10^((clip(in,0,1) max_db - max_db + ref_db) / 20),
+ *                   in [rows][n_mels], mat [n_mels][n_bins] (the transposed mel-to-linear matrix)
+ *   AVC_MAG_TO_MEL: out[rows][n_mels] = clip((20 log10(max(1e-5, in x mat)) - ref_db + max_db) / max_db, 1e-8, 1),
+ *                   in [rows][n_bins], mat [n_bins][n_mels] (the transposed filterbank) */
+#define AVC_MEL_TO_MAG 0
+#define AVC_MAG_TO_MEL 1
+typedef struct avc_mel_desc {
+  int32_t rows, n_mels, n_bins, dir;
+  float max_db, ref_db;
+  const float* in;
+  const float* mat;
+  float* out;
+} avc_mel_desc;
+int avc_mel_project(const avc_mel_desc* d, void* stream);
+
 /* wgmma self-test (one CTA): D[128][N] = sum_k A_k * B_k^T over nk K=8 tf32 steps, the
  * operands given as raw shared-memory images; strides[10] = {a_lbo, a_sbo, b_lbo, b_sbo,
  * a_kstep, b_kstep, a_off, b_off (bytes), a_layout, b_layout (must be 0: no swizzle)}; a_mn/b_mn must be 0
