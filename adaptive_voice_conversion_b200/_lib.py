@@ -159,7 +159,8 @@ PROTOTYPES = {
     "avc_pack_conv_weights_batch": (_i, [_p, _i, _i64, _p]),
     "avc_norm_apply_fwd": (_i, [C.POINTER(ConvDesc), _p]),
     "avc_norm_bwd": (_i, [C.POINTER(ConvDesc), _p]),
-    "avc_conv_wgrad": (_i, [C.POINTER(WgradDesc), _p]),
+    "avc_conv_wgrad_scratch_floats": (_i64, [C.POINTER(WgradDesc)]),
+    "avc_conv_wgrad": (_i, [C.POINTER(WgradDesc), _p, _p]),
     "avc_wgrad_tc_scratch_floats": (_i64, [C.POINTER(WgradDesc)]),
     "avc_conv_wgrad_tc": (_i, [C.POINTER(WgradDesc), _p, _p, _p]),
     "avc_wgrad_acc_floats": (_i64, [_i, _i, _i]),

@@ -16,6 +16,9 @@ namespace avc {
 
 void set_error(const char* fmt, ...);
 void count_launch(int n = 1);
+// dw += sum over slices of scratch[slice][tap][ci/4][coutp][4], in a fixed order (wgrad_tc.cu; both weight-gradient
+// kernels write their per-slice partial sums in this layout)
+int wgrad_reduce(const float* scratch, float* dw, int Cout, int Cin, int K, int coutp, int nslices, cudaStream_t stream);
 
 #define AVC_REQUIRE(cond, code, ...) \
   do {                               \

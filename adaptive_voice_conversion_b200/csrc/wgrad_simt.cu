@@ -1,8 +1,10 @@
 // Weight gradient of pad_layer + Conv1d (autograd of model.py:21-32 under solver.py:90):
 //   dW[co][ci][j] += sum_{b, t} dc[b][co][t] * xpad[b][ci][t*stride + j]
 // A [co x ci] GEMM per tap with the reduction over (sample, time).  One CTA: 128 co x
-// 128 ci for one tap and one slice of the batch; partial results are accumulated into the
-// (pre-zeroed) canonical nn.Conv1d-layout gradient with fp32 atomics.
+// 128 ci for one tap and one slice of the batch; its partial sums go to a scratch buffer
+// [slice][tap][ci/4][coutp][4] (the tensor-core kernel's layout) and wgrad_tc_reduce_kernel adds
+// them into the canonical nn.Conv1d-layout gradient in a fixed order: no atomics, so the
+// gradient is the same on every run.
 #include "common.cuh"
 
 namespace avc {
@@ -12,7 +14,8 @@ constexpr int WG_LD = 132;  // 128 + 4: conflict-free float4 staging stores
 
 struct WgradArgs {
   avc_wgrad_desc d;
-  int nsl, bps;  // batch slices, samples per slice
+  float* scratch;
+  int nsl, bps, coutp;  // batch slices, samples per slice, Cout rounded up to the 128-row tile
 };
 
 __global__ void __launch_bounds__(256, 2) conv_wgrad_kernel(const WgradArgs a) {
@@ -70,32 +73,26 @@ __global__ void __launch_bounds__(256, 2) conv_wgrad_kernel(const WgradArgs a) {
       __syncthreads();
     }
   }
+  // rows co >= Cout of the last tile hold zeros (their dc was staged as zeros); the reduction skips them
+  float* part = a.scratch + ((int64_t)sl * d.K + j) * (int64_t)(d.Cin >> 2) * a.coutp * 4;
 #pragma unroll
-  for (int i = 0; i < 8; ++i) {
-    const int co = co0 + ty * 8 + i;
-    if (co >= d.Cout) continue;
+  for (int h = 0; h < 2; ++h) {
+    const int ci = ci0 + tx * 8 + 4 * h;
+    if (ci >= d.Cin) continue;
 #pragma unroll
-    for (int k = 0; k < 8; ++k) {
-      const int ci = ci0 + tx * 8 + k;
-      if (ci < d.Cin) atomicAdd(d.dw + ((int64_t)co * d.Cin + ci) * d.K + j, acc[i][k]);
+    for (int i = 0; i < 8; ++i) {
+      const int co = co0 + ty * 8 + i;
+      st4(part + ((int64_t)(ci >> 2) * a.coutp + co) * 4,
+          make_float4(acc[i][4 * h], acc[i][4 * h + 1], acc[i][4 * h + 2], acc[i][4 * h + 3]));
     }
   }
 }
 
-}  // namespace avc
-
-using namespace avc;
-
-extern "C" int avc_conv_wgrad(const avc_wgrad_desc* d, void* stream) {
-  AVC_REQUIRE(d && d->x && d->dc && d->dw, AVC_ERR_INVALID, "avc_conv_wgrad: null argument");
-  AVC_REQUIRE(d->B > 0 && d->Cin > 0 && d->Cout > 0 && d->K >= 1 && d->Tin > 0 && d->Tout > 0, AVC_ERR_INVALID,
-              "avc_conv_wgrad: bad shape");
-  AVC_REQUIRE(d->Cin % 4 == 0 && d->Cout % 4 == 0, AVC_ERR_INVALID, "avc_conv_wgrad: channels must be multiples of 4");
-  WgradArgs a;
+static void wgrad_simt_plan(const avc_wgrad_desc* d, WgradArgs& a) {
   a.d = *d;
   const int tiles = cdiv(d->Cin, 128) * cdiv(d->Cout, 128) * d->K;
   // enough CTAs for ~2 waves of 148 SMs, but keep >= 256 reduction steps per CTA so the
-  // atomic epilogue stays a minor cost
+  // partial sums' round trip through the scratch buffer stays a minor cost
   int64_t kdepth = (int64_t)d->B * d->Tout;
   int nsl = (int)cdiv64(2 * 148 * 2, tiles);
   int max_by_depth = (int)(kdepth / 256);
@@ -105,8 +102,34 @@ extern "C" int avc_conv_wgrad(const avc_wgrad_desc* d, void* stream) {
   if (nsl < 1) nsl = 1;
   a.bps = cdiv(d->B, nsl);
   a.nsl = cdiv(d->B, a.bps);
+  a.coutp = cdiv(d->Cout, 128) * 128;
+}
+
+static bool wgrad_simt_valid(const avc_wgrad_desc* d) {
+  return d->B > 0 && d->Cin > 0 && d->Cout > 0 && d->K >= 1 && d->Tin > 0 && d->Tout > 0 && d->Cin % 4 == 0 && d->Cout % 4 == 0;
+}
+
+}  // namespace avc
+
+using namespace avc;
+
+extern "C" int64_t avc_conv_wgrad_scratch_floats(const avc_wgrad_desc* d) {
+  if (!d || !wgrad_simt_valid(d)) return -1;
+  WgradArgs a;
+  wgrad_simt_plan(d, a);
+  return (int64_t)a.nsl * d->K * d->Cin * a.coutp;
+}
+
+extern "C" int avc_conv_wgrad(const avc_wgrad_desc* d, float* scratch, void* stream) {
+  AVC_REQUIRE(d && d->x && d->dc && d->dw && scratch, AVC_ERR_INVALID, "avc_conv_wgrad: null argument");
+  AVC_REQUIRE(d->B > 0 && d->Cin > 0 && d->Cout > 0 && d->K >= 1 && d->Tin > 0 && d->Tout > 0, AVC_ERR_INVALID,
+              "avc_conv_wgrad: bad shape");
+  AVC_REQUIRE(d->Cin % 4 == 0 && d->Cout % 4 == 0, AVC_ERR_INVALID, "avc_conv_wgrad: channels must be multiples of 4");
+  WgradArgs a;
+  wgrad_simt_plan(d, a);
+  a.scratch = scratch;
   dim3 grid(cdiv(d->Cin, 128), cdiv(d->Cout, 128), d->K * a.nsl);
   AVC_LAUNCH(conv_wgrad_kernel, grid, 256, 0, (cudaStream_t)stream, a);
   AVC_CHECK_LAUNCH("conv_wgrad");
-  return AVC_OK;
+  return wgrad_reduce(scratch, d->dw, d->Cout, d->Cin, d->K, a.coutp, a.nsl, (cudaStream_t)stream);
 }

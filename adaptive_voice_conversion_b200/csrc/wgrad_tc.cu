@@ -295,6 +295,13 @@ static bool wgrad_tc_supported(const avc_wgrad_desc* d) {
          d->Cout % 4 == 0 && d->Tin + d->K - 1 >= (d->Tout - 1) * d->stride + 1 && (d->stride == 1 || d->Tout <= 64);
 }
 
+int wgrad_reduce(const float* scratch, float* dw, int Cout, int Cin, int K, int coutp, int nslices, cudaStream_t stream) {
+  const int64_t n = (int64_t)K * (Cin / 4) * coutp;
+  AVC_LAUNCH(wgrad_tc_reduce_kernel, (int)cdiv64(n, 32), dim3(32, 8), 0, stream, scratch, dw, Cout, Cin, K, coutp, nslices);
+  AVC_CHECK_LAUNCH("wgrad_tc_reduce");
+  return AVC_OK;
+}
+
 }  // namespace avc
 
 using namespace avc;
@@ -331,10 +338,7 @@ static int wgrad_tc_launch(const avc_wgrad_desc* d, float* scratch, int* status,
   else AVC_LAUNCH(conv_wgrad_split_kernel<false>, grid, WG_THREADS, smem, (cudaStream_t)stream, a);
   AVC_CHECK_LAUNCH(who);
   if (accumulate) return AVC_OK;
-  const int64_t n = (int64_t)d->K * (d->Cin / 4) * a.coutp;
-  AVC_LAUNCH(wgrad_tc_reduce_kernel, (int)cdiv64(n, 32), dim3(32, 8), 0, (cudaStream_t)stream, scratch, d->dw, d->Cout, d->Cin, d->K, a.coutp, a.nslices);
-  AVC_CHECK_LAUNCH("wgrad_tc_reduce");
-  return AVC_OK;
+  return wgrad_reduce(scratch, d->dw, d->Cout, d->Cin, d->K, a.coutp, a.nslices, (cudaStream_t)stream);
 }
 
 extern "C" int avc_conv_wgrad_tc(const avc_wgrad_desc* d, float* scratch, int* status, void* stream) {

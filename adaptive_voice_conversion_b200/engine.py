@@ -458,7 +458,8 @@ class Engine:
                 scratch = self.empty(n)
                 self._ck(self.lib.avc_conv_wgrad_tc(C.byref(wd), scratch.data_ptr(), self.tc_status.data_ptr(), self.stream), f"conv_wgrad_tc[{name}]")
                 return
-        self._ck(self.lib.avc_conv_wgrad(C.byref(wd), self.stream), f"conv_wgrad[{name}]")
+        scratch = self.empty(int(self.lib.avc_conv_wgrad_scratch_floats(C.byref(wd))))
+        self._ck(self.lib.avc_conv_wgrad(C.byref(wd), scratch.data_ptr(), self.stream), f"conv_wgrad[{name}]")
 
     @staticmethod
     def _fill_epilogue(d, out, shuffle, norm, relu, cond, res, res_mode, stats):

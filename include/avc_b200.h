@@ -174,8 +174,10 @@ int avc_norm_apply_fwd(const avc_conv_desc* d, void* stream);
 int avc_norm_bwd(const avc_conv_desc* d, void* stream);
 
 /* Weight gradient of pad_layer+Conv1d: dW[co][ci][j] += sum_{b,t} dc[b][co][t] *
- * xpad[b][ci][t*stride + j]  (canonical nn.Conv1d layout, accumulated with atomics into a
- * zeroed buffer).  x is the conv input A4, dc the dense grad of the raw conv output. */
+ * xpad[b][ci][t*stride + j]  (canonical nn.Conv1d layout, added to dw's content).  x is the conv
+ * input A4, dc the dense grad of the raw conv output.  Exact fp32 on the FMA pipe, any shape with
+ * Cin % 4 == Cout % 4 == 0; deterministic: per-slice partial sums go to `scratch`, of
+ * avc_conv_wgrad_scratch_floats(d) floats (-1: invalid shape), and are reduced in a fixed order. */
 typedef struct avc_wgrad_desc {
   int32_t B, Cin, Cout, K, stride, pad_left, Tin, Tout;
   const float* x;
@@ -184,7 +186,8 @@ typedef struct avc_wgrad_desc {
   int64_t dc_bstride;
   float* dw; /* [Cout][Cin][K] */
 } avc_wgrad_desc;
-int avc_conv_wgrad(const avc_wgrad_desc* d, void* stream);
+int64_t avc_conv_wgrad_scratch_floats(const avc_wgrad_desc* d);
+int avc_conv_wgrad(const avc_wgrad_desc* d, float* scratch, void* stream);
 /* The same gradient on the tensor cores (mma.sync TF32, fp32
  * accumulate; deterministic two-stage reduction through `scratch`).  Supported for Tout % 8 == 0 with
  * stride 1 and Tout <= 128 or stride 2 and Tout <= 64: avc_wgrad_tc_scratch_floats returns the scratch size in floats,

@@ -17,7 +17,7 @@ class RecordingLib:
     def __getattr__(self, name):
         def f(*a):
             self.calls.append(name)
-            if name in ("avc_tc_packed_floats", "avc_wgrad_tc_scratch_floats"):
+            if name in ("avc_tc_packed_floats", "avc_wgrad_tc_scratch_floats", "avc_conv_wgrad_scratch_floats"):
                 return 64
             if name == "avc_wgrad_acc_floats":
                 return a[2] * a[1] * (((a[0] + 127) // 128) * 128)
