@@ -147,6 +147,11 @@ class MelDesc(C.Structure):
                 ("max_db", C.c_float), ("ref_db", C.c_float), ("in_", _fp), ("mat", _fp), ("out", _fp)]
 
 
+class GatherDesc(C.Structure):
+    _fields_ = [("corpus", _fp), ("starts", _fp), ("order", _fp), ("x", _fp), ("first", C.c_int64),
+                ("batch", C.c_int32), ("seg", C.c_int32), ("frame", C.c_int32), ("n_mels", C.c_int32)]
+
+
 # name -> (restype, argtypes); the single source of truth for tests/test_cabi_symbols.py
 _i, _i64, _p = C.c_int, C.c_int64, C.c_void_p
 PROTOTYPES = {
@@ -187,6 +192,7 @@ PROTOTYPES = {
     "avc_sqnorm": (_i, [_p, _i64, _p, _p, _p]),
     "avc_adam_step": (_i, [_p, _p, _p, _p, _p, _i64, _p, _p, _p, _p]),
     "avc_fill_zero": (_i, [_p, _i64, _p]),
+    "avc_segment_gather": (_i, [C.POINTER(GatherDesc), _p]),
     "avc_stft": (_i, [C.POINTER(AudioDesc), _p]),
     "avc_istft": (_i, [C.POINTER(AudioDesc), _p]),
     "avc_griffin_lim": (_i, [C.POINTER(AudioDesc), _p]),

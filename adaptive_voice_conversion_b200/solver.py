@@ -6,17 +6,21 @@ What changed underneath: the model is the H100-native ``AE``; one optimizer step
 ``FusedTrainer.step`` (hand-written forward+backward kernels, a single NCCL all-reduce of
 the flat gradient when launched with torchrun, fused clip+Adam(amsgrad)); checkpoints stay
 ``<path>.ckpt`` (model state_dict) + ``<path>.opt`` (torch.optim.Adam state_dict format),
-written by rank 0 only.  ``args.data_dir == 'synthetic'`` trains on N(0,1) segments.
+written by rank 0 only.  ``args.data_dir == 'synthetic'`` trains on N(0,1) segments.  A real data directory is
+loaded once; when the corpus fits in half of the device's memory it stays there and every batch is cut on the GPU
+(``DeviceSegments``, in a seeded order that a resumed run continues), otherwise the stock DataLoader reads it.
 """
 from __future__ import annotations
 
 import json
 import os
 
+import numpy as np
 import torch
 import yaml
 
-from .data_utils import PickleDataset, SyntheticSegments, get_data_loader
+from .data_utils import (DeviceSegments, PickleDataset, SyntheticSegments, corpus_device_bytes, device_corpus_fits,
+                         get_data_loader, load_corpus)
 from .model import AE
 from .optim import FusedAdam
 from .trainer import FusedTrainer
@@ -27,6 +31,10 @@ def _dist_info():
     if torch.distributed.is_available() and torch.distributed.is_initialized():
         return torch.distributed.get_rank(), torch.distributed.get_world_size()
     return 0, 1
+
+
+def _device_total_memory(dev) -> int:
+    return torch.cuda.get_device_properties(dev).total_memory
 
 
 class Solver(object):
@@ -76,6 +84,8 @@ class Solver(object):
         if os.path.exists(it_path):    # absent for checkpoints written by the reference: start at 0 like it does
             with open(it_path) as f:
                 self.iteration = int(json.load(f)["iteration"])
+        if isinstance(self.train_loader, DeviceSegments):   # continue the uninterrupted run's batch sequence
+            self.train_loader.seek(self.iteration)
         self.trainer.eng.pack_weights(self.trainer.P, need_dgrad=True)
 
     # ---- data (solver.py:57-68)
@@ -88,11 +98,28 @@ class Solver(object):
             self.train_loader = SyntheticSegments(dl["batch_size"], n_mels * dl["frame_size"], dl["segment_size"] // dl["frame_size"],
                                                   seed=1 + self.rank)
         else:
-            self.train_dataset = PickleDataset(os.path.join(data_dir, f"{self.args.train_set}.pkl"),
-                                               os.path.join(data_dir, self.args.train_index_file),
-                                               segment_size=dl["segment_size"])
-            self.train_loader = get_data_loader(self.train_dataset, frame_size=dl["frame_size"], batch_size=dl["batch_size"],
-                                                shuffle=dl["shuffle"], num_workers=4, drop_last=False)
+            data, indexes = load_corpus(os.path.join(data_dir, f"{self.args.train_set}.pkl"),
+                                        os.path.join(data_dir, self.args.train_index_file))
+            # a corpus that fits in half of the device's memory is kept there and every batch is cut on the GPU;
+            # a larger one is read by the stock DataLoader, as the reference does
+            total_frames = sum(len(a) for a in data.values())
+            n_mels = np.shape(next(iter(data.values())))[-1] if data else 0
+            total_mem = _device_total_memory(local_device())
+            nbytes = corpus_device_bytes(total_frames, n_mels, len(indexes))
+            on_device = device_corpus_fits(total_frames, n_mels, len(indexes), total_mem)
+            if self.rank == 0:
+                print(f"training data: {len(data)} utterances, {total_frames} frames x {n_mels} mels, {len(indexes)} index entries; "
+                      f"{'device-resident corpus' if on_device else 'host DataLoader'} ({nbytes / 1e9:.2f} GB on the device "
+                      f"{'<=' if nbytes <= total_mem // 2 else '>'} half of its {total_mem / 1e9:.1f} GB)")
+            if on_device:
+                self.train_dataset = None
+                self.train_loader = DeviceSegments(data, indexes, dl["segment_size"], dl["frame_size"], dl["batch_size"],
+                                                   self.config["ContentEncoder"]["c_in"], rank=self.rank, shuffle=dl["shuffle"])
+            else:
+                self.train_dataset = PickleDataset.from_loaded(data, indexes, segment_size=dl["segment_size"])
+                self.train_loader = get_data_loader(self.train_dataset, frame_size=dl["frame_size"], batch_size=dl["batch_size"],
+                                                    shuffle=dl["shuffle"], num_workers=4, drop_last=False)
+            del data, indexes
         self.train_iter = infinite_iter(self.train_loader)
 
     # ---- model + optimizer (solver.py:70-79)

@@ -342,6 +342,23 @@ int avc_adam_step(float* p, const float* g, float* m, float* v, float* vmax, int
 
 int avc_fill_zero(void* ptr, int64_t bytes, void* stream);
 
+/* ---- Device-resident training corpus (csrc/corpus.cu, data_utils.DeviceSegments).
+ * One training batch cut out of the corpus in the layout CollateFn (data_utils.py:10-22) gives, bit for bit:
+ *   x[b][j*n_mels + m][tau] = corpus[(starts[order[first + b]] + tau*frame + j) * n_mels + m],
+ *   tau < seg/frame, j < frame, b < batch.
+ * A plain copy (no atomics, one thread per output element).  The kernel trusts `starts` and `order`: every crop must lie
+ * inside the corpus and first + batch must not exceed the table (the host validates them once, at load).
+ * AVC_ERR_INVALID for null pointers, n_mels % 4 != 0, seg % frame != 0 or batch < 1. */
+typedef struct avc_gather_desc {
+  const float* corpus;   /* [total_frames][n_mels]: every utterance's [T][n_mels] frames, end to end */
+  const int64_t* starts; /* [entries] absolute start frame of each index entry (utterance offset + t) */
+  const int32_t* order;  /* a permutation of the index entries (the epoch order) */
+  float* x;              /* [batch][frame*n_mels][seg/frame] */
+  int64_t first;         /* position in `order` of the batch's first entry */
+  int32_t batch, seg, frame, n_mels; /* seg = segment_size in frames, frame = frame_size */
+} avc_gather_desc;
+int avc_segment_gather(const avc_gather_desc* d, void* stream);
+
 /* ---- Vocoder DSP (csrc/audio.cu): the reference's librosa STFT / Griffin-Lim path
  * (preprocess/tacotron/utils.py get_spectrograms, melspectrogram2wav), fp32.
  *
