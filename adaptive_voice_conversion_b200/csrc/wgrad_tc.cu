@@ -1,189 +1,205 @@
-// Conv weight gradient on the tensor cores (mma.sync m16n8k8, TF32 in, fp32 accumulate in registers):
-//   dW[co][ci][j] += sum_{b,t} dc[b][co][t] * xpad[b][ci][t + j]        (stride 1)
+// Conv weight gradient on the tensor cores (wgmma m64nNk8, TF32 in, fp32 accumulate in registers):
+//   dW[co][ci][j] += sum_{b,t} dc[b][co][t] * xpad[b][ci][t * stride + j]
 // (autograd of pad_layer + nn.Conv1d w.r.t. the weight, model.py:21-32 under solver.py:90).
 //
-// GEMM view: M = co (128 per CTA), N = taps x ci (WT_NT ci per CTA), reduction K = time rows of a batch
-// slice.  The A4 activation layout [c/4][t][4] keeps 4 channels of one time step in a 16-byte unit,
-// so staging is a plain cp.async of units into an XOR-swizzled MN-major tile:
-//     byte(c, row) = (c/32)*LBO + row*128 + ((((c%32)/8) ^ (row%4)) * 32) + (c%8)*4
-// (conflict-free 16-byte stores).  tf32 wgmma reads K-major operands only, so the MMAs are warp-level:
-// every warp owns 16 co rows and loads its fragments from the staged tile with 32-bit shared loads.
-// The K taps are row shifts into ONE staged input tile whose reflect padding is resolved while staging.
-// Each CTA owns (co tile, ci tile, batch slice); partial sums go to a scratch buffer
-// [slice][tap][ci/4][co][4] and are reduced into the canonical nn.Conv1d gradient layout by
-// wgrad_tc_reduce_kernel (deterministic, no atomics), or added in place (ATOMIC, see below).
+// GEMM view: M = co (128 per CTA: two consumer warpgroups of m64), N = taps x ci (K taps x WT_NT = 32 ci per CTA, so
+// N = 32 K <= 256 and the accumulator is N / 2 <= 128 registers per consumer thread), reduction = the time rows of a
+// batch slice, WG_ROWS rows per pipeline stage.
+//
+// tf32 wgmma reads K-major operands only, and here K is time: the A4 activation layout [c/4][t][4] is MN-major for this
+// reduction.  So a staging warpgroup moves the operands through registers: it loads four 16-byte A4 units (4 channels x 4
+// consecutive time steps, 64 contiguous bytes for dc), transposes the 4 x 4 block and stores four 16-byte K-major units
+// into the no-swizzle core-matrix layout of tc_common.cuh -- per stage, plane p (time steps 4p..4p+3) holds one 16-byte
+// unit per operand row:
+//     A (dc):        [8 planes][128 co][4 t]        LBO = 128 x 16 B, SBO = 128 B
+//     B (x, by tap): [8 planes][K x 32 rows][4 t]   row j * 32 + ci holds xpad[ci][t * stride + j]
+// The tap shifts, the reflect padding and the stride-2 gather are all resolved while staging, so ONE wgmma per k-step
+// covers every tap.  The fp32 bit patterns are stored as they are: the tensor core reads their TF32 part (truncation
+// toward zero, the operand model of tests/test_gpu_wgrad_exact.py).
+//
+// Each CTA owns (ci tile, co tile, batch slice); its partial sums go to a scratch buffer [slice][tap][ci/4][co][4] and
+// are reduced into the canonical nn.Conv1d gradient layout by wgrad_tc_reduce_kernel (fixed order, no atomics), or
+// added in place (ATOMIC, see below).
 #include "common.cuh"
 #include "tc_common.cuh"
 
 namespace avc {
 
-constexpr int WT_NT = 32;  // ci columns per CTA (K x 32 accumulator columns: <= 128 registers per thread)
+constexpr int WT_NT = 32;          // ci columns per CTA per tap
+constexpr int WG_ROWS = 32;        // reduction rows (time steps) per pipeline stage: 4 wgmma k-steps, 8 K-major planes
+constexpr int WG_A_BYTES = (WG_ROWS / 4) * 128 * 16;   // dc planes of one stage
+constexpr int WG_MAX_STAGES = 8;
+constexpr int WG_SMEM_MAX = 224 * 1024;
+constexpr int WG_THREADS = 384;    // warpgroup 0 stages the operands, warpgroups 1 and 2 issue the MMAs for co rows 0-63 / 64-127
 
 struct WgTcArgs {
   avc_wgrad_desc d;
   float* scratch;
-  int nslices, tiles_per_slice, G, RA, RX, ntpad, coutp, TX, H;  // H: rows of one parity block (stride 2)
-  uint32_t buf_bytes, x_off;
+  int nslices, samp_per_slice, nstage, coutp;
   int* status;
 };
 
-__device__ __forceinline__ float rtf32(float x) {
-  uint32_t r;
-  asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(x));
-  return __uint_as_float(r);
-}
-__device__ __forceinline__ float4 rtf32_4(float4 v) { return make_float4(rtf32(v.x), rtf32(v.y), rtf32(v.z), rtf32(v.w)); }
+// 4 x 4 transpose of the staging step: unit c of the K-major side = component c of the four A4 units
+__device__ __forceinline__ float comp4(const float4& v, int c) { return c == 0 ? v.x : c == 1 ? v.y : c == 2 ? v.z : v.w; }
 
-// 16-byte async global->shared copy; !valid writes zeros (src-size 0, nothing is read)
-__device__ __forceinline__ void cp_async16(void* smem_dst, const void* gsrc, bool valid) {
-  const int sz = valid ? 16 : 0;
-  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(tc::smem_u32(smem_dst)), "l"(gsrc), "r"(sz) : "memory");
-}
+// One staging job: four A4 units (4 channels at 4 consecutive reduction rows) -> four K-major units (4 reduction rows of
+// one channel) at operand rows row0 .. row0 + 3 of one plane.  Store k writes channel (k + rot) & 3 with rot = (c4 >> 1) & 3
+// of the job's 4-channel chunk c4: the 8 lanes of a 16-byte store phase (consecutive c4) then hit 8 different 16-byte
+// bank groups (a fixed order would put 4 of them on the same group).
+struct WgJob {
+  float4 v[4];
+  uint32_t dst;   // byte offset of operand row row0 of its plane inside the stage
+  int rot;
+};
 
-// byte offset of the 16-byte unit (channel chunk q = c/4, row) inside an operand buffer
-__device__ __forceinline__ uint32_t mn_unit_off(int q, int row, uint32_t atom_bytes) {
-  return (uint32_t)(q >> 3) * atom_bytes + (uint32_t)row * 128u + (uint32_t)((((q & 7) >> 1) ^ (row & 3)) << 5) + (uint32_t)((q & 1) << 4);
-}
-
-// one m16n8k8 TF32 tensor-core MMA (operands are fp32 bit patterns; the tensor core reads their TF32 part)
-__device__ __forceinline__ void mma_tf32_16x8x8(float* c, uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint32_t b0, uint32_t b1) {
-  asm volatile("mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, {%0, %1, %2, %3};"
-               : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
-               : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "r"(b0), "r"(b1));
-}
-__device__ __forceinline__ uint32_t lds_u32(const uint8_t* p) { return *reinterpret_cast<const uint32_t*>(p); }
-
-// Accumulator of one warp: co rows 16 warp + lane / 4 (+ 8) of the 128-row tile, n8 tile nt = 4 tap + (ci / 8) of the
-// WT_NT = 32 ci columns; acc[4 nt + {0, 1}] = columns 8 (nt % 4) + 2 (lane % 4) + {0, 1}, acc[4 nt + {2, 3}] the row + 8.
-constexpr int WG_NT_MAX = 4 * 8;   // n8 tiles for K <= 8
-
-// All MMAs of one staged tile (nsamp samples, reduction over their time rows) for the warp's 16 co rows.
-__device__ __forceinline__ void wgrad_mma_tile(const WgTcArgs& a, const uint8_t* sA, const uint8_t* sX, int nsamp, float* acc, int warp,
-                                               int lane) {
-  const int K = a.d.K, T = a.d.Tout, S = a.d.stride, H = a.H, TX = a.TX;
-  const uint32_t atomA = (uint32_t)a.RA * 128u, atomX = (uint32_t)a.RX * 128u;
-  const int gid = lane >> 2, tig = lane & 3;
-  const int m0 = warp * 16 + gid, m1 = m0 + 8;
-  const uint8_t* pA0 = sA + ((m0 & 3) << 2);
-  const uint8_t* pA1 = sA + ((m1 & 3) << 2);
-  for (int g = 0; g < nsamp; ++g) {
-    for (int ks = 0; ks < T / 8; ++ks) {
-      const int r0 = g * T + 8 * ks + tig;
-      const uint32_t a0 = lds_u32(pA0 + mn_unit_off(m0 >> 2, r0, atomA)), a1 = lds_u32(pA1 + mn_unit_off(m1 >> 2, r0, atomA));
-      const uint32_t a2 = lds_u32(pA0 + mn_unit_off(m0 >> 2, r0 + 4, atomA)), a3 = lds_u32(pA1 + mn_unit_off(m1 >> 2, r0 + 4, atomA));
-#pragma unroll
-      for (int nt = 0; nt < WG_NT_MAX; ++nt) {
-        if (nt < 4 * K) {
-          const int j = nt >> 2, n = (nt & 3) * 8 + gid;
-          // tap j reads padded input position t + j (stride 1), or parity block j & 1, row t + j / 2 (stride 2)
-          const int xr = (S == 1 ? g * TX + j : g * 2 * H + (j & 1) * H + (j >> 1)) + 8 * ks + tig;
-          const uint8_t* pX = sX + ((n & 3) << 2);
-          const uint32_t b0 = lds_u32(pX + mn_unit_off(n >> 2, xr, atomX)), b1 = lds_u32(pX + mn_unit_off(n >> 2, xr + 4, atomX));
-          mma_tf32_16x8x8(acc + 4 * nt, a0, a1, a2, a3, b0, b1);
-        }
-      }
-    }
-  }
-}
-
-// partial dW of this CTA: scratch[sl][tap][ci/4][co][4] (ATOMIC: added into the layer's accumulation buffer)
-template <bool ATOMIC>
-__device__ __forceinline__ void wgrad_store(const WgTcArgs& a, const float* acc, int warp, int lane) {
+// Job e of stage chunk `ch` (rows ch * WG_ROWS .. of the CTA's slice): e < 256 stages dc (co chunk e % 32, plane e / 32),
+// the rest stage x (ci chunk e % 8, plane e / 8 % 8, tap e / 64).  Rows past the slice and channels past Cin / Cout are zeros.
+template <int K>
+__device__ __forceinline__ WgJob wgrad_job_load(const WgTcArgs& a, int e, int ch, int b0, int R) {
   const avc_wgrad_desc& d = a.d;
-  const int ci0 = blockIdx.x * WT_NT, co0 = blockIdx.y * 128, sl = blockIdx.z;
-  const int gid = lane >> 2, tig = lane & 3;
+  const int T = d.Tout;
+  WgJob J;
+  const bool is_dc = e < 256;
+  const int f = is_dc ? e : e - 256;
+  const int c4 = is_dc ? (f & 31) : (f & 7), pl = is_dc ? (f >> 5) : ((f >> 3) & 7), j = is_dc ? 0 : (f >> 6);
+  const int r = ch * WG_ROWS + 4 * pl;
+  const int g = r / T, t = r - g * T;   // T % 8 == 0: the 4 rows lie in one sample
+  J.rot = (c4 >> 1) & 3;
+  if (is_dc) {
+    J.dst = (uint32_t)pl * (128u * 16u) + (uint32_t)(4 * c4) * 16u;
+    const int co = blockIdx.y * 128 + 4 * c4;
+    if (r < R && co < d.Cout) {
+      const float* src = d.dc + (size_t)(b0 + g) * d.dc_bstride + ((size_t)(co >> 2) * T + t) * 4;
 #pragma unroll
-  for (int nt = 0; nt < WG_NT_MAX; ++nt) {
-    if (nt < 4 * d.K) {
-      const int j = nt >> 2, ci = ci0 + (nt & 3) * 8 + 2 * tig;
-      if (ci < d.Cin) {
-        float* sbase = a.scratch + (((size_t)(ATOMIC ? 0 : sl) * d.K + j) * (size_t)(d.Cin >> 2)) * (size_t)a.coutp * 4;
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          const int co = co0 + warp * 16 + gid + 8 * h;
-          float* p = sbase + ((size_t)(ci >> 2) * a.coutp + co) * 4 + (ci & 3);
-          const float v0 = acc[4 * nt + 2 * h], v1 = acc[4 * nt + 2 * h + 1];
-          if constexpr (ATOMIC)
-            asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(p), "f"(v0), "f"(v1) : "memory");
-          else
-            *reinterpret_cast<float2*>(p) = make_float2(v0, v1);
-        }
-      }
-    }
-  }
-}
-
-constexpr int WG_THREADS = 256;   // 8 warps: staging, then 16 co rows of MMAs each
-
-// Stage one tile of operands with cp.async: dc as [4 atoms of 32 co][G*T rows][128 B], x with the reflect padding resolved
-// as [ntpad/32 atoms][G*(T+K-1) rows][128 B] (stride 2: even and odd padded positions in separate row blocks, so tap j
-// addresses rows (j&1)*H + t + (j>>1) -- contiguous in t).  A warp writes 4 rows x the 8 units of one 128-byte atom row
-// (four whole bank sweeps); each thread walks its rows with (g, t) kept incrementally.
-__device__ __forceinline__ void wgrad_stage(const WgTcArgs& a, uint8_t* sA, uint8_t* sX, int b0, int nsamp, int tid) {
-  const avc_wgrad_desc& d = a.d;
-  const int ci0 = blockIdx.x * WT_NT, co0 = blockIdx.y * 128;
-  const int T = d.Tout, TX = a.TX, S = d.stride, H = a.H;
-  const uint32_t atomA = (uint32_t)a.RA * 128u, atomX = (uint32_t)a.RX * 128u;
-  {
-    const int q = ((tid >> 5) & 3) * 8 + (tid & 7), r_lo = ((tid >> 7) << 2) + ((tid >> 3) & 3);
-    const int co = co0 + 4 * q;
-    const bool cv = co < d.Cout;
-    const float* colsrc = d.dc + (size_t)((cv ? co : 0) >> 2) * T * 4;
-    int g = r_lo / T, t = r_lo - g * T;
-    for (int r = r_lo; r < nsamp * T; r += 8) {
-      cp_async16(sA + mn_unit_off(q, r, atomA), colsrc + (size_t)(b0 + g) * d.dc_bstride + (size_t)t * 4, cv);
-      t += 8;
-      while (t >= T) { t -= T; ++g; }
-    }
-  }
-  {
-    const int nq_x = a.ntpad >> 2;
-    const int natom = nq_x >> 3, wpa = 8 / natom;             // warps per atom
-    const int w = tid >> 5, atom = w % natom, rg = w / natom;  // row group of this warp
-    const int q = atom * 8 + (tid & 7), r_lo = (rg << 2) + ((tid >> 3) & 3), rstep = wpa << 2;
-    const int ci = ci0 + 4 * q;
-    const bool civ = ci < d.Cin;
-    const float* colsrc = d.x + (size_t)((civ ? ci : 0) >> 2) * d.Tin * 4;
-    int g = r_lo / TX, u = r_lo - g * TX;
-    for (int r0 = r_lo; r0 < nsamp * TX; r0 += rstep) {
-      const int r = S == 1 ? r0 : g * 2 * H + (u & 1) * H + (u >> 1);
-      const int p = src_pos(u - d.pad_left, d.Tin, AVC_PAD_REFLECT, 1);
-      const bool v = civ && p >= 0;
-      cp_async16(sX + mn_unit_off(q, r, atomX), colsrc + (size_t)(b0 + g) * d.x_bstride + (size_t)(p >= 0 ? p : 0) * 4, v);
-      u += rstep;
-      while (u >= TX) { u -= TX; ++g; }
-    }
-  }
-  asm volatile("cp.async.commit_group;" ::: "memory");
-}
-
-// Weight gradient of one (ci tile, co tile, batch slice): the copies of tile i+1 are in flight (cp.async, second
-// buffer) while the MMAs of tile i run.
-template <bool ATOMIC>
-__global__ void __launch_bounds__(WG_THREADS, 1) conv_wgrad_split_kernel(const WgTcArgs a) {
-  extern __shared__ __align__(1024) uint8_t smem[];
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int tile0 = blockIdx.z * a.tiles_per_slice;
-  const int tile1 = min(cdiv(a.d.B, a.G), tile0 + a.tiles_per_slice);
-  float acc[4 * WG_NT_MAX];
-#pragma unroll
-  for (int i = 0; i < 4 * WG_NT_MAX; ++i) acc[i] = 0.f;
-  if (tile1 > tile0) wgrad_stage(a, smem, smem + a.x_off, tile0 * a.G, min(a.G, a.d.B - tile0 * a.G), tid);
-  for (int tile = tile0; tile < tile1; ++tile) {
-    const int it = tile - tile0;
-    uint8_t* sA = smem + (size_t)(it & 1) * a.buf_bytes;
-    if (tile + 1 < tile1) {
-      uint8_t* sN = smem + (size_t)((it + 1) & 1) * a.buf_bytes;
-      wgrad_stage(a, sN, sN + a.x_off, (tile + 1) * a.G, min(a.G, a.d.B - (tile + 1) * a.G), tid);
-      asm volatile("cp.async.wait_group 1;" ::: "memory");
+      for (int i = 0; i < 4; ++i) J.v[i] = ldg4(src + 4 * i);
     } else {
-      asm volatile("cp.async.wait_group 0;" ::: "memory");
+#pragma unroll
+      for (int i = 0; i < 4; ++i) J.v[i] = zero4();
     }
-    __syncthreads();
-    wgrad_mma_tile(a, sA, sA + a.x_off, min(a.G, a.d.B - tile * a.G), acc, warp, lane);
-    __syncthreads();   // the buffer is restaged two tiles later
+  } else {
+    J.dst = (uint32_t)WG_A_BYTES + (uint32_t)pl * (uint32_t)(K * WT_NT * 16) + (uint32_t)(j * WT_NT + 4 * c4) * 16u;
+    const int ci = blockIdx.x * WT_NT + 4 * c4;
+    const bool v = r < R && ci < d.Cin;
+    const float* col = d.x + (size_t)(v ? b0 + g : 0) * d.x_bstride + (size_t)((v ? ci : 0) >> 2) * d.Tin * 4;
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      const int p = src_pos((t + i) * d.stride + j - d.pad_left, d.Tin, AVC_PAD_REFLECT, 1);
+      J.v[i] = (v && p >= 0) ? ldg4(col + (size_t)p * 4) : zero4();
+    }
   }
-  if (tile1 > tile0) wgrad_store<ATOMIC>(a, acc, warp, lane);
+  return J;
+}
+
+__device__ __forceinline__ void wgrad_job_store(uint8_t* stage, const WgJob& J) {
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    const int c = (k + J.rot) & 3;
+    *reinterpret_cast<float4*>(stage + J.dst + (uint32_t)c * 16u) = make_float4(comp4(J.v[0], c), comp4(J.v[1], c), comp4(J.v[2], c), comp4(J.v[3], c));
+  }
+}
+
+// Weight gradient of one (ci tile, co tile, batch slice).  mbarrier ring over the slice's row chunks: full[s] = the four
+// staging warps wrote stage s, empty[s] = both consumer warpgroups' MMAs on stage s retired.  A consumer queues the MMAs of
+// stage i, then wait_group 1 retires those of stage i - 1 and releases it; every CTA accumulates its rows in a fixed order.
+// 168 registers per thread (the __launch_bounds__ cap of 384 threads) hold the N / 2 <= 128 accumulators without a
+// register split between the roles.
+template <int K, bool ATOMIC>
+__global__ void __launch_bounds__(WG_THREADS, 1) conv_wgrad_wgmma_kernel(const WgTcArgs a) {
+  constexpr int N = K * WT_NT;
+  constexpr uint32_t B_PLANE = N * 16;
+  extern __shared__ __align__(1024) uint8_t smem[];
+  __shared__ uint64_t bar_full[WG_MAX_STAGES], bar_empty[WG_MAX_STAGES];
+  const avc_wgrad_desc& d = a.d;
+  const int tid = threadIdx.x, warp = tc::warp_idx_sync(), lane = tid & 31;
+  const int sl = blockIdx.z, b0 = sl * a.samp_per_slice;
+  const int R = max(0, min(a.samp_per_slice, d.B - b0)) * d.Tout;   // reduction rows of the slice
+  const int nchunk = cdiv(R, WG_ROWS);
+  const uint32_t stage_bytes = (uint32_t)WG_A_BYTES + 8u * B_PLANE;
+
+  if (tid == 0) {
+    for (int s = 0; s < a.nstage; ++s) {
+      tc::mbar_init(&bar_full[s], 4);
+      tc::mbar_init(&bar_empty[s], 2);
+    }
+    tc::fence_mbar_init();
+  }
+  __syncthreads();
+
+  if (warp < 4) {
+    // ================================================================ staging warpgroup
+    // The global loads are the latency the staging has to hide: every load of a thread's JPT jobs of a stage is issued
+    // before the first store, and before the wait for the stage to be free.
+    constexpr int NJOBS = 256 + 64 * K, JPT = (NJOBS + 127) / 128;
+    int s = 0;
+    uint32_t ph = 0;
+    for (int ch = 0; ch < nchunk; ++ch) {
+      WgJob J[JPT];
+#pragma unroll
+      for (int q = 0; q < JPT; ++q)
+        if (tid + 128 * q < NJOBS) J[q] = wgrad_job_load<K>(a, tid + 128 * q, ch, b0, R);
+      if (ch >= a.nstage && !__all_sync(0xffffffffu, tc::mbar_wait(&bar_empty[s], ph ^ 1u, a.status, 5))) return;
+      uint8_t* stage = smem + (size_t)s * stage_bytes;
+#pragma unroll
+      for (int q = 0; q < JPT; ++q)
+        if (tid + 128 * q < NJOBS) wgrad_job_store(stage, J[q]);
+      tc::fence_proxy_async_smem();   // the generic-proxy stores, before the async proxy (wgmma) reads them
+      __syncwarp();
+      if (lane == 0) tc::mbar_arrive(&bar_full[s]);
+      if (++s == a.nstage) { s = 0; ph ^= 1u; }
+    }
+    return;
+  }
+
+  // ================================================================ MMA warpgroups
+  const int wg = (warp >> 2) - 1, wt = tid & 127;
+  float acc[N / 2];
+#pragma unroll
+  for (int i = 0; i < N / 2; ++i) acc[i] = 0.f;
+  const uint32_t smem0 = tc::smem_u32(smem), d_hi = tc::sdesc_hi(128);
+  int s = 0, s_prev = -1;
+  uint32_t ph = 0;
+  tc::acc_fence(acc, N / 2);
+  for (int ch = 0; ch < nchunk; ++ch) {
+    if (!__all_sync(0xffffffffu, tc::mbar_wait(&bar_full[s], ph, a.status, 6))) {
+      tc::wgmma_wait<0>();
+      return;
+    }
+    const uint32_t sw = smem0 + (uint32_t)s * stage_bytes;
+    const uint32_t a_lo = tc::sdesc_lo(sw + (uint32_t)wg * 1024u, 128u * 16u), b_lo = tc::sdesc_lo(sw + (uint32_t)WG_A_BYTES, B_PLANE);
+    tc::wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < WG_ROWS / 8; ++k)   // k-step k: planes 2k and 2k + 1
+      tc::wgmma_tf32<N>(acc, tc::sdesc64(a_lo + (uint32_t)k * ((2u * 128u * 16u) >> 4), d_hi),
+                        tc::sdesc64(b_lo + (uint32_t)k * ((2u * B_PLANE) >> 4), d_hi), 1u);
+    tc::wgmma_commit();
+    tc::wgmma_wait<1>();
+    tc::acc_fence(acc, N / 2);
+    if (s_prev >= 0 && wt == 0) tc::mbar_arrive(&bar_empty[s_prev]);
+    s_prev = s;
+    if (++s == a.nstage) { s = 0; ph ^= 1u; }
+  }
+  tc::wgmma_wait<0>();
+  tc::acc_fence(acc, N / 2);
+  if (nchunk == 0) return;
+
+  // partial dW of this CTA: scratch[sl][tap][ci/4][co][4] (ATOMIC: added into the layer's accumulation buffer)
+  const int co = blockIdx.y * 128 + 64 * wg + tc::wg_acc_row(wt, 0);
+#pragma unroll
+  for (int jj = 0; jj < N / 8; ++jj) {
+    const int n = tc::wg_acc_col(wt, 4 * jj), j = n / WT_NT, ci = blockIdx.x * WT_NT + n % WT_NT;
+    if (ci < d.Cin) {
+      float* sbase = a.scratch + (((size_t)(ATOMIC ? 0 : sl) * K + j) * (size_t)(d.Cin >> 2)) * (size_t)a.coutp * 4;
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        float* p = sbase + ((size_t)(ci >> 2) * a.coutp + co + 8 * h) * 4 + (ci & 3);
+        const float v0 = acc[4 * jj + 2 * h], v1 = acc[4 * jj + 2 * h + 1];
+        if constexpr (ATOMIC)
+          asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(p), "f"(v0), "f"(v1) : "memory");
+        else
+          *reinterpret_cast<float2*>(p) = make_float2(v0, v1);
+      }
+    }
+  }
 }
 
 // dW[co][ci][j] += sum over slices of scratch[sl][j][ci/4][co][ci%4]
@@ -262,31 +278,23 @@ __global__ void __launch_bounds__(256) wgrad_acc_flush_kernel(const avc_wgrad_ac
   }
 }
 
+// The batch is split into slices of whole G-sample tiles (G * Tout ~ 128 rows, 64 for stride 2) so that the slices and
+// the CTAs of one slice fill the 132 SMs; the scratch buffer holds one partial dW per slice.
 static int wgrad_tc_plan(const avc_wgrad_desc* d, WgTcArgs& a) {
-  const int T = d->Tout, K = d->K;
+  const int T = d->Tout;
   a.d = *d;
-  a.G = T >= 128 ? 1 : 128 / T;
-  if (d->stride == 2) a.G = T >= 64 ? 1 : 64 / T;  // the parity-split input tile is twice as tall
-  a.RA = a.G * T;
-  // padded input positions one sample contributes: stride 1: T+K-1; stride 2: 2(T-1)+K
-  a.TX = d->stride == 1 ? T + K - 1 : 2 * (T - 1) + K;
-  a.H = ((a.TX + 1) / 2 + 3) / 4 * 4;
-  // atom stride must keep every atom base 512 B aligned: the swizzle XOR is keyed on absolute
-  // shared-memory address bits [7,9)
-  // (and 1024 B aligned for the tensor-map copies of the TMA-staged kernel: a swizzled destination must sit on the
-  // swizzle pattern's 8-row period)
-  a.RX = d->stride == 1 ? (a.G * a.TX + 7) / 8 * 8 : a.G * 2 * a.H;
-  a.ntpad = WT_NT;
+  int G = T >= 128 ? 1 : 128 / T;
+  if (d->stride == 2) G = T >= 64 ? 1 : 64 / T;
   a.coutp = cdiv(d->Cout, 128) * 128;
-  a.x_off = (uint32_t)(4 * a.RA * 128 + 1023) / 1024 * 1024;
-  a.buf_bytes = (a.x_off + (uint32_t)((a.ntpad / 32) * a.RX * 128) + 1023) / 1024 * 1024;
-  const int ntiles = cdiv(d->B, a.G);
+  const int ntiles = cdiv(d->B, G);
   const int cta_per_slice = cdiv(d->Cin, WT_NT) * cdiv(d->Cout, 128);
   int nsl = 132 / cta_per_slice;
   if (nsl < 1) nsl = 1;
   if (nsl > ntiles) nsl = ntiles;
-  a.tiles_per_slice = cdiv(ntiles, nsl);
-  a.nslices = cdiv(ntiles, a.tiles_per_slice);
+  const int tiles_per_slice = cdiv(ntiles, nsl);
+  a.nslices = cdiv(ntiles, tiles_per_slice);
+  a.samp_per_slice = tiles_per_slice * G;
+  a.nstage = min(WG_MAX_STAGES, WG_SMEM_MAX / (WG_A_BYTES + 8 * 16 * WT_NT * d->K));
   return AVC_OK;
 }
 
@@ -300,6 +308,39 @@ int wgrad_reduce(const float* scratch, float* dw, int Cout, int Cin, int K, int 
   AVC_LAUNCH(wgrad_tc_reduce_kernel, (int)cdiv64(n, 32), dim3(32, 8), 0, stream, scratch, dw, Cout, Cin, K, coutp, nslices);
   AVC_CHECK_LAUNCH("wgrad_tc_reduce");
   return AVC_OK;
+}
+
+// one kernel instance per tap count (N = 32 K accumulator columns) and output mode
+template <int K, bool ATOMIC>
+static int wgrad_wgmma_launch(const WgTcArgs& a, cudaStream_t stream, const char* who) {
+  static bool attr_done = false;
+  if (!attr_done) {
+    const cudaError_t e = cudaFuncSetAttribute(conv_wgrad_wgmma_kernel<K, ATOMIC>, cudaFuncAttributeMaxDynamicSharedMemorySize, WG_SMEM_MAX);
+    if (e != cudaSuccess) {
+      set_error("%s: cudaFuncSetAttribute: %s", who, cudaGetErrorString(e));
+      return AVC_ERR_CUDA;
+    }
+    attr_done = true;
+  }
+  const dim3 grid(cdiv(a.d.Cin, WT_NT), cdiv(a.d.Cout, 128), a.nslices);
+  const int smem = a.nstage * (WG_A_BYTES + 8 * 16 * WT_NT * K);
+  AVC_LAUNCH((conv_wgrad_wgmma_kernel<K, ATOMIC>), grid, WG_THREADS, smem, stream, a);
+  AVC_CHECK_LAUNCH(who);
+  return AVC_OK;
+}
+
+template <bool ATOMIC>
+static int wgrad_wgmma_dispatch(const WgTcArgs& a, cudaStream_t stream, const char* who) {
+  switch (a.d.K) {
+    case 1: return wgrad_wgmma_launch<1, ATOMIC>(a, stream, who);
+    case 2: return wgrad_wgmma_launch<2, ATOMIC>(a, stream, who);
+    case 3: return wgrad_wgmma_launch<3, ATOMIC>(a, stream, who);
+    case 4: return wgrad_wgmma_launch<4, ATOMIC>(a, stream, who);
+    case 5: return wgrad_wgmma_launch<5, ATOMIC>(a, stream, who);
+    case 6: return wgrad_wgmma_launch<6, ATOMIC>(a, stream, who);
+    case 7: return wgrad_wgmma_launch<7, ATOMIC>(a, stream, who);
+    default: return wgrad_wgmma_launch<8, ATOMIC>(a, stream, who);
+  }
 }
 
 }  // namespace avc
@@ -321,23 +362,8 @@ static int wgrad_tc_launch(const avc_wgrad_desc* d, float* scratch, int* status,
   wgrad_tc_plan(d, a);
   a.scratch = scratch;
   a.status = status;
-  const int smem = 2 * (int)a.buf_bytes;
-  AVC_REQUIRE(smem <= 224 * 1024, AVC_ERR_UNSUPPORTED, "%s: tile does not fit shared memory", who);
-  static bool attr_done = false;
-  if (!attr_done) {
-    cudaError_t e = cudaFuncSetAttribute(conv_wgrad_split_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 224 * 1024);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(conv_wgrad_split_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 224 * 1024);
-    if (e != cudaSuccess) {
-      set_error("%s: cudaFuncSetAttribute: %s", who, cudaGetErrorString(e));
-      return AVC_ERR_CUDA;
-    }
-    attr_done = true;
-  }
-  dim3 grid(cdiv(d->Cin, WT_NT), cdiv(d->Cout, 128), a.nslices);
-  if (accumulate) AVC_LAUNCH(conv_wgrad_split_kernel<true>, grid, WG_THREADS, smem, (cudaStream_t)stream, a);
-  else AVC_LAUNCH(conv_wgrad_split_kernel<false>, grid, WG_THREADS, smem, (cudaStream_t)stream, a);
-  AVC_CHECK_LAUNCH(who);
-  if (accumulate) return AVC_OK;
+  const int rc = accumulate ? wgrad_wgmma_dispatch<true>(a, (cudaStream_t)stream, who) : wgrad_wgmma_dispatch<false>(a, (cudaStream_t)stream, who);
+  if (rc != AVC_OK || accumulate) return rc;
   return wgrad_reduce(scratch, d->dw, d->Cout, d->Cin, d->K, a.coutp, a.nslices, (cudaStream_t)stream);
 }
 
