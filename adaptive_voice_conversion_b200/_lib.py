@@ -152,6 +152,26 @@ class GatherDesc(C.Structure):
                 ("batch", C.c_int32), ("seg", C.c_int32), ("frame", C.c_int32), ("n_mels", C.c_int32)]
 
 
+PCM_S16, PCM_F32 = 0, 1
+RESAMPLE_TILE, RESAMPLE_MAX_TAPS, RESAMPLE_MAX_PHASE_TAPS = 512, 8192, 96
+
+
+class ResampleSeg(C.Structure):
+    _fields_ = [("in_off", C.c_int64), ("out_off", C.c_int64), ("n_in", C.c_int32), ("n_out", C.c_int32),
+                ("channels", C.c_int32), ("tile0", C.c_int32)]
+
+
+class ResampleDesc(C.Structure):
+    _fields_ = [("format", C.c_int32), ("up", C.c_int32), ("down", C.c_int32), ("half_len", C.c_int32),
+                ("n_taps", C.c_int32), ("n_seg", C.c_int32), ("n_tiles", C.c_int32), ("reserved", C.c_int32),
+                ("segs", _fp), ("pcm", _fp), ("taps", _fp), ("out", _fp)]
+
+
+class MomentsDesc(C.Structure):
+    _fields_ = [("n_mels", C.c_int32), ("n_seg", C.c_int32), ("first", C.c_int64), ("segs", _fp), ("mels", _fp),
+                ("moments", _fp)]
+
+
 # name -> (restype, argtypes); the single source of truth for tests/test_cabi_symbols.py
 _i, _i64, _p = C.c_int, C.c_int64, C.c_void_p
 PROTOTYPES = {
@@ -199,6 +219,9 @@ PROTOTYPES = {
     "avc_frame_power": (_i, [C.POINTER(AudioDesc), _p, _p]),
     "avc_deemphasis": (_i, [C.POINTER(AudioDesc), C.c_float, _p]),
     "avc_mel_project": (_i, [C.POINTER(MelDesc), _p]),
+    "avc_resample_poly": (_i, [C.POINTER(ResampleDesc), _p]),
+    "avc_mel_moments": (_i, [C.POINTER(MomentsDesc), _p]),
+    "avc_mel_moments_merge": (_i, [_p, _p, C.c_int32, C.c_int32, _p, _p, _p, _p, _p]),
     "avc_tc_probe_gemm": (_i, [_p, _i, _p, _i, C.POINTER(C.c_uint32), _i, _i, _i, _i, _i, _p, _p, _p]),
     "avc_tc_probe_set_ld_shift": (None, [_i]),
     "avc_probe_store": (_i, [_p, C.c_longlong, _i, _i, _p, _p]),

@@ -89,12 +89,14 @@ def mel_to_linear_matrix(fb: np.ndarray) -> np.ndarray:
     return fb.T * d[None, :]
 
 
-def load_wav(path: str, sr: int) -> np.ndarray:
-    """A wav file as float32 mono at sr: channels averaged, integer PCM scaled to [-1, 1), resampled with
-    scipy.signal.resample_poly when the file has another rate."""
+def read_pcm(path: str):
+    """(rate, samples) of a wav file as stored: [n] or [n, channels], the file's own sample type."""
     from scipy.io import wavfile
-    from scipy.signal import resample_poly
-    rate, data = wavfile.read(path)
+    return wavfile.read(path)
+
+
+def scale_pcm(data: np.ndarray) -> np.ndarray:
+    """PCM samples as float64: integer PCM scaled to [-1, 1), float PCM as is."""
     if data.dtype.kind == "i":
         y = data / float(2 ** (8 * data.dtype.itemsize - 1))
     elif data.dtype.kind == "u":
@@ -102,6 +104,15 @@ def load_wav(path: str, sr: int) -> np.ndarray:
         y = (data - half) / half
     else:
         y = data.astype(np.float64)
+    return y
+
+
+def load_wav(path: str, sr: int) -> np.ndarray:
+    """A wav file as float32 mono at sr: channels averaged, integer PCM scaled to [-1, 1), resampled with
+    scipy.signal.resample_poly when the file has another rate."""
+    from scipy.signal import resample_poly
+    rate, data = read_pcm(path)
+    y = scale_pcm(data)
     if y.ndim == 2:
         y = y.mean(axis=1)
     if rate != sr:

@@ -431,6 +431,63 @@ typedef struct avc_mel_desc {
 } avc_mel_desc;
 int avc_mel_project(const avc_mel_desc* d, void* stream);
 
+/* ---- Corpus preparation (csrc/prep.cu, prepare.py): resampling from raw PCM and per-mel corpus statistics.
+ * No allocation, no synchronisation, no atomics: every output element is written by one thread in a fixed order, so
+ * an utterance gets the same bits in any batch and in any chunking.
+ *
+ * avc_resample_poly: per utterance, its channels averaged, then exactly the sum scipy.signal.resample_poly(x, up, down)
+ * computes (zero padding), in fp32 with a fixed accumulation order:
+ *   y[m] = sum_i x[k_m - i] * taps[r_m][i],  p_m = m*down + half_len, k_m = p_m / up, r_m = p_m % up,
+ *   i < (2*half_len - r_m) / up + 1, x[k] = 0 outside [0, n_in);  n_out = ceil(n_in * up / down)
+ * taps[r][i] = h[r + i*up] (zero past h's end), h = firwin(2*half_len + 1, 1/max(up, down), ('kaiser', 5.0)) * up,
+ * half_len = 10*max(up, down): the polyphase table [up][n_taps], n_taps = ceil((2*half_len + 1) / up).
+ * up = down = 1: y = x (conversion and channel mix only; taps may be null).
+ * AVC_ERR_INVALID for null pointers, n_seg < 1, n_tiles < 0, up/down < 1, an unknown format, or a tap table whose shape
+ * is not the one above; AVC_ERR_UNSUPPORTED for tables of more than AVC_RESAMPLE_MAX_TAPS floats or
+ * AVC_RESAMPLE_MAX_PHASE_TAPS taps per phase.  The kernel trusts the utterance table (offsets inside the buffers). */
+#define AVC_PCM_S16 0 /* int16, scaled by 1/32768 */
+#define AVC_PCM_F32 1 /* float32 as is */
+#define AVC_RESAMPLE_TILE 512          /* output samples per CTA */
+#define AVC_RESAMPLE_MAX_TAPS 8192     /* up * n_taps */
+#define AVC_RESAMPLE_MAX_PHASE_TAPS 96 /* n_taps */
+typedef struct avc_resample_seg {
+  int64_t in_off;    /* first PCM element of the utterance (element = one channel's sample) */
+  int64_t out_off;   /* first output sample */
+  int32_t n_in;      /* samples per channel */
+  int32_t n_out;     /* ceil(n_in * up / down) */
+  int32_t channels;  /* interleaved channels, >= 1 */
+  int32_t tile0;     /* first CTA of the utterance: sum of ceil(n_out / AVC_RESAMPLE_TILE) over the ones before it */
+} avc_resample_seg;
+typedef struct avc_resample_desc {
+  int32_t format;    /* AVC_PCM_* */
+  int32_t up, down, half_len, n_taps;
+  int32_t n_seg;     /* entries of segs */
+  int32_t n_tiles;   /* CTAs: tile0 + ceil(n_out / AVC_RESAMPLE_TILE) of the last utterance */
+  int32_t reserved;
+  const avc_resample_seg* segs; /* DEVICE table, sorted by tile0 */
+  const void* pcm;   /* interleaved PCM of every utterance */
+  const float* taps; /* [up][n_taps] */
+  float* out;        /* mono float32 at the new rate */
+} avc_resample_desc;
+int avc_resample_poly(const avc_resample_desc* d, void* stream);
+
+/* avc_mel_moments: for every utterance u of a ragged batch of [frames][n_mels] fp32 mels (segs frame_off / n_frames as in
+ * avc_audio_seg), in float64, two fixed-order passes over its own frames:
+ *   moments[first + u][m] = (mean_u[m], M2_u[m] = sum_t (x[t][m] - mean_u[m])^2).
+ * avc_mel_moments_merge: Chan's pairwise update over utterances 0 .. n_utts-1 in order (counts = their frame counts),
+ *   mean64[m], std64[m] = sqrt(M2[m] / N) (ddof 0) and their float32 roundings mean[m], std[m].
+ * AVC_ERR_INVALID for null pointers, n_seg < 1, n_mels < 1, first < 0 or n_utts < 1. */
+typedef struct avc_moments_desc {
+  int32_t n_mels, n_seg;
+  int64_t first;                /* global index of the batch's first utterance */
+  const avc_audio_seg* segs;    /* DEVICE table */
+  const float* mels;            /* [frames][n_mels] */
+  double* moments;              /* [n_utts][n_mels][2] */
+} avc_moments_desc;
+int avc_mel_moments(const avc_moments_desc* d, void* stream);
+int avc_mel_moments_merge(const double* moments, const int32_t* counts, int32_t n_utts, int32_t n_mels, float* mean,
+                          float* std, double* mean64, double* std64, void* stream);
+
 /* wgmma self-test (one CTA): D[128][N] = sum_k A_k * B_k^T over nk K=8 tf32 steps, the
  * operands given as raw shared-memory images; strides[10] = {a_lbo, a_sbo, b_lbo, b_sbo,
  * a_kstep, b_kstep, a_off, b_off (bytes), a_layout, b_layout (must be 0: no swizzle)}; a_mn/b_mn must be 0
