@@ -172,6 +172,15 @@ class MomentsDesc(C.Structure):
                 ("moments", _fp)]
 
 
+SN_ITERATE, SN_FIXED = 0, 1
+SN_MAX_ITEMS, SN_MAX_H, SN_MAX_W = 64, 4096, 4096
+
+
+class SnItem(C.Structure):
+    _fields_ = [("weight", _fp), ("w_bar", _fp), ("u", _fp), ("v", _fp), ("sigma", _fp), ("grad", _fp),
+                ("scratch_off", C.c_int64), ("h", C.c_int32), ("w", C.c_int32)]
+
+
 # name -> (restype, argtypes); the single source of truth for tests/test_cabi_symbols.py
 _i, _i64, _p = C.c_int, C.c_int64, C.c_void_p
 PROTOTYPES = {
@@ -222,6 +231,9 @@ PROTOTYPES = {
     "avc_resample_poly": (_i, [C.POINTER(ResampleDesc), _p]),
     "avc_mel_moments": (_i, [C.POINTER(MomentsDesc), _p]),
     "avc_mel_moments_merge": (_i, [_p, _p, C.c_int32, C.c_int32, _p, _p, _p, _p, _p]),
+    "avc_spectral_norm_scratch_floats": (_i64, [_i, _i]),
+    "avc_spectral_norm": (_i, [_p, _i, _i, _i, _i, _p, _p]),
+    "avc_spectral_norm_bwd": (_i, [_p, _i, _i, _i, _p, _p]),
     "avc_tc_probe_gemm": (_i, [_p, _i, _p, _i, C.POINTER(C.c_uint32), _i, _i, _i, _i, _i, _p, _p, _p]),
     "avc_tc_probe_set_ld_shift": (None, [_i]),
     "avc_probe_store": (_i, [_p, C.c_longlong, _i, _i, _p, _p]),

@@ -81,8 +81,8 @@ class Engine:
         for c in (se, ce):
             if c.get("act", "relu") != "relu" or c.get("dropout_rate", 0) != 0:
                 raise L.AvcError("only act='relu', dropout_rate=0 (the reference config.yaml) are implemented")
-        if de.get("act", "relu") != "relu" or de.get("dropout_rate", 0) != 0 or de.get("sn", False):
-            raise L.AvcError("Decoder: only act='relu', dropout_rate=0, sn=False are implemented")
+        if de.get("act", "relu") != "relu" or de.get("dropout_rate", 0) != 0:
+            raise L.AvcError("Decoder: only act='relu', dropout_rate=0 are implemented")
         for up in de["upsample"]:
             if up not in (1, 2):
                 raise L.AvcError("Decoder.upsample entries must be 1 or 2")
@@ -173,6 +173,10 @@ class Engine:
             for enc, key in (("speaker_encoder", "SpeakerEncoder"), ("content_encoder", "ContentEncoder")):
                 c = self.cfg[key]
                 self._bank_bias_table(enc, len(range(c["bank_scale"], c["bank_size"] + 1, c["bank_scale"])), G)
+        if self.sn_names():
+            self._sn_table(P, None)
+            if G is not None:
+                self._sn_table(P, G)
         if not self.fused_dense:
             return
         for names in (self._dense_names(), self._affine_names()):
@@ -277,6 +281,7 @@ class Engine:
         self._ck(self.lib.avc_pack_conv_weights_batch(raw.data_ptr(), n, max_elems, self.stream), "pack_weights_batch")
         for name in names:
             slot = self.packed[name]
+            slot["_ver"] = self._pack_version     # per layer: a pack of some prefixes leaves the others' packs valid
             for k in ("fwd", "dgrad"):
                 if k in slot:
                     slot[k + "_ver"] = self._pack_version if (self.precision == "fp32" or name in self._stride2_names()) else slot.get(k + "_ver", -1)
@@ -284,7 +289,7 @@ class Engine:
     def _ensure_simt_pack(self, P, name, key):
         """FFMA-layout pack of one layer on demand (shapes the tensor-core path does not cover)."""
         slot = self.packed.setdefault(name, {})
-        if slot.get(key + "_ver", -1) == getattr(self, "_pack_version", 0) and key in slot:
+        if slot.get(key + "_ver", -1) == slot.get("_ver", 0) and key in slot:
             return
         w = P[name + ".weight"]
         Cout, Cin, K = w.shape
@@ -292,7 +297,75 @@ class Engine:
             slot[key] = self.empty(w.numel())
         mode = L.PACK_FWD if key == "fwd" else L.PACK_DGRAD
         self._ck(self.lib.avc_pack_conv_weight(w.data_ptr(), slot[key].data_ptr(), Cout, Cin, K, mode, self.stream), "pack_w")
-        slot[key + "_ver"] = getattr(self, "_pack_version", 0)
+        slot[key + "_ver"] = slot.get("_ver", 0)
+
+    # ------------------------------------------------------------------ spectral norm (Decoder sn=True)
+    def sn_names(self) -> List[str]:
+        """The decoder layers the reference wraps in torch.nn.utils.spectral_norm when Decoder.sn is set (its
+        model.py:334-344), in construction order; empty without sn."""
+        de = self.cfg["Decoder"]
+        if not de.get("sn", False):
+            return []
+        n = de["n_conv_blocks"]
+        return (["decoder.in_conv_layer"] + [f"decoder.first_conv_layers.{l}" for l in range(n)]
+                + [f"decoder.second_conv_layers.{l}" for l in range(n)] + self._affine_names() + ["decoder.out_conv_layer"])
+
+    def bind_spectral_norm(self, P, G=None):
+        """Point P[name + '.weight'] of every wrapped layer at its static W_bar buffer and G[name + '.weight'] at the
+        gradient of its weight_orig, so that the conv / linear code keeps reading '.weight'.  P must hold the layer's
+        weight_orig, weight_u and weight_v."""
+        bufs = self.__dict__.setdefault("_sn_wbar", {})
+        for n in self.sn_names():
+            w = P[n + ".weight_orig"]
+            if n not in bufs or bufs[n].shape != w.shape:
+                bufs[n] = torch.zeros_like(w)
+            P[n + ".weight"] = bufs[n]
+            if G is not None and n + ".weight_orig" in G:
+                G[n + ".weight"] = G[n + ".weight_orig"]
+        return P
+
+    def _sn_table(self, P, G):
+        """Device item table of avc_spectral_norm(_bwd), cached until a pointer moves (it must exist before a graph
+        capture).  The sigma and scratch buffers are the engine's own."""
+        names = self.sn_names()
+        ptrs = tuple((P[n + ".weight_orig"].data_ptr(), P[n + ".weight"].data_ptr(), P[n + ".weight_u"].data_ptr(),
+                      P[n + ".weight_v"].data_ptr(), G[n + ".weight_orig"].data_ptr() if G is not None else 0) for n in names)
+        tabs = self.__dict__.setdefault("_sn_tables", {})   # every table kept: a captured graph may read any of them
+        if ptrs in tabs:
+            return tabs[ptrs]
+        shapes = [(P[n + ".weight_orig"].shape[0], P[n + ".weight_orig"][0].numel()) for n in names]
+        sizes = [int(self.lib.avc_spectral_norm_scratch_floats(h, w)) for h, w in shapes]
+        if getattr(self, "_sn_sigma", None) is None or self._sn_sigma.numel() != len(names):
+            self._sn_sigma = torch.zeros(len(names), dtype=torch.float32, device=self.dev)
+        if getattr(self, "_sn_scratch", None) is None or self._sn_scratch.numel() < sum(sizes):
+            self._sn_scratch = self.empty(sum(sizes))
+        items = (L.SnItem * len(names))()
+        off = 0
+        for i, (n, (h, w), sz) in enumerate(zip(names, shapes, sizes)):
+            it = items[i]
+            it.weight, it.w_bar, it.u, it.v, grad = ptrs[i]
+            it.sigma = self._sn_sigma.data_ptr() + 4 * i
+            it.grad = grad or None
+            it.scratch_off, it.h, it.w = off, h, w
+            off += sz
+        raw = torch.frombuffer(bytearray(bytes(items)), dtype=torch.uint8).to(self.dev)
+        tab = (raw, len(names), max(h for h, _ in shapes), max(w for _, w in shapes))
+        tabs[ptrs] = tab
+        return tab
+
+    def spectral_norm(self, P, iterate: bool):
+        """W_bar = weight_orig / sigma for every wrapped layer (P bound by bind_spectral_norm); iterate: one power
+        iteration first, updating weight_u / weight_v in place (training mode), otherwise the stored ones (eval)."""
+        raw, n, max_h, max_w = self._sn_table(P, None)
+        self._ck(self.lib.avc_spectral_norm(raw.data_ptr(), n, max_h, max_w, L.SN_ITERATE if iterate else L.SN_FIXED,
+                                            self._sn_scratch.data_ptr(), self.stream), "spectral_norm")
+
+    def spectral_norm_bwd(self, P, G):
+        """Turn the W_bar gradients in G[name + '.weight_orig'] into weight_orig gradients, with the u, v and sigma of
+        the last spectral_norm call."""
+        raw, n, max_h, max_w = self._sn_table(P, G)
+        self._ck(self.lib.avc_spectral_norm_bwd(raw.data_ptr(), n, max_h, max_w, self._sn_scratch.data_ptr(), self.stream),
+                 "spectral_norm_bwd")
 
     # ------------------------------------------------------------------ one conv block
     def conv(self, P, name, xin: A4, *, stride=1, shuffle=False, norm=False, cond=None, relu=False,

@@ -84,8 +84,8 @@ class Inferencer(object):
 
     def _param_version(self):
         # in-place updates (optimizer steps, load_state_dict) bump a tensor's version counter: a captured graph reads
-        # the weight packs of the version it was captured with
-        return sum(int(p._version) for p in self.model.parameters())
+        # the weight packs of the version it was captured with; the spectral norm's u and v are buffers
+        return sum(int(p._version) for p in self.model.parameters()) + sum(int(b._version) for b in self.model.buffers())
 
     @torch.no_grad()
     def inference_ragged(self, xs, x_conds):

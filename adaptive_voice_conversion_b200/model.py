@@ -6,7 +6,7 @@ Drop-in for the reference's ``model.py`` classes used by its Solver / Inferencer
   * ``AE(config)`` with ``forward(x) -> (mu, log_sigma, emb, dec)``, ``inference(x, x_cond)``
     and ``get_speaker_embeddings(x)``;
   * identical constructor kwargs (the keys of config.yaml) and an identical ``state_dict``:
-    166 fp32 tensors named ``speaker_encoder.conv_bank.0.weight`` ... with nn.Conv1d
+    166 fp32 tensors (218 with the decoder's spectral norm, ``Decoder.sn``) named ``speaker_encoder.conv_bank.0.weight`` ... with nn.Conv1d
     ``[Cout, Cin, k]`` / nn.Linear ``[out, in]`` shapes, so reference checkpoints load both
     ways.  nn.Conv1d / nn.Linear modules are kept purely as *parameter containers* (names,
     shapes, default init); their ``forward`` is never called.
@@ -37,11 +37,11 @@ class _ParamStack(nn.Module):
     """Base: a bag of nn.Conv1d / nn.Linear parameter holders registered under the
     reference's attribute names."""
 
-    def _convs(self, attr: str, specs):
-        setattr(self, attr, nn.ModuleList([nn.Conv1d(ci, co, kernel_size=k, stride=s) for (ci, co, k, s) in specs]))
+    def _convs(self, attr: str, specs, f=lambda m: m):
+        setattr(self, attr, nn.ModuleList([f(nn.Conv1d(ci, co, kernel_size=k, stride=s)) for (ci, co, k, s) in specs]))
 
-    def _linears(self, attr: str, specs):
-        setattr(self, attr, nn.ModuleList([nn.Linear(i, o) for (i, o) in specs]))
+    def _linears(self, attr: str, specs, f=lambda m: m):
+        setattr(self, attr, nn.ModuleList([f(nn.Linear(i, o)) for (i, o) in specs]))
 
     def forward(self, *a, **k):  # pragma: no cover
         raise L.AvcError("sub-stacks are parameter containers; call AE.forward / AE.inference / AE.get_speaker_embeddings")
@@ -79,17 +79,23 @@ class ContentEncoder(_ParamStack):
 
 
 class Decoder(_ParamStack):
-    """Parameters of the reference Decoder (model.py:325-345)."""
+    """Parameters of the reference Decoder (model.py:325-345).
+
+    sn=True wraps every layer in ``torch.nn.utils.spectral_norm`` as the reference does, in its order: the state_dict
+    then holds ``weight_orig`` / ``weight_u`` / ``weight_v`` (with the ``spectral_norm`` metadata), ``parameters()``
+    lists ``bias`` before ``weight_orig``, and u and v are drawn from the global generator right after each layer's
+    init.  The hook torch installs is never run (the containers' forward is not called): ``Engine.spectral_norm``
+    computes W / sigma on the device."""
 
     def __init__(self, c_in, c_cond, c_h, c_out, kernel_size, n_conv_blocks, upsample, act, sn, dropout_rate):
         super().__init__()
-        if sn:
-            raise L.AvcError("spectral norm (sn=True) is not implemented; the reference config uses sn: False")
-        self.in_conv_layer = nn.Conv1d(c_in, c_h, kernel_size=1)
-        self._convs("first_conv_layers", [(c_h, c_h, kernel_size, 1)] * n_conv_blocks)
-        self._convs("second_conv_layers", [(c_h, c_h * up, kernel_size, 1) for _, up in zip(range(n_conv_blocks), upsample)])
-        self._linears("conv_affine_layers", [(c_cond, c_h * 2)] * (2 * n_conv_blocks))
-        self.out_conv_layer = nn.Conv1d(c_h, c_out, kernel_size=1)
+        self.sn = bool(sn)
+        f = nn.utils.spectral_norm if sn else (lambda m: m)
+        self.in_conv_layer = f(nn.Conv1d(c_in, c_h, kernel_size=1))
+        self._convs("first_conv_layers", [(c_h, c_h, kernel_size, 1)] * n_conv_blocks, f)
+        self._convs("second_conv_layers", [(c_h, c_h * up, kernel_size, 1) for _, up in zip(range(n_conv_blocks), upsample)], f)
+        self._linears("conv_affine_layers", [(c_cond, c_h * 2)] * (2 * n_conv_blocks), f)
+        self.out_conv_layer = f(nn.Conv1d(c_h, c_out, kernel_size=1))
 
 
 def _check_input(x: torch.Tensor, what: str) -> torch.Tensor:
@@ -109,6 +115,11 @@ class _StackFn(torch.autograd.Function):
         names = model._names_by_prefix[prefix]
         P = dict(zip(names, params))
         eng = model.engine(params[0].device)
+        if prefix == "decoder." and model.decoder.sn:
+            # torch's spectral_norm: one power iteration per forward in training mode (also under no_grad), none in eval
+            P.update((n, b) for n, b in model.named_buffers() if n.startswith(prefix))
+            eng.bind_spectral_norm(P)
+            eng.spectral_norm(P, iterate=model.training)
         eng.pack_weights(P, need_dgrad=train, prefixes=(prefix,))
         ctx.model, ctx.prefix, ctx.P, ctx.train = model, prefix, P, train
         return eng, P
@@ -186,7 +197,12 @@ class _DecoderFn(_StackFn):
         B, Cc, T = ddec.shape
         ddec4 = A4.empty(B, Cc, T, ddec.device)
         eng.pack_a4(ddec.contiguous(), ddec4)
+        sn = ctx.model.decoder.sn
+        if sn:
+            eng.bind_spectral_norm(ctx.P, G)
         dz4, demb = eng.decoder_bwd(ctx.P, G, ctx.saved, ddec4)
+        if sn:
+            eng.spectral_norm_bwd(ctx.P, G)
         dmu4, dls4 = eng.reparam_bwd(dz4, ctx.ls4, ctx.eps, None, None)
         dmu, dls = eng.unpack_a4(dmu4), eng.unpack_a4(dls4)
         ctx.saved = None

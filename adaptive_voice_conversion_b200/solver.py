@@ -125,9 +125,11 @@ class Solver(object):
     # ---- model + optimizer (solver.py:70-79)
     def build_model(self):
         self.model = cc(AE(self.config))
-        if self.world > 1:  # replicas start identical: broadcast rank 0's init
+        if self.world > 1:  # replicas start identical: broadcast rank 0's init (and the spectral norm's u, v)
             for p in self.model.parameters():
                 torch.distributed.broadcast(p.data, src=0)
+            for b in self.model.buffers():
+                torch.distributed.broadcast(b, src=0)
         self.model.flatten_parameters()
         o = self.config["optimizer"]
         self.opt = FusedAdam(self.model, lr=o["lr"], betas=(o["beta1"], o["beta2"]), amsgrad=o["amsgrad"],

@@ -29,6 +29,9 @@ from .engine import A4, Engine
 from .optim import FusedAdam
 
 
+_ENCODERS = ("speaker_encoder.", "content_encoder.")
+
+
 class FusedTrainer:
     def __init__(self, model, opt: FusedAdam, config: dict, process_group=None):
         self.model, self.opt, self.cfg = model, opt, config
@@ -37,6 +40,12 @@ class FusedTrainer:
         self.lib = L.load()
         self.P: Dict[str, torch.Tensor] = dict(model.named_parameters())
         self.G: Dict[str, torch.Tensor] = opt.named_grad_views(model)
+        # Decoder.sn: the engine reads P[name + ".weight"] = W_bar (recomputed at the start of every forward) and writes
+        # G[name + ".weight"] = the weight_orig slot, which the backward correction turns into the weight_orig gradient
+        self.sn = bool(self.eng.sn_names())
+        if self.sn:
+            self.P.update(model.named_buffers())
+            self.eng.bind_spectral_norm(self.P, self.G)
         self.pg = process_group
         self.world = opt.world_size
         # one 16-byte report block so that reading a step's scalars is ONE device->host copy:
@@ -55,7 +64,11 @@ class FusedTrainer:
         self.auto_graph = os.environ.get("AVC_GRAPH", "1") == "1"
         self._eager_shape, self._eager_n = None, 0
         self.launches_per_step = 0
-        self.eng.pack_weights(self.P, need_dgrad=True)
+        if self.sn:   # the two partial packs a step makes: their tables must exist before a graph capture
+            self.eng.pack_weights(self.P, need_dgrad=True, prefixes=("decoder.",))
+            self.eng.pack_weights(self.P, need_dgrad=True, prefixes=_ENCODERS)
+        else:
+            self.eng.pack_weights(self.P, need_dgrad=True)
         self.eng.prepare_tables(self.P, self.G)   # before any CUDA-graph capture
         self.eng.prepare_wgrad_acc(self.P, self.G)
         self.overlap = os.environ.get("AVC_OVERLAP", "1") == "1"
@@ -86,9 +99,11 @@ class FusedTrainer:
         if side is not None:
             side.wait_stream(main)
             with torch.cuda.stream(side):
+                self._sn_fwd()   # beside the content encoder; decoder_affine_fwd is the first reader of W_bar
                 emb, cs = eng.speaker_fwd(P, x, True)
                 aff = eng.decoder_affine_fwd(P, emb, True)   # the AdaIN rows need the speaker embedding only
         else:
+            self._sn_fwd()
             emb, cs = eng.speaker_fwd(P, x, True)
             aff = None
         mu4, ls4, ce = eng.content_fwd(P, x, True)
@@ -108,10 +123,19 @@ class FusedTrainer:
         eng.pack_a4(ddec, ddec4)
         eng.wgrad_stream = self._wgs
         try:
-            return self._bwd(x, eps, mu, ls, emb, dec, ls4, dmu, dls, cs, ce, cd, ddec4)
+            outs = self._bwd(x, eps, mu, ls, emb, dec, ls4, dmu, dls, cs, ce, cd, ddec4)
         finally:
             eng.wgrad_stream = None
             eng._wg_keep.clear()
+        if self.sn:   # every decoder gradient producer has joined; before the all-reduce and the norm
+            eng.spectral_norm_bwd(P, G)
+        return outs
+
+    def _sn_fwd(self):
+        """Decoder.sn: one power iteration, W_bar = weight_orig / sigma, and the re-pack of the decoder's convs."""
+        if self.sn:
+            self.eng.spectral_norm(self.P, iterate=True)
+            self.eng.pack_weights(self.P, need_dgrad=True, prefixes=("decoder.",))
 
     def _bwd(self, x, eps, mu, ls, emb, dec, ls4, dmu, dls, cs, ce, cd, ddec4):
         eng, P, G = self.eng, self.P, self.G
@@ -147,7 +171,8 @@ class FusedTrainer:
 
     def _update(self):
         self.opt.step()
-        self.eng.pack_weights(self.P, need_dgrad=True)
+        # with sn the decoder's packs are made from W_bar at the start of the next forward
+        self.eng.pack_weights(self.P, need_dgrad=True, prefixes=_ENCODERS if self.sn else None)
 
     def set_lambda_kl(self, lambda_kl: float):
         """Push lambda_kl and the optimizer's param_group hyper-parameters (an lr scheduler may have changed

@@ -488,6 +488,38 @@ int avc_mel_moments(const avc_moments_desc* d, void* stream);
 int avc_mel_moments_merge(const double* moments, const int32_t* counts, int32_t n_utts, int32_t n_mels, float* mean,
                           float* std, double* mean64, double* std64, void* stream);
 
+/* ---- Spectral norm of the decoder weights (csrc/spectral_norm.cu): torch.nn.utils.spectral_norm with
+ * n_power_iterations=1, eps=1e-12, dim=0, for a DEVICE-resident table of n layers.  W = weight viewed as [h][w]
+ * (nn.Conv1d: h = Cout, w = Cin*K; nn.Linear: [out][in]); normalize(x) = x / max(||x||, eps).
+ *   AVC_SN_ITERATE (training mode): v = normalize(W^T u), u = normalize(W v) (both written back),
+ *                                   sigma = u . (W v), w_bar = W / sigma.
+ *   AVC_SN_FIXED   (eval mode):     sigma = u . (W v) with the stored u and v, w_bar = W / sigma.
+ * avc_spectral_norm_bwd: grad <- (grad - <grad, w_bar> u v^T) / sigma, in place, with the u, v, sigma and w_bar of
+ * the forward (the gradient of weight_orig when grad held the gradient of w_bar).
+ * Every reduction runs in a fixed order without atomics: repeated calls give the same bits, and an item's result does
+ * not depend on the other items of the launch.  scratch: each item owns avc_spectral_norm_scratch_floats(h, w) floats
+ * from scratch + scratch_off; the regions must not overlap.  Every item must have 1 <= h <= max_h and 1 <= w <= max_w
+ * (an item outside them is left untouched).  AVC_ERR_INVALID for null pointers, n < 1 or an unknown mode;
+ * AVC_ERR_UNSUPPORTED for n > AVC_SN_MAX_ITEMS, max_h > AVC_SN_MAX_H or max_w > AVC_SN_MAX_W. */
+#define AVC_SN_ITERATE 0
+#define AVC_SN_FIXED 1
+#define AVC_SN_MAX_ITEMS 64
+#define AVC_SN_MAX_H 4096
+#define AVC_SN_MAX_W 4096
+typedef struct avc_sn_item {
+  const float* weight;  /* weight_orig [h][w] */
+  float* w_bar;         /* weight_orig / sigma, same layout */
+  float* u;             /* [h] (weight_u) */
+  float* v;             /* [w] (weight_v) */
+  float* sigma;         /* [1] */
+  float* grad;          /* [h][w], avc_spectral_norm_bwd only */
+  int64_t scratch_off;  /* floats */
+  int32_t h, w;
+} avc_sn_item;
+int64_t avc_spectral_norm_scratch_floats(int h, int w);
+int avc_spectral_norm(const avc_sn_item* items, int n, int max_h, int max_w, int mode, float* scratch, void* stream);
+int avc_spectral_norm_bwd(const avc_sn_item* items, int n, int max_h, int max_w, float* scratch, void* stream);
+
 /* wgmma self-test (one CTA): D[128][N] = sum_k A_k * B_k^T over nk K=8 tf32 steps, the
  * operands given as raw shared-memory images; strides[10] = {a_lbo, a_sbo, b_lbo, b_sbo,
  * a_kstep, b_kstep, a_off, b_off (bytes), a_layout, b_layout (must be 0: no swizzle)}; a_mn/b_mn must be 0
