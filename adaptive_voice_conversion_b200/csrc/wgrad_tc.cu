@@ -30,7 +30,6 @@ constexpr int WG_ROWS = 32;        // reduction rows (time steps) per pipeline s
 constexpr int WG_A_BYTES = (WG_ROWS / 4) * 128 * 16;   // dc planes of one stage
 constexpr int WG_MAX_STAGES = 8;
 constexpr int WG_SMEM_MAX = 224 * 1024;
-constexpr int WG_THREADS = 384;    // warpgroup 0 stages the operands, warpgroups 1 and 2 issue the MMAs for co rows 0-63 / 64-127
 
 struct WgTcArgs {
   avc_wgrad_desc d;
@@ -98,13 +97,22 @@ __device__ __forceinline__ void wgrad_job_store(uint8_t* stage, const WgJob& J) 
   }
 }
 
+// Staging warpgroups per CTA.  A staging thread issues all loads of its jobs of a chunk, then stores them: the chunk's
+// global-load latency is exposed once per chunk and sets the pace (the tensor cores idle most of the time).  With two
+// staging warpgroups, each takes every other chunk, so two chunks' loads are in flight at once.  512 threads leave 128
+// registers per thread, enough for the N / 2 <= 80 accumulators and the 5 jobs per thread of K <= 5; K >= 6 keeps one
+// staging warpgroup and 168 registers per thread for its up to 128 accumulators.
+__host__ __device__ constexpr int wg_stagers(int K) { return K <= 5 ? 2 : 1; }
+__host__ __device__ constexpr int wg_threads(int K) { return 128 * (wg_stagers(K) + 2); }
+
 // Weight gradient of one (ci tile, co tile, batch slice).  mbarrier ring over the slice's row chunks: full[s] = the four
-// staging warps wrote stage s, empty[s] = both consumer warpgroups' MMAs on stage s retired.  A consumer queues the MMAs of
-// stage i, then wait_group 1 retires those of stage i - 1 and releases it; every CTA accumulates its rows in a fixed order.
-// 168 registers per thread (the __launch_bounds__ cap of 384 threads) hold the N / 2 <= 128 accumulators without a
-// register split between the roles.
+// warps of the staging warpgroup that owns the chunk wrote stage s, empty[s] = both consumer warpgroups' MMAs on stage s
+// retired.  A consumer queues the MMAs of stage i, then wait_group 1 retires those of stage i - 1 and releases it; every
+// CTA accumulates its rows in a fixed order.  No register split between the roles: the __launch_bounds__ cap (168
+// registers at 384 threads, 128 at 512) holds each instance's accumulators.
 template <int K, bool ATOMIC>
-__global__ void __launch_bounds__(WG_THREADS, 1) conv_wgrad_wgmma_kernel(const WgTcArgs a) {
+__global__ void __launch_bounds__(wg_threads(K), 1) conv_wgrad_wgmma_kernel(const WgTcArgs a) {
+  constexpr int STAGERS = wg_stagers(K);
   constexpr int N = K * WT_NT;
   constexpr uint32_t B_PLANE = N * 16;
   extern __shared__ __align__(1024) uint8_t smem[];
@@ -125,33 +133,35 @@ __global__ void __launch_bounds__(WG_THREADS, 1) conv_wgrad_wgmma_kernel(const W
   }
   __syncthreads();
 
-  if (warp < 4) {
-    // ================================================================ staging warpgroup
+  if (warp < 4 * STAGERS) {
+    // ================================================================ staging warpgroups
     // The global loads are the latency the staging has to hide: every load of a thread's JPT jobs of a stage is issued
-    // before the first store, and before the wait for the stage to be free.
+    // before the first store, and before the wait for the stage to be free.  Staging warpgroup g owns the chunks
+    // ch = g (mod STAGERS).  The parity wait on empty[s] cannot alias an older phase: before chunk ch this warpgroup
+    // waited for the release of chunk ch - STAGERS - nstage, and releases come in chunk order (nstage >= 4).
     constexpr int NJOBS = 256 + 64 * K, JPT = (NJOBS + 127) / 128;
-    int s = 0;
-    uint32_t ph = 0;
-    for (int ch = 0; ch < nchunk; ++ch) {
+    const int stid = tid & 127;
+    for (int ch = warp >> 2; ch < nchunk; ch += STAGERS) {
+      const int s = ch % a.nstage;
+      const uint32_t ph = (uint32_t)(ch / a.nstage) & 1u;
       WgJob J[JPT];
 #pragma unroll
       for (int q = 0; q < JPT; ++q)
-        if (tid + 128 * q < NJOBS) J[q] = wgrad_job_load<K>(a, tid + 128 * q, ch, b0, R);
+        if (stid + 128 * q < NJOBS) J[q] = wgrad_job_load<K>(a, stid + 128 * q, ch, b0, R);
       if (ch >= a.nstage && !__all_sync(0xffffffffu, tc::mbar_wait(&bar_empty[s], ph ^ 1u, a.status, 5))) return;
       uint8_t* stage = smem + (size_t)s * stage_bytes;
 #pragma unroll
       for (int q = 0; q < JPT; ++q)
-        if (tid + 128 * q < NJOBS) wgrad_job_store(stage, J[q]);
+        if (stid + 128 * q < NJOBS) wgrad_job_store(stage, J[q]);
       tc::fence_proxy_async_smem();   // the generic-proxy stores, before the async proxy (wgmma) reads them
       __syncwarp();
       if (lane == 0) tc::mbar_arrive(&bar_full[s]);
-      if (++s == a.nstage) { s = 0; ph ^= 1u; }
     }
     return;
   }
 
   // ================================================================ MMA warpgroups
-  const int wg = (warp >> 2) - 1, wt = tid & 127;
+  const int wg = (warp >> 2) - STAGERS, wt = tid & 127;
   float acc[N / 2];
 #pragma unroll
   for (int i = 0; i < N / 2; ++i) acc[i] = 0.f;
@@ -324,7 +334,7 @@ static int wgrad_wgmma_launch(const WgTcArgs& a, cudaStream_t stream, const char
   }
   const dim3 grid(cdiv(a.d.Cin, WT_NT), cdiv(a.d.Cout, 128), a.nslices);
   const int smem = a.nstage * (WG_A_BYTES + 8 * 16 * WT_NT * K);
-  AVC_LAUNCH((conv_wgrad_wgmma_kernel<K, ATOMIC>), grid, WG_THREADS, smem, stream, a);
+  AVC_LAUNCH((conv_wgrad_wgmma_kernel<K, ATOMIC>), grid, wg_threads(K), smem, stream, a);
   AVC_CHECK_LAUNCH(who);
   return AVC_OK;
 }
