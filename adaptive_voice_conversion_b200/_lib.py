@@ -152,6 +152,11 @@ class GatherDesc(C.Structure):
                 ("batch", C.c_int32), ("seg", C.c_int32), ("frame", C.c_int32), ("n_mels", C.c_int32)]
 
 
+class EvalDesc(C.Structure):
+    _fields_ = [("B", C.c_int32), ("C", C.c_int32), ("T", C.c_int32), ("C_lat", C.c_int32), ("T_lat", C.c_int32),
+                ("reserved", C.c_int32), ("dec", _fp), ("x", _fp), ("mu", _fp), ("ls", _fp), ("out", _fp), ("first", C.c_int64)]
+
+
 PCM_S16, PCM_F32 = 0, 1
 RESAMPLE_TILE, RESAMPLE_MAX_TAPS, RESAMPLE_MAX_PHASE_TAPS = 512, 8192, 96
 
@@ -222,6 +227,7 @@ PROTOTYPES = {
     "avc_adam_step": (_i, [_p, _p, _p, _p, _p, _i64, _p, _p, _p, _p]),
     "avc_fill_zero": (_i, [_p, _i64, _p]),
     "avc_segment_gather": (_i, [C.POINTER(GatherDesc), _p]),
+    "avc_eval_losses": (_i, [C.POINTER(EvalDesc), _p]),
     "avc_stft": (_i, [C.POINTER(AudioDesc), _p]),
     "avc_istft": (_i, [C.POINTER(AudioDesc), _p]),
     "avc_griffin_lim": (_i, [C.POINTER(AudioDesc), _p]),

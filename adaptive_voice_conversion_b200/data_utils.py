@@ -237,12 +237,17 @@ class DeviceSegments:
         L.check(self.lib.avc_segment_gather(d, stream.cuda_stream), "avc_segment_gather")
         return x
 
-    def __next__(self) -> torch.Tensor:
-        epoch, first, count = self.sampler.step()
-        if epoch != self._epoch:     # once per epoch: draw the order on the host, upload it (int32, 4 bytes per entry)
+    def load_epoch(self, epoch: int):
+        """Make `epoch`'s order the one gather() reads: drawn on the host and uploaded (int32, 4 bytes per entry) once
+        per epoch."""
+        if epoch != self._epoch:
             host = self.sampler.order(epoch).to(torch.int32).pin_memory()
             self._order = host.to(self.dev, non_blocking=True)
             self._epoch = epoch
+
+    def __next__(self) -> torch.Tensor:
+        epoch, first, count = self.sampler.step()
+        self.load_epoch(epoch)
         return self.gather(first, count)
 
 

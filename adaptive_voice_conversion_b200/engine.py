@@ -912,6 +912,35 @@ class Engine:
                                           dmu4.ptr, dls4.ptr, B, Cc, T, self.stream), "reparam_bwd")
         return dmu4, dls4
 
+    # ------------------------------------------------------------------ held-out evaluation
+    def prepare_eval(self, P):
+        """Eval-mode weights for eval_losses: W_bar from the stored u and v (Decoder.sn, no power iteration) and the
+        forward packs of every conv.  Writes into the existing W_bar and pack buffers only (pack_weights' buf() keeps a
+        slot of the right size): a captured training graph still reads the buffers it was recorded with, and its next
+        forward recomputes W_bar and the decoder's packs anyway."""
+        if self.sn_names():
+            self.spectral_norm(P, iterate=False)
+        self.pack_weights(P, need_dgrad=False)
+
+    def eval_losses(self, P, x_planar: torch.Tensor, out: torch.Tensor, first: int) -> A4:
+        """The conversion path on a batch x [B, C, T] -- AE.inference(x, x): content mean, the speaker of the same
+        segment, no noise -- with the same kernels, then out[first + b] = (sum |dec_b - x_b|, sum exp(ls_b) + mu_b^2 - 1 -
+        ls_b) in float64 (avc_eval_losses).  out: float64 [n_entries, 2] on this device.  Reads P as prepare_eval left
+        it; touches no RNG and no trainer state.  Returns dec (A4)."""
+        assert out.dtype == torch.float64 and out.is_contiguous() and out.dim() == 2 and out.shape[1] == 2
+        x_planar = x_planar.contiguous()
+        B, Cc, T = x_planar.shape
+        if first < 0 or first + B > out.shape[0]:
+            raise L.AvcError(f"eval_losses: rows [{first}, {first + B}) outside a table of {out.shape[0]}")
+        emb, _ = self.speaker_fwd(P, x_planar, False)
+        mu4, ls4, _ = self.content_fwd(P, x_planar, False)
+        dec4, _ = self.decoder_fwd(P, mu4, emb, False)
+        assert (dec4.C, dec4.T) == (Cc, T), ((dec4.C, dec4.T), (Cc, T))
+        d = L.EvalDesc(B=B, C=Cc, T=T, C_lat=mu4.C, T_lat=mu4.T, dec=dec4.ptr, x=x_planar.data_ptr(), mu=mu4.ptr, ls=ls4.ptr,
+                       out=out.data_ptr(), first=first)
+        self._ck(self.lib.avc_eval_losses(C.byref(d), self.stream), "eval_losses")
+        return dec4
+
     # ------------------------------------------------------------------ decoder
     def decoder_affine_fwd(self, P, emb: torch.Tensor, train: bool):
         """The 2*n AdaIN rows (beta|gamma) of every decoder block: conv_affine_layers (model.py:342-343, used :356,:363).

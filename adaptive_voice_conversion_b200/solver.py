@@ -21,6 +21,7 @@ import yaml
 
 from .data_utils import (DeviceSegments, PickleDataset, SyntheticSegments, corpus_device_bytes, device_corpus_fits,
                          get_data_loader, load_corpus)
+from .evaluate import HeldOut
 from .model import AE
 from .optim import FusedAdam
 from .trainer import FusedTrainer
@@ -47,7 +48,11 @@ class Solver(object):
             print(args)
         self.logger = Logger(getattr(args, "logdir", "log/")) if self.rank == 0 else None
         self.iteration = 0   # optimizer steps done so far (checkpointed: the KL-annealing position survives a resume)
+        self.train_device_bytes = 0   # device memory held by the training corpus
+        self.held_out = None
         self.get_data_loaders()
+        if getattr(args, "eval_steps", 0) > 0:   # load the held-out sets now: a bad file fails before any step
+            self.get_eval_sets()
         self.build_model()
         if self.rank == 0 and getattr(args, "store_model_path", None):
             self.save_config()
@@ -112,6 +117,7 @@ class Solver(object):
                       f"{'device-resident corpus' if on_device else 'host DataLoader'} ({nbytes / 1e9:.2f} GB on the device "
                       f"{'<=' if nbytes <= total_mem // 2 else '>'} half of its {total_mem / 1e9:.1f} GB)")
             if on_device:
+                self.train_device_bytes = nbytes
                 self.train_dataset = None
                 self.train_loader = DeviceSegments(data, indexes, dl["segment_size"], dl["frame_size"], dl["batch_size"],
                                                    self.config["ContentEncoder"]["c_in"], rank=self.rank, shuffle=dl["shuffle"])
@@ -121,6 +127,30 @@ class Solver(object):
                                                     shuffle=dl["shuffle"], num_workers=4, drop_last=False)
             del data, indexes
         self.train_iter = infinite_iter(self.train_loader)
+
+    def get_eval_sets(self):
+        """The held-out sets of -eval_sets (default in_test,out_test) from the data directory, kept on the device."""
+        sets = [s for s in getattr(self.args, "eval_sets", "in_test,out_test").split(",") if s]
+        self.held_out = HeldOut(sets, getattr(self.args, "data_dir", "synthetic"), self.config, rank=self.rank,
+                                world=self.world, reserved_bytes=self.train_device_bytes,
+                                total_memory=_device_total_memory(local_device()))
+
+    # ---- held-out evaluation (evaluate.py)
+    def evaluate(self, per_speaker=False):
+        """{set: {"loss_rec", "loss_kl", "n"}} of the current parameters on the held-out sets (evaluate.HeldOut).
+        Collective under data parallelism: every rank calls it."""
+        if self.held_out is None:
+            self.get_eval_sets()
+        return self.held_out.evaluate(self.model, per_speaker=per_speaker)
+
+    def _log_eval(self, iteration, res):
+        tag = getattr(self.args, "tag", "init")
+        for s, r in res.items():
+            self.logger.scalars_summary(f"{tag}/eval_{s}", {"loss_rec": r["loss_rec"], "loss_kl": r["loss_kl"]}, iteration)
+        print(f"EVAL:[{iteration}], " + ", ".join(f"{s}: loss_rec={r['loss_rec']:.4f}, loss_kl={r['loss_kl']:.4f} (n={r['n']})"
+                                                  for s, r in res.items()))
+        with open(f"{self.args.store_model_path}.eval.jsonl", "a") as f:
+            f.write(json.dumps({"iteration": int(iteration), "sets": res}) + "\n")
 
     # ---- model + optimizer (solver.py:70-79)
     def build_model(self):
@@ -224,4 +254,22 @@ class Solver(object):
                 self.save_model(iteration=iteration)
                 print()
 
-        self.run_steps(n_iterations, lambda_of=lambda it: lam if it >= anneal else lam * (it + 1) / anneal, on_step=on_step)
+        lambda_of = lambda it: lam if it >= anneal else lam * (it + 1) / anneal   # noqa: E731
+        every = getattr(self.args, "eval_steps", 0)
+        if every <= 0:
+            self.run_steps(n_iterations, lambda_of=lambda_of, on_step=on_step)
+            return
+        # chunks that end at multiples of eval_steps and at the last iteration; run_steps drains its pipeline before it
+        # returns, so the evaluation after a chunk sees exactly the parameters after self.iteration optimizer steps
+        for end in eval_chunk_ends(self.iteration, last, every):
+            self.run_steps(end - self.iteration, lambda_of=lambda_of, on_step=on_step)
+            res = self.evaluate()
+            if self.rank == 0:
+                self._log_eval(self.iteration, res)
+
+
+def eval_chunk_ends(start: int, last: int, every: int):
+    """The iterations at which a run from `start` to `last` steps evaluates: every multiple of `every` after start, and
+    last."""
+    ends = list(range((start // every + 1) * every, last, every))
+    return ends + [last] if last > start else []

@@ -359,6 +359,24 @@ typedef struct avc_gather_desc {
 } avc_gather_desc;
 int avc_segment_gather(const avc_gather_desc* d, void* stream);
 
+/* ---- Held-out evaluation (csrc/eval.cu, evaluate.HeldOut): the per-segment sums of the conversion path's losses.
+ * For every sample b < B, in float64 (each term and each sum):
+ *   out[first + b][0] = sum_{c < C, t < T} |dec[b][c][t] - x[b][c][t]|
+ *   out[first + b][1] = sum_{c < C_lat, t < T_lat} (exp(ls) + mu^2 - 1 - ls)[b][c][t]
+ * dec, mu and ls are whole A4 tensors ([B][C/4][T][4], batch stride C*T), x is planar [B][C][T].  One CTA per sample
+ * adds in a fixed order without atomics: a sample's two sums have the same bits on every run and in any batch.
+ * AVC_ERR_INVALID for null pointers, non-positive sizes, C or C_lat not a multiple of 4, or first < 0. */
+typedef struct avc_eval_desc {
+  int32_t B, C, T, C_lat, T_lat, reserved;
+  const float* dec; /* A4 [B][C/4][T][4] */
+  const float* x;   /* planar [B][C][T] */
+  const float* mu;  /* A4 [B][C_lat/4][T_lat][4] */
+  const float* ls;  /* A4 [B][C_lat/4][T_lat][4] */
+  double* out;      /* [n_entries][2] */
+  int64_t first;    /* row of sample 0 in out */
+} avc_eval_desc;
+int avc_eval_losses(const avc_eval_desc* d, void* stream);
+
 /* ---- Vocoder DSP (csrc/audio.cu): the reference's librosa STFT / Griffin-Lim path
  * (preprocess/tacotron/utils.py get_spectrograms, melspectrogram2wav), fp32.
  *

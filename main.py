@@ -5,6 +5,10 @@
 
 Under ``torchrun --nproc-per-node N`` every rank trains on its own batches with one NCCL
 gradient all-reduce per step (data parallel).
+
+With ``-eval_steps k`` the run also evaluates the held-out sets of ``-eval_sets`` (default ``in_test,out_test``, as
+preprocess.py writes them into the data directory) after every k steps and at the end, and appends the results to
+``<store_model_path>.eval.jsonl`` (adaptive_voice_conversion_b200/evaluate.py).
 """
 import os
 from argparse import ArgumentParser
@@ -24,9 +28,11 @@ OPTIONS = [
     (("-store_model_path",), "model", str),
     (("-load_model_path",), "model", str),
     (("-tag", "-t"), "init", str),
+    (("-eval_sets",), "in_test,out_test", str),
     (("-summary_steps",), 100, int),
     (("-save_steps",), 5000, int),
     (("-iters",), 0, int),
+    (("-eval_steps",), 0, int),
 ]
 
 
