@@ -124,7 +124,7 @@ class LinearBatchDesc(C.Structure):
     ]
 
 
-STFT_MAG, STFT_COMPLEX, STFT_PROJECT = 0, 1, 2
+STFT_MAG, STFT_COMPLEX, STFT_PROJECT, STFT_PROJECT_FIRST = 0, 1, 2, 3
 MEL_TO_MAG, MAG_TO_MEL = 0, 1
 
 
@@ -137,8 +137,9 @@ class AudioDesc(C.Structure):
     _fields_ = [
         ("n_fft", C.c_int32), ("hop", C.c_int32), ("win", C.c_int32), ("n_seg", C.c_int32),
         ("n_frames", C.c_int32), ("n_samples", C.c_int32), ("mode", C.c_int32), ("n_iter", C.c_int32),
-        ("preemph", C.c_float), ("max_db", C.c_float), ("ref_db", C.c_float), ("reserved", C.c_int32),
+        ("preemph", C.c_float), ("max_db", C.c_float), ("ref_db", C.c_float), ("momentum", C.c_float),
         ("segs", _fp), ("y", _fp), ("mag", _fp), ("X", _fp), ("frames", _fp), ("mag_out", _fp), ("mag_db", _fp),
+        ("X_prev", _fp),
     ]
 
 

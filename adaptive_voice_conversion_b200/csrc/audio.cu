@@ -3,6 +3,8 @@
 // element is computed by one thread in a fixed order, so a ragged batch gives each utterance the bits it gets alone.
 #include <float.h>
 
+#include <cmath>
+
 #include "common.cuh"
 
 namespace avc {
@@ -103,6 +105,9 @@ __device__ __forceinline__ int reflect(int i, int L) {
 // ------------------------------------------------------------------ forward STFT
 // One frame per 128 threads: the windowed frame is read straight from the signal (reflect padding and pre-emphasis
 // applied on the fly), packed as z[n] = x[2n] + i x[2n+1], transformed, and split into the 1025 rfft bins.
+// MOMENTUM: the fast Griffin-Lim projection (X_prev set, mode PROJECT or PROJECT_FIRST).  It is its own instance so
+// that the other epilogues keep their 32 registers (4 CTAs per SM).
+template <bool MOMENTUM>
 __global__ void __launch_bounds__(FFT_THREADS) stft_kernel(avc_audio_desc d) {
   __shared__ float2 tab[NC];
   __shared__ float2 buf[FPB][NC];
@@ -135,6 +140,14 @@ __global__ void __launch_bounds__(FFT_THREADS) stft_kernel(avc_audio_desc d) {
   fft1024(z, tab, t);
   if (!live) return;
   const int64_t row = (int64_t)f * NBIN;
+  // fast Griffin-Lim: P, the previous iteration's E, is loaded one bin ahead of its use, so each load is in flight
+  // during a bin's shared-memory reads and arithmetic.  P is never read on the first iteration, where it holds
+  // whatever the caller's buffer held.
+  float2* P = reinterpret_cast<float2*>(d.X_prev) + row;
+  const bool read_p = MOMENTUM && d.mode == AVC_STFT_PROJECT;
+  const float c = d.momentum / (1.f + d.momentum);
+  float2 p = make_float2(0.f, 0.f);
+  if (read_p) p = P[t];
   for (int k = t; k <= NC; k += TPF) {
     const float2 zk = z[k & (NC - 1)], zr = z[(NC - k) & (NC - 1)];
     // Xe = (Z[k] + conj Z[N-k]) / 2, Xo = (Z[k] - conj Z[N-k]) / 2i, X[k] = Xe + W^k Xo
@@ -143,7 +156,13 @@ __global__ void __launch_bounds__(FFT_THREADS) stft_kernel(avc_audio_desc d) {
     const float2 w = k < NC ? tab[k] : make_float2(-1.f, 0.f);
     const float2 wx = cmul(w, xo);
     const float2 X = make_float2(xe.x + wx.x, xe.y + wx.y);
-    if (d.mode == AVC_STFT_COMPLEX) {
+    if (MOMENTUM) {  // A = E - c P, P = E, the next spectrum S * A / max(1e-8, |A|)
+      const float2 A = read_p ? make_float2(X.x - c * p.x, X.y - c * p.y) : X;
+      P[k] = X;
+      if (read_p && k + TPF <= NC) p = P[k + TPF];
+      const float s = __ldg(d.mag + row + k) / fmaxf(1e-8f, sqrtf(A.x * A.x + A.y * A.y));
+      reinterpret_cast<float2*>(d.X)[row + k] = make_float2(A.x * s, A.y * s);
+    } else if (d.mode == AVC_STFT_COMPLEX) {
       reinterpret_cast<float2*>(d.X)[row + k] = X;
     } else {
       const float a = sqrtf(X.x * X.x + X.y * X.y);
@@ -153,7 +172,7 @@ __global__ void __launch_bounds__(FFT_THREADS) stft_kernel(avc_audio_desc d) {
           const float db = 20.f * log10f(fmaxf(1e-5f, a));
           d.mag_db[row + k] = fminf(1.f, fmaxf(1e-8f, (db - d.ref_db + d.max_db) / d.max_db));
         }
-      } else {  // AVC_STFT_PROJECT: the next Griffin-Lim spectrum S * E / max(1e-8, |E|)
+      } else {  // AVC_STFT_PROJECT(_FIRST) without momentum: the next Griffin-Lim spectrum S * E / max(1e-8, |E|)
         const float s = __ldg(d.mag + row + k) / fmaxf(1e-8f, a);
         reinterpret_cast<float2*>(d.X)[row + k] = make_float2(X.x * s, X.y * s);
       }
@@ -365,9 +384,26 @@ int check_audio(const avc_audio_desc* d, const char* who) {
   return AVC_OK;
 }
 
+// The momentum of a projecting call.  X_prev is cleared when the momentum is 0, so the kernel takes the momentum
+// branch exactly when X_prev is set.
+int check_momentum(avc_audio_desc& d, const char* who) {
+  const float m = d.momentum;
+  AVC_REQUIRE(std::isfinite(m) && m >= 0.f && m < 1.f, AVC_ERR_INVALID, "%s: momentum must be in [0, 1) (got %g)", who,
+              (double)m);
+  if (m == 0.f) {
+    d.X_prev = nullptr;
+    return AVC_OK;
+  }
+  AVC_REQUIRE(d.X_prev != nullptr, AVC_ERR_INVALID, "%s: momentum > 0 needs X_prev", who);
+  const uintptr_t p = (uintptr_t)d.X_prev, x = (uintptr_t)d.X, bytes = (uintptr_t)d.n_frames * NBIN * sizeof(float2);
+  AVC_REQUIRE(p != x && (p + bytes <= x || x + bytes <= p), AVC_ERR_INVALID, "%s: X_prev overlaps X", who);
+  return AVC_OK;
+}
+
 int launch_stft(const avc_audio_desc& d, cudaStream_t st) {
   if (d.n_frames == 0) return AVC_OK;
-  stft_kernel<<<cdiv(d.n_frames, FPB), FFT_THREADS, 0, st>>>(d);
+  if (d.X_prev != nullptr) stft_kernel<true><<<cdiv(d.n_frames, FPB), FFT_THREADS, 0, st>>>(d);
+  else stft_kernel<false><<<cdiv(d.n_frames, FPB), FFT_THREADS, 0, st>>>(d);
   AVC_CHECK_LAUNCH("avc_stft");
   return AVC_OK;
 }
@@ -392,15 +428,22 @@ using namespace avc;
 extern "C" int avc_stft(const avc_audio_desc* d, void* stream) {
   if (int rc = check_audio(d, "avc_stft")) return rc;
   AVC_REQUIRE(d->y != nullptr, AVC_ERR_INVALID, "avc_stft: null signal");
-  AVC_REQUIRE(d->mode == AVC_STFT_MAG || d->mode == AVC_STFT_COMPLEX || d->mode == AVC_STFT_PROJECT, AVC_ERR_INVALID,
+  const bool project = d->mode == AVC_STFT_PROJECT || d->mode == AVC_STFT_PROJECT_FIRST;
+  AVC_REQUIRE(d->mode == AVC_STFT_MAG || d->mode == AVC_STFT_COMPLEX || project, AVC_ERR_INVALID,
               "avc_stft: unknown mode %d", d->mode);
   AVC_REQUIRE(d->mode != AVC_STFT_MAG || d->mag_out != nullptr || d->mag_db != nullptr, AVC_ERR_INVALID,
               "avc_stft: MAG needs mag_out or mag_db");
   AVC_REQUIRE(d->mode == AVC_STFT_MAG || d->X != nullptr, AVC_ERR_INVALID, "avc_stft: null X");
-  AVC_REQUIRE(d->mode != AVC_STFT_PROJECT || d->mag != nullptr, AVC_ERR_INVALID, "avc_stft: PROJECT needs mag");
+  AVC_REQUIRE(!project || d->mag != nullptr, AVC_ERR_INVALID, "avc_stft: PROJECT needs mag");
   AVC_REQUIRE(d->mode != AVC_STFT_MAG || d->mag_db == nullptr || d->max_db > 0.f, AVC_ERR_INVALID,
               "avc_stft: max_db must be positive");
-  return launch_stft(*d, (cudaStream_t)stream);
+  avc_audio_desc a = *d;
+  if (project) {
+    if (int rc = check_momentum(a, "avc_stft")) return rc;
+  } else {
+    a.X_prev = nullptr;
+  }
+  return launch_stft(a, (cudaStream_t)stream);
 }
 
 extern "C" int avc_istft(const avc_audio_desc* d, void* stream) {
@@ -417,13 +460,14 @@ extern "C" int avc_griffin_lim(const avc_audio_desc* d, void* stream) {
   AVC_REQUIRE(d->n_iter >= 0, AVC_ERR_INVALID, "avc_griffin_lim: n_iter < 0");
   cudaStream_t st = (cudaStream_t)stream;
   avc_audio_desc a = *d;
+  if (int rc = check_momentum(a, "avc_griffin_lim")) return rc;
   a.preemph = 0.f;
-  a.mode = AVC_STFT_PROJECT;
   for (int it = 0; it <= a.n_iter; ++it) {
     avc_audio_desc s = a;
     if (it == 0) s.X = nullptr;  // X = S with zero phase
     if (int rc = launch_istft(s, st)) return rc;
     if (it == a.n_iter) break;
+    a.mode = it == 0 ? AVC_STFT_PROJECT_FIRST : AVC_STFT_PROJECT;  // the same projection when X_prev is null
     if (int rc = launch_stft(a, st)) return rc;
   }
   return AVC_OK;

@@ -36,6 +36,7 @@ class AudioParams:
     win_length: int = 1200
     n_mels: int = 512
     n_iter: int = 100
+    momentum: float = 0.0      # fast Griffin-Lim momentum in [0, 1); 0 is the reference's plain Griffin-Lim
     preemphasis: float = 0.97
     max_db: float = 100.0
     ref_db: float = 20.0
@@ -225,9 +226,16 @@ def istft(specs, hp: AudioParams = AudioParams()):
 
 class GriffinLim:
     """One ragged Griffin-Lim call with its buffers.  ``run()`` enqueues the whole loop (3 n_iter + 2 launches) on
-    the current stream, so it can be captured into a CUDA graph; ``outputs()`` are views of the signal buffer."""
+    the current stream, so it can be captured into a CUDA graph; ``outputs()`` are views of the signal buffer.
 
-    def __init__(self, mags, hp: AudioParams = AudioParams(), n_iter: int | None = None):
+    ``momentum`` m > 0 (default ``hp.momentum``) runs fast Griffin-Lim (Perraudin, Balazs & Sondergaard 2013) in the
+    form of librosa's and torchaudio's ``momentum``: each projection uses A = E - m/(1+m) P, P the previous iteration's
+    spectrum E, and P takes a second complex buffer the size of X.  The start is zero-phase (librosa's init=None).
+    Where librosa divides by |A| + tiny, this divides by max(1e-8, |A|); the two differ only where |A| < 1e-8.
+    A momentum that is not finite or outside [0, 1) raises ``AvcError`` from ``run()``."""
+
+    def __init__(self, mags, hp: AudioParams = AudioParams(), n_iter: int | None = None,
+                 momentum: float | None = None):
         _frames(mags, hp, "griffin_lim")
         self.dev = mags[0].device
         self.S = torch.cat([m.float() for m in mags]).contiguous()
@@ -238,8 +246,10 @@ class GriffinLim:
         self.X = torch.empty(n_frames, hp.n_bins, 2, device=self.dev)
         self.frames = torch.empty(n_frames, hp.win_length, device=self.dev)
         self.y = torch.empty(int(self.r.sample_offs[-1]), device=self.dev)
-        self.desc = self.r.desc(hp, n_iter=hp.n_iter if n_iter is None else n_iter, mag=self.S, X=self.X,
-                                frames=self.frames, y=self.y)
+        m = float(hp.momentum if momentum is None else momentum)
+        self.X_prev = torch.empty_like(self.X) if m > 0 else None
+        self.desc = self.r.desc(hp, n_iter=hp.n_iter if n_iter is None else n_iter, momentum=m, mag=self.S, X=self.X,
+                                frames=self.frames, y=self.y, X_prev=self.X_prev)
 
     def run(self):
         _call("avc_griffin_lim", self.desc, self.dev)
@@ -249,9 +259,10 @@ class GriffinLim:
         return self.r.split_samples(self.y)
 
 
-def griffin_lim(mags, hp: AudioParams = AudioParams(), n_iter: int | None = None):
-    """Griffin-Lim from linear magnitudes [T, n_bins]; signals of hop * (T - 1) samples (untrimmed)."""
-    return GriffinLim(mags, hp, n_iter).run().outputs()
+def griffin_lim(mags, hp: AudioParams = AudioParams(), n_iter: int | None = None, momentum: float | None = None):
+    """Griffin-Lim from linear magnitudes [T, n_bins]; signals of hop * (T - 1) samples (untrimmed).  ``momentum``
+    (default ``hp.momentum``) as in ``GriffinLim``."""
+    return GriffinLim(mags, hp, n_iter, momentum).run().outputs()
 
 
 def deemphasis(wavs, coef: float = 0.97):
@@ -343,15 +354,15 @@ class Vocoder:
         r = [m.shape[0] for m in mels]
         return list(torch.split(_mel_project(torch.cat(mels), self.m_t, L.MEL_TO_MAG, self.hp), r))
 
-    def mel_to_wav(self, mels, n_iter: int | None = None):
+    def mel_to_wav(self, mels, n_iter: int | None = None, momentum: float | None = None):
         """Normalised mels [T, n_mels] (device tensors) -> float32 signals: amplitude, mel-to-linear, Griffin-Lim,
-        de-emphasis, trim (out_top_db)."""
+        de-emphasis, trim (out_top_db).  ``n_iter`` and ``momentum`` default to ``hp.n_iter`` and ``hp.momentum``."""
         hp = self.hp
         for i, m in enumerate(mels):
             if m.dim() != 2 or m.shape[1] != hp.n_mels:
                 raise ValueError(f"mel_to_wav: utterance {i} has shape {tuple(m.shape)}, expected [T, {hp.n_mels}]")
         _frames(mels, hp, "mel_to_wav")
-        ys = deemphasis(griffin_lim(self.mel_to_mag(mels), hp, n_iter), hp.preemphasis)
+        ys = deemphasis(griffin_lim(self.mel_to_mag(mels), hp, n_iter, momentum), hp.preemphasis)
         return trim(ys, hp.out_top_db)
 
     def get_spectrograms(self, path):

@@ -395,7 +395,10 @@ typedef struct avc_audio_seg {
 
 #define AVC_STFT_MAG 0     /* mag_out = |X| and / or mag_db = clip((20 log10(max(1e-5,|X|)) - ref_db + max_db) / max_db, 1e-8, 1) */
 #define AVC_STFT_COMPLEX 1 /* X = the half spectrum */
-#define AVC_STFT_PROJECT 2 /* X = mag * E / max(1e-8, |E|), E the half spectrum: one Griffin-Lim projection */
+#define AVC_STFT_PROJECT 2 /* X = mag * A / max(1e-8, |A|), E the half spectrum: one Griffin-Lim projection.
+                              momentum 0: A = E.  momentum m > 0 (fast Griffin-Lim): A = E - m/(1+m) * X_prev,
+                              then X_prev = E */
+#define AVC_STFT_PROJECT_FIRST 3 /* as PROJECT for the first iteration: A = E, X_prev is written but not read */
 
 typedef struct avc_audio_desc {
   int32_t n_fft, hop, win;
@@ -406,7 +409,7 @@ typedef struct avc_audio_desc {
   int32_t n_iter;    /* avc_griffin_lim */
   float preemph;     /* avc_stft: y'[n] = y[n] - preemph * y[n-1] applied on the fly (0: none) */
   float max_db, ref_db; /* avc_stft MAG with mag_db */
-  int32_t reserved;
+  float momentum;    /* avc_griffin_lim / avc_stft PROJECT: fast Griffin-Lim momentum m in [0, 1) (0: plain) */
   const avc_audio_seg* segs; /* DEVICE table */
   float* y;          /* signal: avc_stft / avc_frame_power input, avc_istft / avc_griffin_lim output, avc_deemphasis in place */
   const float* mag;  /* [n_frames][n_fft/2+1]: target magnitude S of PROJECT / avc_griffin_lim; avc_istft input when X is null */
@@ -415,6 +418,8 @@ typedef struct avc_audio_desc {
   float* frames;     /* [n_frames][win] workspace of avc_istft / avc_griffin_lim: windowed inverse frames */
   float* mag_out;    /* avc_stft MAG: [n_frames][n_fft/2+1] or null */
   float* mag_db;     /* avc_stft MAG: [n_frames][n_fft/2+1] or null */
+  float* X_prev;     /* [n_frames][n_fft/2+1] complex: the previous iteration's spectrum E when momentum > 0 (must not
+                        overlap X); ignored when momentum is 0 */
 } avc_audio_desc;
 
 /* STFT (center, reflect padding) of every utterance: one launch. */
@@ -424,7 +429,11 @@ int avc_stft(const avc_audio_desc* d, void* stream);
  * Two launches. */
 int avc_istft(const avc_audio_desc* d, void* stream);
 /* Griffin-Lim: X = mag (zero phase); n_iter x { X = mag * E / max(1e-8, |E|), E = stft(istft(X)) }; y = istft(X).
- * 3 n_iter + 2 launches (iSTFT frames, overlap-add, projecting STFT per iteration). */
+ * 3 n_iter + 2 launches (iSTFT frames, overlap-add, projecting STFT per iteration).
+ * momentum m > 0: fast Griffin-Lim (Perraudin, Balazs & Sondergaard 2013, librosa's form), c = m / (1 + m):
+ * n_iter x { E = stft(istft(X)); A = E - c P (A = E the first time); P = E; X = mag * A / max(1e-8, |A|) }, with P in
+ * X_prev; same launches.  AVC_ERR_INVALID before any launch when m is not finite or outside [0, 1), or when m > 0 and
+ * X_prev is null or overlaps X.  m = 0 ignores X_prev. */
 int avc_griffin_lim(const avc_audio_desc* d, void* stream);
 /* power[frame] = mean of y^2 over frames of n_fft samples hop apart, reflect-padded by n_fft/2 (librosa's trim
  * statistic): segs frame_off / n_frames count these frames, 1 + n_samples / hop per utterance.  Any even n_fft. */
