@@ -65,22 +65,31 @@ __global__ void __launch_bounds__(256) norm_apply_fwd_kernel(const avc_conv_desc
     s = warp_sum4(s);
     const float inv = 1.f / (float)Tn;
     mean[0] = s.x * inv; mean[1] = s.y * inv; mean[2] = s.z * inv; mean[3] = s.w * inv;
-    float4 m2 = zero4();
+    // corrected two-pass: the deviations also sum to the rounding error of the first pass's mean, which is removed
+    // from the mean and the variance.  Without it a channel that is constant over time (rstd = eps^-1/2) normalises
+    // to (c - mean) * 316 instead of 0.
+    float4 m1 = zero4(), m2 = zero4();
     for (int t = lane; t < d.Tout; t += 32) {
       float v[2][4];
       load_rows<SHUF>(cb, qn, d.Tout, t, v);
 #pragma unroll
       for (int sx = 0; sx < NS; ++sx) {
         float e;
-        e = v[sx][0] - mean[0]; m2.x += e * e;
-        e = v[sx][1] - mean[1]; m2.y += e * e;
-        e = v[sx][2] - mean[2]; m2.z += e * e;
-        e = v[sx][3] - mean[3]; m2.w += e * e;
+        e = v[sx][0] - mean[0]; m1.x += e; m2.x += e * e;
+        e = v[sx][1] - mean[1]; m1.y += e; m2.y += e * e;
+        e = v[sx][2] - mean[2]; m1.z += e; m2.z += e * e;
+        e = v[sx][3] - mean[3]; m1.w += e; m2.w += e * e;
       }
     }
+    m1 = warp_sum4(m1);
     m2 = warp_sum4(m2);
-    rstd[0] = rsqrtf(m2.x * inv + d.eps); rstd[1] = rsqrtf(m2.y * inv + d.eps);
-    rstd[2] = rsqrtf(m2.z * inv + d.eps); rstd[3] = rsqrtf(m2.w * inv + d.eps);
+    const float s1[4] = {m1.x, m1.y, m1.z, m1.w}, s2[4] = {m2.x, m2.y, m2.z, m2.w};
+#pragma unroll
+    for (int c = 0; c < 4; ++c) {
+      const float dm = s1[c] * inv;
+      mean[c] += dm;
+      rstd[c] = rsqrtf(fmaxf(s2[c] * inv - dm * dm, 0.f) + d.eps);
+    }
     if (d.stats && lane == 0) {
 #pragma unroll
       for (int c = 0; c < 4; ++c) {
