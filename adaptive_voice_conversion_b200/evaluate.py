@@ -1,5 +1,6 @@
 """Held-out evaluation: the reconstruction and KL losses of the conversion path on the sets preprocess.py writes
-(``in_test``: seen speakers, unseen utterances; ``out_test``: unseen speakers).
+(``in_test``: seen speakers, unseen utterances; ``out_test``: unseen speakers), or preprocess_libri.py (``dev``: held
+out of the training subset; ``test``: the test subset).
 
 For a set S (``<S>.pkl`` and its index ``<S>_samples_<segment_size>.json``) every index entry i is cut into a segment
 x_i exactly as ``DeviceSegments`` cuts a training batch, and
@@ -38,7 +39,8 @@ def rank_batches(n: int, batch_size: int, rank: int = 0, world: int = 1) -> List
 
 
 def speaker_of(utt_id: str) -> str:
-    """The speaker of a VCTK utterance id: everything up to its first '_' (p225_001 -> p225)."""
+    """The speaker of an utterance id: everything up to its first '_'.  VCTK: p225_001.wav -> p225; LibriTTS
+    (<speaker>_<chapter>_<paragraph>_<sentence>.wav): 103_1241_000000_000001.wav -> 103."""
     return str(utt_id).split("_", 1)[0]
 
 

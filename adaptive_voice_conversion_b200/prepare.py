@@ -1,5 +1,6 @@
-"""Training corpus preparation from a VCTK 0.80 wav tree: the reference's preprocess_vctk.sh (make_datasets_vctk.py,
-reduce_dataset.py, sample_single_segments.py) without librosa or tensorflow, with the signal work on the GPU.
+"""Training corpus preparation from a VCTK 0.80 or a LibriTTS wav tree: the reference's preprocess_vctk.sh
+(make_datasets_vctk.py, reduce_dataset.py, sample_single_segments.py) and preprocess_libri.sh (make_datasets_libri.py
+and the same two scripts) without librosa or tensorflow, with the signal work on the GPU.
 
 The split, the file order, the output formats and the index sampling are the reference's.  Its one unseeded source of
 randomness, the module-level ``random``, is a ``random.Random(seed)`` here, used in the reference's call order: the
@@ -7,7 +8,10 @@ split is exactly what the reference produces after ``random.seed(seed)``.  The f
 one respect only: files not at ``sample_rate`` are resampled with scipy.signal.resample_poly's filter (on the GPU,
 csrc/prep.cu), where librosa used resampy.
 
-Each set is processed in sorted path order, in chunks of at most ``chunk_seconds`` of output audio.  Per chunk: the
+Each set is processed in the reference's order for its corpus: VCTK sets in sorted path order; LibriTTS's train and
+dev sets in their shuffled split order and its test set sorted.  The pickles' key order is that order, and attr.pkl
+covers the first ``n_utts_attr`` training utterances in it.  Processing runs in chunks of at most ``chunk_seconds`` of
+output audio.  Per chunk: the
 files' PCM is decoded on the host as stored, packed into one pinned buffer and copied to the device once; one
 ``avc_resample_poly`` launch per (rate pair, sample format); the silence trim's frame powers find the files too short
 for the STFT; ``Vocoder.wav_to_mel`` analyses the untrimmed signals of the others (it trims them itself); the mels are
@@ -35,6 +39,7 @@ from . import _lib as L
 from . import vocoder as V
 
 SETS = ("train", "in_test", "out_test")
+LIBRI_SETS = ("train", "dev", "test")
 RAGGED_MAX = 2 ** 31 - 1     # vocoder._Ragged: samples and frames of one ragged batch
 _NAME = re.compile(r"p(\d+)_(\d+)\.wav")
 SILENCE_POWER = 1e-10      # librosa's amin of the trim's power_to_db: -100 dB
@@ -80,6 +85,36 @@ def split_files(speaker_ids, speaker2filenames, n_out_speakers, test_prop, seed)
     for speaker in ids[-n_out_speakers:]:
         out_test += speaker2filenames.get(speaker, [])
     return train, in_test, out_test
+
+
+# ------------------------------------------------------------------ file list and split (make_datasets_libri.py)
+def read_libri_paths(root, subset):
+    """Sorted <root>/<subset>/*/*/*.wav: speaker / chapter / file, exactly three levels down.  The transcripts beside
+    the wavs, and wavs at any other depth, are not listed."""
+    return sorted(glob.glob(os.path.join(root, subset, "*/*/*.wav")))
+
+
+def split_libri(train_paths, test_paths, test_prop, seed):
+    """(train, dev, test) path lists in processing order.  The training subset's listing is shuffled once and its last
+    int(len * test_prop) paths are dev; test is the test subset's listing as given (sorted).  Where the reference
+    would go on with an empty train set (int(len * test_prop) == 0 makes paths[:-0] empty) this raises ValueError."""
+    paths = list(train_paths)
+    random.Random(seed).shuffle(paths)
+    n = int(len(paths) * test_prop)
+    if n == 0:
+        raise ValueError(f"test_prop = {test_prop} of {len(paths)} training files gives no dev file, and the "
+                         "reference's split would leave the training set empty")
+    return paths[:-n], paths[-n:], list(test_paths)
+
+
+def check_basenames(name, paths):
+    """A set's pickle is keyed by file name, so two files of one set with the same name would silently keep one."""
+    seen = {}
+    for p in paths:
+        b = os.path.basename(p)
+        if b in seen:
+            raise ValueError(f"the {name} set holds two files named {b}: {seen[b]} and {p}")
+        seen[b] = p
 
 
 # ------------------------------------------------------------------ reduce and index sampling
@@ -330,6 +365,52 @@ def _load(path):
         return pickle.load(f)
 
 
+def _features(sets, out_dir, cache, n_mels, sample_rate, n_utts_attr, chunk_seconds, device, timer, log):
+    """Stage 0's features: each set of `sets` ({name: paths in processing order}, "train" first) analysed in that
+    order; attr.pkl over the first n_utts_attr analysed training utterances; every set normalised by it and pickled
+    (and kept in `cache`); the skipped files in skipped_files.txt."""
+    prep = Preparer(n_mels, sample_rate, device, timer)
+    chunk = max(1, int(chunk_seconds * sample_rate))
+    skipped, mean = [], None
+    for name, paths in sets.items():
+        log(f"processing {name} set, {len(paths)} files")
+        raw, skip, attr = prep.process(paths, chunk, n_utts_attr if name == "train" else 0)
+        skipped += skip
+        if name == "train":
+            if attr is None:
+                raise ValueError("no training utterance could be analysed: attr.pkl cannot be computed")
+            mean, std = attr[0], attr[1]
+            with timer.host("pickle"):
+                _dump({"mean": mean, "std": std}, os.path.join(out_dir, "attr.pkl"))
+        with timer.host("pickle"):
+            cache[name] = normalise(raw, mean, std)
+            del raw
+            _dump(cache[name], os.path.join(out_dir, f"{name}.pkl"))
+    with open(os.path.join(out_dir, "skipped_files.txt"), "w") as f:
+        f.writelines(f"{p}\t{why}\n" for p, why in skipped)
+    log(f"{len(skipped)} files skipped (listed in skipped_files.txt)")
+
+
+def _reduce_and_index(out_dir, cache, test_sets, segment_size, training_samples, testing_samples, seed, stage, timer):
+    """Stages 1-3: train_<seg>.pkl, train_samples_<seg>.json and <set>_samples_<seg>.json for each of `test_sets`,
+    from the sets in `cache` or, when stage 0 did not run, from their pickles."""
+    def load_set(name):
+        if name not in cache:
+            cache[name] = _load(os.path.join(out_dir, f"{name}.pkl"))
+        return cache[name]
+
+    with timer.host("reduce_and_index"):
+        if stage <= 1:
+            _dump(reduce_set(load_set("train"), segment_size), os.path.join(out_dir, f"train_{segment_size}.pkl"))
+        if stage <= 2:
+            with open(os.path.join(out_dir, f"train_samples_{segment_size}.json"), "w") as f:
+                json.dump(sample_segments(load_set("train"), training_samples, segment_size, seed), f)
+        if stage <= 3:
+            for name in test_sets:
+                with open(os.path.join(out_dir, f"{name}_samples_{segment_size}.json"), "w") as f:
+                    json.dump(sample_segments(load_set(name), testing_samples, segment_size, seed), f)
+
+
 # ------------------------------------------------------------------ the whole preprocess_vctk.sh
 def run(wav_dir, speaker_info, out_dir, n_out_speakers=20, test_prop=0.1, sample_rate=24000, n_utts_attr=5000,
         n_mels=512, segment_size=128, training_samples=10000000, testing_samples=10000, seed=0, stage=0,
@@ -338,12 +419,6 @@ def run(wav_dir, speaker_info, out_dir, n_out_speakers=20, test_prop=0.1, sample
     os.makedirs(out_dir, exist_ok=True)
     timer = timer or _NoTimer()
     cache = {}
-
-    def load_set(name):
-        if name not in cache:
-            cache[name] = _load(os.path.join(out_dir, f"{name}.pkl"))
-        return cache[name]
-
     if stage <= 0:
         if n_utts_attr < 1:
             raise ValueError("n_utts_attr must be >= 1")
@@ -352,34 +427,38 @@ def run(wav_dir, speaker_info, out_dir, n_out_speakers=20, test_prop=0.1, sample
         for name in ("in_test", "out_test"):
             with open(os.path.join(out_dir, f"{name}_files.txt"), "w") as f:
                 f.writelines(f"{p}\n" for p in sets[name])
-        prep = Preparer(n_mels, sample_rate, device, timer)
-        chunk = max(1, int(chunk_seconds * sample_rate))
-        skipped, mean = [], None
-        for name in SETS:
-            paths = sorted(sets[name])
-            log(f"processing {name} set, {len(paths)} files")
-            raw, skip, attr = prep.process(paths, chunk, n_utts_attr if name == "train" else 0)
-            skipped += skip
-            if name == "train":
-                if attr is None:
-                    raise ValueError("no training utterance could be analysed: attr.pkl cannot be computed")
-                mean, std = attr[0], attr[1]
-                with timer.host("pickle"):
-                    _dump({"mean": mean, "std": std}, os.path.join(out_dir, "attr.pkl"))
-            with timer.host("pickle"):
-                cache[name] = normalise(raw, mean, std)
-                del raw
-                _dump(cache[name], os.path.join(out_dir, f"{name}.pkl"))
-        with open(os.path.join(out_dir, "skipped_files.txt"), "w") as f:
-            f.writelines(f"{p}\t{why}\n" for p, why in skipped)
-        log(f"{len(skipped)} files skipped (listed in skipped_files.txt)")
-    with timer.host("reduce_and_index"):
-        if stage <= 1:
-            _dump(reduce_set(load_set("train"), segment_size), os.path.join(out_dir, f"train_{segment_size}.pkl"))
-        if stage <= 2:
-            with open(os.path.join(out_dir, f"train_samples_{segment_size}.json"), "w") as f:
-                json.dump(sample_segments(load_set("train"), training_samples, segment_size, seed), f)
-        if stage <= 3:
-            for name in ("in_test", "out_test"):
-                with open(os.path.join(out_dir, f"{name}_samples_{segment_size}.json"), "w") as f:
-                    json.dump(sample_segments(load_set(name), testing_samples, segment_size, seed), f)
+        _features({name: sorted(sets[name]) for name in SETS}, out_dir, cache, n_mels, sample_rate, n_utts_attr,
+                  chunk_seconds, device, timer, log)
+    _reduce_and_index(out_dir, cache, ("in_test", "out_test"), segment_size, training_samples, testing_samples, seed,
+                      stage, timer)
+
+
+# ------------------------------------------------------------------ the whole preprocess_libri.sh
+def run_libri(root, out_dir, train_set="train-clean-100", test_set="dev-clean", test_prop=0.05, sample_rate=24000,
+              n_utts_attr=5000, n_mels=512, segment_size=128, training_samples=10000000, testing_samples=10000, seed=0,
+              stage=0, chunk_seconds=1800.0, device=None, timer=None, log=print):
+    """Stages as preprocess_libri.sh: 0 = split and features, 1 = reduce, 2 = train index, 3 = dev and test indexes.
+
+    train and dev are processed in their shuffled split order, test in sorted order, so attr.pkl covers the first
+    n_utts_attr analysed utterances of the *shuffled* training list (VCTK's covers its sorted list).  The file lists
+    hold the sorted basenames of each set."""
+    os.makedirs(out_dir, exist_ok=True)
+    timer = timer or _NoTimer()
+    cache = {}
+    if stage <= 0:
+        if n_utts_attr < 1:
+            raise ValueError("n_utts_attr must be >= 1")
+        listings = {s: read_libri_paths(root, s) for s in (train_set, test_set)}
+        for s, paths in listings.items():
+            if not paths:
+                raise ValueError(f"no {os.path.join(root, s, '*/*/*.wav')} files")
+        sets = dict(zip(LIBRI_SETS, split_libri(listings[train_set], listings[test_set], test_prop, seed)))
+        for name, paths in sets.items():
+            check_basenames(name, paths)
+        log(f"{len(sets['train'])} training data, {len(sets['dev'])} dev data, {len(sets['test'])} test data")
+        for name, paths in sets.items():
+            with open(os.path.join(out_dir, f"{name}_files.txt"), "w") as f:
+                f.writelines(f"{os.path.basename(p)}\n" for p in sorted(paths))
+        _features(sets, out_dir, cache, n_mels, sample_rate, n_utts_attr, chunk_seconds, device, timer, log)
+    _reduce_and_index(out_dir, cache, ("dev", "test"), segment_size, training_samples, testing_samples, seed, stage,
+                      timer)

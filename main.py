@@ -7,7 +7,8 @@ Under ``torchrun --nproc-per-node N`` every rank trains on its own batches with 
 gradient all-reduce per step (data parallel).
 
 With ``-eval_steps k`` the run also evaluates the held-out sets of ``-eval_sets`` (default ``in_test,out_test``, as
-preprocess.py writes them into the data directory) after every k steps and at the end, and appends the results to
+preprocess.py writes them into the data directory; ``dev,test`` for preprocess_libri.py's) after every k steps and at
+the end, and appends the results to
 ``<store_model_path>.eval.jsonl`` (adaptive_voice_conversion_b200/evaluate.py).
 """
 import os

@@ -1,18 +1,23 @@
-"""Corpus preparation throughput: preprocess.py's pipeline on a seeded synthetic VCTK-shaped corpus, stage by stage,
-against today's single-file path (Vocoder.get_spectrograms per file: host resample_poly, then GPU analysis).
+"""Corpus preparation throughput: preprocess.py's (or preprocess_libri.py's) pipeline on a seeded synthetic corpus,
+stage by stage, against today's single-file path (Vocoder.get_spectrograms per file: host resample_poly, then GPU
+analysis).
 
-    python tools/bench_prepare.py [--utts 2000] [--speakers 40] [--n_mels 512] [--chunk_seconds 1800] [--out DIR]
+    python tools/bench_prepare.py [--corpus vctk|libri] [--utts 2000] [--speakers 40] [--n_mels 512]
+        [--chunk_seconds 1800] [--out DIR]
 
-The corpus is 48 kHz int16 mono, 2-5 s of tone and noise between leading and trailing silence per file, written to a
-temporary directory (deleted afterwards).  Host stages are wall-clock; device stages are CUDA events around their
-launches, summed over chunks.  End to end is one preprocess.py run (all four stages); stage 0 is that run less
-the timed stages 1-3 (reduce, index sampling).  "headers" is the first pass over the files (their lengths, for the
-chunk planner); "decode" is the full read of each chunk's files.  avc_resample_poly's traffic is 2 bytes read per input sample and 4 written per output
-sample (plus its tap table and the staged windows' overlap, not counted).  The card's name, power limit and clock are
-read in the same run.
+--corpus vctk (default): VCTK-shaped, 48 kHz int16 mono, so the resampler halves the rate.  --corpus libri:
+LibriTTS-shaped (train-clean-100 and dev-clean, speaker / chapter / file, a tenth of the speakers in dev-clean), 24 kHz
+int16 mono, so the resampler only converts the format.  Each file is 2-5 s of tone and noise between leading and
+trailing silence, written to a temporary directory (deleted afterwards).  Host stages are wall-clock; device stages
+are CUDA events around their launches, summed over chunks.  End to end is one run of all four stages; stage 0 is that
+run less the timed stages 1-3 (reduce, index sampling).  "headers" is the first pass over the files (their lengths,
+for the chunk planner); "decode" is the full read of each chunk's files.  avc_resample_poly's traffic is 2 bytes read
+per input sample and 4 written per output sample (plus its tap table and the staged windows' overlap, not counted).
+The card's name, power limit and clock are read in the same run.
 """
 import argparse
 import contextlib
+import functools
 import json
 import os
 import shutil
@@ -57,6 +62,16 @@ class Timer:
         return {k: sum(a.elapsed_time(b) for a, b in v) / 1e3 for k, v in self.events.items()}
 
 
+def synth_pcm(rng, sr):
+    n = int(sr * rng.uniform(2.0, 5.0))
+    t = np.arange(n) / sr
+    f0 = rng.uniform(100, 250)
+    y = sum(rng.uniform(0.05, 0.2) / k * np.sin(2 * np.pi * k * f0 * t + rng.uniform(0, 6.3)) for k in range(1, 5))
+    y += 0.02 * rng.standard_normal(n)
+    y = np.concatenate([np.zeros(int(0.3 * sr)), y, np.zeros(int(0.4 * sr))])
+    return np.round(np.clip(y, -1, 1 - 2 ** -15) * 32768).astype(np.int16)
+
+
 def write_corpus(root, n_utts, n_speakers, seed):
     rng = np.random.default_rng(seed)
     wav = os.path.join(root, "wav48")
@@ -65,21 +80,33 @@ def write_corpus(root, n_utts, n_speakers, seed):
     for u in range(n_utts):
         spk = speakers[u % n_speakers]
         os.makedirs(os.path.join(wav, f"p{spk}"), exist_ok=True)
-        sr = 48000
-        n = int(sr * rng.uniform(2.0, 5.0))
-        t = np.arange(n) / sr
-        f0 = rng.uniform(100, 250)
-        y = sum(rng.uniform(0.05, 0.2) / k * np.sin(2 * np.pi * k * f0 * t + rng.uniform(0, 6.3)) for k in range(1, 5))
-        y += 0.02 * rng.standard_normal(n)
-        y = np.concatenate([np.zeros(int(0.3 * sr)), y, np.zeros(int(0.4 * sr))])
-        pcm = np.round(np.clip(y, -1, 1 - 2 ** -15) * 32768).astype(np.int16)
-        wavfile.write(os.path.join(wav, f"p{spk}", f"p{spk}_{u // n_speakers + 1:03d}.wav"), sr, pcm)
+        pcm = synth_pcm(rng, 48000)
+        wavfile.write(os.path.join(wav, f"p{spk}", f"p{spk}_{u // n_speakers + 1:03d}.wav"), 48000, pcm)
         n_in.append(pcm.size)
     info = os.path.join(root, "speaker-info.txt")
     with open(info, "w") as f:
         f.write("ID  AGE  GENDER  ACCENTS  REGION\n")
         f.writelines(f"{s}  23  F  English  Somewhere\n" for s in speakers)
     return wav, info, np.array(n_in, np.int64)
+
+
+def write_libri_corpus(root, n_utts, n_speakers, seed):
+    """<root>/LibriTTS/{train-clean-100,dev-clean}/<speaker>/<chapter>/<speaker>_<chapter>_<p>_<s>.wav, two chapters
+    per speaker, the last tenth of the speakers (at least one) in dev-clean."""
+    rng = np.random.default_rng(seed)
+    libri = os.path.join(root, "LibriTTS")
+    speakers = [str(100 + 7 * i) for i in range(n_speakers)]
+    n_dev = max(1, n_speakers // 10)
+    n_in = []
+    for u in range(n_utts):
+        i = u % n_speakers
+        spk, ch, k = speakers[i], str(1000 + 10 * i + (u // n_speakers) % 2), u // n_speakers
+        d = os.path.join(libri, "dev-clean" if i >= n_speakers - n_dev else "train-clean-100", spk, ch)
+        os.makedirs(d, exist_ok=True)
+        pcm = synth_pcm(rng, 24000)
+        wavfile.write(os.path.join(d, f"{spk}_{ch}_{k:06d}_{k + 1:06d}.wav"), 24000, pcm)
+        n_in.append(pcm.size)
+    return libri, np.array(n_in, np.int64)
 
 
 def card():
@@ -90,6 +117,7 @@ def card():
 
 def main():
     ap = argparse.ArgumentParser()
+    ap.add_argument("--corpus", choices=("vctk", "libri"), default="vctk")
     ap.add_argument("--utts", type=int, default=2000)
     ap.add_argument("--speakers", type=int, default=40)
     ap.add_argument("--n_mels", type=int, default=512)
@@ -99,23 +127,38 @@ def main():
     a = ap.parse_args()
     assert torch.cuda.is_available(), "bench_prepare needs a GPU"
     root = tempfile.mkdtemp(prefix="bench_prepare_")
+    opts = dict(n_mels=a.n_mels, n_utts_attr=5000, training_samples=100000, testing_samples=10000,
+                chunk_seconds=a.chunk_seconds, log=lambda *x: None)
+    if a.corpus == "vctk":
+        rate = 48000
+
+        def corpus(d, n_utts, n_speakers, seed):
+            wav, info, n_in = write_corpus(d, n_utts, n_speakers, seed)
+            paths = sorted(os.path.join(wav, s, f) for s in os.listdir(wav) for f in os.listdir(os.path.join(wav, s)))
+            prepare = functools.partial(P.run, wav, info, n_out_speakers=max(1, n_speakers // 10), **opts)
+            return prepare, paths, n_in
+    else:
+        rate = 24000
+
+        def corpus(d, n_utts, n_speakers, seed):
+            libri, n_in = write_libri_corpus(d, n_utts, n_speakers, seed)
+            paths = P.read_libri_paths(libri, "train-clean-100") + P.read_libri_paths(libri, "dev-clean")
+            return functools.partial(P.run_libri, libri, test_prop=0.05, **opts), paths, n_in
     try:
         t0 = time.perf_counter()
-        wav, info, n_in = write_corpus(root, a.utts, a.speakers, a.seed)
-        print(f"corpus: {a.utts} files, {n_in.sum() / 48000 / 3600:.2f} h at 48 kHz, written in "
+        prepare, paths, n_in = corpus(root, a.utts, a.speakers, a.seed)
+        print(f"corpus: {a.corpus}, {a.utts} files, {n_in.sum() / rate / 3600:.2f} h at {rate // 1000} kHz, written in "
               f"{time.perf_counter() - t0:.1f} s", flush=True)
-        opts = dict(n_out_speakers=max(1, a.speakers // 10), n_mels=a.n_mels, n_utts_attr=5000,
-                    training_samples=100000, testing_samples=10000, chunk_seconds=a.chunk_seconds, log=lambda *x: None)
         # warm-up: modules, tap tables and the allocator, on a small tree of its own
         warm = os.path.join(root, "warm")
-        wav_w, info_w, _ = write_corpus(warm, 40, 4, a.seed + 1)
-        P.run(wav_w, info_w, os.path.join(warm, "out"), **{**opts, "n_out_speakers": 1})
+        prepare_w, _, _ = corpus(warm, 40, 4, a.seed + 1)
+        prepare_w(os.path.join(warm, "out"))
         torch.cuda.synchronize()
 
-        # one preprocess.py run (stage 0 runs every stage, as the shell script's -le rule does)
+        # one preprocess run (stage 0 runs every stage, as the shell script's -le rule does)
         timer = Timer()
         t0 = time.perf_counter()
-        P.run(wav, info, os.path.join(root, "out"), stage=0, timer=timer, **opts)
+        prepare(os.path.join(root, "out"), stage=0, timer=timer)
         torch.cuda.synchronize()
         t_all = time.perf_counter() - t0
         t_index = timer.host_s["reduce_and_index"]
@@ -124,13 +167,12 @@ def main():
         dev = timer.device_s()
         skipped = open(os.path.join(root, "out", "skipped_files.txt")).read().count("\n")
 
-        n_out = -(-n_in // 2)
+        n_out = -(-n_in * 24000 // rate)
         rs_bytes = 2 * int(n_in.sum()) + 4 * int(n_out.sum())
-        audio_s = n_in.sum() / 48000
+        audio_s = n_in.sum() / rate
 
         # today's path: one file at a time through Vocoder.get_spectrograms
         voc = V.Vocoder(n_mels=a.n_mels)
-        paths = sorted(p for s in os.listdir(wav) for p in (os.path.join(wav, s, f) for f in os.listdir(os.path.join(wav, s))))
         voc.get_spectrograms(paths[0])
         torch.cuda.synchronize()
         t0 = time.perf_counter()
@@ -140,7 +182,7 @@ def main():
 
         res = {
             "card": card(),
-            "files": a.utts, "audio_hours": round(float(audio_s) / 3600, 3), "n_mels": a.n_mels,
+            "corpus": a.corpus, "files": a.utts, "audio_hours": round(float(audio_s) / 3600, 3), "n_mels": a.n_mels,
             "chunk_seconds": a.chunk_seconds, "skipped": skipped,
             "host_s": {k: round(v, 3) for k, v in timer.host_s.items()},
             "device_s": {k: round(v, 4) for k, v in dev.items()},
