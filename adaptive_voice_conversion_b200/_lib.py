@@ -178,6 +178,24 @@ class MomentsDesc(C.Structure):
                 ("moments", _fp)]
 
 
+CEPSTRUM_MAX_DIMS, CEPSTRUM_MAX_MELS, DTW_MAX_SHORT = 64, 4096, 4096
+
+
+class CepstrumDesc(C.Structure):
+    _fields_ = [("rows", C.c_int32), ("n_mels", C.c_int32), ("dims", C.c_int32), ("reserved", C.c_int32),
+                ("max_db", C.c_float), ("ref_db", C.c_float),
+                ("in_", _fp), ("mean", _fp), ("std", _fp), ("dct", _fp), ("out", _fp)]
+
+
+class DtwPair(C.Structure):
+    _fields_ = [("x_off", C.c_int64), ("y_off", C.c_int64), ("tx", C.c_int32), ("ty", C.c_int32)]
+
+
+class DtwDesc(C.Structure):
+    _fields_ = [("n_pairs", C.c_int32), ("dims", C.c_int32), ("max_short", C.c_int32), ("reserved", C.c_int32),
+                ("pairs", _fp), ("x", _fp), ("y", _fp), ("out", _fp)]
+
+
 SN_ITERATE, SN_FIXED = 0, 1
 SN_MAX_ITEMS, SN_MAX_H, SN_MAX_W = 64, 4096, 4096
 
@@ -238,6 +256,8 @@ PROTOTYPES = {
     "avc_resample_poly": (_i, [C.POINTER(ResampleDesc), _p]),
     "avc_mel_moments": (_i, [C.POINTER(MomentsDesc), _p]),
     "avc_mel_moments_merge": (_i, [_p, _p, C.c_int32, C.c_int32, _p, _p, _p, _p, _p]),
+    "avc_mel_cepstrum": (_i, [C.POINTER(CepstrumDesc), _p]),
+    "avc_dtw": (_i, [C.POINTER(DtwDesc), _p]),
     "avc_spectral_norm_scratch_floats": (_i64, [_i, _i]),
     "avc_spectral_norm": (_i, [_p, _i, _i, _i, _i, _p, _p]),
     "avc_spectral_norm_bwd": (_i, [_p, _i, _i, _i, _p, _p]),

@@ -2,11 +2,16 @@
 data directory (adaptive_voice_conversion_b200/evaluate.py gives the definition).
 
     python evaluate.py -c config.yaml -m model.ckpt -d data/ [-eval_sets in_test,out_test] [-o eval.json]
+                       [-mcd -transcripts VCTK-Corpus/txt [-attr data/attr.pkl] [-mcd_dims 24] [-max_pairs 0] [-seed 0]]
 
 The checkpoint is loaded strictly (reference checkpoints too, and the `sn: True` layout).  Each set's losses are
-printed; -o writes them with the per-speaker means as JSON.
+printed; -o writes them with the per-speaker means as JSON.  -mcd also measures conversion itself: the mel-cepstral
+distortion after DTW between speaker A's utterance converted to speaker B and B's recording of the same sentence
+(adaptive_voice_conversion_b200/mcd.py gives the definition), one more line per set and an "mcd" entry per set in -o.
 """
 import json
+import os
+import pickle
 from argparse import ArgumentParser
 
 import torch
@@ -24,7 +29,15 @@ def main(argv=None):
     p.add_argument("-data_dir", "-d", required=True, help="data directory written by preprocess.py")
     p.add_argument("-eval_sets", default="in_test,out_test", help="comma-separated set names (<set>.pkl)")
     p.add_argument("-output", "-o", default=None, help="JSON file for the per-set and per-speaker results")
+    p.add_argument("-mcd", action="store_true", help="also measure MCD-DTW of conversions on parallel utterances")
+    p.add_argument("-transcripts", default=None, help="directory searched for <id>.txt / <id>.normalized.txt (-mcd)")
+    p.add_argument("-attr", default=None, help="mel statistics (default <data_dir>/attr.pkl) (-mcd)")
+    p.add_argument("-mcd_dims", type=int, default=24, help="cepstral coefficients c_1..c_D (-mcd)")
+    p.add_argument("-max_pairs", type=int, default=0, help="keep at most this many triplets per set, 0 = all (-mcd)")
+    p.add_argument("-seed", type=int, default=0, help="seed of the reference choice and the sampling (-mcd)")
     args = p.parse_args(argv)
+    if args.mcd and not args.transcripts:
+        p.error("-mcd needs -transcripts DIR")
     config = load_config(args.config)
     dev = local_device()
     model = AE(config).to(dev)
@@ -34,6 +47,19 @@ def main(argv=None):
     res = held.evaluate(model, per_speaker=True)
     for s, r in res.items():
         print(f"{s}: n={r['n']} loss_rec={r['loss_rec']:.6f} loss_kl={r['loss_kl']:.6f} ({len(r['speakers'])} speakers)")
+    if args.mcd:
+        from adaptive_voice_conversion_b200.mcd import evaluate_mcd, read_transcripts
+        with open(args.attr or os.path.join(args.data_dir, "attr.pkl"), "rb") as f:
+            attr = pickle.load(f)
+        for s in res:
+            with open(os.path.join(args.data_dir, f"{s}.pkl"), "rb") as f:
+                data = pickle.load(f)
+            m = evaluate_mcd(model, data, attr, read_transcripts(args.transcripts, data), dims=args.mcd_dims,
+                             max_pairs=args.max_pairs, seed=args.seed, device=dev)
+            res[s]["mcd"] = m
+            means = f" mcd={m['mcd']:.4f} mcd_source={m['mcd_source']:.4f}" if m["n"] else ""
+            print(f"{s}: mcd n={m['n']} n_short={m['n_short']}{means} (dims {m['dims']}, "
+                  f"{len(m['speakers'])} target speakers)")
     if args.output:
         with open(args.output, "w") as f:
             json.dump(res, f, indent=1)

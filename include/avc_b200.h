@@ -515,6 +515,53 @@ int avc_mel_moments(const avc_moments_desc* d, void* stream);
 int avc_mel_moments_merge(const double* moments, const int32_t* counts, int32_t n_utts, int32_t n_mels, float* mean,
                           float* std, double* mean64, double* std64, void* stream);
 
+/* ---- Mel-cepstral distortion (csrc/mcd.cu, mcd.py).  No allocation, no synchronisation, no atomics.
+ *
+ * avc_mel_cepstrum: for every row r of a ragged batch of attr-normalised mel frames in[rows][n_mels], and k < dims:
+ *   a_m = clip(in[r][m] * std[m] + mean[m], 0, 1)           (float32, as the vocoder's AVC_MEL_TO_MAG input)
+ *   l_m = (a_m max_db - max_db + ref_db) ln(10) / 20         (float64: the natural-log amplitude)
+ *   out[r][k] = sum_m l_m dct[m][k]  (float64, ascending m; stored as float32)
+ * dct[n_mels][dims] is the orthonormal DCT-II without c_0, built by the caller: dct[m][k] =
+ * sqrt(2 / n_mels) cos(pi (k + 1) (2m + 1) / (2 n_mels)).  A row gets the same bits in any batch.
+ * AVC_ERR_INVALID for null pointers or non-positive sizes; AVC_ERR_UNSUPPORTED for dims > AVC_CEPSTRUM_MAX_DIMS or
+ * n_mels > AVC_CEPSTRUM_MAX_MELS.
+ *
+ * avc_dtw: for every pair p of a DEVICE table, X = x rows [x_off, x_off + tx), Y = y rows [y_off, y_off + ty) of two
+ * [rows][dims] float32 cepstrum buffers, in float64 with every operation rounded on its own (no fused multiply-add):
+ *   d(i,j) = sqrt(sum_k (X[i][k] - Y[j][k])^2)   (terms added in ascending k)
+ *   S(i,j) = d(i,j) + min(S(i-1,j-1), S(i-1,j), S(i,j-1)) over the predecessors that exist, ties preferring them in
+ *            that order;  L(i,j) = L(pred) + 1;  S(0,0) = d(0,0), L(0,0) = 1
+ *   out[p] = (S(tx-1, ty-1), L(tx-1, ty-1)).
+ * max_short must be at least min(tx, ty) of every pair: the launch sizes its shared memory by it.  A pair that breaks
+ * this, or has tx or ty < 1, is not computed: its out row is (NaN, 0).  A pair gets the same bits in any batch.
+ * AVC_ERR_INVALID for null pointers or non-positive sizes; AVC_ERR_UNSUPPORTED for dims > AVC_CEPSTRUM_MAX_DIMS or
+ * max_short > AVC_DTW_MAX_SHORT.  The kernel trusts the offsets (rows inside the buffers). */
+#define AVC_CEPSTRUM_MAX_DIMS 64
+#define AVC_CEPSTRUM_MAX_MELS 4096
+#define AVC_DTW_MAX_SHORT 4096
+typedef struct avc_cepstrum_desc {
+  int32_t rows, n_mels, dims, reserved;
+  float max_db, ref_db;
+  const float* in;     /* [rows][n_mels] */
+  const float* mean;   /* [n_mels] */
+  const float* std;    /* [n_mels] */
+  const double* dct;   /* [n_mels][dims] */
+  float* out;          /* [rows][dims] */
+} avc_cepstrum_desc;
+int avc_mel_cepstrum(const avc_cepstrum_desc* d, void* stream);
+typedef struct avc_dtw_pair {
+  int64_t x_off, y_off; /* first row of each sequence */
+  int32_t tx, ty;       /* rows of each sequence */
+} avc_dtw_pair;
+typedef struct avc_dtw_desc {
+  int32_t n_pairs, dims, max_short, reserved;
+  const avc_dtw_pair* pairs; /* DEVICE table [n_pairs] */
+  const float* x;            /* [rows][dims] */
+  const float* y;            /* [rows][dims] */
+  double* out;               /* [n_pairs][2] */
+} avc_dtw_desc;
+int avc_dtw(const avc_dtw_desc* d, void* stream);
+
 /* ---- Spectral norm of the decoder weights (csrc/spectral_norm.cu): torch.nn.utils.spectral_norm with
  * n_power_iterations=1, eps=1e-12, dim=0, for a DEVICE-resident table of n layers.  W = weight viewed as [h][w]
  * (nn.Conv1d: h = Cout, w = Cin*K; nn.Linear: [out][in]); normalize(x) = x / max(||x||, eps).
