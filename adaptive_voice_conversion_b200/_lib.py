@@ -63,6 +63,16 @@ class TcPlan(C.Structure):
         "stage_bytes", "smem_bytes", "smem_max", "instance")]
 
 
+class SimtPlan(C.Structure):
+    """avc_simt_plan: the tile plan of avc_conv_block_fwd for one descriptor (avc_conv_block_fwd_plan)."""
+    _fields_ = [(n, C.c_int32) for n in (
+        "TT", "TCO", "tiled", "seg_out", "nseg", "segp", "ntt", "grid_x", "grid_y", "xrow", "smem_bytes", "instance")]
+
+
+# avc_simt_plan.instance -> (K, stride, TCO, TT) of the conv_block_fwd_kernel instance
+SIMT_INSTANCES = [(k, 1, 128, 128) for k in range(1, 9)] + [(5, 2, 128, 128), (1, 1, 64, 256), (5, 1, 64, 256), (5, 2, 64, 256)]
+
+
 class WgradDesc(C.Structure):
     _fields_ = [
         ("B", C.c_int32), ("Cin", C.c_int32), ("Cout", C.c_int32), ("K", C.c_int32),
@@ -209,6 +219,7 @@ class SnItem(C.Structure):
 _i, _i64, _p = C.c_int, C.c_int64, C.c_void_p
 PROTOTYPES = {
     "avc_conv_block_fwd": (_i, [C.POINTER(ConvDesc), _p]),
+    "avc_conv_block_fwd_plan": (_i, [C.POINTER(ConvDesc), C.POINTER(SimtPlan)]),
     "avc_conv_block_tc": (_i, [C.POINTER(ConvDesc), _p, _p]),
     "avc_conv_block_tc_plan": (_i, [C.POINTER(ConvDesc), _i, C.POINTER(TcPlan)]),
     "avc_pack_conv_weight_tc": (_i, [_p, _p, _i, _i, _i, _i, _p]),

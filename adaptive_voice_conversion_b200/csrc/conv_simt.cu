@@ -327,6 +327,21 @@ static int next_pow2(int v) {
   return p;
 }
 
+// The fixed table of kernel instances; avc_simt_plan.instance indexes it.
+struct SimtInstance {
+  int K, S, TCO, TT, xrow, smem_bytes;
+  int (*launch)(const ConvArgs&, dim3, cudaStream_t);
+};
+#define SIMT_INST(KK, SS, TCO_, TT_) \
+  {KK, SS, TCO_, TT_, ConvCfg<KK, SS, TCO_, TT_>::XROW, ConvCfg<KK, SS, TCO_, TT_>::SMEM_BYTES, launch_conv<KK, SS, TCO_, TT_>}
+static const SimtInstance kSimtInstances[] = {
+    SIMT_INST(1, 1, 128, 128), SIMT_INST(2, 1, 128, 128), SIMT_INST(3, 1, 128, 128), SIMT_INST(4, 1, 128, 128),
+    SIMT_INST(5, 1, 128, 128), SIMT_INST(6, 1, 128, 128), SIMT_INST(7, 1, 128, 128), SIMT_INST(8, 1, 128, 128),
+    SIMT_INST(5, 2, 128, 128), SIMT_INST(1, 1, 64, 256),  SIMT_INST(5, 1, 64, 256),  SIMT_INST(5, 2, 64, 256),
+};
+#undef SIMT_INST
+constexpr int kNumSimtInstances = sizeof(kSimtInstances) / sizeof(kSimtInstances[0]);
+
 int validate_conv_desc(const avc_conv_desc* d, const char* who) {
   AVC_REQUIRE(d != nullptr, AVC_ERR_INVALID, "%s: null descriptor", who);
   AVC_REQUIRE(d->B > 0 && d->Cin > 0 && d->Cout > 0 && d->Tin > 0 && d->Tout > 0, AVC_ERR_INVALID,
@@ -337,11 +352,9 @@ int validate_conv_desc(const avc_conv_desc* d, const char* who) {
   return AVC_OK;
 }
 
-}  // namespace avc
-
-using namespace avc;
-
-extern "C" int avc_conv_block_fwd(const avc_conv_desc* d, void* stream) {
+// The argument checks and the tile plan of avc_conv_block_fwd, shared by the launch and the host-only plan query:
+// reads no pointer (only whether it is null), launches nothing.
+static int simt_plan(const avc_conv_desc* d, avc_simt_plan* p) {
   int rc = validate_conv_desc(d, "avc_conv_block_fwd");
   if (rc != AVC_OK) return rc;
   AVC_REQUIRE(d->in && d->w_packed && d->out, AVC_ERR_INVALID, "avc_conv_block_fwd: null in/w/out");
@@ -350,49 +363,75 @@ extern "C" int avc_conv_block_fwd(const avc_conv_desc* d, void* stream) {
               "avc_conv_block_fwd: stride %d with K=%d unsupported", d->stride, d->K);
   AVC_REQUIRE(d->w_ld % 4 == 0 && d->w_ld >= d->Cout, AVC_ERR_INVALID, "avc_conv_block_fwd: bad w_ld");
   AVC_REQUIRE(!d->res || d->res_mode != AVC_RES_NONE, AVC_ERR_INVALID, "avc_conv_block_fwd: res without res_mode");
-  cudaStream_t st = (cudaStream_t)stream;
+  // fields of the tensor-core kernel this one does not implement: refuse them rather than write a dense, unfolded
+  // output (AVC_F_IN_TF32 is only a hint and stays accepted)
+  AVC_REQUIRE(!(d->flags & (AVC_F_FOLD | AVC_F_NORMBWD)), AVC_ERR_UNSUPPORTED,
+              "avc_conv_block_fwd: AVC_F_FOLD / AVC_F_NORMBWD are avc_conv_block_tc only (flags 0x%x)", d->flags);
+  AVC_REQUIRE(d->out_tstride == 0 && d->out_toff == 0 && d->out_T == 0, AVC_ERR_UNSUPPORTED,
+              "avc_conv_block_fwd: out_tstride / out_toff / out_T are avc_conv_block_tc only (got %d, %d, %d)",
+              d->out_tstride, d->out_toff, d->out_T);
+  const int S = d->stride, K = d->K;
+  avc_simt_plan q;
+  q.ntt = 1;
+  q.tiled = 0;
+  if (d->Tout <= 128) {
+    q.TT = 128;
+    q.TCO = 128;
+    q.seg_out = next_pow2(d->Tout < 8 ? 8 : d->Tout);
+  } else if (d->norm && d->Tout <= 256 && (K == 1 || K == 5)) {
+    q.TT = 256;
+    q.TCO = 64;
+    q.seg_out = 256;
+  } else if (!d->norm) {
+    q.TT = 128;
+    q.TCO = 128;
+    q.tiled = 1;
+    q.seg_out = 128;
+    q.ntt = cdiv(d->Tout, q.TT);
+  } else {
+    set_error("avc_conv_block_fwd: fused InstanceNorm needs Tout <= 128, or <= 256 at K 1 or 5 (got Tout %d, K %d); "
+              "use avc_norm_apply_fwd", d->Tout, K);
+    return AVC_ERR_UNSUPPORTED;
+  }
+  q.nseg = q.TT / q.seg_out;
+  q.segp = ((q.seg_out * S + K - 1) + 3) / 4 * 4;
+  q.grid_x = q.tiled ? d->B * q.ntt : cdiv(d->B, q.nseg);
+  q.grid_y = cdiv(d->Cout, q.TCO);
+  q.instance = -1;
+  q.xrow = q.smem_bytes = 0;
+  for (int i = 0; i < kNumSimtInstances; ++i) {
+    const SimtInstance& in = kSimtInstances[i];
+    if (in.K == K && in.S == S && in.TCO == q.TCO && in.TT == q.TT) {
+      q.instance = i;
+      q.xrow = in.xrow;
+      q.smem_bytes = in.smem_bytes;
+    }
+  }
+  *p = q;
+  AVC_REQUIRE(q.instance >= 0, AVC_ERR_UNSUPPORTED, "avc_conv_block_fwd: no kernel for K=%d stride=%d tile=%d", K, S, q.TT);
+  return AVC_OK;
+}
+
+}  // namespace avc
+
+using namespace avc;
+
+extern "C" int avc_conv_block_fwd_plan(const avc_conv_desc* d, avc_simt_plan* out) {
+  AVC_REQUIRE(out, AVC_ERR_INVALID, "avc_conv_block_fwd_plan: null out");
+  return simt_plan(d, out);
+}
+
+extern "C" int avc_conv_block_fwd(const avc_conv_desc* d, void* stream) {
+  avc_simt_plan p;
+  const int rc = simt_plan(d, &p);
+  if (rc != AVC_OK) return rc;
   ConvArgs a;
   a.d = *d;
   if (!a.d.res) a.d.res_mode = AVC_RES_NONE;
-  const int S = d->stride, K = d->K;
-  int TT, TCO;
-  if (d->Tout <= 128) {
-    TT = 128;
-    TCO = 128;
-    a.tiled = 0;
-    a.seg_out = next_pow2(d->Tout < 8 ? 8 : d->Tout);
-    a.nseg = TT / a.seg_out;
-    a.ntt = 1;
-  } else if (d->norm && d->Tout <= 256 && (K == 1 || K == 5)) {
-    TT = 256;
-    TCO = 64;
-    a.tiled = 0;
-    a.seg_out = 256;
-    a.nseg = 1;
-    a.ntt = 1;
-  } else if (!d->norm) {
-    TT = 128;
-    TCO = 128;
-    a.tiled = 1;
-    a.seg_out = 128;
-    a.nseg = 1;
-    a.ntt = cdiv(d->Tout, TT);
-  } else {
-    set_error("avc_conv_block_fwd: fused InstanceNorm needs Tout <= 256 (got %d); use avc_norm_apply_fwd", d->Tout);
-    return AVC_ERR_UNSUPPORTED;
-  }
-  a.segp = ((a.seg_out * S + K - 1) + 3) / 4 * 4;
-  dim3 grid(a.tiled ? d->B * a.ntt : cdiv(d->B, a.nseg), cdiv(d->Cout, TCO));
-#define CASE(KK, SS)                                                          \
-  if (K == KK && S == SS) {                                                   \
-    if (TT == 128) return launch_conv<KK, SS, 128, 128>(a, grid, st);         \
-  }
-#define CASE256(KK, SS)                                                       \
-  if (K == KK && S == SS && TT == 256) return launch_conv<KK, SS, 64, 256>(a, grid, st);
-  CASE(1, 1) CASE(2, 1) CASE(3, 1) CASE(4, 1) CASE(5, 1) CASE(6, 1) CASE(7, 1) CASE(8, 1) CASE(5, 2)
-  CASE256(1, 1) CASE256(5, 1) CASE256(5, 2)
-#undef CASE
-#undef CASE256
-  set_error("avc_conv_block_fwd: no kernel for K=%d stride=%d tile=%d", K, S, TT);
-  return AVC_ERR_UNSUPPORTED;
+  a.seg_out = p.seg_out;
+  a.nseg = p.nseg;
+  a.segp = p.segp;
+  a.tiled = p.tiled;
+  a.ntt = p.ntt;
+  return kSimtInstances[p.instance].launch(a, dim3(p.grid_x, p.grid_y), (cudaStream_t)stream);
 }

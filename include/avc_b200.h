@@ -114,9 +114,22 @@ typedef struct avc_conv_desc {
 } avc_conv_desc;
 
 /* Fused block forward.  norm=1 needs the whole Tn of a sample inside one CTA tile:
- * supported for Tout <= 256, otherwise AVC_ERR_UNSUPPORTED -- run it with norm=0, relu=0,
- * res=null, save_c=out-of-conv and follow with avc_norm_apply_fwd. */
+ * supported for Tout <= 128, and Tout <= 256 at K = 1 or 5; otherwise AVC_ERR_UNSUPPORTED -- run it with norm=0,
+ * relu=0, res=null, save_c=out-of-conv and follow with avc_norm_apply_fwd.  AVC_F_FOLD, AVC_F_NORMBWD and a non-zero
+ * out_tstride / out_toff / out_T (avc_conv_block_tc only) are AVC_ERR_UNSUPPORTED; AVC_F_IN_TF32 is ignored. */
 int avc_conv_block_fwd(const avc_conv_desc* d, void* stream);
+/* The tile plan avc_conv_block_fwd runs a descriptor with.  Host only: launches nothing, reads no pointer; runs the same
+ * argument checks and returns the same code (and avc_last_error() message) as the launch.  A CTA of 256 threads owns TCO
+ * output channels x TT output steps; untiled, the tile holds nseg = TT / seg_out samples of seg_out >= Tout columns
+ * (staged input segments segp floats apart); tiled (no InstanceNorm), one sample's output is cut into ntt tiles of TT. */
+typedef struct avc_simt_plan {
+  int32_t TT, TCO, tiled, seg_out, nseg, segp, ntt, grid_x, grid_y;
+  int32_t xrow;       /* floats per staged input row (one channel) in shared memory */
+  int32_t smem_bytes; /* dynamic shared memory of the launch */
+  int32_t instance;   /* index into the fixed table of kernel instances (K, stride, TCO, TT): (K, 1, 128, 128) for
+                         K = 1..8, (5, 2, 128, 128), (1, 1, 64, 256), (5, 1, 64, 256), (5, 2, 64, 256); or -1 */
+} avc_simt_plan;
+int avc_conv_block_fwd_plan(const avc_conv_desc* d, avc_simt_plan* out);
 /* The same fused block on the tensor cores (wgmma, TF32 inputs rounded to nearest, fp32
  * accumulation).  Covers stride 1|2, in_ups 1, Cin % 16 == 0; whole samples up to 144 columns, folded
  * (AVC_F_FOLD) ones up to 256 staged rows (longer ones time-tiled without InstanceNorm / fold / pixel shuffle); otherwise

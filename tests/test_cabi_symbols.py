@@ -30,7 +30,7 @@ def test_struct_layouts_match_header_sizes():
     """ctypes mirrors of the descriptor structs have the size the C compiler gives them."""
     import ctypes, subprocess, tempfile
     from adaptive_voice_conversion_b200 import _lib as L
-    prog = '#include <stdio.h>\n#include "avc_b200.h"\nint main(){printf("%zu %zu %zu %zu %zu %zu %zu\\n", sizeof(avc_conv_desc), sizeof(avc_wgrad_desc), sizeof(avc_fold_desc), sizeof(avc_linear_desc), sizeof(avc_dense_stack_desc), sizeof(avc_linear_batch_desc), sizeof(avc_tc_plan));return 0;}\n'
+    prog = '#include <stdio.h>\n#include "avc_b200.h"\nint main(){printf("%zu %zu %zu %zu %zu %zu %zu %zu\\n", sizeof(avc_conv_desc), sizeof(avc_wgrad_desc), sizeof(avc_fold_desc), sizeof(avc_linear_desc), sizeof(avc_dense_stack_desc), sizeof(avc_linear_batch_desc), sizeof(avc_tc_plan), sizeof(avc_simt_plan));return 0;}\n'
     with tempfile.TemporaryDirectory() as td:
         c = os.path.join(td, "s.c")
         open(c, "w").write(prog)
@@ -38,7 +38,8 @@ def test_struct_layouts_match_header_sizes():
         subprocess.check_call(["gcc", "-I", os.path.join(ROOT, "include"), c, "-o", exe])
         sizes = [int(v) for v in subprocess.check_output([exe]).split()]
     assert sizes == [ctypes.sizeof(L.ConvDesc), ctypes.sizeof(L.WgradDesc), ctypes.sizeof(L.FoldDesc), ctypes.sizeof(L.LinearDesc),
-                     ctypes.sizeof(L.DenseStackDesc), ctypes.sizeof(L.LinearBatchDesc), ctypes.sizeof(L.TcPlan)]
+                     ctypes.sizeof(L.DenseStackDesc), ctypes.sizeof(L.LinearBatchDesc), ctypes.sizeof(L.TcPlan),
+                     ctypes.sizeof(L.SimtPlan)]
 
 
 def test_sass_is_sm90a():
