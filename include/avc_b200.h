@@ -241,7 +241,8 @@ int avc_fold_add_fwd(const avc_fold_desc* d, void* stream);
 /* nn.Conv1d weight [Cout][Cin][K] -> kernel operand layout (AVC_PACK_*). */
 int avc_pack_conv_weight(const float* w, float* packed, int Cout, int Cin, int K, int mode, void* stream);
 
-/* planar [B][C][T] <-> A4.  add != 0 accumulates into dst instead of overwriting. */
+/* planar [B][C][T] <-> A4.  round_tf32 != 0 rounds every packed value to TF32 (cvt.rna: to nearest, ties away from
+ * zero), so each stored value has its low 13 bits clear. */
 int avc_pack_a4(const float* planar, float* a4, int64_t a4_bstride, int B, int C, int T, int round_tf32, void* stream);
 int avc_unpack_a4(const float* a4, int64_t a4_bstride, float* planar, int B, int C, int T, void* stream);
 
