@@ -30,6 +30,7 @@ PAD_REFLECT, PAD_ZERO = 0, 1
 RES_NONE, RES_SAME, RES_POOL, RES_UP = 0, 1, 2, 3
 PACK_FWD, PACK_DGRAD = 0, 1
 F_ROUND_OUT, F_IN_TF32, F_FOLD, F_NORMBWD = 1, 2, 4, 8
+TAIL_REFLECT, TAIL_REPLICATE, TAIL_ZERO = 0, 1, 2
 OK, ERR_INVALID, ERR_UNSUPPORTED, ERR_CUDA = 0, -1, -2, -3
 
 _fp = C.c_void_p  # device pointers travel as integers
@@ -243,6 +244,9 @@ PROTOTYPES = {
     "avc_bias_grad_groups": (_i, [_p, _i64, _p, _i, _i, _i, _i, _p]),
     "avc_time_mean_fwd": (_i, [_p, _i64, _p, _i, _i, _i, _p]),
     "avc_time_mean_bwd": (_i, [_p, _p, _i64, _i, _i, _i, _p]),
+    "avc_norm_apply_varlen": (_i, [C.POINTER(ConvDesc), _p, _i, _i, _p]),
+    "avc_time_mean_varlen_fwd": (_i, [_p, _i64, _p, _i, _i, _i, _p, _i, _i, _p]),
+    "avc_varlen_tail": (_i, [_p, _i64, _i, _i, _i, _p, _i, _i, _i, _i, _p]),
     "avc_linear_fwd": (_i, [C.POINTER(LinearDesc), _p]),
     "avc_linear_bwd": (_i, [C.POINTER(LinearDesc), _p]),
     "avc_dense_stack_fwd": (_i, [C.POINTER(DenseStackDesc), _p]),

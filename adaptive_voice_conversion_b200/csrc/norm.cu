@@ -1,6 +1,8 @@
 // HBM-bound epilogue kernels on A4 tensors:
 //  * avc_norm_apply_fwd : two-pass InstanceNorm/AdaIN/ReLU/residual for sequences too long
 //                         for the fused conv tile (nn.InstanceNorm1d, append_cond; model.py:296,341,77-83)
+//  * avc_norm_apply_varlen : the same over each sample's valid frames of a padded batch
+//  * avc_varlen_tail    : rewrites the frames just past each sample's length of a padded batch
 //  * avc_norm_bwd       : backward of that epilogue (autograd under solver.py:90)
 //  * avc_fold_add_fwd   : adjoint of F.pad(mode='reflect') (model.py:28-30) + residual adjoint
 //  * avc_bias_grad      : bias gradient of a conv without epilogue
@@ -42,8 +44,16 @@ __device__ __forceinline__ void load_rows(const float* cb /*sample base*/, int q
   }
 }
 
+// Valid frames of sample b of a padded batch: ceil(lengths[b] / div) * mul (avc_b200.h).
+__device__ __forceinline__ int varlen_len(const int32_t* lengths, int b, int div, int mul) {
+  return ((__ldg(lengths + b) + div - 1) / div) * mul;
+}
+
+// lengths null: every sample has Tout conv outputs; otherwise sample b has L_b = varlen_len(...) and only its first
+// L_b (2 L_b after the shuffle) frames enter the statistics and are written
 template <bool SHUF>
-__global__ void __launch_bounds__(256) norm_apply_fwd_kernel(const avc_conv_desc d) {
+__global__ void __launch_bounds__(256) norm_apply_fwd_kernel(const avc_conv_desc d, const int32_t* __restrict__ lengths,
+                                                             int div, int mul) {
   constexpr int NS = SHUF ? 2 : 1;
   const int Cn = SHUF ? d.Cout / 2 : d.Cout;
   const int Tn = SHUF ? d.Tout * 2 : d.Tout;
@@ -52,24 +62,25 @@ __global__ void __launch_bounds__(256) norm_apply_fwd_kernel(const avc_conv_desc
   const int lane = threadIdx.x & 31;
   if (warp >= d.B * Cnq) return;
   const int b = warp / Cnq, qn = warp - b * Cnq;
+  const int Lc = lengths ? min(varlen_len(lengths, b, div, mul), d.Tout) : d.Tout;   // conv outputs used
   const float* cb = d.save_c + (int64_t)b * d.Cout * d.Tout;
   float mean[4] = {0, 0, 0, 0}, rstd[4] = {1, 1, 1, 1};
   if (d.norm) {
     float4 s = zero4();
-    for (int t = lane; t < d.Tout; t += 32) {
+    for (int t = lane; t < Lc; t += 32) {
       float v[2][4];
       load_rows<SHUF>(cb, qn, d.Tout, t, v);
 #pragma unroll
       for (int sx = 0; sx < NS; ++sx) { s.x += v[sx][0]; s.y += v[sx][1]; s.z += v[sx][2]; s.w += v[sx][3]; }
     }
     s = warp_sum4(s);
-    const float inv = 1.f / (float)Tn;
+    const float inv = 1.f / (float)(SHUF ? 2 * Lc : Lc);
     mean[0] = s.x * inv; mean[1] = s.y * inv; mean[2] = s.z * inv; mean[3] = s.w * inv;
     // corrected two-pass: the deviations also sum to the rounding error of the first pass's mean, which is removed
     // from the mean and the variance.  Without it a channel that is constant over time (rstd = eps^-1/2) normalises
     // to (c - mean) * 316 instead of 0.
     float4 m1 = zero4(), m2 = zero4();
-    for (int t = lane; t < d.Tout; t += 32) {
+    for (int t = lane; t < Lc; t += 32) {
       float v[2][4];
       load_rows<SHUF>(cb, qn, d.Tout, t, v);
 #pragma unroll
@@ -106,7 +117,9 @@ __global__ void __launch_bounds__(256) norm_apply_fwd_kernel(const avc_conv_desc
       gamma[c] = __ldg(d.cond + (int64_t)b * d.cond_bstride + Cn + qn * 4 + c);
     }
   }
-  for (int t = lane; t < d.Tout; t += 32) {
+  // a POOL residual's input holds ceil(lengths[b] / (div / 2)) * mul valid frames; an odd last one is averaged alone
+  const int res_L = (lengths && d.res_mode == AVC_RES_POOL) ? min(varlen_len(lengths, b, div / 2, mul), d.res_T) : d.res_T;
+  for (int t = lane; t < Lc; t += 32) {
     float v[2][4];
     load_rows<SHUF>(cb, qn, d.Tout, t, v);
 #pragma unroll
@@ -127,7 +140,7 @@ __global__ void __launch_bounds__(256) norm_apply_fwd_kernel(const avc_conv_desc
         else if (d.res_mode == AVC_RES_UP) r = ldg4(rb + (int64_t)(tn >> 1) * 4);
         else {
           r = ldg4(rb + (int64_t)(2 * tn) * 4);
-          if (2 * tn + 1 < d.res_T) {
+          if (2 * tn + 1 < res_L) {
             const float4 r2 = ldg4(rb + (int64_t)(2 * tn + 1) * 4);
             r.x = 0.5f * (r.x + r2.x); r.y = 0.5f * (r.y + r2.y); r.z = 0.5f * (r.z + r2.z); r.w = 0.5f * (r.w + r2.w);
           }
@@ -358,6 +371,24 @@ __global__ void __launch_bounds__(256) norm_bwd_cached_kernel(const avc_conv_des
   }
 }
 
+// thread = (sample, 4-channel chunk, frame j past the sample's L_b); the modes of avc_varlen_tail (avc_b200.h)
+__global__ void __launch_bounds__(256) varlen_tail_kernel(float* __restrict__ a4, int64_t bstride, int B, int C, int T,
+                                                          const int32_t* __restrict__ lengths, int div, int mul, int mode, int n) {
+  const int Cq = C >> 2;
+  const int64_t total = (int64_t)B * Cq * n;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+    const int j = (int)(i % n);
+    const int64_t bq = i / n;
+    const int q = (int)(bq % Cq), b = (int)(bq / Cq);
+    const int Lb = varlen_len(lengths, b, div, mul), t = Lb + j;
+    if (t >= T) continue;
+    float* row = a4 + (int64_t)b * bstride + (int64_t)q * T * 4;
+    if (mode == AVC_TAIL_ZERO) st4(row + (int64_t)t * 4, zero4());
+    else if (mode == AVC_TAIL_REFLECT) st4(row + (int64_t)t * 4, *reinterpret_cast<const float4*>(row + (int64_t)abs(Lb - 2 - j) * 4));
+    else if (Lb & 1) st4(row + (int64_t)t * 4, *reinterpret_cast<const float4*>(row + (int64_t)(Lb - 1) * 4));   // REPLICATE
+  }
+}
+
 __global__ void __launch_bounds__(256) fold_add_kernel(const avc_fold_desc d) {
   const int Cq = d.C >> 2;
   const int64_t total = (int64_t)d.B * Cq * d.Tin;
@@ -448,9 +479,42 @@ extern "C" int avc_norm_apply_fwd(const avc_conv_desc* d, void* stream) {
   const int Cn = d->shuffle ? d->Cout / 2 : d->Cout;
   const int64_t warps = (int64_t)d->B * (Cn / 4);
   const int blocks = (int)cdiv64(warps * 32, 256);
-  if (d->shuffle) AVC_LAUNCH(norm_apply_fwd_kernel<true>, blocks, 256, 0, (cudaStream_t)stream, *d);
-  else AVC_LAUNCH(norm_apply_fwd_kernel<false>, blocks, 256, 0, (cudaStream_t)stream, *d);
+  if (d->shuffle) AVC_LAUNCH(norm_apply_fwd_kernel<true>, blocks, 256, 0, (cudaStream_t)stream, *d, nullptr, 1, 1);
+  else AVC_LAUNCH(norm_apply_fwd_kernel<false>, blocks, 256, 0, (cudaStream_t)stream, *d, nullptr, 1, 1);
   AVC_CHECK_LAUNCH("norm_apply_fwd");
+  return AVC_OK;
+}
+
+extern "C" int avc_norm_apply_varlen(const avc_conv_desc* d, const int32_t* lengths, int len_div, int len_mul, void* stream) {
+  int rc = validate_conv_desc(d, "avc_norm_apply_varlen");
+  if (rc != AVC_OK) return rc;
+  AVC_REQUIRE(lengths && len_div >= 1 && len_mul >= 1, AVC_ERR_INVALID, "avc_norm_apply_varlen: lengths null or len_div/len_mul < 1");
+  AVC_REQUIRE(d->save_c && d->out, AVC_ERR_INVALID, "avc_norm_apply_varlen: null save_c/out");
+  AVC_REQUIRE(!d->res || d->res_mode != AVC_RES_NONE, AVC_ERR_INVALID, "avc_norm_apply_varlen: res without res_mode");
+  AVC_REQUIRE(!d->res || d->res_mode != AVC_RES_POOL || len_div % 2 == 0, AVC_ERR_INVALID,
+              "avc_norm_apply_varlen: a POOL residual needs an even len_div");
+  AVC_REQUIRE(!d->mask, AVC_ERR_UNSUPPORTED, "avc_norm_apply_varlen: mask is not supported");
+  const int Cn = d->shuffle ? d->Cout / 2 : d->Cout;
+  const int blocks = (int)cdiv64((int64_t)d->B * (Cn / 4) * 32, 256);
+  if (d->shuffle) AVC_LAUNCH(norm_apply_fwd_kernel<true>, blocks, 256, 0, (cudaStream_t)stream, *d, lengths, len_div, len_mul);
+  else AVC_LAUNCH(norm_apply_fwd_kernel<false>, blocks, 256, 0, (cudaStream_t)stream, *d, lengths, len_div, len_mul);
+  AVC_CHECK_LAUNCH("norm_apply_varlen");
+  return AVC_OK;
+}
+
+extern "C" int avc_varlen_tail(float* a4, int64_t bstride, int B, int C, int T, const int32_t* lengths, int len_div, int len_mul,
+                               int mode, int n, void* stream) {
+  AVC_REQUIRE(a4 && B > 0 && C > 0 && C % 4 == 0 && T > 0, AVC_ERR_INVALID, "avc_varlen_tail: bad argument");
+  AVC_REQUIRE(lengths && len_div >= 1 && len_mul >= 1, AVC_ERR_INVALID, "avc_varlen_tail: lengths null or len_div/len_mul < 1");
+  AVC_REQUIRE(mode == AVC_TAIL_REFLECT || mode == AVC_TAIL_REPLICATE || mode == AVC_TAIL_ZERO, AVC_ERR_INVALID,
+              "avc_varlen_tail: bad mode %d", mode);
+  if (mode == AVC_TAIL_REPLICATE) n = 1;
+  else if (mode == AVC_TAIL_ZERO) n = T;
+  AVC_REQUIRE(n >= 1 && n <= T, AVC_ERR_INVALID, "avc_varlen_tail: n=%d outside [1, T=%d]", n, T);
+  int blocks = (int)cdiv64((int64_t)B * (C / 4) * n, 256);
+  if (blocks > 148 * 16) blocks = 148 * 16;
+  AVC_LAUNCH(varlen_tail_kernel, blocks, 256, 0, (cudaStream_t)stream, a4, bstride, B, C, T, lengths, len_div, len_mul, mode, n);
+  AVC_CHECK_LAUNCH("varlen_tail");
   return AVC_OK;
 }
 

@@ -73,19 +73,22 @@ __global__ void unpack_a4_kernel(const float* __restrict__ a4, int64_t bstride, 
 }
 
 // ------------------------------------------------------------------ mean over time
-__global__ void time_mean_fwd_kernel(const float* __restrict__ a4, int64_t bstride, float* __restrict__ out, int B, int C, int T) {
+// lengths non-null (a padded batch): sample b's mean over its first ceil(lengths[b] / div) * mul frames
+__global__ void time_mean_fwd_kernel(const float* __restrict__ a4, int64_t bstride, float* __restrict__ out, int B, int C, int T,
+                                     const int32_t* __restrict__ lengths, int div, int mul) {
   const int Cq = C >> 2;
   const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
   if (warp >= B * Cq) return;
   const int b = warp / Cq, q = warp - b * Cq;
+  const int Lb = lengths ? min((__ldg(lengths + b) + div - 1) / div * mul, T) : T;
   float4 s = zero4();
-  for (int t = lane; t < T; t += 32) {
+  for (int t = lane; t < Lb; t += 32) {
     const float4 v = ldg4(a4 + (int64_t)b * bstride + ((int64_t)q * T + t) * 4);
     s.x += v.x; s.y += v.y; s.z += v.z; s.w += v.w;
   }
   s.x = warp_sum(s.x); s.y = warp_sum(s.y); s.z = warp_sum(s.z); s.w = warp_sum(s.w);
   if (lane == 0) {
-    const float inv = 1.f / (float)T;
+    const float inv = 1.f / (float)Lb;
     st4(out + (int64_t)b * C + q * 4, make_float4(s.x * inv, s.y * inv, s.z * inv, s.w * inv));
   }
 }
@@ -405,8 +408,18 @@ extern "C" int avc_unpack_a4(const float* a4, int64_t a4_bstride, float* planar,
 extern "C" int avc_time_mean_fwd(const float* a4, int64_t bstride, float* out, int B, int C, int T, void* stream) {
   AVC_REQUIRE(a4 && out && B > 0 && C > 0 && C % 4 == 0 && T > 0, AVC_ERR_INVALID, "avc_time_mean_fwd: bad argument");
   const int64_t warps = (int64_t)B * (C / 4);
-  AVC_LAUNCH(time_mean_fwd_kernel, (int)cdiv64(warps * 32, 256), 256, 0, (cudaStream_t)stream, a4, bstride, out, B, C, T);
+  AVC_LAUNCH(time_mean_fwd_kernel, (int)cdiv64(warps * 32, 256), 256, 0, (cudaStream_t)stream, a4, bstride, out, B, C, T,
+             (const int32_t*)nullptr, 1, 1);
   AVC_CHECK_LAUNCH("time_mean_fwd");
+  return AVC_OK;
+}
+extern "C" int avc_time_mean_varlen_fwd(const float* a4, int64_t bstride, float* out, int B, int C, int T, const int32_t* lengths,
+                                        int len_div, int len_mul, void* stream) {
+  AVC_REQUIRE(a4 && out && B > 0 && C > 0 && C % 4 == 0 && T > 0, AVC_ERR_INVALID, "avc_time_mean_varlen_fwd: bad argument");
+  AVC_REQUIRE(lengths && len_div >= 1 && len_mul >= 1, AVC_ERR_INVALID, "avc_time_mean_varlen_fwd: lengths null or len_div/len_mul < 1");
+  AVC_LAUNCH(time_mean_fwd_kernel, (int)cdiv64((int64_t)B * (C / 4) * 32, 256), 256, 0, (cudaStream_t)stream, a4, bstride, out, B, C,
+             T, lengths, len_div, len_mul);
+  AVC_CHECK_LAUNCH("time_mean_varlen_fwd");
   return AVC_OK;
 }
 extern "C" int avc_time_mean_bwd(const float* dout, float* da4, int64_t bstride, int B, int C, int T, void* stream) {

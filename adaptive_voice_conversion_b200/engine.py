@@ -58,6 +58,59 @@ def conv_geometry(K: int, stride: int, Tin: int):
     return pl, pr, Tout
 
 
+class Lengths:
+    """Valid frames per sample of a padded batch at one layer: ceil(t[b] / div) * mul, with t the batch's input lengths
+    (int32 [B] on the device) -- the avc_b200.h convention.  A stride-2 layer doubles div, an upsampling block
+    doubles mul (conv_geometry of the odd kernels the stacks use: Tout = ceil(Tin / stride))."""
+    __slots__ = ("t", "div", "mul")
+
+    def __init__(self, t: torch.Tensor, div: int = 1, mul: int = 1):
+        self.t, self.div, self.mul = t, div, mul
+
+    def down(self, s: int) -> "Lengths":
+        assert s == 1 or self.mul == 1, "subsampling after an upsampling"
+        return self if s == 1 else Lengths(self.t, self.div * s, 1)
+
+    def up(self, u: int) -> "Lengths":
+        return self if u == 1 else Lengths(self.t, self.div, self.mul * u)
+
+    def of(self, L: int) -> int:
+        """The layer's length of an input of L frames (host arithmetic: tests, extents)."""
+        return -(-L // self.div) * self.mul
+
+
+def _varlen_layers(config: dict, source: bool):
+    """[(level, pad_right)] of every reflect-padded conv on the path of an input, in order: the content encoder and the
+    decoder (source) or the speaker encoder (reference).  level = (div, mul) of the layer's input, as in Lengths."""
+    c = config["ContentEncoder" if source else "SpeakerEncoder"]
+    out, div = [], 1
+    ks = range(c["bank_scale"], c["bank_size"] + 1, c["bank_scale"])
+    out.append(((1, 1), max(conv_geometry(k, 1, 1)[1] for k in ks)))
+    K = c["kernel_size"]
+    for s in c["subsample"][: c["n_conv_blocks"]]:
+        out += [((div, 1), conv_geometry(K, 1, 1)[1]), ((div, 1), conv_geometry(K, s, 1)[1])]
+        div *= s
+    if source:
+        de, mul = config["Decoder"], 1
+        for up in de["upsample"][: de["n_conv_blocks"]]:
+            out += [((div, mul), conv_geometry(de["kernel_size"], 1, 1)[1])] * 2
+            mul *= up
+    return out
+
+
+def varlen_extent(config: dict, T: int, source: bool) -> int:
+    """Time extent the engine gives a padded batch of inputs of at most T frames: the least multiple of 8, >= T, at
+    which every reflect-padded conv of the path (see _varlen_layers) finds room past every sample's valid frames for
+    its pad_right reflected frames (avc_varlen_tail rewrites them before the conv).  The layer extents follow
+    conv_geometry from this one; a sample of T frames is the tightest (ceil is monotone)."""
+    layers = _varlen_layers(config, source)
+    Te = -(-T // 8) * 8
+    while True:
+        if all(Lengths(None, div, mul).of(Te) - Lengths(None, div, mul).of(T) >= pr for (div, mul), pr in layers):
+            return Te
+        Te += 8
+
+
 class Engine:
     """Launch sequencer for one AE configuration on one device."""
 
@@ -368,17 +421,34 @@ class Engine:
                  "spectral_norm_bwd")
 
     # ------------------------------------------------------------------ one conv block
+    def tail(self, x: A4, lens: Lengths, mode: int, n: int = 1):
+        """avc_varlen_tail on x: the frames just past each sample's valid ones (padded batches)."""
+        self._ck(self.lib.avc_varlen_tail(x.ptr, x.bstride, x.B, x.C, x.T, lens.t.data_ptr(), lens.div, lens.mul, mode, n,
+                                          self.stream), "varlen_tail")
+
     def conv(self, P, name, xin: A4, *, stride=1, shuffle=False, norm=False, cond=None, relu=False,
-             res: Optional[A4] = None, res_mode=L.RES_NONE, out: Optional[A4] = None, train=False, round_out=False):
+             res: Optional[A4] = None, res_mode=L.RES_NONE, out: Optional[A4] = None, train=False, round_out=False,
+             lens: Optional[Lengths] = None, tail=True):
         """One fused conv block.  round_out (tf32 mode only): round the block output to TF32 -- set ONLY when
         every consumer of `out` is a tensor-core conv operand (the first conv of a block, the bank convs), so
         that the consumer can skip its rounding pass.  The residual stream, the mean/std heads and out_conv
-        stay full fp32 like the reference's activations (cuDNN-TF32 rounds matmul inputs only)."""
+        stay full fp32 like the reference's activations (cuDNN-TF32 rounds matmul inputs only).
+
+        lens: the valid frames of each sample of xin (a padded batch, inference only).  The conv first reflects each
+        sample's last frames into its pad_right frames past them (unless tail=False: the caller did), and an
+        InstanceNorm block runs as a plain conv + avc_norm_apply_varlen whatever its length, so that its statistics
+        cover the valid frames only.  Frames of out past a sample's valid ones are undefined."""
         w = P[name + ".weight"]
         Cout, Cin, K = w.shape
         assert Cin == xin.C, (name, Cin, xin.C)
         pl, pr, Tout = conv_geometry(K, stride, xin.T)
         B = xin.B
+        if lens is not None:
+            if train:
+                raise L.AvcError("padded batches (lengths) are inference-only; training runs on fixed segments")
+            assert stride == 1 or K % 2 == 1, "a padded batch needs Tout = ceil(Tin / stride)"
+            if tail and pr > 0:
+                self.tail(xin, lens, L.TAIL_REFLECT, pr)
         Cn, Tn = (Cout // 2, Tout * 2) if shuffle else (Cout, Tout)
         if out is None:
             out = A4.empty(B, Cn, Tn, self.dev)
@@ -390,9 +460,10 @@ class Engine:
         # (shuffle / InstanceNorm / AdaIN / residual)
         tc_ok = (self.precision == "tf32" and not self.fwd_fp32 and Cin % 16 == 0 and not (stride == 2 and shuffle)
                  and "fwd_tc" in self.packed[name])
-        use_tc = tc_ok and (Tout * stride <= 144 or (not norm and not shuffle))
+        varlen_norm = lens is not None and norm
+        use_tc = tc_ok and not varlen_norm and (Tout * stride <= 144 or (not norm and not shuffle))
         tc_split = tc_ok and not use_tc and norm
-        fused = use_tc or (not tc_split and ((not norm) or (Tout <= 128) or (Tout <= 256 and K in (1, 5))))
+        fused = use_tc or (not tc_split and not varlen_norm and ((not norm) or (Tout <= 128) or (Tout <= 256 and K in (1, 5))))
         c = A4.empty(B, Cout, Tout, self.dev) if (need_c or not fused) else None
         stats = self.empty(B, Cn, 2) if norm else None
         d = L.ConvDesc()
@@ -429,7 +500,12 @@ class Engine:
                 self._ck(self.lib.avc_conv_block_fwd(C.byref(d), self.stream), f"conv_block_fwd[{name}]")
             self._fill_epilogue(d, out, shuffle, norm, relu, cond, res, res_mode, stats)
             d.save_c = c.ptr
-            self._ck(self.lib.avc_norm_apply_fwd(C.byref(d), self.stream), f"norm_apply_fwd[{name}]")
+            if varlen_norm:
+                lo = lens.down(stride)
+                self._ck(self.lib.avc_norm_apply_varlen(C.byref(d), lo.t.data_ptr(), lo.div, lo.mul, self.stream),
+                         f"norm_apply_varlen[{name}]")
+            else:
+                self._ck(self.lib.avc_norm_apply_fwd(C.byref(d), self.stream), f"norm_apply_fwd[{name}]")
             if not need_c:
                 c = None
         rec = None
@@ -727,7 +803,8 @@ class Engine:
         return dx
 
     # ------------------------------------------------------------------ encoders
-    def _bank_and_in_conv(self, P, enc, c, x_planar: torch.Tensor, norm: bool, train: bool, ctx: dict):
+    def _bank_and_in_conv(self, P, enc, c, x_planar: torch.Tensor, norm: bool, train: bool, ctx: dict,
+                          lens: Optional[Lengths] = None):
         """conv_bank + in_conv_layer (model.py:85-91, 266-269 / 302-307).  The concat is never
         assembled by a copy: every bank conv writes its channel range of one A4 buffer and
         x itself is packed straight into the last c_in channels."""
@@ -738,41 +815,57 @@ class Engine:
         cat = A4.empty(B, ctot, T, self.dev)
         x4 = cat.channels(c_bank * len(ks), ctot)
         self.pack_a4(x_planar, x4)
+        if lens is not None:   # one reflection, as wide as the widest bank kernel's, serves every bank conv
+            self.tail(x4, lens, L.TAIL_REFLECT, max(conv_geometry(k, 1, T)[1] for k in ks))
         recs = []
         for i, _k in enumerate(ks):
             _, r = self.conv(P, f"{enc}.conv_bank.{i}", x4, relu=True, out=cat.channels(i * c_bank, (i + 1) * c_bank), train=False,
-                             round_out=True)   # the concat is read by in_conv (and its weight gradient) only
+                             round_out=True, lens=lens, tail=False)   # the concat is read by in_conv (and its weight gradient) only
             recs.append(r)
         # every writer of `cat` (pack_a4 and the bank convs' epilogues) rounds to TF32 in tf32 mode
         cat.tf32 = self.precision == "tf32" and not self.fwd_fp32
-        out, rec_in = self.conv(P, f"{enc}.in_conv_layer", cat, norm=norm, relu=True, train=train)
+        out, rec_in = self.conv(P, f"{enc}.in_conv_layer", cat, norm=norm, relu=True, train=train, lens=lens)
         if train:
             ctx["cat"], ctx["x4"], ctx["in"] = cat, x4, rec_in
             ctx["n_bank"], ctx["c_bank"] = len(ks), c_bank
         return out
 
-    def _enc_blocks(self, P, enc, c, out: A4, norm: bool, train: bool, ctx: dict):
+    def _enc_blocks(self, P, enc, c, out: A4, norm: bool, train: bool, ctx: dict, lens: Optional[Lengths] = None):
         blocks = []
         for l, s in enumerate(c["subsample"][: c["n_conv_blocks"]]):
-            y, r1 = self.conv(P, f"{enc}.first_conv_layers.{l}", out, norm=norm, relu=True, train=train, round_out=True)
+            y, r1 = self.conv(P, f"{enc}.first_conv_layers.{l}", out, norm=norm, relu=True, train=train, round_out=True, lens=lens)
+            if lens is not None and s > 1 and not norm:
+                # the block input was the first conv's input (reflected tail); as the fused conv's POOL residual its
+                # frame past an odd length must now repeat the last one
+                self.tail(out, lens, L.TAIL_REPLICATE)
             new, r2 = self.conv(P, f"{enc}.second_conv_layers.{l}", y, stride=s, norm=norm, relu=True, res=out,
-                                res_mode=L.RES_POOL if s > 1 else L.RES_SAME, train=train)
+                                res_mode=L.RES_POOL if s > 1 else L.RES_SAME, train=train, lens=lens)
             blocks.append((r1, r2, s, out))
             out = new
+            if lens is not None:
+                lens = lens.down(s)
         if train:
             ctx["blocks"] = blocks
+        if lens is not None:
+            ctx["lens"] = lens
         return out
 
-    def speaker_fwd(self, P, x_planar: torch.Tensor, train: bool):
-        """SpeakerEncoder.forward (model.py:265-277) -> emb [B, c_out]."""
+    def speaker_fwd(self, P, x_planar: torch.Tensor, train: bool, lens: Optional[Lengths] = None):
+        """SpeakerEncoder.forward (model.py:265-277) -> emb [B, c_out].  lens: a padded batch (inference only): x_planar
+        holds lens.t[b] valid frames of sample b in an extent of varlen_extent(cfg, T, source=False)."""
         c = self.cfg["SpeakerEncoder"]
         enc = "speaker_encoder"
         ctx: dict = {}
-        out = self._bank_and_in_conv(P, enc, c, x_planar, norm=False, train=train, ctx=ctx)
-        out = self._enc_blocks(P, enc, c, out, norm=False, train=train, ctx=ctx)
+        out = self._bank_and_in_conv(P, enc, c, x_planar, norm=False, train=train, ctx=ctx, lens=lens)
+        out = self._enc_blocks(P, enc, c, out, norm=False, train=train, ctx=ctx, lens=lens)
         B = out.B
         pooled = self.empty(B, out.C)
-        self._ck(self.lib.avc_time_mean_fwd(out.ptr, out.bstride, pooled.data_ptr(), B, out.C, out.T, self.stream), "time_mean_fwd")
+        if lens is not None:
+            lo = ctx.pop("lens")
+            self._ck(self.lib.avc_time_mean_varlen_fwd(out.ptr, out.bstride, pooled.data_ptr(), B, out.C, out.T, lo.t.data_ptr(),
+                                                       lo.div, lo.mul, self.stream), "time_mean_varlen_fwd")
+        else:
+            self._ck(self.lib.avc_time_mean_fwd(out.ptr, out.bstride, pooled.data_ptr(), B, out.C, out.T, self.stream), "time_mean_fwd")
         nd = c["n_dense_blocks"]
         if self.fused_dense and out.C == 128 and c["c_out"] == 128:
             names = self._dense_names(enc)
@@ -829,13 +922,14 @@ class Engine:
         self._ck(self.lib.avc_time_mean_bwd(dh.data_ptr(), dout.ptr, dout.bstride, last.B, last.C, last.T, self.stream), "time_mean_bwd")
         self._enc_bwd(P, G, "speaker_encoder", c, ctx, dout)
 
-    def content_fwd(self, P, x_planar: torch.Tensor, train: bool):
-        """ContentEncoder.forward (model.py:301-323) -> (mu4, ls4) A4 [B, c_out, T/8]."""
+    def content_fwd(self, P, x_planar: torch.Tensor, train: bool, lens: Optional[Lengths] = None):
+        """ContentEncoder.forward (model.py:301-323) -> (mu4, ls4) A4 [B, c_out, T/8].  lens: a padded batch (inference
+        only) in an extent of varlen_extent(cfg, T, source=True); ctx["lens"] then holds the latent's valid frames."""
         c = self.cfg["ContentEncoder"]
         enc = "content_encoder"
         ctx: dict = {}
-        out = self._bank_and_in_conv(P, enc, c, x_planar, norm=True, train=train, ctx=ctx)
-        out = self._enc_blocks(P, enc, c, out, norm=True, train=train, ctx=ctx)
+        out = self._bank_and_in_conv(P, enc, c, x_planar, norm=True, train=train, ctx=ctx, lens=lens)
+        out = self._enc_blocks(P, enc, c, out, norm=True, train=train, ctx=ctx, lens=lens)
         mu4, r_mu = self.conv(P, f"{enc}.mean_layer", out, train=train)
         ls4, r_ls = self.conv(P, f"{enc}.std_layer", out, train=train)
         if train:
@@ -972,24 +1066,29 @@ class Engine:
                 aff.append(r)
         return conds, aff
 
-    def decoder_fwd(self, P, z4: A4, emb: torch.Tensor, train: bool, affine=None):
+    def decoder_fwd(self, P, z4: A4, emb: torch.Tensor, train: bool, affine=None, lens: Optional[Lengths] = None):
         """Decoder.forward (model.py:347-371) -> dec4 A4 [B, c_out, 8*T].  affine: the result of decoder_affine_fwd
-        when the caller already computed it (on the speaker branch's stream)."""
+        when the caller already computed it (on the speaker branch's stream).  lens: the valid frames of each sample of
+        z4 (a padded batch, inference only); dec4 is then exactly 0 past each sample's valid frames."""
         c = self.cfg["Decoder"]
         dn = "decoder"
         ctx: dict = {}
-        out, r_in = self.conv(P, f"{dn}.in_conv_layer", z4, norm=True, relu=True, train=train)
+        out, r_in = self.conv(P, f"{dn}.in_conv_layer", z4, norm=True, relu=True, train=train, lens=lens)
         nblk = c["n_conv_blocks"]
         conds, aff = affine if affine is not None else self.decoder_affine_fwd(P, emb, train)
         blocks = []
         for l, up in enumerate(c["upsample"][:nblk]):
             y, r1 = self.conv(P, f"{dn}.first_conv_layers.{l}", out, norm=True, cond=conds[:, 2 * l], relu=True, train=train,
-                              round_out=True)
+                              round_out=True, lens=lens)
             new, r2 = self.conv(P, f"{dn}.second_conv_layers.{l}", y, shuffle=(up > 1), norm=True, cond=conds[:, 2 * l + 1],
-                                relu=True, res=out, res_mode=L.RES_UP if up > 1 else L.RES_SAME, train=train)
+                                relu=True, res=out, res_mode=L.RES_UP if up > 1 else L.RES_SAME, train=train, lens=lens)
             blocks.append((r1, r2, up))
             out = new
-        dec4, r_out = self.conv(P, f"{dn}.out_conv_layer", out, train=train)
+            if lens is not None:
+                lens = lens.up(up)
+        dec4, r_out = self.conv(P, f"{dn}.out_conv_layer", out, train=train, lens=lens)
+        if lens is not None:
+            self.tail(dec4, lens, L.TAIL_ZERO)
         if train:
             ctx.update(in_rec=r_in, aff=aff, blocks=blocks, out_rec=r_out, conds=conds, emb=emb)
         return dec4, ctx

@@ -8,14 +8,45 @@ the batched entry point BASELINE config 5 measures.
 """
 from __future__ import annotations
 
+import collections
 import os
 import pickle
+from typing import List, Sequence, Tuple
 
 import torch
 import torch.nn.functional as F
 
+from .mcd import min_frames
 from .model import AE
 from .utils import cc, local_device
+
+# Inferencer.inference_padded: pairs per padded batch, and the graphs of padded shapes kept (least recently used evicted)
+PADDED_BATCH_MAX = 64
+PADDED_GRAPHS = 64
+
+
+def padded_extent(T: int) -> int:
+    """The grid extent a padded batch whose longest utterance has T frames gets: the next multiple of 32 up to 256
+    frames, of 64 up to 1024, of 128 beyond -- eleven extents (128 ... 640) cover 100 to 600 frames."""
+    step = 32 if T <= 256 else 64 if T <= 1024 else 128
+    return -(-T // step) * step
+
+
+def padded_batches(src_lens: Sequence[int], ref_lens: Sequence[int], batch_max: int = PADDED_BATCH_MAX
+                   ) -> List[Tuple[List[int], int, int, int]]:
+    """[(pair indices, T, T_c, B)]: pairs sorted by (source frames, reference frames, index), cut into runs of
+    batch_max, each padded to the padded_extent of its longest source and reference and to a power-of-two B."""
+    if len(src_lens) != len(ref_lens):
+        raise ValueError("padded_batches: src_lens and ref_lens must have the same length")
+    if batch_max < 1:
+        raise ValueError("padded_batches: batch_max must be >= 1")
+    order = sorted(range(len(src_lens)), key=lambda i: (int(src_lens[i]), int(ref_lens[i]), i))
+    out = []
+    for f in range(0, len(order), batch_max):
+        idx = order[f:f + batch_max]
+        B = min(batch_max, 1 << (len(idx) - 1).bit_length())
+        out.append((idx, padded_extent(max(int(src_lens[i]) for i in idx)), padded_extent(max(int(ref_lens[i]) for i in idx)), B))
+    return out
 
 
 class Inferencer(object):
@@ -23,6 +54,7 @@ class Inferencer(object):
         self.config = config
         self.args = args
         self.vocoder = vocoder
+        self.padded_captures = 0     # CUDA graphs inference_padded has captured
         self.build_model()
         if getattr(args, "model", None):
             self.load_model()
@@ -109,6 +141,67 @@ class Inferencer(object):
                 out[i] = dec[j].transpose(0, 1)
         self.model.engine(xs[0].device).check_tc_status()
         return out
+
+    @torch.no_grad()
+    def inference_padded(self, xs, x_conds, batch_max: int = PADDED_BATCH_MAX):
+        """inference_ragged's lists and results, as padded batches: the pairs run as the few shapes padded_batches
+        gives, through AE.inference with per-utterance lengths; each gets its stand-alone conversion within rounding.
+        Each shape is one CUDA graph (AVC_INFER_GRAPH=1, default) with the inputs and lengths in its static device
+        buffers, so a later call on the same shapes only replays; PADDED_GRAPHS shapes are kept, least recently used
+        evicted."""
+        if len(xs) != len(x_conds):
+            raise ValueError("inference_padded: xs and x_conds must have the same length")
+        if not xs:
+            return []
+        src = [self.utt_make_frames(x)[0] for x in xs]          # [C, T_i]
+        ref = [self.utt_make_frames(c)[0] for c in x_conds]
+        min_src, min_ref = min_frames(self.config)
+        for i, (s, r) in enumerate(zip(src, ref)):
+            if s.shape[1] < min_src or r.shape[1] < min_ref:
+                raise ValueError(f"inference_padded: pair {i} has {s.shape[1]} source / {r.shape[1]} reference frames; "
+                                 f"the model needs at least {min_src} / {min_ref}")
+        dev = src[0].device
+        out = [None] * len(xs)
+        for idx, T, Tc, Bp in padded_batches([s.shape[1] for s in src], [r.shape[1] for r in ref], batch_max):
+            xb, cb, lx, lc, run = self._padded_slot(Bp, src[0].shape[0], T, ref[0].shape[0], Tc, dev)
+            lens = [(src[i].shape[1], ref[i].shape[1]) for i in idx]
+            lens += [lens[0]] * (Bp - len(idx))                 # rows past the batch repeat its first pair
+            for j, i in enumerate(idx + [idx[0]] * (Bp - len(idx))):
+                xb[j, :, :lens[j][0]].copy_(src[i])
+                cb[j, :, :lens[j][1]].copy_(ref[i])
+            hl = torch.tensor(lens, dtype=torch.int32)
+            lx.copy_(hl[:, 0])
+            lc.copy_(hl[:, 1])
+            dec = run()
+            for j, i in enumerate(idx):
+                out[i] = dec[j, :, :8 * -(-lens[j][0] // 8)].transpose(0, 1)
+        self.model.engine(dev).check_tc_status()
+        return out
+
+    def _padded_slot(self, B, C, T, Cc, Tc, dev):
+        """(x, x_cond, lengths, cond_lengths, convert) of one padded shape: static buffers and a CUDA-graph replay
+        (captured on first use) or, with AVC_INFER_GRAPH=0, an eager AE.inference."""
+        graph_on = os.environ.get("AVC_INFER_GRAPH", "1") == "1"
+        key = (B, C, T, Cc, Tc, str(dev), self._param_version())
+        graphs = self.__dict__.setdefault("_padded_graphs", collections.OrderedDict())
+        if graph_on and key in graphs:
+            graphs.move_to_end(key)
+            return graphs[key]
+        xb, cb = torch.zeros(B, C, T, device=dev), torch.zeros(B, Cc, Tc, device=dev)
+        lx, lc = (torch.full((B,), n, dtype=torch.int32, device=dev) for n in (T, Tc))
+        slot = (xb, cb, lx, lc, lambda: self.model.inference(xb, cb, lengths=lx, cond_lengths=lc))
+        if not graph_on:
+            return slot
+        slot[4]()                          # eager once: weight packs, allocator warm-up, argument checks
+        torch.cuda.synchronize(dev)
+        graph = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(graph, capture_error_mode="thread_local"):
+            out = slot[4]()
+        self.padded_captures += 1
+        while len(graphs) >= PADDED_GRAPHS:
+            graphs.popitem(last=False)
+        graphs[key] = (xb, cb, lx, lc, lambda: (graph.replay(), out.clone())[1])
+        return graphs[key]
 
     @torch.no_grad()
     def inference_one_utterance(self, x, x_cond):

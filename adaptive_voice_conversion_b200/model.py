@@ -19,6 +19,7 @@ model on CPU tensors raises.
 from __future__ import annotations
 
 import os
+import types
 
 from typing import Dict, List, Optional
 
@@ -26,7 +27,7 @@ import torch
 import torch.nn as nn
 
 from . import _lib as L
-from .engine import A4, Engine
+from .engine import A4, Engine, Lengths, varlen_extent
 
 
 def _bank_kernel_sizes(bank_size: int, bank_scale: int) -> List[int]:
@@ -104,6 +105,34 @@ def _check_input(x: torch.Tensor, what: str) -> torch.Tensor:
     if x.dtype != torch.float32 or x.dim() != 3:
         raise L.AvcError(f"{what}: expected float32 [B, C, T], got {x.dtype} {tuple(x.shape)}")
     return x.contiguous()
+
+
+def _check_lengths(lengths: Optional[torch.Tensor], x: torch.Tensor, min_len: int, what: str) -> torch.Tensor:
+    """lengths of a padded batch x [B, C, T] as int32 [B] on x's device (None: all T); AvcError on a wrong type, shape
+    or range.  Device values are not read during a graph capture (inference_padded checks them on the host)."""
+    B, _, T = x.shape
+    if lengths is None:
+        return torch.full((B,), T, dtype=torch.int32, device=x.device)
+    if not isinstance(lengths, torch.Tensor) or lengths.dtype == torch.bool or lengths.is_floating_point() or lengths.is_complex():
+        raise L.AvcError(f"{what}: expected an integer tensor, got {getattr(lengths, 'dtype', type(lengths).__name__)}")
+    if lengths.dim() != 1 or lengths.shape[0] != B:
+        raise L.AvcError(f"{what}: expected shape [{B}] (the batch size), got {tuple(lengths.shape)}")
+    if lengths.device.type == "cuda" and lengths.device != x.device:
+        raise L.AvcError(f"{what}: on {lengths.device}, the batch on {x.device}")
+    if not (lengths.is_cuda and torch.cuda.is_current_stream_capturing()):
+        v = lengths.cpu()
+        lo, hi = int(v.min()), int(v.max())
+        if lo < min_len or hi > T:
+            raise L.AvcError(f"{what}: lengths must lie in [{min_len}, {T}] (the shortest input the model accepts, the "
+                             f"batch's extent); got min {lo}, max {hi}")
+    return lengths.to(device=x.device, dtype=torch.int32)
+
+
+def _pad_time(x: torch.Tensor, Te: int) -> torch.Tensor:
+    """x [B, C, T] in the first T frames of a [B, C, Te] buffer (the later frames are never read for a valid output)."""
+    xp = x.new_empty(x.shape[0], x.shape[1], Te)
+    xp[:, :, :x.shape[2]].copy_(x)
+    return xp
 
 
 class _StackFn(torch.autograd.Function):
@@ -255,9 +284,12 @@ class AE(nn.Module):
         return flat
 
     # ---- the reference API
-    def forward(self, x: torch.Tensor, *, eps: Optional[torch.Tensor] = None):
+    def forward(self, x: torch.Tensor, *, eps: Optional[torch.Tensor] = None, lengths: Optional[torch.Tensor] = None):
         """AE.forward (model.py:380-385).  ``eps`` (keyword-only extension) injects the
-        N(0,1) draw for parity tests; by default it is drawn from the device generator."""
+        N(0,1) draw for parity tests; by default it is drawn from the device generator.  Training runs on fixed
+        segments: ``lengths`` (padded batches) raise."""
+        if lengths is not None:
+            raise L.AvcError("AE.forward: padded batches (lengths) are inference-only; training runs on fixed segments")
         x = _check_input(x, "AE.forward(x)")
         emb = _SpeakerFn.apply(self, x, *self._params("speaker_encoder."))
         mu, log_sigma = _ContentFn.apply(self, x, *self._params("content_encoder."))
@@ -266,10 +298,25 @@ class AE(nn.Module):
         dec = _DecoderFn.apply(self, mu, log_sigma, eps, emb, *self._params("decoder."))
         return mu, log_sigma, emb, dec
 
-    def inference(self, x: torch.Tensor, x_cond: torch.Tensor):
-        """AE.inference (model.py:387-391): content mean of x, speaker of x_cond."""
+    def inference(self, x: torch.Tensor, x_cond: torch.Tensor, *, lengths: Optional[torch.Tensor] = None,
+                  cond_lengths: Optional[torch.Tensor] = None):
+        """AE.inference (model.py:387-391): content mean of x, speaker of x_cond.
+
+        lengths / cond_lengths (keyword-only extension): a padded batch.  x [B, C, T] holds lengths[b] valid frames of
+        sample b, x_cond [B, C, T_c] cond_lengths[b] (integer [B] tensors on the host or the device; one of them None =
+        every sample full length).  Frames past a sample's length are ignored, whatever they hold.  Returns dec
+        [B, C, 8 ceil(T/8)] whose dec[b, :, :8 ceil(lengths[b]/8)] is the conversion of the unpadded pair and whose
+        later frames are exactly 0.  Lengths below mcd.min_frames or above the extent raise before any launch."""
         x = _check_input(x, "AE.inference(x)")
         x_cond = _check_input(x_cond, "AE.inference(x_cond)")
+        if lengths is not None or cond_lengths is not None:
+            if x.shape[0] != x_cond.shape[0]:
+                raise L.AvcError(f"AE.inference: x has {x.shape[0]} samples, x_cond {x_cond.shape[0]}")
+            min_src, min_ref = self._min_frames()
+            lx = _check_lengths(lengths, x, min_src, "AE.inference(lengths)")
+            lc = _check_lengths(cond_lengths, x_cond, min_ref, "AE.inference(cond_lengths)")
+            with torch.no_grad():
+                return self._inference_padded(x, x_cond, lx, lc)
         with torch.no_grad():
             side = self._side_stream(x.device)
             if side is None:
@@ -298,7 +345,46 @@ class AE(nn.Module):
             st[dev] = torch.cuda.Stream(dev)
         return st[dev]
 
-    def get_speaker_embeddings(self, x: torch.Tensor):
-        """AE.get_speaker_embeddings (model.py:393-395)."""
+    def get_speaker_embeddings(self, x: torch.Tensor, *, lengths: Optional[torch.Tensor] = None):
+        """AE.get_speaker_embeddings (model.py:393-395).  lengths: a padded batch, as in inference (no gradient)."""
         x = _check_input(x, "AE.get_speaker_embeddings(x)")
+        if lengths is not None:
+            lx = _check_lengths(lengths, x, self._min_frames()[1], "AE.get_speaker_embeddings(lengths)")
+            with torch.no_grad():
+                eng, P = self._eval_stack("speaker_encoder.", x.device)
+                return eng.speaker_fwd(P, _pad_time(x, varlen_extent(self.config, x.shape[2], source=False)), False,
+                                       lens=Lengths(lx))[0]
         return _SpeakerFn.apply(self, x, *self._params("speaker_encoder."))
+
+    # ---- padded batches
+    def _min_frames(self):
+        from .mcd import min_frames
+        return min_frames(self.config)
+
+    def _eval_stack(self, prefix, dev):
+        """(engine, parameters) of one stack for an inference call outside autograd (the padded path)."""
+        return _StackFn._begin(types.SimpleNamespace(), self, prefix, self._params(prefix), False)
+
+    def _inference_padded(self, x, x_cond, lx, lc):
+        B, Cc, T = x.shape
+        xp = _pad_time(x, varlen_extent(self.config, T, source=True))
+        cp = _pad_time(x_cond, varlen_extent(self.config, x_cond.shape[2], source=False))
+        dev = x.device
+        side = self._side_stream(dev)
+        main = torch.cuda.current_stream(dev)
+        if side is not None:   # the speaker branch on a second stream, as in the unpadded call
+            side.wait_stream(main)
+        with torch.cuda.stream(side if side is not None else main):
+            eng, P = self._eval_stack("speaker_encoder.", dev)
+            emb, _ = eng.speaker_fwd(P, cp, False, lens=Lengths(lc))
+        eng, P = self._eval_stack("content_encoder.", dev)
+        mu4, ls4, ctx = eng.content_fwd(P, xp, False, lens=Lengths(lx))
+        _, _, z4 = eng.reparam_fwd(mu4, ls4, None, want_planar=False)
+        if side is not None:
+            main.wait_stream(side)
+            if not torch.cuda.is_current_stream_capturing():
+                emb.record_stream(main)
+        eng, P = self._eval_stack("decoder.", dev)
+        dec4, _ = eng.decoder_fwd(P, z4, emb, False, lens=ctx["lens"])
+        To = 8 * -(-T // 8)
+        return eng.unpack_a4(dec4)[:, :, :To].contiguous()

@@ -258,6 +258,33 @@ int avc_bias_grad_groups(const float* dc, int64_t bstride, float* const* dbias_t
 int avc_time_mean_fwd(const float* a4, int64_t bstride, float* out /*[B][C]*/, int B, int C, int T, void* stream);
 int avc_time_mean_bwd(const float* dout /*[B][C]*/, float* da4, int64_t bstride, int B, int C, int T, void* stream);
 
+/* Padded batches of different-length utterances (AE.inference with lengths; norm.cu, small_ops.cu).  `lengths` is a DEVICE
+ * int32 [B] array; at a layer, sample b holds L_b = ceil(lengths[b] / len_div) * len_mul valid frames (len_div: the
+ * product of the strides above the layer, len_mul: of the upsamplings) and every later frame is padding, whatever it
+ * holds.  The caller keeps L_b <= T.
+ *
+ * avc_norm_apply_varlen: avc_norm_apply_fwd with the statistics over each sample's L_b conv outputs (2 L_b normalized
+ * frames after a pixel shuffle), corrected two-pass form; writes out's first L_b (2 L_b) frames of each sample and
+ * nothing past them.  L_b counts d->save_c's frames (before the shuffle).  AdaIN, ReLU, AVC_F_ROUND_OUT and the SAME /
+ * UP / POOL residuals as in avc_norm_apply_fwd; a POOL residual's input holds ceil(lengths[b] / (len_div / 2)) *
+ * len_mul valid frames (len_div even) and its odd last frame is divided by 1.  mask must be null. */
+int avc_norm_apply_varlen(const avc_conv_desc* d, const int32_t* lengths, int len_div, int len_mul, void* stream);
+/* avc_time_mean_fwd over each sample's L_b frames. */
+int avc_time_mean_varlen_fwd(const float* a4, int64_t bstride, float* out /*[B][C]*/, int B, int C, int T,
+                             const int32_t* lengths, int len_div, int len_mul, void* stream);
+/* Rewrites, in place, frames of an A4 tensor (or a channel range of one: C channels of T frames, samples bstride floats
+ * apart) just past each sample's L_b:
+ *   AVC_TAIL_REFLECT   x[L_b + j] = x[L_b - 2 - j] for j < n (and L_b + j < T): the reflect padding F.pad applies to the
+ *                      sample alone, for a conv that reads n = pad_right frames past its input (needs L_b > n);
+ *   AVC_TAIL_REPLICATE x[L_b] = x[L_b - 1] when L_b is odd (and < T), so that a POOL residual's 0.5 (a + b) at the
+ *                      sample's last output gives a, as avg_pool1d(ceil_mode=True) does; n is ignored;
+ *   AVC_TAIL_ZERO      x[t] = 0 for L_b <= t < T; n is ignored. */
+#define AVC_TAIL_REFLECT 0
+#define AVC_TAIL_REPLICATE 1
+#define AVC_TAIL_ZERO 2
+int avc_varlen_tail(float* a4, int64_t bstride, int B, int C, int T, const int32_t* lengths, int len_div, int len_mul,
+                    int mode, int n, void* stream);
+
 /* nn.Linear (+ReLU, + residual): y_act = act(x W^T + b); out = y_act + res.
  * (model.py:252-263 dense blocks, :276 output layer, :342-343 AdaIN affine layers) */
 typedef struct avc_linear_desc {
