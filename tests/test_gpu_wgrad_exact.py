@@ -38,6 +38,8 @@ from dataclasses import dataclass
 import pytest
 import torch
 
+from _layer_ref import tf32_rna  # noqa: F401  (cvt.rna.tf32.f32 on the bit pattern; also imported from here by _small_ref)
+
 pytestmark = pytest.mark.gpu
 
 TOL = {"tc": 2e-6, "acc": 2e-6, "simt": 1e-6}
@@ -208,12 +210,6 @@ def make_desc(case, x, dc, dw):
 
 
 # ------------------------------------------------------------------ reference
-def tf32_rna(x):
-    """cvt.rna.tf32.f32: round to nearest (ties away from zero) at 10 mantissa bits."""
-    b = x.contiguous().view(torch.int32)
-    return ((b + 0x1000) & -0x2000).view(torch.float32)
-
-
 def tf32_trunc(x):
     """The top 19 bits of the fp32 pattern (sign, exponent, 10 mantissa bits): truncation toward zero."""
     return (x.contiguous().view(torch.int32) & -0x2000).view(torch.float32)
