@@ -207,6 +207,19 @@ class DtwDesc(C.Structure):
                 ("pairs", _fp), ("x", _fp), ("y", _fp), ("out", _fp)]
 
 
+SPK_MAX_N, SPK_MAX_DIMS, SPK_STATE_BYTES = 32768, 2048, 65536
+
+
+class EerResult(C.Structure):
+    _fields_ = [("eer", C.c_double), ("threshold", C.c_double), ("frr", C.c_double), ("far", C.c_double),
+                ("n_target", C.c_int64), ("n_nontarget", C.c_int64)]
+
+
+class SpkGroupDesc(C.Structure):
+    _fields_ = [("m", C.c_int32), ("n", C.c_int32), ("dims", C.c_int32), ("reserved", C.c_int32),
+                ("queries", _fp), ("q_labels", _fp), ("q_exclude", _fp), ("set", _fp), ("labels", _fp), ("out", _fp)]
+
+
 SN_ITERATE, SN_FIXED = 0, 1
 SN_MAX_ITEMS, SN_MAX_H, SN_MAX_W = 64, 4096, 4096
 
@@ -273,6 +286,10 @@ PROTOTYPES = {
     "avc_mel_moments_merge": (_i, [_p, _p, C.c_int32, C.c_int32, _p, _p, _p, _p, _p]),
     "avc_mel_cepstrum": (_i, [C.POINTER(CepstrumDesc), _p]),
     "avc_dtw": (_i, [C.POINTER(DtwDesc), _p]),
+    "avc_time_stats_varlen": (_i, [_p, _p, _i, _i, _i, _p, _p]),
+    "avc_spk_eer_workspace_bytes": (_i64, [_i]),
+    "avc_spk_eer": (_i, [_p, _p, _i, _i, _p, _i64, _p, _p]),
+    "avc_spk_group_mean": (_i, [C.POINTER(SpkGroupDesc), _p]),
     "avc_spectral_norm_scratch_floats": (_i64, [_i, _i]),
     "avc_spectral_norm": (_i, [_p, _i, _i, _i, _i, _p, _p]),
     "avc_spectral_norm_bwd": (_i, [_p, _i, _i, _i, _p, _p]),

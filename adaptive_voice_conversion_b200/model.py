@@ -356,6 +356,19 @@ class AE(nn.Module):
                                        lens=Lengths(lx))[0]
         return _SpeakerFn.apply(self, x, *self._params("speaker_encoder."))
 
+    def get_content_means(self, x: torch.Tensor, *, lengths: torch.Tensor):
+        """(mu [B, c_out, T_lat], latent lengths int32 [B]) of a padded batch x [B, C, T]: the content encoder's mean
+        head as the padded AE.inference computes it (no gradient); mu[b, :, :latent[b]] is sample b's, later frames are
+        padding."""
+        x = _check_input(x, "AE.get_content_means(x)")
+        lx = _check_lengths(lengths, x, self._min_frames()[0], "AE.get_content_means(lengths)")
+        with torch.no_grad():
+            eng, P = self._eval_stack("content_encoder.", x.device)
+            xp = _pad_time(x, varlen_extent(self.config, x.shape[2], source=True))
+            mu4, _, ctx = eng.content_fwd(P, xp, False, lens=Lengths(lx))
+            lat = ctx["lens"]
+            return eng.unpack_a4(mu4), ((lat.t + (lat.div - 1)) // lat.div * lat.mul).to(torch.int32)
+
     # ---- padded batches
     def _min_frames(self):
         from .mcd import min_frames

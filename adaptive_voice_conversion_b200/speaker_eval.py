@@ -1,0 +1,353 @@
+"""Speaker measures of a held-out set: how well the speaker embedding, the content code and the input mel separate
+speakers (verification EER), and whether a conversion carries the target speaker's identity (speaker similarity).
+
+Utterances: the whole utterances of ``<set>.pkl`` (attr-normalised [T, n_mels]; ``frame_size`` 1 only) in sorted key
+order, the speaker from ``evaluate.speaker_of``.  An utterance shorter than max(min_frames) (``mcd.min_frames``: 17
+frames for the shipped config) is dropped from all three representations and counted in ``n_short``, so the three
+EERs cover the same trials.
+
+Representations, one vector per utterance, the model in eval mode, in padded batches (``inference.padded_batches``):
+  * ``speaker``: ``AE.get_speaker_embeddings(x, lengths=)`` (c_out of the speaker encoder, 128);
+  * ``content``: statistics pooling of the content encoder's mean head mu over the utterance's valid latent frames
+    (``AE.get_content_means``, the padded path ``AE.inference`` runs): 2 c_out (256);
+  * ``mel``: the same pooling of the normalised input mel itself (2 n_mels): the baseline.
+InstanceNorm removes each channel's mean and variance, which is why the pooling keeps both.
+
+Pooling (``avc_time_stats_varlen``), per channel over the L valid frames, in float64 adding in ascending t:
+mean = (sum x) / L, then var = (sum (x - mean)^2) / L, std = sqrt(var); the vector is [means | stds], each rounded once
+to float32.
+
+Score: s(a, b) = dot(a, b) / (sqrt(|a|^2) sqrt(|b|^2)) of the float32 vectors promoted to float64, sums over d in
+ascending order, every multiply, add, sqrt and divide rounded on its own; s = 0 when either norm is 0.  So s(a, b) ==
+s(b, a) bit for bit and a permuted set gives the same scores.
+
+EER: the trials are all unordered pairs i < j, target trials when both utterances share a speaker.  FRR(t) =
+#{target < t} / n_target, FAR(t) = #{non-target >= t} / n_nontarget; over t in {all scores} U {+inf}, ``eer`` = min
+max(FRR, FAR) and ``threshold`` the smallest t reaching it, with ``frr`` and ``far`` there (no interpolation).  ``eer``
+and the rest are None when either count is 0.  Scores and the threshold search run on the GPU (``avc_spk_eer``, by
+counting: radix selection over the scores' order-preserving keys).
+
+Conversion pairs: ``rng = random.Random(seed)``; for every utterance u in sorted order whose speaker has at least two
+utterances in the set, the reference r is ``rng.choice`` over the sorted such utterances of the other speakers.  A pair
+is then dropped and counted in ``n_short`` when u is not embedded (shorter than max(min_frames)), r is shorter than the
+reference minimum, or u's or r's speaker has no other embedded utterance (both means below need one).  The draws do not
+depend on the lengths.  With
+``max_pairs > 0`` and more pairs than that, ``sorted(rng.sample(range(n), max_pairs))`` of them are kept.
+
+Each pair is converted with ``AE.inference(x, x_cond, lengths=, cond_lengths=)`` in padded batches; ``dec`` cropped to
+u's T frames is embedded y by the padded speaker path.  With emb(v) the speaker embedding of utterance v:
+  * ``sim_target`` = mean of s(y, emb(v)) over r's speaker's utterances v != r;
+  * ``sim_source`` = mean of s(y, emb(v)) over u's speaker's utterances v != u;
+  * ``success`` = [sim_target > sim_source];
+  * ``sim_target_source`` = sim_target of the unconverted source emb(u): the baseline, as mcd_source is for MCD.
+Means over utterances are float64 added in index order (``avc_spk_group_mean``); a set reports the means of the four
+values over its pairs (float64, pair order), ``n``, ``n_short`` and the same means per target speaker.
+
+The speaker encoder that embeds y is the model's own: these similarities compare checkpoints of this project, not an
+independent verifier's judgement.  The ``speaker`` EER on real recordings, in the same report, shows how far that
+encoder can be trusted.
+"""
+from __future__ import annotations
+
+import ctypes as C
+import random
+from typing import Dict, List, Mapping, Sequence
+
+import numpy as np
+import torch
+
+from . import _lib as L
+from .evaluate import speaker_of
+from .inference import padded_batches
+from .mcd import min_frames
+
+REPRESENTATIONS = ("speaker", "content", "mel")
+
+
+# ------------------------------------------------------------------ conversion pairs
+class _Others:
+    """The sorted utterances of `utts` outside [a, b) (one speaker's run), as a sequence for rng.choice."""
+
+    def __init__(self, utts, a, b):
+        self.utts, self.a, self.b = utts, a, b
+
+    def __len__(self):
+        return len(self.utts) - (self.b - self.a)
+
+    def __getitem__(self, i):
+        if not 0 <= i < len(self):
+            raise IndexError(i)
+        return self.utts[i if i < self.a else i + self.b - self.a]
+
+
+def conversion_pairs(utts: Sequence[str], lengths: Mapping[str, int], seed: int = 0, max_pairs: int = 0,
+                     min_src: int = 1, min_ref: int = 1, min_set: int = 1):
+    """([(source, reference)], n_short) of the utterance keys `utts` of a set, as the module docstring defines;
+    lengths[u] = frames of u, min_set = the frames an utterance needs to be embedded."""
+    utts = sorted(utts)
+    count: Dict[str, int] = {}
+    for u in utts:
+        count[speaker_of(u)] = count.get(speaker_of(u), 0) + 1
+    qual = [u for u in utts if count[speaker_of(u)] >= 2]
+    run: Dict[str, List[int]] = {}          # a speaker's utterances are one run of the sorted keys
+    for i, u in enumerate(qual):
+        run.setdefault(speaker_of(u), [i, i])[1] = i + 1
+    embedded: Dict[str, int] = {}
+    for u in utts:
+        if lengths[u] >= min_set:
+            embedded[speaker_of(u)] = embedded.get(speaker_of(u), 0) + 1
+
+    def others_embedded(v):
+        return embedded.get(speaker_of(v), 0) - (lengths[v] >= min_set) > 0
+
+    rng = random.Random(seed)
+    out, n_short = [], 0
+    for u in qual:
+        a, b = run[speaker_of(u)]
+        if b - a == len(qual):
+            break                           # a single speaker qualifies: no pair at all
+        r = rng.choice(_Others(qual, a, b))
+        if lengths[u] < min_src or lengths[r] < min_ref or not others_embedded(u) or not others_embedded(r):
+            n_short += 1
+            continue
+        out.append((u, r))
+    if max_pairs > 0 and len(out) > max_pairs:
+        out = [out[i] for i in sorted(rng.sample(range(len(out)), max_pairs))]
+    return out, n_short
+
+
+# ------------------------------------------------------------------ the three kernels
+def _stream(dev):
+    return C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+
+
+def _lengths(lengths, B, dev) -> torch.Tensor:
+    if isinstance(lengths, torch.Tensor):
+        if lengths.dtype == torch.bool or lengths.is_floating_point() or lengths.is_complex():
+            raise ValueError(f"lengths must be integers (got {lengths.dtype})")
+        lengths = lengths.to(dev)
+    else:
+        lengths = torch.as_tensor(np.asarray(lengths, np.int64), device=dev)
+    if lengths.dim() != 1 or lengths.shape[0] != B:
+        raise ValueError(f"lengths has shape {tuple(lengths.shape)}; expected [{B}]")
+    return lengths
+
+
+def time_stats(x: torch.Tensor, lengths) -> torch.Tensor:
+    """[B, 2C] float32 (device): per-channel mean then std (ddof 0) of each sample's first lengths[b] frames of a
+    padded batch x [B, C, T] (float32 on a CUDA device), one launch.  Frames past a length are never read."""
+    if not isinstance(x, torch.Tensor) or x.dim() != 3 or x.dtype != torch.float32 or not x.is_cuda or min(x.shape) < 1:
+        raise ValueError(f"time_stats: x is {getattr(x, 'dtype', type(x).__name__)} {tuple(getattr(x, 'shape', ()))}; "
+                         f"expected float32 [B, C, T >= 1] on a CUDA device")
+    B, Cc, T = x.shape
+    lens = _lengths(lengths, B, x.device)
+    lo, hi = int(lens.min()), int(lens.max())
+    if lo < 1 or hi > T:
+        raise ValueError(f"time_stats: lengths must lie in [1, {T}] (got min {lo}, max {hi})")
+    x = x.contiguous()
+    lens = lens.to(torch.int32)
+    out = torch.empty(B, 2 * Cc, device=x.device)
+    L.check(L.load().avc_time_stats_varlen(x.data_ptr(), out.data_ptr(), B, Cc, T, lens.data_ptr(), _stream(x.device)),
+            "avc_time_stats_varlen")
+    return out
+
+
+def _check_vectors(v, what: str, n_max: int = L.SPK_MAX_N):
+    if not isinstance(v, torch.Tensor) or v.dim() != 2 or v.dtype != torch.float32 or not v.is_cuda:
+        raise ValueError(f"{what}: expected float32 [N, D] on a CUDA device (got {getattr(v, 'dtype', type(v).__name__)} "
+                         f"{tuple(getattr(v, 'shape', ()))})")
+    n, d = v.shape
+    if not 1 <= n <= n_max:
+        raise ValueError(f"{what}: {n} vectors; 1 to {n_max} are supported")
+    if not 1 <= d <= L.SPK_MAX_DIMS:
+        raise ValueError(f"{what}: {d} dimensions; 1 to {L.SPK_MAX_DIMS} are supported")
+    if not bool(torch.isfinite(v).all()):
+        raise ValueError(f"{what}: the vectors must be finite")
+    return v.contiguous()
+
+
+def _labels(labels, n, dev, what):
+    lab = torch.as_tensor(np.asarray(labels), device=dev) if not isinstance(labels, torch.Tensor) else labels.to(dev)
+    if lab.dim() != 1 or lab.shape[0] != n or lab.dtype == torch.bool or lab.is_floating_point() or lab.is_complex():
+        raise ValueError(f"{what}: expected {n} integer labels (got {lab.dtype} {tuple(lab.shape)})")
+    if lab.numel() and (int(lab.min()) < -2 ** 31 or int(lab.max()) >= 2 ** 31):
+        raise ValueError(f"{what}: labels must fit in int32")
+    return lab.to(torch.int32).contiguous()
+
+
+def eer_workspace(n: int, device) -> torch.Tensor:
+    """A workspace for avc_spk_eer over n vectors (uint8, 256-byte aligned by the caching allocator)."""
+    nbytes = int(L.load().avc_spk_eer_workspace_bytes(int(n)))
+    if nbytes < 0:
+        raise ValueError(f"eer: {n} vectors; 1 to {L.SPK_MAX_N} are supported")
+    return torch.empty(nbytes, dtype=torch.uint8, device=device)
+
+
+def eer(vecs: torch.Tensor, labels, workspace: torch.Tensor = None) -> dict:
+    """{eer, threshold, frr, far, n_target, n_nontarget} of every pair of the rows of vecs [N, D] (float32, CUDA) as
+    trials, target when labels (N integers) agree; the module docstring gives the definition.  eer, threshold, frr and
+    far are None when either count is 0.  `workspace` (eer_workspace(N)) keeps the scores for trial_scores."""
+    vecs = _check_vectors(vecs, "eer")
+    n, d = vecs.shape
+    dev = vecs.device
+    lab = _labels(labels, n, dev, "eer")
+    ws = eer_workspace(n, dev) if workspace is None else workspace
+    need = int(L.load().avc_spk_eer_workspace_bytes(n))
+    if ws.dtype != torch.uint8 or ws.device != dev or ws.numel() < need or ws.data_ptr() % 256:
+        raise ValueError(f"eer: the workspace must be a 256-byte aligned uint8 tensor of at least {need} bytes on {dev}")
+    res = torch.empty(C.sizeof(L.EerResult), dtype=torch.uint8, device=dev)
+    L.check(L.load().avc_spk_eer(vecs.data_ptr(), lab.data_ptr(), n, d, ws.data_ptr(), ws.numel(), res.data_ptr(),
+                                 _stream(dev)), "avc_spk_eer")
+    r = L.EerResult.from_buffer_copy(bytes(res.cpu().numpy()))
+    null = r.n_target == 0 or r.n_nontarget == 0
+    out = {k: None if null else float(getattr(r, k)) for k in ("eer", "threshold", "frr", "far")}
+    out.update(n_target=int(r.n_target), n_nontarget=int(r.n_nontarget))
+    return out
+
+
+def trial_scores(workspace: torch.Tensor, n: int) -> np.ndarray:
+    """float64 [n, n] (host): s(i, j) at [i][j] for i < j, read from the keys avc_spk_eer left in `workspace`; NaN
+    elsewhere."""
+    nt = -(-n // 64)
+    off = L.SPK_STATE_BYTES + -(-8 * n // 256) * 256
+    keys = workspace[off:off + nt * (nt + 1) // 2 * 4096 * 8].cpu().numpy().view(np.uint64).reshape(-1, 64, 64)
+    neg = keys >> np.uint64(63) == 0
+    bits = np.where(neg, ~keys, keys & np.uint64(0x7FFFFFFFFFFFFFFF))
+    tiles = bits.view(np.float64)
+    full = np.full((nt * 64, nt * 64), np.nan)
+    for tj in range(nt):
+        for ti in range(tj + 1):
+            full[ti * 64:(ti + 1) * 64, tj * 64:(tj + 1) * 64] = tiles[tj * (tj + 1) // 2 + ti]
+    full = full[:n, :n]
+    full[np.tril_indices(n)] = np.nan
+    return full
+
+
+def group_means(queries: torch.Tensor, q_labels, q_exclude, vecs: torch.Tensor, labels) -> torch.Tensor:
+    """float64 [M] (device): for each query m, the mean of s(queries[m], vecs[v]) over the v with labels[v] ==
+    q_labels[m] and v != q_exclude[m] (-1: none), added in ascending v; NaN when there is none.  One launch."""
+    queries = _check_vectors(queries, "group_means(queries)", n_max=2 ** 31 - 1)
+    vecs = _check_vectors(vecs, "group_means(vecs)")
+    if queries.shape[1] != vecs.shape[1] or queries.device != vecs.device:
+        raise ValueError(f"group_means: queries {tuple(queries.shape)} on {queries.device}, vectors {tuple(vecs.shape)} "
+                         f"on {vecs.device}; the dimensions and devices must agree")
+    (m, d), n, dev = queries.shape, vecs.shape[0], vecs.device
+    ql = _labels(q_labels, m, dev, "group_means(q_labels)")
+    qe = _labels(q_exclude, m, dev, "group_means(q_exclude)")
+    lab = _labels(labels, n, dev, "group_means(labels)")
+    out = torch.empty(m, dtype=torch.float64, device=dev)
+    desc = L.SpkGroupDesc(m=m, n=n, dims=d, queries=queries.data_ptr(), q_labels=ql.data_ptr(), q_exclude=qe.data_ptr(),
+                          set=vecs.data_ptr(), labels=lab.data_ptr(), out=out.data_ptr())
+    L.check(L.load().avc_spk_group_mean(C.byref(desc), _stream(dev)), "avc_spk_group_mean")
+    return out
+
+
+# ------------------------------------------------------------------ representations and conversions
+def _batch(mels, idx, T, dev):
+    x = torch.zeros(len(idx), int(mels[idx[0]].shape[1]), T, device=dev)
+    for j, i in enumerate(idx):
+        x[j, :, :mels[i].shape[0]].copy_(mels[i].t())
+    return x, torch.tensor([int(mels[i].shape[0]) for i in idx], dtype=torch.int32, device=dev)
+
+
+def representations(model, mels: Sequence[torch.Tensor]) -> Dict[str, torch.Tensor]:
+    """{speaker, content, mel}: [N, D] float32 (device) of the attr-normalised mels [T_i, n_mels] (device tensors, each
+    at least max(min_frames) long), in padded batches.  The model must be in eval mode."""
+    dev = mels[0].device
+    lens = [int(m.shape[0]) for m in mels]
+    out = {k: [None] * len(mels) for k in REPRESENTATIONS}
+    for idx, T, _, _ in padded_batches(lens, lens):
+        x, lx = _batch(mels, idx, T, dev)
+        emb = model.get_speaker_embeddings(x, lengths=lx)
+        mu, lat = model.get_content_means(x, lengths=lx)
+        rows = {"speaker": emb, "content": time_stats(mu, lat), "mel": time_stats(x, lx)}
+        for k, v in rows.items():
+            for j, i in enumerate(idx):
+                out[k][i] = v[j]
+    return {k: torch.stack(v) for k, v in out.items()}
+
+
+def converted_embeddings(model, sources: Sequence[torch.Tensor], refs: Sequence[torch.Tensor]) -> torch.Tensor:
+    """[P, c_out] float32 (device): the speaker embedding of each conversion of sources[i] (cropped to its T frames)
+    with the reference refs[i], in padded batches of AE.inference.  The model must be in eval mode."""
+    dev = sources[0].device
+    out = [None] * len(sources)
+    for idx, T, Tc, _ in padded_batches([int(s.shape[0]) for s in sources], [int(r.shape[0]) for r in refs]):
+        x, lx = _batch(sources, idx, T, dev)
+        c, lc = _batch(refs, idx, Tc, dev)
+        dec = model.inference(x, c, lengths=lx, cond_lengths=lc)
+        emb = model.get_speaker_embeddings(dec, lengths=lx)
+        for j, i in enumerate(idx):
+            out[i] = emb[j]
+    return torch.stack(out)
+
+
+def _means(rows: np.ndarray) -> Dict[str, float]:
+    """The four columns' means (added sequentially in row order) and n of a float64 [n][4] array."""
+    s = np.cumsum(rows, axis=0)[-1] / len(rows)
+    return {"sim_target": float(s[0]), "sim_source": float(s[1]), "success": float(s[2]),
+            "sim_target_source": float(s[3]), "n": len(rows)}
+
+
+def evaluate_speakers(model, data: Mapping[str, np.ndarray], seed: int = 0, max_pairs: int = 0, device=None,
+                      per_pair: bool = False) -> dict:
+    """Speaker measures of `model` (an AE) on one set: data = {utterance key: attr-normalised [T, n_mels]} (the set's
+    pickle).  Returns {"eer": {"speaker", "content", "mel": {eer, threshold, frr, far, n_target, n_nontarget}},
+    "n_utts", "n_short", "conversion": {"sim_target", "sim_source", "success", "sim_target_source" (when n > 0), "n",
+    "n_short", "speakers": {target speaker: the four means and n}}}; per_pair adds conversion["pairs"]: [[source,
+    reference, sim_target, sim_source, success, sim_target_source], ...].  The module docstring gives the definitions."""
+    cfg = model.config
+    if int(cfg["data_loader"]["frame_size"]) != 1:
+        raise ValueError(f"speaker evaluation supports data_loader.frame_size 1 only (got {cfg['data_loader']['frame_size']})")
+    dev = torch.device(device) if device is not None else next(model.parameters()).device
+    min_src, min_ref = min_frames(cfg)
+    min_set = max(min_src, min_ref)
+    lengths = {u: len(v) for u, v in data.items()}
+    utts = [u for u in sorted(data) if lengths[u] >= min_set]
+    pairs, n_short_pairs = conversion_pairs(list(data), lengths, seed, max_pairs, min_set, min_ref, min_set)
+    used = sorted(set(utts) | {u for p in pairs for u in p})
+    mels = {u: torch.from_numpy(np.ascontiguousarray(data[u], np.float32)).to(dev) for u in used}
+    speakers = sorted({speaker_of(u) for u in utts})
+    label = {s: i for i, s in enumerate(speakers)}
+    labels = [label[speaker_of(u)] for u in utts]
+    res = {"eer": {}, "n_utts": len(utts), "n_short": len(data) - len(utts)}
+    was_training = model.training
+    model.eval()
+    try:
+        if utts:
+            reps = representations(model, [mels[u] for u in utts])
+            for k in REPRESENTATIONS:
+                res["eer"][k] = eer(reps[k], labels)
+        else:
+            res["eer"] = {k: {"eer": None, "threshold": None, "frr": None, "far": None, "n_target": 0,
+                              "n_nontarget": 0} for k in REPRESENTATIONS}
+        conv = {"n": len(pairs), "n_short": n_short_pairs}
+        if pairs:
+            y = converted_embeddings(model, [mels[u] for u, _ in pairs], [mels[r] for _, r in pairs])
+            index = {u: i for i, u in enumerate(utts)}
+            emb = reps["speaker"]
+            tgt = [label[speaker_of(r)] for _, r in pairs]
+            src = [label[speaker_of(u)] for u, _ in pairs]
+            ex_r = [index.get(r, -1) for _, r in pairs]
+            ex_u = [index.get(u, -1) for u, _ in pairs]
+            both = group_means(torch.cat([y, y, emb[torch.tensor(ex_u, device=dev)]]), tgt + src + tgt,
+                               ex_r + ex_u + ex_r, emb, labels).cpu().numpy()
+            P = len(pairs)
+            st, ss, sts = both[:P], both[P:2 * P], both[2 * P:]
+            vals = np.stack([st, ss, (st > ss).astype(np.float64), sts], axis=1)
+            conv.update(_means(vals))
+            groups: Dict[str, List[int]] = {}
+            for i, (_, r) in enumerate(pairs):
+                groups.setdefault(speaker_of(r), []).append(i)
+            conv["speakers"] = {s: _means(vals[rows]) for s, rows in groups.items()}
+            if per_pair:
+                conv["pairs"] = [[u, r, float(v[0]), float(v[1]), bool(v[2]), float(v[3])] for (u, r), v in zip(pairs, vals)]
+        else:
+            conv["speakers"] = {}
+            if per_pair:
+                conv["pairs"] = []
+        model.engine(dev).check_tc_status()
+    finally:
+        model.train(was_training)
+    res["conversion"] = conv
+    return res

@@ -2,12 +2,17 @@
 data directory (adaptive_voice_conversion_b200/evaluate.py gives the definition).
 
     python evaluate.py -c config.yaml -m model.ckpt -d data/ [-eval_sets in_test,out_test] [-o eval.json]
-                       [-mcd -transcripts VCTK-Corpus/txt [-attr data/attr.pkl] [-mcd_dims 24] [-max_pairs 0] [-seed 0]]
+                       [-mcd -transcripts VCTK-Corpus/txt [-attr data/attr.pkl] [-mcd_dims 24]] [-spk]
+                       [-max_pairs 0] [-seed 0]
 
 The checkpoint is loaded strictly (reference checkpoints too, and the `sn: True` layout).  Each set's losses are
 printed; -o writes them with the per-speaker means as JSON.  -mcd also measures conversion itself: the mel-cepstral
 distortion after DTW between speaker A's utterance converted to speaker B and B's recording of the same sentence
 (adaptive_voice_conversion_b200/mcd.py gives the definition), one more line per set and an "mcd" entry per set in -o.
+-spk measures speakers: the verification EER of the speaker embedding, the pooled content code and the pooled input
+mel, and the speaker similarity of conversions to the target speaker's other utterances
+(adaptive_voice_conversion_b200/speaker_eval.py gives the definitions), two more lines per set and a "spk" entry per
+set in -o.
 """
 import json
 import os
@@ -33,8 +38,10 @@ def main(argv=None):
     p.add_argument("-transcripts", default=None, help="directory searched for <id>.txt / <id>.normalized.txt (-mcd)")
     p.add_argument("-attr", default=None, help="mel statistics (default <data_dir>/attr.pkl) (-mcd)")
     p.add_argument("-mcd_dims", type=int, default=24, help="cepstral coefficients c_1..c_D (-mcd)")
-    p.add_argument("-max_pairs", type=int, default=0, help="keep at most this many triplets per set, 0 = all (-mcd)")
-    p.add_argument("-seed", type=int, default=0, help="seed of the reference choice and the sampling (-mcd)")
+    p.add_argument("-spk", action="store_true", help="also measure speaker EERs and the speaker similarity of conversions")
+    p.add_argument("-max_pairs", type=int, default=0,
+                   help="keep at most this many triplets (-mcd) and conversion pairs (-spk) per set, 0 = all")
+    p.add_argument("-seed", type=int, default=0, help="seed of the reference choice and the sampling (-mcd, -spk)")
     args = p.parse_args(argv)
     if args.mcd and not args.transcripts:
         p.error("-mcd needs -transcripts DIR")
@@ -60,6 +67,20 @@ def main(argv=None):
             means = f" mcd={m['mcd']:.4f} mcd_source={m['mcd_source']:.4f}" if m["n"] else ""
             print(f"{s}: mcd n={m['n']} n_short={m['n_short']}{means} (dims {m['dims']}, "
                   f"{len(m['speakers'])} target speakers)")
+    if args.spk:
+        from adaptive_voice_conversion_b200.speaker_eval import evaluate_speakers
+        for s in res:
+            with open(os.path.join(args.data_dir, f"{s}.pkl"), "rb") as f:
+                data = pickle.load(f)
+            r = evaluate_speakers(model, data, seed=args.seed, max_pairs=args.max_pairs, device=dev)
+            res[s]["spk"] = r
+            e = r["eer"]
+            eers = " ".join(f"{k}=" + ("n/a" if e[k]["eer"] is None else f"{e[k]['eer']:.4f}") for k in ("speaker", "content", "mel"))
+            print(f"{s}: spk eer {eers} (n_utts={r['n_utts']} n_short={r['n_short']})")
+            c = r["conversion"]
+            means = (f" sim_target={c['sim_target']:.4f} sim_source={c['sim_source']:.4f} success={c['success']:.4f} "
+                     f"sim_target_source={c['sim_target_source']:.4f}") if c["n"] else ""
+            print(f"{s}: spk conversion n={c['n']} n_short={c['n_short']}{means} ({len(c['speakers'])} target speakers)")
     if args.output:
         with open(args.output, "w") as f:
             json.dump(res, f, indent=1)

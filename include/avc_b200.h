@@ -603,6 +603,58 @@ typedef struct avc_dtw_desc {
 } avc_dtw_desc;
 int avc_dtw(const avc_dtw_desc* d, void* stream);
 
+/* ---- Speaker measures (csrc/spk.cu, speaker_eval.py).  No allocation, no synchronisation, no atomics on floats;
+ * every float64 operation below is rounded on its own (no fused multiply-add).
+ *
+ * avc_time_stats_varlen: statistics pooling of a padded batch x[B][C][T] (planar fp32) over each sample's L_b =
+ * lengths[b] frames (DEVICE int32 [B]); frames past L_b are never read.  In float64, ascending t:
+ *   mean = (sum_t x) / L_b,   var = (sum_t (x - mean)^2) / L_b,   std = sqrt(var)
+ *   out[b][c] = (float)mean,  out[b][C + c] = (float)std     (out [B][2C])
+ * A sample with L_b < 1 or L_b > T gets NaN.  AVC_ERR_INVALID for null pointers or non-positive sizes.
+ *
+ * avc_spk_eer: every unordered pair i < j of the n vectors vecs[n][dims] is a trial, a target trial when labels[i] ==
+ * labels[j] (DEVICE int32 [n]).  Its score, from the float32 values promoted to float64 and sums in ascending d:
+ *   s(a, b) = dot(a, b) / (sqrt(|a|^2) sqrt(|b|^2)),  s = 0 when either norm is 0;  s(a, b) == s(b, a) bit for bit.
+ * With FRR(t) = #{target < t} / n_target and FAR(t) = #{non-target >= t} / n_nontarget over the candidate thresholds
+ * t in {every score} U {+inf}: threshold = the smallest t minimising max(FRR, FAR); frr, far at it (float64
+ * quotients of the exact counts), eer = max(frr, far).  n_target / n_nontarget count the trials; when either is 0,
+ * eer, threshold, frr and far are NaN.  The result is written to the DEVICE struct `out` and does not depend on the
+ * order of the vectors.  Vectors must be finite.  workspace (DEVICE, 256-byte aligned) holds at least
+ * avc_spk_eer_workspace_bytes(n) bytes: AVC_SPK_STATE_BYTES of search state, then rnorm[n] = sqrt(|v_i|^2) (float64,
+ * padded to 256 bytes), then the scores of the 64 x 64 tiles (ti <= tj) of the trial matrix: tile (ti, tj) at index
+ * tj (tj + 1) / 2 + ti holds key(s(64 ti + r, 64 tj + c)) at [r][c] (uint64), key(s) = bits(s) | 2^63 for s >= +0
+ * and ~bits(s) for s < 0 (order-preserving; entries outside i < j < n are unspecified).  A fixed sequence of 40
+ * launches, no host synchronisation: the call can be captured in a CUDA graph.  avc_spk_eer_workspace_bytes returns
+ * -1 outside 1 <= n <= AVC_SPK_MAX_N.
+ * AVC_ERR_INVALID for null pointers, non-positive sizes, a short or misaligned workspace; AVC_ERR_UNSUPPORTED for
+ * n > AVC_SPK_MAX_N or dims > AVC_SPK_MAX_DIMS.
+ *
+ * avc_spk_group_mean: for every query m < m_count (queries[m][dims], q_labels[m], q_exclude[m]): out[m] = the float64
+ * mean of s(queries[m], set[v]) over the v < n with labels[v] == q_labels[m] and v != q_exclude[m], the scores added
+ * in ascending v, NaN when there is no such v.  All arrays on the DEVICE.  AVC_ERR_INVALID for null pointers or
+ * non-positive sizes; AVC_ERR_UNSUPPORTED for n > AVC_SPK_MAX_N or dims > AVC_SPK_MAX_DIMS. */
+#define AVC_SPK_MAX_N 32768
+#define AVC_SPK_MAX_DIMS 2048
+#define AVC_SPK_STATE_BYTES 65536
+typedef struct avc_eer_result {
+  double eer, threshold, frr, far;
+  int64_t n_target, n_nontarget;
+} avc_eer_result;
+int avc_time_stats_varlen(const float* x, float* out, int B, int C, int T, const int32_t* lengths, void* stream);
+int64_t avc_spk_eer_workspace_bytes(int n);
+int avc_spk_eer(const float* vecs, const int32_t* labels, int n, int dims, void* workspace, int64_t workspace_bytes,
+                avc_eer_result* out, void* stream);
+typedef struct avc_spk_group_desc {
+  int32_t m, n, dims, reserved;
+  const float* queries;     /* [m][dims] */
+  const int32_t* q_labels;  /* [m] */
+  const int32_t* q_exclude; /* [m]: an index into the set, or any value outside [0, n) for none */
+  const float* set;         /* [n][dims] */
+  const int32_t* labels;    /* [n] */
+  double* out;              /* [m] */
+} avc_spk_group_desc;
+int avc_spk_group_mean(const avc_spk_group_desc* d, void* stream);
+
 /* ---- Spectral norm of the decoder weights (csrc/spectral_norm.cu): torch.nn.utils.spectral_norm with
  * n_power_iterations=1, eps=1e-12, dim=0, for a DEVICE-resident table of n layers.  W = weight viewed as [h][w]
  * (nn.Conv1d: h = Cout, w = Cin*K; nn.Linear: [out][in]); normalize(x) = x / max(||x||, eps).
