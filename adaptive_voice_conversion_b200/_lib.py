@@ -259,6 +259,7 @@ PROTOTYPES = {
     "avc_time_mean_bwd": (_i, [_p, _p, _i64, _i, _i, _i, _p]),
     "avc_norm_apply_varlen": (_i, [C.POINTER(ConvDesc), _p, _i, _i, _p]),
     "avc_time_mean_varlen_fwd": (_i, [_p, _i64, _p, _i, _i, _i, _p, _i, _i, _p]),
+    "avc_time_mean_grouped_fwd": (_i, [_p, _i64, _p, _i, _i, _i, _p, _i, _i, _p, _i, _p]),
     "avc_varlen_tail": (_i, [_p, _i64, _i, _i, _i, _p, _i, _i, _i, _i, _p]),
     "avc_linear_fwd": (_i, [C.POINTER(LinearDesc), _p]),
     "avc_linear_bwd": (_i, [C.POINTER(LinearDesc), _p]),
@@ -290,6 +291,7 @@ PROTOTYPES = {
     "avc_spk_eer_workspace_bytes": (_i64, [_i]),
     "avc_spk_eer": (_i, [_p, _p, _i, _i, _p, _i64, _p, _p]),
     "avc_spk_group_mean": (_i, [C.POINTER(SpkGroupDesc), _p]),
+    "avc_spk_group_mean_multi": (_i, [C.POINTER(SpkGroupDesc), _i, _p]),
     "avc_spectral_norm_scratch_floats": (_i64, [_i, _i]),
     "avc_spectral_norm": (_i, [_p, _i, _i, _i, _i, _p, _p]),
     "avc_spectral_norm_bwd": (_i, [_p, _i, _i, _i, _p, _p]),

@@ -73,6 +73,18 @@ __global__ void unpack_a4_kernel(const float* __restrict__ a4, int64_t bstride, 
 }
 
 // ------------------------------------------------------------------ mean over time
+// The float32 sums over frames [0, L) of channel quad q of one sample (a: its first float): lane-strided, then a warp
+// reduction.  Every lane returns the sums.
+__device__ __forceinline__ float4 time_sum4(const float* __restrict__ a, int q, int T, int L, int lane) {
+  float4 s = zero4();
+  for (int t = lane; t < L; t += 32) {
+    const float4 v = ldg4(a + ((int64_t)q * T + t) * 4);
+    s.x += v.x; s.y += v.y; s.z += v.z; s.w += v.w;
+  }
+  s.x = warp_sum(s.x); s.y = warp_sum(s.y); s.z = warp_sum(s.z); s.w = warp_sum(s.w);
+  return s;
+}
+
 // lengths non-null (a padded batch): sample b's mean over its first ceil(lengths[b] / div) * mul frames
 __global__ void time_mean_fwd_kernel(const float* __restrict__ a4, int64_t bstride, float* __restrict__ out, int B, int C, int T,
                                      const int32_t* __restrict__ lengths, int div, int mul) {
@@ -81,15 +93,38 @@ __global__ void time_mean_fwd_kernel(const float* __restrict__ a4, int64_t bstri
   if (warp >= B * Cq) return;
   const int b = warp / Cq, q = warp - b * Cq;
   const int Lb = lengths ? min((__ldg(lengths + b) + div - 1) / div * mul, T) : T;
-  float4 s = zero4();
-  for (int t = lane; t < Lb; t += 32) {
-    const float4 v = ldg4(a4 + (int64_t)b * bstride + ((int64_t)q * T + t) * 4);
-    s.x += v.x; s.y += v.y; s.z += v.z; s.w += v.w;
-  }
-  s.x = warp_sum(s.x); s.y = warp_sum(s.y); s.z = warp_sum(s.z); s.w = warp_sum(s.w);
+  const float4 s = time_sum4(a4 + (int64_t)b * bstride, q, T, Lb, lane);
   if (lane == 0) {
     const float inv = 1.f / (float)Lb;
     st4(out + (int64_t)b * C + q * 4, make_float4(s.x * inv, s.y * inv, s.z * inv, s.w * inv));
+  }
+}
+// Group g = rows offsets[g] .. offsets[g+1]-1: the members' sums (each as time_mean_fwd_kernel adds it) added in
+// ascending row, times 1 / (the members' frame count).  A one-member group gives time_mean_fwd_kernel's bits.
+__global__ void time_mean_grouped_kernel(const float* __restrict__ a4, int64_t bstride, float* __restrict__ out, int B, int C,
+                                         int T, const int32_t* __restrict__ lengths, int div, int mul,
+                                         const int32_t* __restrict__ offsets, int G) {
+  const int Cq = C >> 2;
+  const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+  if (warp >= G * Cq) return;
+  const int g = warp / Cq, q = warp - g * Cq;
+  // the caller validates the offsets; the clamps only keep a bad table inside the batch
+  const int m0 = max(__ldg(offsets + g), 0), m1 = min(__ldg(offsets + g + 1), B);
+  float4 acc = zero4();
+  int n = 0;
+  for (int m = m0; m < m1; ++m) {
+    const int Lm = min((__ldg(lengths + m) + div - 1) / div * mul, T);
+    const float4 s = time_sum4(a4 + (int64_t)m * bstride, q, T, Lm, lane);
+    if (m == m0) {
+      acc = s;
+    } else {
+      acc.x += s.x; acc.y += s.y; acc.z += s.z; acc.w += s.w;
+    }
+    n += Lm;
+  }
+  if (lane == 0) {
+    const float inv = 1.f / (float)n;
+    st4(out + (int64_t)g * C + q * 4, make_float4(acc.x * inv, acc.y * inv, acc.z * inv, acc.w * inv));
   }
 }
 __global__ void time_mean_bwd_kernel(const float* __restrict__ dout, float* __restrict__ da4, int64_t bstride, int B, int C, int T) {
@@ -420,6 +455,20 @@ extern "C" int avc_time_mean_varlen_fwd(const float* a4, int64_t bstride, float*
   AVC_LAUNCH(time_mean_fwd_kernel, (int)cdiv64((int64_t)B * (C / 4) * 32, 256), 256, 0, (cudaStream_t)stream, a4, bstride, out, B, C,
              T, lengths, len_div, len_mul);
   AVC_CHECK_LAUNCH("time_mean_varlen_fwd");
+  return AVC_OK;
+}
+extern "C" int avc_time_mean_grouped_fwd(const float* a4, int64_t bstride, float* out, int B, int C, int T, const int32_t* lengths,
+                                         int len_div, int len_mul, const int32_t* group_offsets, int G, void* stream) {
+  AVC_REQUIRE(a4 && out && lengths && group_offsets, AVC_ERR_INVALID,
+              "avc_time_mean_grouped_fwd: null pointer (a4 %p, out %p, lengths %p, group_offsets %p)", (const void*)a4,
+              (const void*)out, (const void*)lengths, (const void*)group_offsets);
+  AVC_REQUIRE(B > 0 && C > 0 && C % 4 == 0 && T > 0 && len_div >= 1 && len_mul >= 1, AVC_ERR_INVALID,
+              "avc_time_mean_grouped_fwd: bad sizes (B %d, C %d (a multiple of 4), T %d, len_div %d, len_mul %d)", B, C, T,
+              len_div, len_mul);
+  AVC_REQUIRE(G >= 1 && G <= B, AVC_ERR_INVALID, "avc_time_mean_grouped_fwd: G %d must lie in [1, B = %d]", G, B);
+  AVC_LAUNCH(time_mean_grouped_kernel, (int)cdiv64((int64_t)G * (C / 4) * 32, 256), 256, 0, (cudaStream_t)stream, a4, bstride,
+             out, B, C, T, lengths, len_div, len_mul, group_offsets, G);
+  AVC_CHECK_LAUNCH("time_mean_grouped_fwd");
   return AVC_OK;
 }
 extern "C" int avc_time_mean_bwd(const float* dout, float* da4, int64_t bstride, int B, int C, int T, void* stream) {

@@ -327,26 +327,33 @@ __global__ void spk_result_kernel(const SpkState* st, avc_eer_result* out) {
 }
 
 // ---------------------------------------------------------------- group means
-__global__ void __launch_bounds__(SPK_THREADS) spk_group_mean_kernel(const avc_spk_group_desc d) {
+constexpr int SPK_MAX_EXCLUDE = 64;
+
+// q_exclude read as [m][n_ex]: query m skips every v its list names (n_ex = 1: avc_spk_group_mean)
+__global__ void __launch_bounds__(SPK_THREADS) spk_group_mean_kernel(const avc_spk_group_desc d, int n_ex) {
   extern __shared__ double qv[];   // [dims]
   __shared__ double sc[SPK_THREADS];
   __shared__ int ok[SPK_THREADS];
+  __shared__ int exl[SPK_MAX_EXCLUDE];
   __shared__ double rq;
   const int m = blockIdx.x, D = d.dims;
   for (int k = threadIdx.x; k < D; k += SPK_THREADS) qv[k] = (double)__ldg(d.queries + (int64_t)m * D + k);
+  if (threadIdx.x < n_ex) exl[threadIdx.x] = __ldg(d.q_exclude + (int64_t)m * n_ex + threadIdx.x);
   __syncthreads();
   if (threadIdx.x == 0) {
     double acc = 0.0;
     for (int k = 0; k < D; ++k) acc = __dadd_rn(acc, __dmul_rn(qv[k], qv[k]));
     rq = __dsqrt_rn(acc);
   }
-  const int lab = __ldg(d.q_labels + m), ex = __ldg(d.q_exclude + m);
+  const int lab = __ldg(d.q_labels + m);
   double sum = 0.0;
   long long cnt = 0;
   for (int base = 0; base < d.n; base += SPK_THREADS) {
     const int v = base + threadIdx.x;
     __syncthreads();   // rq is written; the previous chunk's scores are consumed
-    const bool take = v < d.n && v != ex && __ldg(d.labels + v) == lab;
+    bool excluded = false;
+    for (int e = 0; e < n_ex; ++e) excluded |= v == exl[e];
+    const bool take = v < d.n && !excluded && __ldg(d.labels + v) == lab;
     ok[threadIdx.x] = take;
     if (take) {
       const float* p = d.set + (int64_t)v * D;
@@ -431,19 +438,28 @@ extern "C" int avc_spk_eer(const float* vecs, const int32_t* labels, int n, int 
   return AVC_OK;
 }
 
-extern "C" int avc_spk_group_mean(const avc_spk_group_desc* d, void* stream) {
-  AVC_REQUIRE(d != nullptr, AVC_ERR_INVALID, "avc_spk_group_mean: null descriptor");
+static int group_mean(const avc_spk_group_desc* d, int n_exclude, const char* what, void* stream) {
+  AVC_REQUIRE(d != nullptr, AVC_ERR_INVALID, "%s: null descriptor", what);
   AVC_REQUIRE(d->queries != nullptr && d->q_labels != nullptr && d->q_exclude != nullptr && d->set != nullptr &&
                   d->labels != nullptr && d->out != nullptr,
-              AVC_ERR_INVALID, "avc_spk_group_mean: null pointer (queries %p, q_labels %p, q_exclude %p, set %p, "
-              "labels %p, out %p)", (const void*)d->queries, (const void*)d->q_labels, (const void*)d->q_exclude,
-              (const void*)d->set, (const void*)d->labels, (const void*)d->out);
-  AVC_REQUIRE(d->m > 0 && d->n > 0 && d->dims > 0, AVC_ERR_INVALID,
-              "avc_spk_group_mean: sizes must be positive (m %d, n %d, dims %d)", d->m, d->n, d->dims);
-  AVC_REQUIRE(d->n <= AVC_SPK_MAX_N, AVC_ERR_UNSUPPORTED, "avc_spk_group_mean: n %d > %d", d->n, AVC_SPK_MAX_N);
-  AVC_REQUIRE(d->dims <= AVC_SPK_MAX_DIMS, AVC_ERR_UNSUPPORTED, "avc_spk_group_mean: dims %d > %d", d->dims,
-              AVC_SPK_MAX_DIMS);
-  spk_group_mean_kernel<<<(unsigned)d->m, SPK_THREADS, d->dims * 8, (cudaStream_t)stream>>>(*d);
-  AVC_CHECK_LAUNCH("avc_spk_group_mean");
+              AVC_ERR_INVALID, "%s: null pointer (queries %p, q_labels %p, q_exclude %p, set %p, labels %p, out %p)", what,
+              (const void*)d->queries, (const void*)d->q_labels, (const void*)d->q_exclude, (const void*)d->set,
+              (const void*)d->labels, (const void*)d->out);
+  AVC_REQUIRE(d->m > 0 && d->n > 0 && d->dims > 0, AVC_ERR_INVALID, "%s: sizes must be positive (m %d, n %d, dims %d)",
+              what, d->m, d->n, d->dims);
+  AVC_REQUIRE(n_exclude >= 1 && n_exclude <= SPK_MAX_EXCLUDE, AVC_ERR_INVALID, "%s: n_exclude %d must lie in [1, %d]",
+              what, n_exclude, SPK_MAX_EXCLUDE);
+  AVC_REQUIRE(d->n <= AVC_SPK_MAX_N, AVC_ERR_UNSUPPORTED, "%s: n %d > %d", what, d->n, AVC_SPK_MAX_N);
+  AVC_REQUIRE(d->dims <= AVC_SPK_MAX_DIMS, AVC_ERR_UNSUPPORTED, "%s: dims %d > %d", what, d->dims, AVC_SPK_MAX_DIMS);
+  spk_group_mean_kernel<<<(unsigned)d->m, SPK_THREADS, d->dims * 8, (cudaStream_t)stream>>>(*d, n_exclude);
+  AVC_CHECK_LAUNCH(what);
   return AVC_OK;
+}
+
+extern "C" int avc_spk_group_mean(const avc_spk_group_desc* d, void* stream) {
+  return group_mean(d, 1, "avc_spk_group_mean", stream);
+}
+
+extern "C" int avc_spk_group_mean_multi(const avc_spk_group_desc* d, int n_exclude, void* stream) {
+  return group_mean(d, n_exclude, "avc_spk_group_mean_multi", stream);
 }

@@ -850,17 +850,27 @@ class Engine:
             ctx["lens"] = lens
         return out
 
-    def speaker_fwd(self, P, x_planar: torch.Tensor, train: bool, lens: Optional[Lengths] = None):
+    def speaker_fwd(self, P, x_planar: torch.Tensor, train: bool, lens: Optional[Lengths] = None,
+                    groups: Optional[torch.Tensor] = None):
         """SpeakerEncoder.forward (model.py:265-277) -> emb [B, c_out].  lens: a padded batch (inference only): x_planar
-        holds lens.t[b] valid frames of sample b in an extent of varlen_extent(cfg, T, source=False)."""
+        holds lens.t[b] valid frames of sample b in an extent of varlen_extent(cfg, T, source=False).  groups (with lens,
+        inference only): int32 [G+1] row offsets on the device; the time mean pools each group's rows over the union of
+        their valid frames (avc_time_mean_grouped_fwd) and the dense stack runs on the G pooled rows -> emb [G, c_out]."""
+        if groups is not None and (lens is None or train):
+            raise L.AvcError("Engine.speaker_fwd: groups need lens and train=False")
         c = self.cfg["SpeakerEncoder"]
         enc = "speaker_encoder"
         ctx: dict = {}
         out = self._bank_and_in_conv(P, enc, c, x_planar, norm=False, train=train, ctx=ctx, lens=lens)
         out = self._enc_blocks(P, enc, c, out, norm=False, train=train, ctx=ctx, lens=lens)
-        B = out.B
+        B = out.B if groups is None else groups.shape[0] - 1
         pooled = self.empty(B, out.C)
-        if lens is not None:
+        if groups is not None:
+            lo = ctx.pop("lens")
+            self._ck(self.lib.avc_time_mean_grouped_fwd(out.ptr, out.bstride, pooled.data_ptr(), out.B, out.C, out.T,
+                                                        lo.t.data_ptr(), lo.div, lo.mul, groups.data_ptr(), B, self.stream),
+                     "time_mean_grouped_fwd")
+        elif lens is not None:
             lo = ctx.pop("lens")
             self._ck(self.lib.avc_time_mean_varlen_fwd(out.ptr, out.bstride, pooled.data_ptr(), B, out.C, out.T, lo.t.data_ptr(),
                                                        lo.div, lo.mul, self.stream), "time_mean_varlen_fwd")

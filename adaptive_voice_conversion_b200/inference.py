@@ -49,6 +49,46 @@ def padded_batches(src_lens: Sequence[int], ref_lens: Sequence[int], batch_max: 
     return out
 
 
+def pack_sets(set_sizes: Sequence[int], set_lens: Sequence[int], batch_max: int = PADDED_BATCH_MAX
+              ) -> List[Tuple[List[int], int]]:
+    """[(set indices, T)]: reference sets of set_sizes[g] utterances, the longest set_lens[g] frames, sorted by (longest
+    member, index) and packed greedily into padded batches of at most batch_max utterances, each set whole in one
+    batch; T = the padded_extent of the batch's longest member."""
+    if len(set_sizes) != len(set_lens):
+        raise ValueError("pack_sets: set_sizes and set_lens must have the same length")
+    for g, n in enumerate(set_sizes):
+        if not 1 <= int(n) <= batch_max:
+            raise ValueError(f"pack_sets: reference set {g} has {n} utterances; 1 to {batch_max} are supported")
+    order = sorted(range(len(set_sizes)), key=lambda g: (int(set_lens[g]), g))
+    out, cur, rows = [], [], 0
+    for g in order:
+        if rows + int(set_sizes[g]) > batch_max:
+            out.append(cur)
+            cur, rows = [], 0
+        cur.append(g)
+        rows += int(set_sizes[g])
+    if cur:
+        out.append(cur)
+    return [(idx, padded_extent(max(int(set_lens[g]) for g in idx))) for idx in out]
+
+
+def embed_reference_sets(model, sets) -> torch.Tensor:
+    """[G, c_out] (device): the pooled speaker code of each set of sets, lists of [C, T] model inputs (device tensors,
+    validated by the caller), through AE.get_speaker_embeddings(groups=) in pack_sets' padded batches."""
+    dev = sets[0][0].device
+    out = torch.empty(len(sets), model.config["SpeakerEncoder"]["c_out"], device=dev)
+    for idx, T in pack_sets([len(s) for s in sets], [max(int(r.shape[1]) for r in s) for s in sets]):
+        members = [r for g in idx for r in sets[g]]
+        x = torch.zeros(len(members), int(members[0].shape[0]), T, device=dev)
+        for j, r in enumerate(members):
+            x[j, :, :r.shape[1]].copy_(r)
+        lens = torch.tensor([int(r.shape[1]) for r in members], dtype=torch.int32)
+        offs = torch.tensor([0] + [len(sets[g]) for g in idx]).cumsum(0).to(torch.int32)
+        emb = model.get_speaker_embeddings(x, lengths=lens.to(dev), groups=offs.to(dev))
+        out.index_copy_(0, torch.tensor(idx, device=dev), emb)
+    return out
+
+
 class Inferencer(object):
     def __init__(self, config, args, vocoder=None):
         self.config = config
@@ -148,11 +188,18 @@ class Inferencer(object):
         gives, through AE.inference with per-utterance lengths; each gets its stand-alone conversion within rounding.
         Each shape is one CUDA graph (AVC_INFER_GRAPH=1, default) with the inputs and lengths in its static device
         buffers, so a later call on the same shapes only replays; PADDED_GRAPHS shapes are kept, least recently used
-        evicted."""
+        evicted.  x_conds[i] may instead be a list of references of the target speaker (every entry then a list or
+        tuple; a mix raises): the sets are embedded by embed_speakers, one list object shared by several pairs once,
+        and the pairs converted with those codes (AE.inference_from_embeddings) in the same grid."""
         if len(xs) != len(x_conds):
             raise ValueError("inference_padded: xs and x_conds must have the same length")
         if not xs:
             return []
+        sets = [isinstance(c, (list, tuple)) for c in x_conds]
+        if any(sets):
+            if not all(sets):
+                raise ValueError("inference_padded: x_conds mixes single references (tensors) and reference sets (lists)")
+            return self._inference_padded_sets(xs, x_conds, batch_max)
         src = [self.utt_make_frames(x)[0] for x in xs]          # [C, T_i]
         ref = [self.utt_make_frames(c)[0] for c in x_conds]
         min_src, min_ref = min_frames(self.config)
@@ -181,32 +228,115 @@ class Inferencer(object):
     def _padded_slot(self, B, C, T, Cc, Tc, dev):
         """(x, x_cond, lengths, cond_lengths, convert) of one padded shape: static buffers and a CUDA-graph replay
         (captured on first use) or, with AVC_INFER_GRAPH=0, an eager AE.inference."""
+        def make():
+            xb, cb = torch.zeros(B, C, T, device=dev), torch.zeros(B, Cc, Tc, device=dev)
+            lx, lc = (torch.full((B,), n, dtype=torch.int32, device=dev) for n in (T, Tc))
+            return (xb, cb, lx, lc), lambda: self.model.inference(xb, cb, lengths=lx, cond_lengths=lc)
+        return self._graph_slot((B, C, T, Cc, Tc, str(dev), self._param_version()), make)
+
+    def _emb_slot(self, B, C, T, dev):
+        """(x, emb, lengths, convert) of one padded shape converted with given speaker codes (AE.inference_from_embeddings),
+        as _padded_slot."""
+        def make():
+            xb = torch.zeros(B, C, T, device=dev)
+            eb = torch.zeros(B, self.config["SpeakerEncoder"]["c_out"], device=dev)
+            lx = torch.full((B,), T, dtype=torch.int32, device=dev)
+            return (xb, eb, lx), lambda: self.model.inference_from_embeddings(xb, eb, lengths=lx)
+        return self._graph_slot(("emb", B, C, T, str(dev), self._param_version()), make)
+
+    def _graph_slot(self, key, make):
+        """(*static buffers, convert) for `key`: make() gives the buffers and the eager call; with AVC_INFER_GRAPH=1 the
+        call is captured once into a CUDA graph replayed on those buffers, PADDED_GRAPHS graphs kept (LRU)."""
         graph_on = os.environ.get("AVC_INFER_GRAPH", "1") == "1"
-        key = (B, C, T, Cc, Tc, str(dev), self._param_version())
         graphs = self.__dict__.setdefault("_padded_graphs", collections.OrderedDict())
         if graph_on and key in graphs:
             graphs.move_to_end(key)
             return graphs[key]
-        xb, cb = torch.zeros(B, C, T, device=dev), torch.zeros(B, Cc, Tc, device=dev)
-        lx, lc = (torch.full((B,), n, dtype=torch.int32, device=dev) for n in (T, Tc))
-        slot = (xb, cb, lx, lc, lambda: self.model.inference(xb, cb, lengths=lx, cond_lengths=lc))
+        bufs, call = make()
         if not graph_on:
-            return slot
-        slot[4]()                          # eager once: weight packs, allocator warm-up, argument checks
-        torch.cuda.synchronize(dev)
+            return (*bufs, call)
+        call()                             # eager once: weight packs, allocator warm-up, argument checks
+        torch.cuda.synchronize(bufs[0].device)
         graph = torch.cuda.CUDAGraph()
         with torch.cuda.graph(graph, capture_error_mode="thread_local"):
-            out = slot[4]()
+            out = call()
         self.padded_captures += 1
         while len(graphs) >= PADDED_GRAPHS:
             graphs.popitem(last=False)
-        graphs[key] = (xb, cb, lx, lc, lambda: (graph.replay(), out.clone())[1])
+        graphs[key] = (*bufs, lambda: (graph.replay(), out.clone())[1])
         return graphs[key]
+
+    def _ref_frames(self, ref_sets, what):
+        """[[C, T] per reference] per set of ref_sets (lists of [T, n_mels] mels); ValueError naming a bad set."""
+        _, min_ref = min_frames(self.config)
+        out = []
+        for g, refs in enumerate(ref_sets):
+            if not isinstance(refs, (list, tuple)) or not refs:
+                raise ValueError(f"{what}: reference set {g} must be a non-empty list of tensors")
+            if len(refs) > PADDED_BATCH_MAX:
+                raise ValueError(f"{what}: reference set {g} has {len(refs)} references; at most {PADDED_BATCH_MAX} "
+                                 f"are supported")
+            frames = [self.utt_make_frames(r)[0] for r in refs]
+            for j, r in enumerate(frames):
+                if r.shape[1] < min_ref:
+                    raise ValueError(f"{what}: reference {j} of set {g} has {r.shape[1]} frames; the model needs at "
+                                     f"least {min_ref}")
+            out.append(frames)
+        return out
+
+    @torch.no_grad()
+    def embed_speakers(self, ref_sets):
+        """[G, c_out] speaker codes (device) of G reference sets, each a list of [T, n_mels] normalised mels of one
+        speaker on the device: AE.get_speaker_embeddings(groups=) over padded batches (pack_sets: at most
+        PADDED_BATCH_MAX references, each set whole in one batch).  A set of more than PADDED_BATCH_MAX references or
+        a reference shorter than the model accepts raises ValueError naming it."""
+        frames = self._ref_frames(ref_sets, "embed_speakers")
+        if not frames:
+            raise ValueError("embed_speakers: no reference sets")
+        out = embed_reference_sets(self.model, frames)
+        self.model.engine(out.device).check_tc_status()
+        return out
+
+    def _inference_padded_sets(self, xs, ref_sets, batch_max):
+        """inference_padded with a reference set per pair: a set object shared by several pairs is embedded once
+        (embed_speakers), then the sources run in padded_batches' grid through AE.inference_from_embeddings, one CUDA
+        graph per shape with the codes in a static buffer."""
+        slot_of, uniq = {}, []
+        for refs in ref_sets:
+            if id(refs) not in slot_of:
+                slot_of[id(refs)] = len(uniq)
+                uniq.append(refs)
+        src = [self.utt_make_frames(x)[0] for x in xs]
+        min_src, _ = min_frames(self.config)
+        for i, s in enumerate(src):
+            if s.shape[1] < min_src:
+                raise ValueError(f"inference_padded: pair {i} has {s.shape[1]} source frames; the model needs at least "
+                                 f"{min_src}")
+        emb = self.embed_speakers(uniq)
+        which = [slot_of[id(refs)] for refs in ref_sets]
+        dev = src[0].device
+        out = [None] * len(xs)
+        for idx, T, _, Bp in padded_batches([s.shape[1] for s in src], [0] * len(src), batch_max):
+            xb, eb, lx, run = self._emb_slot(Bp, src[0].shape[0], T, dev)
+            rows = idx + [idx[0]] * (Bp - len(idx))                # rows past the batch repeat its first pair
+            for j, i in enumerate(rows):
+                xb[j, :, :src[i].shape[1]].copy_(src[i])
+            eb.copy_(emb.index_select(0, torch.tensor([which[i] for i in rows], device=dev)))
+            lx.copy_(torch.tensor([src[i].shape[1] for i in rows], dtype=torch.int32))
+            dec = run()
+            for j, i in enumerate(idx):
+                out[i] = dec[j, :, :8 * -(-src[i].shape[1] // 8)].transpose(0, 1)
+        self.model.engine(dev).check_tc_status()
+        return out
 
     @torch.no_grad()
     def inference_one_utterance(self, x, x_cond):
-        """x, x_cond: [T, n_mels] normalised mels on the device (inference.py:62-70)."""
-        dec = self.model.inference(self.utt_make_frames(x), self.utt_make_frames(x_cond))
+        """x, x_cond: [T, n_mels] normalised mels on the device (inference.py:62-70).  x_cond may also be a list of
+        references of the target speaker: their pooled code (embed_speakers) conditions the decoder."""
+        if isinstance(x_cond, (list, tuple)):
+            dec = self.model.inference_from_embeddings(self.utt_make_frames(x), self.embed_speakers([x_cond]))
+        else:
+            dec = self.model.inference(self.utt_make_frames(x), self.utt_make_frames(x_cond))
         dec = dec.transpose(1, 2).squeeze(0).detach().cpu().numpy()
         self.model.engine(x.device).check_tc_status()
         if self.attr is not None:

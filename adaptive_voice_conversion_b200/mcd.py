@@ -25,6 +25,10 @@ with (S, L) the accumulated distance and the length of the DTW path (``avc_dtw``
 ground truth; ``mcd_source`` is the same measure between the unconverted source and the ground truth.  A set reports
 the means over its triplets (added in triplet order in float64), ``n``, ``n_short``, ``dims`` and the means per target
 speaker.  Cepstra and DTW run on the GPU (csrc/mcd.cu); both kernels give a row or a pair the same bits in any batch.
+
+Few-shot (``n_refs`` K > 1): each triplet keeps its reference and gets K - 1 more (``fewshot_triplets``, drawn from
+``random.Random(seed + 1)`` after the ``max_pairs`` subsample); ``dec = AE.inference_from_embeddings(source, code)``
+with the set's pooled code, in the same batches as K = 1.
 """
 from __future__ import annotations
 
@@ -148,6 +152,27 @@ def parallel_triplets(utts: Sequence[str], texts: Mapping[str, str], lengths: Ma
     return out, n_short
 
 
+def fewshot_triplets(trip, utts: Sequence[str], texts: Mapping[str, str], lengths: Mapping[str, int], n_refs: int,
+                     seed: int = 0, min_ref: int = 1):
+    """([(source, [reference, extra, ...], ground truth)], n_few): parallel_triplets' triplets with n_refs - 1 extra
+    references each.  rng2 = random.Random(seed + 1) draws, in triplet order, rng2.sample over the target speaker's
+    other utterances (sorted) whose text is not the group's and that have at least min_ref frames; a triplet whose
+    speaker has fewer than n_refs such utterances (the reference included) is dropped and counted in n_few."""
+    by_speaker: Dict[str, List[str]] = {}
+    for u in sorted(utts):
+        by_speaker.setdefault(speaker_of(u), []).append(u)
+    rng2 = random.Random(seed + 1)
+    out, n_few = [], 0
+    for s, r, g in trip:
+        text = texts.get(g)
+        others = [u for u in by_speaker[speaker_of(g)] if u != r and texts.get(u) != text and lengths[u] >= min_ref]
+        if len(others) + 1 < n_refs:
+            n_few += 1
+            continue
+        out.append((s, [r] + rng2.sample(others, n_refs - 1), g))
+    return out, n_few
+
+
 # ------------------------------------------------------------------ the two kernels
 def _stream(dev):
     return C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
@@ -224,10 +249,12 @@ def dtw(xs, ys):
 
 
 # ------------------------------------------------------------------ conversion and the measure
-def converted(model, sources, refs, batch_max: int = 64):
+def converted(model, sources, refs, batch_max: int = 64, codes=None):
     """Yields (indices, [dec cropped to T_i, as [T_i, n_mels]]) per batch of the pairs (sources[i], refs[i]) of
     attr-normalised device mels [T, n_mels]: pairs bucketed by their exact (T, T_ref), each bucket in eager
-    AE.inference calls of at most batch_max pairs.  The model must be in eval mode."""
+    AE.inference calls of at most batch_max pairs.  codes [P, c_out] (few-shot): the same batches through
+    AE.inference_from_embeddings with pair i's speaker code codes[i] instead of refs[i]'s.  The model must be in eval
+    mode."""
     buckets: Dict[Tuple[int, int], List[int]] = {}
     for i, (x, c) in enumerate(zip(sources, refs)):
         buckets.setdefault((int(x.shape[0]), int(c.shape[0])), []).append(i)
@@ -236,6 +263,10 @@ def converted(model, sources, refs, batch_max: int = 64):
             for f in range(0, len(idx), batch_max):
                 part = idx[f:f + batch_max]
                 xb = torch.stack([sources[i].t() for i in part]).contiguous()
+                if codes is not None:
+                    dec = model.inference_from_embeddings(xb, codes[torch.tensor(part, device=codes.device)])
+                    yield part, [dec[j, :, :T].t() for j in range(len(part))]
+                    continue
                 cb = torch.stack([refs[i].t() for i in part]).contiguous()
                 dec = model.inference(xb, cb)
                 yield part, [dec[j, :, :T].t() for j in range(len(part))]
@@ -249,24 +280,33 @@ def _means(rows: np.ndarray) -> Dict[str, float]:
 
 def evaluate_mcd(model, data: Mapping[str, np.ndarray], attr, texts: Mapping[str, str], dims: int = 24,
                  max_pairs: int = 0, seed: int = 0, hp: AudioParams = AudioParams(), device=None,
-                 per_triplet: bool = False) -> dict:
+                 per_triplet: bool = False, n_refs: int = 1) -> dict:
     """MCD-DTW of `model` (an AE) on one set: data = {utterance key: attr-normalised [T, n_mels]} (the set's pickle),
     texts = read_transcripts(...) of its keys.  Returns {"n", "n_short", "dims", "speakers": {target speaker: {"mcd",
     "mcd_source", "n"}}} with "mcd" and "mcd_source" when n > 0; per_triplet adds "triplets": [[source, reference,
-    target, mcd, mcd_source], ...].  Only the utterances the triplets use are uploaded."""
+    target, mcd, mcd_source], ...].  Only the utterances the triplets use are uploaded.
+
+    n_refs > 1 (few-shot): each triplet keeps its reference and gets n_refs - 1 more (fewshot_triplets); the source is
+    converted with the set's pooled speaker code in the batches n_refs = 1 uses.  The result then also reports
+    "n_refs" and "n_few", and a triplet row lists the references: [source, [reference, ...], target, ...]."""
     cfg = model.config
     if int(cfg["data_loader"]["frame_size"]) != 1:
         raise ValueError(f"MCD evaluation supports data_loader.frame_size 1 only (got {cfg['data_loader']['frame_size']})")
     _check_dims(dims)
+    if not 1 <= int(n_refs) <= 64:
+        raise ValueError(f"n_refs must lie in [1, 64] (got {n_refs})")
     dev = torch.device(device) if device is not None else next(model.parameters()).device
     min_src, min_ref = min_frames(cfg)
-    trip, n_short = parallel_triplets(list(data), texts, {u: len(v) for u, v in data.items()}, seed, max_pairs,
-                                      min_src, min_ref)
+    lengths = {u: len(v) for u, v in data.items()}
+    trip, n_short = parallel_triplets(list(data), texts, lengths, seed, max_pairs, min_src, min_ref)
     res = {"n": len(trip), "n_short": n_short, "dims": int(dims)}
+    if n_refs > 1:
+        trip, n_few = fewshot_triplets(trip, list(data), texts, lengths, n_refs, seed, min_ref)
+        res.update(n=len(trip), n_refs=int(n_refs), n_few=n_few)
     if not trip:
         res["speakers"] = {}
         return res
-    used = sorted({u for t in trip for u in t})
+    used = sorted({u for s, r, g in trip for u in [s, g] + (r if n_refs > 1 else [r])})
     mels = {u: torch.from_numpy(np.ascontiguousarray(data[u], np.float32)).to(dev) for u in used}
     plain = sorted({t[0] for t in trip} | {t[2] for t in trip})
     ceps = dict(zip(plain, mel_cepstrum([mels[u] for u in plain], attr, hp, dims)))
@@ -274,7 +314,12 @@ def evaluate_mcd(model, data: Mapping[str, np.ndarray], attr, texts: Mapping[str
     was_training = model.training
     model.eval()
     try:
-        for idx, decs in converted(model, [mels[s] for s, _, _ in trip], [mels[r] for _, r, _ in trip]):
+        codes = None
+        if n_refs > 1:
+            from .inference import embed_reference_sets
+            codes = embed_reference_sets(model, [[mels[u].t() for u in r] for _, r, _ in trip])
+        first = [mels[r if n_refs == 1 else r[0]] for _, r, _ in trip]
+        for idx, decs in converted(model, [mels[s] for s, _, _ in trip], first, codes=codes):
             for i, c in zip(idx, mel_cepstrum(decs, attr, hp, dims)):
                 conv[i] = c
         model.engine(dev).check_tc_status()

@@ -128,6 +128,23 @@ def _check_lengths(lengths: Optional[torch.Tensor], x: torch.Tensor, min_len: in
     return lengths.to(device=x.device, dtype=torch.int32)
 
 
+def _check_groups(groups, x: torch.Tensor, what: str) -> torch.Tensor:
+    """Row offsets [G+1] of groups of a batch x [B, C, T] as int32 on x's device: 0 first, strictly increasing, B last
+    (1 <= G <= B); AvcError otherwise.  As in _check_lengths, device values are not read during a graph capture."""
+    B = x.shape[0]
+    if not isinstance(groups, torch.Tensor) or groups.dtype == torch.bool or groups.is_floating_point() or groups.is_complex():
+        raise L.AvcError(f"{what}: expected an integer tensor, got {getattr(groups, 'dtype', type(groups).__name__)}")
+    if groups.dim() != 1 or not 2 <= groups.shape[0] <= B + 1:
+        raise L.AvcError(f"{what}: expected shape [G + 1] with 1 <= G <= {B} (the batch size), got {tuple(groups.shape)}")
+    if groups.device.type == "cuda" and groups.device != x.device:
+        raise L.AvcError(f"{what}: on {groups.device}, the batch on {x.device}")
+    if not (groups.is_cuda and torch.cuda.is_current_stream_capturing()):
+        v = groups.cpu().tolist()
+        if v[0] != 0 or v[-1] != B or any(b <= a for a, b in zip(v, v[1:])):
+            raise L.AvcError(f"{what}: offsets must start at 0, increase strictly and end at {B} (the batch size); got {v}")
+    return groups.to(device=x.device, dtype=torch.int32)
+
+
 def _pad_time(x: torch.Tensor, Te: int) -> torch.Tensor:
     """x [B, C, T] in the first T frames of a [B, C, Te] buffer (the later frames are never read for a valid output)."""
     xp = x.new_empty(x.shape[0], x.shape[1], Te)
@@ -345,16 +362,45 @@ class AE(nn.Module):
             st[dev] = torch.cuda.Stream(dev)
         return st[dev]
 
-    def get_speaker_embeddings(self, x: torch.Tensor, *, lengths: Optional[torch.Tensor] = None):
-        """AE.get_speaker_embeddings (model.py:393-395).  lengths: a padded batch, as in inference (no gradient)."""
+    def get_speaker_embeddings(self, x: torch.Tensor, *, lengths: Optional[torch.Tensor] = None,
+                               groups: Optional[torch.Tensor] = None):
+        """AE.get_speaker_embeddings (model.py:393-395).  lengths: a padded batch, as in inference (no gradient).
+
+        groups (keyword-only, no gradient): integer row offsets [G+1] (0, strictly increasing, B) cutting the batch into G
+        reference sets of one speaker; returns one code per set, [G, c_out].  The encoder's only operation across time
+        is its time mean, so a set's code pools the last conv layer over the valid frames of all its members together
+        (what the encoder computes on their concatenation, but for the conv context at the joins) before the dense
+        stack.  lengths=None with groups: every row full length.  A one-member set gives the row the call with lengths
+        gives, bit for bit."""
         x = _check_input(x, "AE.get_speaker_embeddings(x)")
-        if lengths is not None:
+        if lengths is not None or groups is not None:
             lx = _check_lengths(lengths, x, self._min_frames()[1], "AE.get_speaker_embeddings(lengths)")
+            g = None if groups is None else _check_groups(groups, x, "AE.get_speaker_embeddings(groups)")
             with torch.no_grad():
                 eng, P = self._eval_stack("speaker_encoder.", x.device)
                 return eng.speaker_fwd(P, _pad_time(x, varlen_extent(self.config, x.shape[2], source=False)), False,
-                                       lens=Lengths(lx))[0]
+                                       lens=Lengths(lx), groups=g)[0]
         return _SpeakerFn.apply(self, x, *self._params("speaker_encoder."))
+
+    def inference_from_embeddings(self, x: torch.Tensor, emb: torch.Tensor, *, lengths: Optional[torch.Tensor] = None):
+        """AE.inference with a given speaker code: content mean of x [B, C, T], decoder conditioned on emb [B, c_out]
+        (e.g. get_speaker_embeddings(..., groups=) of several references).  lengths: a padded batch, as in inference.
+        inference_from_embeddings(x, get_speaker_embeddings(c)) is inference(x, c) bit for bit, and so with lengths on
+        both sides."""
+        x = _check_input(x, "AE.inference_from_embeddings(x)")
+        c_out = self.config["SpeakerEncoder"]["c_out"]
+        if (not isinstance(emb, torch.Tensor) or emb.dtype != torch.float32 or tuple(emb.shape) != (x.shape[0], c_out)
+                or emb.device != x.device):
+            raise L.AvcError(f"AE.inference_from_embeddings(emb): expected float32 [{x.shape[0]}, {c_out}] on {x.device}, "
+                             f"got {getattr(emb, 'dtype', type(emb).__name__)} {tuple(getattr(emb, 'shape', ()))} on "
+                             f"{getattr(emb, 'device', None)}")
+        emb = emb.contiguous()
+        with torch.no_grad():
+            if lengths is not None:
+                lx = _check_lengths(lengths, x, self._min_frames()[0], "AE.inference_from_embeddings(lengths)")
+                return self._decode_padded(x, lx, emb)
+            mu, log_sigma = _ContentFn.apply(self, x, *self._params("content_encoder."))
+            return _DecoderFn.apply(self, mu, log_sigma, None, emb, *self._params("decoder."))
 
     def get_content_means(self, x: torch.Tensor, *, lengths: torch.Tensor):
         """(mu [B, c_out, T_lat], latent lengths int32 [B]) of a padded batch x [B, C, T]: the content encoder's mean
@@ -379,8 +425,6 @@ class AE(nn.Module):
         return _StackFn._begin(types.SimpleNamespace(), self, prefix, self._params(prefix), False)
 
     def _inference_padded(self, x, x_cond, lx, lc):
-        B, Cc, T = x.shape
-        xp = _pad_time(x, varlen_extent(self.config, T, source=True))
         cp = _pad_time(x_cond, varlen_extent(self.config, x_cond.shape[2], source=False))
         dev = x.device
         side = self._side_stream(dev)
@@ -390,13 +434,26 @@ class AE(nn.Module):
         with torch.cuda.stream(side if side is not None else main):
             eng, P = self._eval_stack("speaker_encoder.", dev)
             emb, _ = eng.speaker_fwd(P, cp, False, lens=Lengths(lc))
+
+        def join():
+            if side is not None:
+                main.wait_stream(side)
+                if not torch.cuda.is_current_stream_capturing():
+                    emb.record_stream(main)
+        return self._decode_padded(x, lx, emb, join)
+
+    def _decode_padded(self, x, lx, emb, join=None):
+        """The content and decoder half of the padded AE.inference: dec [B, C, 8 ceil(T/8)] of x's content mean
+        conditioned on emb.  join(), when given, runs between the content encoder and the decoder (the speaker branch's
+        stream join)."""
+        B, Cc, T = x.shape
+        xp = _pad_time(x, varlen_extent(self.config, T, source=True))
+        dev = x.device
         eng, P = self._eval_stack("content_encoder.", dev)
         mu4, ls4, ctx = eng.content_fwd(P, xp, False, lens=Lengths(lx))
         _, _, z4 = eng.reparam_fwd(mu4, ls4, None, want_planar=False)
-        if side is not None:
-            main.wait_stream(side)
-            if not torch.cuda.is_current_stream_capturing():
-                emb.record_stream(main)
+        if join is not None:
+            join()
         eng, P = self._eval_stack("decoder.", dev)
         dec4, _ = eng.decoder_fwd(P, z4, emb, False, lens=ctx["lens"])
         To = 8 * -(-T // 8)

@@ -43,6 +43,13 @@ u's T frames is embedded y by the padded speaker path.  With emb(v) the speaker 
 Means over utterances are float64 added in index order (``avc_spk_group_mean``); a set reports the means of the four
 values over its pairs (float64, pair order), ``n``, ``n_short`` and the same means per target speaker.
 
+Few-shot (``n_refs`` K > 1): the pairs above (``max_pairs`` already applied) each get K - 1 more references of r's
+speaker (``fewshot_pairs``: ``rng2 = random.Random(seed + 1)``, ``rng2.sample`` in pair order over that speaker's other
+utterances of at least the reference minimum, sorted); a pair is dropped and counted in ``n_few`` when the speaker has
+fewer than K such utterances or no embedded utterance outside the K.  u is converted with the set's pooled code
+(``AE.get_speaker_embeddings(groups=)``, then ``AE.inference_from_embeddings`` in padded batches), and ``sim_target``
+skips all K references (``avc_spk_group_mean_multi``); ``sim_source`` and ``sim_target_source`` are as with one.
+
 The speaker encoder that embeds y is the model's own: these similarities compare checkpoints of this project, not an
 independent verifier's judgement.  The ``speaker`` EER on real recordings, in the same report, shows how far that
 encoder can be trusted.
@@ -114,6 +121,32 @@ def conversion_pairs(utts: Sequence[str], lengths: Mapping[str, int], seed: int 
     if max_pairs > 0 and len(out) > max_pairs:
         out = [out[i] for i in sorted(rng.sample(range(len(out)), max_pairs))]
     return out, n_short
+
+
+def fewshot_pairs(pairs, utts: Sequence[str], lengths: Mapping[str, int], n_refs: int, seed: int = 0,
+                  min_ref: int = 1, min_set: int = 1):
+    """([(source, [reference, extra, ...])], n_few): conversion_pairs' pairs with n_refs - 1 extra references each.
+    rng2 = random.Random(seed + 1) draws, in pair order, rng2.sample over the reference's speaker's other utterances of
+    at least min_ref frames (sorted).  A pair is dropped and counted in n_few when that speaker has fewer than n_refs
+    such utterances (the reference included), or no utterance of at least min_set frames outside the drawn set (the
+    embedded utterances sim_target averages over)."""
+    by_speaker: Dict[str, List[str]] = {}
+    for u in sorted(utts):
+        by_speaker.setdefault(speaker_of(u), []).append(u)
+    rng2 = random.Random(seed + 1)
+    out, n_few = [], 0
+    for u, r in pairs:
+        spk = by_speaker[speaker_of(r)]
+        others = [v for v in spk if v != r and lengths[v] >= min_ref]
+        if len(others) + 1 < n_refs:
+            n_few += 1
+            continue
+        refs = [r] + rng2.sample(others, n_refs - 1)
+        if not any(lengths[v] >= min_set and v not in refs for v in spk):
+            n_few += 1
+            continue
+        out.append((u, refs))
+    return out, n_few
 
 
 # ------------------------------------------------------------------ the three kernels
@@ -223,9 +256,14 @@ def trial_scores(workspace: torch.Tensor, n: int) -> np.ndarray:
     return full
 
 
+SPK_MAX_EXCLUDE = 64   # avc_spk_group_mean_multi's n_exclude
+
+
 def group_means(queries: torch.Tensor, q_labels, q_exclude, vecs: torch.Tensor, labels) -> torch.Tensor:
     """float64 [M] (device): for each query m, the mean of s(queries[m], vecs[v]) over the v with labels[v] ==
-    q_labels[m] and v != q_exclude[m] (-1: none), added in ascending v; NaN when there is none.  One launch."""
+    q_labels[m] and v != q_exclude[m] (-1: none), added in ascending v; NaN when there is none.  One launch.
+    q_exclude may also be [M, n_exclude] (1 to 64 indices per query, -1 or any index outside the set: none;
+    avc_spk_group_mean_multi)."""
     queries = _check_vectors(queries, "group_means(queries)", n_max=2 ** 31 - 1)
     vecs = _check_vectors(vecs, "group_means(vecs)")
     if queries.shape[1] != vecs.shape[1] or queries.device != vecs.device:
@@ -233,12 +271,23 @@ def group_means(queries: torch.Tensor, q_labels, q_exclude, vecs: torch.Tensor, 
                          f"on {vecs.device}; the dimensions and devices must agree")
     (m, d), n, dev = queries.shape, vecs.shape[0], vecs.device
     ql = _labels(q_labels, m, dev, "group_means(q_labels)")
-    qe = _labels(q_exclude, m, dev, "group_means(q_exclude)")
+    multi = np.ndim(q_exclude) == 2 if not isinstance(q_exclude, torch.Tensor) else q_exclude.dim() == 2
+    if multi:
+        qe = torch.as_tensor(np.asarray(q_exclude), device=dev) if not isinstance(q_exclude, torch.Tensor) else q_exclude.to(dev)
+        k = qe.shape[1]
+        if qe.shape[0] != m or not 1 <= k <= SPK_MAX_EXCLUDE:
+            raise ValueError(f"group_means(q_exclude): expected [{m}, 1..{SPK_MAX_EXCLUDE}], got {tuple(qe.shape)}")
+        qe = _labels(qe.reshape(-1), m * k, dev, "group_means(q_exclude)")
+    else:
+        qe = _labels(q_exclude, m, dev, "group_means(q_exclude)")
     lab = _labels(labels, n, dev, "group_means(labels)")
     out = torch.empty(m, dtype=torch.float64, device=dev)
     desc = L.SpkGroupDesc(m=m, n=n, dims=d, queries=queries.data_ptr(), q_labels=ql.data_ptr(), q_exclude=qe.data_ptr(),
                           set=vecs.data_ptr(), labels=lab.data_ptr(), out=out.data_ptr())
-    L.check(L.load().avc_spk_group_mean(C.byref(desc), _stream(dev)), "avc_spk_group_mean")
+    if multi:
+        L.check(L.load().avc_spk_group_mean_multi(C.byref(desc), k, _stream(dev)), "avc_spk_group_mean_multi")
+    else:
+        L.check(L.load().avc_spk_group_mean(C.byref(desc), _stream(dev)), "avc_spk_group_mean")
     return out
 
 
@@ -269,9 +318,21 @@ def representations(model, mels: Sequence[torch.Tensor]) -> Dict[str, torch.Tens
 
 def converted_embeddings(model, sources: Sequence[torch.Tensor], refs: Sequence[torch.Tensor]) -> torch.Tensor:
     """[P, c_out] float32 (device): the speaker embedding of each conversion of sources[i] (cropped to its T frames)
-    with the reference refs[i], in padded batches of AE.inference.  The model must be in eval mode."""
+    with the reference refs[i], in padded batches of AE.inference.  refs[i] may instead be a list of references of
+    one speaker: the sources are then converted with the sets' pooled codes (inference.embed_reference_sets) through
+    AE.inference_from_embeddings.  The model must be in eval mode."""
     dev = sources[0].device
     out = [None] * len(sources)
+    if isinstance(refs[0], (list, tuple)):
+        from .inference import embed_reference_sets
+        codes = embed_reference_sets(model, [[r.t() for r in s] for s in refs])
+        for idx, T, _, _ in padded_batches([int(s.shape[0]) for s in sources], [0] * len(sources)):
+            x, lx = _batch(sources, idx, T, dev)
+            dec = model.inference_from_embeddings(x, codes[torch.tensor(idx, device=dev)], lengths=lx)
+            emb = model.get_speaker_embeddings(dec, lengths=lx)
+            for j, i in enumerate(idx):
+                out[i] = emb[j]
+        return torch.stack(out)
     for idx, T, Tc, _ in padded_batches([int(s.shape[0]) for s in sources], [int(r.shape[0]) for r in refs]):
         x, lx = _batch(sources, idx, T, dev)
         c, lc = _batch(refs, idx, Tc, dev)
@@ -290,22 +351,33 @@ def _means(rows: np.ndarray) -> Dict[str, float]:
 
 
 def evaluate_speakers(model, data: Mapping[str, np.ndarray], seed: int = 0, max_pairs: int = 0, device=None,
-                      per_pair: bool = False) -> dict:
+                      per_pair: bool = False, n_refs: int = 1) -> dict:
     """Speaker measures of `model` (an AE) on one set: data = {utterance key: attr-normalised [T, n_mels]} (the set's
     pickle).  Returns {"eer": {"speaker", "content", "mel": {eer, threshold, frr, far, n_target, n_nontarget}},
     "n_utts", "n_short", "conversion": {"sim_target", "sim_source", "success", "sim_target_source" (when n > 0), "n",
     "n_short", "speakers": {target speaker: the four means and n}}}; per_pair adds conversion["pairs"]: [[source,
-    reference, sim_target, sim_source, success, sim_target_source], ...].  The module docstring gives the definitions."""
+    reference, sim_target, sim_source, success, sim_target_source], ...].  The module docstring gives the definitions.
+
+    n_refs > 1 (few-shot): each pair keeps its reference and gets n_refs - 1 more (fewshot_pairs), the source is
+    converted with the set's pooled code, and sim_target skips all n_refs references; sim_source and
+    sim_target_source are as with one.  conversion then also reports "n_refs" and "n_few" (the pairs fewshot_pairs
+    dropped), and a per-pair row lists the references: [source, [reference, ...], ...]."""
     cfg = model.config
     if int(cfg["data_loader"]["frame_size"]) != 1:
         raise ValueError(f"speaker evaluation supports data_loader.frame_size 1 only (got {cfg['data_loader']['frame_size']})")
+    if not 1 <= int(n_refs) <= SPK_MAX_EXCLUDE:
+        raise ValueError(f"n_refs must lie in [1, {SPK_MAX_EXCLUDE}] (got {n_refs})")
     dev = torch.device(device) if device is not None else next(model.parameters()).device
     min_src, min_ref = min_frames(cfg)
     min_set = max(min_src, min_ref)
     lengths = {u: len(v) for u, v in data.items()}
     utts = [u for u in sorted(data) if lengths[u] >= min_set]
     pairs, n_short_pairs = conversion_pairs(list(data), lengths, seed, max_pairs, min_set, min_ref, min_set)
-    used = sorted(set(utts) | {u for p in pairs for u in p})
+    if n_refs > 1:
+        pairs, n_few = fewshot_pairs(pairs, list(data), lengths, n_refs, seed, min_ref, min_set)
+        used = sorted(set(utts) | {u for u, _ in pairs} | {r for _, refs in pairs for r in refs})
+    else:
+        used = sorted(set(utts) | {u for p in pairs for u in p})
     mels = {u: torch.from_numpy(np.ascontiguousarray(data[u], np.float32)).to(dev) for u in used}
     speakers = sorted({speaker_of(u) for u in utts})
     label = {s: i for i, s in enumerate(speakers)}
@@ -322,26 +394,39 @@ def evaluate_speakers(model, data: Mapping[str, np.ndarray], seed: int = 0, max_
             res["eer"] = {k: {"eer": None, "threshold": None, "frr": None, "far": None, "n_target": 0,
                               "n_nontarget": 0} for k in REPRESENTATIONS}
         conv = {"n": len(pairs), "n_short": n_short_pairs}
+        if n_refs > 1:
+            conv.update(n_refs=int(n_refs), n_few=n_few)
         if pairs:
-            y = converted_embeddings(model, [mels[u] for u, _ in pairs], [mels[r] for _, r in pairs])
             index = {u: i for i, u in enumerate(utts)}
             emb = reps["speaker"]
-            tgt = [label[speaker_of(r)] for _, r in pairs]
             src = [label[speaker_of(u)] for u, _ in pairs]
-            ex_r = [index.get(r, -1) for _, r in pairs]
             ex_u = [index.get(u, -1) for u, _ in pairs]
+            if n_refs > 1:
+                y = converted_embeddings(model, [mels[u] for u, _ in pairs], [[mels[r] for r in refs] for _, refs in pairs])
+                tgt = [label[speaker_of(refs[0])] for _, refs in pairs]
+                ex_r = [index.get(refs[0], -1) for _, refs in pairs]
+                # one launch: sim_target skips every reference, the other two rows exactly what n_refs = 1 skips
+                pad = [-1] * (n_refs - 1)
+                ex = ([[index.get(r, -1) for r in refs] for _, refs in pairs] + [[e] + pad for e in ex_u]
+                      + [[e] + pad for e in ex_r])
+            else:
+                y = converted_embeddings(model, [mels[u] for u, _ in pairs], [mels[r] for _, r in pairs])
+                tgt = [label[speaker_of(r)] for _, r in pairs]
+                ex_r = [index.get(r, -1) for _, r in pairs]
+                ex = ex_r + ex_u + ex_r
             both = group_means(torch.cat([y, y, emb[torch.tensor(ex_u, device=dev)]]), tgt + src + tgt,
-                               ex_r + ex_u + ex_r, emb, labels).cpu().numpy()
+                               ex, emb, labels).cpu().numpy()
             P = len(pairs)
             st, ss, sts = both[:P], both[P:2 * P], both[2 * P:]
             vals = np.stack([st, ss, (st > ss).astype(np.float64), sts], axis=1)
             conv.update(_means(vals))
             groups: Dict[str, List[int]] = {}
             for i, (_, r) in enumerate(pairs):
-                groups.setdefault(speaker_of(r), []).append(i)
+                groups.setdefault(speaker_of(r if n_refs == 1 else r[0]), []).append(i)
             conv["speakers"] = {s: _means(vals[rows]) for s, rows in groups.items()}
             if per_pair:
-                conv["pairs"] = [[u, r, float(v[0]), float(v[1]), bool(v[2]), float(v[3])] for (u, r), v in zip(pairs, vals)]
+                conv["pairs"] = [[u, list(r) if n_refs > 1 else r, float(v[0]), float(v[1]), bool(v[2]), float(v[3])]
+                                 for (u, r), v in zip(pairs, vals)]
         else:
             conv["speakers"] = {}
             if per_pair:

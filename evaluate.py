@@ -3,7 +3,7 @@ data directory (adaptive_voice_conversion_b200/evaluate.py gives the definition)
 
     python evaluate.py -c config.yaml -m model.ckpt -d data/ [-eval_sets in_test,out_test] [-o eval.json]
                        [-mcd -transcripts VCTK-Corpus/txt [-attr data/attr.pkl] [-mcd_dims 24]] [-spk]
-                       [-max_pairs 0] [-seed 0]
+                       [-max_pairs 0] [-seed 0] [-n_refs 1]
 
 The checkpoint is loaded strictly (reference checkpoints too, and the `sn: True` layout).  Each set's losses are
 printed; -o writes them with the per-speaker means as JSON.  -mcd also measures conversion itself: the mel-cepstral
@@ -13,6 +13,10 @@ distortion after DTW between speaker A's utterance converted to speaker B and B'
 mel, and the speaker similarity of conversions to the target speaker's other utterances
 (adaptive_voice_conversion_b200/speaker_eval.py gives the definitions), two more lines per set and a "spk" entry per
 set in -o.
+-n_refs K (default 1) converts with K references of the target speaker per conversion, their speaker codes pooled
+(-mcd and -spk): the first reference is drawn as with one, the K - 1 others from a second generator seeded with
+seed + 1; sim_target then skips all K.  With K > 1 each result also reports n_refs and n_few (conversions dropped for
+want of K references).
 """
 import json
 import os
@@ -42,9 +46,14 @@ def main(argv=None):
     p.add_argument("-max_pairs", type=int, default=0,
                    help="keep at most this many triplets (-mcd) and conversion pairs (-spk) per set, 0 = all")
     p.add_argument("-seed", type=int, default=0, help="seed of the reference choice and the sampling (-mcd, -spk)")
+    p.add_argument("-n_refs", type=int, default=1,
+                   help="references of the target speaker per conversion, their speaker codes pooled (-mcd, -spk)")
     args = p.parse_args(argv)
     if args.mcd and not args.transcripts:
         p.error("-mcd needs -transcripts DIR")
+    if not 1 <= args.n_refs <= 64:
+        p.error("-n_refs must lie in [1, 64]")
+    few = {} if args.n_refs == 1 else {"n_refs": args.n_refs}
     config = load_config(args.config)
     dev = local_device()
     model = AE(config).to(dev)
@@ -62,9 +71,10 @@ def main(argv=None):
             with open(os.path.join(args.data_dir, f"{s}.pkl"), "rb") as f:
                 data = pickle.load(f)
             m = evaluate_mcd(model, data, attr, read_transcripts(args.transcripts, data), dims=args.mcd_dims,
-                             max_pairs=args.max_pairs, seed=args.seed, device=dev)
+                             max_pairs=args.max_pairs, seed=args.seed, device=dev, **few)
             res[s]["mcd"] = m
             means = f" mcd={m['mcd']:.4f} mcd_source={m['mcd_source']:.4f}" if m["n"] else ""
+            means += f" n_refs={m['n_refs']} n_few={m['n_few']}" if few else ""
             print(f"{s}: mcd n={m['n']} n_short={m['n_short']}{means} (dims {m['dims']}, "
                   f"{len(m['speakers'])} target speakers)")
     if args.spk:
@@ -72,7 +82,7 @@ def main(argv=None):
         for s in res:
             with open(os.path.join(args.data_dir, f"{s}.pkl"), "rb") as f:
                 data = pickle.load(f)
-            r = evaluate_speakers(model, data, seed=args.seed, max_pairs=args.max_pairs, device=dev)
+            r = evaluate_speakers(model, data, seed=args.seed, max_pairs=args.max_pairs, device=dev, **few)
             res[s]["spk"] = r
             e = r["eer"]
             eers = " ".join(f"{k}=" + ("n/a" if e[k]["eer"] is None else f"{e[k]['eer']:.4f}") for k in ("speaker", "content", "mel"))
@@ -80,6 +90,7 @@ def main(argv=None):
             c = r["conversion"]
             means = (f" sim_target={c['sim_target']:.4f} sim_source={c['sim_source']:.4f} success={c['success']:.4f} "
                      f"sim_target_source={c['sim_target_source']:.4f}") if c["n"] else ""
+            means += f" n_refs={c['n_refs']} n_few={c['n_few']}" if few else ""
             print(f"{s}: spk conversion n={c['n']} n_short={c['n_short']}{means} ({len(c['speakers'])} target speakers)")
     if args.output:
         with open(args.output, "w") as f:

@@ -272,6 +272,16 @@ int avc_norm_apply_varlen(const avc_conv_desc* d, const int32_t* lengths, int le
 /* avc_time_mean_fwd over each sample's L_b frames. */
 int avc_time_mean_varlen_fwd(const float* a4, int64_t bstride, float* out /*[B][C]*/, int B, int C, int T,
                              const int32_t* lengths, int len_div, int len_mul, void* stream);
+/* Frame-weighted pooling over groups of samples (few-shot speaker codes): group g is the rows group_offsets[g] ..
+ * group_offsets[g+1] - 1 of the padded batch (DEVICE int32 [G+1], 0 = offsets[0] < offsets[1] < ... < offsets[G] = B,
+ * validated by the caller).  With S_m[c] member m's float32 sum over its L_m frames, added as avc_time_mean_varlen_fwd
+ * adds it: out[g][c] = (S_first + S_next + ..., in ascending row) * (1.f / (float)N_g), N_g = sum of the members' L_m
+ * -- the mean over the union of the members' valid frames.  A one-member group gives avc_time_mean_varlen_fwd's row
+ * bit for bit; frames past L_m are never read.  AVC_ERR_INVALID for null pointers, non-positive sizes, C % 4 != 0,
+ * len_div or len_mul < 1, G < 1 or G > B.  No allocation, no synchronisation, no atomics: graph-capturable. */
+int avc_time_mean_grouped_fwd(const float* a4, int64_t bstride, float* out /*[G][C]*/, int B, int C, int T,
+                              const int32_t* lengths, int len_div, int len_mul, const int32_t* group_offsets, int G,
+                              void* stream);
 /* Rewrites, in place, frames of an A4 tensor (or a channel range of one: C channels of T frames, samples bstride floats
  * apart) just past each sample's L_b:
  *   AVC_TAIL_REFLECT   x[L_b + j] = x[L_b - 2 - j] for j < n (and L_b + j < T): the reflect padding F.pad applies to the
@@ -654,6 +664,10 @@ typedef struct avc_spk_group_desc {
   double* out;              /* [m] */
 } avc_spk_group_desc;
 int avc_spk_group_mean(const avc_spk_group_desc* d, void* stream);
+/* avc_spk_group_mean with q_exclude read as [m][n_exclude]: query m skips every v its list names.  Entries outside
+ * [0, n) mean "none" and duplicates are allowed; n_exclude = 1 gives avc_spk_group_mean's bits.  AVC_ERR_INVALID also
+ * for n_exclude outside [1, 64]. */
+int avc_spk_group_mean_multi(const avc_spk_group_desc* d, int n_exclude, void* stream);
 
 /* ---- Spectral norm of the decoder weights (csrc/spectral_norm.cu): torch.nn.utils.spectral_norm with
  * n_power_iterations=1, eps=1e-12, dim=0, for a DEVICE-resident table of n layers.  W = weight viewed as [h][w]

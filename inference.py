@@ -12,12 +12,20 @@ Any of the three may instead be a .npy mel ([T, n_mels], already normalised when
 
     python inference.py -c config.yaml -m model.ckpt -s src.npy -t tgt.npy -o out.npy
 
+Few-shot: several -t files of the target speaker condition the decoder on their pooled speaker code
+(AE.get_speaker_embeddings with groups); one -t file runs the one-shot path:
+
+    python inference.py -c config.yaml -m model.ckpt -a attr.pkl -s src.wav -t tgt1.wav tgt2.wav tgt3.wav -o out.wav
+
 Many pairs in one call: -pairs FILE names one pair per line, ``source target [output_name]`` (blank lines and lines
 starting with # are skipped), and -o is the output directory:
 
     python inference.py -c config.yaml -m model.ckpt -a attr.pkl -pairs pairs.txt -o out_dir
 
-output_name defaults to ``<source stem>_to_<target stem>.wav``; a name ending in .npy saves the converted mel, any other
+The target field is one file when it names an existing file (even one whose name contains commas); otherwise it is a
+comma-separated reference set, ``a.wav,b.wav,c.wav``, whose every member must be an existing .wav or .npy.  Lines
+naming the same set share one speaker code.
+output_name defaults to ``<source stem>_to_<target stem>.wav`` (a set: its first file's stem); a name ending in .npy saves the converted mel, any other
 name gets a .wav.  The sources and targets are analysed in one batched Vocoder.wav_to_mel call (.npy mels are read
 as in the single-pair mode), converted by Inferencer.inference_padded, and the .wav outputs synthesised in one batched
 Vocoder.mel_to_wav call (-gl_iters, -gl_momentum).  A missing file, a malformed line or an utterance shorter than the
@@ -38,9 +46,17 @@ def is_wav(path):
     return str(path).lower().endswith(".wav")
 
 
+def target_field(field):
+    """A pairs file's target field: the path itself when it names an existing file (a name containing commas too),
+    otherwise a tuple of the comma-separated paths of a reference set.  The caller checks that each exists."""
+    if os.path.isfile(field) or "," not in field:
+        return field
+    return tuple(field.split(","))
+
+
 def read_pairs(path):
     """[(line number, source, target, output name)] of a pairs file; ValueError naming the line of a malformed entry
-    or a missing input."""
+    or a missing input.  target is a path, or a tuple of paths for a comma-separated reference set (target_field)."""
     out = []
     with open(path) as f:
         for n, line in enumerate(f, 1):
@@ -50,27 +66,51 @@ def read_pairs(path):
             err = lambda msg: ValueError(f"{path} line {n}: {msg}")  # noqa: E731
             if len(parts) not in (2, 3):
                 raise err(f"expected 'source target [output_name]', got {len(parts)} fields")
-            for fp in parts[:2]:
+            tgt = target_field(parts[1])
+            for fp in [parts[0]] + ([tgt] if isinstance(tgt, str) else list(tgt)):
                 if not os.path.isfile(fp) or not (is_wav(fp) or fp.lower().endswith(".npy")):
                     raise err(f"{fp} is not an existing .wav or .npy file")
             stem = lambda p: os.path.splitext(os.path.basename(p))[0]  # noqa: E731
-            name = parts[2] if len(parts) == 3 else f"{stem(parts[0])}_to_{stem(parts[1])}"
+            first = tgt if isinstance(tgt, str) else tgt[0]
+            name = parts[2] if len(parts) == 3 else f"{stem(parts[0])}_to_{stem(first)}"
             ext = os.path.splitext(name)[1].lower()
             if os.path.basename(name) != name or ext not in ("", ".wav", ".npy"):
                 raise err(f"output_name {name} must be a file name ending in .wav, .npy or nothing")
-            out.append((n, parts[0], parts[1], name if ext else name + ".wav"))
+            out.append((n, parts[0], tgt, name if ext else name + ".wav"))
     if not out:
         raise ValueError(f"{path}: no pairs")
     return out
 
 
 def check_frames(pairs, src_frames, tgt_frames, minimum):
-    """ValueError naming the line of the first pair whose source / target is shorter than (min_src, min_ref)."""
+    """ValueError naming the line of the first pair whose source / target is shorter than (min_src, min_ref).  A
+    reference set's entry in tgt_frames lists its members' frames."""
     for (n, src, tgt, _), ts, tt in zip(pairs, src_frames, tgt_frames):
         if ts < minimum[0]:
             raise ValueError(f"line {n}: source {src} has {ts} frames; the model needs at least {minimum[0]}")
-        if tt < minimum[1]:
-            raise ValueError(f"line {n}: target {tgt} has {tt} frames; the model needs at least {minimum[1]}")
+        for t, f in zip((tgt,) if isinstance(tgt, str) else tgt, (tt,) if isinstance(tgt, str) else tt):
+            if f < minimum[1]:
+                raise ValueError(f"line {n}: target {t} has {f} frames; the model needs at least {minimum[1]}")
+
+
+def convert_pairs(inf, pairs, mels):
+    """Converted mels of every pair (normalised mels by path in `mels`): the single-target lines through
+    Inferencer.inference_padded as one batch, the reference-set lines as another, lines naming the same set sharing
+    one list object (embedded once)."""
+    single = [i for i, (_, _, t, _) in enumerate(pairs) if isinstance(t, str)]
+    multi = [i for i, (_, _, t, _) in enumerate(pairs) if not isinstance(t, str)]
+    decs = [None] * len(pairs)
+    if single:
+        for i, d in zip(single, inf.inference_padded([mels[pairs[i][1]] for i in single],
+                                                     [mels[pairs[i][2]] for i in single])):
+            decs[i] = d
+    if multi:
+        sets = {}
+        for i in multi:
+            sets.setdefault(pairs[i][2], [mels[p] for p in pairs[i][2]])
+        for i, d in zip(multi, inf.inference_padded([mels[pairs[i][1]] for i in multi], [sets[pairs[i][2]] for i in multi])):
+            decs[i] = d
+    return decs
 
 
 def run_pairs(args, config):
@@ -80,7 +120,7 @@ def run_pairs(args, config):
     pairs = read_pairs(args.pairs)
     os.makedirs(args.output, exist_ok=True)
     dev = local_device()
-    files = sorted({p for _, s, t, _ in pairs for p in (s, t)})
+    files = sorted({p for _, s, t, _ in pairs for p in (s,) + ((t,) if isinstance(t, str) else t)})
     need_voc = any(is_wav(f) for f in files) or any(is_wav(name) for *_, name in pairs)
     vocoder = Vocoder(n_mels=config["SpeakerEncoder"]["c_in"] // config["data_loader"]["frame_size"],
                       hp=AudioParams(n_iter=args.gl_iters, momentum=args.gl_momentum)) if need_voc else None
@@ -90,14 +130,15 @@ def run_pairs(args, config):
         sigs = [torch.from_numpy(load_wav(f, vocoder.hp.sr)).to(dev) for f in wavs]
         mels.update((f, m) for f, (m, _) in zip(wavs, vocoder.wav_to_mel(sigs)))
     mels.update((f, torch.from_numpy(np.load(f).astype(np.float32)).to(dev)) for f in files if not is_wav(f))
-    check_frames(pairs, [mels[s].shape[0] for _, s, _, _ in pairs], [mels[t].shape[0] for _, _, t, _ in pairs],
+    check_frames(pairs, [mels[s].shape[0] for _, s, _, _ in pairs],
+                 [mels[t].shape[0] if isinstance(t, str) else [mels[p].shape[0] for p in t] for _, _, t, _ in pairs],
                  min_frames(config))
     inf = Inferencer(config=config, args=args, vocoder=vocoder)
     if inf.attr is not None:
         mean = torch.as_tensor(np.asarray(inf.attr["mean"], np.float32)).to(dev)
         std = torch.as_tensor(np.asarray(inf.attr["std"], np.float32)).to(dev)
         mels = {f: (m - mean) / std for f, m in mels.items()}
-    decs = inf.inference_padded([mels[s] for _, s, _, _ in pairs], [mels[t] for _, _, t, _ in pairs])
+    decs = convert_pairs(inf, pairs, mels)
     if inf.attr is not None:
         decs = [d * std + mean for d in decs]
     to_wav = [i for i, (*_, name) in enumerate(pairs) if is_wav(name)]
@@ -115,7 +156,8 @@ if __name__ == "__main__":
     p.add_argument("-config", "-c", help="config file path")
     p.add_argument("-model", "-m", help="model path")
     p.add_argument("-source", "-s", help="source .wav or mel .npy")
-    p.add_argument("-target", "-t", help="target .wav or mel .npy")
+    p.add_argument("-target", "-t", nargs="+",
+                   help="target .wav or mel .npy; several files of the target speaker pool their speaker code")
     p.add_argument("-output", "-o", help="output .wav or mel .npy")
     p.add_argument("-sample_rate", "-sr", default=24000, type=int)
     p.add_argument("-gl_iters", default=100, type=int, help="Griffin-Lim iterations of a .wav output")
@@ -127,8 +169,10 @@ if __name__ == "__main__":
     if args.pairs:
         run_pairs(args, config)
         raise SystemExit(0)
+    targets = args.target or [None]
+    args.target = targets[0] if len(targets) == 1 else targets
     vocoder = None
-    if any(is_wav(f) for f in (args.source, args.target, args.output)):
+    if any(is_wav(f) for f in (args.source, *targets, args.output)):
         from adaptive_voice_conversion_b200.vocoder import AudioParams, Vocoder
         vocoder = Vocoder(n_mels=config["SpeakerEncoder"]["c_in"] // config["data_loader"]["frame_size"],
                           hp=AudioParams(n_iter=args.gl_iters, momentum=args.gl_momentum))
@@ -137,11 +181,12 @@ if __name__ == "__main__":
     def read(path):
         return vocoder.get_spectrograms(path)[0] if is_wav(path) else np.load(path).astype(np.float32)
 
-    src, tgt = read(args.source), read(args.target)
+    src, tgts = read(args.source), [read(t) for t in targets]
     if inf.attr is not None:
-        src, tgt = inf.normalize(src), inf.normalize(tgt)
+        src, tgts = inf.normalize(src), [inf.normalize(t) for t in tgts]
     dev = local_device()
-    wav, mel = inf.inference_one_utterance(torch.from_numpy(src).to(dev), torch.from_numpy(tgt).to(dev))
+    tgt = [torch.from_numpy(t).to(dev) for t in tgts]     # several targets: one reference set
+    wav, mel = inf.inference_one_utterance(torch.from_numpy(src).to(dev), tgt[0] if len(tgt) == 1 else tgt)
     if is_wav(args.output):
         inf.write_wav_to_file(wav, args.output)
     else:
