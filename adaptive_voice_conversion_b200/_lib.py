@@ -220,6 +220,12 @@ class SpkGroupDesc(C.Structure):
                 ("queries", _fp), ("q_labels", _fp), ("q_exclude", _fp), ("set", _fp), ("labels", _fp), ("out", _fp)]
 
 
+class SpkIdentifyDesc(C.Structure):
+    _fields_ = [("m", C.c_int32), ("s", C.c_int32), ("dims", C.c_int32), ("reserved", C.c_int32),
+                ("queries", _fp), ("bank", _fp), ("q_target", _fp), ("best", _fp), ("best_score", _fp),
+                ("target_score", _fp), ("target_rank", _fp)]
+
+
 SN_ITERATE, SN_FIXED = 0, 1
 SN_MAX_ITEMS, SN_MAX_H, SN_MAX_W = 64, 4096, 4096
 
@@ -260,6 +266,8 @@ PROTOTYPES = {
     "avc_norm_apply_varlen": (_i, [C.POINTER(ConvDesc), _p, _i, _i, _p]),
     "avc_time_mean_varlen_fwd": (_i, [_p, _i64, _p, _i, _i, _i, _p, _i, _i, _p]),
     "avc_time_mean_grouped_fwd": (_i, [_p, _i64, _p, _i, _i, _i, _p, _i, _i, _p, _i, _p]),
+    "avc_time_sum_varlen": (_i, [_p, _i64, _p, _p, _i, _i, _i, _p, _i, _i, _p]),
+    "avc_pooled_group_mean": (_i, [_p, _p, _i64, _i, _p, _i, _p, _p]),
     "avc_varlen_tail": (_i, [_p, _i64, _i, _i, _i, _p, _i, _i, _i, _i, _p]),
     "avc_linear_fwd": (_i, [C.POINTER(LinearDesc), _p]),
     "avc_linear_bwd": (_i, [C.POINTER(LinearDesc), _p]),
@@ -292,6 +300,7 @@ PROTOTYPES = {
     "avc_spk_eer": (_i, [_p, _p, _i, _i, _p, _i64, _p, _p]),
     "avc_spk_group_mean": (_i, [C.POINTER(SpkGroupDesc), _p]),
     "avc_spk_group_mean_multi": (_i, [C.POINTER(SpkGroupDesc), _i, _p]),
+    "avc_spk_identify": (_i, [C.POINTER(SpkIdentifyDesc), _p]),
     "avc_spectral_norm_scratch_floats": (_i64, [_i, _i]),
     "avc_spectral_norm": (_i, [_p, _i, _i, _i, _i, _p, _p]),
     "avc_spectral_norm_bwd": (_i, [_p, _i, _i, _i, _p, _p]),

@@ -99,6 +99,17 @@ __global__ void time_mean_fwd_kernel(const float* __restrict__ a4, int64_t bstri
     st4(out + (int64_t)b * C + q * 4, make_float4(s.x * inv, s.y * inv, s.z * inv, s.w * inv));
   }
 }
+// The add step of every grouped pooling: the first member's sums are assigned, each later member's added.  Shared by
+// time_mean_grouped_kernel and pooled_group_mean_kernel, so that the same members in the same order give the same bits
+// whether they are pooled in one batch or from a table of per-sample sums.
+__device__ __forceinline__ void group_add4(float4& acc, const float4& s, bool first) {
+  if (first) {
+    acc = s;
+  } else {
+    acc.x += s.x; acc.y += s.y; acc.z += s.z; acc.w += s.w;
+  }
+}
+
 // Group g = rows offsets[g] .. offsets[g+1]-1: the members' sums (each as time_mean_fwd_kernel adds it) added in
 // ascending row, times 1 / (the members' frame count).  A one-member group gives time_mean_fwd_kernel's bits.
 __global__ void time_mean_grouped_kernel(const float* __restrict__ a4, int64_t bstride, float* __restrict__ out, int B, int C,
@@ -115,17 +126,55 @@ __global__ void time_mean_grouped_kernel(const float* __restrict__ a4, int64_t b
   for (int m = m0; m < m1; ++m) {
     const int Lm = min((__ldg(lengths + m) + div - 1) / div * mul, T);
     const float4 s = time_sum4(a4 + (int64_t)m * bstride, q, T, Lm, lane);
-    if (m == m0) {
-      acc = s;
-    } else {
-      acc.x += s.x; acc.y += s.y; acc.z += s.z; acc.w += s.w;
-    }
+    group_add4(acc, s, m == m0);
     n += Lm;
   }
   if (lane == 0) {
     const float inv = 1.f / (float)n;
     st4(out + (int64_t)g * C + q * 4, make_float4(acc.x * inv, acc.y * inv, acc.z * inv, acc.w * inv));
   }
+}
+// sample b's float32 sums over its L_b frames (time_sum4, as the grouped mean forms a member's) and L_b
+__global__ void time_sum_varlen_kernel(const float* __restrict__ a4, int64_t bstride, float* __restrict__ sums,
+                                       int32_t* __restrict__ counts, int B, int C, int T,
+                                       const int32_t* __restrict__ lengths, int div, int mul) {
+  const int Cq = C >> 2;
+  const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+  if (warp >= B * Cq) return;
+  const int b = warp / Cq, q = warp - b * Cq;
+  const int Lb = min((__ldg(lengths + b) + div - 1) / div * mul, T);
+  const float4 s = time_sum4(a4 + (int64_t)b * bstride, q, T, Lb, lane);
+  if (lane == 0) {
+    st4(sums + (int64_t)b * C + q * 4, s);
+    if (q == 0) counts[b] = Lb;
+  }
+}
+// Group g = rows offsets[g] .. offsets[g+1]-1 of a table of per-sample sums: added in ascending row with
+// time_mean_grouped_kernel's add step, times 1 / (the rows' frame count).  One thread per (group, channel quad).  A
+// group whose frame count is not in [1, 2^31) gets NaN.
+__global__ void pooled_group_mean_kernel(const float* __restrict__ sums, const int32_t* __restrict__ counts, int64_t N, int C,
+                                         const int64_t* __restrict__ offsets, int G, float* __restrict__ out) {
+  const int Cq = C >> 2;
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= (int64_t)G * Cq) return;
+  const int g = (int)(i / Cq), q = (int)(i - (int64_t)g * Cq);
+  // the caller validates the offsets; the clamps only keep a bad table inside the rows
+  const int64_t m0 = max(__ldg(offsets + g), (int64_t)0), m1 = min(__ldg(offsets + g + 1), N);
+  float4 acc = zero4();
+  int64_t n = 0;
+  for (int64_t m = m0; m < m1; ++m) {
+    group_add4(acc, ldg4(sums + m * C + q * 4), m == m0);
+    n += __ldg(counts + m);
+  }
+  float4 r;
+  if (n >= 1 && n < (1ll << 31)) {
+    const float inv = 1.f / (float)(int)n;
+    r = make_float4(acc.x * inv, acc.y * inv, acc.z * inv, acc.w * inv);
+  } else {
+    const float nan = __int_as_float(0x7fc00000);
+    r = make_float4(nan, nan, nan, nan);
+  }
+  st4(out + (int64_t)g * C + q * 4, r);
 }
 __global__ void time_mean_bwd_kernel(const float* __restrict__ dout, float* __restrict__ da4, int64_t bstride, int B, int C, int T) {
   const int Cq = C >> 2;
@@ -469,6 +518,38 @@ extern "C" int avc_time_mean_grouped_fwd(const float* a4, int64_t bstride, float
   AVC_LAUNCH(time_mean_grouped_kernel, (int)cdiv64((int64_t)G * (C / 4) * 32, 256), 256, 0, (cudaStream_t)stream, a4, bstride,
              out, B, C, T, lengths, len_div, len_mul, group_offsets, G);
   AVC_CHECK_LAUNCH("time_mean_grouped_fwd");
+  return AVC_OK;
+}
+extern "C" int avc_time_sum_varlen(const float* a4, int64_t bstride, float* sums, int32_t* counts, int B, int C, int T,
+                                   const int32_t* lengths, int len_div, int len_mul, void* stream) {
+  AVC_REQUIRE(a4 && sums && counts && lengths, AVC_ERR_INVALID,
+              "avc_time_sum_varlen: null pointer (a4 %p, sums %p, counts %p, lengths %p)", (const void*)a4, (const void*)sums,
+              (const void*)counts, (const void*)lengths);
+  AVC_REQUIRE(B > 0 && C > 0 && C % 4 == 0 && T > 0 && len_div >= 1 && len_mul >= 1, AVC_ERR_INVALID,
+              "avc_time_sum_varlen: bad sizes (B %d, C %d (a multiple of 4), T %d, len_div %d, len_mul %d)", B, C, T, len_div,
+              len_mul);
+  AVC_REQUIRE(((uintptr_t)a4 & 15) == 0 && ((uintptr_t)sums & 15) == 0 && bstride % 4 == 0, AVC_ERR_INVALID,
+              "avc_time_sum_varlen: a4 %p, sums %p and bstride %lld must be 16-byte aligned", (const void*)a4,
+              (const void*)sums, (long long)bstride);
+  AVC_LAUNCH(time_sum_varlen_kernel, (int)cdiv64((int64_t)B * (C / 4) * 32, 256), 256, 0, (cudaStream_t)stream, a4, bstride,
+             sums, counts, B, C, T, lengths, len_div, len_mul);
+  AVC_CHECK_LAUNCH("time_sum_varlen");
+  return AVC_OK;
+}
+extern "C" int avc_pooled_group_mean(const float* sums, const int32_t* counts, int64_t n_rows, int C,
+                                     const int64_t* group_offsets, int G, float* out, void* stream) {
+  AVC_REQUIRE(sums && counts && group_offsets && out, AVC_ERR_INVALID,
+              "avc_pooled_group_mean: null pointer (sums %p, counts %p, group_offsets %p, out %p)", (const void*)sums,
+              (const void*)counts, (const void*)group_offsets, (const void*)out);
+  AVC_REQUIRE(n_rows > 0 && C > 0 && C % 4 == 0, AVC_ERR_INVALID,
+              "avc_pooled_group_mean: bad sizes (n_rows %lld, C %d (a multiple of 4))", (long long)n_rows, C);
+  AVC_REQUIRE(G >= 1 && G <= n_rows, AVC_ERR_INVALID, "avc_pooled_group_mean: G %d must lie in [1, n_rows = %lld]", G,
+              (long long)n_rows);
+  AVC_REQUIRE(((uintptr_t)sums & 15) == 0 && ((uintptr_t)out & 15) == 0, AVC_ERR_INVALID,
+              "avc_pooled_group_mean: sums %p and out %p must be 16-byte aligned", (const void*)sums, (const void*)out);
+  AVC_LAUNCH(pooled_group_mean_kernel, (int)cdiv64((int64_t)G * (C / 4), 256), 256, 0, (cudaStream_t)stream, sums, counts,
+             n_rows, C, group_offsets, G, out);
+  AVC_CHECK_LAUNCH("pooled_group_mean");
   return AVC_OK;
 }
 extern "C" int avc_time_mean_bwd(const float* dout, float* da4, int64_t bstride, int B, int C, int T, void* stream) {

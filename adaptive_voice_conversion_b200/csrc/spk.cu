@@ -326,6 +326,30 @@ __global__ void spk_result_kernel(const SpkState* st, avc_eer_result* out) {
   *out = r;
 }
 
+// ---------------------------------------------------------------- query scores
+// The block stages query q (float32, promoted) in qv[D]; after a __syncthreads thread 0 writes *rq = sqrt(sum_k q[k]^2),
+// ascending k.  The caller syncs again before reading *rq.
+__device__ __forceinline__ void stage_query(const float* __restrict__ q, int D, double* qv, double* rq) {
+  for (int k = threadIdx.x; k < D; k += blockDim.x) qv[k] = (double)__ldg(q + k);
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double acc = 0.0;
+    for (int k = 0; k < D; ++k) acc = __dadd_rn(acc, __dmul_rn(qv[k], qv[k]));
+    *rq = __dsqrt_rn(acc);
+  }
+}
+
+// s(q, v) of the staged query (qv, rq) and the float32 row p[D]: dot(q, v) and |v|^2 each added in ascending k
+__device__ __forceinline__ double staged_score(const double* qv, double rq, const float* __restrict__ p, int D) {
+  double dot = 0.0, nv = 0.0;
+  for (int k = 0; k < D; ++k) {
+    const double b = (double)__ldg(p + k);
+    dot = __dadd_rn(dot, __dmul_rn(qv[k], b));
+    nv = __dadd_rn(nv, __dmul_rn(b, b));
+  }
+  return cosine(dot, rq, __dsqrt_rn(nv));
+}
+
 // ---------------------------------------------------------------- group means
 constexpr int SPK_MAX_EXCLUDE = 64;
 
@@ -337,14 +361,8 @@ __global__ void __launch_bounds__(SPK_THREADS) spk_group_mean_kernel(const avc_s
   __shared__ int exl[SPK_MAX_EXCLUDE];
   __shared__ double rq;
   const int m = blockIdx.x, D = d.dims;
-  for (int k = threadIdx.x; k < D; k += SPK_THREADS) qv[k] = (double)__ldg(d.queries + (int64_t)m * D + k);
   if (threadIdx.x < n_ex) exl[threadIdx.x] = __ldg(d.q_exclude + (int64_t)m * n_ex + threadIdx.x);
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    double acc = 0.0;
-    for (int k = 0; k < D; ++k) acc = __dadd_rn(acc, __dmul_rn(qv[k], qv[k]));
-    rq = __dsqrt_rn(acc);
-  }
+  stage_query(d.queries + (int64_t)m * D, D, qv, &rq);
   const int lab = __ldg(d.q_labels + m);
   double sum = 0.0;
   long long cnt = 0;
@@ -355,16 +373,7 @@ __global__ void __launch_bounds__(SPK_THREADS) spk_group_mean_kernel(const avc_s
     for (int e = 0; e < n_ex; ++e) excluded |= v == exl[e];
     const bool take = v < d.n && !excluded && __ldg(d.labels + v) == lab;
     ok[threadIdx.x] = take;
-    if (take) {
-      const float* p = d.set + (int64_t)v * D;
-      double dot = 0.0, nv = 0.0;
-      for (int k = 0; k < D; ++k) {
-        const double b = (double)__ldg(p + k);
-        dot = __dadd_rn(dot, __dmul_rn(qv[k], b));
-        nv = __dadd_rn(nv, __dmul_rn(b, b));
-      }
-      sc[threadIdx.x] = cosine(dot, rq, __dsqrt_rn(nv));
-    }
+    if (take) sc[threadIdx.x] = staged_score(qv, rq, d.set + (int64_t)v * D, D);
     __syncthreads();
     if (threadIdx.x == 0)
       for (int t = 0; t < SPK_THREADS; ++t)
@@ -374,6 +383,69 @@ __global__ void __launch_bounds__(SPK_THREADS) spk_group_mean_kernel(const avc_s
         }
   }
   if (threadIdx.x == 0) d.out[m] = cnt ? __ddiv_rn(sum, (double)cnt) : __longlong_as_double(0x7ff8000000000000ll);
+}
+
+// ---------------------------------------------------------------- identification against a bank
+// (score, index) a beats (score, index) b: a higher score, or the same score at a lower index; index -1 is "none yet"
+__device__ __forceinline__ bool beats(double sa, int ia, double sb, int ib) {
+  return ia >= 0 && (ib < 0 || sa > sb || (sa == sb && ia < ib));
+}
+
+// one CTA per query: the target's score first (thread 0), then every bank row, each thread keeping its best row and
+// its count of rows above the target; a warp then a block reduction combines them
+__global__ void __launch_bounds__(SPK_THREADS) spk_identify_kernel(const avc_spk_identify_desc d) {
+  extern __shared__ double qv[];   // [dims]
+  __shared__ double rq, tsc;
+  __shared__ double w_best[SPK_THREADS / 32];
+  __shared__ int w_idx[SPK_THREADS / 32], w_above[SPK_THREADS / 32];
+  const int m = blockIdx.x, D = d.dims;
+  stage_query(d.queries + (int64_t)m * D, D, qv, &rq);
+  __syncthreads();
+  const int t = d.q_target ? __ldg(d.q_target + m) : -1;
+  const bool has_t = t >= 0 && t < d.s;
+  if (threadIdx.x == 0) tsc = has_t ? staged_score(qv, rq, d.bank + (int64_t)t * D, D) : __longlong_as_double(0x7ff8000000000000ll);
+  __syncthreads();
+  const double ts = tsc, r = rq;
+  double best = 0.0;
+  int idx = -1, above = 0;
+  for (int v = threadIdx.x; v < d.s; v += SPK_THREADS) {
+    const double sc = staged_score(qv, r, d.bank + (int64_t)v * D, D);
+    if (beats(sc, v, best, idx)) {
+      best = sc;
+      idx = v;
+    }
+    above += sc > ts;   // never with no target: ts is NaN
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    const double ob = __shfl_down_sync(0xffffffffu, best, o);
+    const int oi = __shfl_down_sync(0xffffffffu, idx, o);
+    above += __shfl_down_sync(0xffffffffu, above, o);
+    if (beats(ob, oi, best, idx)) {
+      best = ob;
+      idx = oi;
+    }
+  }
+  const int w = threadIdx.x >> 5;
+  if ((threadIdx.x & 31) == 0) {
+    w_best[w] = best;
+    w_idx[w] = idx;
+    w_above[w] = above;
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    for (int k = 1; k < SPK_THREADS / 32; ++k) {
+      if (beats(w_best[k], w_idx[k], best, idx)) {
+        best = w_best[k];
+        idx = w_idx[k];
+      }
+      above += w_above[k];
+    }
+    d.best[m] = idx;
+    d.best_score[m] = best;
+    d.target_score[m] = ts;
+    d.target_rank[m] = has_t ? above : -1;
+  }
 }
 
 int64_t eer_tiles(int n) {
@@ -462,4 +534,21 @@ extern "C" int avc_spk_group_mean(const avc_spk_group_desc* d, void* stream) {
 
 extern "C" int avc_spk_group_mean_multi(const avc_spk_group_desc* d, int n_exclude, void* stream) {
   return group_mean(d, n_exclude, "avc_spk_group_mean_multi", stream);
+}
+
+extern "C" int avc_spk_identify(const avc_spk_identify_desc* d, void* stream) {
+  AVC_REQUIRE(d != nullptr, AVC_ERR_INVALID, "avc_spk_identify: null descriptor");
+  AVC_REQUIRE(d->queries != nullptr && d->bank != nullptr && d->best != nullptr && d->best_score != nullptr &&
+                  d->target_score != nullptr && d->target_rank != nullptr,
+              AVC_ERR_INVALID,
+              "avc_spk_identify: null pointer (queries %p, bank %p, best %p, best_score %p, target_score %p, target_rank %p)",
+              (const void*)d->queries, (const void*)d->bank, (const void*)d->best, (const void*)d->best_score,
+              (const void*)d->target_score, (const void*)d->target_rank);
+  AVC_REQUIRE(d->m > 0 && d->s > 0 && d->dims > 0, AVC_ERR_INVALID, "avc_spk_identify: sizes must be positive (m %d, s %d, dims %d)",
+              d->m, d->s, d->dims);
+  AVC_REQUIRE(d->s <= AVC_SPK_MAX_N, AVC_ERR_UNSUPPORTED, "avc_spk_identify: s %d > %d", d->s, AVC_SPK_MAX_N);
+  AVC_REQUIRE(d->dims <= AVC_SPK_MAX_DIMS, AVC_ERR_UNSUPPORTED, "avc_spk_identify: dims %d > %d", d->dims, AVC_SPK_MAX_DIMS);
+  spk_identify_kernel<<<(unsigned)d->m, SPK_THREADS, d->dims * 8, (cudaStream_t)stream>>>(*d);
+  AVC_CHECK_LAUNCH("avc_spk_identify");
+  return AVC_OK;
 }

@@ -876,8 +876,19 @@ class Engine:
                                                        lo.div, lo.mul, self.stream), "time_mean_varlen_fwd")
         else:
             self._ck(self.lib.avc_time_mean_fwd(out.ptr, out.bstride, pooled.data_ptr(), B, out.C, out.T, self.stream), "time_mean_fwd")
+        emb = self._speaker_dense(P, pooled, train, ctx)
+        if train:
+            ctx["last"] = out
+        return emb, ctx
+
+    def _speaker_dense(self, P, pooled: torch.Tensor, train: bool, ctx: dict) -> torch.Tensor:
+        """The speaker encoder's dense stack and output layer on the pooled rows [B, c_h] -> emb [B, c_out]: the fused
+        stack when it applies, else the per-layer linears.  train: their records go to ctx (speaker_bwd)."""
+        c = self.cfg["SpeakerEncoder"]
+        enc = "speaker_encoder"
+        B = pooled.shape[0]
         nd = c["n_dense_blocks"]
-        if self.fused_dense and out.C == 128 and c["c_out"] == 128:
+        if self.fused_dense and pooled.shape[1] == 128 and c["c_out"] == 128:
             names = self._dense_names(enc)
             tab = self._param_table("params", names, P)
             save = self.empty(3 * nd + 1, B, 128) if train else None
@@ -887,8 +898,8 @@ class Engine:
             d.params, d.x, d.save, d.out = tab.data_ptr(), pooled.data_ptr(), _ptr(save), emb.data_ptr()
             self._ck(self.lib.avc_dense_stack_fwd(C.byref(d), self.stream), "dense_stack_fwd")
             if train:
-                ctx.update(dense_fused=dict(save=save, tab=tab, names=names, pooled=pooled), last=out)
-            return emb, ctx
+                ctx.update(dense_fused=dict(save=save, tab=tab, names=names, pooled=pooled))
+            return emb
         h = pooled
         dense = []
         for l in range(nd):
@@ -897,8 +908,34 @@ class Engine:
             dense.append((r1, r2))
         emb, r_out = self.linear(P, f"{enc}.output_layer", h, train=train)
         if train:
-            ctx.update(dense=dense, out_rec=r_out, last=out)
-        return emb, ctx
+            ctx.update(dense=dense, out_rec=r_out)
+        return emb
+
+    def speaker_sums(self, P, x_planar: torch.Tensor, lens: Lengths):
+        """The speaker encoder up to its time mean on a padded batch (inference only; x_planar and lens as in
+        speaker_fwd), then each sample's sums over its valid frames of the last conv layer (avc_time_sum_varlen) ->
+        (sums [B, c_h] float32, counts [B] int32): the rows speaker_codes_from_sums pools."""
+        c = self.cfg["SpeakerEncoder"]
+        enc = "speaker_encoder"
+        ctx: dict = {}
+        out = self._bank_and_in_conv(P, enc, c, x_planar, norm=False, train=False, ctx=ctx, lens=lens)
+        out = self._enc_blocks(P, enc, c, out, norm=False, train=False, ctx=ctx, lens=lens)
+        lo = ctx.pop("lens")
+        sums = self.empty(out.B, out.C)
+        counts = torch.empty(out.B, dtype=torch.int32, device=self.dev)
+        self._ck(self.lib.avc_time_sum_varlen(out.ptr, out.bstride, sums.data_ptr(), counts.data_ptr(), out.B, out.C, out.T,
+                                              lo.t.data_ptr(), lo.div, lo.mul, self.stream), "time_sum_varlen")
+        return sums, counts
+
+    def speaker_codes_from_sums(self, P, sums: torch.Tensor, counts: torch.Tensor, offsets: torch.Tensor) -> torch.Tensor:
+        """Speaker codes [G, c_out] of groups of rows of a (sums [N, c_h], counts [N] int32) table (speaker_sums' rows,
+        from any number of batches): int64 offsets [G+1] on the device, validated by the caller.  Each group's rows
+        are pooled by avc_pooled_group_mean, then the dense tail of speaker_fwd runs on the G pooled rows."""
+        G = offsets.shape[0] - 1
+        pooled = self.empty(G, sums.shape[1])
+        self._ck(self.lib.avc_pooled_group_mean(sums.data_ptr(), counts.data_ptr(), sums.shape[0], sums.shape[1],
+                                                offsets.data_ptr(), G, pooled.data_ptr(), self.stream), "pooled_group_mean")
+        return self._speaker_dense(P, pooled, False, {})
 
     def speaker_bwd(self, P, G, ctx, demb: torch.Tensor):
         c = self.cfg["SpeakerEncoder"]

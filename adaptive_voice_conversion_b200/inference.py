@@ -306,22 +306,49 @@ class Inferencer(object):
             if id(refs) not in slot_of:
                 slot_of[id(refs)] = len(uniq)
                 uniq.append(refs)
+        src = self._source_frames(xs, "inference_padded")
+        emb = self.embed_speakers(uniq)
+        which = torch.tensor([slot_of[id(refs)] for refs in ref_sets], device=emb.device)
+        return self._convert_with_codes(src, emb.index_select(0, which), batch_max)
+
+    def _source_frames(self, xs, what):
+        """[C, T_i] model inputs of the sources xs ([T_i, n_mels]); ValueError naming a source shorter than the model
+        accepts."""
         src = [self.utt_make_frames(x)[0] for x in xs]
         min_src, _ = min_frames(self.config)
         for i, s in enumerate(src):
             if s.shape[1] < min_src:
-                raise ValueError(f"inference_padded: pair {i} has {s.shape[1]} source frames; the model needs at least "
-                                 f"{min_src}")
-        emb = self.embed_speakers(uniq)
-        which = [slot_of[id(refs)] for refs in ref_sets]
+                raise ValueError(f"{what}: pair {i} has {s.shape[1]} source frames; the model needs at least {min_src}")
+        return src
+
+    @torch.no_grad()
+    def inference_with_codes(self, xs, codes, batch_max: int = PADDED_BATCH_MAX):
+        """Convert each source xs[i] ([T_i, n_mels] normalised mel on the device) with the speaker code codes[i]
+        (float32 [len(xs), c_out] on the device, or a list of [c_out] codes: rows of embed_speakers, SpeakerBank.code,
+        ...) in inference_padded's grid: padded_batches' shapes, one CUDA graph per shape (AVC_INFER_GRAPH=1) with the
+        codes in a static buffer, through AE.inference_from_embeddings.  Returns inference_padded's list of mels.
+        inference_padded(xs, sets) runs exactly this on embed_speakers' codes of the pairs' sets."""
+        if not isinstance(codes, torch.Tensor):
+            codes = torch.stack(list(codes)) if len(codes) else None
+        c_out = self.config["SpeakerEncoder"]["c_out"]
+        if (codes is None or codes.dtype != torch.float32 or tuple(codes.shape) != (len(xs), c_out)
+                or (xs and codes.device != xs[0].device)):
+            raise ValueError(f"inference_with_codes: codes must be float32 [{len(xs)}, {c_out}] on the sources' device, "
+                             f"got {getattr(codes, 'dtype', None)} {tuple(getattr(codes, 'shape', ()))}")
+        if not xs:
+            return []
+        return self._convert_with_codes(self._source_frames(xs, "inference_with_codes"), codes.contiguous(), batch_max)
+
+    def _convert_with_codes(self, src, codes, batch_max):
+        """The sources src ([C, T_i] model inputs) converted with codes[i] in padded_batches' grid (_emb_slot)."""
         dev = src[0].device
-        out = [None] * len(xs)
+        out = [None] * len(src)
         for idx, T, _, Bp in padded_batches([s.shape[1] for s in src], [0] * len(src), batch_max):
             xb, eb, lx, run = self._emb_slot(Bp, src[0].shape[0], T, dev)
             rows = idx + [idx[0]] * (Bp - len(idx))                # rows past the batch repeat its first pair
             for j, i in enumerate(rows):
                 xb[j, :, :src[i].shape[1]].copy_(src[i])
-            eb.copy_(emb.index_select(0, torch.tensor([which[i] for i in rows], device=dev)))
+            eb.copy_(codes.index_select(0, torch.tensor(rows, device=dev)))
             lx.copy_(torch.tensor([src[i].shape[1] for i in rows], dtype=torch.int32))
             dec = run()
             for j, i in enumerate(idx):

@@ -128,9 +128,10 @@ def _check_lengths(lengths: Optional[torch.Tensor], x: torch.Tensor, min_len: in
     return lengths.to(device=x.device, dtype=torch.int32)
 
 
-def _check_groups(groups, x: torch.Tensor, what: str) -> torch.Tensor:
-    """Row offsets [G+1] of groups of a batch x [B, C, T] as int32 on x's device: 0 first, strictly increasing, B last
-    (1 <= G <= B); AvcError otherwise.  As in _check_lengths, device values are not read during a graph capture."""
+def _check_groups(groups, x: torch.Tensor, what: str, dtype=torch.int32) -> torch.Tensor:
+    """Row offsets [G+1] of groups of a batch x [B, C, T] (or of the rows of a table x [B, ...]) as `dtype` on x's
+    device: 0 first, strictly increasing, B last (1 <= G <= B); AvcError otherwise.  As in _check_lengths, device
+    values are not read during a graph capture."""
     B = x.shape[0]
     if not isinstance(groups, torch.Tensor) or groups.dtype == torch.bool or groups.is_floating_point() or groups.is_complex():
         raise L.AvcError(f"{what}: expected an integer tensor, got {getattr(groups, 'dtype', type(groups).__name__)}")
@@ -142,7 +143,7 @@ def _check_groups(groups, x: torch.Tensor, what: str) -> torch.Tensor:
         v = groups.cpu().tolist()
         if v[0] != 0 or v[-1] != B or any(b <= a for a, b in zip(v, v[1:])):
             raise L.AvcError(f"{what}: offsets must start at 0, increase strictly and end at {B} (the batch size); got {v}")
-    return groups.to(device=x.device, dtype=torch.int32)
+    return groups.to(device=x.device, dtype=dtype)
 
 
 def _pad_time(x: torch.Tensor, Te: int) -> torch.Tensor:
@@ -381,6 +382,50 @@ class AE(nn.Module):
                 return eng.speaker_fwd(P, _pad_time(x, varlen_extent(self.config, x.shape[2], source=False)), False,
                                        lens=Lengths(lx), groups=g)[0]
         return _SpeakerFn.apply(self, x, *self._params("speaker_encoder."))
+
+    def get_speaker_sums(self, x: torch.Tensor, *, lengths: torch.Tensor):
+        """(sums [B, c_h] float32, counts [B] int32) of a padded batch x [B, C, T] (lengths as in get_speaker_embeddings;
+        no gradient): the speaker encoder up to its time mean, then each sample's float32 sum over its valid frames of
+        the last conv layer and the number of those frames.  Rows from any number of calls, gathered into one table,
+        pool into speaker codes with speaker_codes_from_sums, bit for bit as get_speaker_embeddings(groups=) pools the
+        same members in one batch."""
+        x = _check_input(x, "AE.get_speaker_sums(x)")
+        lx = _check_lengths(lengths, x, self._min_frames()[1], "AE.get_speaker_sums(lengths)")
+        with torch.no_grad():
+            eng, P = self._eval_stack("speaker_encoder.", x.device)
+            return eng.speaker_sums(P, _pad_time(x, varlen_extent(self.config, x.shape[2], source=False)), Lengths(lx))
+
+    def speaker_codes_from_sums(self, sums: torch.Tensor, counts: torch.Tensor, *, groups: torch.Tensor):
+        """Speaker codes [G, c_out] (no gradient) of groups of rows of a get_speaker_sums table: groups holds integer row
+        offsets [G+1] (0, strictly increasing, N = the table's rows).  A group's code pools its rows' sums in ascending
+        row over their frames together, then runs the dense stack: the same members in the same order give
+        get_speaker_embeddings(groups=)'s code bit for bit, however the rows were spread over batches.  Any number of
+        rows per group; a group of 2^31 frames or more raises.  Everything is checked before any launch."""
+        c = self.config["SpeakerEncoder"]
+        if (not isinstance(sums, torch.Tensor) or sums.dtype != torch.float32 or sums.dim() != 2 or not sums.is_cuda
+                or sums.shape[1] != c["c_h"] or sums.shape[0] < 1):
+            raise L.AvcError(f"AE.speaker_codes_from_sums(sums): expected float32 [N >= 1, {c['c_h']}] on a CUDA device, got "
+                             f"{getattr(sums, 'dtype', type(sums).__name__)} {tuple(getattr(sums, 'shape', ()))} on "
+                             f"{getattr(sums, 'device', None)}")
+        N = sums.shape[0]
+        if (not isinstance(counts, torch.Tensor) or counts.dtype != torch.int32 or tuple(counts.shape) != (N,)
+                or counts.device != sums.device):
+            raise L.AvcError(f"AE.speaker_codes_from_sums(counts): expected int32 [{N}] on {sums.device}, got "
+                             f"{getattr(counts, 'dtype', type(counts).__name__)} {tuple(getattr(counts, 'shape', ()))} on "
+                             f"{getattr(counts, 'device', None)}")
+        offs = _check_groups(groups, sums, "AE.speaker_codes_from_sums(groups)", dtype=torch.int64)
+        hc, ho = counts.cpu().to(torch.int64), offs.cpu()
+        if int(hc.min()) < 1:
+            raise L.AvcError(f"AE.speaker_codes_from_sums(counts): counts must be >= 1 (got min {int(hc.min())})")
+        frames = torch.cat([torch.zeros(1, dtype=torch.int64), hc.cumsum(0)])
+        per_group = frames[ho[1:]] - frames[ho[:-1]]
+        if int(per_group.max()) >= 2 ** 31:
+            g = int(per_group.argmax())
+            raise L.AvcError(f"AE.speaker_codes_from_sums: group {g} pools {int(per_group[g])} frames; fewer than 2^31 "
+                             f"are supported")
+        with torch.no_grad():
+            eng, P = self._eval_stack("speaker_encoder.", sums.device)
+            return eng.speaker_codes_from_sums(P, sums.contiguous(), counts.contiguous(), offs)
 
     def inference_from_embeddings(self, x: torch.Tensor, emb: torch.Tensor, *, lengths: Optional[torch.Tensor] = None):
         """AE.inference with a given speaker code: content mean of x [B, C, T], decoder conditioned on emb [B, c_out]

@@ -291,6 +291,56 @@ def group_means(queries: torch.Tensor, q_labels, q_exclude, vecs: torch.Tensor, 
     return out
 
 
+def identify(queries: torch.Tensor, bank: torch.Tensor, targets=None) -> Dict[str, np.ndarray]:
+    """Closed-set identification of queries [M, D] against bank codes [S, D] (float32, one CUDA device), one launch
+    (avc_spk_identify): {"best": int32 [M] (the highest-scoring bank row, the lowest among ties), "best_score": float64,
+    "target_score": float64 (NaN without a target), "target_rank": int32 (rows scoring strictly above the target; -1
+    without one)} on the host.  targets: M bank rows, -1 = none (None: no targets).  Scores are s(a, b) above."""
+    queries = _check_vectors(queries, "identify(queries)", n_max=2 ** 31 - 1)
+    bank = _check_vectors(bank, "identify(bank)")
+    if queries.shape[1] != bank.shape[1] or queries.device != bank.device:
+        raise ValueError(f"identify: queries {tuple(queries.shape)} on {queries.device}, bank {tuple(bank.shape)} on "
+                         f"{bank.device}; the dimensions and devices must agree")
+    (m, d), s, dev = queries.shape, bank.shape[0], bank.device
+    tg = None if targets is None else _labels(targets, m, dev, "identify(targets)")
+    best = torch.empty(m, dtype=torch.int32, device=dev)
+    rank = torch.empty(m, dtype=torch.int32, device=dev)
+    best_score = torch.empty(m, dtype=torch.float64, device=dev)
+    target_score = torch.empty(m, dtype=torch.float64, device=dev)
+    desc = L.SpkIdentifyDesc(m=m, s=s, dims=d, queries=queries.data_ptr(), bank=bank.data_ptr(),
+                             q_target=None if tg is None else tg.data_ptr(), best=best.data_ptr(),
+                             best_score=best_score.data_ptr(), target_score=target_score.data_ptr(),
+                             target_rank=rank.data_ptr())
+    L.check(L.load().avc_spk_identify(C.byref(desc), _stream(dev)), "avc_spk_identify")
+    return {"best": best.cpu().numpy(), "best_score": best_score.cpu().numpy(),
+            "target_score": target_score.cpu().numpy(), "target_rank": rank.cpu().numpy()}
+
+
+def bank_identification(bank, y: torch.Tensor, src_speakers, tgt_speakers, real: torch.Tensor, real_speakers) -> dict:
+    """The bank fields of a set's conversion entry: id_target / id_source = the shares of the conversions y (rows of
+    pairs whose source and target speakers are both banked) whose nearest bank code is the target's / the source's;
+    id_real = the share of the real utterance embeddings `real` of banked speakers nearest their own speaker's code;
+    n_banked / n_unbanked pairs; bank_speakers.  Shares are None over no rows.  One identify call."""
+    pi = [i for i, (s, t) in enumerate(zip(src_speakers, tgt_speakers)) if s in bank and t in bank]
+    ri = [i for i, s in enumerate(real_speakers) if s in bank]
+    out = {"id_target": None, "id_source": None, "id_real": None, "n_banked": len(pi),
+           "n_unbanked": len(src_speakers) - len(pi), "bank_speakers": len(bank)}
+    if not pi and not ri:
+        return out
+    dev = bank.codes.device
+    q = torch.cat([v[torch.tensor(rows, dtype=torch.long, device=v.device)].to(dev) for v, rows in ((y, pi), (real, ri))
+                   if rows])
+    targets = [bank.index(tgt_speakers[i]) for i in pi] + [bank.index(real_speakers[i]) for i in ri]
+    best = identify(q, bank.codes, targets)["best"]
+    P = len(pi)
+    if P:
+        out["id_target"] = float(np.mean(best[:P] == np.array(targets[:P])))
+        out["id_source"] = float(np.mean(best[:P] == np.array([bank.index(src_speakers[i]) for i in pi])))
+    if ri:
+        out["id_real"] = float(np.mean(best[P:] == np.array(targets[P:])))
+    return out
+
+
 # ------------------------------------------------------------------ representations and conversions
 def _batch(mels, idx, T, dev):
     x = torch.zeros(len(idx), int(mels[idx[0]].shape[1]), T, device=dev)
@@ -351,7 +401,7 @@ def _means(rows: np.ndarray) -> Dict[str, float]:
 
 
 def evaluate_speakers(model, data: Mapping[str, np.ndarray], seed: int = 0, max_pairs: int = 0, device=None,
-                      per_pair: bool = False, n_refs: int = 1) -> dict:
+                      per_pair: bool = False, n_refs: int = 1, bank=None) -> dict:
     """Speaker measures of `model` (an AE) on one set: data = {utterance key: attr-normalised [T, n_mels]} (the set's
     pickle).  Returns {"eer": {"speaker", "content", "mel": {eer, threshold, frr, far, n_target, n_nontarget}},
     "n_utts", "n_short", "conversion": {"sim_target", "sim_source", "success", "sim_target_source" (when n > 0), "n",
@@ -361,8 +411,15 @@ def evaluate_speakers(model, data: Mapping[str, np.ndarray], seed: int = 0, max_
     n_refs > 1 (few-shot): each pair keeps its reference and gets n_refs - 1 more (fewshot_pairs), the source is
     converted with the set's pooled code, and sim_target skips all n_refs references; sim_source and
     sim_target_source are as with one.  conversion then also reports "n_refs" and "n_few" (the pairs fewshot_pairs
-    dropped), and a per-pair row lists the references: [source, [reference, ...], ...]."""
+    dropped), and a per-pair row lists the references: [source, [reference, ...], ...].
+
+    bank (a speaker_bank.SpeakerBank of this model, built from utterances outside `data`: ValueError naming the
+    overlap otherwise): conversion also reports bank_identification's id_target, id_source, id_real, n_banked,
+    n_unbanked and bank_speakers, by nearest bank code (avc_spk_identify)."""
     cfg = model.config
+    if bank is not None:
+        from .speaker_bank import check_disjoint
+        check_disjoint(bank, data.keys())
     if int(cfg["data_loader"]["frame_size"]) != 1:
         raise ValueError(f"speaker evaluation supports data_loader.frame_size 1 only (got {cfg['data_loader']['frame_size']})")
     if not 1 <= int(n_refs) <= SPK_MAX_EXCLUDE:
@@ -427,10 +484,17 @@ def evaluate_speakers(model, data: Mapping[str, np.ndarray], seed: int = 0, max_
             if per_pair:
                 conv["pairs"] = [[u, list(r) if n_refs > 1 else r, float(v[0]), float(v[1]), bool(v[2]), float(v[3])]
                                  for (u, r), v in zip(pairs, vals)]
+            if bank is not None:
+                conv.update(bank_identification(bank, y, [speaker_of(u) for u, _ in pairs],
+                                                [speaker_of(r if n_refs == 1 else r[0]) for _, r in pairs], emb,
+                                                [speaker_of(u) for u in utts]))
         else:
             conv["speakers"] = {}
             if per_pair:
                 conv["pairs"] = []
+            if bank is not None:
+                conv.update(bank_identification(bank, None, [], [], reps["speaker"] if utts else None,
+                                                [speaker_of(u) for u in utts]))
         model.engine(dev).check_tc_status()
     finally:
         model.train(was_training)

@@ -3,7 +3,7 @@ data directory (adaptive_voice_conversion_b200/evaluate.py gives the definition)
 
     python evaluate.py -c config.yaml -m model.ckpt -d data/ [-eval_sets in_test,out_test] [-o eval.json]
                        [-mcd -transcripts VCTK-Corpus/txt [-attr data/attr.pkl] [-mcd_dims 24]] [-spk]
-                       [-max_pairs 0] [-seed 0] [-n_refs 1]
+                       [-max_pairs 0] [-seed 0] [-n_refs 1] [-bank bank.pt]
 
 The checkpoint is loaded strictly (reference checkpoints too, and the `sn: True` layout).  Each set's losses are
 printed; -o writes them with the per-speaker means as JSON.  -mcd also measures conversion itself: the mel-cepstral
@@ -17,6 +17,12 @@ set in -o.
 (-mcd and -spk): the first reference is drawn as with one, the K - 1 others from a second generator seeded with
 seed + 1; sim_target then skips all K.  With K > 1 each result also reports n_refs and n_few (conversions dropped for
 want of K references).
+-bank bank.pt (with -spk; speaker_bank.py) also identifies each conversion among the banked speakers by nearest
+speaker code: id_target and id_source are the shares of conversions nearest the target's and the source's code,
+id_real the share of the set's own utterances nearest their speaker's (the encoder's ceiling), over the n_banked
+pairs whose two speakers are banked (n_unbanked the others), with bank_speakers.  A bank that pooled any of the
+evaluated utterances is refused; a train bank leaves in_test leak-free and reports out_test's unseen speakers as
+unbanked.
 """
 import json
 import os
@@ -48,9 +54,12 @@ def main(argv=None):
     p.add_argument("-seed", type=int, default=0, help="seed of the reference choice and the sampling (-mcd, -spk)")
     p.add_argument("-n_refs", type=int, default=1,
                    help="references of the target speaker per conversion, their speaker codes pooled (-mcd, -spk)")
+    p.add_argument("-bank", default=None, help="speaker bank: identify conversions among its speakers (-spk)")
     args = p.parse_args(argv)
     if args.mcd and not args.transcripts:
         p.error("-mcd needs -transcripts DIR")
+    if args.bank and not args.spk:
+        p.error("-bank needs -spk")
     if not 1 <= args.n_refs <= 64:
         p.error("-n_refs must lie in [1, 64]")
     few = {} if args.n_refs == 1 else {"n_refs": args.n_refs}
@@ -79,10 +88,14 @@ def main(argv=None):
                   f"{len(m['speakers'])} target speakers)")
     if args.spk:
         from adaptive_voice_conversion_b200.speaker_eval import evaluate_speakers
+        banked = {}
+        if args.bank:
+            from adaptive_voice_conversion_b200.speaker_bank import SpeakerBank
+            banked["bank"] = SpeakerBank.load(args.bank, model)
         for s in res:
             with open(os.path.join(args.data_dir, f"{s}.pkl"), "rb") as f:
                 data = pickle.load(f)
-            r = evaluate_speakers(model, data, seed=args.seed, max_pairs=args.max_pairs, device=dev, **few)
+            r = evaluate_speakers(model, data, seed=args.seed, max_pairs=args.max_pairs, device=dev, **few, **banked)
             res[s]["spk"] = r
             e = r["eer"]
             eers = " ".join(f"{k}=" + ("n/a" if e[k]["eer"] is None else f"{e[k]['eer']:.4f}") for k in ("speaker", "content", "mel"))
@@ -92,6 +105,10 @@ def main(argv=None):
                      f"sim_target_source={c['sim_target_source']:.4f}") if c["n"] else ""
             means += f" n_refs={c['n_refs']} n_few={c['n_few']}" if few else ""
             print(f"{s}: spk conversion n={c['n']} n_short={c['n_short']}{means} ({len(c['speakers'])} target speakers)")
+            if args.bank:
+                ids = " ".join(f"{k}=" + ("n/a" if c[k] is None else f"{c[k]:.4f}") for k in ("id_target", "id_source", "id_real"))
+                print(f"{s}: spk bank {ids} n_banked={c['n_banked']} n_unbanked={c['n_unbanked']} "
+                      f"({c['bank_speakers']} banked speakers)")
     if args.output:
         with open(args.output, "w") as f:
             json.dump(res, f, indent=1)

@@ -282,6 +282,24 @@ int avc_time_mean_varlen_fwd(const float* a4, int64_t bstride, float* out /*[B][
 int avc_time_mean_grouped_fwd(const float* a4, int64_t bstride, float* out /*[G][C]*/, int B, int C, int T,
                               const int32_t* lengths, int len_div, int len_mul, const int32_t* group_offsets, int G,
                               void* stream);
+/* The two halves of avc_time_mean_grouped_fwd, for groups spread over several batches (speaker banks).
+ * avc_time_sum_varlen: sums[b][c] = sample b's float32 sum over its L_b = min(ceil(lengths[b] / len_div) * len_mul, T)
+ * frames, formed exactly as avc_time_mean_grouped_fwd forms a member's sum, and counts[b] = L_b (DEVICE int32 [B]).
+ * sums[b] * (1.f / L_b) is avc_time_mean_varlen_fwd's row bit for bit; frames past L_b are never read.
+ * avc_pooled_group_mean: group g is the rows group_offsets[g] .. group_offsets[g+1] - 1 of a table sums[n_rows][C],
+ * counts[n_rows] (DEVICE int64 [G+1] offsets, 0 = offsets[0] < ... < offsets[G] <= n_rows, validated by the caller):
+ * out[g][c] = (S_first + S_next + ..., in ascending row) * (1.f / (float)N_g), N_g = the sum of the rows' counts, the
+ * first row assigned, not added to zero, with avc_time_mean_grouped_fwd's add step.  So the same members in the same
+ * order give avc_time_mean_grouped_fwd's row bit for bit, however they were spread over batches.  The counts are
+ * device values the host does not read: a group with N_g outside [1, 2^31) gets NaN, and callers reject such a group
+ * before the launch (AE.speaker_codes_from_sums does).
+ * Both: AVC_ERR_INVALID for null pointers, non-positive sizes, C % 4 != 0, len_div or len_mul < 1, G outside
+ * [1, n_rows], a4, sums, out or the sample stride not 16-byte aligned.  No allocation, no synchronisation, no atomics:
+ * graph-capturable. */
+int avc_time_sum_varlen(const float* a4, int64_t bstride, float* sums /*[B][C]*/, int32_t* counts /*[B]*/, int B, int C,
+                        int T, const int32_t* lengths, int len_div, int len_mul, void* stream);
+int avc_pooled_group_mean(const float* sums /*[n_rows][C]*/, const int32_t* counts /*[n_rows]*/, int64_t n_rows, int C,
+                          const int64_t* group_offsets /*[G+1]*/, int G, float* out /*[G][C]*/, void* stream);
 /* Rewrites, in place, frames of an A4 tensor (or a channel range of one: C channels of T frames, samples bstride floats
  * apart) just past each sample's L_b:
  *   AVC_TAIL_REFLECT   x[L_b + j] = x[L_b - 2 - j] for j < n (and L_b + j < T): the reflect padding F.pad applies to the
@@ -668,6 +686,28 @@ int avc_spk_group_mean(const avc_spk_group_desc* d, void* stream);
  * [0, n) mean "none" and duplicates are allowed; n_exclude = 1 gives avc_spk_group_mean's bits.  AVC_ERR_INVALID also
  * for n_exclude outside [1, 64]. */
 int avc_spk_group_mean_multi(const avc_spk_group_desc* d, int n_exclude, void* stream);
+/* avc_spk_identify: closed-set identification of m queries against a bank of s codes (speaker banks).  For query i,
+ * with s(q, v) scored exactly as avc_spk_group_mean scores it (so s(queries[i], bank[v]) is avc_spk_group_mean of the
+ * one-member group {v} bit for bit):
+ *   best[i]         = the v maximising s(queries[i], bank[v]), the lowest such v among equal scores;
+ *   best_score[i]   = that score;
+ *   target_score[i] = s(queries[i], bank[t]) for t = q_target[i] in [0, s); NaN when q_target is NULL or t is outside;
+ *   target_rank[i]  = #{v : s(queries[i], bank[v]) > target_score[i]} (0: the target is nearest); -1 with no target.
+ * One CTA per query, every bank row scored once.  All arrays on the DEVICE; no allocation, no synchronisation, no
+ * atomics: graph-capturable, and a second launch gives the same bits.  AVC_ERR_INVALID for a null descriptor or
+ * pointer (q_target may be NULL) or non-positive sizes; AVC_ERR_UNSUPPORTED for s > AVC_SPK_MAX_N or
+ * dims > AVC_SPK_MAX_DIMS. */
+typedef struct avc_spk_identify_desc {
+  int32_t m, s, dims, reserved;
+  const float* queries;     /* [m][dims] */
+  const float* bank;        /* [s][dims] */
+  const int32_t* q_target;  /* [m] bank rows, -1 = none; or NULL */
+  int32_t* best;            /* [m] */
+  double* best_score;       /* [m] */
+  double* target_score;     /* [m] */
+  int32_t* target_rank;     /* [m] */
+} avc_spk_identify_desc;
+int avc_spk_identify(const avc_spk_identify_desc* d, void* stream);
 
 /* ---- Spectral norm of the decoder weights (csrc/spectral_norm.cu): torch.nn.utils.spectral_norm with
  * n_power_iterations=1, eps=1e-12, dim=0, for a DEVICE-resident table of n layers.  W = weight viewed as [h][w]
