@@ -6,15 +6,18 @@
 // N = 32 K <= 256 and the accumulator is N / 2 <= 128 registers per consumer thread), reduction = the time rows of a
 // batch slice, WG_ROWS rows per pipeline stage.
 //
-// tf32 wgmma reads K-major operands only, and here K is time: the A4 activation layout [c/4][t][4] is MN-major for this
-// reduction.  So a staging warpgroup moves the operands through registers: it loads four 16-byte A4 units (4 channels x 4
-// consecutive time steps, 64 contiguous bytes for dc), transposes the 4 x 4 block and stores four 16-byte K-major units
-// into the no-swizzle core-matrix layout of tc_common.cuh -- per stage, plane p (time steps 4p..4p+3) holds one 16-byte
-// unit per operand row:
-//     A (dc):        [8 planes][128 co][4 t]        LBO = 128 x 16 B, SBO = 128 B
-//     B (x, by tap): [8 planes][K x 32 rows][4 t]   row j * 32 + ci holds xpad[ci][t * stride + j]
+// The A4 activation layout [c/4][t][4] is MN-major for this reduction (K is time), and tf32 wgmma reads shared-memory
+// operands K-major only.  The two operands take different routes into a stage:
+//   A (dc):  TMA copies the A4 tensor as it is, eight boxes of (4 co, 4 rows, 32 co chunks) per stage:
+//            [8 planes][32 co chunks][4 t][4 co], plane p = rows 4p..4p+3 of the chunk.  Every 4-row group lies in one
+//            sample (Tout % 8 == 0), so a box never straddles samples; rows past the slice are copied from sample B,
+//            past the end of the tensor, and arrive as zeros like co past Cout.  The consumers load their A fragments
+//            from there with ld.shared and feed wgmma from registers (wgmma_tf32_rs), which takes A in any layout.
+//   B (x, by tap): a staging warpgroup loads four 16-byte A4 units (4 channels x 4 consecutive time steps), transposes
+//            the 4 x 4 block and stores four 16-byte K-major units into the no-swizzle core-matrix layout of
+//            tc_common.cuh: [8 planes][K x 32 rows][4 t], row j * 32 + ci holds xpad[ci][t * stride + j].
 // The tap shifts, the reflect padding and the stride-2 gather are all resolved while staging, so ONE wgmma per k-step
-// covers every tap.  The fp32 bit patterns are stored as they are: the tensor core reads their TF32 part (truncation
+// covers every tap.  The fp32 bit patterns are used as they are: the tensor core reads their TF32 part (truncation
 // toward zero, the operand model of tests/test_gpu_wgrad_exact.py).
 //
 // Each CTA owns (ci tile, co tile, batch slice); its partial sums go to a scratch buffer [slice][tap][ci/4][co][4] and
@@ -22,12 +25,14 @@
 // added in place (ATOMIC, see below).
 #include "common.cuh"
 #include "tc_common.cuh"
+#include "tmap.cuh"
 
 namespace avc {
 
 constexpr int WT_NT = 32;          // ci columns per CTA per tap
-constexpr int WG_ROWS = 32;        // reduction rows (time steps) per pipeline stage: 4 wgmma k-steps, 8 K-major planes
-constexpr int WG_A_BYTES = (WG_ROWS / 4) * 128 * 16;   // dc planes of one stage
+constexpr int WG_ROWS = 32;        // reduction rows (time steps) per pipeline stage: 4 wgmma k-steps, 8 planes
+constexpr int WG_A_PLANE = 32 * 4 * 16;                  // one dc box: 32 co chunks x 4 rows x 16 bytes
+constexpr int WG_A_BYTES = (WG_ROWS / 4) * WG_A_PLANE;   // dc planes of one stage
 constexpr int WG_MAX_STAGES = 8;
 constexpr int WG_SMEM_MAX = 224 * 1024;
 
@@ -51,40 +56,25 @@ struct WgJob {
   int rot;
 };
 
-// Job e of stage chunk `ch` (rows ch * WG_ROWS .. of the CTA's slice): e < 256 stages dc (co chunk e % 32, plane e / 32),
-// the rest stage x (ci chunk e % 8, plane e / 8 % 8, tap e / 64).  Rows past the slice and channels past Cin / Cout are zeros.
+// Job e of stage chunk `ch` (rows ch * WG_ROWS .. of the CTA's slice) stages x: ci chunk e % 8, plane e / 8 % 8, tap e / 64.
+// Rows past the slice and channels past Cin are zeros.
 template <int K>
 __device__ __forceinline__ WgJob wgrad_job_load(const WgTcArgs& a, int e, int ch, int b0, int R) {
   const avc_wgrad_desc& d = a.d;
   const int T = d.Tout;
   WgJob J;
-  const bool is_dc = e < 256;
-  const int f = is_dc ? e : e - 256;
-  const int c4 = is_dc ? (f & 31) : (f & 7), pl = is_dc ? (f >> 5) : ((f >> 3) & 7), j = is_dc ? 0 : (f >> 6);
+  const int c4 = e & 7, pl = (e >> 3) & 7, j = e >> 6;
   const int r = ch * WG_ROWS + 4 * pl;
   const int g = r / T, t = r - g * T;   // T % 8 == 0: the 4 rows lie in one sample
   J.rot = (c4 >> 1) & 3;
-  if (is_dc) {
-    J.dst = (uint32_t)pl * (128u * 16u) + (uint32_t)(4 * c4) * 16u;
-    const int co = blockIdx.y * 128 + 4 * c4;
-    if (r < R && co < d.Cout) {
-      const float* src = d.dc + (size_t)(b0 + g) * d.dc_bstride + ((size_t)(co >> 2) * T + t) * 4;
+  J.dst = (uint32_t)WG_A_BYTES + (uint32_t)pl * (uint32_t)(K * WT_NT * 16) + (uint32_t)(j * WT_NT + 4 * c4) * 16u;
+  const int ci = blockIdx.x * WT_NT + 4 * c4;
+  const bool v = r < R && ci < d.Cin;
+  const float* col = d.x + (size_t)(v ? b0 + g : 0) * d.x_bstride + (size_t)((v ? ci : 0) >> 2) * d.Tin * 4;
 #pragma unroll
-      for (int i = 0; i < 4; ++i) J.v[i] = ldg4(src + 4 * i);
-    } else {
-#pragma unroll
-      for (int i = 0; i < 4; ++i) J.v[i] = zero4();
-    }
-  } else {
-    J.dst = (uint32_t)WG_A_BYTES + (uint32_t)pl * (uint32_t)(K * WT_NT * 16) + (uint32_t)(j * WT_NT + 4 * c4) * 16u;
-    const int ci = blockIdx.x * WT_NT + 4 * c4;
-    const bool v = r < R && ci < d.Cin;
-    const float* col = d.x + (size_t)(v ? b0 + g : 0) * d.x_bstride + (size_t)((v ? ci : 0) >> 2) * d.Tin * 4;
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      const int p = src_pos((t + i) * d.stride + j - d.pad_left, d.Tin, AVC_PAD_REFLECT, 1);
-      J.v[i] = (v && p >= 0) ? ldg4(col + (size_t)p * 4) : zero4();
-    }
+  for (int i = 0; i < 4; ++i) {
+    const int p = src_pos((t + i) * d.stride + j - d.pad_left, d.Tin, AVC_PAD_REFLECT, 1);
+    J.v[i] = (v && p >= 0) ? ldg4(col + (size_t)p * 4) : zero4();
   }
   return J;
 }
@@ -99,19 +89,54 @@ __device__ __forceinline__ void wgrad_job_store(uint8_t* stage, const WgJob& J) 
 
 // Staging warpgroups per CTA.  A staging thread issues all loads of its jobs of a chunk, then stores them: the chunk's
 // global-load latency is exposed once per chunk and sets the pace (the tensor cores idle most of the time).  With two
-// staging warpgroups, each takes every other chunk, so two chunks' loads are in flight at once.  512 threads leave 128
-// registers per thread, enough for the N / 2 <= 80 accumulators and the 5 jobs per thread of K <= 5; K >= 6 keeps one
-// staging warpgroup and 168 registers per thread for its up to 128 accumulators.
-__host__ __device__ constexpr int wg_stagers(int K) { return K <= 5 ? 2 : 1; }
+// staging warpgroups, each takes every other chunk, so two chunks' loads are in flight at once.  K <= 6 runs 512
+// threads; K = 7, 8 one staging warpgroup and 384 threads, because their 4 jobs per staging thread and up to 128
+// accumulators per consumer do not fit the 128 registers per thread of 512 threads.
+__host__ __device__ constexpr int wg_stagers(int K) { return K <= 6 ? 2 : 1; }
 __host__ __device__ constexpr int wg_threads(int K) { return 128 * (wg_stagers(K) + 2); }
+// Registers per thread after the setmaxnreg split of the launch allocation (the __launch_bounds__ cap: 128 at 512
+// threads, 168 at 384) between the staging warpgroups (at most 4 jobs, 18 registers each) and the consumers (N / 2
+// accumulators and two stages of A fragments, 32 registers).
+__host__ __device__ constexpr int wg_regs_stage(int K) { return wg_stagers(K) == 2 ? 96 : 104; }
+__host__ __device__ constexpr int wg_regs_mma(int K) { return wg_stagers(K) == 2 ? 160 : 200; }
+static_assert(2 * 128 * wg_regs_stage(1) + 256 * wg_regs_mma(1) <= 512 * 128 && 128 * wg_regs_stage(8) + 256 * wg_regs_mma(8) <= 384 * 168,
+              "setmaxnreg budget exceeds the launch allocation");
+
+// One stage of a consumer warpgroup: wait for the stage, load this thread's A fragments of its 4 k-steps into `af`
+// (a0..a3 of k-step k in af[4k..4k+3]), queue the 4 MMAs, then retire the previous stage's (wait_group 1).  The
+// previous stage's fragments `af_prev` were read by those MMAs: they stay live up to the wait.
+template <int N>
+__device__ __forceinline__ bool wgrad_mma_stage(const WgTcArgs& a, float* acc, uint32_t* af, uint32_t* af_prev, uint64_t* full, int s, uint32_t ph,
+                                                const uint8_t* stage, uint32_t a_off, uint32_t b_lo, uint32_t d_hi) {
+  constexpr uint32_t B_PLANE = N * 16;
+  if (!__all_sync(0xffffffffu, tc::mbar_wait(&full[s], ph, a.status, 6))) {
+    tc::wgmma_wait<0>();
+    return false;
+  }
+  // a0 = (row, t), a1 = (row + 8, t): two co chunks further; a2, a3: t + 4, the next plane
+#pragma unroll
+  for (int k = 0; k < WG_ROWS / 8; ++k)
+#pragma unroll
+    for (int q = 0; q < 4; ++q)
+      af[4 * k + q] = *reinterpret_cast<const uint32_t*>(stage + a_off + (uint32_t)(2 * k + (q >> 1)) * WG_A_PLANE + (uint32_t)(q & 1) * 128u);
+  tc::wgmma_fence();
+#pragma unroll
+  for (int k = 0; k < WG_ROWS / 8; ++k)   // k-step k: planes 2k and 2k + 1
+    tc::wgmma_tf32_rs<N>(acc, af + 4 * k, tc::sdesc64(b_lo + (uint32_t)k * ((2u * B_PLANE) >> 4), d_hi), 1u);
+  tc::wgmma_commit();
+  tc::wgmma_wait<1>();
+  tc::acc_fence(acc, N / 2);
+  tc::reg_fence(af_prev, 16);
+  return true;
+}
 
 // Weight gradient of one (ci tile, co tile, batch slice).  mbarrier ring over the slice's row chunks: full[s] = the four
-// warps of the staging warpgroup that owns the chunk wrote stage s, empty[s] = both consumer warpgroups' MMAs on stage s
-// retired.  A consumer queues the MMAs of stage i, then wait_group 1 retires those of stage i - 1 and releases it; every
-// CTA accumulates its rows in a fixed order.  No register split between the roles: the __launch_bounds__ cap (168
-// registers at 384 threads, 128 at 512) holds each instance's accumulators.
+// warps of the staging warpgroup that owns the chunk wrote the x planes of stage s, and the dc boxes of its TMA copies
+// landed (transaction bytes); empty[s] = both consumer warpgroups' MMAs on stage s retired.  A consumer queues the MMAs
+// of stage i, then wait_group 1 retires those of stage i - 1 and releases it; every CTA accumulates its rows in a fixed
+// order.  setmaxnreg moves registers from the staging warpgroups to the consumers (wg_regs_*).
 template <int K, bool ATOMIC>
-__global__ void __launch_bounds__(wg_threads(K), 1) conv_wgrad_wgmma_kernel(const WgTcArgs a) {
+__global__ void __launch_bounds__(wg_threads(K), 1) conv_wgrad_wgmma_kernel(const WgTcArgs a, const __grid_constant__ CUtensorMap tmdc) {
   constexpr int STAGERS = wg_stagers(K);
   constexpr int N = K * WT_NT;
   constexpr uint32_t B_PLANE = N * 16;
@@ -126,7 +151,7 @@ __global__ void __launch_bounds__(wg_threads(K), 1) conv_wgrad_wgmma_kernel(cons
 
   if (tid == 0) {
     for (int s = 0; s < a.nstage; ++s) {
-      tc::mbar_init(&bar_full[s], 4);
+      tc::mbar_init(&bar_full[s], 5);   // four staging warps + the arrival that carries the dc copies' bytes
       tc::mbar_init(&bar_empty[s], 2);
     }
     tc::fence_mbar_init();
@@ -138,8 +163,10 @@ __global__ void __launch_bounds__(wg_threads(K), 1) conv_wgrad_wgmma_kernel(cons
     // The global loads are the latency the staging has to hide: every load of a thread's JPT jobs of a stage is issued
     // before the first store, and before the wait for the stage to be free.  Staging warpgroup g owns the chunks
     // ch = g (mod STAGERS).  The parity wait on empty[s] cannot alias an older phase: before chunk ch this warpgroup
-    // waited for the release of chunk ch - STAGERS - nstage, and releases come in chunk order (nstage >= 4).
-    constexpr int NJOBS = 256 + 64 * K, JPT = (NJOBS + 127) / 128;
+    // waited for the release of chunk ch - STAGERS - nstage, and releases come in chunk order (nstage >= 4).  Once the
+    // stage is free, thread 0 of the warpgroup starts the TMA copies of its dc planes; they land while the x stores run.
+    tc::setmaxnreg_dec<wg_regs_stage(K)>();
+    constexpr int NJOBS = 64 * K, JPT = (NJOBS + 127) / 128;
     const int stid = tid & 127;
     for (int ch = warp >> 2; ch < nchunk; ch += STAGERS) {
       const int s = ch % a.nstage;
@@ -150,6 +177,14 @@ __global__ void __launch_bounds__(wg_threads(K), 1) conv_wgrad_wgmma_kernel(cons
         if (stid + 128 * q < NJOBS) J[q] = wgrad_job_load<K>(a, stid + 128 * q, ch, b0, R);
       if (ch >= a.nstage && !__all_sync(0xffffffffu, tc::mbar_wait(&bar_empty[s], ph ^ 1u, a.status, 5))) return;
       uint8_t* stage = smem + (size_t)s * stage_bytes;
+      if (stid == 0) {
+        tc::mbar_arrive_expect_tx(&bar_full[s], (uint32_t)WG_A_BYTES);
+#pragma unroll
+        for (int p = 0; p < WG_ROWS / 4; ++p) {
+          const int r = ch * WG_ROWS + 4 * p, g = r / d.Tout;
+          tc::tensor_g2s_4d(stage + p * WG_A_PLANE, &tmdc, 0, r - g * d.Tout, blockIdx.y * 32, r < R ? b0 + g : d.B, &bar_full[s]);
+        }
+      }
 #pragma unroll
       for (int q = 0; q < JPT; ++q)
         if (stid + 128 * q < NJOBS) wgrad_job_store(stage, J[q]);
@@ -161,39 +196,40 @@ __global__ void __launch_bounds__(wg_threads(K), 1) conv_wgrad_wgmma_kernel(cons
   }
 
   // ================================================================ MMA warpgroups
+  tc::setmaxnreg_inc<wg_regs_mma(K)>();
   const int wg = (warp >> 2) - STAGERS, wt = tid & 127;
   float acc[N / 2];
 #pragma unroll
   for (int i = 0; i < N / 2; ++i) acc[i] = 0.f;
+  // A fragment of this thread: co row m = 64 wg + 16 (wt / 32) + (wt % 32) / 4 (and m + 8), time t = wt % 4 (and t + 4)
+  // of each k-step, at [plane][m / 4][t][m % 4].  The 8 row groups of a warp's load sit in two co chunks, 64 bytes
+  // apart: with t over 4 x 16 bytes and m % 4 over 4 x 4 bytes, the 32 lanes hit 32 different banks.
+  const int m = 64 * wg + tc::wg_acc_row(wt, 0);
+  const uint32_t a_off = (uint32_t)(m >> 2) * 64u + (uint32_t)(wt & 3) * 16u + (uint32_t)(m & 3) * 4u;
+  uint32_t af[2][16];
   const uint32_t smem0 = tc::smem_u32(smem), d_hi = tc::sdesc_hi(128);
   int s = 0, s_prev = -1;
   uint32_t ph = 0;
   tc::acc_fence(acc, N / 2);
   for (int ch = 0; ch < nchunk; ++ch) {
-    if (!__all_sync(0xffffffffu, tc::mbar_wait(&bar_full[s], ph, a.status, 6))) {
-      tc::wgmma_wait<0>();
-      return;
-    }
-    const uint32_t sw = smem0 + (uint32_t)s * stage_bytes;
-    const uint32_t a_lo = tc::sdesc_lo(sw + (uint32_t)wg * 1024u, 128u * 16u), b_lo = tc::sdesc_lo(sw + (uint32_t)WG_A_BYTES, B_PLANE);
-    tc::wgmma_fence();
-#pragma unroll
-    for (int k = 0; k < WG_ROWS / 8; ++k)   // k-step k: planes 2k and 2k + 1
-      tc::wgmma_tf32<N>(acc, tc::sdesc64(a_lo + (uint32_t)k * ((2u * 128u * 16u) >> 4), d_hi),
-                        tc::sdesc64(b_lo + (uint32_t)k * ((2u * B_PLANE) >> 4), d_hi), 1u);
-    tc::wgmma_commit();
-    tc::wgmma_wait<1>();
-    tc::acc_fence(acc, N / 2);
+    const uint32_t b_lo = tc::sdesc_lo(smem0 + (uint32_t)s * stage_bytes + (uint32_t)WG_A_BYTES, B_PLANE);
+    const uint8_t* stage = smem + (size_t)s * stage_bytes;
+    // the two fragment buffers alternate by chunk (static indices: the registers stay in place under the async MMAs)
+    const bool ok = (ch & 1) ? wgrad_mma_stage<N>(a, acc, af[1], af[0], bar_full, s, ph, stage, a_off, b_lo, d_hi)
+                             : wgrad_mma_stage<N>(a, acc, af[0], af[1], bar_full, s, ph, stage, a_off, b_lo, d_hi);
+    if (!ok) return;
     if (s_prev >= 0 && wt == 0) tc::mbar_arrive(&bar_empty[s_prev]);
     s_prev = s;
     if (++s == a.nstage) { s = 0; ph ^= 1u; }
   }
   tc::wgmma_wait<0>();
   tc::acc_fence(acc, N / 2);
+  tc::reg_fence(af[0], 16);
+  tc::reg_fence(af[1], 16);
   if (nchunk == 0) return;
 
   // partial dW of this CTA: scratch[sl][tap][ci/4][co][4] (ATOMIC: added into the layer's accumulation buffer)
-  const int co = blockIdx.y * 128 + 64 * wg + tc::wg_acc_row(wt, 0);
+  const int co = blockIdx.y * 128 + m;
 #pragma unroll
   for (int jj = 0; jj < N / 8; ++jj) {
     const int n = tc::wg_acc_col(wt, 4 * jj), j = n / WT_NT, ci = blockIdx.x * WT_NT + n % WT_NT;
@@ -322,7 +358,7 @@ int wgrad_reduce(const float* scratch, float* dw, int Cout, int Cin, int K, int 
 
 // one kernel instance per tap count (N = 32 K accumulator columns) and output mode
 template <int K, bool ATOMIC>
-static int wgrad_wgmma_launch(const WgTcArgs& a, cudaStream_t stream, const char* who) {
+static int wgrad_wgmma_launch(const WgTcArgs& a, const CUtensorMap& tmdc, cudaStream_t stream, const char* who) {
   static bool attr_done = false;
   if (!attr_done) {
     const cudaError_t e = cudaFuncSetAttribute(conv_wgrad_wgmma_kernel<K, ATOMIC>, cudaFuncAttributeMaxDynamicSharedMemorySize, WG_SMEM_MAX);
@@ -334,22 +370,22 @@ static int wgrad_wgmma_launch(const WgTcArgs& a, cudaStream_t stream, const char
   }
   const dim3 grid(cdiv(a.d.Cin, WT_NT), cdiv(a.d.Cout, 128), a.nslices);
   const int smem = a.nstage * (WG_A_BYTES + 8 * 16 * WT_NT * K);
-  AVC_LAUNCH((conv_wgrad_wgmma_kernel<K, ATOMIC>), grid, wg_threads(K), smem, stream, a);
+  AVC_LAUNCH((conv_wgrad_wgmma_kernel<K, ATOMIC>), grid, wg_threads(K), smem, stream, a, tmdc);
   AVC_CHECK_LAUNCH(who);
   return AVC_OK;
 }
 
 template <bool ATOMIC>
-static int wgrad_wgmma_dispatch(const WgTcArgs& a, cudaStream_t stream, const char* who) {
+static int wgrad_wgmma_dispatch(const WgTcArgs& a, const CUtensorMap& tmdc, cudaStream_t stream, const char* who) {
   switch (a.d.K) {
-    case 1: return wgrad_wgmma_launch<1, ATOMIC>(a, stream, who);
-    case 2: return wgrad_wgmma_launch<2, ATOMIC>(a, stream, who);
-    case 3: return wgrad_wgmma_launch<3, ATOMIC>(a, stream, who);
-    case 4: return wgrad_wgmma_launch<4, ATOMIC>(a, stream, who);
-    case 5: return wgrad_wgmma_launch<5, ATOMIC>(a, stream, who);
-    case 6: return wgrad_wgmma_launch<6, ATOMIC>(a, stream, who);
-    case 7: return wgrad_wgmma_launch<7, ATOMIC>(a, stream, who);
-    default: return wgrad_wgmma_launch<8, ATOMIC>(a, stream, who);
+    case 1: return wgrad_wgmma_launch<1, ATOMIC>(a, tmdc, stream, who);
+    case 2: return wgrad_wgmma_launch<2, ATOMIC>(a, tmdc, stream, who);
+    case 3: return wgrad_wgmma_launch<3, ATOMIC>(a, tmdc, stream, who);
+    case 4: return wgrad_wgmma_launch<4, ATOMIC>(a, tmdc, stream, who);
+    case 5: return wgrad_wgmma_launch<5, ATOMIC>(a, tmdc, stream, who);
+    case 6: return wgrad_wgmma_launch<6, ATOMIC>(a, tmdc, stream, who);
+    case 7: return wgrad_wgmma_launch<7, ATOMIC>(a, tmdc, stream, who);
+    default: return wgrad_wgmma_launch<8, ATOMIC>(a, tmdc, stream, who);
   }
 }
 
@@ -368,11 +404,29 @@ static int wgrad_tc_launch(const avc_wgrad_desc* d, float* scratch, int* status,
   AVC_REQUIRE(d && d->x && d->dc && scratch && status && (accumulate || d->dw), AVC_ERR_INVALID, "%s: null argument", who);
   AVC_REQUIRE(d->B > 0 && d->Cin > 0 && d->Cout > 0 && d->Tin > 0 && d->Tout > 0, AVC_ERR_INVALID, "%s: bad shape", who);
   AVC_REQUIRE(wgrad_tc_supported(d), AVC_ERR_UNSUPPORTED, "%s: needs stride 1 (Tout <= 128) or 2 (Tout <= 64), Tout %% 8 == 0, K <= 8", who);
+  // dc goes through TMA: its base and sample stride must be 16-byte aligned (the engine's A4 tensors always are)
+  AVC_REQUIRE(((uintptr_t)d->dc & 15u) == 0 && d->dc_bstride % 4 == 0, AVC_ERR_UNSUPPORTED,
+              "%s: dc and its sample stride (%lld floats) must be 16-byte aligned", who, (long long)d->dc_bstride);
   WgTcArgs a;
   wgrad_tc_plan(d, a);
   a.scratch = scratch;
   a.status = status;
-  const int rc = accumulate ? wgrad_wgmma_dispatch<true>(a, (cudaStream_t)stream, who) : wgrad_wgmma_dispatch<false>(a, (cudaStream_t)stream, who);
+  // dc as (4 co, t, co chunk, sample); box = 4 rows x one co tile (32 chunks), out-of-range elements read as zeros
+  CUtensorMap tmdc;
+  {
+    PFN_tmap_encode enc = tmap_encode_fn();
+    AVC_REQUIRE(enc, AVC_ERR_CUDA, "%s: cuTensorMapEncodeTiled is not available from this driver", who);
+    const cuuint64_t gdim[4] = {4, (cuuint64_t)d->Tout, (cuuint64_t)(d->Cout / 4), (cuuint64_t)d->B};
+    const cuuint64_t gstr[3] = {16, (cuuint64_t)d->Tout * 16u, (cuuint64_t)d->dc_bstride * 4u};
+    const cuuint32_t box[4] = {4, 4, 32, 1};
+    const cuuint32_t estr[4] = {1, 1, 1, 1};
+    const CUresult r = enc(&tmdc, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, (void*)d->dc, gdim, gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                           CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    AVC_REQUIRE(r == CUDA_SUCCESS, AVC_ERR_CUDA, "%s: cuTensorMapEncodeTiled failed (%d) for dc: B=%d Cout=%d Tout=%d bstride=%lld", who, (int)r,
+                d->B, d->Cout, d->Tout, (long long)d->dc_bstride);
+  }
+  const int rc = accumulate ? wgrad_wgmma_dispatch<true>(a, tmdc, (cudaStream_t)stream, who)
+                            : wgrad_wgmma_dispatch<false>(a, tmdc, (cudaStream_t)stream, who);
   if (rc != AVC_OK || accumulate) return rc;
   return wgrad_reduce(scratch, d->dw, d->Cout, d->Cin, d->K, a.coutp, a.nslices, (cudaStream_t)stream);
 }
