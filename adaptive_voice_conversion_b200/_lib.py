@@ -169,6 +169,11 @@ class EvalDesc(C.Structure):
                 ("reserved", C.c_int32), ("dec", _fp), ("x", _fp), ("mu", _fp), ("ls", _fp), ("out", _fp), ("first", C.c_int64)]
 
 
+class RecVarlenDesc(C.Structure):
+    _fields_ = [("B", C.c_int32), ("C", C.c_int32), ("T", C.c_int32), ("reserved", C.c_int32), ("dec", _fp), ("x", _fp),
+                ("lengths", _fp), ("out", _fp)]
+
+
 PCM_S16, PCM_F32 = 0, 1
 RESAMPLE_TILE, RESAMPLE_MAX_TAPS, RESAMPLE_MAX_PHASE_TAPS = 512, 8192, 96
 
@@ -284,6 +289,7 @@ PROTOTYPES = {
     "avc_fill_zero": (_i, [_p, _i64, _p]),
     "avc_segment_gather": (_i, [C.POINTER(GatherDesc), _p]),
     "avc_eval_losses": (_i, [C.POINTER(EvalDesc), _p]),
+    "avc_rec_loss_varlen": (_i, [C.POINTER(RecVarlenDesc), _p]),
     "avc_stft": (_i, [C.POINTER(AudioDesc), _p]),
     "avc_istft": (_i, [C.POINTER(AudioDesc), _p]),
     "avc_griffin_lim": (_i, [C.POINTER(AudioDesc), _p]),

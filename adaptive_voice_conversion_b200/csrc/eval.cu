@@ -69,6 +69,25 @@ __global__ void __launch_bounds__(EV_THREADS) eval_losses_kernel(const avc_eval_
   }
 }
 
+// Held-out reconstruction of padded batches of different-length utterances (speaker adaptation's check).  One CTA per
+// sample; thread i adds the units i, i + 512, ... of the sample's first L_b frames in row-major (c, t) order, then the
+// block adds the partial sums in block_sum_f64's fixed tree.  Frames past L_b are never read.
+__global__ void __launch_bounds__(EV_THREADS) rec_loss_varlen_kernel(const avc_rec_varlen_desc d) {
+  __shared__ double sh[EV_THREADS / 32];
+  const int b = blockIdx.x, T = d.T;
+  const int Lb = min(max(__ldg(d.lengths + b), 0), T);
+  const int64_t units = (int64_t)d.C * Lb;
+  const float* dec = d.dec + (int64_t)b * d.C * T;
+  const float* x = d.x + (int64_t)b * d.C * T;
+  double rec = 0.0;
+  for (int64_t u = threadIdx.x; u < units; u += EV_THREADS) {
+    const int64_t c = u / Lb, t = u - c * Lb;
+    rec += fabs((double)__ldg(dec + c * T + t) - (double)__ldg(x + c * T + t));
+  }
+  rec = block_sum_f64(rec, sh);
+  if (threadIdx.x == 0) d.out[b] = rec;
+}
+
 }  // namespace avc
 
 using namespace avc;
@@ -86,5 +105,17 @@ extern "C" int avc_eval_losses(const avc_eval_desc* d, void* stream) {
   AVC_REQUIRE(d->first >= 0, AVC_ERR_INVALID, "avc_eval_losses: first must be >= 0 (got %lld)", (long long)d->first);
   eval_losses_kernel<<<(unsigned)d->B, EV_THREADS, 0, (cudaStream_t)stream>>>(*d);
   AVC_CHECK_LAUNCH("avc_eval_losses");
+  return AVC_OK;
+}
+
+extern "C" int avc_rec_loss_varlen(const avc_rec_varlen_desc* d, void* stream) {
+  AVC_REQUIRE(d != nullptr, AVC_ERR_INVALID, "avc_rec_loss_varlen: null descriptor");
+  AVC_REQUIRE(d->dec != nullptr && d->x != nullptr && d->lengths != nullptr && d->out != nullptr, AVC_ERR_INVALID,
+              "avc_rec_loss_varlen: null pointer (dec %p, x %p, lengths %p, out %p)", (const void*)d->dec,
+              (const void*)d->x, (const void*)d->lengths, (const void*)d->out);
+  AVC_REQUIRE(d->B > 0 && d->C > 0 && d->T > 0, AVC_ERR_INVALID,
+              "avc_rec_loss_varlen: sizes must be positive (B %d, C %d, T %d)", d->B, d->C, d->T);
+  rec_loss_varlen_kernel<<<(unsigned)d->B, EV_THREADS, 0, (cudaStream_t)stream>>>(*d);
+  AVC_CHECK_LAUNCH("avc_rec_loss_varlen");
   return AVC_OK;
 }

@@ -78,24 +78,33 @@ def order_seed(rank: int, epoch: int) -> int:
     return z ^ (z >> 31)
 
 
-def epoch_order(n: int, rank: int, epoch: int, shuffle: bool = True) -> torch.Tensor:
+def epoch_order(n: int, rank: int, epoch: int, shuffle: bool = True, seed: int = 0) -> torch.Tensor:
     """The order in which rank `rank` visits the n index entries in epoch `epoch` (int64, on the host): a pure
-    function of (rank, epoch), so a resumed run draws the same orders again; the index order when not shuffling."""
+    function of (rank, epoch, seed), so a resumed run draws the same orders again; the index order when not shuffling.
+    seed 0 is the training run's order; another seed (speaker adaptation's -seed) XORs seed * 0x9E3779B97F4A7C15
+    (mod 2^64, distinct for distinct seeds below 2^64) into the shuffle's generator seed."""
     if not shuffle:
         return torch.arange(n, dtype=torch.int64)
-    return torch.randperm(n, generator=torch.Generator().manual_seed(order_seed(rank, epoch)))
+    s = order_seed(rank, epoch) ^ ((seed * 0x9E3779B97F4A7C15) & _M64)
+    return torch.randperm(n, generator=torch.Generator().manual_seed(s))
 
 
 class SegmentSampler:
     """The batch schedule of a run over n index entries: batch k of the run is batch k mod ceil(n/B) of epoch
     k div ceil(n/B).  Every entry is visited once per epoch, in ``epoch_order``; the last batch of an epoch is short
-    when B does not divide n (the loader's drop_last=False).  Iterating yields the entries of each batch."""
+    when B does not divide n (the loader's drop_last=False).  Iterating yields the entries of each batch.
 
-    def __init__(self, n: int, batch_size: int, rank: int = 0, shuffle: bool = True):
+    drop_last=True (speaker adaptation): every batch has exactly B entries; an epoch is its order's first
+    floor(n/B) * B entries, the rest of that epoch's order is not visited (B <= n is required)."""
+
+    def __init__(self, n: int, batch_size: int, rank: int = 0, shuffle: bool = True, seed: int = 0,
+                 drop_last: bool = False):
         if n < 1 or batch_size < 1:
             raise ValueError(f"SegmentSampler: need n >= 1 and batch_size >= 1 (got n={n}, batch_size={batch_size})")
-        self.n, self.batch_size, self.rank, self.shuffle = n, batch_size, rank, shuffle
-        self.batches_per_epoch = -(-n // batch_size)
+        if drop_last and batch_size > n:
+            raise ValueError(f"SegmentSampler: drop_last needs batch_size <= n (got n={n}, batch_size={batch_size})")
+        self.n, self.batch_size, self.rank, self.shuffle, self.seed = n, batch_size, rank, shuffle, seed
+        self.batches_per_epoch = n // batch_size if drop_last else -(-n // batch_size)
         self.position = 0          # batches handed out so far
         self._cached = (None, None)
 
@@ -113,7 +122,7 @@ class SegmentSampler:
 
     def order(self, epoch: int) -> torch.Tensor:
         if self._cached[0] != epoch:
-            self._cached = (epoch, epoch_order(self.n, self.rank, epoch, self.shuffle))
+            self._cached = (epoch, epoch_order(self.n, self.rank, epoch, self.shuffle, self.seed))
         return self._cached[1]
 
     def step(self):
@@ -196,7 +205,8 @@ class DeviceSegments:
 
     _UPLOAD_FLOATS = 1 << 26    # host staging per host-to-device copy while loading (256 MB)
 
-    def __init__(self, data, indexes, segment_size, frame_size, batch_size, c_in, rank=0, shuffle=True, device=None):
+    def __init__(self, data, indexes, segment_size, frame_size, batch_size, c_in, rank=0, shuffle=True, device=None,
+                 seed=0, drop_last=False):
         starts, n_mels, total = validate_corpus(data, indexes, segment_size, frame_size, c_in)
         if n_mels % 4 != 0:
             raise ValueError(f"n_mels {n_mels} is not a multiple of 4: the device corpus needs 16-byte rows")
@@ -204,7 +214,7 @@ class DeviceSegments:
         self.dev = torch.device(device) if device is not None else local_device()
         self.n_mels, self.frame_size, self.segment_size, self.c_in = n_mels, frame_size, segment_size, c_in
         self.T = segment_size // frame_size
-        self.sampler = SegmentSampler(len(indexes), batch_size, rank, shuffle)
+        self.sampler = SegmentSampler(len(indexes), batch_size, rank, shuffle, seed, drop_last)
         self.corpus = torch.empty((total, n_mels), dtype=torch.float32, device=self.dev)
         row, rows, chunk = 0, 0, []
         for i, a in enumerate(data.values()):

@@ -235,7 +235,7 @@ class Engine:
         for names in (self._dense_names(), self._affine_names()):
             if all(n + ".weight" in P for n in names):
                 self._param_table("params", names, P)
-                if G is not None:
+                if G is not None and all(n + ".weight" in G for n in names):   # (speaker adaptation: decoder only)
                     self._param_table("grads", names, G)
 
     def pack_a4(self, planar: torch.Tensor, dst: A4):
@@ -1095,7 +1095,9 @@ class Engine:
         conds = self.empty(B, 2 * nblk, ch2)
         aff = []
         naff = 2 * nblk
-        fused_aff = self.fused_dense and naff <= L.LINEAR_BATCH_MAX and emb.is_contiguous()
+        # a batch stride of 0 as well: speaker adaptation conditions every sample on one code (a broadcast row)
+        fused_aff = self.fused_dense and naff <= L.LINEAR_BATCH_MAX and (
+            emb.is_contiguous() or (emb.stride(0) == 0 and emb.stride(1) == 1))
         if fused_aff:
             anames = self._affine_names(dn)
             tab = self._param_table("params", anames, P)

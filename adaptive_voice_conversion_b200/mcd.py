@@ -280,7 +280,7 @@ def _means(rows: np.ndarray) -> Dict[str, float]:
 
 def evaluate_mcd(model, data: Mapping[str, np.ndarray], attr, texts: Mapping[str, str], dims: int = 24,
                  max_pairs: int = 0, seed: int = 0, hp: AudioParams = AudioParams(), device=None,
-                 per_triplet: bool = False, n_refs: int = 1) -> dict:
+                 per_triplet: bool = False, n_refs: int = 1, target_codes=None) -> dict:
     """MCD-DTW of `model` (an AE) on one set: data = {utterance key: attr-normalised [T, n_mels]} (the set's pickle),
     texts = read_transcripts(...) of its keys.  Returns {"n", "n_short", "dims", "speakers": {target speaker: {"mcd",
     "mcd_source", "n"}}} with "mcd" and "mcd_source" when n > 0; per_triplet adds "triplets": [[source, reference,
@@ -288,7 +288,12 @@ def evaluate_mcd(model, data: Mapping[str, np.ndarray], attr, texts: Mapping[str
 
     n_refs > 1 (few-shot): each triplet keeps its reference and gets n_refs - 1 more (fewshot_triplets); the source is
     converted with the set's pooled speaker code in the batches n_refs = 1 uses.  The result then also reports
-    "n_refs" and "n_few", and a triplet row lists the references: [source, [reference, ...], target, ...]."""
+    "n_refs" and "n_few", and a triplet row lists the references: [source, [reference, ...], target, ...].
+
+    target_codes {speaker: float32 [c_out] code} (an adapted or banked speaker; n_refs 1 only): only the triplets whose
+    target speaker has a code are scored, each source converted with its target's code instead of the triplet's
+    reference (converted(..., codes=), the same batches).  The result then also reports "n_no_code", the triplets left
+    out.  None (the default) changes nothing."""
     cfg = model.config
     if int(cfg["data_loader"]["frame_size"]) != 1:
         raise ValueError(f"MCD evaluation supports data_loader.frame_size 1 only (got {cfg['data_loader']['frame_size']})")
@@ -303,6 +308,12 @@ def evaluate_mcd(model, data: Mapping[str, np.ndarray], attr, texts: Mapping[str
     if n_refs > 1:
         trip, n_few = fewshot_triplets(trip, list(data), texts, lengths, n_refs, seed, min_ref)
         res.update(n=len(trip), n_refs=int(n_refs), n_few=n_few)
+    if target_codes is not None:
+        if n_refs > 1:
+            raise ValueError("target_codes replaces the references: n_refs must be 1")
+        kept = [t for t in trip if speaker_of(t[2]) in target_codes]
+        res.update(n=len(kept), n_no_code=len(trip) - len(kept))
+        trip = kept
     if not trip:
         res["speakers"] = {}
         return res
@@ -315,7 +326,10 @@ def evaluate_mcd(model, data: Mapping[str, np.ndarray], attr, texts: Mapping[str
     model.eval()
     try:
         codes = None
-        if n_refs > 1:
+        if target_codes is not None:
+            codes = torch.stack([torch.as_tensor(target_codes[speaker_of(g)], dtype=torch.float32).reshape(-1).to(dev)
+                                 for _, _, g in trip]).contiguous()
+        elif n_refs > 1:
             from .inference import embed_reference_sets
             codes = embed_reference_sets(model, [[mels[u].t() for u in r] for _, r, _ in trip])
         first = [mels[r if n_refs == 1 else r[0]] for _, r, _ in trip]

@@ -445,6 +445,20 @@ typedef struct avc_eval_desc {
   int64_t first;    /* row of sample 0 in out */
 } avc_eval_desc;
 int avc_eval_losses(const avc_eval_desc* d, void* stream);
+/* Per-utterance reconstruction sums of a padded batch (speaker adaptation's held-out check).  For every sample b < B,
+ * with L_b = min(max(lengths[b], 0), T) (lengths: DEVICE int32 [B]; callers keep 1 <= lengths[b] <= T):
+ *   out[b] = sum_{c < C, t < L_b} |dec[b][c][t] - x[b][c][t]|    in float64 (each term and each sum)
+ * dec and x are planar [B][C][T]; frames t >= L_b are never read, whatever they hold.  One CTA per sample adds in a fixed
+ * order without atomics (avc_eval_losses' tree): a sample's sum has the same bits on every run and in any batch.
+ * AVC_ERR_INVALID, before any launch, for a null descriptor or pointer or non-positive sizes. */
+typedef struct avc_rec_varlen_desc {
+  int32_t B, C, T, reserved;
+  const float* dec;       /* planar [B][C][T] */
+  const float* x;         /* planar [B][C][T] */
+  const int32_t* lengths; /* DEVICE [B] */
+  double* out;            /* [B] */
+} avc_rec_varlen_desc;
+int avc_rec_loss_varlen(const avc_rec_varlen_desc* d, void* stream);
 
 /* ---- Vocoder DSP (csrc/audio.cu): the reference's librosa STFT / Griffin-Lim path
  * (preprocess/tacotron/utils.py get_spectrograms, melspectrogram2wav), fp32.
