@@ -174,6 +174,21 @@ class RecVarlenDesc(C.Structure):
                 ("lengths", _fp), ("out", _fp)]
 
 
+class GroupL1Desc(C.Structure):
+    _fields_ = [("B", C.c_int32), ("C", C.c_int32), ("T", C.c_int32), ("m", C.c_int32), ("round_tf32", C.c_int32),
+                ("reserved", C.c_int32), ("dec", _fp), ("x", _fp), ("hp", _fp), ("ddec", _fp), ("part", _fp), ("sums", _fp),
+                ("total", _fp)]
+
+
+CODE_MAX_C = 256
+
+
+class CodeAdamDesc(C.Structure):
+    _fields_ = [("S", C.c_int32), ("m", C.c_int32), ("C", C.c_int32), ("reserved", C.c_int32), ("demb", _fp),
+                ("codes", _fp), ("exp_avg", _fp), ("exp_avg_sq", _fp), ("max_exp_avg_sq", _fp), ("steps", _fp),
+                ("grad", _fp), ("gnorm", _fp), ("emb", _fp), ("hp", _fp)]
+
+
 PCM_S16, PCM_F32 = 0, 1
 RESAMPLE_TILE, RESAMPLE_MAX_TAPS, RESAMPLE_MAX_PHASE_TAPS = 512, 8192, 96
 
@@ -290,6 +305,8 @@ PROTOTYPES = {
     "avc_segment_gather": (_i, [C.POINTER(GatherDesc), _p]),
     "avc_eval_losses": (_i, [C.POINTER(EvalDesc), _p]),
     "avc_rec_loss_varlen": (_i, [C.POINTER(RecVarlenDesc), _p]),
+    "avc_group_l1": (_i, [C.POINTER(GroupL1Desc), _p]),
+    "avc_code_adam": (_i, [C.POINTER(CodeAdamDesc), _p]),
     "avc_stft": (_i, [C.POINTER(AudioDesc), _p]),
     "avc_istft": (_i, [C.POINTER(AudioDesc), _p]),
     "avc_griffin_lim": (_i, [C.POINTER(AudioDesc), _p]),

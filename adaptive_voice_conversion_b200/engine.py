@@ -518,6 +518,8 @@ class Engine:
         """Register the persistent gradient buffers G for in-place accumulation: one zeroed arena
         with a [K][Cin/4][coutp][4] region per conv layer and the device item table of the flush
         kernel.  Must run before a CUDA-graph capture (it copies the table to the device)."""
+        if G is None:   # no gradient buffer (a data-gradient-only backward): nothing to register, keep the arena
+            return
         if not self.wgrad_acc or self.precision != "tf32":
             self._wg_acc = None
             return
@@ -635,9 +637,12 @@ class Engine:
 
     def conv_bwd(self, P, G, rec, dy: Optional[A4], *, need_dx=True, dres: Optional[A4] = None, dres_mode=L.RES_NONE,
                  dcond: Optional[torch.Tensor] = None, mask: Optional[A4] = None, dx_channels=None,
-                 dc_pre: Optional[A4] = None, fuse_up: Optional[dict] = None) -> Optional[A4]:
+                 dc_pre: Optional[A4] = None, fuse_up: Optional[dict] = None, need_wgrad=True) -> Optional[A4]:
         """Backward of one conv block.  dy: grad w.r.t. the block output *before* the residual
         add.  Returns grad w.r.t. the block input (+ adjoint of the residual branch `dres`).
+
+        need_wgrad=False: data gradients only -- no weight-gradient launch and no bias-gradient write (neither this
+        block's nor, in a fused norm backward, the upstream block's); G is not read and may be None.
 
         dc_pre: the gradient w.r.t. this block's raw conv output, already produced by the downstream block's fused
         epilogue (then dy is ignored).  fuse_up = {"rec": upstream block, "dcond": its AdaIN-row gradient or None,
@@ -647,7 +652,7 @@ class Engine:
         name, xin, B = rec["name"], rec["xin"], rec["xin"].B
         K, Cin, Cout, Tout, stride = rec["K"], rec["Cin"], rec["Cout"], rec["Tout"], rec["stride"]
         st = self.stream
-        gb = G[name + ".bias"]
+        gb = G[name + ".bias"] if need_wgrad else None
         if fuse_up is not None:
             fuse_up["dc"] = None
         if dc_pre is not None:
@@ -666,7 +671,7 @@ class Engine:
             # the bias of a conv that feeds an InstanceNorm has an identically zero gradient (the norm removes the
             # per-channel mean); autograd returns ~1e-9 rounding noise there, we leave the zeroed buffer untouched
             # (not with pixel shuffle: there two conv rows with different biases share one normalised channel)
-            d.dc, d.dbias = dc.ptr, (None if (rec["norm"] and not rec["shuffle"]) else gb.data_ptr())
+            d.dc, d.dbias = dc.ptr, (None if (rec["norm"] and not rec["shuffle"]) or gb is None else gb.data_ptr())
             if d.dbias:
                 # per-block partial sums reduced in a fixed order: atomics would make the gradient (and every later
                 # step) vary from run to run
@@ -680,14 +685,16 @@ class Engine:
                 self.debug(name, "dc", dc)
         else:
             dc = dy
-            self._ck(self.lib.avc_bias_grad(dc.ptr, dc.bstride, gb.data_ptr(), B, Cout, Tout, st), f"bias_grad[{name}]")
-        wd = L.WgradDesc()
-        wd.B, wd.Cin, wd.Cout, wd.K, wd.stride, wd.pad_left, wd.Tin, wd.Tout = B, Cin, Cout, K, stride, rec["pl"], xin.T, Tout
-        wd.x, wd.x_bstride, wd.dc, wd.dc_bstride = xin.ptr, xin.bstride, dc.ptr, dc.bstride
-        wd.dw = G[name + ".weight"].data_ptr()
-        self.wgrad(wd, name, keep=(xin.t, dc.t))
-        if self.debug:
-            self.debug(name, "dw", G[name + ".weight"])
+            if need_wgrad:
+                self._ck(self.lib.avc_bias_grad(dc.ptr, dc.bstride, gb.data_ptr(), B, Cout, Tout, st), f"bias_grad[{name}]")
+        if need_wgrad:
+            wd = L.WgradDesc()
+            wd.B, wd.Cin, wd.Cout, wd.K, wd.stride, wd.pad_left, wd.Tin, wd.Tout = B, Cin, Cout, K, stride, rec["pl"], xin.T, Tout
+            wd.x, wd.x_bstride, wd.dc, wd.dc_bstride = xin.ptr, xin.bstride, dc.ptr, dc.bstride
+            wd.dw = G[name + ".weight"].data_ptr()
+            self.wgrad(wd, name, keep=(xin.t, dc.t))
+            if self.debug:
+                self.debug(name, "dw", G[name + ".weight"])
         if not need_dx:
             return None
         # data gradient: full transposed conv (zero pad) then fold the reflect halo back
@@ -738,7 +745,7 @@ class Engine:
                         d.cond, d.cond_bstride = up["cond"].data_ptr(), up["cond"].stride(0)
                         d.dcond, d.dcond_bstride = fuse_up["dcond"].data_ptr(), fuse_up["dcond"].stride(0)
                     d.dc = dc_up.ptr
-                    d.dbias = None if up["norm"] else G[up["name"] + ".bias"].data_ptr()
+                    d.dbias = None if (up["norm"] or not need_wgrad) else G[up["name"] + ".bias"].data_ptr()
                     if not fuse_up.get("need_dx", True):
                         d.out = None
                     self._ck(self.lib.avc_conv_block_tc(C.byref(d), self.tc_status.data_ptr(), st), f"conv_dgrad_tc_fold_normbwd[{name}]")
@@ -1142,56 +1149,65 @@ class Engine:
             ctx.update(in_rec=r_in, aff=aff, blocks=blocks, out_rec=r_out, conds=conds, emb=emb)
         return dec4, ctx
 
-    def decoder_bwd(self, P, G, ctx, ddec4: A4, need_dz=True, affine_stream=None):
+    def decoder_bwd(self, P, G, ctx, ddec4: A4, need_dz=True, affine_stream=None, need_wgrad=True):
         """Returns (dz4, demb).  affine_stream: the gradients of the AdaIN affine layers (and demb, which only the
         speaker encoder's backward needs) are complete after the block loop; with a stream given they fork onto it
         there, beside the in_conv data gradient -- demb is then produced ON that stream (the caller continues the
-        speaker branch on it) and the tensors the forked launches read stay alive in ctx."""
+        speaker branch on it) and the tensors the forked launches read stay alive in ctx.
+
+        need_wgrad=False: the data gradients dz and demb only (speaker-code fitting).  No weight- or bias-gradient
+        launch, no affine-layer weight gradient; nothing is written to a gradient buffer and G may be None.  dz and
+        demb are those of the full backward bit for bit (no data gradient reads a weight gradient)."""
         c = self.cfg["Decoder"]
         nblk = c["n_conv_blocks"]
-        dout = self.conv_bwd(P, G, ctx["out_rec"], ddec4)
+        wg = {} if need_wgrad else {"need_wgrad": False}   # (the default keeps every call exactly as it was)
+        dout = self.conv_bwd(P, G, ctx["out_rec"], ddec4, **wg)
         dconds = self.empty(*ctx["conds"].shape)
         blocks = ctx["blocks"]
         dc2 = None
         for l in reversed(range(nblk)):
             r1, r2, up = blocks[l]
             f1 = dict(rec=r1, dcond=dconds[:, 2 * l], need_dx=False)
-            dy1 = self.conv_bwd(P, G, r2, dout, dcond=dconds[:, 2 * l + 1], dc_pre=dc2, fuse_up=f1)
+            dy1 = self.conv_bwd(P, G, r2, dout, dcond=dconds[:, 2 * l + 1], dc_pre=dc2, fuse_up=f1, **wg)
             if l > 0:
                 f2 = dict(rec=blocks[l - 1][1], dcond=dconds[:, 2 * l - 1], need_dx=True)
             else:
                 f2 = dict(rec=ctx["in_rec"], dcond=None, need_dx=False)
             dout = self.conv_bwd(P, G, r1, dy1, dc_pre=f1["dc"], dres=dout, dres_mode=L.RES_UP if up > 1 else L.RES_SAME,
-                                 dcond=dconds[:, 2 * l], fuse_up=f2)
+                                 dcond=dconds[:, 2 * l], fuse_up=f2, **wg)
             dc2 = f2["dc"]
         if affine_stream is not None:
             affine_stream.wait_stream(torch.cuda.current_stream(self.dev))
             with torch.cuda.stream(affine_stream):
-                demb = self._decoder_affine_bwd(P, G, ctx, dconds)
+                demb = self._decoder_affine_bwd(P, G, ctx, dconds, **wg)
             ctx["_keep_bwd"] = (dconds,)
-            dz4 = self.conv_bwd(P, G, ctx["in_rec"], dout, dc_pre=dc2, need_dx=need_dz)
+            dz4 = self.conv_bwd(P, G, ctx["in_rec"], dout, dc_pre=dc2, need_dx=need_dz, **wg)
             return dz4, demb
-        dz4 = self.conv_bwd(P, G, ctx["in_rec"], dout, dc_pre=dc2, need_dx=need_dz)
-        return dz4, self._decoder_affine_bwd(P, G, ctx, dconds)
+        dz4 = self.conv_bwd(P, G, ctx["in_rec"], dout, dc_pre=dc2, need_dx=need_dz, **wg)
+        return dz4, self._decoder_affine_bwd(P, G, ctx, dconds, **wg)
 
-    def _decoder_affine_bwd(self, P, G, ctx, dconds):
+    def _decoder_affine_bwd(self, P, G, ctx, dconds, need_wgrad=True):
         demb = None
         aff = ctx["aff"]
-        if isinstance(aff, dict):   # the 2n affine layers in three launches
+        if isinstance(aff, dict):   # the 2n affine layers in three launches (two without the weight gradients)
             emb = ctx["emb"]
             naff, B, ch2, K = len(aff["names"]), emb.shape[0], dconds.shape[2], emb.shape[1]
-            gtab = self._param_table("grads", aff["names"], G)
+            gtab = self._param_table("grads", aff["names"], G) if need_wgrad else None
             part, demb = self.empty(naff, B, K), self.empty(B, K)
             bd = L.LinearBatchDesc()
             bd.L, bd.B, bd.N, bd.K = naff, B, ch2, K
-            bd.params, bd.grads = aff["tab"].data_ptr(), gtab.data_ptr()
+            bd.params, bd.grads = aff["tab"].data_ptr(), _ptr(gtab)
             bd.x, bd.x_bstride = emb.data_ptr(), emb.stride(0)
             bd.y, bd.y_bstride = dconds.data_ptr(), naff * ch2
             for i in range(naff):
                 bd.x_off[i], bd.y_off[i] = 0, i * ch2
             bd.part, bd.dx = part.data_ptr(), demb.data_ptr()
             self._ck(self.lib.avc_linear_batch_dx(C.byref(bd), self.stream), "linear_batch_dx[affine]")
-            self._ck(self.lib.avc_linear_batch_dw(C.byref(bd), self.stream), "linear_batch_dw[affine]")
+            if need_wgrad:
+                self._ck(self.lib.avc_linear_batch_dw(C.byref(bd), self.stream), "linear_batch_dw[affine]")
+        elif not need_wgrad:
+            raise L.AvcError("decoder_bwd(need_wgrad=False) needs the fused AdaIN affine path (AVC_FUSED_DENSE=1, "
+                             "contiguous speaker codes)")
         else:
             for i, r in enumerate(aff):
                 demb = self.linear_bwd(P, G, r, dconds[:, i], dx_add=demb)

@@ -16,6 +16,10 @@ same order in one batch, whatever the packing.
 A bank records a fingerprint of the speaker encoder that made it (sha256 over its state_dict entries: names, shapes and
 float32 bytes in key order, then its config).  A code only means something to that encoder, so ``load`` refuses a bank
 whose fingerprint does not match the model.
+
+A bank whose codes were fitted to the model (``fit.fit_bank``) also carries a ``fitted`` record: the run's steps and
+settings and ``model_fingerprint``, a sha256 of the content encoder and the decoder the codes were fitted through.
+``load`` refuses such a bank against a model whose record does not match; a bank without the record loads as before.
 """
 from __future__ import annotations
 
@@ -77,10 +81,12 @@ class SpeakerBank:
 
     speakers: names in sorted order; codes: float32 [S, c_out] (row s is speakers[s]'s); n_utts[s]: the utterances
     pooled into code s, which are utterances[s] (sorted ids); n_skipped: utterances too short to embed; fingerprint:
-    the speaker encoder's (``fingerprint``)."""
+    the speaker encoder's (``fingerprint``); fitted: None, or the record of the fitting run that tuned the codes to a
+    content encoder and decoder (``fit.fit_bank``; plain values only, with "model_fingerprint")."""
 
     def __init__(self, speakers: Sequence[str], codes: torch.Tensor, n_utts: Sequence[int],
-                 utterances: Sequence[Sequence[str]], fingerprint: str, n_skipped: int = 0):
+                 utterances: Sequence[Sequence[str]], fingerprint: str, n_skipped: int = 0,
+                 fitted: Optional[dict] = None):
         speakers = [str(s) for s in speakers]
         if len(set(speakers)) != len(speakers) or list(speakers) != sorted(speakers):
             raise ValueError("SpeakerBank: speakers must be unique and sorted")
@@ -96,6 +102,9 @@ class SpeakerBank:
         self.utterances = [[str(u) for u in us] for us in utterances]
         self.fingerprint = str(fingerprint)
         self.n_skipped = int(n_skipped)
+        if fitted is not None and not isinstance(fitted.get("model_fingerprint"), str):
+            raise ValueError("SpeakerBank: a fitted record needs its model_fingerprint")
+        self.fitted = None if fitted is None else dict(fitted)
         self._index = {s: i for i, s in enumerate(speakers)}
 
     def __len__(self):
@@ -130,15 +139,20 @@ class SpeakerBank:
         return (acc / wsum).to(dtype=torch.float32, device=self.codes.device)
 
     def save(self, path: str):
-        """torch.save of plain tensors, lists and strings (loadable with weights_only=True)."""
-        torch.save({"format": FORMAT, "speakers": list(self.speakers), "codes": self.codes.detach().cpu().contiguous(),
-                    "n_utts": list(self.n_utts), "utterances": [list(u) for u in self.utterances],
-                    "fingerprint": self.fingerprint, "n_skipped": self.n_skipped}, path)
+        """torch.save of plain tensors, lists and strings (loadable with weights_only=True).  The "fitted" entry is
+        written only for a fitted bank."""
+        d = {"format": FORMAT, "speakers": list(self.speakers), "codes": self.codes.detach().cpu().contiguous(),
+             "n_utts": list(self.n_utts), "utterances": [list(u) for u in self.utterances],
+             "fingerprint": self.fingerprint, "n_skipped": self.n_skipped}
+        if self.fitted is not None:
+            d["fitted"] = dict(self.fitted)
+        torch.save(d, path)
 
     @classmethod
     def load(cls, path: str, model) -> "SpeakerBank":
         """The bank saved at `path`, its codes on `model`'s device.  ValueError when it was not made by `model`'s speaker
-        encoder (fingerprint mismatch) or is not a bank file."""
+        encoder (fingerprint mismatch), when its codes were fitted to another content encoder or decoder (the fitted
+        record's model_fingerprint), or when it is not a bank file."""
         d = torch.load(path, map_location="cpu", weights_only=True)
         if not isinstance(d, dict) or d.get("format") != FORMAT:
             raise ValueError(f"{path}: not a speaker bank ({FORMAT})")
@@ -146,8 +160,17 @@ class SpeakerBank:
         if d["fingerprint"] != fp:
             raise ValueError(f"{path}: the bank was made by a different speaker encoder (fingerprint "
                              f"{d['fingerprint'][:12]}..., the model's {fp[:12]}...); its codes mean nothing to this model")
+        fitted = d.get("fitted")
+        if fitted is not None:
+            from .fit import model_fingerprint
+            mf = model_fingerprint(model)
+            if fitted.get("model_fingerprint") != mf:
+                raise ValueError(f"{path}: the codes were fitted to a different content encoder or decoder (fingerprint "
+                                 f"{str(fitted.get('model_fingerprint'))[:12]}..., the model's {mf[:12]}...); they are "
+                                 f"tuned to that model")
         dev = next(model.parameters()).device
-        return cls(d["speakers"], d["codes"].to(dev), d["n_utts"], d["utterances"], d["fingerprint"], d["n_skipped"])
+        return cls(d["speakers"], d["codes"].to(dev), d["n_utts"], d["utterances"], d["fingerprint"], d["n_skipped"],
+                   fitted=fitted)
 
 
 def bank_order(ids: Sequence[str], lengths: Mapping[str, int], min_len: int,

@@ -460,6 +460,57 @@ typedef struct avc_rec_varlen_desc {
 } avc_rec_varlen_desc;
 int avc_rec_loss_varlen(const avc_rec_varlen_desc* d, void* stream);
 
+/* ---- Speaker-code fitting (csrc/fit.cu, fit.CodeFitTrainer).  A batch of B = G * m samples holds G groups (speakers)
+ * of m consecutive samples each: sample b belongs to group b / m.
+ *
+ * avc_group_l1: the grouped L1 loss and its gradient in one pass.  With grec = hp[0] / (float)(m * C * T):
+ *   ddec = grec * sign(dec - x), 0 where dec == x (avc_vae_loss's convention), written in dec's A4 layout; with
+ *          round_tf32 != 0 each value is rounded to TF32 (cvt.rna) as avc_pack_a4 rounds, so the result is what
+ *          avc_vae_loss + avc_pack_a4 give for one group of m = B;
+ *   part[b] = sum_{c, t} |dec - x| of sample b in float64, in avc_eval_losses' fixed order;
+ *   sums[g] = part[g m] + part[g m + 1] + ... in ascending sample order (float64);
+ *   total (or null) = (float)(sums[0] + sums[1] + ...), the batch's L1 sum.
+ * dec and ddec are whole A4 tensors [B][C/4][T][4] (batch stride C*T), x is planar [B][C][T].  Two launches, no
+ * atomics: every sum has the same bits on every run and whatever the other groups hold.
+ * AVC_ERR_INVALID for null pointers (but total), non-positive sizes, C % 4 != 0 or B % m != 0. */
+typedef struct avc_group_l1_desc {
+  int32_t B, C, T, m;
+  int32_t round_tf32, reserved;
+  const float* dec; /* A4 [B][C/4][T][4] */
+  const float* x;   /* planar [B][C][T] */
+  const float* hp;  /* DEVICE: hp[0] = lambda (the trainers' hyper-parameter vector) */
+  float* ddec;      /* A4, dec's layout */
+  double* part;     /* [B] */
+  double* sums;     /* [G] */
+  float* total;     /* [1] or null */
+} avc_group_l1_desc;
+int avc_group_l1(const avc_group_l1_desc* d, void* stream);
+
+/* avc_code_adam: clip_grad_norm_ + Adam(amsgrad, L2 weight decay) of every code on its own.  One CTA per code s < S:
+ *   g_s[c]   = sum_{j < m} demb[s m + j][c], added in avc_bias_grad's order at T = 1 (so avc_bias_grad over the same
+ *              m rows gives g_s bit for bit); written to grad[s][c];
+ *   gnorm[s] = hp[2] * sqrt(sum_c g_s[c]^2) (sum in a fixed order);
+ *   steps[s] += 1, then avc_adam_step's clip coefficient min(1, hp[8] / (gnorm + 1e-6)) * hp[2], L2 decay and Adam
+ *              (hp layout of avc_adam_step) on codes[s], exp_avg[s], exp_avg_sq[s], max_exp_avg_sq[s];
+ *   emb[s m + j] = the updated codes[s] for j < m: the expanded rows the next step's AdaIN affine layers read.
+ * A code's bits depend on its own rows only.  No atomics.  AVC_ERR_INVALID for null pointers, S, m or C < 1,
+ * C % 4 != 0 or C > AVC_CODE_MAX_C. */
+#define AVC_CODE_MAX_C 256
+typedef struct avc_code_adam_desc {
+  int32_t S, m, C, reserved;
+  const float* demb;     /* [S*m][C] dense */
+  float* codes;          /* [S][C] */
+  float* exp_avg;        /* [S][C] */
+  float* exp_avg_sq;     /* [S][C] */
+  float* max_exp_avg_sq; /* [S][C] */
+  float* steps;          /* [S] */
+  float* grad;           /* [S][C] */
+  float* gnorm;          /* [S] */
+  float* emb;            /* [S*m][C] */
+  const float* hp;       /* DEVICE, avc_adam_step's layout */
+} avc_code_adam_desc;
+int avc_code_adam(const avc_code_adam_desc* d, void* stream);
+
 /* ---- Vocoder DSP (csrc/audio.cu): the reference's librosa STFT / Griffin-Lim path
  * (preprocess/tacotron/utils.py get_spectrograms, melspectrogram2wav), fp32.
  *

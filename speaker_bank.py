@@ -10,6 +10,17 @@ From your own recordings, analysed by the GPU vocoder and normalised with -a (re
     python speaker_bank.py -c config.yaml -m model.ckpt -a attr.pkl -wav alice a1.wav a2.wav -wav bob b1.wav -o bank.pt
 
 Prints the number of speakers, the utterances pooled and the utterances skipped (shorter than the model accepts).
+
+With -fit_steps the pooled codes are then fitted to the model (adaptive_voice_conversion_b200/fit.py): each speaker's
+code is optimised on that speaker's own recordings with every model weight frozen, many speakers per step, and the bank
+records the content encoder and decoder it was fitted to.  Held out on another set, with MCD-DTW on its parallel
+utterances when -transcripts is given:
+
+    python speaker_bank.py -c config.yaml -m model.ckpt -d data/ -set train -o bank.pt -fit_steps 300 \
+        [-fit_lr LR] [-fit_crops 8] [-fit_speakers 16] [-seed 0] [-holdout_set in_test] [-transcripts DIR] \
+        [-report out.json]
+
+The defaults of -fit_steps, -fit_lr (the config's rate), -fit_crops and -fit_speakers are not tuned.
 data_loader.frame_size 1 only.
 """
 import os
@@ -33,6 +44,14 @@ def parser():
     p.add_argument("-attr", "-a", help="mel statistics for -wav recordings")
     p.add_argument("-wav", nargs="+", action="append", metavar=("NAME", "FILE"),
                    help="a speaker's name and recordings (repeatable)")
+    p.add_argument("-fit_steps", type=int, default=None, help="fit every code to the model for this many steps")
+    p.add_argument("-fit_lr", type=float, default=None, help="Adam's rate of the fit (default: the config's; not tuned)")
+    p.add_argument("-fit_crops", type=int, default=8, help="crops per speaker and step (not tuned)")
+    p.add_argument("-fit_speakers", type=int, default=16, help="speakers per step (a speed-up only; not tuned)")
+    p.add_argument("-seed", type=int, default=0, help="seed of every speaker's crop order")
+    p.add_argument("-holdout_set", help="held-out set of the banked speakers: <data_dir>/<holdout_set>.pkl (with -d)")
+    p.add_argument("-transcripts", help="directory of <id>.txt transcripts: MCD-DTW on -holdout_set")
+    p.add_argument("-report", help="fit report to write (JSON)")
     return p
 
 
@@ -56,6 +75,19 @@ def check_args(p, args):
                     p.error(f"-wav {w[0]}: {f} is not a file")
     elif not (args.data_dir and args.set):
         p.error("-d and -set go together")
+    fit_only = [f"-{k}" for k in ("fit_lr", "holdout_set", "transcripts", "report") if getattr(args, k) is not None]
+    if args.fit_steps is None:
+        if fit_only:
+            p.error(f"{', '.join(fit_only)} go(es) with -fit_steps")
+        return
+    if args.fit_steps < 1 or args.fit_crops < 1 or args.fit_speakers < 1:
+        p.error("-fit_steps, -fit_crops and -fit_speakers must be >= 1")
+    if args.fit_lr is not None and not args.fit_lr > 0:
+        p.error("-fit_lr must be > 0")
+    if args.holdout_set and not args.data_dir:
+        p.error("-holdout_set goes with -d (a held-out set of the prepared data)")
+    if args.transcripts and not args.holdout_set:
+        p.error("-transcripts needs -holdout_set (the set MCD-DTW is measured on)")
 
 
 def set_mels(args):
@@ -92,6 +124,41 @@ def wav_mels(args, config, dev):
     return mels, owner.__getitem__
 
 
+def holdout_mels(args, bank, speaker_of):
+    """(the held-out set's pickle, {speaker: {id: mel}} of the bank's speakers in it).  SystemExit when a held-out
+    utterance is one the bank pooled (and so would be fitted on)."""
+    from adaptive_voice_conversion_b200.adapt import check_disjoint
+    with open(os.path.join(args.data_dir, f"{args.holdout_set}.pkl"), "rb") as f:
+        data = pickle.load(f)
+    try:
+        check_disjoint(bank.utterance_ids(), list(data))
+    except ValueError as e:
+        raise SystemExit(f"speaker_bank.py: {e}")
+    held = {}
+    for u in sorted(data):
+        if speaker_of(u) in bank:
+            held.setdefault(speaker_of(u), {})[u] = data[u]
+    return data, held
+
+
+def fit(args, model, bank, mels, speaker_of):
+    """fit_bank with the -fit_* settings; held out on -holdout_set (MCD-DTW with -transcripts).  -> (bank, report)"""
+    from adaptive_voice_conversion_b200.fit import fit_bank
+    held, mcd = None, None
+    if args.holdout_set:
+        data, held = holdout_mels(args, bank, speaker_of)
+        if args.transcripts:
+            from adaptive_voice_conversion_b200.mcd import evaluate_mcd, read_transcripts
+            with open(os.path.join(args.data_dir, "attr.pkl"), "rb") as f:
+                attr = pickle.load(f)
+            texts = read_transcripts(args.transcripts, data)
+
+            def mcd(m, codes):
+                return evaluate_mcd(m, data, attr, texts, seed=args.seed, target_codes=codes)
+    return fit_bank(model, bank, mels, args.fit_steps, lr=args.fit_lr, crops=args.fit_crops,
+                    speakers_per_wave=args.fit_speakers, seed=args.seed, heldout=held, mcd=mcd)
+
+
 def main(argv=None):
     p = parser()
     args = p.parse_args(argv)
@@ -108,8 +175,19 @@ def main(argv=None):
     model.eval()
     mels, speaker_of = wav_mels(args, config, dev) if args.wav else set_mels(args)
     bank = build_bank(model, mels, speaker_of=speaker_of)
+    if args.fit_steps is None:
+        bank.save(args.output)
+        print(f"bank: {len(bank)} speakers, {sum(bank.n_utts)} utterances pooled, {bank.n_skipped} skipped -> {args.output}")
+        return bank
+    bank, report = fit(args, model, bank, mels, speaker_of)
     bank.save(args.output)
-    print(f"bank: {len(bank)} speakers, {sum(bank.n_utts)} utterances pooled, {bank.n_skipped} skipped -> {args.output}")
+    if args.report:
+        import json
+        with open(args.report, "w") as f:
+            json.dump(report, f, indent=1)
+    n_fit = len(bank) - len(report["unfitted"])
+    print(f"bank: {len(bank)} speakers, {sum(bank.n_utts)} utterances pooled, {bank.n_skipped} skipped; {n_fit} codes "
+          f"fitted for {args.fit_steps} steps, {len(report['unfitted'])} unfitted -> {args.output}")
     return bank
 
 
