@@ -137,6 +137,8 @@ class LinearBatchDesc(C.Structure):
 
 STFT_MAG, STFT_COMPLEX, STFT_PROJECT, STFT_PROJECT_FIRST = 0, 1, 2, 3
 MEL_TO_MAG, MAG_TO_MEL = 0, 1
+GL_START_ZERO, GL_START_X, GL_START_PGHI = 0, 1, 2
+PGHI_NONE, PGHI_TIME, PGHI_LEFT, PGHI_RIGHT, PGHI_SEED = 0, 1, 2, 3, 4
 
 
 class AudioSeg(C.Structure):
@@ -310,6 +312,8 @@ PROTOTYPES = {
     "avc_stft": (_i, [C.POINTER(AudioDesc), _p]),
     "avc_istft": (_i, [C.POINTER(AudioDesc), _p]),
     "avc_griffin_lim": (_i, [C.POINTER(AudioDesc), _p]),
+    "avc_griffin_lim_from": (_i, [C.POINTER(AudioDesc), C.c_int32, C.c_float, _p]),
+    "avc_pghi": (_i, [C.POINTER(AudioDesc), C.c_float, _p, _p]),
     "avc_frame_power": (_i, [C.POINTER(AudioDesc), _p, _p]),
     "avc_deemphasis": (_i, [C.POINTER(AudioDesc), C.c_float, _p]),
     "avc_mel_project": (_i, [C.POINTER(MelDesc), _p]),

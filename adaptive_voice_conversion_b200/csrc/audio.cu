@@ -1,6 +1,7 @@
-// The vocoder's DSP: STFT / iSTFT on a shared-memory 2048-point real FFT, Griffin-Lim, the mel projections, the
-// de-emphasis recurrence and the per-frame power of the silence trim.  fp32 throughout, no atomics: every output
-// element is computed by one thread in a fixed order, so a ragged batch gives each utterance the bits it gets alone.
+// The vocoder's DSP: STFT / iSTFT on a shared-memory 2048-point real FFT, Griffin-Lim and its PGHI start phase, the
+// mel projections, the de-emphasis recurrence and the per-frame power of the silence trim.  fp32 (PGHI's phases in
+// float64), no atomics: every output element is computed by one thread in a fixed order, so a ragged batch gives each
+// utterance the bits it gets alone.
 #include <float.h>
 
 #include <cmath>
@@ -373,6 +374,296 @@ __global__ void __launch_bounds__(256) mel_gemm_kernel(avc_mel_desc d) {
   }
 }
 
+// ------------------------------------------------------------------ PGHI start phase
+// One CTA per utterance walks its frames in order.  Thread t owns the PG_PER contiguous bins from PG_PER t, so each
+// per-frame block scan folds a thread's bins in order and combines threads with warp shuffles and one shared-memory
+// pass over the warp totals: a fixed order, no atomics.  Three rows of ln-magnitude (frames f-1, f, f+1) sit in shared
+// memory in float64; each thread keeps its bins' phases of frame f-1 in registers, wrapped, in float64.
+//
+// A heap key orders the integration's sources: larger magnitude, then frame f-1 before frame f, then the lower bin.
+// It is (float bits of s) << 12 | (frame f-1) << 11 | (2047 - k); 0 is "insignificant" (-inf).  With a_k the key of
+// (f-1, k) and c_k that of (f, k), the heap assigns (f, k) from the largest of three candidates: the time source a_k,
+// the left path min(L_{k-1}, c_{k-1}) and the right path min(R_{k+1}, c_{k+1}), with the directional levels
+// L_k = max(a_k, min(L_{k-1}, c_{k-1})) and R_k = max(a_k, min(R_{k+1}, c_{k+1})).  Both are scans of the clamp maps
+// x -> max(a, min(x, b)).  A significant bin with no candidate is in a run that no source reaches; the heap seeds
+// such a run at its largest key and the run's other bins point toward the seed.  Phases are then segmented sums of
+// the trapezoid steps along the left- and right-parented chains, from their time-parented or seed roots.
+constexpr int PG_THREADS = 256;
+constexpr int PG_WARPS = PG_THREADS / 32;
+constexpr int PG_PER = 5;                                      // bins per thread: 205 threads cover the 1025 bins
+constexpr int PG_LOADS = (NBIN + PG_THREADS - 1) / PG_THREADS; // coalesced loads of a row per thread
+static_assert(PG_THREADS * PG_PER >= NBIN, "every bin needs a thread");
+
+typedef unsigned long long u64;
+struct Pair {
+  u64 a, b;
+};
+// clamp map x -> min(max(x, a), b) with a <= b (x -> max(a, min(x, b')) is the clamp to [a, max(a, b')]);
+// f(e, l) applies e, then l
+struct ClampOp {
+  __device__ static Pair id() { return {0ull, ~0ull}; }
+  __device__ static Pair f(Pair e, Pair l) {
+    return {min(max(e.a, l.a), l.b), min(max(e.b, l.a), l.b)};
+  }
+};
+// segmented max: a = starts a segment, b = key
+struct SegMaxOp {
+  __device__ static Pair id() { return {0ull, 0ull}; }
+  __device__ static Pair f(Pair e, Pair l) { return l.a ? l : Pair{e.a, max(e.b, l.b)}; }
+};
+// segmented sum: a = starts a segment, b = float64 bits
+struct SegSumOp {
+  __device__ static Pair id() { return {0ull, 0ull}; }
+  __device__ static Pair f(Pair e, Pair l) {
+    return l.a ? l : Pair{e.a, (u64)__double_as_longlong(__longlong_as_double((long long)e.b) +
+                                                         __longlong_as_double((long long)l.b))};
+  }
+};
+
+// Exclusive block scan of one element per thread, in thread order (REV: from the last thread down).
+template <class Op, bool REV>
+__device__ __forceinline__ Pair block_scan_excl(Pair v, Pair* sh) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    Pair u;
+    u.a = REV ? __shfl_down_sync(0xffffffffu, v.a, o) : __shfl_up_sync(0xffffffffu, v.a, o);
+    u.b = REV ? __shfl_down_sync(0xffffffffu, v.b, o) : __shfl_up_sync(0xffffffffu, v.b, o);
+    if (REV ? lane + o < 32 : lane >= o) v = Op::f(u, v);
+  }
+  Pair ex;
+  ex.a = REV ? __shfl_down_sync(0xffffffffu, v.a, 1) : __shfl_up_sync(0xffffffffu, v.a, 1);
+  ex.b = REV ? __shfl_down_sync(0xffffffffu, v.b, 1) : __shfl_up_sync(0xffffffffu, v.b, 1);
+  if (lane == (REV ? 31 : 0)) ex = Op::id();
+  if (lane == (REV ? 0 : 31)) sh[warp] = v;
+  __syncthreads();
+  Pair p = Op::id();
+  if (REV) {
+    for (int w = PG_WARPS - 1; w > warp; --w) p = Op::f(p, sh[w]);
+  } else {
+    for (int w = 0; w < warp; ++w) p = Op::f(p, sh[w]);
+  }
+  __syncthreads();
+  return Op::f(p, ex);
+}
+
+__device__ __forceinline__ u64 pghi_key(float s, double thr, int k, bool prev) {
+  return (s > 0.f && (double)s >= thr) ? ((u64)__float_as_uint(s) << 12 | (prev ? 2048ull : 0ull) | (u64)(2047 - k))
+                                       : 0ull;
+}
+// centred difference over bins, one-sided at the edges (numpy.gradient)
+__device__ __forceinline__ double diff_bins(const double* l, int k) {
+  return k == 0 ? l[1] - l[0] : k == NC ? l[NC] - l[NC - 1] : 0.5 * (l[k + 1] - l[k - 1]);
+}
+
+__global__ void __launch_bounds__(PG_THREADS) pghi_kernel(avc_audio_desc d, float tol, int8_t* parent) {
+  __shared__ double lrow[3][NBIN];  // ln max(s, tol s_max) of frames f-1, f, f+1 (slot = frame % 3)
+  __shared__ float srow[3][NBIN];
+  __shared__ Pair sh[PG_WARPS];
+  __shared__ float red[PG_WARPS];
+  const avc_audio_seg g = d.segs[blockIdx.x];
+  const int nF = g.n_frames, t = threadIdx.x, k0 = t * PG_PER;
+  if (nF <= 0) return;
+  const float* mag = d.mag + (int64_t)g.frame_off * NBIN;
+  float2* X = reinterpret_cast<float2*>(d.X) + (int64_t)g.frame_off * NBIN;
+  int8_t* par = parent ? parent + (int64_t)g.frame_off * NBIN : nullptr;
+
+  // s_max of the utterance (fmaxf is exact, so the order does not matter)
+  float m = 0.f;
+  for (int64_t i = t; i < (int64_t)nF * NBIN; i += PG_THREADS) m = fmaxf(m, __ldg(mag + i));
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+  if ((t & 31) == 0) red[t >> 5] = m;
+  __syncthreads();
+  m = red[0];
+  for (int w = 1; w < PG_WARPS; ++w) m = fmaxf(m, red[w]);
+  const double thr = (double)tol * (double)m;
+  const double lambda = 0.25645 * (double)d.win * (double)d.win;
+  const double a_t = (double)d.hop * (double)NFFT / lambda, b_t = (double)d.hop * 2.0 * M_PI / (double)NFFT;
+  const double a_f = -lambda / ((double)NFFT * (double)d.hop);
+
+  float nxt[PG_LOADS];
+  auto fetch = [&](int f) {
+#pragma unroll
+    for (int i = 0; i < PG_LOADS; ++i) {
+      const int k = t + i * PG_THREADS;
+      nxt[i] = (f < nF && k < NBIN) ? __ldg(mag + (int64_t)f * NBIN + k) : 0.f;
+    }
+  };
+  auto store = [&](int f) {
+    if (f >= nF) return;
+#pragma unroll
+    for (int i = 0; i < PG_LOADS; ++i) {
+      const int k = t + i * PG_THREADS;
+      if (k < NBIN) {
+        srow[f % 3][k] = nxt[i];
+        lrow[f % 3][k] = log(fmax((double)nxt[i], thr));
+      }
+    }
+  };
+  fetch(0);
+  store(0);
+  fetch(1);
+  store(1);
+  fetch(2);
+  __syncthreads();
+
+  double phi_prev[PG_PER];
+#pragma unroll
+  for (int j = 0; j < PG_PER; ++j) phi_prev[j] = 0.0;
+
+  for (int f = 0; f < nF; ++f) {
+    const double* lm = lrow[(f + 2) % 3];
+    const double* l0 = lrow[f % 3];
+    const double* lp = lrow[(f + 1) % 3];
+    const float* sm = srow[(f + 2) % 3];
+    const float* s0 = srow[f % 3];
+    // step per bin at frame f, bin k: -(lambda / (N hop)) d_f l - pi
+    auto dkphi = [&](int k) {
+      const double df = nF == 1 ? 0.0 : f == 0 ? lp[k] - l0[k] : f == nF - 1 ? l0[k] - lm[k] : 0.5 * (lp[k] - lm[k]);
+      return a_f * df - M_PI;
+    };
+    float s[PG_PER];
+    u64 a[PG_PER], c[PG_PER];
+    double troot[PG_PER], dk[PG_PER];
+#pragma unroll
+    for (int j = 0; j < PG_PER; ++j) {
+      const int k = k0 + j;
+      s[j] = 0.f; a[j] = c[j] = 0ull; troot[j] = dk[j] = 0.0;
+      if (k < NBIN) {
+        s[j] = s0[k];
+        c[j] = pghi_key(s[j], thr, k, false);
+        a[j] = f > 0 ? pghi_key(sm[k], thr, k, true) : 0ull;
+        dk[j] = dkphi(k);
+        // trapezoid of the advances per frame, hop ((N / lambda) d_k l + 2 pi k / N), at frames f-1 and f
+        if (a[j] && c[j]) troot[j] = 0.5 * (a_t * (diff_bins(lm, k) + diff_bins(l0, k)) + 2.0 * b_t * (double)k);
+      }
+    }
+    const bool any = k0 < NBIN;
+    const int kl = k0 - 1, kr = k0 + PG_PER;
+    const u64 c_left = any && kl >= 0 ? pghi_key(s0[kl], thr, kl, false) : 0ull;
+    const u64 c_right = any && kr < NBIN ? pghi_key(s0[kr], thr, kr, false) : 0ull;
+    const double dk_left = any && kl >= 0 ? dkphi(kl) : 0.0;
+    const double dk_right = any && kr < NBIN ? dkphi(kr) : 0.0;
+
+    // directional levels: left to right, then right to left
+    u64 lc[PG_PER], rc[PG_PER];
+    Pair M = ClampOp::id();
+#pragma unroll
+    for (int j = 0; j < PG_PER; ++j) {
+      const u64 cb = j == 0 ? c_left : c[j - 1];
+      M = ClampOp::f(M, Pair{a[j], max(a[j], cb)});
+    }
+    u64 x = block_scan_excl<ClampOp, false>(M, sh).a;
+#pragma unroll
+    for (int j = 0; j < PG_PER; ++j) {
+      lc[j] = min(x, j == 0 ? c_left : c[j - 1]);
+      x = max(a[j], lc[j]);
+    }
+    M = ClampOp::id();
+#pragma unroll
+    for (int j = PG_PER - 1; j >= 0; --j) {
+      const u64 cb = j == PG_PER - 1 ? c_right : c[j + 1];
+      M = ClampOp::f(M, Pair{a[j], max(a[j], cb)});
+    }
+    x = block_scan_excl<ClampOp, true>(M, sh).a;
+#pragma unroll
+    for (int j = PG_PER - 1; j >= 0; --j) {
+      rc[j] = min(x, j == PG_PER - 1 ? c_right : c[j + 1]);
+      x = max(a[j], rc[j]);
+    }
+
+    // parents; ISLAND marks a significant bin no source reaches until the seeds are chosen
+    constexpr int ISLAND = 5;
+    int pr[PG_PER];
+    bool island = false;
+#pragma unroll
+    for (int j = 0; j < PG_PER; ++j) {
+      pr[j] = AVC_PGHI_NONE;
+      if (c[j]) {
+        if (a[j] && a[j] >= lc[j] && a[j] >= rc[j]) pr[j] = AVC_PGHI_TIME;
+        else if (lc[j] > rc[j]) pr[j] = AVC_PGHI_LEFT;
+        else if (rc[j] > lc[j]) pr[j] = AVC_PGHI_RIGHT;
+        else pr[j] = ISLAND;
+      }
+      island |= pr[j] == ISLAND;
+    }
+    if (__syncthreads_or(island)) {  // seed each run of island bins at its largest key (segmented max both ways)
+      u64 fw[PG_PER];
+      Pair S = SegMaxOp::id();
+#pragma unroll
+      for (int j = 0; j < PG_PER; ++j) S = SegMaxOp::f(S, pr[j] == ISLAND ? Pair{0ull, c[j]} : Pair{1ull, 0ull});
+      u64 run = block_scan_excl<SegMaxOp, false>(S, sh).b;
+#pragma unroll
+      for (int j = 0; j < PG_PER; ++j) fw[j] = run = pr[j] == ISLAND ? max(run, c[j]) : 0ull;
+      S = SegMaxOp::id();
+#pragma unroll
+      for (int j = PG_PER - 1; j >= 0; --j) S = SegMaxOp::f(S, pr[j] == ISLAND ? Pair{0ull, c[j]} : Pair{1ull, 0ull});
+      run = block_scan_excl<SegMaxOp, true>(S, sh).b;
+#pragma unroll
+      for (int j = PG_PER - 1; j >= 0; --j) {
+        run = pr[j] == ISLAND ? max(run, c[j]) : 0ull;
+        if (pr[j] == ISLAND) {
+          const u64 top = max(fw[j], run);
+          pr[j] = c[j] == top ? AVC_PGHI_SEED : run == top ? AVC_PGHI_RIGHT : AVC_PGHI_LEFT;
+        }
+      }
+    }
+
+    // phases: roots (time steps and seeds), then the chains to their right and to their left
+    double root[PG_PER];
+#pragma unroll
+    for (int j = 0; j < PG_PER; ++j) root[j] = pr[j] == AVC_PGHI_TIME ? phi_prev[j] + troot[j] : 0.0;
+    Pair S = SegSumOp::id();
+#pragma unroll
+    for (int j = 0; j < PG_PER; ++j) {
+      const double inc = 0.5 * ((j == 0 ? dk_left : dk[j - 1]) + dk[j]);
+      S = SegSumOp::f(S, pr[j] == AVC_PGHI_LEFT ? Pair{0ull, (u64)__double_as_longlong(inc)}
+                                                : Pair{1ull, (u64)__double_as_longlong(root[j])});
+    }
+    double run = __longlong_as_double((long long)block_scan_excl<SegSumOp, false>(S, sh).b);
+    double phi[PG_PER];
+#pragma unroll
+    for (int j = 0; j < PG_PER; ++j) {
+      run = pr[j] == AVC_PGHI_LEFT ? run + 0.5 * ((j == 0 ? dk_left : dk[j - 1]) + dk[j]) : root[j];
+      phi[j] = run;
+    }
+    S = SegSumOp::id();
+#pragma unroll
+    for (int j = PG_PER - 1; j >= 0; --j) {
+      const double inc = -0.5 * ((j == PG_PER - 1 ? dk_right : dk[j + 1]) + dk[j]);
+      S = SegSumOp::f(S, pr[j] == AVC_PGHI_RIGHT ? Pair{0ull, (u64)__double_as_longlong(inc)}
+                                                 : Pair{1ull, (u64)__double_as_longlong(root[j])});
+    }
+    run = __longlong_as_double((long long)block_scan_excl<SegSumOp, true>(S, sh).b);
+#pragma unroll
+    for (int j = PG_PER - 1; j >= 0; --j) {
+      run = pr[j] == AVC_PGHI_RIGHT ? run - 0.5 * ((j == PG_PER - 1 ? dk_right : dk[j + 1]) + dk[j]) : root[j];
+      if (pr[j] == AVC_PGHI_RIGHT) phi[j] = run;
+    }
+
+    // X = s e^{i phi}, phi wrapped
+    const int64_t row = (int64_t)f * NBIN;
+#pragma unroll
+    for (int j = 0; j < PG_PER; ++j) {
+      const int k = k0 + j;
+      double p = pr[j] == AVC_PGHI_NONE ? 0.0 : phi[j];
+      p -= 2.0 * M_PI * rint(p * (0.5 / M_PI));
+      phi_prev[j] = p;
+      if (k < NBIN) {
+        double sn, cs;
+        sincospi(p * M_1_PI, &sn, &cs);  // |p| <= pi: no argument reduction, so no local-memory slow path
+        X[row + k] = make_float2((float)((double)s[j] * cs), (float)((double)s[j] * sn));
+        if (par) par[row + k] = (int8_t)pr[j];
+      }
+    }
+    // frame f-1's slot takes frame f+2 (every read of it this frame is behind the scans' barriers)
+    store(f + 2);
+    fetch(f + 3);
+    __syncthreads();
+  }
+}
+
 int check_audio(const avc_audio_desc* d, const char* who) {
   AVC_REQUIRE(d != nullptr, AVC_ERR_INVALID, "%s: null descriptor", who);
   AVC_REQUIRE(d->n_fft == NFFT, AVC_ERR_UNSUPPORTED, "%s: only n_fft = %d is supported (got %d)", who, NFFT, d->n_fft);
@@ -397,6 +688,19 @@ int check_momentum(avc_audio_desc& d, const char* who) {
   AVC_REQUIRE(d.X_prev != nullptr, AVC_ERR_INVALID, "%s: momentum > 0 needs X_prev", who);
   const uintptr_t p = (uintptr_t)d.X_prev, x = (uintptr_t)d.X, bytes = (uintptr_t)d.n_frames * NBIN * sizeof(float2);
   AVC_REQUIRE(p != x && (p + bytes <= x || x + bytes <= p), AVC_ERR_INVALID, "%s: X_prev overlaps X", who);
+  return AVC_OK;
+}
+
+int check_tol(float tol, const char* who) {
+  AVC_REQUIRE(std::isfinite(tol) && tol > 0.f && tol < 1.f, AVC_ERR_INVALID, "%s: tol must be in (0, 1) (got %g)", who,
+              (double)tol);
+  return AVC_OK;
+}
+
+int launch_pghi(const avc_audio_desc& d, float tol, int8_t* parent, cudaStream_t st) {
+  if (d.n_frames == 0) return AVC_OK;
+  pghi_kernel<<<d.n_seg, PG_THREADS, 0, st>>>(d, tol, parent);
+  AVC_CHECK_LAUNCH("avc_pghi");
   return AVC_OK;
 }
 
@@ -453,24 +757,44 @@ extern "C" int avc_istft(const avc_audio_desc* d, void* stream) {
   return launch_istft(*d, (cudaStream_t)stream);
 }
 
-extern "C" int avc_griffin_lim(const avc_audio_desc* d, void* stream) {
+extern "C" int avc_griffin_lim_from(const avc_audio_desc* d, int32_t start, float tol, void* stream) {
   if (int rc = check_audio(d, "avc_griffin_lim")) return rc;
   AVC_REQUIRE(d->mag != nullptr && d->X != nullptr && d->frames != nullptr && d->y != nullptr, AVC_ERR_INVALID,
               "avc_griffin_lim: null mag, X, frames or y");
   AVC_REQUIRE(d->n_iter >= 0, AVC_ERR_INVALID, "avc_griffin_lim: n_iter < 0");
+  AVC_REQUIRE(start == AVC_GL_START_ZERO || start == AVC_GL_START_X || start == AVC_GL_START_PGHI, AVC_ERR_INVALID,
+              "avc_griffin_lim: unknown start %d", start);
+  if (start == AVC_GL_START_PGHI) {
+    if (int rc = check_tol(tol, "avc_griffin_lim")) return rc;
+  }
   cudaStream_t st = (cudaStream_t)stream;
   avc_audio_desc a = *d;
   if (int rc = check_momentum(a, "avc_griffin_lim")) return rc;
   a.preemph = 0.f;
+  // every argument is checked: the PGHI start is the call's first launch
+  if (start == AVC_GL_START_PGHI) {
+    if (int rc = launch_pghi(a, tol, nullptr, st)) return rc;
+  }
   for (int it = 0; it <= a.n_iter; ++it) {
     avc_audio_desc s = a;
-    if (it == 0) s.X = nullptr;  // X = S with zero phase
+    if (it == 0 && start == AVC_GL_START_ZERO) s.X = nullptr;  // X = S with zero phase
     if (int rc = launch_istft(s, st)) return rc;
     if (it == a.n_iter) break;
     a.mode = it == 0 ? AVC_STFT_PROJECT_FIRST : AVC_STFT_PROJECT;  // the same projection when X_prev is null
     if (int rc = launch_stft(a, st)) return rc;
   }
   return AVC_OK;
+}
+
+extern "C" int avc_griffin_lim(const avc_audio_desc* d, void* stream) {
+  return avc_griffin_lim_from(d, AVC_GL_START_ZERO, 0.f, stream);
+}
+
+extern "C" int avc_pghi(const avc_audio_desc* d, float tol, int8_t* parent, void* stream) {
+  if (int rc = check_audio(d, "avc_pghi")) return rc;
+  AVC_REQUIRE(d->mag != nullptr && d->X != nullptr, AVC_ERR_INVALID, "avc_pghi: null mag or X");
+  if (int rc = check_tol(tol, "avc_pghi")) return rc;
+  return launch_pghi(*d, tol, parent, (cudaStream_t)stream);
 }
 
 extern "C" int avc_frame_power(const avc_audio_desc* d, float* power, void* stream) {

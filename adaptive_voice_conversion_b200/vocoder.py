@@ -37,6 +37,8 @@ class AudioParams:
     n_mels: int = 512
     n_iter: int = 100
     momentum: float = 0.0      # fast Griffin-Lim momentum in [0, 1); 0 is the reference's plain Griffin-Lim
+    gl_init: str = "zero"      # Griffin-Lim start phase: "zero" (the reference's) or "pghi" (phase-gradient estimate)
+    pghi_tol: float = 1e-5     # PGHI significance threshold relative to an utterance's largest magnitude (not tuned)
     preemphasis: float = 0.97
     max_db: float = 100.0
     ref_db: float = 20.0
@@ -224,18 +226,57 @@ def istft(specs, hp: AudioParams = AudioParams()):
     return r.split_samples(y)
 
 
+GL_INITS = ("zero", "pghi")
+
+
+def _init(init, hp: AudioParams) -> str:
+    init = hp.gl_init if init is None else init
+    if init not in GL_INITS:
+        raise ValueError(f"griffin_lim: init must be one of {GL_INITS} (got {init!r})")
+    return init
+
+
+def pghi(mags, hp: AudioParams = AudioParams(), tol: float | None = None, parent: bool = False):
+    """Phase Gradient Heap Integration start spectra: [T, n_bins] complex64 S e^{i phi} per utterance of linear
+    magnitudes S [T, n_bins], in one avc_pghi launch.  phi is integrated frame by frame from the phase derivatives the
+    Gaussian approximation of the window gives from ln S (Prusa, Balazs & Sondergaard 2017; Prusa & Holighaus 2017);
+    bins below ``tol`` (default ``hp.pghi_tol``) times the utterance's largest magnitude get phase 0.
+    ``parent=True`` also returns each bin's int8 AVC_PGHI_* source, per utterance."""
+    if not mags:
+        raise ValueError("pghi: empty batch")
+    dev = mags[0].device
+    S = torch.cat([m.float() for m in mags]).contiguous()
+    if S.dim() != 2 or S.shape[1] != hp.n_bins:
+        raise ValueError(f"pghi: magnitudes have shape {tuple(S.shape)}, n_fft={hp.n_fft} gives {hp.n_bins} bins")
+    r = _Ragged([0] * len(mags), [m.shape[0] for m in mags], dev)
+    X = torch.empty(S.shape[0], hp.n_bins, 2, device=dev)
+    par = torch.empty(S.shape[0], hp.n_bins, dtype=torch.int8, device=dev) if parent else None
+    tol = float(hp.pghi_tol if tol is None else tol)
+    _call("avc_pghi", r.desc(hp, mag=S, X=X), dev, C.c_float(tol), _ptr(par))
+    out = [torch.view_as_complex(x) for x in r.split_frames(X)]
+    return (out, r.split_frames(par)) if parent else out
+
+
 class GriffinLim:
-    """One ragged Griffin-Lim call with its buffers.  ``run()`` enqueues the whole loop (3 n_iter + 2 launches) on
-    the current stream, so it can be captured into a CUDA graph; ``outputs()`` are views of the signal buffer.
+    """One ragged Griffin-Lim call with its buffers.  ``run()`` enqueues the whole loop (3 n_iter + 2 launches, one
+    more with the PGHI start) on the current stream, so it can be captured into a CUDA graph; ``outputs()`` are views
+    of the signal buffer.
 
     ``momentum`` m > 0 (default ``hp.momentum``) runs fast Griffin-Lim (Perraudin, Balazs & Sondergaard 2013) in the
     form of librosa's and torchaudio's ``momentum``: each projection uses A = E - m/(1+m) P, P the previous iteration's
     spectrum E, and P takes a second complex buffer the size of X.  The start is zero-phase (librosa's init=None).
     Where librosa divides by |A| + tiny, this divides by max(1e-8, |A|); the two differ only where |A| < 1e-8.
-    A momentum that is not finite or outside [0, 1) raises ``AvcError`` from ``run()``."""
+    A momentum that is not finite or outside [0, 1) raises ``AvcError`` from ``run()``.
+
+    ``init`` (default ``hp.gl_init``) picks the start phase: "zero" (the reference's, and librosa's init=None), or
+    "pghi", which first writes ``pghi``'s start spectrum into X (tolerance ``hp.pghi_tol``) and starts the loop's
+    first iSTFT from it.  It composes with ``momentum``.  Either way ``run()`` is one C call
+    (``avc_griffin_lim_from``) that checks every argument, the tolerance included, before its first launch."""
 
     def __init__(self, mags, hp: AudioParams = AudioParams(), n_iter: int | None = None,
-                 momentum: float | None = None):
+                 momentum: float | None = None, init: str | None = None):
+        self.init = _init(init, hp)
+        self.tol = float(hp.pghi_tol)
         _frames(mags, hp, "griffin_lim")
         self.dev = mags[0].device
         self.S = torch.cat([m.float() for m in mags]).contiguous()
@@ -252,17 +293,21 @@ class GriffinLim:
                                 frames=self.frames, y=self.y, X_prev=self.X_prev)
 
     def run(self):
-        _call("avc_griffin_lim", self.desc, self.dev)
+        if self.init == "pghi":
+            _call("avc_griffin_lim_from", self.desc, self.dev, C.c_int32(L.GL_START_PGHI), C.c_float(self.tol))
+        else:
+            _call("avc_griffin_lim", self.desc, self.dev)
         return self
 
     def outputs(self):
         return self.r.split_samples(self.y)
 
 
-def griffin_lim(mags, hp: AudioParams = AudioParams(), n_iter: int | None = None, momentum: float | None = None):
+def griffin_lim(mags, hp: AudioParams = AudioParams(), n_iter: int | None = None, momentum: float | None = None,
+                init: str | None = None):
     """Griffin-Lim from linear magnitudes [T, n_bins]; signals of hop * (T - 1) samples (untrimmed).  ``momentum``
-    (default ``hp.momentum``) as in ``GriffinLim``."""
-    return GriffinLim(mags, hp, n_iter, momentum).run().outputs()
+    and ``init`` (defaults ``hp.momentum``, ``hp.gl_init``) as in ``GriffinLim``."""
+    return GriffinLim(mags, hp, n_iter, momentum, init).run().outputs()
 
 
 def deemphasis(wavs, coef: float = 0.97):
@@ -354,15 +399,17 @@ class Vocoder:
         r = [m.shape[0] for m in mels]
         return list(torch.split(_mel_project(torch.cat(mels), self.m_t, L.MEL_TO_MAG, self.hp), r))
 
-    def mel_to_wav(self, mels, n_iter: int | None = None, momentum: float | None = None):
+    def mel_to_wav(self, mels, n_iter: int | None = None, momentum: float | None = None, init: str | None = None):
         """Normalised mels [T, n_mels] (device tensors) -> float32 signals: amplitude, mel-to-linear, Griffin-Lim,
-        de-emphasis, trim (out_top_db).  ``n_iter`` and ``momentum`` default to ``hp.n_iter`` and ``hp.momentum``."""
+        de-emphasis, trim (out_top_db).  ``n_iter``, ``momentum`` and ``init`` default to ``hp.n_iter``,
+        ``hp.momentum`` and ``hp.gl_init``."""
         hp = self.hp
         for i, m in enumerate(mels):
             if m.dim() != 2 or m.shape[1] != hp.n_mels:
                 raise ValueError(f"mel_to_wav: utterance {i} has shape {tuple(m.shape)}, expected [T, {hp.n_mels}]")
+        _init(init, hp)
         _frames(mels, hp, "mel_to_wav")
-        ys = deemphasis(griffin_lim(self.mel_to_mag(mels), hp, n_iter, momentum), hp.preemphasis)
+        ys = deemphasis(griffin_lim(self.mel_to_mag(mels), hp, n_iter, momentum, init), hp.preemphasis)
         return trim(ys, hp.out_top_db)
 
     def get_spectrograms(self, path):

@@ -569,6 +569,36 @@ int avc_istft(const avc_audio_desc* d, void* stream);
  * X_prev; same launches.  AVC_ERR_INVALID before any launch when m is not finite or outside [0, 1), or when m > 0 and
  * X_prev is null or overlaps X.  m = 0 ignores X_prev. */
 int avc_griffin_lim(const avc_audio_desc* d, void* stream);
+/* avc_griffin_lim with a choice of start.  AVC_GL_START_ZERO is avc_griffin_lim itself.  AVC_GL_START_X starts the first
+ * iSTFT from X as the caller left it instead of mag with zero phase.  AVC_GL_START_PGHI first writes avc_pghi's start
+ * spectrum (threshold tol) into X and starts from it: one more launch, 3 n_iter + 3.  tol is read only with
+ * AVC_GL_START_PGHI.  Every argument of the call (the start, tol, and all of avc_griffin_lim's) is checked before its
+ * first launch; AVC_ERR_INVALID otherwise.
+ * The start is an argument rather than a descriptor field on purpose: avc_griffin_lim would have to read such a field
+ * on every call, past the end of a descriptor built against the previous header, and the descriptor's size is part
+ * of the ABI.  (X_prev could be appended because it is read only when the in-struct momentum is non-zero.) */
+#define AVC_GL_START_ZERO 0
+#define AVC_GL_START_X 1
+#define AVC_GL_START_PGHI 2
+int avc_griffin_lim_from(const avc_audio_desc* d, int32_t start, float tol, void* stream);
+/* Phase Gradient Heap Integration (Prusa, Balazs & Sondergaard 2017; RTPGHI per frame, Prusa & Holighaus 2017): a
+ * start spectrum X = mag * e^{i phi} for avc_griffin_lim_from (AVC_GL_START_X, or AVC_GL_START_PGHI in one call).  Per utterance, s_max = its largest
+ * magnitude; bins with s = 0 or s < tol * s_max are insignificant (phi = 0).  l = ln max(s, tol * s_max) and, with
+ * lambda = 0.25645 win^2 and d_k, d_f centred differences over bins and frames (one-sided at the edges),
+ *   phase advance per frame  dt(f,k) = hop ((n_fft / lambda) d_k l + 2 pi k / n_fft),
+ *   phase step per bin       dk(f,k) = -(lambda / (n_fft hop)) d_f l - pi.
+ * Frame by frame, phi is what the literal heap integration gives: sources are the significant bins of frame f-1,
+ * larger magnitude first (then frame f-1 first, then the lower bin), a time step adds (dt(f-1,k) + dt(f,k)) / 2, a
+ * bin step to k+-1 adds +-(dk(f,k) + dk(f,k+-1)) / 2, and each run of bins with no source is seeded at its largest
+ * bin with phi = 0.  The kernel computes it with block scans (one CTA per utterance, float64 phases, no atomics).
+ * parent (nullable, [n_frames][n_fft/2+1]) receives each bin's AVC_PGHI_* choice.  Reads mag, writes X.
+ * AVC_ERR_INVALID before any launch when tol is not finite or not in (0, 1), or mag or X is null. */
+#define AVC_PGHI_NONE 0  /* insignificant */
+#define AVC_PGHI_TIME 1  /* from (f-1, k) */
+#define AVC_PGHI_LEFT 2  /* from (f, k-1) */
+#define AVC_PGHI_RIGHT 3 /* from (f, k+1) */
+#define AVC_PGHI_SEED 4  /* largest bin of a run with no source: phi = 0 */
+int avc_pghi(const avc_audio_desc* d, float tol, int8_t* parent, void* stream);
 /* power[frame] = mean of y^2 over frames of n_fft samples hop apart, reflect-padded by n_fft/2 (librosa's trim
  * statistic): segs frame_off / n_frames count these frames, 1 + n_samples / hop per utterance.  Any even n_fft. */
 int avc_frame_power(const avc_audio_desc* d, float* power, void* stream);

@@ -6,7 +6,8 @@ as the reference does:
     python inference.py -c config.yaml -m model.ckpt -a attr.pkl -s src.wav -t tgt.wav -o out.wav
 
 -gl_iters (default 100) and -gl_momentum (default 0, plain Griffin-Lim) set the synthesis of a .wav output; a
-momentum such as 0.99 runs fast Griffin-Lim.
+momentum such as 0.99 runs fast Griffin-Lim.  -gl_init pghi starts Griffin-Lim from a phase-gradient (PGHI) estimate
+instead of zero phase (the default, -gl_init zero).
 
 Any of the three may instead be a .npy mel ([T, n_mels], already normalised when -attr is omitted):
 
@@ -38,7 +39,7 @@ With -bank, a -pairs target field ``@SPEC`` is resolved through the bank (a fiel
 file, even one whose name starts with @), and its output name defaults to ``<source stem>_to_<SPEC>.wav`` (``:`` and
 ``,`` replaced by ``-`` and ``+``).  Without -bank every field is read as above.  The sources and targets are analysed in one batched Vocoder.wav_to_mel call (.npy mels are read
 as in the single-pair mode), converted by Inferencer.inference_padded, and the .wav outputs synthesised in one batched
-Vocoder.mel_to_wav call (-gl_iters, -gl_momentum).  A missing file, a malformed line or an utterance shorter than the
+Vocoder.mel_to_wav call (-gl_iters, -gl_momentum, -gl_init).  A missing file, a malformed line or an utterance shorter than the
 model accepts is reported with its line number before anything runs on the GPU.
 """
 import os
@@ -166,8 +167,9 @@ def run_pairs(args, config):
     files = sorted({p for _, s, t, _ in pairs
                     for p in (s,) + ((t,) if isinstance(t, str) else () if isinstance(t, BankTarget) else t)})
     need_voc = any(is_wav(f) for f in files) or any(is_wav(name) for *_, name in pairs)
+    hp = AudioParams(n_iter=args.gl_iters, momentum=args.gl_momentum, gl_init=args.gl_init)
     vocoder = Vocoder(n_mels=config["SpeakerEncoder"]["c_in"] // config["data_loader"]["frame_size"],
-                      hp=AudioParams(n_iter=args.gl_iters, momentum=args.gl_momentum)) if need_voc else None
+                      hp=hp) if need_voc else None
     wavs = [f for f in files if is_wav(f)]
     mels = {}
     if wavs:
@@ -232,6 +234,8 @@ def parser():
     p.add_argument("-gl_iters", default=100, type=int, help="Griffin-Lim iterations of a .wav output")
     p.add_argument("-gl_momentum", default=0.0, type=float,
                    help="fast Griffin-Lim momentum in [0, 1) of a .wav output (0: plain Griffin-Lim)")
+    p.add_argument("-gl_init", default="zero", choices=["zero", "pghi"],
+                   help="Griffin-Lim start phase of a .wav output: zero phase, or the PGHI phase-gradient estimate")
     p.add_argument("-pairs", help="file of 'source target [output_name]' lines: convert them all, into the -o directory")
     p.add_argument("-bank", help="speaker bank (speaker_bank.py) for -speaker and the @SPEC fields of -pairs")
     p.add_argument("-speaker", help="banked target: NAME or a weighted mix NAME:W,NAME:W,... (needs -bank)")
@@ -252,7 +256,7 @@ if __name__ == "__main__":
     if any(is_wav(f) for f in (args.source, *targets, args.output)):
         from adaptive_voice_conversion_b200.vocoder import AudioParams, Vocoder
         vocoder = Vocoder(n_mels=config["SpeakerEncoder"]["c_in"] // config["data_loader"]["frame_size"],
-                          hp=AudioParams(n_iter=args.gl_iters, momentum=args.gl_momentum))
+                          hp=AudioParams(n_iter=args.gl_iters, momentum=args.gl_momentum, gl_init=args.gl_init))
     inf = Inferencer(config=config, args=args, vocoder=vocoder if is_wav(args.output) else None)
 
     def read(path):

@@ -104,15 +104,16 @@ def spectral_convergence(V, mags, ys):
     return out
 
 
-def convergence_table(V, mags, hp, iters, momenta):
-    """{momentum: {n_iter: median spectral convergence over the batch}}"""
-    return {m: {n: statistics.median(spectral_convergence(V, mags, V.griffin_lim(mags, hp, n, m))) for n in iters}
-            for m in momenta}
+def convergence_table(V, mags, hp, iters, momenta, init=None):
+    """{momentum: {n_iter: median spectral convergence over the batch}}, from the start ``init`` (default hp's)."""
+    return {m: {n: statistics.median(spectral_convergence(V, mags, V.griffin_lim(mags, hp, n, m, init)))
+                for n in iters} for m in momenta}
 
 
-def fewest_iterations(table, momentum, plain_iters=100):
-    """The fewest iterations whose median with momentum is at or below plain Griffin-Lim's at plain_iters."""
-    target = table[0.0][plain_iters]
+def fewest_iterations(table, momentum, plain_iters=100, target=None):
+    """The fewest iterations of the table's grid whose median with momentum is at or below ``target``, by default
+    plain Griffin-Lim's at plain_iters in the same table."""
+    target = table[0.0][plain_iters] if target is None else target
     ok = [n for n, sc in sorted(table[momentum].items()) if sc <= target]
     return ok[0] if ok else None
 
