@@ -223,7 +223,12 @@ def _encoder_fwd(P, cfg, key, x, tap, tc, acts):
 
 def dense_fwd(P, cfg, h):
     """The speaker encoder after its conv blocks: time mean, the dense blocks and output_layer."""
-    h = h.double().mean(dim=2)
+    return dense_pooled(P, cfg, h.double().mean(dim=2))
+
+
+def dense_pooled(P, cfg, h):
+    """The dense blocks and output_layer on time-pooled rows h [B, c_h]."""
+    h = h.double()
     for l in range(cfg["SpeakerEncoder"]["n_dense_blocks"]):
         n1, n2 = f"speaker_encoder.first_dense_layers.{l}", f"speaker_encoder.second_dense_layers.{l}"
         y = F.relu(F.linear(h, P[n1 + ".weight"].double(), P[n1 + ".bias"].double()))
@@ -231,10 +236,17 @@ def dense_fwd(P, cfg, h):
     return F.linear(h, P["speaker_encoder.output_layer.weight"].double(), P["speaker_encoder.output_layer.bias"].double())
 
 
-def speaker_fwd(P, cfg, x, tap=_ident, tc=_no_tc, acts=None):
+def speaker_convs(P, cfg, x, tap=_ident, tc=_no_tc, acts=None):
+    """The speaker encoder's conv layers -> the last one's output [B, c_h, T/8], before the time mean."""
     acts = {} if acts is None else acts
     out = _encoder_fwd(P, cfg, "SpeakerEncoder", x, tap, tc, acts)
     acts["speaker_encoder.last"] = out
+    return out
+
+
+def speaker_fwd(P, cfg, x, tap=_ident, tc=_no_tc, acts=None):
+    acts = {} if acts is None else acts
+    out = speaker_convs(P, cfg, x, tap, tc, acts)
     return tap("emb", "speaker_encoder", dense_fwd(P, cfg, out)), acts
 
 

@@ -80,7 +80,7 @@ class RecordingLib:
 class Capture:
     def __init__(self):
         self.fwd, self.dc, self.dx, self.launches = {}, {}, {}, []
-        self.cur, self.emb, self.demb, self.dconds, self.sn = None, None, None, None, {}
+        self.cur, self.emb, self.demb, self.dconds, self.sn, self.wbar = None, None, None, None, {}, {}
 
     def tagged(self, tag, fn):
         prev, self.cur = self.cur, tag
@@ -101,15 +101,20 @@ def install(monkeypatch, eng, cap):
     from adaptive_voice_conversion_b200 import engine as E
     Eng = E.Engine
     conv0, bwd0, wg0 = Eng.conv, Eng.conv_bwd, Eng._wgrad_launch
-    sfwd0, sbwd0, aff0, snb0 = Eng.speaker_fwd, Eng.speaker_bwd, Eng._decoder_affine_bwd, Eng.spectral_norm_bwd
+    sfwd0, sbwd0, aff0, sn0, snb0 = Eng.speaker_fwd, Eng.speaker_bwd, Eng._decoder_affine_bwd, Eng.spectral_norm, Eng.spectral_norm_bwd
 
     def conv(self, P, name, xin, **kw):
         out, rec = cap.tagged((name, "fwd"), lambda: conv0(self, P, name, xin, **kw))
         cond = kw.get("cond")
         # (a bank conv rounds its output into its channel range of the concat: that view carries no tf32 flag)
         rounded = out.tf32 or (kw.get("round_out", False) and self.precision == "tf32" and not self.fwd_fp32)
+        # a padded batch: the valid frames of xin, and of out before a pixel shuffle doubles them
+        lens = kw.get("lens")
+        lo = None if lens is None else lens.down(kw.get("stride", 1))
         cap.fwd[name] = dict(x=planar(xin), x_tf32=xin.tf32, out=planar(out), out_tf32=out.tf32, rounded=rounded,
-                             cond=None if cond is None else cond.clone())
+                             cond=None if cond is None else cond.clone(), shuffle=kw.get("shuffle", False),
+                             lens=None if lens is None else (lens.t.clone(), lens.div, lens.mul),
+                             lens_out=None if lo is None else (lo.t.clone(), lo.div, lo.mul))
         return out, rec
 
     def conv_bwd(self, P, G, rec, dy, **kw):
@@ -124,8 +129,8 @@ def install(monkeypatch, eng, cap):
     def wgrad_launch(self, wd, name):
         return cap.tagged((name, "wgrad"), lambda: wg0(self, wd, name))
 
-    def speaker_fwd(self, P, x, train, lens=None):
-        emb, ctx = sfwd0(self, P, x, train, lens)
+    def speaker_fwd(self, P, x, train, lens=None, groups=None):
+        emb, ctx = sfwd0(self, P, x, train, lens, groups)
         cap.emb = emb.clone()
         return emb, ctx
 
@@ -137,6 +142,11 @@ def install(monkeypatch, eng, cap):
         cap.dconds = dconds.clone()
         return aff0(self, P, G, ctx, dconds)
 
+    def sn_fwd(self, P, iterate):
+        sn0(self, P, iterate)
+        for n in self.sn_names():
+            cap.wbar[n] = (P[n + ".weight"].clone(), iterate)
+
     def sn_bwd(self, P, G):
         for n in self.sn_names():
             cap.sn[n] = (P[n + ".weight"].clone(), G[n + ".weight"].clone())
@@ -147,7 +157,8 @@ def install(monkeypatch, eng, cap):
             cap.dc[name] = (planar(obj), obj.tf32)
 
     for attr, f in (("conv", conv), ("conv_bwd", conv_bwd), ("_wgrad_launch", wgrad_launch), ("speaker_fwd", speaker_fwd),
-                    ("speaker_bwd", speaker_bwd), ("_decoder_affine_bwd", affine_bwd), ("spectral_norm_bwd", sn_bwd)):
+                    ("speaker_bwd", speaker_bwd), ("_decoder_affine_bwd", affine_bwd), ("spectral_norm", sn_fwd),
+                    ("spectral_norm_bwd", sn_bwd)):
         monkeypatch.setattr(Eng, attr, f)
     monkeypatch.setattr(eng, "debug", debug)
     monkeypatch.setattr(eng, "lib", RecordingLib(eng.lib, cap))
@@ -171,7 +182,9 @@ class Checker:
 
     def err(self, kind, unit, e):
         e = float(e)
-        if not (e <= self.worst[kind]):   # (NaN counts as worse than anything)
+        w = self.worst.get(kind)
+        # NaN counts as worse than anything, and stays the worst once recorded (a later e <= NaN is False too)
+        if w is None or (w == w and not (e <= w)):
             self.worst[kind], self.where[kind] = e, unit
 
     def honest(self, what, t, flag):
@@ -424,19 +437,47 @@ def test_training_step_layers(monkeypatch, kind, precision, B, env):
 INFER_CASES = [(17, 9), (145, 600), (1000, 333)]
 
 
-@pytest.mark.parametrize("precision", ["fp32", "tf32"])
-@pytest.mark.parametrize("T,T_c", INFER_CASES)
-def test_inference_layers(monkeypatch, precision, T, T_c):
+def eval_wbar(m, cap, chk):
+    """W_bar of every spectral-norm layer as the engine computed it for a model in eval() (no power iteration: the
+    stored u and v), checked against the float64 restatement -> {name + ".weight": W_bar} for the reference chain.
+    The stored u and v are not W's singular vectors, so sigma = u^T W v may cancel: the error is measured against the
+    magnitude of its terms, sum |u_i W_ij v_j| / |sigma| times W_bar's largest."""
+    from _sn_ref import power_iteration64
+    P, bufs = dict(m.named_parameters()), dict(m.named_buffers())
+    wbar = {}
+    for n, (w, iterate) in cap.wbar.items():
+        if iterate:
+            chk.problems.append(f"{n}: the spectral norm of an eval() model iterated u and v")
+        w0, u, v = P[n + ".weight_orig"].detach(), bufs[n + ".weight_u"].double(), bufs[n + ".weight_v"].double()
+        ref = power_iteration64(w0, u, v, iterate=False)[3]
+        wm = w0.double().reshape(w0.shape[0], -1)
+        cancel = float(u.abs() @ wm.abs() @ v.abs()) / abs(float(u @ wm @ v))
+        chk.err("misc", n + ".W_bar", Checker._rel(w, ref, ref.abs().max() * cancel))
+        wbar[n + ".weight"] = w
+    return wbar
+
+
+def inference_model(kind):
+    """-> (AE on cuda in eval(), config).  eval() as a converter runs the model: with Decoder.sn, W_bar then comes
+    from the stored u and v without a power iteration (torch's default init and its u and v: the oracle's init_state
+    has no spectral norm)."""
     from adaptive_voice_conversion_b200.model import AE
+    cfg = _config(kind)
+    torch.manual_seed(0)
+    m = AE(cfg)
+    if kind != "sn":
+        m.load_state_dict(orc.init_state(cfg, seed=0), strict=True)
+    return m.cuda().eval(), cfg
+
+
+def inference_layers(monkeypatch, kind, precision, T, T_c):
+    """Every layer of an unpadded AE.inference of 3 pairs (T source and T_c reference frames)."""
     monkeypatch.setenv("AVC_PRECISION", precision)
     monkeypatch.setenv("AVC_INFER_GRAPH", "0")
-    cfg = orc.default_config(80)
-    m = AE(cfg)
-    m.load_state_dict(orc.init_state(cfg, seed=0), strict=True)
-    m = m.cuda()
+    m, cfg = inference_model(kind)
     g = torch.Generator().manual_seed(5)
-    x = torch.randn((3, 80, T), generator=g).cuda()
-    xc = torch.randn((3, 80, T_c), generator=g).cuda()
+    x = torch.randn((3, cfg["SpeakerEncoder"]["c_in"], T), generator=g).cuda()
+    xc = torch.randn((3, cfg["SpeakerEncoder"]["c_in"], T_c), generator=g).cuda()
     m.inference(x, xc)            # packs the weights
     eng = m.engine(x.device)
     cap = Capture()
@@ -446,9 +487,11 @@ def test_inference_layers(monkeypatch, precision, T, T_c):
     eng.check_tc_status()
     P = dict(m.named_parameters())
     chk = Checker(cap, {}, cfg, precision == "tf32")
+    assert set(cap.wbar) == set(eng.sn_names())
+    P.update(eval_wbar(m, cap, chk))
     ref, _ = LR.ae_inference(P, cfg, x, xc, chk, cap.tc)
     chk.err("misc", "dec", Checker._rel(dec, ref, ref.abs().max()))
-    _report(f"inference {precision} T={T} T_c={T_c}", chk)
+    _report(f"inference {kind} {precision} T={T} T_c={T_c}", chk)
     paths = {n for n, _ in cap.launches}
     print("entry points:", sorted(p for p in paths if p in CONV_FAMILY or "norm_apply" in p))
     assert len(cap.fwd) == len(eng.conv_names())
@@ -457,7 +500,14 @@ def test_inference_layers(monkeypatch, precision, T, T_c):
     if precision == "tf32" and T < 32:
         # the decoder's in_conv normalises 3 latent frames here, and one row has |mean| / std = 80.  The fused tensor-core
         # epilogue takes the variance in one pass (E[c^2] - mean^2, csrc/conv_tc2.cu), which loses (mean / std)^2 * 2^-24
-        # = 3.8e-4 of it to cancellation: measured 3.8e-4.  The same case in fp32 (FFMA kernels) stays at 5.5e-6.
+        # = 3.8e-4 of it to cancellation: measured 3.8e-4 (c512 5.5e-5, sn 1.6e-4).  The same case in fp32 (FFMA kernels)
+        # stays at 5.5e-6 (c512 1.1e-5).
         tol["fwd"] = 1.2e-3
     bad = {k: (v, chk.where[k]) for k, v in chk.worst.items() if not v <= tol[k]}
     assert not bad, bad
+
+
+@pytest.mark.parametrize("precision", ["fp32", "tf32"])
+@pytest.mark.parametrize("T,T_c", INFER_CASES)
+def test_inference_layers(monkeypatch, precision, T, T_c):
+    inference_layers(monkeypatch, "c80", precision, T, T_c)
