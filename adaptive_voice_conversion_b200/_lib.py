@@ -122,6 +122,7 @@ class DenseStackDesc(C.Structure):
 
 
 LINEAR_BATCH_MAX = 16
+MORPH_MAX_K = 64      # AVC_MORPH_MAX_K
 VAE_PARTIALS = 2112   # AVC_VAE_PARTIALS
 
 
@@ -286,6 +287,8 @@ PROTOTYPES = {
     "avc_time_mean_fwd": (_i, [_p, _i64, _p, _i, _i, _i, _p]),
     "avc_time_mean_bwd": (_i, [_p, _p, _i64, _i, _i, _i, _p]),
     "avc_norm_apply_varlen": (_i, [C.POINTER(ConvDesc), _p, _i, _i, _p]),
+    "avc_norm_apply_morph": (_i, [C.POINTER(ConvDesc), _p, _i, _i, _p, _i, _i64, _p]),
+    "avc_morph_weights": (_i, [_p, _p, _i, _i, _i, _i, _p, _i, _p]),
     "avc_time_mean_varlen_fwd": (_i, [_p, _i64, _p, _i, _i, _i, _p, _i, _i, _p]),
     "avc_time_mean_grouped_fwd": (_i, [_p, _i64, _p, _i, _i, _i, _p, _i, _i, _p, _i, _p]),
     "avc_time_sum_varlen": (_i, [_p, _i64, _p, _p, _i, _i, _i, _p, _i, _i, _p]),

@@ -2,6 +2,8 @@
 //  * avc_norm_apply_fwd : two-pass InstanceNorm/AdaIN/ReLU/residual for sequences too long
 //                         for the fused conv tile (nn.InstanceNorm1d, append_cond; model.py:296,341,77-83)
 //  * avc_norm_apply_varlen : the same over each sample's valid frames of a padded batch
+//  * avc_norm_apply_morph : avc_norm_apply_varlen with a per-frame AdaIN mix of K anchor rows (time-varying morphs)
+//  * avc_morph_weights    : the per-layer-frame anchor weights avc_norm_apply_morph reads
 //  * avc_varlen_tail    : rewrites the frames just past each sample's length of a padded batch
 //  * avc_norm_bwd       : backward of that epilogue (autograd under solver.py:90)
 //  * avc_fold_add_fwd   : adjoint of F.pad(mode='reflect') (model.py:28-30) + residual adjoint
@@ -49,11 +51,20 @@ __device__ __forceinline__ int varlen_len(const int32_t* lengths, int b, int div
   return ((__ldg(lengths + b) + div - 1) / div) * mul;
 }
 
+// avc_norm_apply_morph: the layer's weight table [B][Tn][K] and the stride between a sample's K anchor rows in d.cond
+struct MorphArgs {
+  const float* wtab;
+  int64_t kstride;
+  int K;
+};
+
 // lengths null: every sample has Tout conv outputs; otherwise sample b has L_b = varlen_len(...) and only its first
-// L_b (2 L_b after the shuffle) frames enter the statistics and are written
-template <bool SHUF>
+// L_b (2 L_b after the shuffle) frames enter the statistics and are written.
+// MORPH: frame tn's AdaIN row is sum_k wtab[b][tn][k] * (anchor k's row), formed with fmaf in k order from 0; each warp
+// stages its sample's K anchor rows of its 4 channels in shared memory (blockDim / 32 * K * 2 float4)
+template <bool SHUF, bool MORPH = false>
 __global__ void __launch_bounds__(256) norm_apply_fwd_kernel(const avc_conv_desc d, const int32_t* __restrict__ lengths,
-                                                             int div, int mul) {
+                                                             int div, int mul, MorphArgs m = {}) {
   constexpr int NS = SHUF ? 2 : 1;
   const int Cn = SHUF ? d.Cout / 2 : d.Cout;
   const int Tn = SHUF ? d.Tout * 2 : d.Tout;
@@ -110,7 +121,17 @@ __global__ void __launch_bounds__(256) norm_apply_fwd_kernel(const avc_conv_desc
     }
   }
   float beta[4] = {0, 0, 0, 0}, gamma[4] = {1, 1, 1, 1};
-  if (d.cond) {
+  float4* sh_beta = nullptr;   // MORPH: [K] anchor rows of this warp's 4 channels, then [K] gamma rows
+  if constexpr (MORPH) {
+    extern __shared__ float4 morph_sh[];
+    sh_beta = morph_sh + (int64_t)(threadIdx.x >> 5) * 2 * m.K;
+    for (int k = lane; k < m.K; k += 32) {
+      const float* row = d.cond + (int64_t)b * d.cond_bstride + k * m.kstride + qn * 4;
+      sh_beta[k] = make_float4(__ldg(row), __ldg(row + 1), __ldg(row + 2), __ldg(row + 3));
+      sh_beta[m.K + k] = make_float4(__ldg(row + Cn), __ldg(row + Cn + 1), __ldg(row + Cn + 2), __ldg(row + Cn + 3));
+    }
+    __syncwarp();
+  } else if (d.cond) {
 #pragma unroll
     for (int c = 0; c < 4; ++c) {
       beta[c] = __ldg(d.cond + (int64_t)b * d.cond_bstride + qn * 4 + c);
@@ -125,6 +146,19 @@ __global__ void __launch_bounds__(256) norm_apply_fwd_kernel(const avc_conv_desc
 #pragma unroll
     for (int sx = 0; sx < NS; ++sx) {
       const int tn = SHUF ? 2 * t + sx : t;
+      if constexpr (MORPH) {
+        const float* wr = m.wtab + ((int64_t)b * Tn + tn) * m.K;
+        float4 bs = zero4(), gs = zero4();
+#pragma unroll 1
+        for (int k = 0; k < m.K; ++k) {
+          const float w = __ldg(wr + k);
+          const float4 bk = sh_beta[k], gk = sh_beta[m.K + k];
+          bs.x = fmaf(w, bk.x, bs.x); bs.y = fmaf(w, bk.y, bs.y); bs.z = fmaf(w, bk.z, bs.z); bs.w = fmaf(w, bk.w, bs.w);
+          gs.x = fmaf(w, gk.x, gs.x); gs.y = fmaf(w, gk.y, gs.y); gs.z = fmaf(w, gk.z, gs.z); gs.w = fmaf(w, gk.w, gs.w);
+        }
+        beta[0] = bs.x; beta[1] = bs.y; beta[2] = bs.z; beta[3] = bs.w;
+        gamma[0] = gs.x; gamma[1] = gs.y; gamma[2] = gs.z; gamma[3] = gs.w;
+      }
       float o[4];
 #pragma unroll
       for (int c = 0; c < 4; ++c) {
@@ -371,6 +405,32 @@ __global__ void __launch_bounds__(256) norm_bwd_cached_kernel(const avc_conv_des
   }
 }
 
+// thread = (sample b, layer frame j, anchor k): out[b][j][k] = mean over the f output frames t = j f + i of
+// w[b][k][s] / sum_k' w[b][k'][s], s = min(t, L_b - 1); frames j >= 8 ceil(L_b / 8) / f are 0
+__global__ void __launch_bounds__(256) morph_weights_kernel(const float* __restrict__ w, const int32_t* __restrict__ lengths,
+                                                            int B, int K, int T, int f, float* __restrict__ out, int T_l) {
+  const int64_t total = (int64_t)B * T_l * K;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+    const int k = (int)(i % K);
+    const int64_t bj = i / K;
+    const int j = (int)(bj % T_l), b = (int)(bj / T_l);
+    const int L = __ldg(lengths + b);
+    const int n = ((L + 7) / 8) * 8 / f;
+    float acc = 0.f;
+    if (j < n) {
+      const float* wb = w + (int64_t)b * K * T;
+      for (int u = 0; u < f; ++u) {
+        const int s = min(j * f + u, L - 1);
+        float sum = 0.f;
+        for (int kk = 0; kk < K; ++kk) sum += __ldg(wb + (int64_t)kk * T + s);
+        acc += __ldg(wb + (int64_t)k * T + s) / sum;
+      }
+      acc *= 1.f / (float)f;   // f is a power of two: exact
+    }
+    out[i] = acc;
+  }
+}
+
 // thread = (sample, 4-channel chunk, frame j past the sample's L_b); the modes of avc_varlen_tail (avc_b200.h)
 __global__ void __launch_bounds__(256) varlen_tail_kernel(float* __restrict__ a4, int64_t bstride, int B, int C, int T,
                                                           const int32_t* __restrict__ lengths, int div, int mul, int mode, int n) {
@@ -499,6 +559,39 @@ extern "C" int avc_norm_apply_varlen(const avc_conv_desc* d, const int32_t* leng
   if (d->shuffle) AVC_LAUNCH(norm_apply_fwd_kernel<true>, blocks, 256, 0, (cudaStream_t)stream, *d, lengths, len_div, len_mul);
   else AVC_LAUNCH(norm_apply_fwd_kernel<false>, blocks, 256, 0, (cudaStream_t)stream, *d, lengths, len_div, len_mul);
   AVC_CHECK_LAUNCH("norm_apply_varlen");
+  return AVC_OK;
+}
+
+extern "C" int avc_norm_apply_morph(const avc_conv_desc* d, const int32_t* lengths, int len_div, int len_mul, const float* wtab,
+                                    int K, int64_t cond_kstride, void* stream) {
+  int rc = validate_conv_desc(d, "avc_norm_apply_morph");
+  if (rc != AVC_OK) return rc;
+  AVC_REQUIRE(lengths && len_div >= 1 && len_mul >= 1, AVC_ERR_INVALID, "avc_norm_apply_morph: lengths null or len_div/len_mul < 1");
+  AVC_REQUIRE(d->save_c && d->out, AVC_ERR_INVALID, "avc_norm_apply_morph: null save_c/out");
+  AVC_REQUIRE(d->cond && wtab, AVC_ERR_INVALID, "avc_norm_apply_morph: null cond (anchor rows) or weight table");
+  AVC_REQUIRE(K >= 1 && K <= AVC_MORPH_MAX_K, AVC_ERR_INVALID, "avc_norm_apply_morph: K=%d outside [1, %d]", K, AVC_MORPH_MAX_K);
+  AVC_REQUIRE(!d->res || d->res_mode == AVC_RES_SAME || d->res_mode == AVC_RES_UP, AVC_ERR_INVALID,
+              "avc_norm_apply_morph: the residual must be SAME or UP");
+  AVC_REQUIRE(!d->mask, AVC_ERR_UNSUPPORTED, "avc_norm_apply_morph: mask is not supported");
+  const int Cn = d->shuffle ? d->Cout / 2 : d->Cout;
+  const int blocks = (int)cdiv64((int64_t)d->B * (Cn / 4) * 32, 256);
+  const size_t smem = (size_t)(256 / 32) * 2 * K * sizeof(float4);
+  const MorphArgs m{wtab, cond_kstride, K};
+  const auto kern = d->shuffle ? norm_apply_fwd_kernel<true, true> : norm_apply_fwd_kernel<false, true>;
+  AVC_LAUNCH(kern, blocks, 256, smem, (cudaStream_t)stream, *d, lengths, len_div, len_mul, m);
+  AVC_CHECK_LAUNCH("norm_apply_morph");
+  return AVC_OK;
+}
+
+extern "C" int avc_morph_weights(const float* w, const int32_t* lengths, int B, int K, int T, int f, float* out, int T_l,
+                                 void* stream) {
+  AVC_REQUIRE(w && lengths && out && B > 0 && T > 0 && T_l > 0, AVC_ERR_INVALID, "avc_morph_weights: bad argument");
+  AVC_REQUIRE(K >= 1 && K <= AVC_MORPH_MAX_K, AVC_ERR_INVALID, "avc_morph_weights: K=%d outside [1, %d]", K, AVC_MORPH_MAX_K);
+  AVC_REQUIRE(f >= 1 && f <= 8 && (f & (f - 1)) == 0, AVC_ERR_INVALID, "avc_morph_weights: f=%d is not 1, 2, 4 or 8", f);
+  int blocks = (int)cdiv64((int64_t)B * T_l * K, 256);
+  if (blocks > 148 * 16) blocks = 148 * 16;
+  AVC_LAUNCH(morph_weights_kernel, blocks, 256, 0, (cudaStream_t)stream, w, lengths, B, K, T, f, out, T_l);
+  AVC_CHECK_LAUNCH("morph_weights");
   return AVC_OK;
 }
 

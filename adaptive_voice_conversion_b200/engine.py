@@ -13,6 +13,7 @@ only provides device memory (torch.empty) and the current CUDA stream.
 from __future__ import annotations
 
 import ctypes as C
+import math
 import os
 from typing import Dict, List, Optional
 
@@ -428,7 +429,7 @@ class Engine:
 
     def conv(self, P, name, xin: A4, *, stride=1, shuffle=False, norm=False, cond=None, relu=False,
              res: Optional[A4] = None, res_mode=L.RES_NONE, out: Optional[A4] = None, train=False, round_out=False,
-             lens: Optional[Lengths] = None, tail=True):
+             lens: Optional[Lengths] = None, tail=True, morph=None):
         """One fused conv block.  round_out (tf32 mode only): round the block output to TF32 -- set ONLY when
         every consumer of `out` is a tensor-core conv operand (the first conv of a block, the bank convs), so
         that the consumer can skip its rounding pass.  The residual stream, the mean/std heads and out_conv
@@ -437,7 +438,11 @@ class Engine:
         lens: the valid frames of each sample of xin (a padded batch, inference only).  The conv first reflects each
         sample's last frames into its pad_right frames past them (unless tail=False: the caller did), and an
         InstanceNorm block runs as a plain conv + avc_norm_apply_varlen whatever its length, so that its statistics
-        cover the valid frames only.  Frames of out past a sample's valid ones are undefined."""
+        cover the valid frames only.  Frames of out past a sample's valid ones are undefined.
+
+        morph (with lens and cond): (wtab, K) -- the block's AdaIN row varies per frame, a mix of the K anchor rows
+        cond[:, k] (cond [B, K, 2 Cn]) with the weights of the layer's avc_morph_weights table wtab [B, Tn, K]; the
+        epilogue runs as avc_norm_apply_morph."""
         w = P[name + ".weight"]
         Cout, Cin, K = w.shape
         assert Cin == xin.C, (name, Cin, xin.C)
@@ -461,6 +466,8 @@ class Engine:
         tc_ok = (self.precision == "tf32" and not self.fwd_fp32 and Cin % 16 == 0 and not (stride == 2 and shuffle)
                  and "fwd_tc" in self.packed[name])
         varlen_norm = lens is not None and norm
+        if morph is not None and not (varlen_norm and cond is not None and not train):
+            raise L.AvcError(f"{name}: a morph needs a padded batch (lens), InstanceNorm and AdaIN, in inference")
         use_tc = tc_ok and not varlen_norm and (Tout * stride <= 144 or (not norm and not shuffle))
         tc_split = tc_ok and not use_tc and norm
         fused = use_tc or (not tc_split and not varlen_norm and ((not norm) or (Tout <= 128) or (Tout <= 256 and K in (1, 5))))
@@ -500,7 +507,12 @@ class Engine:
                 self._ck(self.lib.avc_conv_block_fwd(C.byref(d), self.stream), f"conv_block_fwd[{name}]")
             self._fill_epilogue(d, out, shuffle, norm, relu, cond, res, res_mode, stats)
             d.save_c = c.ptr
-            if varlen_norm:
+            if varlen_norm and morph is not None:
+                lo = lens.down(stride)
+                wtab, K = morph
+                self._ck(self.lib.avc_norm_apply_morph(C.byref(d), lo.t.data_ptr(), lo.div, lo.mul, wtab.data_ptr(), K,
+                                                       cond.stride(1), self.stream), f"norm_apply_morph[{name}]")
+            elif varlen_norm:
                 lo = lens.down(stride)
                 self._ck(self.lib.avc_norm_apply_varlen(C.byref(d), lo.t.data_ptr(), lo.div, lo.mul, self.stream),
                          f"norm_apply_varlen[{name}]")
@@ -1122,22 +1134,71 @@ class Engine:
                 aff.append(r)
         return conds, aff
 
-    def decoder_fwd(self, P, z4: A4, emb: torch.Tensor, train: bool, affine=None, lens: Optional[Lengths] = None):
+    def adain_factors(self) -> List[int]:
+        """f of each of the decoder's 2n AdaIN layers, in order: how many times coarser than the decoder output the
+        layer's normalised frames are (the product of the upsampling factors after it)."""
+        c = self.cfg["Decoder"]
+        ups = c["upsample"][: c["n_conv_blocks"]]
+        return [math.prod(ups[l + s:]) for l in range(len(ups)) for s in (0, 1)]
+
+    def morph_tables(self, weights: torch.Tensor, lens: Lengths, T_dec: int) -> Dict[int, torch.Tensor]:
+        """{f: [B, T_dec / f, K] table of avc_morph_weights} for every f at which a decoder AdaIN layer normalises: f is
+        the product of the upsampling factors after the layer.  weights: float32 [B, K, T] at the source frame rate;
+        lens.t: the source lengths; T_dec: the decoder output's extent."""
+        B, K, T = weights.shape
+        tabs = {}
+        for f in sorted(set(self.adain_factors())):
+            tabs[f] = self.empty(B, T_dec // f, K)
+            self._ck(self.lib.avc_morph_weights(weights.data_ptr(), lens.t.data_ptr(), B, K, T, f, tabs[f].data_ptr(),
+                                                T_dec // f, self.stream), f"morph_weights[f={f}]")
+        return tabs
+
+    def decoder_fwd(self, P, z4: A4, emb: Optional[torch.Tensor], train: bool, affine=None, lens: Optional[Lengths] = None,
+                    morph=None):
         """Decoder.forward (model.py:347-371) -> dec4 A4 [B, c_out, 8*T].  affine: the result of decoder_affine_fwd
         when the caller already computed it (on the speaker branch's stream).  lens: the valid frames of each sample of
-        z4 (a padded batch, inference only); dec4 is then exactly 0 past each sample's valid frames."""
+        z4 (a padded batch, inference only); dec4 is then exactly 0 past each sample's valid frames.
+
+        morph (with lens, inference only; emb is then unused): (codes [B, K, c_out], weights [B, K, T]) -- a time-varying
+        mix of K anchor codes (AE.inference_morph).  The anchors' AdaIN rows are one decoder_affine_fwd on the B K codes,
+        the per-layer weight tables come from morph_tables (lens.t: the source lengths), and every AdaIN layer's
+        epilogue is avc_norm_apply_morph; in_conv_layer (no AdaIN) stays on avc_norm_apply_varlen."""
         c = self.cfg["Decoder"]
         dn = "decoder"
         ctx: dict = {}
         out, r_in = self.conv(P, f"{dn}.in_conv_layer", z4, norm=True, relu=True, train=train, lens=lens)
         nblk = c["n_conv_blocks"]
-        conds, aff = affine if affine is not None else self.decoder_affine_fwd(P, emb, train)
+        ups = c["upsample"][:nblk]
+        if morph is not None:
+            if lens is None or train or affine is not None:
+                raise L.AvcError("Engine.decoder_fwd: a morph needs lens, train=False and no precomputed affine rows")
+            codes, weights = morph
+            B, K = codes.shape[0], codes.shape[1]
+            rows, aff = self.decoder_affine_fwd(P, codes.reshape(B * K, codes.shape[2]), False)
+            conds = rows.view(B, K, *rows.shape[1:])            # [B, K, 2n, 2 c_h]
+            fs = self.adain_factors()
+            tabs = self.morph_tables(weights, lens, z4.T * fs[0])
+
+            def layer(i):
+                return conds[:, :, i]
+
+            def mix(i):
+                return tabs[fs[i]], K
+        else:
+            conds, aff = affine if affine is not None else self.decoder_affine_fwd(P, emb, train)
+
+            def layer(i):
+                return conds[:, i]
+
+            def mix(i):
+                return None
         blocks = []
-        for l, up in enumerate(c["upsample"][:nblk]):
-            y, r1 = self.conv(P, f"{dn}.first_conv_layers.{l}", out, norm=True, cond=conds[:, 2 * l], relu=True, train=train,
-                              round_out=True, lens=lens)
-            new, r2 = self.conv(P, f"{dn}.second_conv_layers.{l}", y, shuffle=(up > 1), norm=True, cond=conds[:, 2 * l + 1],
-                                relu=True, res=out, res_mode=L.RES_UP if up > 1 else L.RES_SAME, train=train, lens=lens)
+        for l, up in enumerate(ups):
+            y, r1 = self.conv(P, f"{dn}.first_conv_layers.{l}", out, norm=True, cond=layer(2 * l), relu=True, train=train,
+                              round_out=True, lens=lens, morph=mix(2 * l))
+            new, r2 = self.conv(P, f"{dn}.second_conv_layers.{l}", y, shuffle=(up > 1), norm=True, cond=layer(2 * l + 1),
+                                relu=True, res=out, res_mode=L.RES_UP if up > 1 else L.RES_SAME, train=train, lens=lens,
+                                morph=mix(2 * l + 1))
             blocks.append((r1, r2, up))
             out = new
             if lens is not None:

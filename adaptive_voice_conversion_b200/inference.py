@@ -8,6 +8,7 @@ the batched entry point BASELINE config 5 measures.
 """
 from __future__ import annotations
 
+import bisect
 import collections
 import os
 import pickle
@@ -355,6 +356,77 @@ class Inferencer(object):
                 out[i] = dec[j, :, :8 * -(-src[i].shape[1] // 8)].transpose(0, 1)
         self.model.engine(dev).check_tc_status()
         return out
+
+    @torch.no_grad()
+    def inference_morph(self, xs, codes, weights, batch_max: int = PADDED_BATCH_MAX):
+        """Time-varying speaker morphs (AE.inference_morph) of many sources: xs[i] a [T_i, n_mels] normalised mel,
+        codes[i] its [K_i, c_out] anchor codes and weights[i] their [K_i, T_i] weights at the source frame rate (device
+        tensors).  The sources run in padded_batches' grid; a batch's K is its largest K_i, shorter anchor lists padded
+        with zero-weight anchors (which change no bit).  One CUDA graph per (B, T, K) shape (AVC_INFER_GRAPH=1) with the
+        sources, anchors and weights in static buffers, bit for bit the eager result.  Returns inference_padded's list
+        of mels.  ValueError, before anything runs, naming a source whose shapes or weights are invalid (weights finite,
+        >= 0, a positive sum on every frame)."""
+        if not len(xs) == len(codes) == len(weights):
+            raise ValueError("inference_morph: xs, codes and weights must have the same length")
+        if not xs:
+            return []
+        if int(self.config["data_loader"]["frame_size"]) != 1:
+            raise ValueError("inference_morph: supports data_loader.frame_size 1 only")
+        from ._lib import MORPH_MAX_K
+        c_out = self.config["SpeakerEncoder"]["c_out"]
+        dev = xs[0].device
+        for i, (x, c, w) in enumerate(zip(xs, codes, weights)):
+            K = int(c.shape[0]) if isinstance(c, torch.Tensor) and c.dim() == 2 else 0
+            for t in (c, w):
+                if not isinstance(t, torch.Tensor) or t.dtype != torch.float32 or t.device != dev:
+                    raise ValueError(f"inference_morph: source {i}: codes and weights must be float32 on {dev}")
+            if (not 1 <= K <= MORPH_MAX_K or tuple(c.shape) != (K, c_out)
+                    or tuple(w.shape) != (K, int(x.shape[0]))):
+                raise ValueError(f"inference_morph: source {i}: expected codes [K, {c_out}] with 1 <= K <= {MORPH_MAX_K} "
+                                 f"and weights [K, {int(x.shape[0])}], got {tuple(c.shape)} and {tuple(w.shape)}")
+        # every source's frames as rows of one table (absent anchors 0): a handful of launches and one synchronise
+        offs = [0]
+        for w in weights:
+            offs.append(offs[-1] + int(w.shape[1]))
+        table = torch.zeros(offs[-1], max(int(w.shape[0]) for w in weights), device=dev)
+        for i, w in enumerate(weights):
+            table[offs[i]:offs[i + 1], :w.shape[0]].copy_(w.t())
+        s = table.sum(1)
+        bad = (~torch.isfinite(table) | (table < 0)).any(1) | ~(s > 0) | ~torch.isfinite(s)
+        if bool(bad.any()):
+            i = bisect.bisect_right(offs, int(bad.nonzero()[0])) - 1
+            raise ValueError(f"inference_morph: source {i}: weights must be finite and >= 0 with a positive sum on every "
+                             f"frame")
+        src = self._source_frames(xs, "inference_morph")
+        out = [None] * len(src)
+        for idx, T, _, Bp in padded_batches([s.shape[1] for s in src], [0] * len(src), batch_max):
+            K = max(int(codes[i].shape[0]) for i in idx)
+            xb, cb, wb, lx, run = self._morph_slot(Bp, src[0].shape[0], T, K, dev)
+            rows = idx + [idx[0]] * (Bp - len(idx))                # rows past the batch repeat its first source
+            cb.zero_()
+            wb.zero_()
+            for j, i in enumerate(rows):
+                n, k = src[i].shape[1], codes[i].shape[0]
+                xb[j, :, :n].copy_(src[i])
+                cb[j, :k].copy_(codes[i])
+                wb[j, :k, :n].copy_(weights[i])
+            lx.copy_(torch.tensor([src[i].shape[1] for i in rows], dtype=torch.int32))
+            dec = run()
+            for j, i in enumerate(idx):
+                out[i] = dec[j, :, :8 * -(-src[i].shape[1] // 8)].transpose(0, 1)
+        self.model.engine(dev).check_tc_status()
+        return out
+
+    def _morph_slot(self, B, C, T, K, dev):
+        """(x, codes, weights, lengths, convert) of one padded morph shape (AE.inference_morph), as _padded_slot.  The
+        weights start at 1 so that the capture's eager call is a valid morph."""
+        def make():
+            xb = torch.zeros(B, C, T, device=dev)
+            cb = torch.zeros(B, K, self.config["SpeakerEncoder"]["c_out"], device=dev)
+            wb = torch.ones(B, K, T, device=dev)
+            lx = torch.full((B,), T, dtype=torch.int32, device=dev)
+            return (xb, cb, wb, lx), lambda: self.model.inference_morph(xb, cb, wb, lengths=lx)
+        return self._graph_slot(("morph", B, C, T, K, str(dev), self._param_version()), make)
 
     @torch.no_grad()
     def inference_one_utterance(self, x, x_cond):

@@ -18,6 +18,7 @@ model on CPU tensors raises.
 """
 from __future__ import annotations
 
+import math
 import os
 import types
 
@@ -447,6 +448,57 @@ class AE(nn.Module):
             mu, log_sigma = _ContentFn.apply(self, x, *self._params("content_encoder."))
             return _DecoderFn.apply(self, mu, log_sigma, None, emb, *self._params("decoder."))
 
+    def inference_morph(self, x: torch.Tensor, codes: torch.Tensor, weights: torch.Tensor, *,
+                        lengths: Optional[torch.Tensor] = None):
+        """A time-varying speaker morph (no gradient): content mean of x [B, C, T], decoder conditioned at every frame
+        on a mix of K anchor codes codes [B, K, c_out] with weights [B, K, T] at the source frame rate.  lengths: the
+        valid frames L_b of each sample (None: every sample full length); frames past L_b of x and of weights are
+        ignored, whatever they hold.  Returns dec [B, C, 8 ceil(T/8)], exactly 0 past each sample's 8 ceil(L_b/8) frames.
+
+        Output frame t < 8 ceil(L_b/8) uses the weights of source frame min(t, L_b - 1), normalised to sum 1; a decoder
+        AdaIN layer whose frames are f times coarser uses their mean over its f output frames.  Each AdaIN affine layer
+        is affine in the code, so a frame's AdaIN scale and shift are the same mix of the anchors' ordinary ones: one-hot
+        weights constant over time give inference_from_embeddings(x, codes[:, k], lengths=) bit for bit, and anchors of
+        zero weight change no bit.  Every decoder InstanceNorm still pools its statistics over the whole utterance, so a
+        switch of speaker at one time also moves the frames before it a little: a morph is not a splice of separate
+        conversions.
+
+        Always the padded path, frame_size 1 only.  AvcError before any launch for wrong shapes, dtypes or devices,
+        lengths below mcd.min_frames, K outside [1, AVC_MORPH_MAX_K], or weights on a valid frame that are not finite
+        and >= 0 with a positive sum (not checked while a CUDA graph is being captured: the caller checks them)."""
+        x = _check_input(x, "AE.inference_morph(x)")
+        B, _, T = x.shape
+        c_out = self.config["SpeakerEncoder"]["c_out"]
+        fs = int(self.config.get("data_loader", {}).get("frame_size", 1))
+        ups, subs = self.config["Decoder"]["upsample"], self.config["ContentEncoder"]["subsample"]
+        if (fs != 1 or math.prod(ups[: self.config["Decoder"]["n_conv_blocks"]]) != 8
+                or math.prod(subs[: self.config["ContentEncoder"]["n_conv_blocks"]]) != 8):
+            raise L.AvcError("AE.inference_morph: supports frame_size 1 and a content encoder / decoder that subsample / "
+                             "upsample by 8")
+        for t, what, shape in ((codes, "codes", "[B, K, c_out]"), (weights, "weights", "[B, K, T]")):
+            if (not isinstance(t, torch.Tensor) or t.dtype != torch.float32 or t.dim() != 3 or t.device != x.device):
+                raise L.AvcError(f"AE.inference_morph({what}): expected float32 {shape} on {x.device}, got "
+                                 f"{getattr(t, 'dtype', type(t).__name__)} {tuple(getattr(t, 'shape', ()))} on "
+                                 f"{getattr(t, 'device', None)}")
+        K = codes.shape[1]
+        if not 1 <= K <= L.MORPH_MAX_K:
+            raise L.AvcError(f"AE.inference_morph(codes): K={K} anchors; 1 to {L.MORPH_MAX_K} are supported")
+        if tuple(codes.shape) != (B, K, c_out) or tuple(weights.shape) != (B, K, T):
+            raise L.AvcError(f"AE.inference_morph: expected codes [{B}, K, {c_out}] and weights [{B}, K, {T}] (x is "
+                             f"{tuple(x.shape)}), got {tuple(codes.shape)} and {tuple(weights.shape)}")
+        lx = _check_lengths(lengths, x, self._min_frames()[0], "AE.inference_morph(lengths)")
+        if not torch.cuda.is_current_stream_capturing():
+            valid = torch.arange(T, device=x.device)[None, :] < lx[:, None].to(torch.int64)       # [B, T]
+            w = torch.where(valid[:, None, :], weights, torch.ones((), device=x.device))
+            s = w.sum(1)
+            bad = (~torch.isfinite(w) | (w < 0)).any(1) | ~(s > 0) | ~torch.isfinite(s)           # [B, T]
+            if bool(bad.any()):
+                b, t = (int(v) for v in bad.nonzero()[0])
+                raise L.AvcError(f"AE.inference_morph(weights): sample {b}, frame {t}: the weights must be finite and "
+                                 f">= 0 with a positive sum on every valid frame, got {weights[b, :, t].tolist()}")
+        with torch.no_grad():
+            return self._decode_padded(x, lx, None, morph=(codes.contiguous(), weights.contiguous()))
+
     def get_content_means(self, x: torch.Tensor, *, lengths: torch.Tensor):
         """(mu [B, c_out, T_lat], latent lengths int32 [B]) of a padded batch x [B, C, T]: the content encoder's mean
         head as the padded AE.inference computes it (no gradient); mu[b, :, :latent[b]] is sample b's, later frames are
@@ -487,10 +539,10 @@ class AE(nn.Module):
                     emb.record_stream(main)
         return self._decode_padded(x, lx, emb, join)
 
-    def _decode_padded(self, x, lx, emb, join=None):
+    def _decode_padded(self, x, lx, emb, join=None, morph=None):
         """The content and decoder half of the padded AE.inference: dec [B, C, 8 ceil(T/8)] of x's content mean
         conditioned on emb.  join(), when given, runs between the content encoder and the decoder (the speaker branch's
-        stream join)."""
+        stream join).  morph: (codes, weights) of inference_morph instead of emb."""
         B, Cc, T = x.shape
         xp = _pad_time(x, varlen_extent(self.config, T, source=True))
         dev = x.device
@@ -500,6 +552,6 @@ class AE(nn.Module):
         if join is not None:
             join()
         eng, P = self._eval_stack("decoder.", dev)
-        dec4, _ = eng.decoder_fwd(P, z4, emb, False, lens=ctx["lens"])
+        dec4, _ = eng.decoder_fwd(P, z4, emb, False, lens=ctx["lens"], morph=morph)
         To = 8 * -(-T // 8)
         return eng.unpack_a4(dec4)[:, :, :To].contiguous()

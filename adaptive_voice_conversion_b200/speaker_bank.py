@@ -76,6 +76,75 @@ def parse_spec(spec: str) -> List[tuple]:
     return out
 
 
+def parse_keyframe(text: str) -> tuple:
+    """(spec, seconds) of a morph keyframe ``SPEC@SECONDS``: SPEC in parse_spec's syntax, SECONDS a finite number >= 0.
+    ValueError for a missing @, a malformed or negative time, or a bad SPEC."""
+    spec, sep, sec = str(text).rpartition("@")
+    if not sep:
+        raise ValueError(f"keyframe {text!r}: expected SPEC@SECONDS, e.g. p225@0 or p225:0.5,p226:0.5@12")
+    parse_spec(spec)
+    try:
+        t = float(sec)
+    except ValueError:
+        raise ValueError(f"keyframe {text!r}: time {sec!r} is not a number") from None
+    if not math.isfinite(t) or t < 0:
+        raise ValueError(f"keyframe {text!r}: time {sec!r} must be a finite number of seconds >= 0")
+    return spec, t
+
+
+def morph_weights(keyframes: Sequence[tuple], n_frames: int, frames_per_second: float):
+    """(names, weights float32 [K, n_frames]) of a morph given as keyframes [(SPEC, seconds), ...]: names are the K
+    distinct speakers in order of first mention.  A keyframe's weight vector is its spec's weights over the names,
+    divided by their sum (the mix SpeakerBank.code makes of it).  Frame t lies at t / frames_per_second seconds; between
+    consecutive keyframes the vectors are interpolated linearly, the first keyframe's is held before it and the last
+    one's after it, and at two keyframes of the same time the later one takes over there (a hard cut).  Computed in
+    float64, rounded once.  ValueError for an empty list, times that are negative or decrease, or a bad spec."""
+    if not keyframes:
+        raise ValueError("morph: no keyframes")
+    if int(n_frames) < 1 or not frames_per_second > 0:
+        raise ValueError("morph: n_frames must be >= 1 and frames_per_second > 0")
+    names: List[str] = []
+    vecs, times = [], []
+    for spec, t in keyframes:
+        t = float(t)
+        if not math.isfinite(t) or t < 0:
+            raise ValueError(f"morph: keyframe time {t} must be a finite number of seconds >= 0")
+        if times and t < times[-1]:
+            raise ValueError(f"morph: keyframe times must not decrease ({spec}@{t} follows a keyframe at {times[-1]})")
+        parts = parse_spec(spec)
+        for n, _ in parts:
+            if n not in names:
+                names.append(n)
+        vecs.append(parts)
+        times.append(t)
+    V = np.zeros((len(vecs), len(names)), dtype=np.float64)
+    for i, parts in enumerate(vecs):
+        total = sum(w for _, w in parts)
+        for n, w in parts:
+            V[i, names.index(n)] = w / total
+    ts = np.arange(int(n_frames), dtype=np.float64) / float(frames_per_second)
+    tk = np.asarray(times, dtype=np.float64)
+    i = np.searchsorted(tk, ts, side="right") - 1                 # last keyframe at or before the frame
+    out = np.empty((int(n_frames), len(names)), dtype=np.float64)
+    before, after = i < 0, i >= len(tk) - 1
+    out[before] = V[0]
+    out[after & ~before] = V[-1]
+    mid = ~before & ~after
+    if mid.any():
+        j = i[mid]
+        a = ((ts[mid] - tk[j]) / (tk[j + 1] - tk[j]))[:, None]
+        out[mid] = (1 - a) * V[j] + a * V[j + 1]
+    return names, out.T.astype(np.float32)
+
+
+def morph_table(bank: "SpeakerBank", keyframes: Sequence[tuple], n_frames: int, frames_per_second: float):
+    """(codes float32 [K, c_out] on the bank's device, weights float32 [K, n_frames] on the host) of a morph through
+    `bank` (morph_weights; Inferencer.inference_morph takes them).  ValueError for a speaker not in the bank."""
+    names, w = morph_weights(keyframes, n_frames, frames_per_second)
+    rows = [bank.index(n) for n in names]
+    return bank.codes[rows].contiguous(), torch.from_numpy(w)
+
+
 class SpeakerBank:
     """Per-speaker codes of one speaker encoder.
 

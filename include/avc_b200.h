@@ -269,6 +269,32 @@ int avc_time_mean_bwd(const float* dout /*[B][C]*/, float* da4, int64_t bstride,
  * UP / POOL residuals as in avc_norm_apply_fwd; a POOL residual's input holds ceil(lengths[b] / (len_div / 2)) *
  * len_mul valid frames (len_div even) and its odd last frame is divided by 1.  mask must be null. */
 int avc_norm_apply_varlen(const avc_conv_desc* d, const int32_t* lengths, int len_div, int len_mul, void* stream);
+/* Time-varying speaker morphs (AE.inference_morph): the decoder's AdaIN layers conditioned on a per-frame mix of K anchor
+ * codes.  Each AdaIN affine layer is affine in the code, so conditioning frame j on sum_k w_k c_k (sum_k w_k = 1) gives
+ * it the AdaIN row sum_k w_k row_k of the anchors' ordinary rows.
+ *
+ * avc_morph_weights: w is a DEVICE float32 [B][K][T] table of anchor weights at the source frame rate, lengths the
+ * source lengths L_b (DEVICE int32 [B], 1 <= L_b <= T).  Output frame t < T_o(b) = 8 ceil(L_b / 8) of the decoder uses
+ * the normalised weights of source frame s = min(t, L_b - 1): wbar_k = w_k / (w_0 + w_1 + ...), the sum in k order, in
+ * float32.  A layer whose frames are f times coarser than the decoder output (f in {1, 2, 4, 8}: the product of the
+ * upsampling factors after it) uses at frame j the mean of wbar over t in [j f, (j + 1) f), added in t order and
+ * multiplied by 1 / f (exact).  out: float32 [B][T_l][K] (frame-major: a frame's K weights are contiguous); frames
+ * j >= T_o(b) / f are 0.  The caller validates the weights (finite, >= 0, a positive sum on every valid frame); frames
+ * of w past L_b are never read.  AVC_ERR_INVALID for null pointers, non-positive sizes, K outside [1, AVC_MORPH_MAX_K]
+ * or another f.
+ *
+ * avc_norm_apply_morph: avc_norm_apply_varlen (the same statistics over L_b conv outputs, shuffle, ReLU, SAME / UP
+ * residuals, AVC_F_ROUND_OUT, nothing written past L_b) whose AdaIN row varies with the normalised frame tn: anchor k's
+ * row of sample b is beta_k = d->cond[b * cond_bstride + k * cond_kstride + c], gamma_k = the same + Cn, and frame tn
+ * gets beta = sum_k wtab[b][tn][k] beta_k, gamma likewise, each formed with fmaf in k order from 0.  wtab is a layer's
+ * avc_morph_weights table, [B][Tn][K] with Tn = d->Tout * (1 + d->shuffle).  One-hot weights give avc_norm_apply_varlen's
+ * bits with that anchor's row; anchors of zero weight change no bit.  Each warp stages its sample's K anchor rows of its 4
+ * channels in shared memory (2 K float4 per warp).  AVC_ERR_INVALID for a bad descriptor, null lengths / save_c / out /
+ * cond / wtab, K outside [1, AVC_MORPH_MAX_K] or a POOL residual; AVC_ERR_UNSUPPORTED for a mask. */
+#define AVC_MORPH_MAX_K 64
+int avc_morph_weights(const float* w, const int32_t* lengths, int B, int K, int T, int f, float* out, int T_l, void* stream);
+int avc_norm_apply_morph(const avc_conv_desc* d, const int32_t* lengths, int len_div, int len_mul, const float* wtab, int K,
+                         int64_t cond_kstride, void* stream);
 /* avc_time_mean_fwd over each sample's L_b frames. */
 int avc_time_mean_varlen_fwd(const float* a4, int64_t bstride, float* out /*[B][C]*/, int B, int C, int T,
                              const int32_t* lengths, int len_div, int len_mul, void* stream);

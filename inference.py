@@ -35,6 +35,15 @@ Speaker banks (speaker_bank.py): -bank bank.pt -speaker SPEC converts to a banke
 
     python inference.py -c config.yaml -m model.ckpt -a attr.pkl -s src.wav -bank bank.pt -speaker p225 -o out.wav
 
+Time-varying morphs: -bank bank.pt -morph SPEC@SECONDS [SPEC@SECONDS ...] converts one source with the decoder
+conditioned, frame by frame, on a mix of banked speakers (Inferencer.inference_morph).  Each keyframe names a speaker
+or a mix at a time in seconds (frames at the vocoder's sr / hop_length per second); the mix glides linearly from one
+keyframe to the next, is held before the first and after the last, and two keyframes at the same time make a hard
+cut.  -morph excludes -t, -speaker and -pairs:
+
+    python inference.py -c config.yaml -m model.ckpt -a attr.pkl -s dialogue.wav -bank bank.pt \
+        -morph p225@0 p225@4.0 p226@4.3 p226@9 p225:0.5,p226:0.5@12 -o out.wav
+
 With -bank, a -pairs target field ``@SPEC`` is resolved through the bank (a field naming an existing file stays that
 file, even one whose name starts with @), and its output name defaults to ``<source stem>_to_<SPEC>.wav`` (``:`` and
 ``,`` replaced by ``-`` and ``+``).  Without -bank every field is read as above.  The sources and targets are analysed in one batched Vocoder.wav_to_mel call (.npy mels are read
@@ -210,7 +219,22 @@ def load_bank(path, model):
 
 
 def check_args(p, args):
-    """Argument errors (p.error): -t, or -bank with -speaker, for one conversion; -speaker needs -bank."""
+    """Argument errors (p.error): -t, or -bank with -speaker, for one conversion; -speaker needs -bank; -morph needs
+    -bank, excludes -t, -speaker and -pairs, and its keyframes must parse."""
+    if args.morph is not None:
+        if not args.bank:
+            p.error("-morph needs -bank")
+        if args.target is not None or args.speaker is not None or args.pairs:
+            p.error("-morph converts one source with banked speakers: it excludes -t, -speaker and -pairs")
+        from adaptive_voice_conversion_b200.speaker_bank import parse_keyframe
+        try:
+            args.keyframes = [parse_keyframe(k) for k in args.morph]
+        except ValueError as e:
+            p.error(str(e))
+        times = [t for _, t in args.keyframes]
+        if any(b < a for a, b in zip(times, times[1:])):
+            p.error(f"-morph: keyframe times must not decrease, got {times}")
+        return
     if args.speaker is not None and not args.bank:
         p.error("-speaker needs -bank")
     if args.pairs:
@@ -239,6 +263,8 @@ def parser():
     p.add_argument("-pairs", help="file of 'source target [output_name]' lines: convert them all, into the -o directory")
     p.add_argument("-bank", help="speaker bank (speaker_bank.py) for -speaker and the @SPEC fields of -pairs")
     p.add_argument("-speaker", help="banked target: NAME or a weighted mix NAME:W,NAME:W,... (needs -bank)")
+    p.add_argument("-morph", nargs="+", metavar="SPEC@SECONDS",
+                   help="time-varying target: banked speakers or mixes at keyframe times, interpolated (needs -bank)")
     return p
 
 
@@ -265,7 +291,15 @@ if __name__ == "__main__":
     src = read(args.source)
     src = inf.normalize(src) if inf.attr is not None else src
     dev = local_device()
-    if args.bank:
+    if args.morph:
+        from adaptive_voice_conversion_b200.speaker_bank import morph_table
+        from adaptive_voice_conversion_b200.vocoder import AudioParams
+        hp = vocoder.hp if vocoder is not None else AudioParams()
+        codes, weights = morph_table(load_bank(args.bank, inf.model), args.keyframes, src.shape[0], hp.sr / hp.hop_length)
+        mel = inf.inference_morph([torch.from_numpy(src).to(dev)], [codes], [weights.to(dev)])[0].cpu().numpy()
+        mel = inf.denormalize(mel) if inf.attr is not None else mel
+        wav = inf.vocoder.melspectrogram2wav(mel) if inf.vocoder is not None else None
+    elif args.bank:
         code = load_bank(args.bank, inf.model).code(args.speaker)
         mel = inf.inference_with_codes([torch.from_numpy(src).to(dev)], code[None])[0].cpu().numpy()
         mel = inf.denormalize(mel) if inf.attr is not None else mel
