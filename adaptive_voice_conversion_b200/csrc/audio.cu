@@ -319,6 +319,8 @@ __global__ void __launch_bounds__(1024) deemphasis_kernel(avc_audio_desc d, floa
 // out[rows][N] = pro(in)[rows][K] x mat[K][N], 64 x 64 tiles, 16-deep k slices, 4 x 4 outputs per thread.
 //   MEL_TO_MAG: pro = normalised mel -> amplitude 10^((clip(v,0,1) max_db - max_db + ref_db)/20), K = n_mels, N = bins
 //   MAG_TO_MEL: epilogue amplitude -> clip((20 log10(max(1e-5, v)) - ref_db + max_db)/max_db, 1e-8, 1), K = bins
+// Column tiles on gridDim.x; row tiles on gridDim.y, which is capped at 65 535, so a CTA takes row tiles blockIdx.y,
+// blockIdx.y + gridDim.y, ...: every row count fits, and each output is still one thread's sum in k order.
 template <int DIR>
 __global__ void __launch_bounds__(256) mel_gemm_kernel(avc_mel_desc d) {
   __shared__ float As[16][64 + 4];
@@ -326,50 +328,53 @@ __global__ void __launch_bounds__(256) mel_gemm_kernel(avc_mel_desc d) {
   const int M = d.rows;
   const int K = DIR == AVC_MEL_TO_MAG ? d.n_mels : d.n_bins;
   const int N = DIR == AVC_MEL_TO_MAG ? d.n_bins : d.n_mels;
-  const int r0 = blockIdx.y * 64, c0 = blockIdx.x * 64;
+  const int row_tiles = cdiv(M, 64), c0 = blockIdx.x * 64;
   const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
-  float acc[4][4] = {};
-  for (int k0 = 0; k0 < K; k0 += 16) {
+  for (int rt = blockIdx.y; rt < row_tiles; rt += gridDim.y) {
+    const int r0 = rt * 64;
+    float acc[4][4] = {};
+    for (int k0 = 0; k0 < K; k0 += 16) {
 #pragma unroll
-    for (int e = 0; e < 4; ++e) {
-      const int id = threadIdx.x + 256 * e;
-      const int r = id >> 4, kk = id & 15;
-      float v = 0.f;
-      if (r0 + r < M && k0 + kk < K) {
-        v = __ldg(d.in + (int64_t)(r0 + r) * K + k0 + kk);
-        if (DIR == AVC_MEL_TO_MAG) v = exp10f((fminf(1.f, fmaxf(0.f, v)) * d.max_db - d.max_db + d.ref_db) / 20.f);
+      for (int e = 0; e < 4; ++e) {
+        const int id = threadIdx.x + 256 * e;
+        const int r = id >> 4, kk = id & 15;
+        float v = 0.f;
+        if (r0 + r < M && k0 + kk < K) {
+          v = __ldg(d.in + (int64_t)(r0 + r) * K + k0 + kk);
+          if (DIR == AVC_MEL_TO_MAG) v = exp10f((fminf(1.f, fmaxf(0.f, v)) * d.max_db - d.max_db + d.ref_db) / 20.f);
+        }
+        As[kk][r] = v;
+        const int kb = id >> 6, c = id & 63;
+        Bs[kb][c] = (k0 + kb < K && c0 + c < N) ? __ldg(d.mat + (int64_t)(k0 + kb) * N + c0 + c) : 0.f;
       }
-      As[kk][r] = v;
-      const int kb = id >> 6, c = id & 63;
-      Bs[kb][c] = (k0 + kb < K && c0 + c < N) ? __ldg(d.mat + (int64_t)(k0 + kb) * N + c0 + c) : 0.f;
-    }
-    __syncthreads();
+      __syncthreads();
 #pragma unroll
-    for (int kk = 0; kk < 16; ++kk) {
-      float av[4], bv[4];
+      for (int kk = 0; kk < 16; ++kk) {
+        float av[4], bv[4];
 #pragma unroll
-      for (int i = 0; i < 4; ++i) { av[i] = As[kk][ty + 16 * i]; bv[i] = Bs[kk][tx + 16 * i]; }
+        for (int i = 0; i < 4; ++i) { av[i] = As[kk][ty + 16 * i]; bv[i] = Bs[kk][tx + 16 * i]; }
 #pragma unroll
-      for (int i = 0; i < 4; ++i)
+        for (int i = 0; i < 4; ++i)
 #pragma unroll
-        for (int jj = 0; jj < 4; ++jj) acc[i][jj] = fmaf(av[i], bv[jj], acc[i][jj]);
-    }
-    __syncthreads();
-  }
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    const int r = r0 + ty + 16 * i;
-    if (r >= M) continue;
-#pragma unroll
-    for (int jj = 0; jj < 4; ++jj) {
-      const int c = c0 + tx + 16 * jj;
-      if (c >= N) continue;
-      float v = acc[i][jj];
-      if (DIR == AVC_MAG_TO_MEL) {
-        const float db = 20.f * log10f(fmaxf(1e-5f, v));
-        v = fminf(1.f, fmaxf(1e-8f, (db - d.ref_db + d.max_db) / d.max_db));
+          for (int jj = 0; jj < 4; ++jj) acc[i][jj] = fmaf(av[i], bv[jj], acc[i][jj]);
       }
-      d.out[(int64_t)r * N + c] = v;
+      __syncthreads();
+    }
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      const int r = r0 + ty + 16 * i;
+      if (r >= M) continue;
+#pragma unroll
+      for (int jj = 0; jj < 4; ++jj) {
+        const int c = c0 + tx + 16 * jj;
+        if (c >= N) continue;
+        float v = acc[i][jj];
+        if (DIR == AVC_MAG_TO_MEL) {
+          const float db = 20.f * log10f(fmaxf(1e-5f, v));
+          v = fminf(1.f, fmaxf(1e-8f, (db - d.ref_db + d.max_db) / d.max_db));
+        }
+        d.out[(int64_t)r * N + c] = v;
+      }
     }
   }
 }
@@ -824,7 +829,8 @@ extern "C" int avc_mel_project(const avc_mel_desc* d, void* stream) {
   AVC_REQUIRE(d->dir == AVC_MEL_TO_MAG || d->dir == AVC_MAG_TO_MEL, AVC_ERR_INVALID, "avc_mel_project: unknown dir %d", d->dir);
   if (d->rows == 0) return AVC_OK;
   const int N = d->dir == AVC_MEL_TO_MAG ? d->n_bins : d->n_mels;
-  const dim3 grid(cdiv(N, 64), cdiv(d->rows, 64));
+  // gridDim.x (column tiles) allows 2^31 - 1, more than any int N needs; gridDim.y is clamped and looped over
+  const dim3 grid(cdiv(N, 64), min(cdiv(d->rows, 64), 65535));
   cudaStream_t st = (cudaStream_t)stream;
   if (d->dir == AVC_MEL_TO_MAG) mel_gemm_kernel<AVC_MEL_TO_MAG><<<grid, 256, 0, st>>>(*d);
   else mel_gemm_kernel<AVC_MAG_TO_MEL><<<grid, 256, 0, st>>>(*d);

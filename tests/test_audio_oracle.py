@@ -104,6 +104,14 @@ def test_deemphasis_equals_lfilter_and_inverts_preemphasis():
     assert np.abs(ao.deemphasis(ao.preemphasis(x)) - x).max() < 1e-11
 
 
+@pytest.mark.parametrize("coef", [0.0, 0.5, 0.999, 1.0, -0.97])
+def test_deemphasis_equals_lfilter_at_other_coefficients(coef):
+    """tests/test_gpu_vocoder_kernels.py checks avc_deemphasis against lfilter at these coefficients."""
+    x = signal(20000, 4)
+    ref = ss.lfilter([1.0], [1.0, -coef], x)
+    assert np.abs(ao.deemphasis(x, coef) - ref).max() <= 1e-11 * max(1.0, np.abs(ref).max())
+
+
 def test_too_short_is_rejected():
     with pytest.raises(ValueError, match="n_fft/2"):
         ao.stft(np.zeros(1024))

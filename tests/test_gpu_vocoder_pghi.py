@@ -100,6 +100,31 @@ def test_parents_and_phases_match_the_heap(batch, device_run):
     assert worst < PHASE_BOUND, worst
 
 
+@pytest.mark.parametrize("win,hop", [(2048, 512), (600, 150)])
+def test_parents_and_phases_match_the_heap_at_other_windows(V, win, hop):
+    """λ = 0.25645 win² and the hop enter every phase step: the same kinds of magnitude as the batch above, with the
+    consistent ones taken at this window and hop."""
+    hp = V.AudioParams(win_length=win, hop_length=hop)
+    mags = []
+    for i, n in enumerate([1, 5, 40, 120]):
+        y = utterance(max(1025, hop * (n - 1)), 110 + i, silence=(0, 0))
+        mags += [("consistent", np.abs(ao.stft(y, ao.N_FFT, hop, win))[:n].astype(np.float32)),
+                 ("mel80", mel_inverse(V, n, 80, 120 + i)), ("tied", tied(n, 130 + i)),
+                 ("silent", np.zeros((n, 1025), np.float32))]
+    X, par = V.pghi([dev(s) for _, s in mags], hp, parent=True)
+    worst = 0.0
+    for (kind, s), x, p in zip(mags, X, par):
+        phi, want = ref.pghi_heap(s, hop=hop, win=win)
+        got = p.cpu().numpy()
+        assert np.array_equal(got, want), (kind, s.shape, np.argwhere(got != want)[:5])
+        x = x.cpu().numpy()
+        sig = want != ref.NONE
+        if sig.any():
+            worst = max(worst, float(np.abs(ref.wrap(np.angle(x[sig]) - phi[sig])).max()))
+    print(f"win={win} hop={hop}: max wrapped phase error {worst:.2e} rad")
+    assert worst < PHASE_BOUND, worst
+
+
 def test_batches_are_bitwise_per_utterance_and_run_to_run(V, device_run):
     mags, X, par, X2, par2 = device_run
     for m, x, p, x2, p2 in zip(mags, X, par, X2, par2):
