@@ -140,6 +140,7 @@ STFT_MAG, STFT_COMPLEX, STFT_PROJECT, STFT_PROJECT_FIRST = 0, 1, 2, 3
 MEL_TO_MAG, MAG_TO_MEL = 0, 1
 GL_START_ZERO, GL_START_X, GL_START_PGHI = 0, 1, 2
 PGHI_NONE, PGHI_TIME, PGHI_LEFT, PGHI_RIGHT, PGHI_SEED = 0, 1, 2, 3, 4
+YIN_MAX_SPAN = 3072   # AVC_YIN_MAX_SPAN
 
 
 class AudioSeg(C.Structure):
@@ -319,6 +320,7 @@ PROTOTYPES = {
     "avc_pghi": (_i, [C.POINTER(AudioDesc), C.c_float, _p, _p]),
     "avc_frame_power": (_i, [C.POINTER(AudioDesc), _p, _p]),
     "avc_deemphasis": (_i, [C.POINTER(AudioDesc), C.c_float, _p]),
+    "avc_yin": (_i, [C.POINTER(AudioDesc), C.c_int32, C.c_int32, C.c_int32, C.c_float, _p, _p, _p, _p]),
     "avc_mel_project": (_i, [C.POINTER(MelDesc), _p]),
     "avc_resample_poly": (_i, [C.POINTER(ResampleDesc), _p]),
     "avc_mel_moments": (_i, [C.POINTER(MomentsDesc), _p]),

@@ -1,0 +1,198 @@
+// YIN F0 tracking (de Cheveigne & Kawahara 2002) of a ragged batch of signals: the difference function, its cumulative
+// mean normalisation, the lag choice and the parabolic refinement, in float64.  One CTA per frame, no atomics: a
+// frame's outputs depend on its own samples only, so a signal gets the same bits alone or in any batch.
+#include <climits>
+#include <cmath>
+
+#include "common.cuh"
+
+namespace avc {
+namespace {
+
+constexpr int YIN_LAGS = 8;       // consecutive lags per thread: a register window of 8 samples slides along j
+constexpr int YIN_MAX_THREADS = 256;  // 8 x 192 lags at the span cap
+static_assert(YIN_MAX_THREADS * YIN_LAGS >= AVC_YIN_MAX_SPAN / 2, "a CTA must cover tau_max <= AVC_YIN_MAX_SPAN / 2");
+
+// samples staged per frame: the span W + tau_max and a zero tail that the last thread's window reads past tau_max
+__host__ __device__ inline int yin_staged(int win, int tau_max) { return win + tau_max + YIN_LAGS + 1; }
+
+// Shared-memory slot of sample i: one pad double after every 16, so that the lanes of a warp, 8 lags apart, read 8
+// doubles apart plus one slot per two lanes and hit distinct bank pairs.
+__device__ __forceinline__ int skew(int i) { return i + (i >> 4); }
+
+// index of the last table entry whose frame_off <= f (the table is sorted by frame_off)
+__device__ __forceinline__ int seg_of_frame_yin(const avc_audio_seg* s, int n, int f) {
+  int lo = 0, hi = n - 1;
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if (__ldg(&s[mid].frame_off) <= f) lo = mid; else hi = mid - 1;
+  }
+  return lo;
+}
+
+// sample i of a signal of length L under numpy 'reflect' padding, one reflection (the STFT's and frame power's);
+// clamped so that no index leaves the signal
+__device__ __forceinline__ int reflect1(int i, int L) {
+  if (i < 0) i = -i;
+  if (i >= L) i = 2 * (L - 1) - i;
+  return min(max(i, 0), L - 1);
+}
+
+__device__ __forceinline__ double warp_sum_d(double v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  return v;
+}
+
+// Shared memory: the frame's samples x[0, yin_staged) (skewed, float64; zero past W + tau_max), then dp[0, tau_max].
+// Thread t owns lags tau0 = 1 + 8t .. tau0 + 7 and sums d(tau) = sum_{j<W} (x[j] - x[j+tau])^2 in ascending j with
+// one fma per term; lags past tau_max are computed on the zero tail and dropped.  Warp 0 then computes the energy,
+// the prefix sums of d (a lane per chunk of consecutive lags, a fixed shuffle scan of the chunk totals), d', the lag
+// choice and the refinement.
+__global__ void __launch_bounds__(YIN_MAX_THREADS) yin_kernel(avc_audio_desc d, int win, int tau_min, int tau_max,
+                                                              double theta, double* __restrict__ tau_out,
+                                                              double* __restrict__ ap_out, double* __restrict__ en_out) {
+  extern __shared__ double sm[];
+  const int f = blockIdx.x, t = threadIdx.x, nt = blockDim.x;
+  const int n_stage = yin_staged(win, tau_max);
+  double* xs = sm;
+  double* dp = sm + skew(n_stage) + 1;
+  const avc_audio_seg g = d.segs[seg_of_frame_yin(d.segs, d.n_seg, f)];
+  const int span = win + tau_max, half = span / 2, L = g.n_samples;
+  const int64_t centre = (int64_t)(f - g.frame_off) * d.hop;
+  // one reflection on each side: -half >= -(L-1) and centre + span - half - 1 <= 2 (L-1)
+  if (L < 1 || half > L - 1 || centre + (span - half - 1) > 2 * (int64_t)(L - 1)) {
+    if (t == 0) tau_out[f] = ap_out[f] = en_out[f] = __longlong_as_double(0x7ff8000000000000LL);
+    return;
+  }
+  const float* y = d.y + g.sample_off;
+  const int base = (int)centre - half;
+  for (int i = t; i < n_stage; i += nt) xs[skew(i)] = i < span ? (double)__ldg(y + reflect1(base + i, L)) : 0.0;
+  __syncthreads();
+
+  const int tau0 = 1 + YIN_LAGS * t;
+  if (tau0 <= tau_max) {
+    double acc[YIN_LAGS], w[YIN_LAGS];
+#pragma unroll
+    for (int k = 0; k < YIN_LAGS; ++k) {
+      acc[k] = 0.0;
+      w[k] = xs[skew(tau0 + k)];
+    }
+    // w[(jj + k) & 7] holds x[j + jj + tau0 + k]; after step jj the slot of k = 0 takes x[j + jj + tau0 + 8]
+    int j = 0;
+    for (; j + YIN_LAGS <= win; j += YIN_LAGS) {
+#pragma unroll
+      for (int jj = 0; jj < YIN_LAGS; ++jj) {
+        const double a = xs[skew(j + jj)];
+#pragma unroll
+        for (int k = 0; k < YIN_LAGS; ++k) {
+          const double e = a - w[(jj + k) & (YIN_LAGS - 1)];
+          acc[k] = fma(e, e, acc[k]);
+        }
+        w[jj] = xs[skew(j + jj + tau0 + YIN_LAGS)];
+      }
+    }
+    for (; j < win; ++j) {
+      const double a = xs[skew(j)];
+#pragma unroll
+      for (int k = 0; k < YIN_LAGS; ++k) {
+        const double e = a - xs[skew(j + tau0 + k)];
+        acc[k] = fma(e, e, acc[k]);
+      }
+    }
+#pragma unroll
+    for (int k = 0; k < YIN_LAGS; ++k)
+      if (tau0 + k <= tau_max) dp[tau0 + k] = acc[k];
+  }
+  __syncthreads();
+  if (t >= 32) return;
+
+  // energy = (1/W) sum_{j<W} x[j]^2: lane-strided in ascending j, then a fixed shuffle tree
+  double e = 0.0;
+  for (int i = t; i < win; i += 32) e = fma(xs[skew(i)], xs[skew(i)], e);
+  e = warp_sum_d(e) / (double)win;
+
+  // S(tau) = sum_{k<=tau} d(k): lane l sums lags [1 + l c, (l + 1) c] in order, then adds the lanes before it
+  const int c = (tau_max + 31) / 32;
+  const int lo = 1 + t * c, hi = min(tau_max, (t + 1) * c);
+  double part = 0.0;
+  for (int i = lo; i <= hi; ++i) part += dp[i];
+  double incl = part;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const double v = __shfl_up_sync(0xffffffffu, incl, o);
+    if (t >= o) incl += v;
+  }
+  double run = __shfl_up_sync(0xffffffffu, incl, 1);  // the lanes before this one
+  if (t == 0) run = 0.0;
+  for (int i = lo; i <= hi; ++i) {
+    const double di = dp[i];
+    run += di;
+    dp[i] = run == 0.0 ? 1.0 : di * (double)i / run;
+  }
+  __syncwarp();
+
+  // the smallest tau in [tau_min, tau_max] with d' < theta, and the argmin (smallest tau on ties)
+  int first = INT_MAX, amin = INT_MAX;
+  double vmin = INFINITY;
+  for (int i = tau_min + t; i <= tau_max; i += 32) {
+    const double v = dp[i];
+    if (v < theta && i < first) first = i;
+    if (v < vmin) { vmin = v; amin = i; }
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    first = min(first, __shfl_xor_sync(0xffffffffu, first, o));
+    const double v2 = __shfl_xor_sync(0xffffffffu, vmin, o);
+    const int a2 = __shfl_xor_sync(0xffffffffu, amin, o);
+    if (v2 < vmin || (v2 == vmin && a2 < amin)) { vmin = v2; amin = a2; }
+  }
+  if (t != 0) return;
+  int ts;
+  if (first != INT_MAX) {
+    ts = first;
+    while (ts < tau_max && dp[ts + 1] < dp[ts]) ++ts;
+  } else {
+    ts = amin;  // every d' is finite (d >= 0, S >= d), so the argmin exists
+  }
+  double delta = 0.0;
+  if (ts - 1 >= 1 && ts + 1 <= tau_max) {
+    const double a = dp[ts - 1], b = dp[ts], cc = dp[ts + 1];
+    const double den = a - 2.0 * b + cc;
+    if (den > 0.0) delta = fmin(0.5, fmax(-0.5, (a - cc) / (2.0 * den)));
+  }
+  tau_out[f] = (double)ts + delta;
+  ap_out[f] = dp[ts];
+  en_out[f] = e;
+}
+
+}  // namespace
+}  // namespace avc
+
+using namespace avc;
+
+extern "C" int avc_yin(const avc_audio_desc* d, int32_t win, int32_t tau_min, int32_t tau_max, float threshold,
+                       double* tau, double* aperiodicity, double* energy, void* stream) {
+  AVC_REQUIRE(d != nullptr, AVC_ERR_INVALID, "avc_yin: null descriptor");
+  AVC_REQUIRE(d->segs != nullptr && d->n_seg > 0 && d->n_frames >= 0, AVC_ERR_INVALID,
+              "avc_yin: empty or missing utterance table (n_seg %d, n_frames %d)", d->n_seg, d->n_frames);
+  AVC_REQUIRE(d->y != nullptr, AVC_ERR_INVALID, "avc_yin: null signal y");
+  AVC_REQUIRE(d->hop > 0, AVC_ERR_INVALID, "avc_yin: hop must be positive (got %d)", d->hop);
+  AVC_REQUIRE(tau != nullptr && aperiodicity != nullptr && energy != nullptr, AVC_ERR_INVALID,
+              "avc_yin: null tau, aperiodicity or energy");
+  AVC_REQUIRE(tau_min >= 1 && tau_min < tau_max, AVC_ERR_INVALID,
+              "avc_yin: tau_min / tau_max must satisfy 1 <= tau_min < tau_max (got %d, %d)", tau_min, tau_max);
+  AVC_REQUIRE(win >= tau_max, AVC_ERR_INVALID, "avc_yin: win must be >= tau_max (got win %d, tau_max %d)", win, tau_max);
+  AVC_REQUIRE((int64_t)win + tau_max <= AVC_YIN_MAX_SPAN, AVC_ERR_UNSUPPORTED,
+              "avc_yin: win + tau_max = %lld exceeds AVC_YIN_MAX_SPAN = %d", (long long)win + tau_max, AVC_YIN_MAX_SPAN);
+  AVC_REQUIRE(std::isfinite(threshold) && threshold > 0.f && threshold <= 1.f, AVC_ERR_INVALID,
+              "avc_yin: threshold must be finite and in (0, 1] (got %g)", (double)threshold);
+  if (d->n_frames == 0) return AVC_OK;
+  const int threads = 32 * cdiv(cdiv(tau_max, YIN_LAGS), 32);
+  const size_t smem = sizeof(double) * (size_t)((yin_staged(win, tau_max) + (yin_staged(win, tau_max) >> 4) + 1) +
+                                                 (tau_max + 1));
+  yin_kernel<<<d->n_frames, threads, smem, (cudaStream_t)stream>>>(*d, win, tau_min, tau_max, (double)threshold, tau,
+                                                                   aperiodicity, energy);
+  AVC_CHECK_LAUNCH("avc_yin");
+  return AVC_OK;
+}

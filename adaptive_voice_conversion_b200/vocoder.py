@@ -10,7 +10,8 @@ scipy.signal.resample_poly; librosa used resampy, so such input does not match t
 Every stage function takes a ragged batch, a list of device tensors of different lengths, and converts it with one
 launch per kernel.  No kernel uses atomics, so each utterance gets the bits it gets when converted alone.
 ``Vocoder`` has the duck type ``Inferencer`` accepts (``get_spectrograms(path)``, ``melspectrogram2wav(mel)``, numpy
-in and out) and the batched device forms ``wav_to_mel`` / ``mel_to_wav``.
+in and out) and the batched device forms ``wav_to_mel`` / ``mel_to_wav`` (``mel_to_signal`` leaves the synthesis
+untrimmed, aligned with the mel frames).
 """
 from __future__ import annotations
 
@@ -399,18 +400,22 @@ class Vocoder:
         r = [m.shape[0] for m in mels]
         return list(torch.split(_mel_project(torch.cat(mels), self.m_t, L.MEL_TO_MAG, self.hp), r))
 
-    def mel_to_wav(self, mels, n_iter: int | None = None, momentum: float | None = None, init: str | None = None):
-        """Normalised mels [T, n_mels] (device tensors) -> float32 signals: amplitude, mel-to-linear, Griffin-Lim,
-        de-emphasis, trim (out_top_db).  ``n_iter``, ``momentum`` and ``init`` default to ``hp.n_iter``,
-        ``hp.momentum`` and ``hp.gl_init``."""
+    def mel_to_signal(self, mels, n_iter: int | None = None, momentum: float | None = None, init: str | None = None,
+                      what: str = "mel_to_signal"):
+        """Normalised mels [T, n_mels] (device tensors) -> untrimmed float32 signals of hop * (T - 1) samples, sample
+        f * hop at mel frame f: amplitude, mel-to-linear, Griffin-Lim, de-emphasis.  ``n_iter``, ``momentum`` and
+        ``init`` default to ``hp.n_iter``, ``hp.momentum`` and ``hp.gl_init``."""
         hp = self.hp
         for i, m in enumerate(mels):
             if m.dim() != 2 or m.shape[1] != hp.n_mels:
-                raise ValueError(f"mel_to_wav: utterance {i} has shape {tuple(m.shape)}, expected [T, {hp.n_mels}]")
+                raise ValueError(f"{what}: utterance {i} has shape {tuple(m.shape)}, expected [T, {hp.n_mels}]")
         _init(init, hp)
-        _frames(mels, hp, "mel_to_wav")
-        ys = deemphasis(griffin_lim(self.mel_to_mag(mels), hp, n_iter, momentum, init), hp.preemphasis)
-        return trim(ys, hp.out_top_db)
+        _frames(mels, hp, what)
+        return deemphasis(griffin_lim(self.mel_to_mag(mels), hp, n_iter, momentum, init), hp.preemphasis)
+
+    def mel_to_wav(self, mels, n_iter: int | None = None, momentum: float | None = None, init: str | None = None):
+        """``mel_to_signal`` then trim (out_top_db): the waveform a conversion writes."""
+        return trim(self.mel_to_signal(mels, n_iter, momentum, init, what="mel_to_wav"), self.hp.out_top_db)
 
     def get_spectrograms(self, path):
         """The reference's get_spectrograms(fpath): (mel [T, n_mels], mag [T, n_bins]) float32 numpy."""

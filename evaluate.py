@@ -3,6 +3,7 @@ data directory (adaptive_voice_conversion_b200/evaluate.py gives the definition)
 
     python evaluate.py -c config.yaml -m model.ckpt -d data/ [-eval_sets in_test,out_test] [-o eval.json]
                        [-mcd -transcripts VCTK-Corpus/txt [-attr data/attr.pkl] [-mcd_dims 24]] [-spk]
+                       [-f0 [-gl_iters 100] [-gl_momentum 0] [-gl_init zero]]
                        [-max_pairs 0] [-seed 0] [-n_refs 1] [-bank bank.pt]
 
 The checkpoint is loaded strictly (reference checkpoints too, and the `sn: True` layout).  Each set's losses are
@@ -13,6 +14,15 @@ distortion after DTW between speaker A's utterance converted to speaker B and B'
 mel, and the speaker similarity of conversions to the target speaker's other utterances
 (adaptive_voice_conversion_b200/speaker_eval.py gives the definitions), two more lines per set and a "spk" entry per
 set in -o.
+-f0 measures the pitch of conversions as synthesised: every utterance -spk embeds and every conversion of the -spk
+pairs (the same pairs, the same -seed, -max_pairs and -n_refs) is denormalised with -attr, synthesised by the project's
+Griffin-Lim vocoder untrimmed (-gl_iters, -gl_momentum, -gl_init; defaults 100, 0, zero, as inference.py) and tracked
+by YIN on the GPU (adaptive_voice_conversion_b200/f0.py gives the definitions): vuv_agree (voicing agreement with the
+source's copy-synthesis), f0_corr (Pearson correlation of log2 F0 over the frames voiced in both), st_target and
+st_source (semitones between the conversion's mean log2 F0 and the target's and the source's speaker profile, each
+leaving out the pair's own utterances), f0_success = [st_target < st_source] and st_target_source (the unconverted
+baseline); one more line per set and an "f0" entry per set in -o.  These are F0 measures of this project's Griffin-Lim
+output, not of the original recordings.
 -n_refs K (default 1) converts with K references of the target speaker per conversion, their speaker codes pooled
 (-mcd and -spk): the first reference is drawn as with one, the K - 1 others from a second generator seeded with
 seed + 1; sim_target then skips all K.  With K > 1 each result also reports n_refs and n_few (conversions dropped for
@@ -46,14 +56,21 @@ def main(argv=None):
     p.add_argument("-output", "-o", default=None, help="JSON file for the per-set and per-speaker results")
     p.add_argument("-mcd", action="store_true", help="also measure MCD-DTW of conversions on parallel utterances")
     p.add_argument("-transcripts", default=None, help="directory searched for <id>.txt / <id>.normalized.txt (-mcd)")
-    p.add_argument("-attr", default=None, help="mel statistics (default <data_dir>/attr.pkl) (-mcd)")
+    p.add_argument("-attr", default=None, help="mel statistics (default <data_dir>/attr.pkl) (-mcd, -f0)")
     p.add_argument("-mcd_dims", type=int, default=24, help="cepstral coefficients c_1..c_D (-mcd)")
     p.add_argument("-spk", action="store_true", help="also measure speaker EERs and the speaker similarity of conversions")
+    p.add_argument("-f0", action="store_true", help="also measure the F0 of synthesised conversions (YIN on the GPU)")
+    p.add_argument("-gl_iters", default=100, type=int, help="Griffin-Lim iterations of the synthesis (-f0)")
+    p.add_argument("-gl_momentum", default=0.0, type=float, help="fast Griffin-Lim momentum in [0, 1) (-f0)")
+    p.add_argument("-gl_init", default="zero", choices=["zero", "pghi"], help="Griffin-Lim start phase (-f0)")
     p.add_argument("-max_pairs", type=int, default=0,
-                   help="keep at most this many triplets (-mcd) and conversion pairs (-spk) per set, 0 = all")
-    p.add_argument("-seed", type=int, default=0, help="seed of the reference choice and the sampling (-mcd, -spk)")
+                   help="keep at most this many triplets (-mcd) and conversion pairs (-spk) per set, 0 = all; "
+                        "-f0 scores the -spk pairs")
+    p.add_argument("-seed", type=int, default=0, help="seed of the reference choice and the sampling (-mcd, -spk); "
+                                                      "-f0 as -spk")
     p.add_argument("-n_refs", type=int, default=1,
-                   help="references of the target speaker per conversion, their speaker codes pooled (-mcd, -spk)")
+                   help="references of the target speaker per conversion, their speaker codes pooled (-mcd, -spk); "
+                        "-f0 as -spk")
     p.add_argument("-bank", default=None, help="speaker bank: identify conversions among its speakers (-spk)")
     args = p.parse_args(argv)
     if args.mcd and not args.transcripts:
@@ -62,6 +79,13 @@ def main(argv=None):
         p.error("-bank needs -spk")
     if not 1 <= args.n_refs <= 64:
         p.error("-n_refs must lie in [1, 64]")
+    if args.gl_iters < 0:
+        p.error("-gl_iters must be >= 0")
+    if not 0.0 <= args.gl_momentum < 1.0:
+        p.error("-gl_momentum must lie in [0, 1)")
+    attr_path = args.attr or os.path.join(args.data_dir, "attr.pkl")
+    if args.f0 and not os.path.isfile(attr_path):
+        p.error(f"-f0 needs the mel statistics: {attr_path} does not exist (pass -attr)")
     few = {} if args.n_refs == 1 else {"n_refs": args.n_refs}
     config = load_config(args.config)
     dev = local_device()
@@ -74,7 +98,7 @@ def main(argv=None):
         print(f"{s}: n={r['n']} loss_rec={r['loss_rec']:.6f} loss_kl={r['loss_kl']:.6f} ({len(r['speakers'])} speakers)")
     if args.mcd:
         from adaptive_voice_conversion_b200.mcd import evaluate_mcd, read_transcripts
-        with open(args.attr or os.path.join(args.data_dir, "attr.pkl"), "rb") as f:
+        with open(attr_path, "rb") as f:
             attr = pickle.load(f)
         for s in res:
             with open(os.path.join(args.data_dir, f"{s}.pkl"), "rb") as f:
@@ -109,6 +133,23 @@ def main(argv=None):
                 ids = " ".join(f"{k}=" + ("n/a" if c[k] is None else f"{c[k]:.4f}") for k in ("id_target", "id_source", "id_real"))
                 print(f"{s}: spk bank {ids} n_banked={c['n_banked']} n_unbanked={c['n_unbanked']} "
                       f"({c['bank_speakers']} banked speakers)")
+    if args.f0:
+        from adaptive_voice_conversion_b200.f0 import evaluate_f0
+        from adaptive_voice_conversion_b200.vocoder import AudioParams
+        with open(attr_path, "rb") as f:
+            attr = pickle.load(f)
+        hp = AudioParams(n_iter=args.gl_iters, momentum=args.gl_momentum, gl_init=args.gl_init)
+        for s in res:
+            with open(os.path.join(args.data_dir, f"{s}.pkl"), "rb") as f:
+                data = pickle.load(f)
+            r = evaluate_f0(model, data, attr, seed=args.seed, max_pairs=args.max_pairs, device=dev, hp=hp, **few)
+            res[s]["f0"] = r
+            means = (f" vuv_agree={r['vuv_agree']:.4f} f0_corr={r['f0_corr']:.4f} st_target={r['st_target']:.4f} "
+                     f"st_source={r['st_source']:.4f} f0_success={r['f0_success']:.4f} "
+                     f"st_target_source={r['st_target_source']:.4f}") if r["n"] else ""
+            means += f" n_refs={r['n_refs']} n_few={r['n_few']}" if few else ""
+            print(f"{s}: f0 n={r['n']} n_short={r['n_short']} n_unvoiced={r['n_unvoiced']}{means} "
+                  f"({len(r['speakers'])} target speakers)")
     if args.output:
         with open(args.output, "w") as f:
             json.dump(res, f, indent=1)

@@ -632,6 +632,25 @@ int avc_frame_power(const avc_audio_desc* d, float* power, void* stream);
  * scan, one CTA per utterance.  Reads segs, n_seg, y. */
 int avc_deemphasis(const avc_audio_desc* d, float coef, void* stream);
 
+/* YIN F0 tracking (de Cheveigne & Kawahara 2002) of every signal of the table (csrc/pitch.cu), float64.  Frame f of a
+ * signal of L samples (segs frame_off / n_frames count them; 1 + L / hop when they come from a vocoder signal) is
+ * x[j] = y[reflect(f hop - floor((win + tau_max) / 2) + j)], j < win + tau_max, with avc_frame_power's one reflection.
+ *   d(tau)  = sum_{j < win} (x[j] - x[j + tau])^2, tau = 1..tau_max (each term one fma, ascending j)
+ *   d'(tau) = d(tau) tau / sum_{k = 1..tau} d(k), and 1 where that sum is 0
+ *   tau*    = the smallest tau in [tau_min, tau_max] with d'(tau) < threshold, then the descent while
+ *             d'(tau + 1) < d'(tau) and tau < tau_max; without one, the argmin of d' there (smallest tau on ties)
+ *   delta   = (a - c) / (2 (a - 2b + c)) with a, b, c = d'(tau* - 1), d'(tau*), d'(tau* + 1) when tau* - 1 >= 1,
+ *             tau* + 1 <= tau_max and the denominator is > 0, else 0; clamped to [-1/2, 1/2]
+ *   tau[f] = tau* + delta, aperiodicity[f] = d'(tau*), energy[f] = (1/win) sum_{j < win} x[j]^2 (all float64 [n_frames])
+ * One CTA per frame, no atomics: a signal gets the same bits in any batch.  Reads segs, n_seg, n_frames, hop and y.
+ * The length check is the caller's, as the table is device memory: a frame that would need a second reflection
+ * (L < ceil((win + tau_max) / 2) + 1 for the frames above) gets NaN in all three outputs.  AVC_ERR_INVALID before any
+ * launch for a null pointer, n_seg < 1, hop < 1, tau_min < 1, tau_min >= tau_max, win < tau_max, or a threshold that
+ * is not finite or not in (0, 1]; AVC_ERR_UNSUPPORTED for win + tau_max > AVC_YIN_MAX_SPAN. */
+#define AVC_YIN_MAX_SPAN 3072
+int avc_yin(const avc_audio_desc* d, int32_t win, int32_t tau_min, int32_t tau_max, float threshold, double* tau,
+            double* aperiodicity, double* energy, void* stream);
+
 /* Mel projections of the concatenated frames of a ragged batch (rows are independent).
  *   AVC_MEL_TO_MAG: out[rows][n_bins] = A x mat, A = 10^((clip(in,0,1) max_db - max_db + ref_db) / 20),
  *                   in [rows][n_mels], mat [n_mels][n_bins] (the transposed mel-to-linear matrix)
