@@ -166,6 +166,81 @@ __global__ void __launch_bounds__(YIN_MAX_THREADS) yin_kernel(avc_audio_desc d, 
   en_out[f] = e;
 }
 
+// ---------------------------------------------------------------------------------------------- spectral pitch shift
+constexpr int PS_BINS = 1025;                  // n_fft 2048
+constexpr int PS_N1 = PS_BINS - 1;             // the cosines' period is 2 PS_N1 in q k
+constexpr int PS_TAB = 2 * PS_N1;
+constexpr int PS_THREADS = 256;
+constexpr int PS_PER_THREAD = (PS_BINS + PS_THREADS - 1) / PS_THREADS;
+constexpr int PS_MAX_CTAS = 1024;              // CTAs loop over rows, so each builds its cosine table once
+
+// Table slot of cos(pi m / PS_N1): one pad float after every 32, so that lanes whose q k step by a power of two up to
+// 32 spread over several banks.
+__device__ __forceinline__ int ps_slot(int m) { return m + (m >> 5); }
+
+__device__ __forceinline__ float warp_sum_f(float v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  return v;
+}
+
+// One row at a time per CTA.  ls holds l = ln max(S, 1e-5), then F = l - E in place; cs the Q cepstral coefficients.
+// Warp w sums c[q] for q = w, w + 8, ...: lane j takes k = 1 + j + 32 i in ascending i, then a fixed shuffle tree.
+// Thread t owns bins t + 256 i: E is a sequential sum over q, the interpolation reads F after a barrier.
+__global__ void __launch_bounds__(PS_THREADS) pitch_shift_kernel(const float* __restrict__ mag,
+                                                                 const float* __restrict__ ratio,
+                                                                 float* __restrict__ out, int rows, int lifter) {
+  __shared__ float tab[PS_TAB + PS_TAB / 32];
+  __shared__ float ls[PS_BINS];
+  __shared__ float cs[PS_N1];
+  const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
+  for (int m = t; m < PS_TAB; m += PS_THREADS) tab[ps_slot(m)] = cospif((float)m / (float)PS_N1);
+  for (int row = blockIdx.x; row < rows; row += gridDim.x) {
+    const float a = __ldg(ratio + row);
+    const float* S = mag + (size_t)row * PS_BINS;
+    float* o = out + (size_t)row * PS_BINS;
+    if (a == 1.0f) {
+      for (int k = t; k < PS_BINS; k += PS_THREADS) o[k] = __ldg(S + k);
+      continue;
+    }
+    if (!(a > 0.f) || isinf(a)) {
+      for (int k = t; k < PS_BINS; k += PS_THREADS) o[k] = __int_as_float(0x7fc00000);
+      continue;
+    }
+    __syncthreads();  // the previous row's readers of ls and cs are done; the table is written
+    for (int k = t; k < PS_BINS; k += PS_THREADS) ls[k] = logf(fmaxf(__ldg(S + k), 1e-5f));
+    __syncthreads();
+    for (int q = warp; q < lifter; q += PS_THREADS / 32) {
+      float s = 0.f;
+      for (int k = 1 + lane; k < PS_N1; k += 32) s = fmaf(ls[k], tab[ps_slot((q * k) & (PS_TAB - 1))], s);
+      s = warp_sum_f(s);
+      if (lane == 0) cs[q] = (ls[0] + ((q & 1) ? -ls[PS_N1] : ls[PS_N1]) + 2.f * s) / (float)PS_TAB;
+    }
+    __syncthreads();
+    float e[PS_PER_THREAD];
+#pragma unroll
+    for (int i = 0; i < PS_PER_THREAD; ++i) {
+      const int k = t + PS_THREADS * i;
+      if (k >= PS_BINS) break;
+      float acc = 0.f;
+      for (int q = 1; q < lifter; ++q) acc = fmaf(cs[q], tab[ps_slot((q * k) & (PS_TAB - 1))], acc);
+      e[i] = cs[0] + 2.f * acc;
+      ls[k] -= e[i];  // each bin is read and written by its own thread only until the barrier
+    }
+    __syncthreads();
+#pragma unroll
+    for (int i = 0; i < PS_PER_THREAD; ++i) {
+      const int k = t + PS_THREADS * i;
+      if (k >= PS_BINS) break;
+      const float p = fminf((float)k / a, (float)PS_N1);  // correctly rounded: the restatement uses the same position
+      const int i0 = (int)p;
+      const float fr = p - (float)i0;                       // exact
+      const float fl = i0 < PS_N1 ? fmaf(fr, ls[i0 + 1] - ls[i0], ls[i0]) : ls[PS_N1];
+      o[k] = expf(e[i] + fl);
+    }
+  }
+}
+
 }  // namespace
 }  // namespace avc
 
@@ -194,5 +269,23 @@ extern "C" int avc_yin(const avc_audio_desc* d, int32_t win, int32_t tau_min, in
   yin_kernel<<<d->n_frames, threads, smem, (cudaStream_t)stream>>>(*d, win, tau_min, tau_max, (double)threshold, tau,
                                                                    aperiodicity, energy);
   AVC_CHECK_LAUNCH("avc_yin");
+  return AVC_OK;
+}
+
+extern "C" int avc_pitch_shift(const float* mag, const float* ratio, float* out, int32_t rows, int32_t n_bins,
+                               int32_t lifter, void* stream) {
+  AVC_REQUIRE(mag != nullptr && ratio != nullptr && out != nullptr, AVC_ERR_INVALID,
+              "avc_pitch_shift: null mag, ratio or out");
+  AVC_REQUIRE(rows >= 1, AVC_ERR_INVALID, "avc_pitch_shift: rows must be >= 1 (got %d)", rows);
+  AVC_REQUIRE(lifter >= 1 && lifter <= n_bins - 1, AVC_ERR_INVALID,
+              "avc_pitch_shift: lifter must lie in [1, n_bins - 1] (got %d, n_bins %d)", lifter, n_bins);
+  AVC_REQUIRE(n_bins == PS_BINS, AVC_ERR_UNSUPPORTED, "avc_pitch_shift: n_bins must be %d (n_fft 2048), got %d",
+              PS_BINS, n_bins);
+  const size_t bytes = sizeof(float) * (size_t)rows * PS_BINS;
+  const char *m0 = (const char*)mag, *o0 = (const char*)out;
+  AVC_REQUIRE(o0 + bytes <= m0 || m0 + bytes <= o0, AVC_ERR_INVALID, "avc_pitch_shift: out overlaps mag");
+  pitch_shift_kernel<<<rows < PS_MAX_CTAS ? rows : PS_MAX_CTAS, PS_THREADS, 0, (cudaStream_t)stream>>>(mag, ratio, out,
+                                                                                                       rows, lifter);
+  AVC_CHECK_LAUNCH("avc_pitch_shift");
   return AVC_OK;
 }

@@ -54,7 +54,7 @@ import torch
 
 from . import _lib as L
 from .evaluate import speaker_of
-from .vocoder import AudioParams, Vocoder, _Ragged
+from .vocoder import PITCH_SHIFT_MAX, AudioParams, Vocoder, _Ragged
 
 METRICS = ("vuv_agree", "f0_corr", "st_target", "st_source", "f0_success", "st_target_source")
 
@@ -186,19 +186,23 @@ def _means(rows: np.ndarray) -> dict:
     return out
 
 
-def synthesize(vocoder: Vocoder, mels, hp: AudioParams, frame_budget: int = 32768):
-    """mel_to_signal of each (denormalised) mel, in chunks of at most frame_budget frames (one longer mel alone)."""
-    out, chunk, frames = [], [], 0
+def synthesize(vocoder: Vocoder, mels, hp: AudioParams, frame_budget: int = 32768, semitones=None):
+    """mel_to_signal of each (denormalised) mel, in chunks of at most frame_budget frames (one longer mel alone);
+    semitones (one per mel) shifts them, default hp.pitch_shift."""
+    out, chunk, shifts, frames = [], [], [], 0
+    semitones = [hp.pitch_shift] * len(mels) if semitones is None else list(semitones)
 
     def flush():
         if chunk:
-            out.extend(vocoder.mel_to_signal(chunk, hp.n_iter, hp.momentum, hp.gl_init))
+            out.extend(vocoder.mel_to_signal(chunk, hp.n_iter, hp.momentum, hp.gl_init, semitones=list(shifts)))
             chunk.clear()
-    for m in mels:
+            shifts.clear()
+    for m, st in zip(mels, semitones):
         if chunk and frames + int(m.shape[0]) > frame_budget:
             flush()
             frames = 0
         chunk.append(m)
+        shifts.append(st)
         frames += int(m.shape[0])
     flush()
     return out
@@ -219,6 +223,44 @@ def track_chunks(signals, sr: int, hop: int, params: F0Params, frame_budget: int
     return out
 
 
+# ------------------------------------------------------------------ matching the target's pitch level
+def shifts_from_tracks(conv_tracks, ref_track_sets, limit: float = PITCH_SHIFT_MAX):
+    """(shifts, info) from tracks ((f0, voiced) per signal): conversion i's shift is 12 (mu_refs - mu_conv), each mu
+    the mean log2 F0 over voiced frames (``profile``: the references' voiced frames pooled), clamped to +-limit; 0 and
+    unmatched when either side has no voiced frame.  info[i] = {"shift", "voiced_conv", "voiced_refs", "clamped",
+    "unmatched"}."""
+    shifts, info = [], []
+    for (fc, vc), refs in zip(conv_tracks, ref_track_sets):
+        mc, _, nc = profile([np.log2(fc[vc])])
+        mr, _, nr = profile([np.log2(f[v]) for f, v in refs])
+        unmatched = mc is None or mr is None
+        st = 0.0 if unmatched else 12.0 * (mr - mc)
+        clamped = abs(st) > limit
+        st = float(min(limit, max(-limit, st)))
+        shifts.append(st)
+        info.append({"shift": st, "voiced_conv": int(nc), "voiced_refs": int(nr), "clamped": bool(clamped),
+                     "unmatched": bool(unmatched)})
+    return shifts, info
+
+
+def match_shifts(vocoder: Vocoder, conv_mels, ref_sets, hp: AudioParams, params: F0Params = F0Params(),
+                 frame_budget: int = 32768):
+    """Shifts (semitones) that move each conversion's mean log2 F0 to its reference set's: conv_mels [T, n_mels] and
+    ref_sets (lists of [T, n_mels]) denormalised mels on the device.  Both sides are synthesised unshifted by
+    mel_to_signal at hp's Griffin-Lim settings (in synthesize's chunks) and tracked with the same tracker, as
+    evaluate_f0 does, so both carry the same vocoder artefacts; ``shifts_from_tracks`` gives (shifts, info)."""
+    if len(conv_mels) != len(ref_sets):
+        raise ValueError("match_shifts: one reference set per conversion")
+    flat = [r for rs in ref_sets for r in rs]
+    signals = synthesize(vocoder, list(conv_mels) + flat, hp, frame_budget, semitones=[0.0] * (len(conv_mels) + len(flat)))
+    tracks = track_chunks(signals, hp.sr, hp.hop_length, params)
+    refs, k = [], len(conv_mels)
+    for rs in ref_sets:
+        refs.append(tracks[k:k + len(rs)])
+        k += len(rs)
+    return shifts_from_tracks(tracks[:len(conv_mels)], refs)
+
+
 def select_pairs(cfg, lengths: Mapping[str, int], seed: int = 0, max_pairs: int = 0, n_refs: int = 1):
     """(embedded utterances, [(source, reference)], [[reference, ...]] per pair, {"n", "n_short"[, "n_refs",
     "n_few"]}): the utterances and pairs evaluate_speakers uses for the same arguments (lengths[u] = frames of u)."""
@@ -237,16 +279,25 @@ def select_pairs(cfg, lengths: Mapping[str, int], seed: int = 0, max_pairs: int 
 
 def evaluate_f0(model, data: Mapping[str, np.ndarray], attr, seed: int = 0, max_pairs: int = 0, device=None,
                 per_pair: bool = False, n_refs: int = 1, hp: AudioParams = AudioParams(),
-                params: F0Params = F0Params(), frame_budget: int = 32768, timings: dict = None) -> dict:
+                params: F0Params = F0Params(), frame_budget: int = 32768, timings: dict = None,
+                pitch_shift: str | None = None) -> dict:
     """F0 measures of `model` (an AE) on one set: data = {utterance key: attr-normalised [T, n_mels]} (the set's
     pickle), attr its mel statistics.  hp gives the Griffin-Lim settings (n_iter, momentum, gl_init; n_mels is the
-    model's c_in).  Returns the module docstring's set entry; per_pair adds "pairs": [[source, reference(s), the six
+    model's c_in; its pitch_shift is not used).  Returns the module docstring's set entry; per_pair adds "pairs": [[source, reference(s), the six
     values], ...] for the scored pairs.  timings (a dict) receives the wall seconds of conversion, synthesis, tracking
-    and host work, each ended by a device synchronise."""
+    and host work, each ended by a device synchronise.
+
+    pitch_shift="match" shifts each conversion toward its reference(s) (``shifts_from_tracks`` on the unshifted
+    tracks this call computes anyway), re-synthesises and re-tracks it and scores it against the same leave-out
+    profiles; the entry then holds the shifted scores, "pitch_shift": {"mode", "mean_semitones",
+    "mean_abs_semitones", "n_unmatched", "n_clamped"} over the pairs, and "unshifted": the entry of the call without
+    it."""
     import time
     from .mcd import converted
     from .speaker_eval import SPK_MAX_EXCLUDE
     cfg = model.config
+    if pitch_shift not in (None, "match"):
+        raise ValueError(f"evaluate_f0: pitch_shift must be None or 'match' (got {pitch_shift!r})")
     if int(cfg["data_loader"]["frame_size"]) != 1:
         raise ValueError(f"F0 evaluation supports data_loader.frame_size 1 only (got {cfg['data_loader']['frame_size']})")
     if not 1 <= int(n_refs) <= SPK_MAX_EXCLUDE:
@@ -266,7 +317,7 @@ def evaluate_f0(model, data: Mapping[str, np.ndarray], attr, seed: int = 0, max_
     used = sorted(set(utts) | {u for u, _ in pairs} | {v for rs in refs for v in rs})
     mels = {u: torch.from_numpy(np.ascontiguousarray(data[u], np.float32)).to(dev) for u in used}
     n_mels = int(cfg["SpeakerEncoder"]["c_in"])
-    hp = replace(hp, n_mels=n_mels)
+    hp = replace(hp, n_mels=n_mels, pitch_shift=0.0)
     res["tracker"] = params.settings(hp.sr, hp.hop_length)
     res["griffin_lim"] = {"n_iter": int(hp.n_iter), "momentum": float(hp.momentum), "init": hp.gl_init}
     mean = torch.as_tensor(np.asarray(attr["mean"], np.float32).reshape(-1)).to(dev)
@@ -290,8 +341,8 @@ def evaluate_f0(model, data: Mapping[str, np.ndarray], attr, seed: int = 0, max_
         model.train(was_training)
     lap("conversion")
     vocoder = Vocoder(hp=hp, device=dev)
-    signals = synthesize(vocoder, [mels[u] * std + mean for u in utts] + [c * std + mean for c in convs], hp,
-                         frame_budget)
+    conv_mels = [c * std + mean for c in convs]
+    signals = synthesize(vocoder, [mels[u] * std + mean for u in utts] + conv_mels, hp, frame_budget)
     lap("synthesis")
     tracks = track_chunks(signals, hp.sr, hp.hop_length, params)
     lap("tracking")
@@ -305,31 +356,58 @@ def evaluate_f0(model, data: Mapping[str, np.ndarray], attr, seed: int = 0, max_
     def profile_mean(spk, exclude):
         return profile([logs[v] for v in by_speaker.get(spk, []) if v not in exclude])[0]
 
-    rows, kept = [], []
-    for i, ((u, _), rs) in enumerate(zip(pairs, refs)):
-        v = pair_scores(conv_tracks[i], real[u], profile_mean(speaker_of(rs[0]), set(rs)),
-                        profile_mean(speaker_of(u), {u}))
-        if v is None:
-            res["n_unvoiced"] += 1
-        else:
-            rows.append(v)
-            kept.append(i)
-    vals = np.asarray(rows, np.float64).reshape(-1, len(METRICS))
-    res["n"] = len(rows)
-    if rows:
-        res.update({k: v for k, v in _means(vals).items() if k != "n"})
-    groups: Dict[str, List[int]] = {}
-    for j, i in enumerate(kept):
-        groups.setdefault(speaker_of(refs[i][0]), []).append(j)
-    res["speakers"] = {s: _means(vals[js]) for s, js in groups.items()}
-    res["profiles"] = {}
-    for s, us in by_speaker.items():
-        m, sd, nv = profile([logs[u] for u in us])
-        res["profiles"][s] = {"log2_mean": m, "log2_std": sd, "voiced": nv, "frames": sum(len(real[u][1]) for u in us)}
-    if per_pair:
-        res["pairs"] = [[pairs[i][0], refs[i] if n_refs > 1 else refs[i][0]] + [float(x) for x in vals[j]]
-                        for j, i in enumerate(kept)]
+    def score(res, conv_tracks):
+        rows, kept = [], []
+        for i, ((u, _), rs) in enumerate(zip(pairs, refs)):
+            v = pair_scores(conv_tracks[i], real[u], profile_mean(speaker_of(rs[0]), set(rs)),
+                            profile_mean(speaker_of(u), {u}))
+            if v is None:
+                res["n_unvoiced"] += 1
+            else:
+                rows.append(v)
+                kept.append(i)
+        vals = np.asarray(rows, np.float64).reshape(-1, len(METRICS))
+        res["n"] = len(rows)
+        if rows:
+            res.update({k: v for k, v in _means(vals).items() if k != "n"})
+        groups: Dict[str, List[int]] = {}
+        for j, i in enumerate(kept):
+            groups.setdefault(speaker_of(refs[i][0]), []).append(j)
+        res["speakers"] = {s: _means(vals[js]) for s, js in groups.items()}
+        res["profiles"] = {}
+        for s, us in by_speaker.items():
+            m, sd, nv = profile([logs[u] for u in us])
+            res["profiles"][s] = {"log2_mean": m, "log2_std": sd, "voiced": nv,
+                                  "frames": sum(len(real[u][1]) for u in us)}
+        if per_pair:
+            res["pairs"] = [[pairs[i][0], refs[i] if n_refs > 1 else refs[i][0]] + [float(x) for x in vals[j]]
+                            for j, i in enumerate(kept)]
+        return res
+
+    base = dict(res)
+    res = score(res, conv_tracks)
     lap("host")
+    if pitch_shift == "match":
+        # the references' copy-syntheses are the tracks above; a reference too short to be embedded is tracked here
+        extra = sorted({v for rs in refs for v in rs} - set(real))
+        if extra:
+            sig = synthesize(vocoder, [mels[v] * std + mean for v in extra], hp, frame_budget)
+            lap("synthesis")
+            real.update(zip(extra, track_chunks(sig, hp.sr, hp.hop_length, params)))
+            lap("tracking")
+        shifts, info = shifts_from_tracks(conv_tracks, [[real[v] for v in rs] for rs in refs])
+        sig = synthesize(vocoder, conv_mels, hp, frame_budget, semitones=shifts)
+        lap("synthesis")
+        shifted = track_chunks(sig, hp.sr, hp.hop_length, params)
+        lap("tracking")
+        unshifted, res = res, score(base, shifted)
+        n = max(len(shifts), 1)
+        res["pitch_shift"] = {"mode": "match", "mean_semitones": _seq_sum(np.asarray(shifts, np.float64)) / n,
+                              "mean_abs_semitones": _seq_sum(np.abs(np.asarray(shifts, np.float64))) / n,
+                              "n_unmatched": sum(d["unmatched"] for d in info),
+                              "n_clamped": sum(d["clamped"] for d in info)}
+        res["unshifted"] = unshifted
+        lap("host")
     if timings is not None:
         timings.update(clock)
     return res

@@ -11,7 +11,8 @@ Every stage function takes a ragged batch, a list of device tensors of different
 launch per kernel.  No kernel uses atomics, so each utterance gets the bits it gets when converted alone.
 ``Vocoder`` has the duck type ``Inferencer`` accepts (``get_spectrograms(path)``, ``melspectrogram2wav(mel)``, numpy
 in and out) and the batched device forms ``wav_to_mel`` / ``mel_to_wav`` (``mel_to_signal`` leaves the synthesis
-untrimmed, aligned with the mel frames).
+untrimmed, aligned with the mel frames).  ``pitch_shift`` transposes the linear magnitudes before Griffin-Lim
+(``AudioParams.pitch_shift`` or ``semitones=``), keeping the frame grid.
 """
 from __future__ import annotations
 
@@ -40,6 +41,8 @@ class AudioParams:
     momentum: float = 0.0      # fast Griffin-Lim momentum in [0, 1); 0 is the reference's plain Griffin-Lim
     gl_init: str = "zero"      # Griffin-Lim start phase: "zero" (the reference's) or "pghi" (phase-gradient estimate)
     pghi_tol: float = 1e-5     # PGHI significance threshold relative to an utterance's largest magnitude (not tuned)
+    pitch_shift: float = 0.0   # semitones in [-24, 24] applied to the synthesis (formant-preserving, ``pitch_shift``)
+    ps_lifter: int = 40        # cepstral lifter of the shift's envelope: not tuned, below the 48-sample period of 500 Hz
     preemphasis: float = 0.97
     max_db: float = 100.0
     ref_db: float = 20.0
@@ -369,6 +372,42 @@ def _mel_project(x, mat, direction, hp: AudioParams):
     return out
 
 
+PITCH_SHIFT_MAX = 24.0   # semitones: two octaves either way
+
+
+def _semitones(semitones, n: int, what: str) -> list:
+    """Per-utterance shifts of a float or one value per utterance; ValueError outside [-24, 24] or not finite."""
+    s = [float(semitones)] * n if np.ndim(semitones) == 0 else [float(v) for v in semitones]
+    if len(s) != n:
+        raise ValueError(f"{what}: {len(s)} shifts for {n} utterances")
+    for i, v in enumerate(s):
+        if not np.isfinite(v) or abs(v) > PITCH_SHIFT_MAX:
+            raise ValueError(f"{what}: utterance {i}: pitch shift must be finite and in [-{PITCH_SHIFT_MAX:g}, "
+                             f"{PITCH_SHIFT_MAX:g}] semitones (got {v})")
+    return s
+
+
+def pitch_shift(mags, semitones, hp: AudioParams = AudioParams()):
+    """Formant-preserving pitch shift of linear magnitudes [T, n_bins] per utterance by ``semitones`` (a float, or one
+    per utterance), in one avc_pitch_shift launch: the harmonics (the cepstrum above ``hp.ps_lifter``) move by the
+    ratio 2^(s/12), the envelope stays, the frame grid and duration are unchanged.  An utterance with shift 0 is
+    copied bit for bit."""
+    if not mags:
+        raise ValueError("pitch_shift: empty batch")
+    s = _semitones(semitones, len(mags), "pitch_shift")
+    dev = mags[0].device
+    S = torch.cat([m.float() for m in mags]).contiguous()
+    if S.dim() != 2 or S.shape[1] != hp.n_bins:
+        raise ValueError(f"pitch_shift: magnitudes have shape {tuple(S.shape)}, n_fft={hp.n_fft} gives {hp.n_bins} bins")
+    lens = [int(m.shape[0]) for m in mags]
+    ratio = torch.tensor([2.0 ** (v / 12.0) for v in s], dtype=torch.float32).to(dev)
+    ratio = torch.repeat_interleave(ratio, torch.tensor(lens).to(dev), output_size=S.shape[0])
+    out = torch.empty_like(S)
+    L.check(L.load().avc_pitch_shift(_ptr(S), _ptr(ratio), _ptr(out), S.shape[0], hp.n_bins, int(hp.ps_lifter),
+                                     _stream(dev)), "avc_pitch_shift")
+    return list(torch.split(out, lens))
+
+
 # ------------------------------------------------------------------ the vocoder
 class Vocoder:
     """The reference's get_spectrograms / melspectrogram2wav on the GPU.  The filterbank and its pseudo-inverse are
@@ -401,21 +440,28 @@ class Vocoder:
         return list(torch.split(_mel_project(torch.cat(mels), self.m_t, L.MEL_TO_MAG, self.hp), r))
 
     def mel_to_signal(self, mels, n_iter: int | None = None, momentum: float | None = None, init: str | None = None,
-                      what: str = "mel_to_signal"):
+                      what: str = "mel_to_signal", *, semitones=None):
         """Normalised mels [T, n_mels] (device tensors) -> untrimmed float32 signals of hop * (T - 1) samples, sample
-        f * hop at mel frame f: amplitude, mel-to-linear, Griffin-Lim, de-emphasis.  ``n_iter``, ``momentum`` and
-        ``init`` default to ``hp.n_iter``, ``hp.momentum`` and ``hp.gl_init``."""
+        f * hop at mel frame f: amplitude, mel-to-linear, pitch shift, Griffin-Lim, de-emphasis.  ``n_iter``,
+        ``momentum``, ``init`` and ``semitones`` (a float or one per utterance) default to ``hp.n_iter``,
+        ``hp.momentum``, ``hp.gl_init`` and ``hp.pitch_shift``.  With every shift 0 no shift is launched."""
         hp = self.hp
         for i, m in enumerate(mels):
             if m.dim() != 2 or m.shape[1] != hp.n_mels:
                 raise ValueError(f"{what}: utterance {i} has shape {tuple(m.shape)}, expected [T, {hp.n_mels}]")
         _init(init, hp)
         _frames(mels, hp, what)
-        return deemphasis(griffin_lim(self.mel_to_mag(mels), hp, n_iter, momentum, init), hp.preemphasis)
+        s = _semitones(hp.pitch_shift if semitones is None else semitones, len(mels), what)
+        mags = self.mel_to_mag(mels)
+        if any(v != 0.0 for v in s):
+            mags = pitch_shift(mags, s, hp)
+        return deemphasis(griffin_lim(mags, hp, n_iter, momentum, init), hp.preemphasis)
 
-    def mel_to_wav(self, mels, n_iter: int | None = None, momentum: float | None = None, init: str | None = None):
+    def mel_to_wav(self, mels, n_iter: int | None = None, momentum: float | None = None, init: str | None = None, *,
+                   semitones=None):
         """``mel_to_signal`` then trim (out_top_db): the waveform a conversion writes."""
-        return trim(self.mel_to_signal(mels, n_iter, momentum, init, what="mel_to_wav"), self.hp.out_top_db)
+        return trim(self.mel_to_signal(mels, n_iter, momentum, init, what="mel_to_wav", semitones=semitones),
+                    self.hp.out_top_db)
 
     def get_spectrograms(self, path):
         """The reference's get_spectrograms(fpath): (mel [T, n_mels], mag [T, n_bins]) float32 numpy."""

@@ -3,7 +3,7 @@ data directory (adaptive_voice_conversion_b200/evaluate.py gives the definition)
 
     python evaluate.py -c config.yaml -m model.ckpt -d data/ [-eval_sets in_test,out_test] [-o eval.json]
                        [-mcd -transcripts VCTK-Corpus/txt [-attr data/attr.pkl] [-mcd_dims 24]] [-spk]
-                       [-f0 [-gl_iters 100] [-gl_momentum 0] [-gl_init zero]]
+                       [-f0 [-gl_iters 100] [-gl_momentum 0] [-gl_init zero] [-pitch_shift match]]
                        [-max_pairs 0] [-seed 0] [-n_refs 1] [-bank bank.pt]
 
 The checkpoint is loaded strictly (reference checkpoints too, and the `sn: True` layout).  Each set's losses are
@@ -23,6 +23,9 @@ st_source (semitones between the conversion's mean log2 F0 and the target's and 
 leaving out the pair's own utterances), f0_success = [st_target < st_source] and st_target_source (the unconverted
 baseline); one more line per set and an "f0" entry per set in -o.  These are F0 measures of this project's Griffin-Lim
 output, not of the original recordings.
+-pitch_shift match (with -f0) also shifts each conversion toward its reference(s)' mean log2 F0 (f0.match_shifts),
+re-synthesises and re-scores it against the same leave-out profiles: the "f0" entry then holds the shifted scores,
+"pitch_shift" (mean and mean absolute shift, unmatched and clamped pairs) and "unshifted", the scores without it.
 -n_refs K (default 1) converts with K references of the target speaker per conversion, their speaker codes pooled
 (-mcd and -spk): the first reference is drawn as with one, the K - 1 others from a second generator seeded with
 seed + 1; sim_target then skips all K.  With K > 1 each result also reports n_refs and n_few (conversions dropped for
@@ -63,6 +66,8 @@ def main(argv=None):
     p.add_argument("-gl_iters", default=100, type=int, help="Griffin-Lim iterations of the synthesis (-f0)")
     p.add_argument("-gl_momentum", default=0.0, type=float, help="fast Griffin-Lim momentum in [0, 1) (-f0)")
     p.add_argument("-gl_init", default="zero", choices=["zero", "pghi"], help="Griffin-Lim start phase (-f0)")
+    p.add_argument("-pitch_shift", default=None, choices=["match"],
+                   help="also score each conversion shifted to its reference(s)' pitch level (-f0)")
     p.add_argument("-max_pairs", type=int, default=0,
                    help="keep at most this many triplets (-mcd) and conversion pairs (-spk) per set, 0 = all; "
                         "-f0 scores the -spk pairs")
@@ -83,6 +88,8 @@ def main(argv=None):
         p.error("-gl_iters must be >= 0")
     if not 0.0 <= args.gl_momentum < 1.0:
         p.error("-gl_momentum must lie in [0, 1)")
+    if args.pitch_shift and not args.f0:
+        p.error("-pitch_shift needs -f0")
     attr_path = args.attr or os.path.join(args.data_dir, "attr.pkl")
     if args.f0 and not os.path.isfile(attr_path):
         p.error(f"-f0 needs the mel statistics: {attr_path} does not exist (pass -attr)")
@@ -142,7 +149,8 @@ def main(argv=None):
         for s in res:
             with open(os.path.join(args.data_dir, f"{s}.pkl"), "rb") as f:
                 data = pickle.load(f)
-            r = evaluate_f0(model, data, attr, seed=args.seed, max_pairs=args.max_pairs, device=dev, hp=hp, **few)
+            r = evaluate_f0(model, data, attr, seed=args.seed, max_pairs=args.max_pairs, device=dev, hp=hp,
+                            pitch_shift=args.pitch_shift, **few)
             res[s]["f0"] = r
             means = (f" vuv_agree={r['vuv_agree']:.4f} f0_corr={r['f0_corr']:.4f} st_target={r['st_target']:.4f} "
                      f"st_source={r['st_source']:.4f} f0_success={r['f0_success']:.4f} "
@@ -150,6 +158,11 @@ def main(argv=None):
             means += f" n_refs={r['n_refs']} n_few={r['n_few']}" if few else ""
             print(f"{s}: f0 n={r['n']} n_short={r['n_short']} n_unvoiced={r['n_unvoiced']}{means} "
                   f"({len(r['speakers'])} target speakers)")
+            if args.pitch_shift:
+                ps = r["pitch_shift"]
+                print(f"{s}: f0 pitch_shift match mean={ps['mean_semitones']:+.4f} mean_abs={ps['mean_abs_semitones']:.4f} "
+                      f"n_unmatched={ps['n_unmatched']} n_clamped={ps['n_clamped']} (unshifted st_target="
+                      + ("n/a" if not r["unshifted"]["n"] else f"{r['unshifted']['st_target']:.4f}") + ")")
     if args.output:
         with open(args.output, "w") as f:
             json.dump(res, f, indent=1)

@@ -651,6 +651,22 @@ int avc_deemphasis(const avc_audio_desc* d, float coef, void* stream);
 int avc_yin(const avc_audio_desc* d, int32_t win, int32_t tau_min, int32_t tau_max, float threshold, double* tau,
             double* aperiodicity, double* energy, void* stream);
 
+/* Formant-preserving pitch shift of rows of linear magnitudes (csrc/pitch.cu), fp32.  mag and out [rows][n_bins], ratio
+ * [rows] (device memory).  Per row, with N = 2 (n_bins - 1), Q = lifter and alpha = ratio[row]:
+ *   l[k] = ln max(S[k], 1e-5)
+ *   c[q] = (1/N) (l[0] + (-1)^q l[n_bins-1] + 2 sum_{k=1}^{n_bins-2} l[k] cos(pi q k / (n_bins-1))), q < Q
+ *   E[k] = c[0] + 2 sum_{q=1}^{Q-1} c[q] cos(pi q k / (n_bins-1))   (rectangular lifter: the envelope)
+ *   F[k] = l[k] - E[k]                                              (the fine structure)
+ *   out[k] = exp(E[k] + F~(p)), p = min(k / alpha rounded to float, n_bins - 1), F~ F linearly interpolated at p
+ * so the harmonics move by alpha and the envelope stays.  A row with alpha == 1.0f exactly is copied bit for bit; a
+ * row whose alpha is not finite or <= 0 becomes NaN (the ratios are device memory: checking them is the caller's job).
+ * Cosines come from a table of cospif(m / (n_bins-1)), m = q k mod N.  Every sum runs in a fixed order, no atomics: a
+ * row gets the same bits in any batch.  No allocation, no synchronisation.  AVC_ERR_INVALID before any launch for a
+ * null pointer, rows < 1, a lifter outside [1, n_bins - 1] or out overlapping mag; AVC_ERR_UNSUPPORTED for
+ * n_bins != 1025 (n_fft 2048). */
+int avc_pitch_shift(const float* mag, const float* ratio, float* out, int32_t rows, int32_t n_bins, int32_t lifter,
+                    void* stream);
+
 /* Mel projections of the concatenated frames of a ragged batch (rows are independent).
  *   AVC_MEL_TO_MAG: out[rows][n_bins] = A x mat, A = 10^((clip(in,0,1) max_db - max_db + ref_db) / 20),
  *                   in [rows][n_mels], mat [n_mels][n_bins] (the transposed mel-to-linear matrix)

@@ -50,6 +50,19 @@ file, even one whose name starts with @), and its output name defaults to ``<sou
 as in the single-pair mode), converted by Inferencer.inference_padded, and the .wav outputs synthesised in one batched
 Vocoder.mel_to_wav call (-gl_iters, -gl_momentum, -gl_init).  A missing file, a malformed line or an utterance shorter than the
 model accepts is reported with its line number before anything runs on the GPU.
+
+Pitch: -pitch_shift SEMITONES (in [-24, 24], default 0) transposes every .wav output by a formant-preserving shift of
+the synthesis (Vocoder.mel_to_signal's ``semitones``), for one conversion, -t sets, -bank -speaker, -morph and -pairs:
+
+    python inference.py -c config.yaml -m model.ckpt -a attr.pkl -s src.wav -t tgt.wav -o out.wav -pitch_shift -5
+
+-pitch_shift match instead shifts each conversion so that its mean log2 F0 meets its -t file's or set's, both tracked
+as synthesised (adaptive_voice_conversion_b200/f0.py match_shifts), clamped to [-24, 24] and 0 when either side has no
+voiced frame; one line per conversion reports the output, the shift and the voiced frame counts.  It works with -t
+and in -pairs with file and set targets; banked speakers and morphs have no mels to match, so -speaker, -morph and
+@SPEC lines are refused, as is a shift of a .npy output (a mel is not synthesised):
+
+    python inference.py -c config.yaml -m model.ckpt -a attr.pkl -pairs pairs.txt -o out_dir -pitch_shift match
 """
 import os
 from argparse import ArgumentParser
@@ -166,17 +179,35 @@ def convert_pairs(inf, pairs, mels, bank=None):
     return decs
 
 
+def refuse_bank_targets(pairs, path):
+    """ValueError naming the first @SPEC line: -pitch_shift match needs the target's mels."""
+    for n, _, t, _ in pairs:
+        if isinstance(t, BankTarget):
+            raise ValueError(f"{path} line {n}: -pitch_shift match needs the target's recordings; a banked speaker "
+                             f"(@{t.spec}) has none")
+
+
+def print_matches(names, info):
+    for name, d in zip(names, info):
+        note = " (unmatched: no voiced frame)" if d["unmatched"] else " (clamped)" if d["clamped"] else ""
+        print(f"{name}: pitch shift {d['shift']:+.3f} semitones, voiced frames {d['voiced_conv']} conversion / "
+              f"{d['voiced_refs']} target{note}")
+
+
 def run_pairs(args, config):
     """The -pairs mode: every pair of the file, batched (see the module docstring)."""
     from adaptive_voice_conversion_b200.mcd import min_frames
     from adaptive_voice_conversion_b200.vocoder import AudioParams, Vocoder, load_wav
     pairs = read_pairs(args.pairs, bank=bool(args.bank))
+    if args.semitones == "match":
+        refuse_bank_targets(pairs, args.pairs)
     os.makedirs(args.output, exist_ok=True)
     dev = local_device()
     files = sorted({p for _, s, t, _ in pairs
                     for p in (s,) + ((t,) if isinstance(t, str) else () if isinstance(t, BankTarget) else t)})
     need_voc = any(is_wav(f) for f in files) or any(is_wav(name) for *_, name in pairs)
-    hp = AudioParams(n_iter=args.gl_iters, momentum=args.gl_momentum, gl_init=args.gl_init)
+    hp = AudioParams(n_iter=args.gl_iters, momentum=args.gl_momentum, gl_init=args.gl_init,
+                     pitch_shift=0.0 if args.semitones == "match" else args.semitones)
     vocoder = Vocoder(n_mels=config["SpeakerEncoder"]["c_in"] // config["data_loader"]["frame_size"],
                       hp=hp) if need_voc else None
     wavs = [f for f in files if is_wav(f)]
@@ -197,6 +228,7 @@ def run_pairs(args, config):
                 bank.code(t.spec)
             except ValueError as e:
                 raise ValueError(f"{args.pairs} line {n}: {e}") from None
+    raw = mels
     if inf.attr is not None:
         mean = torch.as_tensor(np.asarray(inf.attr["mean"], np.float32)).to(dev)
         std = torch.as_tensor(np.asarray(inf.attr["std"], np.float32)).to(dev)
@@ -205,7 +237,16 @@ def run_pairs(args, config):
     if inf.attr is not None:
         decs = [d * std + mean for d in decs]
     to_wav = [i for i, (*_, name) in enumerate(pairs) if is_wav(name)]
-    ys = vocoder.mel_to_wav([decs[i].contiguous() for i in to_wav]) if to_wav else []
+    shifts = None
+    if args.semitones == "match" and to_wav:
+        from adaptive_voice_conversion_b200.f0 import match_shifts
+        shifts, info = match_shifts(vocoder, [decs[i].contiguous() for i in to_wav],
+                                    [[raw[p] for p in ((pairs[i][2],) if isinstance(pairs[i][2], str) else pairs[i][2])]
+                                     for i in to_wav], vocoder.hp)
+        print_matches([pairs[i][3] for i in to_wav], info)
+    ys = []
+    if to_wav:   # a fixed shift is the vocoder's hp.pitch_shift
+        ys = vocoder.mel_to_wav([decs[i].contiguous() for i in to_wav], **({} if shifts is None else {"semitones": shifts}))
     for i, y in zip(to_wav, ys):
         inf.write_wav_to_file(y.cpu().numpy(), os.path.join(args.output, pairs[i][3]))
     for i, (*_, name) in enumerate(pairs):
@@ -218,9 +259,30 @@ def load_bank(path, model):
     return SpeakerBank.load(path, model)
 
 
+def pitch_shift_arg(p, args):
+    """args.semitones: "match" or the -pitch_shift float; p.error for a value that is not finite or outside [-24, 24],
+    match with -speaker or -morph, and a non-zero shift of a single .npy output."""
+    from adaptive_voice_conversion_b200.vocoder import PITCH_SHIFT_MAX
+    v = str(args.pitch_shift)
+    if v == "match":
+        args.semitones = "match"
+        if args.speaker is not None or args.morph is not None:
+            p.error("-pitch_shift match needs the target's recordings: banked speakers (-speaker, -morph) have none")
+    else:
+        try:
+            args.semitones = float(v)
+        except ValueError:
+            p.error(f"-pitch_shift must be a number of semitones or 'match' (got {v!r})")
+        if not np.isfinite(args.semitones) or abs(args.semitones) > PITCH_SHIFT_MAX:
+            p.error(f"-pitch_shift must be finite and in [-{PITCH_SHIFT_MAX:g}, {PITCH_SHIFT_MAX:g}] semitones (got {v})")
+    if args.semitones != 0.0 and not args.pairs and not is_wav(args.output):
+        p.error("-pitch_shift shifts the synthesis: a .npy output is a mel and is not synthesised")
+
+
 def check_args(p, args):
     """Argument errors (p.error): -t, or -bank with -speaker, for one conversion; -speaker needs -bank; -morph needs
-    -bank, excludes -t, -speaker and -pairs, and its keyframes must parse."""
+    -bank, excludes -t, -speaker and -pairs, and its keyframes must parse; -pitch_shift as pitch_shift_arg."""
+    pitch_shift_arg(p, args)
     if args.morph is not None:
         if not args.bank:
             p.error("-morph needs -bank")
@@ -265,6 +327,9 @@ def parser():
     p.add_argument("-speaker", help="banked target: NAME or a weighted mix NAME:W,NAME:W,... (needs -bank)")
     p.add_argument("-morph", nargs="+", metavar="SPEC@SECONDS",
                    help="time-varying target: banked speakers or mixes at keyframe times, interpolated (needs -bank)")
+    p.add_argument("-pitch_shift", default="0", metavar="{SEMITONES,match}",
+                   help="transpose every .wav output by SEMITONES in [-24, 24] (formant-preserving), or 'match' each "
+                        "conversion's pitch level to its -t target's")
     return p
 
 
@@ -282,8 +347,10 @@ if __name__ == "__main__":
     if any(is_wav(f) for f in (args.source, *targets, args.output)):
         from adaptive_voice_conversion_b200.vocoder import AudioParams, Vocoder
         vocoder = Vocoder(n_mels=config["SpeakerEncoder"]["c_in"] // config["data_loader"]["frame_size"],
-                          hp=AudioParams(n_iter=args.gl_iters, momentum=args.gl_momentum, gl_init=args.gl_init))
-    inf = Inferencer(config=config, args=args, vocoder=vocoder if is_wav(args.output) else None)
+                          hp=AudioParams(n_iter=args.gl_iters, momentum=args.gl_momentum, gl_init=args.gl_init,
+                                         pitch_shift=0.0 if args.semitones == "match" else args.semitones))
+    match = args.semitones == "match" and is_wav(args.output)
+    inf = Inferencer(config=config, args=args, vocoder=vocoder if is_wav(args.output) and not match else None)
 
     def read(path):
         return vocoder.get_spectrograms(path)[0] if is_wav(path) else np.load(path).astype(np.float32)
@@ -305,10 +372,17 @@ if __name__ == "__main__":
         mel = inf.denormalize(mel) if inf.attr is not None else mel
         wav = inf.vocoder.melspectrogram2wav(mel) if inf.vocoder is not None else None
     else:
-        tgts = [read(t) for t in targets]
-        tgts = [inf.normalize(t) for t in tgts] if inf.attr is not None else tgts
+        raw_tgts = [read(t) for t in targets]
+        tgts = [inf.normalize(t) for t in raw_tgts] if inf.attr is not None else raw_tgts
         tgt = [torch.from_numpy(t).to(dev) for t in tgts]     # several targets: one reference set
         wav, mel = inf.inference_one_utterance(torch.from_numpy(src).to(dev), tgt[0] if len(tgt) == 1 else tgt)
+        if match:
+            from adaptive_voice_conversion_b200.f0 import match_shifts
+            m = torch.from_numpy(np.ascontiguousarray(mel, np.float32)).to(dev)
+            refs = [torch.from_numpy(np.ascontiguousarray(t, np.float32)).to(dev) for t in raw_tgts]
+            shifts, info = match_shifts(vocoder, [m], [refs], vocoder.hp)
+            print_matches([args.output], info)
+            wav = vocoder.mel_to_wav([m], semitones=shifts)[0].cpu().numpy()
     if is_wav(args.output):
         inf.write_wav_to_file(wav, args.output)
     else:
