@@ -34,6 +34,7 @@ from .data_utils import DeviceSegments
 from .engine import A4
 from .optim import FusedAdam
 from .trainer import FusedTrainer
+from .utils import _stream, eval_mode
 
 FORMAT = "avc-adapt-1"
 LOG_EVERY = 100
@@ -206,7 +207,7 @@ def rec_loss_varlen(dec: torch.Tensor, x: torch.Tensor, lengths: torch.Tensor) -
     lt = lengths.to(device=dec.device, dtype=torch.int32)
     out = torch.empty(B, dtype=torch.float64, device=dec.device)
     d = L.RecVarlenDesc(B=B, C=Cc, T=T, dec=dec.data_ptr(), x=x.data_ptr(), lengths=lt.data_ptr(), out=out.data_ptr())
-    L.check(L.load().avc_rec_loss_varlen(d, torch.cuda.current_stream(dec.device).cuda_stream), "avc_rec_loss_varlen")
+    L.check(L.load().avc_rec_loss_varlen(d, _stream(dec.device)), "avc_rec_loss_varlen")
     return out
 
 
@@ -214,7 +215,7 @@ def heldout_rec(model, mels: Mapping[str, object], code: torch.Tensor) -> dict:
     """{"rec", "n", "n_skipped", "skipped"} of the held-out clips `mels` ({id: attr-normalised [T, n_mels]}) converted
     with `code`: the conversion path in padded_batches' grid, per utterance the mean |dec - x| over its valid frames,
     then the mean over utterances (float64, in sorted id order).  Clips shorter than the model accepts are skipped."""
-    from .inference import padded_batches
+    from .inference import padded_batch, padded_batches
     from .mcd import min_frames
     dev = code.device
     min_src = min_frames(model.config)[0]
@@ -225,26 +226,17 @@ def heldout_rec(model, mels: Mapping[str, object], code: torch.Tensor) -> dict:
     if not keep:
         return res
     lens = [int(mels[u].shape[0]) for u in keep]
+    frames = [(m if isinstance(m, torch.Tensor) else torch.from_numpy(_host(m))).t() for m in (mels[u] for u in keep)]
     per = np.zeros(len(keep))
-    was_training = model.training
-    model.eval()
-    try:
+    with eval_mode(model, dev):
         for idx, T, _, _ in padded_batches(lens, lens):
-            n_mels = int(mels[keep[idx[0]]].shape[1])
-            x = torch.zeros(len(idx), n_mels, T, device=dev)
-            for j, i in enumerate(idx):
-                m = mels[keep[i]]
-                m = m if isinstance(m, torch.Tensor) else torch.from_numpy(_host(m))
-                x[j, :, :lens[i]].copy_(m.t())
-            lx = torch.tensor([lens[i] for i in idx], dtype=torch.int32, device=dev)
+            x, lx = padded_batch(frames, idx, T, dev)
+            n_mels = x.shape[1]
             emb = code.detach().reshape(1, -1).expand(len(idx), -1).contiguous()
             dec = model.inference_from_embeddings(x, emb, lengths=lx)
             sums = rec_loss_varlen(dec[:, :, :T], x, lx).cpu().numpy()
             for j, i in enumerate(idx):
                 per[i] = sums[j] / (n_mels * lens[i])
-        model.engine(dev).check_tc_status()
-    finally:
-        model.train(was_training)
     res["rec"] = float(np.cumsum(per)[-1] / len(per))
     return res
 

@@ -54,6 +54,7 @@ import torch
 
 from . import _lib as L
 from .evaluate import speaker_of
+from .utils import _stream, eval_mode, upload_mels
 from .vocoder import PITCH_SHIFT_MAX, AudioParams, Vocoder, _Ragged
 
 METRICS = ("vuv_agree", "f0_corr", "st_target", "st_source", "f0_success", "st_target_source")
@@ -85,10 +86,6 @@ class F0Params:
         return {"fmin": self.fmin, "fmax": self.fmax, "win": self.win, "tau_min": self.tau_min(sr),
                 "tau_max": self.tau_max(sr), "threshold": self.threshold, "silence_db": self.silence_db, "sr": int(sr),
                 "hop": int(hop)}
-
-
-def _stream(dev):
-    return C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
 
 
 def yin(wavs, sr: int, hop: int, params: F0Params = F0Params()):
@@ -315,7 +312,7 @@ def evaluate_f0(model, data: Mapping[str, np.ndarray], attr, seed: int = 0, max_
 
     utts, pairs, refs, res = select_pairs(cfg, {u: len(v) for u, v in data.items()}, seed, max_pairs, n_refs)
     used = sorted(set(utts) | {u for u, _ in pairs} | {v for rs in refs for v in rs})
-    mels = {u: torch.from_numpy(np.ascontiguousarray(data[u], np.float32)).to(dev) for u in used}
+    mels = upload_mels(data, used, dev)
     n_mels = int(cfg["SpeakerEncoder"]["c_in"])
     hp = replace(hp, n_mels=n_mels, pitch_shift=0.0)
     res["tracker"] = params.settings(hp.sr, hp.hop_length)
@@ -325,9 +322,7 @@ def evaluate_f0(model, data: Mapping[str, np.ndarray], attr, seed: int = 0, max_
     if mean.numel() != n_mels or std.numel() != n_mels:
         raise ValueError(f"evaluate_f0: attr mean / std have {mean.numel()} / {std.numel()} entries, the mels {n_mels}")
     convs = [None] * len(pairs)
-    was_training = model.training
-    model.eval()
-    try:
+    with eval_mode(model, dev):
         codes = None
         if n_refs > 1 and pairs:
             from .inference import embed_reference_sets
@@ -336,9 +331,6 @@ def evaluate_f0(model, data: Mapping[str, np.ndarray], attr, seed: int = 0, max_
             for idx, decs in converted(model, [mels[u] for u, _ in pairs], [mels[rs[0]] for rs in refs], codes=codes):
                 for i, dec in zip(idx, decs):
                     convs[i] = dec
-        model.engine(dev).check_tc_status()
-    finally:
-        model.train(was_training)
     lap("conversion")
     vocoder = Vocoder(hp=hp, device=dev)
     conv_mels = [c * std + mean for c in convs]

@@ -19,7 +19,7 @@ import torch.nn.functional as F
 
 from .mcd import min_frames
 from .model import AE
-from .utils import cc, local_device
+from .utils import cc, exact_buckets, local_device
 
 # Inferencer.inference_padded: pairs per padded batch, and the graphs of padded shapes kept (least recently used evicted)
 PADDED_BATCH_MAX = 64
@@ -73,6 +73,30 @@ def pack_sets(set_sizes: Sequence[int], set_lens: Sequence[int], batch_max: int 
     return [(idx, padded_extent(max(int(set_lens[g]) for g in idx))) for idx in out]
 
 
+def fill_rows(dst, frames, rows) -> List[int]:
+    """Copies frames[i] ([C, T_i]) into dst[j, :, :T_i] for the j-th entry i of rows and returns those T_i; the frames
+    of dst past T_i are left as they are (a graph slot's static buffers are never re-zeroed)."""
+    lens = []
+    for j, i in enumerate(rows):
+        n = int(frames[i].shape[1])
+        dst[j, :, :n].copy_(frames[i])
+        lens.append(n)
+    return lens
+
+
+def padded_batch(frames, rows, T: int, device):
+    """(x, lengths): x a zero-filled [len(rows), C, T] batch that fill_rows fills, lengths its int32 T_i on device."""
+    x = torch.zeros(len(rows), int(frames[rows[0]].shape[0]), T, device=device)
+    return x, torch.tensor(fill_rows(x, frames, rows), dtype=torch.int32, device=device)
+
+
+def scatter_crops(out, dec, idx, lens):
+    """out[i] = dec[j] cropped to its 8 ceil(lens[j] / 8) output frames, as [frames, n_mels], for the j-th entry i of
+    idx."""
+    for j, i in enumerate(idx):
+        out[i] = dec[j, :, :8 * -(-lens[j] // 8)].transpose(0, 1)
+
+
 def embed_reference_sets(model, sets) -> torch.Tensor:
     """[G, c_out] (device): the pooled speaker code of each set of sets, lists of [C, T] model inputs (device tensors,
     validated by the caller), through AE.get_speaker_embeddings(groups=) in pack_sets' padded batches."""
@@ -80,12 +104,9 @@ def embed_reference_sets(model, sets) -> torch.Tensor:
     out = torch.empty(len(sets), model.config["SpeakerEncoder"]["c_out"], device=dev)
     for idx, T in pack_sets([len(s) for s in sets], [max(int(r.shape[1]) for r in s) for s in sets]):
         members = [r for g in idx for r in sets[g]]
-        x = torch.zeros(len(members), int(members[0].shape[0]), T, device=dev)
-        for j, r in enumerate(members):
-            x[j, :, :r.shape[1]].copy_(r)
-        lens = torch.tensor([int(r.shape[1]) for r in members], dtype=torch.int32)
+        x, lens = padded_batch(members, range(len(members)), T, dev)
         offs = torch.tensor([0] + [len(sets[g]) for g in idx]).cumsum(0).to(torch.int32)
-        emb = model.get_speaker_embeddings(x, lengths=lens.to(dev), groups=offs.to(dev))
+        emb = model.get_speaker_embeddings(x, lengths=lens, groups=offs.to(dev))
         out.index_copy_(0, torch.tensor(idx, device=dev), emb)
     return out
 
@@ -170,11 +191,8 @@ class Inferencer(object):
         in the input order (device tensors, normalised domain)."""
         if len(xs) != len(x_conds):
             raise ValueError("inference_ragged: xs and x_conds must have the same length")
-        buckets = {}
-        for i, (x, c) in enumerate(zip(xs, x_conds)):
-            buckets.setdefault((int(x.shape[0]), int(c.shape[0])), []).append(i)
         out = [None] * len(xs)
-        for (_, _), idx in sorted(buckets.items()):
+        for _, idx in exact_buckets([int(x.shape[0]) for x in xs], [int(c.shape[0]) for c in x_conds]):
             xb = torch.cat([self.utt_make_frames(xs[i]) for i in idx], dim=0)
             cb = torch.cat([self.utt_make_frames(x_conds[i]) for i in idx], dim=0)
             dec = self.inference_batch(xb, cb)               # [n, n_mels, 8*ceil(T/8)]
@@ -212,17 +230,11 @@ class Inferencer(object):
         out = [None] * len(xs)
         for idx, T, Tc, Bp in padded_batches([s.shape[1] for s in src], [r.shape[1] for r in ref], batch_max):
             xb, cb, lx, lc, run = self._padded_slot(Bp, src[0].shape[0], T, ref[0].shape[0], Tc, dev)
-            lens = [(src[i].shape[1], ref[i].shape[1]) for i in idx]
-            lens += [lens[0]] * (Bp - len(idx))                 # rows past the batch repeat its first pair
-            for j, i in enumerate(idx + [idx[0]] * (Bp - len(idx))):
-                xb[j, :, :lens[j][0]].copy_(src[i])
-                cb[j, :, :lens[j][1]].copy_(ref[i])
-            hl = torch.tensor(lens, dtype=torch.int32)
-            lx.copy_(hl[:, 0])
-            lc.copy_(hl[:, 1])
-            dec = run()
-            for j, i in enumerate(idx):
-                out[i] = dec[j, :, :8 * -(-lens[j][0] // 8)].transpose(0, 1)
+            rows = idx + [idx[0]] * (Bp - len(idx))                # rows past the batch repeat its first pair
+            lens, ref_lens = fill_rows(xb, src, rows), fill_rows(cb, ref, rows)
+            lx.copy_(torch.tensor(lens, dtype=torch.int32))
+            lc.copy_(torch.tensor(ref_lens, dtype=torch.int32))
+            scatter_crops(out, run(), idx, lens)
         self.model.engine(dev).check_tc_status()
         return out
 
@@ -347,13 +359,10 @@ class Inferencer(object):
         for idx, T, _, Bp in padded_batches([s.shape[1] for s in src], [0] * len(src), batch_max):
             xb, eb, lx, run = self._emb_slot(Bp, src[0].shape[0], T, dev)
             rows = idx + [idx[0]] * (Bp - len(idx))                # rows past the batch repeat its first pair
-            for j, i in enumerate(rows):
-                xb[j, :, :src[i].shape[1]].copy_(src[i])
+            lens = fill_rows(xb, src, rows)
             eb.copy_(codes.index_select(0, torch.tensor(rows, device=dev)))
-            lx.copy_(torch.tensor([src[i].shape[1] for i in rows], dtype=torch.int32))
-            dec = run()
-            for j, i in enumerate(idx):
-                out[i] = dec[j, :, :8 * -(-src[i].shape[1] // 8)].transpose(0, 1)
+            lx.copy_(torch.tensor(lens, dtype=torch.int32))
+            scatter_crops(out, run(), idx, lens)
         self.model.engine(dev).check_tc_status()
         return out
 
@@ -405,15 +414,13 @@ class Inferencer(object):
             rows = idx + [idx[0]] * (Bp - len(idx))                # rows past the batch repeat its first source
             cb.zero_()
             wb.zero_()
+            lens = fill_rows(xb, src, rows)
             for j, i in enumerate(rows):
-                n, k = src[i].shape[1], codes[i].shape[0]
-                xb[j, :, :n].copy_(src[i])
+                k = codes[i].shape[0]
                 cb[j, :k].copy_(codes[i])
-                wb[j, :k, :n].copy_(weights[i])
-            lx.copy_(torch.tensor([src[i].shape[1] for i in rows], dtype=torch.int32))
-            dec = run()
-            for j, i in enumerate(idx):
-                out[i] = dec[j, :, :8 * -(-src[i].shape[1] // 8)].transpose(0, 1)
+                wb[j, :k, :lens[j]].copy_(weights[i])
+            lx.copy_(torch.tensor(lens, dtype=torch.int32))
+            scatter_crops(out, run(), idx, lens)
         self.model.engine(dev).check_tc_status()
         return out
 

@@ -45,6 +45,7 @@ import torch
 from . import _lib as L
 from .engine import conv_geometry
 from .evaluate import speaker_of
+from .utils import _stream, eval_mode, exact_buckets, upload_mels
 from .vocoder import AudioParams
 
 MCD_SCALE = 10.0 * math.sqrt(2.0) / math.log(10.0)
@@ -174,10 +175,6 @@ def fewshot_triplets(trip, utts: Sequence[str], texts: Mapping[str, str], length
 
 
 # ------------------------------------------------------------------ the two kernels
-def _stream(dev):
-    return C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
-
-
 def dct_matrix(n_mels: int, dims: int) -> np.ndarray:
     """[n_mels][dims] float64: sqrt(2/N) cos(pi k (2m+1) / 2N) at [m][k-1], k = 1..dims (orthonormal DCT-II, no c_0)."""
     m = np.arange(n_mels, dtype=np.float64)[:, None]
@@ -255,11 +252,8 @@ def converted(model, sources, refs, batch_max: int = 64, codes=None):
     AE.inference calls of at most batch_max pairs.  codes [P, c_out] (few-shot): the same batches through
     AE.inference_from_embeddings with pair i's speaker code codes[i] instead of refs[i]'s.  The model must be in eval
     mode."""
-    buckets: Dict[Tuple[int, int], List[int]] = {}
-    for i, (x, c) in enumerate(zip(sources, refs)):
-        buckets.setdefault((int(x.shape[0]), int(c.shape[0])), []).append(i)
     with torch.no_grad():
-        for (T, _), idx in sorted(buckets.items()):
+        for (T, _), idx in exact_buckets([int(x.shape[0]) for x in sources], [int(c.shape[0]) for c in refs]):
             for f in range(0, len(idx), batch_max):
                 part = idx[f:f + batch_max]
                 xb = torch.stack([sources[i].t() for i in part]).contiguous()
@@ -318,13 +312,11 @@ def evaluate_mcd(model, data: Mapping[str, np.ndarray], attr, texts: Mapping[str
         res["speakers"] = {}
         return res
     used = sorted({u for s, r, g in trip for u in [s, g] + (r if n_refs > 1 else [r])})
-    mels = {u: torch.from_numpy(np.ascontiguousarray(data[u], np.float32)).to(dev) for u in used}
+    mels = upload_mels(data, used, dev)
     plain = sorted({t[0] for t in trip} | {t[2] for t in trip})
     ceps = dict(zip(plain, mel_cepstrum([mels[u] for u in plain], attr, hp, dims)))
     conv = [None] * len(trip)
-    was_training = model.training
-    model.eval()
-    try:
+    with eval_mode(model, dev):
         codes = None
         if target_codes is not None:
             codes = torch.stack([torch.as_tensor(target_codes[speaker_of(g)], dtype=torch.float32).reshape(-1).to(dev)
@@ -336,9 +328,6 @@ def evaluate_mcd(model, data: Mapping[str, np.ndarray], attr, texts: Mapping[str
         for idx, decs in converted(model, [mels[s] for s, _, _ in trip], first, codes=codes):
             for i, c in zip(idx, mel_cepstrum(decs, attr, hp, dims)):
                 conv[i] = c
-        model.engine(dev).check_tc_status()
-    finally:
-        model.train(was_training)
     gts = [ceps[g] for _, _, g in trip]
     sl = dtw(conv + [ceps[s] for s, _, _ in trip], gts + gts).cpu().numpy()
     n = len(trip)

@@ -32,8 +32,9 @@ import numpy as np
 import torch
 
 from .evaluate import speaker_of as _speaker_of
-from .inference import padded_batches
+from .inference import padded_batch, padded_batches
 from .mcd import min_frames
+from .utils import eval_mode
 
 FORMAT = "avc-speaker-bank-1"
 
@@ -275,25 +276,17 @@ def build_bank(model, mels: Mapping[str, object], speaker_of: Callable[[str], st
     sums = torch.empty(len(flat), c_h, device=dev)
     counts = torch.empty(len(flat), dtype=torch.int32, device=dev)
     lens = [lengths[u] for u in flat]
-    was_training = model.training
-    model.eval()
-    try:
+    frames = [(m if isinstance(m, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(m, np.float32))).t()
+              for m in (mels[u] for u in flat)]
+    with eval_mode(model, dev):
         for idx, T, _, _ in padded_batches(lens, lens):
-            x = torch.zeros(len(idx), int(mels[flat[idx[0]]].shape[1]), T, device=dev)
-            for j, i in enumerate(idx):
-                m = mels[flat[i]]
-                m = m if isinstance(m, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(m, np.float32))
-                x[j, :, :lens[i]].copy_(m.t())
-            lx = torch.tensor([lens[i] for i in idx], dtype=torch.int32, device=dev)
+            x, lx = padded_batch(frames, idx, T, dev)
             s, n = model.get_speaker_sums(x, lengths=lx)
             rows = torch.tensor(idx, device=dev)
             sums.index_copy_(0, rows, s)
             counts.index_copy_(0, rows, n)
         offsets = torch.tensor([0] + [len(us) for us in utts], dtype=torch.int64).cumsum(0)
         codes = model.speaker_codes_from_sums(sums, counts, groups=offsets.to(dev))
-        model.engine(dev).check_tc_status()
-    finally:
-        model.train(was_training)
     return SpeakerBank(speakers, codes, [len(us) for us in utts], utts, fingerprint(model), skipped)
 
 

@@ -65,8 +65,9 @@ import torch
 
 from . import _lib as L
 from .evaluate import speaker_of
-from .inference import padded_batches
+from .inference import padded_batch, padded_batches
 from .mcd import min_frames
+from .utils import _stream, eval_mode, upload_mels
 
 REPRESENTATIONS = ("speaker", "content", "mel")
 
@@ -150,10 +151,6 @@ def fewshot_pairs(pairs, utts: Sequence[str], lengths: Mapping[str, int], n_refs
 
 
 # ------------------------------------------------------------------ the three kernels
-def _stream(dev):
-    return C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
-
-
 def _lengths(lengths, B, dev) -> torch.Tensor:
     if isinstance(lengths, torch.Tensor):
         if lengths.dtype == torch.bool or lengths.is_floating_point() or lengths.is_complex():
@@ -342,21 +339,15 @@ def bank_identification(bank, y: torch.Tensor, src_speakers, tgt_speakers, real:
 
 
 # ------------------------------------------------------------------ representations and conversions
-def _batch(mels, idx, T, dev):
-    x = torch.zeros(len(idx), int(mels[idx[0]].shape[1]), T, device=dev)
-    for j, i in enumerate(idx):
-        x[j, :, :mels[i].shape[0]].copy_(mels[i].t())
-    return x, torch.tensor([int(mels[i].shape[0]) for i in idx], dtype=torch.int32, device=dev)
-
-
 def representations(model, mels: Sequence[torch.Tensor]) -> Dict[str, torch.Tensor]:
     """{speaker, content, mel}: [N, D] float32 (device) of the attr-normalised mels [T_i, n_mels] (device tensors, each
     at least max(min_frames) long), in padded batches.  The model must be in eval mode."""
     dev = mels[0].device
     lens = [int(m.shape[0]) for m in mels]
+    frames = [m.t() for m in mels]
     out = {k: [None] * len(mels) for k in REPRESENTATIONS}
     for idx, T, _, _ in padded_batches(lens, lens):
-        x, lx = _batch(mels, idx, T, dev)
+        x, lx = padded_batch(frames, idx, T, dev)
         emb = model.get_speaker_embeddings(x, lengths=lx)
         mu, lat = model.get_content_means(x, lengths=lx)
         rows = {"speaker": emb, "content": time_stats(mu, lat), "mel": time_stats(x, lx)}
@@ -372,20 +363,22 @@ def converted_embeddings(model, sources: Sequence[torch.Tensor], refs: Sequence[
     one speaker: the sources are then converted with the sets' pooled codes (inference.embed_reference_sets) through
     AE.inference_from_embeddings.  The model must be in eval mode."""
     dev = sources[0].device
+    src = [s.t() for s in sources]
     out = [None] * len(sources)
     if isinstance(refs[0], (list, tuple)):
         from .inference import embed_reference_sets
         codes = embed_reference_sets(model, [[r.t() for r in s] for s in refs])
         for idx, T, _, _ in padded_batches([int(s.shape[0]) for s in sources], [0] * len(sources)):
-            x, lx = _batch(sources, idx, T, dev)
+            x, lx = padded_batch(src, idx, T, dev)
             dec = model.inference_from_embeddings(x, codes[torch.tensor(idx, device=dev)], lengths=lx)
             emb = model.get_speaker_embeddings(dec, lengths=lx)
             for j, i in enumerate(idx):
                 out[i] = emb[j]
         return torch.stack(out)
+    ref = [r.t() for r in refs]
     for idx, T, Tc, _ in padded_batches([int(s.shape[0]) for s in sources], [int(r.shape[0]) for r in refs]):
-        x, lx = _batch(sources, idx, T, dev)
-        c, lc = _batch(refs, idx, Tc, dev)
+        x, lx = padded_batch(src, idx, T, dev)
+        c, lc = padded_batch(ref, idx, Tc, dev)
         dec = model.inference(x, c, lengths=lx, cond_lengths=lc)
         emb = model.get_speaker_embeddings(dec, lengths=lx)
         for j, i in enumerate(idx):
@@ -435,14 +428,12 @@ def evaluate_speakers(model, data: Mapping[str, np.ndarray], seed: int = 0, max_
         used = sorted(set(utts) | {u for u, _ in pairs} | {r for _, refs in pairs for r in refs})
     else:
         used = sorted(set(utts) | {u for p in pairs for u in p})
-    mels = {u: torch.from_numpy(np.ascontiguousarray(data[u], np.float32)).to(dev) for u in used}
+    mels = upload_mels(data, used, dev)
     speakers = sorted({speaker_of(u) for u in utts})
     label = {s: i for i, s in enumerate(speakers)}
     labels = [label[speaker_of(u)] for u in utts]
     res = {"eer": {}, "n_utts": len(utts), "n_short": len(data) - len(utts)}
-    was_training = model.training
-    model.eval()
-    try:
+    with eval_mode(model, dev):
         if utts:
             reps = representations(model, [mels[u] for u in utts])
             for k in REPRESENTATIONS:
@@ -495,8 +486,5 @@ def evaluate_speakers(model, data: Mapping[str, np.ndarray], seed: int = 0, max_
             if bank is not None:
                 conv.update(bank_identification(bank, None, [], [], reps["speaker"] if utts else None,
                                                 [speaker_of(u) for u in utts]))
-        model.engine(dev).check_tc_status()
-    finally:
-        model.train(was_training)
     res["conversion"] = conv
     return res

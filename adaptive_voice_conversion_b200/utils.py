@@ -6,9 +6,43 @@ Logger keeps the last scalars in memory and prints nothing.
 """
 from __future__ import annotations
 
+import contextlib
+import ctypes as C
 import os
 
+import numpy as np
 import torch
+
+
+def _stream(dev):
+    return C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+
+
+def upload_mels(data, keys, dev):
+    """{key: data[key] as a float32 tensor on dev} of a set's arrays at the keys."""
+    return {u: torch.from_numpy(np.ascontiguousarray(data[u], np.float32)).to(dev) for u in keys}
+
+
+def exact_buckets(src_lens, ref_lens):
+    """[((T, T_ref), pair indices)] in sorted key order: the pairs grouped by their exact lengths, each group in input
+    order."""
+    buckets = {}
+    for i, key in enumerate(zip(src_lens, ref_lens)):
+        buckets.setdefault(key, []).append(i)
+    return sorted(buckets.items())
+
+
+@contextlib.contextmanager
+def eval_mode(model, dev):
+    """Runs the block with `model` in eval mode, checks its engine's tensor-core status word on `dev` when the block
+    ends normally and restores the previous training mode in any case."""
+    was_training = model.training
+    model.eval()
+    try:
+        yield
+        model.engine(dev).check_tc_status()
+    finally:
+        model.train(was_training)
 
 
 def local_device() -> torch.device:

@@ -24,7 +24,7 @@ import numpy as np
 import torch
 
 from . import _lib as L
-from .utils import local_device
+from .utils import _stream, local_device
 
 TRIM_FRAME, TRIM_HOP = 2048, 512   # librosa.effects.trim defaults
 
@@ -132,10 +132,6 @@ def load_wav(path: str, sr: int) -> np.ndarray:
 _SEG = np.dtype([("sample_off", "<i8"), ("n_samples", "<i4"), ("frame_off", "<i4"), ("n_frames", "<i4"),
                  ("reserved", "<i4")])
 assert _SEG.itemsize == C.sizeof(L.AudioSeg)
-
-
-def _stream(dev):
-    return C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
 
 
 def _ptr(t):

@@ -5,10 +5,12 @@
 * the slack invariant: at every reflect-padded conv, each sample of every length <= T has room for its reflected frames
   inside the layer's extent;
 * the bucket grid of Inferencer.inference_padded is deterministic, covers every pair once and bounds the shape count;
-* invalid lengths and pairs-file errors are rejected before any launch.
+* invalid lengths and pairs-file errors are rejected before any launch;
+* the batch helpers the padded paths share: fill_rows, padded_batch, scatter_crops, exact_buckets and eval_mode.
 """
 import os
 import sys
+import types
 
 import pytest
 import torch
@@ -129,6 +131,51 @@ def test_bucket_grid():
     assert padded_extent(17) == 32 and padded_extent(256) == 256 and padded_extent(257) == 320 and padded_extent(1025) == 1152
     with pytest.raises(ValueError):
         padded_batches([1, 2], [1], 4)
+
+
+def test_batch_helpers():
+    """fill_rows writes the rows in `rows` order (repeats included), keeps the tail and returns the lengths;
+    padded_batch zero-fills with int32 lengths; scatter_crops crops to 8 ceil(T / 8); exact_buckets gives sorted keys
+    with indices in input order; eval_mode restores the training mode and checks the status word on a normal exit only."""
+    from adaptive_voice_conversion_b200.inference import fill_rows, padded_batch, scatter_crops
+    from adaptive_voice_conversion_b200.utils import eval_mode, exact_buckets
+    frames = [torch.full((3, n), float(k + 1)) for k, n in enumerate((5, 2, 7))]
+    dst = torch.full((4, 3, 8), -1.0)
+    assert fill_rows(dst, frames, [2, 0, 2, 1]) == [7, 5, 7, 2]
+    for j, i in enumerate([2, 0, 2, 1]):
+        n = frames[i].shape[1]
+        assert torch.equal(dst[j, :, :n], frames[i]) and bool((dst[j, :, n:] == -1).all())
+    x, lens = padded_batch(frames, [1, 2], 8, "cpu")
+    assert x.shape == (2, 3, 8) and lens.dtype == torch.int32 and lens.tolist() == [2, 7]
+    assert torch.equal(x[0, :, :2], frames[1]) and torch.equal(x[1, :, :7], frames[2])
+    assert not x[0, :, 2:].any() and not x[1, :, 7:].any()
+    out, dec = [None] * 3, torch.arange(2 * 3 * 24.0).view(2, 3, 24)
+    scatter_crops(out, dec, [2, 0], [17, 9])
+    assert out[1] is None and torch.equal(out[2], dec[0].t()) and torch.equal(out[0], dec[1, :, :16].t())
+    assert exact_buckets([3, 1, 3, 1, 2], [1, 1, 1, 2, 1]) == [((1, 1), [1]), ((1, 2), [3]), ((2, 1), [4]), ((3, 1), [0, 2])]
+    g = torch.Generator().manual_seed(0)
+    src, ref = torch.randint(17, 25, (300,), generator=g).tolist(), torch.randint(9, 13, (300,), generator=g).tolist()
+    b = exact_buckets(src, ref)
+    assert [k for k, _ in b] == sorted({*zip(src, ref)}) and sorted(i for _, idx in b for i in idx) == list(range(300))
+    assert all(idx == sorted(idx) and all((src[i], ref[i]) == k for i in idx) for k, idx in b)
+
+    class Model(torch.nn.Module):
+        checks = []
+
+        def engine(self, dev):
+            return types.SimpleNamespace(check_tc_status=lambda: self.checks.append(dev))
+    m = Model()
+    with eval_mode(m, "cuda:0"):
+        assert not m.training
+    assert m.training and m.checks == ["cuda:0"]
+    with pytest.raises(RuntimeError, match="inside"):
+        with eval_mode(m, "cuda:0"):
+            raise RuntimeError("inside")
+    assert m.training and m.checks == ["cuda:0"]
+    m.eval()
+    with eval_mode(m, "cuda:1"):
+        pass
+    assert not m.training and m.checks == ["cuda:0", "cuda:1"]
 
 
 def test_invalid_lengths_rejected_before_any_launch(lib):
