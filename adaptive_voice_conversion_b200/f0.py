@@ -240,14 +240,12 @@ def shifts_from_tracks(conv_tracks, ref_track_sets, limit: float = PITCH_SHIFT_M
     return shifts, info
 
 
-def match_shifts(vocoder: Vocoder, conv_mels, ref_sets, hp: AudioParams, params: F0Params = F0Params(),
-                 frame_budget: int = 32768):
-    """Shifts (semitones) that move each conversion's mean log2 F0 to its reference set's: conv_mels [T, n_mels] and
-    ref_sets (lists of [T, n_mels]) denormalised mels on the device.  Both sides are synthesised unshifted by
-    mel_to_signal at hp's Griffin-Lim settings (in synthesize's chunks) and tracked with the same tracker, as
-    evaluate_f0 does, so both carry the same vocoder artefacts; ``shifts_from_tracks`` gives (shifts, info)."""
-    if len(conv_mels) != len(ref_sets):
-        raise ValueError("match_shifts: one reference set per conversion")
+def unshifted_tracks(vocoder: Vocoder, conv_mels, ref_sets, hp: AudioParams, params: F0Params = F0Params(),
+                     frame_budget: int = 32768):
+    """(conversion tracks, reference track sets): conv_mels [T, n_mels] and ref_sets (lists of [T, n_mels])
+    denormalised mels on the device, all synthesised unshifted by mel_to_signal at hp's Griffin-Lim settings (in
+    synthesize's chunks) and tracked with the same tracker, as evaluate_f0 does, so both carry the same vocoder
+    artefacts."""
     flat = [r for rs in ref_sets for r in rs]
     signals = synthesize(vocoder, list(conv_mels) + flat, hp, frame_budget, semitones=[0.0] * (len(conv_mels) + len(flat)))
     tracks = track_chunks(signals, hp.sr, hp.hop_length, params)
@@ -255,7 +253,84 @@ def match_shifts(vocoder: Vocoder, conv_mels, ref_sets, hp: AudioParams, params:
     for rs in ref_sets:
         refs.append(tracks[k:k + len(rs)])
         k += len(rs)
-    return shifts_from_tracks(tracks[:len(conv_mels)], refs)
+    return tracks[:len(conv_mels)], refs
+
+
+def match_shifts(vocoder: Vocoder, conv_mels, ref_sets, hp: AudioParams, params: F0Params = F0Params(),
+                 frame_budget: int = 32768):
+    """Shifts (semitones) that move each conversion's mean log2 F0 to its reference set's, both tracked unshifted
+    (``unshifted_tracks``); ``shifts_from_tracks`` gives (shifts, info)."""
+    if len(conv_mels) != len(ref_sets):
+        raise ValueError("match_shifts: one reference set per conversion")
+    return shifts_from_tracks(*unshifted_tracks(vocoder, conv_mels, ref_sets, hp, params, frame_budget))
+
+
+# ------------------------------------------------------------------ matching the target's pitch level and range
+def track_profile(tracks):
+    """(log2 mean, log2 std) of the voiced frames of tracks ((f0, voiced) per signal) pooled, or None without one."""
+    m, s, _ = profile([np.log2(f[v]) for f, v in tracks])
+    return None if m is None else (m, s)
+
+
+def mv_shifts(conv_tracks, targets, limit: float = PITCH_SHIFT_MAX):
+    """(per-frame shifts, info) of the mean-and-variance log-F0 transform: conversion i's unshifted track (f0, voiced)
+    of T frames toward targets[i], a target profile (mu_t, sigma_t) of log2 F0 (floats, or float64 arrays of T values
+    for a profile that varies per frame) or None (unmatched).
+
+    With (mu_c, sigma_c) = ``profile`` of the conversion's voiced log2 F0 l, the shift on a voiced frame f is
+    12 (mu_t(f) + sigma_t(f) / sigma_c (l - mu_c) - l), clamped to +-limit; an unvoiced frame's is linearly interpolated
+    in frame index between the nearest voiced frames' and held before the first and after the last.  With sigma_c = 0
+    or fewer than 2 voiced frames every frame gets 12 (mu_t(f) - mu_c), clamped ("mean_only"); with no voiced frame on
+    either side every shift is 0 ("unmatched").  All float64.  info[i] = {"mean_shift" (over the T frames),
+    "voiced_conv", "clamped_frames" (the frames whose shift was clamped: voiced ones, or any with mean_only),
+    "mean_only", "unmatched"}."""
+    shifts, info = [], []
+    for (fc, vc), tgt in zip(conv_tracks, targets):
+        T = len(vc)
+        idx = np.flatnonzero(vc)
+        l = np.log2(np.asarray(fc, np.float64)[idx])
+        mc, sc, nc = profile([l])
+        unmatched = mc is None or tgt is None
+        mean_only = not unmatched and (sc == 0.0 or nc < 2)
+        clamped = 0
+        if unmatched:
+            s = np.zeros(T)
+        else:
+            mu_t, sd_t = (np.broadcast_to(np.asarray(x, np.float64), (T,)) for x in tgt)
+            if mean_only:
+                s = 12.0 * (mu_t - mc)
+                clamped = int(np.count_nonzero(np.abs(s) > limit))
+                s = np.clip(s, -limit, limit)
+            else:
+                sv = 12.0 * (mu_t[idx] + sd_t[idx] / sc * (l - mc) - l)
+                clamped = int(np.count_nonzero(np.abs(sv) > limit))
+                s = np.interp(np.arange(T, dtype=np.float64), idx.astype(np.float64), np.clip(sv, -limit, limit))
+        shifts.append(np.ascontiguousarray(s, np.float64))
+        info.append({"mean_shift": _seq_sum(s) / T if T else 0.0, "voiced_conv": int(nc),
+                     "clamped_frames": clamped, "mean_only": bool(mean_only), "unmatched": bool(unmatched)})
+    return shifts, info
+
+
+def mv_match(vocoder: Vocoder, conv_mels, hp: AudioParams, ref_sets=None, profiles=None,
+             params: F0Params = F0Params(), frame_budget: int = 32768):
+    """``mv_shifts`` of denormalised conversion mels [T, n_mels] (device tensors), each toward one target: where
+    ref_sets[i] is a list of denormalised reference mels, their pooled profile (``track_profile``); where it is None
+    (or ref_sets is omitted), profiles[i], a target profile as ``mv_shifts`` takes it (None: unmatched).  The
+    conversions and the references are tracked by ``unshifted_tracks``, as ``match_shifts`` tracks them.  Returns
+    (shifts, info).  ValueError when a conversion has both a reference set and a profile, or when a list's length is
+    not the number of conversions."""
+    n = len(conv_mels)
+    ref_sets = [None] * n if ref_sets is None else list(ref_sets)
+    profiles = [None] * n if profiles is None else list(profiles)
+    if len(ref_sets) != n or len(profiles) != n:
+        raise ValueError("mv_match: one reference set or profile per conversion")
+    for i, (rs, pr) in enumerate(zip(ref_sets, profiles)):
+        if rs is not None and (pr is not None or not isinstance(rs, list) or not rs):
+            raise ValueError(f"mv_match: conversion {i}: give a non-empty list of reference mels or a profile, not both")
+    conv_tracks, ref_tracks = unshifted_tracks(vocoder, conv_mels, [rs or [] for rs in ref_sets], hp, params,
+                                               frame_budget)
+    return mv_shifts(conv_tracks, [pr if rs is None else track_profile(rt)
+                                   for rs, pr, rt in zip(ref_sets, profiles, ref_tracks)])
 
 
 def select_pairs(cfg, lengths: Mapping[str, int], seed: int = 0, max_pairs: int = 0, n_refs: int = 1):
@@ -288,13 +363,18 @@ def evaluate_f0(model, data: Mapping[str, np.ndarray], attr, seed: int = 0, max_
     tracks this call computes anyway), re-synthesises and re-tracks it and scores it against the same leave-out
     profiles; the entry then holds the shifted scores, "pitch_shift": {"mode", "mean_semitones",
     "mean_abs_semitones", "n_unmatched", "n_clamped"} over the pairs, and "unshifted": the entry of the call without
-    it."""
+    it.  pitch_shift="mv" does the same with ``mv_shifts`` toward the profile of the reference(s)' tracks
+    (``track_profile``); a pair's shift is then the mean of its per-frame shifts (mean_abs_semitones: of their absolute
+    values), n_clamped counts the pairs with a clamped frame, and "pitch_shift" adds n_mean_only, n_clamped_frames and
+    sd_target / sd_target_unshifted: the mean over the scored pairs whose references have a voiced frame of
+    12 |sigma_conv - sigma_target|, sigma the log2 std of the (shifted / unshifted) conversion's voiced frames and of
+    the target profile (None without such a pair)."""
     import time
     from .mcd import converted
     from .speaker_eval import SPK_MAX_EXCLUDE
     cfg = model.config
-    if pitch_shift not in (None, "match"):
-        raise ValueError(f"evaluate_f0: pitch_shift must be None or 'match' (got {pitch_shift!r})")
+    if pitch_shift not in (None, "match", "mv"):
+        raise ValueError(f"evaluate_f0: pitch_shift must be None, 'match' or 'mv' (got {pitch_shift!r})")
     if int(cfg["data_loader"]["frame_size"]) != 1:
         raise ValueError(f"F0 evaluation supports data_loader.frame_size 1 only (got {cfg['data_loader']['frame_size']})")
     if not 1 <= int(n_refs) <= SPK_MAX_EXCLUDE:
@@ -348,8 +428,11 @@ def evaluate_f0(model, data: Mapping[str, np.ndarray], attr, seed: int = 0, max_
     def profile_mean(spk, exclude):
         return profile([logs[v] for v in by_speaker.get(spk, []) if v not in exclude])[0]
 
+    kept = []     # the pairs the last score() call scored
+
     def score(res, conv_tracks):
-        rows, kept = [], []
+        rows = []
+        kept.clear()
         for i, ((u, _), rs) in enumerate(zip(pairs, refs)):
             v = pair_scores(conv_tracks[i], real[u], profile_mean(speaker_of(rs[0]), set(rs)),
                             profile_mean(speaker_of(u), {u}))
@@ -379,7 +462,7 @@ def evaluate_f0(model, data: Mapping[str, np.ndarray], attr, seed: int = 0, max_
     base = dict(res)
     res = score(res, conv_tracks)
     lap("host")
-    if pitch_shift == "match":
+    if pitch_shift is not None:
         # the references' copy-syntheses are the tracks above; a reference too short to be embedded is tracked here
         extra = sorted({v for rs in refs for v in rs} - set(real))
         if extra:
@@ -387,17 +470,37 @@ def evaluate_f0(model, data: Mapping[str, np.ndarray], attr, seed: int = 0, max_
             lap("synthesis")
             real.update(zip(extra, track_chunks(sig, hp.sr, hp.hop_length, params)))
             lap("tracking")
-        shifts, info = shifts_from_tracks(conv_tracks, [[real[v] for v in rs] for rs in refs])
+        ref_tracks = [[real[v] for v in rs] for rs in refs]
+        if pitch_shift == "match":
+            shifts, info = shifts_from_tracks(conv_tracks, ref_tracks)
+            pair_shift = np.asarray(shifts, np.float64)
+            pair_abs = np.abs(pair_shift)
+        else:
+            targets = [track_profile(t) for t in ref_tracks]
+            unshifted_kept = list(kept)
+            shifts, info = mv_shifts(conv_tracks, targets)
+            pair_shift = np.asarray([d["mean_shift"] for d in info], np.float64)
+            pair_abs = np.asarray([_seq_sum(np.abs(s)) / max(len(s), 1) for s in shifts], np.float64)
         sig = synthesize(vocoder, conv_mels, hp, frame_budget, semitones=shifts)
         lap("synthesis")
         shifted = track_chunks(sig, hp.sr, hp.hop_length, params)
         lap("tracking")
         unshifted, res = res, score(base, shifted)
         n = max(len(shifts), 1)
-        res["pitch_shift"] = {"mode": "match", "mean_semitones": _seq_sum(np.asarray(shifts, np.float64)) / n,
-                              "mean_abs_semitones": _seq_sum(np.abs(np.asarray(shifts, np.float64))) / n,
-                              "n_unmatched": sum(d["unmatched"] for d in info),
-                              "n_clamped": sum(d["clamped"] for d in info)}
+        res["pitch_shift"] = {"mode": pitch_shift, "mean_semitones": _seq_sum(pair_shift) / n,
+                              "mean_abs_semitones": _seq_sum(pair_abs) / n,
+                              "n_unmatched": sum(d["unmatched"] for d in info)}
+        if pitch_shift == "match":
+            res["pitch_shift"]["n_clamped"] = sum(d["clamped"] for d in info)
+        else:
+            def sd_gap(tracks, pairs_kept):
+                gaps = [12.0 * abs(track_profile([tracks[i]])[1] - targets[i][1]) for i in pairs_kept
+                        if targets[i] is not None]
+                return _seq_sum(np.asarray(gaps, np.float64)) / len(gaps) if gaps else None
+            res["pitch_shift"].update(n_clamped=sum(d["clamped_frames"] > 0 for d in info),
+                                      n_mean_only=sum(d["mean_only"] for d in info),
+                                      n_clamped_frames=sum(d["clamped_frames"] for d in info),
+                                      sd_target=sd_gap(shifted, kept), sd_target_unshifted=sd_gap(conv_tracks, unshifted_kept))
         res["unshifted"] = unshifted
         lap("host")
     if timings is not None:

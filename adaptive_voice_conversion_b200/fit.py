@@ -308,7 +308,7 @@ def fit_bank(model, bank, mels: Mapping[str, object], steps: int, lr=None, crops
                 "precision": model.engine(dev).precision}
     record = dict(settings, model_fingerprint=model_fingerprint(model), fitted=list(fittable))
     out = SpeakerBank(bank.speakers, codes, bank.n_utts, bank.utterances, bank.fingerprint, bank.n_skipped,
-                      fitted=record)
+                      fitted=record, pitch=bank.pitch)     # pitch profiles describe the recordings, not the codes
     speakers = {}
     for s in bank.speakers:
         p = per[s]

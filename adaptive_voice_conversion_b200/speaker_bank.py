@@ -20,6 +20,13 @@ whose fingerprint does not match the model.
 A bank whose codes were fitted to the model (``fit.fit_bank``) also carries a ``fitted`` record: the run's steps and
 settings and ``model_fingerprint``, a sha256 of the content encoder and the decoder the codes were fitted through.
 ``load`` refuses such a bank against a model whose record does not match; a bank without the record loads as before.
+
+A bank built with pitch profiles (``build_pitch_profiles``, speaker_bank.py -f0) carries a ``pitch`` record: per
+speaker the ``f0.profile`` (log2 mean and std, voiced and total frames) of the voiced log2 F0 of that speaker's pooled
+utterances, each copy-synthesised from its denormalised mel by the project's Griffin-Lim vocoder (untrimmed) and
+tracked by ``f0.track_chunks``, as ``evaluate_f0`` makes its speaker profiles; and the tracker and Griffin-Lim settings
+used.  Profiles describe recordings, not codes, so fitting keeps the record.  ``pitch_profile`` and
+``morph_pitch_profile`` give the target profile of a spec or a morph, which ``f0.mv_shifts`` moves conversions toward.
 """
 from __future__ import annotations
 
@@ -146,17 +153,50 @@ def morph_table(bank: "SpeakerBank", keyframes: Sequence[tuple], n_frames: int, 
     return bank.codes[rows].contiguous(), torch.from_numpy(w)
 
 
+PITCH_LISTS = ("log2_mean", "log2_std", "voiced", "frames")
+
+
+def check_pitch(pitch, n_speakers: int) -> dict:
+    """A copy of a bank's pitch record after checking it: the PITCH_LISTS of n_speakers entries each, voiced and frames
+    integers with 0 <= voiced <= frames, mean and std finite (std >= 0) exactly where voiced > 0 and None elsewhere,
+    and the "tracker" and "griffin_lim" settings dicts.  ValueError naming what is wrong."""
+    if not isinstance(pitch, dict):
+        raise ValueError("SpeakerBank: the pitch record must be a dict")
+    for k in PITCH_LISTS:
+        if not isinstance(pitch.get(k), (list, tuple)) or len(pitch[k]) != n_speakers:
+            raise ValueError(f"SpeakerBank: pitch record: {k} must list the {n_speakers} speakers")
+    for k in ("tracker", "griffin_lim"):
+        if not isinstance(pitch.get(k), dict):
+            raise ValueError(f"SpeakerBank: pitch record: {k} settings missing")
+    for i, (m, sd, nv, nf) in enumerate(zip(*(pitch[k] for k in PITCH_LISTS))):
+        if not all(isinstance(n, int) and not isinstance(n, bool) for n in (nv, nf)) or not 0 <= nv <= nf:
+            raise ValueError(f"SpeakerBank: pitch record of speaker {i}: voiced {nv!r} / frames {nf!r} must be integers "
+                             f"with 0 <= voiced <= frames")
+        if nv == 0:
+            if m is not None or sd is not None:
+                raise ValueError(f"SpeakerBank: pitch record of speaker {i}: a mean and std without a voiced frame")
+            continue
+        if not all(isinstance(x, float) and math.isfinite(x) for x in (m, sd)) or sd < 0:
+            raise ValueError(f"SpeakerBank: pitch record of speaker {i}: mean {m!r} and std {sd!r} must be finite "
+                             f"floats, the std >= 0")
+    out = dict(pitch)
+    out.update({k: list(pitch[k]) for k in PITCH_LISTS}, tracker=dict(pitch["tracker"]),
+               griffin_lim=dict(pitch["griffin_lim"]))
+    return out
+
+
 class SpeakerBank:
     """Per-speaker codes of one speaker encoder.
 
     speakers: names in sorted order; codes: float32 [S, c_out] (row s is speakers[s]'s); n_utts[s]: the utterances
     pooled into code s, which are utterances[s] (sorted ids); n_skipped: utterances too short to embed; fingerprint:
     the speaker encoder's (``fingerprint``); fitted: None, or the record of the fitting run that tuned the codes to a
-    content encoder and decoder (``fit.fit_bank``; plain values only, with "model_fingerprint")."""
+    content encoder and decoder (``fit.fit_bank``; plain values only, with "model_fingerprint"); pitch: None, or the
+    speakers' pitch profiles (``build_pitch_profiles``; checked by ``check_pitch``)."""
 
     def __init__(self, speakers: Sequence[str], codes: torch.Tensor, n_utts: Sequence[int],
                  utterances: Sequence[Sequence[str]], fingerprint: str, n_skipped: int = 0,
-                 fitted: Optional[dict] = None):
+                 fitted: Optional[dict] = None, pitch: Optional[dict] = None):
         speakers = [str(s) for s in speakers]
         if len(set(speakers)) != len(speakers) or list(speakers) != sorted(speakers):
             raise ValueError("SpeakerBank: speakers must be unique and sorted")
@@ -175,6 +215,7 @@ class SpeakerBank:
         if fitted is not None and not isinstance(fitted.get("model_fingerprint"), str):
             raise ValueError("SpeakerBank: a fitted record needs its model_fingerprint")
         self.fitted = None if fitted is None else dict(fitted)
+        self.pitch = None if pitch is None else check_pitch(pitch, len(speakers))
         self._index = {s: i for i, s in enumerate(speakers)}
 
     def __len__(self):
@@ -208,14 +249,60 @@ class SpeakerBank:
             wsum += w
         return (acc / wsum).to(dtype=torch.float32, device=self.codes.device)
 
+    def with_pitch(self, pitch: Optional[dict]) -> "SpeakerBank":
+        """This bank with the pitch record `pitch` (the codes shared)."""
+        return SpeakerBank(self.speakers, self.codes, self.n_utts, self.utterances, self.fingerprint, self.n_skipped,
+                           fitted=self.fitted, pitch=pitch)
+
+    def _pitch_rows(self, names):
+        if self.pitch is None:
+            raise ValueError("the bank has no pitch profiles: rebuild it with speaker_bank.py -f0")
+        rows = [self.index(n) for n in names]
+        return [(self.pitch["log2_mean"][r], self.pitch["log2_std"][r]) for r in rows]
+
+    def pitch_profile(self, spec: str):
+        """(log2 mean, log2 std) of the target a spec names, or None (unmatched) when a speaker of positive weight has
+        no voiced frame: p225's own profile, or for ``"p225:0.7,p226:0.3"`` mu = sum_i w_i mu_i / sum_i w_i and the
+        same for the std, in float64 with terms in spec order and zero weights skipped (``code``'s straight line).
+        ValueError for a bank without a pitch record or a bad spec."""
+        parts = parse_spec(spec)
+        profs = self._pitch_rows([n for n, _ in parts])
+        mu = sd = wsum = 0.0
+        for (_, w), (m, s) in zip(parts, profs):
+            if w == 0:
+                continue
+            if m is None:
+                return None
+            mu, sd, wsum = mu + w * m, sd + w * s, wsum + w
+        return mu / wsum, sd / wsum
+
+    def morph_pitch_profile(self, keyframes: Sequence[tuple], n_frames: int, frames_per_second: float):
+        """(log2 mean, log2 std) float64 [n_frames] of a morph's target per frame, or None (unmatched) when a speaker
+        of positive weight on some frame has no voiced frame: with w_k(f) = ``morph_weights`` (the float32 table the
+        decoder gets), mu(f) = sum_k w_k(f) mu_k / sum_k w_k(f) in float64, terms in order of first mention, and the same
+        for the std.  A morph held on one speaker gives that speaker's profile on every frame exactly."""
+        names, w = morph_weights(keyframes, n_frames, frames_per_second)
+        profs = self._pitch_rows(names)
+        w = w.astype(np.float64)
+        mu, sd, wsum = np.zeros(w.shape[1]), np.zeros(w.shape[1]), np.zeros(w.shape[1])
+        for wk, (m, s) in zip(w, profs):
+            if not wk.any():
+                continue
+            if m is None:
+                return None
+            mu, sd, wsum = mu + wk * m, sd + wk * s, wsum + wk
+        return mu / wsum, sd / wsum
+
     def save(self, path: str):
-        """torch.save of plain tensors, lists and strings (loadable with weights_only=True).  The "fitted" entry is
-        written only for a fitted bank."""
+        """torch.save of plain tensors, lists and strings (loadable with weights_only=True).  The "fitted" and "pitch"
+        entries are written only for a fitted bank and one with pitch profiles."""
         d = {"format": FORMAT, "speakers": list(self.speakers), "codes": self.codes.detach().cpu().contiguous(),
              "n_utts": list(self.n_utts), "utterances": [list(u) for u in self.utterances],
              "fingerprint": self.fingerprint, "n_skipped": self.n_skipped}
         if self.fitted is not None:
             d["fitted"] = dict(self.fitted)
+        if self.pitch is not None:
+            d["pitch"] = self.pitch
         torch.save(d, path)
 
     @classmethod
@@ -239,8 +326,14 @@ class SpeakerBank:
                                  f"{str(fitted.get('model_fingerprint'))[:12]}..., the model's {mf[:12]}...); they are "
                                  f"tuned to that model")
         dev = next(model.parameters()).device
+        pitch = d.get("pitch")
+        if pitch is not None:
+            try:
+                pitch = check_pitch(pitch, len(d["speakers"]))
+            except ValueError as e:
+                raise ValueError(f"{path}: {e}") from None
         return cls(d["speakers"], d["codes"].to(dev), d["n_utts"], d["utterances"], d["fingerprint"], d["n_skipped"],
-                   fitted=fitted)
+                   fitted=fitted, pitch=pitch)
 
 
 def bank_order(ids: Sequence[str], lengths: Mapping[str, int], min_len: int,
@@ -288,6 +381,73 @@ def build_bank(model, mels: Mapping[str, object], speaker_of: Callable[[str], st
         offsets = torch.tensor([0] + [len(us) for us in utts], dtype=torch.int64).cumsum(0)
         codes = model.speaker_codes_from_sums(sums, counts, groups=offsets.to(dev))
     return SpeakerBank(speakers, codes, [len(us) for us in utts], utts, fingerprint(model), skipped)
+
+
+def build_pitch_profiles(bank: SpeakerBank, mels: Mapping[str, object], attr, hp=None, params=None,
+                         frame_budget: int = 32768, device=None, timings: dict = None) -> dict:
+    """The pitch record of `bank` (the module docstring) from mels: utterance id -> attr-normalised [T, n_mels] mel
+    (a tensor or an array) of at least every pooled utterance.  Each pooled utterance, in the bank's order, is
+    denormalised with attr (mel * std + mean), copy-synthesised by ``f0.synthesize`` at hp's Griffin-Lim settings
+    (default AudioParams(); unshifted, n_mels the mels') and tracked by ``f0.track_chunks`` with params (default
+    F0Params()), in chunks of at most frame_budget frames: only one chunk's mels and signals are on the device at a
+    time, and its tracks go to the host before the next (an utterance's bits do not depend on its chunk).  timings (a dict) receives the wall seconds of synthesis, tracking and host work, each ended by a
+    device synchronise."""
+    import time
+    from dataclasses import replace
+    from .f0 import F0Params, profile, synthesize, track_chunks
+    from .vocoder import AudioParams, Vocoder
+    hp = AudioParams() if hp is None else hp
+    params = F0Params() if params is None else params
+    dev = torch.device(device) if device is not None else bank.codes.device
+    flat = bank.utterance_ids()
+    missing = [u for u in flat if u not in mels]
+    if missing:
+        raise ValueError(f"build_pitch_profiles: {len(missing)} pooled utterances have no mel (e.g. {missing[0]})")
+    n_mels = int(mels[flat[0]].shape[1])
+    hp = replace(hp, n_mels=n_mels, pitch_shift=0.0)
+    mean = torch.as_tensor(np.asarray(attr["mean"], np.float32).reshape(-1)).to(dev)
+    std = torch.as_tensor(np.asarray(attr["std"], np.float32).reshape(-1)).to(dev)
+    if mean.numel() != n_mels or std.numel() != n_mels:
+        raise ValueError(f"build_pitch_profiles: attr mean / std have {mean.numel()} / {std.numel()} entries, the mels "
+                         f"{n_mels}")
+    clock = {"synthesis": 0.0, "tracking": 0.0, "host": 0.0}
+    t0 = time.perf_counter()
+
+    def lap(k):
+        nonlocal t0
+        torch.cuda.synchronize(dev)
+        t1 = time.perf_counter()
+        clock[k] += t1 - t0
+        t0 = t1
+    vocoder = Vocoder(hp=hp, device=dev)
+    tracks, k = [], 0
+    while k < len(flat):      # one chunk of at most frame_budget frames on the device at a time (one longer mel alone)
+        j, frames = k + 1, int(mels[flat[k]].shape[0])
+        while j < len(flat) and frames + int(mels[flat[j]].shape[0]) <= frame_budget:
+            frames += int(mels[flat[j]].shape[0])
+            j += 1
+        chunk = [(m if isinstance(m, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(m, np.float32))).to(dev)
+                 * std + mean for m in (mels[u] for u in flat[k:j])]
+        signals = synthesize(vocoder, chunk, hp, frame_budget)
+        lap("synthesis")
+        tracks.extend(track_chunks(signals, hp.sr, hp.hop_length, params))
+        del chunk, signals
+        lap("tracking")
+        k = j
+    rec = {k: [] for k in PITCH_LISTS}
+    k = 0
+    for us in bank.utterances:
+        ts = tracks[k:k + len(us)]
+        k += len(us)
+        m, sd, nv = profile([np.log2(f[v]) for f, v in ts])
+        for key, val in zip(PITCH_LISTS, (m, sd, int(nv), sum(len(v) for _, v in ts))):
+            rec[key].append(val)
+    rec["tracker"] = params.settings(hp.sr, hp.hop_length)
+    rec["griffin_lim"] = {"n_iter": int(hp.n_iter), "momentum": float(hp.momentum), "init": hp.gl_init}
+    lap("host")
+    if timings is not None:
+        timings.update(clock)
+    return check_pitch(rec, len(bank))
 
 
 def check_disjoint(bank: SpeakerBank, utterance_ids) -> None:

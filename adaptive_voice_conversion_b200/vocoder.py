@@ -12,7 +12,7 @@ launch per kernel.  No kernel uses atomics, so each utterance gets the bits it g
 ``Vocoder`` has the duck type ``Inferencer`` accepts (``get_spectrograms(path)``, ``melspectrogram2wav(mel)``, numpy
 in and out) and the batched device forms ``wav_to_mel`` / ``mel_to_wav`` (``mel_to_signal`` leaves the synthesis
 untrimmed, aligned with the mel frames).  ``pitch_shift`` transposes the linear magnitudes before Griffin-Lim
-(``AudioParams.pitch_shift`` or ``semitones=``), keeping the frame grid.
+(``AudioParams.pitch_shift`` or ``semitones=``, per utterance or per frame), keeping the frame grid.
 """
 from __future__ import annotations
 
@@ -371,33 +371,65 @@ def _mel_project(x, mat, direction, hp: AudioParams):
 PITCH_SHIFT_MAX = 24.0   # semitones: two octaves either way
 
 
-def _semitones(semitones, n: int, what: str) -> list:
-    """Per-utterance shifts of a float or one value per utterance; ValueError outside [-24, 24] or not finite."""
-    s = [float(semitones)] * n if np.ndim(semitones) == 0 else [float(v) for v in semitones]
-    if len(s) != n:
-        raise ValueError(f"{what}: {len(s)} shifts for {n} utterances")
-    for i, v in enumerate(s):
-        if not np.isfinite(v) or abs(v) > PITCH_SHIFT_MAX:
+def _semitones(semitones, n: int, what: str, frames=None) -> list:
+    """Shifts of n utterances from a float or one entry per utterance, an entry being a float or a 1-D array / tensor
+    of one value per frame (frames[i] of them): a float per constant utterance, a float64 array per per-frame one.
+    ValueError naming the utterance for a value outside [-24, 24] or not finite, or a per-frame entry of the wrong
+    length."""
+    if isinstance(semitones, torch.Tensor):
+        semitones = semitones.detach().cpu().numpy()
+    if isinstance(semitones, (list, tuple)) or (isinstance(semitones, np.ndarray) and semitones.ndim > 0):
+        entries = list(semitones)     # not np.ndim: a list mixing floats and arrays is ragged
+    else:
+        entries = [semitones] * n
+    if len(entries) != n:
+        raise ValueError(f"{what}: {len(entries)} shifts for {n} utterances")
+    out = []
+    for i, e in enumerate(entries):
+        if isinstance(e, torch.Tensor):
+            e = e.detach().cpu().numpy()
+        if np.ndim(e) == 0:
+            v = float(e)
+            bad = not np.isfinite(v) or abs(v) > PITCH_SHIFT_MAX
+            out.append(v)
+        else:
+            v = np.asarray(e, np.float64)
+            if v.ndim != 1 or frames is None or len(v) != int(frames[i]):
+                want = "one per utterance" if frames is None else f"{int(frames[i])}"
+                raise ValueError(f"{what}: utterance {i}: {v.shape} per-frame shifts, expected {want} frames")
+            ok = np.isfinite(v) & (np.abs(v) <= PITCH_SHIFT_MAX)
+            bad = not ok.all()
+            if bad:
+                v = f"{v[~ok][0]} at frame {int(np.flatnonzero(~ok)[0])}"
+            out.append(v)
+        if bad:
             raise ValueError(f"{what}: utterance {i}: pitch shift must be finite and in [-{PITCH_SHIFT_MAX:g}, "
                              f"{PITCH_SHIFT_MAX:g}] semitones (got {v})")
-    return s
+    return out
+
+
+def _ratio(v) -> float:
+    """2^(v/12) in float64: the one place a shift becomes a ratio."""
+    return 2.0 ** (v / 12.0)
 
 
 def pitch_shift(mags, semitones, hp: AudioParams = AudioParams()):
     """Formant-preserving pitch shift of linear magnitudes [T, n_bins] per utterance by ``semitones`` (a float, or one
-    per utterance), in one avc_pitch_shift launch: the harmonics (the cepstrum above ``hp.ps_lifter``) move by the
-    ratio 2^(s/12), the envelope stays, the frame grid and duration are unchanged.  An utterance with shift 0 is
-    copied bit for bit."""
+    entry per utterance: a float or T values, one per frame), in one avc_pitch_shift launch: the harmonics (the
+    cepstrum above ``hp.ps_lifter``) move by the ratio float32(2^(s/12)) of each frame's shift, the envelope stays,
+    the frame grid and duration are unchanged.  A frame with shift 0 is copied bit for bit, and a per-frame entry of
+    equal values gives the bits of that value as a float."""
     if not mags:
         raise ValueError("pitch_shift: empty batch")
-    s = _semitones(semitones, len(mags), "pitch_shift")
+    lens = [int(m.shape[0]) for m in mags]
+    s = _semitones(semitones, len(mags), "pitch_shift", lens)
     dev = mags[0].device
     S = torch.cat([m.float() for m in mags]).contiguous()
     if S.dim() != 2 or S.shape[1] != hp.n_bins:
         raise ValueError(f"pitch_shift: magnitudes have shape {tuple(S.shape)}, n_fft={hp.n_fft} gives {hp.n_bins} bins")
-    lens = [int(m.shape[0]) for m in mags]
-    ratio = torch.tensor([2.0 ** (v / 12.0) for v in s], dtype=torch.float32).to(dev)
-    ratio = torch.repeat_interleave(ratio, torch.tensor(lens).to(dev), output_size=S.shape[0])
+    ratio = np.concatenate([np.full(T, _ratio(v), np.float64) if isinstance(v, float) else
+                            np.array([_ratio(x) for x in v.tolist()], np.float64) for v, T in zip(s, lens)])
+    ratio = torch.from_numpy(ratio.astype(np.float32)).to(dev)
     out = torch.empty_like(S)
     L.check(L.load().avc_pitch_shift(_ptr(S), _ptr(ratio), _ptr(out), S.shape[0], hp.n_bins, int(hp.ps_lifter),
                                      _stream(dev)), "avc_pitch_shift")
@@ -439,17 +471,19 @@ class Vocoder:
                       what: str = "mel_to_signal", *, semitones=None):
         """Normalised mels [T, n_mels] (device tensors) -> untrimmed float32 signals of hop * (T - 1) samples, sample
         f * hop at mel frame f: amplitude, mel-to-linear, pitch shift, Griffin-Lim, de-emphasis.  ``n_iter``,
-        ``momentum``, ``init`` and ``semitones`` (a float or one per utterance) default to ``hp.n_iter``,
-        ``hp.momentum``, ``hp.gl_init`` and ``hp.pitch_shift``.  With every shift 0 no shift is launched."""
+        ``momentum``, ``init`` and ``semitones`` (a float, or one entry per utterance: a float or T values, one per
+        mel frame, as ``pitch_shift``) default to ``hp.n_iter``, ``hp.momentum``, ``hp.gl_init`` and
+        ``hp.pitch_shift``.  With every shift 0 no shift is launched."""
         hp = self.hp
         for i, m in enumerate(mels):
             if m.dim() != 2 or m.shape[1] != hp.n_mels:
                 raise ValueError(f"{what}: utterance {i} has shape {tuple(m.shape)}, expected [T, {hp.n_mels}]")
         _init(init, hp)
         _frames(mels, hp, what)
-        s = _semitones(hp.pitch_shift if semitones is None else semitones, len(mels), what)
+        s = _semitones(hp.pitch_shift if semitones is None else semitones, len(mels), what,
+                       [int(m.shape[0]) for m in mels])
         mags = self.mel_to_mag(mels)
-        if any(v != 0.0 for v in s):
+        if any(np.any(v != 0.0) for v in s):
             mags = pitch_shift(mags, s, hp)
         return deemphasis(griffin_lim(mags, hp, n_iter, momentum, init), hp.preemphasis)
 

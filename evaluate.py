@@ -3,7 +3,7 @@ data directory (adaptive_voice_conversion_b200/evaluate.py gives the definition)
 
     python evaluate.py -c config.yaml -m model.ckpt -d data/ [-eval_sets in_test,out_test] [-o eval.json]
                        [-mcd -transcripts VCTK-Corpus/txt [-attr data/attr.pkl] [-mcd_dims 24]] [-spk]
-                       [-f0 [-gl_iters 100] [-gl_momentum 0] [-gl_init zero] [-pitch_shift match]]
+                       [-f0 [-gl_iters 100] [-gl_momentum 0] [-gl_init zero] [-pitch_shift match|mv]]
                        [-max_pairs 0] [-seed 0] [-n_refs 1] [-bank bank.pt]
 
 The checkpoint is loaded strictly (reference checkpoints too, and the `sn: True` layout).  Each set's losses are
@@ -26,6 +26,9 @@ output, not of the original recordings.
 -pitch_shift match (with -f0) also shifts each conversion toward its reference(s)' mean log2 F0 (f0.match_shifts),
 re-synthesises and re-scores it against the same leave-out profiles: the "f0" entry then holds the shifted scores,
 "pitch_shift" (mean and mean absolute shift, unmatched and clamped pairs) and "unshifted", the scores without it.
+-pitch_shift mv shifts each conversion frame by frame toward the mean and std of its reference(s)' log2 F0
+(f0.mv_shifts) instead; "pitch_shift" then also holds n_mean_only, n_clamped_frames, and sd_target and
+sd_target_unshifted, the mean of 12 |log2 std of the conversion's voiced F0 - the references'| with and without it.
 -n_refs K (default 1) converts with K references of the target speaker per conversion, their speaker codes pooled
 (-mcd and -spk): the first reference is drawn as with one, the K - 1 others from a second generator seeded with
 seed + 1; sim_target then skips all K.  With K > 1 each result also reports n_refs and n_few (conversions dropped for
@@ -66,8 +69,9 @@ def main(argv=None):
     p.add_argument("-gl_iters", default=100, type=int, help="Griffin-Lim iterations of the synthesis (-f0)")
     p.add_argument("-gl_momentum", default=0.0, type=float, help="fast Griffin-Lim momentum in [0, 1) (-f0)")
     p.add_argument("-gl_init", default="zero", choices=["zero", "pghi"], help="Griffin-Lim start phase (-f0)")
-    p.add_argument("-pitch_shift", default=None, choices=["match"],
-                   help="also score each conversion shifted to its reference(s)' pitch level (-f0)")
+    p.add_argument("-pitch_shift", default=None, choices=["match", "mv"],
+                   help="also score each conversion shifted to its reference(s)' pitch level (match) or level and "
+                        "range (mv) (-f0)")
     p.add_argument("-max_pairs", type=int, default=0,
                    help="keep at most this many triplets (-mcd) and conversion pairs (-spk) per set, 0 = all; "
                         "-f0 scores the -spk pairs")
@@ -160,8 +164,13 @@ def main(argv=None):
                   f"({len(r['speakers'])} target speakers)")
             if args.pitch_shift:
                 ps = r["pitch_shift"]
-                print(f"{s}: f0 pitch_shift match mean={ps['mean_semitones']:+.4f} mean_abs={ps['mean_abs_semitones']:.4f} "
-                      f"n_unmatched={ps['n_unmatched']} n_clamped={ps['n_clamped']} (unshifted st_target="
+                mv = "" if args.pitch_shift == "match" else (
+                    f" n_mean_only={ps['n_mean_only']} n_clamped_frames={ps['n_clamped_frames']} sd_target="
+                    + ("n/a" if ps["sd_target"] is None else f"{ps['sd_target']:.4f}") + " (unshifted sd_target="
+                    + ("n/a" if ps["sd_target_unshifted"] is None else f"{ps['sd_target_unshifted']:.4f}") + ")")
+                print(f"{s}: f0 pitch_shift {args.pitch_shift} mean={ps['mean_semitones']:+.4f} "
+                      f"mean_abs={ps['mean_abs_semitones']:.4f} n_unmatched={ps['n_unmatched']} "
+                      f"n_clamped={ps['n_clamped']}{mv} (unshifted st_target="
                       + ("n/a" if not r["unshifted"]["n"] else f"{r['unshifted']['st_target']:.4f}") + ")")
     if args.output:
         with open(args.output, "w") as f:

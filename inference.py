@@ -63,6 +63,19 @@ and in -pairs with file and set targets; banked speakers and morphs have no mels
 @SPEC lines are refused, as is a shift of a .npy output (a mel is not synthesised):
 
     python inference.py -c config.yaml -m model.ckpt -a attr.pkl -pairs pairs.txt -o out_dir -pitch_shift match
+
+-pitch_shift mv matches the pitch range as well as the level, frame by frame (f0.mv_shifts): on each voiced frame the
+conversion's log2 F0 l becomes mu_t + sigma_t / sigma_c (l - mu_c), (mu_c, sigma_c) the mean and std of the
+conversion's voiced log2 F0 and (mu_t, sigma_t) the target's; unvoiced frames take the shift interpolated between
+their voiced neighbours, every shift is clamped to [-24, 24], and with too little voicing it falls back to match's
+constant shift (mean only) or to 0 (unmatched).  It serves every target: a -t file or set and -pairs file and set
+lines (their profile tracked as match does), and banked speakers, mixes (-speaker, @SPEC lines) and -morph (a
+profile per frame), whose profiles the bank records when speaker_bank.py -f0 built it.  A bank without them, and a
+.npy output, are refused before anything runs; a note is printed when the Griffin-Lim settings differ from those the
+bank's profiles were synthesised with:
+
+    python inference.py -c config.yaml -m model.ckpt -a attr.pkl -s src.wav -bank bank.pt -speaker p226 -o out.wav \
+        -pitch_shift mv
 """
 import os
 from argparse import ArgumentParser
@@ -187,6 +200,29 @@ def refuse_bank_targets(pairs, path):
                              f"(@{t.spec}) has none")
 
 
+def refuse_unprofiled_bank(path):
+    """ValueError when the bank file at `path` has no pitch profiles (read on the host, before any model or GPU work):
+    -pitch_shift mv needs them for a banked target."""
+    d = torch.load(path, map_location="cpu", weights_only=True)
+    if not isinstance(d, dict) or d.get("pitch") is None:
+        raise ValueError(f"{path}: the bank has no pitch profiles, which -pitch_shift mv needs for a banked target; "
+                         f"rebuild it with speaker_bank.py -f0")
+
+
+def print_mv(names, info, bank=None, hp=None):
+    """One line per conversion of -pitch_shift mv, and a note when hp's Griffin-Lim settings are not those of the
+    bank's pitch profiles."""
+    if bank is not None and bank.pitch is not None:
+        gl = {"n_iter": int(hp.n_iter), "momentum": float(hp.momentum), "init": hp.gl_init}
+        if gl != bank.pitch["griffin_lim"]:
+            print(f"note: the bank's pitch profiles were synthesised with Griffin-Lim {bank.pitch['griffin_lim']}, "
+                  f"these conversions with {gl}")
+    for name, d in zip(names, info):
+        note = (" (unmatched: no voiced frame)" if d["unmatched"] else " (mean only)" if d["mean_only"] else "")
+        print(f"{name}: pitch shift mv mean {d['mean_shift']:+.3f} semitones, voiced frames {d['voiced_conv']} "
+              f"conversion, {d['clamped_frames']} clamped{note}")
+
+
 def print_matches(names, info):
     for name, d in zip(names, info):
         note = " (unmatched: no voiced frame)" if d["unmatched"] else " (clamped)" if d["clamped"] else ""
@@ -201,13 +237,15 @@ def run_pairs(args, config):
     pairs = read_pairs(args.pairs, bank=bool(args.bank))
     if args.semitones == "match":
         refuse_bank_targets(pairs, args.pairs)
+    if args.semitones == "mv" and any(isinstance(t, BankTarget) and is_wav(name) for _, _, t, name in pairs):
+        refuse_unprofiled_bank(args.bank)
     os.makedirs(args.output, exist_ok=True)
     dev = local_device()
     files = sorted({p for _, s, t, _ in pairs
                     for p in (s,) + ((t,) if isinstance(t, str) else () if isinstance(t, BankTarget) else t)})
     need_voc = any(is_wav(f) for f in files) or any(is_wav(name) for *_, name in pairs)
     hp = AudioParams(n_iter=args.gl_iters, momentum=args.gl_momentum, gl_init=args.gl_init,
-                     pitch_shift=0.0 if args.semitones == "match" else args.semitones)
+                     pitch_shift=0.0 if isinstance(args.semitones, str) else args.semitones)
     vocoder = Vocoder(n_mels=config["SpeakerEncoder"]["c_in"] // config["data_loader"]["frame_size"],
                       hp=hp) if need_voc else None
     wavs = [f for f in files if is_wav(f)]
@@ -244,6 +282,15 @@ def run_pairs(args, config):
                                     [[raw[p] for p in ((pairs[i][2],) if isinstance(pairs[i][2], str) else pairs[i][2])]
                                      for i in to_wav], vocoder.hp)
         print_matches([pairs[i][3] for i in to_wav], info)
+    if args.semitones == "mv" and to_wav:
+        from adaptive_voice_conversion_b200.f0 import mv_match
+        tgts = [pairs[i][2] for i in to_wav]
+        banked = [isinstance(t, BankTarget) for t in tgts]
+        shifts, info = mv_match(vocoder, [decs[i].contiguous() for i in to_wav], vocoder.hp,
+                                ref_sets=[None if b else [raw[p] for p in ((t,) if isinstance(t, str) else t)]
+                                          for t, b in zip(tgts, banked)],
+                                profiles=[bank.pitch_profile(t.spec) if b else None for t, b in zip(tgts, banked)])
+        print_mv([pairs[i][3] for i in to_wav], info, bank if any(banked) else None, vocoder.hp)
     ys = []
     if to_wav:   # a fixed shift is the vocoder's hp.pitch_shift
         ys = vocoder.mel_to_wav([decs[i].contiguous() for i in to_wav], **({} if shifts is None else {"semitones": shifts}))
@@ -260,11 +307,13 @@ def load_bank(path, model):
 
 
 def pitch_shift_arg(p, args):
-    """args.semitones: "match" or the -pitch_shift float; p.error for a value that is not finite or outside [-24, 24],
-    match with -speaker or -morph, and a non-zero shift of a single .npy output."""
+    """args.semitones: "match", "mv" or the -pitch_shift float; p.error for a value that is not finite or outside
+    [-24, 24], match with -speaker or -morph, and a non-zero shift of a single .npy output."""
     from adaptive_voice_conversion_b200.vocoder import PITCH_SHIFT_MAX
     v = str(args.pitch_shift)
-    if v == "match":
+    if v == "mv":
+        args.semitones = "mv"
+    elif v == "match":
         args.semitones = "match"
         if args.speaker is not None or args.morph is not None:
             p.error("-pitch_shift match needs the target's recordings: banked speakers (-speaker, -morph) have none")
@@ -272,7 +321,7 @@ def pitch_shift_arg(p, args):
         try:
             args.semitones = float(v)
         except ValueError:
-            p.error(f"-pitch_shift must be a number of semitones or 'match' (got {v!r})")
+            p.error(f"-pitch_shift must be a number of semitones or 'match' or 'mv' (got {v!r})")
         if not np.isfinite(args.semitones) or abs(args.semitones) > PITCH_SHIFT_MAX:
             p.error(f"-pitch_shift must be finite and in [-{PITCH_SHIFT_MAX:g}, {PITCH_SHIFT_MAX:g}] semitones (got {v})")
     if args.semitones != 0.0 and not args.pairs and not is_wav(args.output):
@@ -327,20 +376,14 @@ def parser():
     p.add_argument("-speaker", help="banked target: NAME or a weighted mix NAME:W,NAME:W,... (needs -bank)")
     p.add_argument("-morph", nargs="+", metavar="SPEC@SECONDS",
                    help="time-varying target: banked speakers or mixes at keyframe times, interpolated (needs -bank)")
-    p.add_argument("-pitch_shift", default="0", metavar="{SEMITONES,match}",
-                   help="transpose every .wav output by SEMITONES in [-24, 24] (formant-preserving), or 'match' each "
-                        "conversion's pitch level to its -t target's")
+    p.add_argument("-pitch_shift", default="0", metavar="{SEMITONES,match,mv}",
+                   help="transpose every .wav output by SEMITONES in [-24, 24] (formant-preserving), 'match' each "
+                        "conversion's pitch level to its -t target's, or 'mv': level and range to any target's")
     return p
 
 
-if __name__ == "__main__":
-    p = parser()
-    args = p.parse_args()
-    check_args(p, args)
-    config = load_config(args.config)
-    if args.pairs:
-        run_pairs(args, config)
-        raise SystemExit(0)
+def run_single(args, config):
+    """One conversion (-t, -bank -speaker or -bank -morph; see the module docstring)."""
     targets = args.target or [None]
     args.target = targets[0] if len(targets) == 1 else targets
     vocoder = None
@@ -348,29 +391,44 @@ if __name__ == "__main__":
         from adaptive_voice_conversion_b200.vocoder import AudioParams, Vocoder
         vocoder = Vocoder(n_mels=config["SpeakerEncoder"]["c_in"] // config["data_loader"]["frame_size"],
                           hp=AudioParams(n_iter=args.gl_iters, momentum=args.gl_momentum, gl_init=args.gl_init,
-                                         pitch_shift=0.0 if args.semitones == "match" else args.semitones))
+                                         pitch_shift=0.0 if isinstance(args.semitones, str) else args.semitones))
     match = args.semitones == "match" and is_wav(args.output)
-    inf = Inferencer(config=config, args=args, vocoder=vocoder if is_wav(args.output) and not match else None)
+    mv = args.semitones == "mv" and is_wav(args.output)
+    inf = Inferencer(config=config, args=args, vocoder=vocoder if is_wav(args.output) and not (match or mv) else None)
+    bank = load_bank(args.bank, inf.model) if args.bank else None
+    dev = local_device()
+
+    def synthesise_mv(mel, ref_sets=None, profiles=None):
+        """The .wav of a denormalised mel shifted by mv toward its reference mels or a target profile."""
+        from adaptive_voice_conversion_b200.f0 import mv_match
+        m = torch.from_numpy(np.ascontiguousarray(mel, np.float32)).to(dev)
+        shifts, info = mv_match(vocoder, [m], vocoder.hp, ref_sets=ref_sets, profiles=profiles)
+        print_mv([args.output], info, bank if ref_sets is None else None, vocoder.hp)
+        return vocoder.mel_to_wav([m], semitones=shifts)[0].cpu().numpy()
 
     def read(path):
         return vocoder.get_spectrograms(path)[0] if is_wav(path) else np.load(path).astype(np.float32)
 
     src = read(args.source)
     src = inf.normalize(src) if inf.attr is not None else src
-    dev = local_device()
     if args.morph:
         from adaptive_voice_conversion_b200.speaker_bank import morph_table
         from adaptive_voice_conversion_b200.vocoder import AudioParams
         hp = vocoder.hp if vocoder is not None else AudioParams()
-        codes, weights = morph_table(load_bank(args.bank, inf.model), args.keyframes, src.shape[0], hp.sr / hp.hop_length)
+        codes, weights = morph_table(bank, args.keyframes, src.shape[0], hp.sr / hp.hop_length)
         mel = inf.inference_morph([torch.from_numpy(src).to(dev)], [codes], [weights.to(dev)])[0].cpu().numpy()
         mel = inf.denormalize(mel) if inf.attr is not None else mel
         wav = inf.vocoder.melspectrogram2wav(mel) if inf.vocoder is not None else None
+        if mv:   # the target profile on the output's frame grid, the morph's frame rate
+            prof = bank.morph_pitch_profile(args.keyframes, mel.shape[0], hp.sr / hp.hop_length)
+            wav = synthesise_mv(mel, profiles=[prof])
     elif args.bank:
-        code = load_bank(args.bank, inf.model).code(args.speaker)
+        code = bank.code(args.speaker)
         mel = inf.inference_with_codes([torch.from_numpy(src).to(dev)], code[None])[0].cpu().numpy()
         mel = inf.denormalize(mel) if inf.attr is not None else mel
         wav = inf.vocoder.melspectrogram2wav(mel) if inf.vocoder is not None else None
+        if mv:
+            wav = synthesise_mv(mel, profiles=[bank.pitch_profile(args.speaker)])
     else:
         raw_tgts = [read(t) for t in targets]
         tgts = [inf.normalize(t) for t in raw_tgts] if inf.attr is not None else raw_tgts
@@ -383,7 +441,30 @@ if __name__ == "__main__":
             shifts, info = match_shifts(vocoder, [m], [refs], vocoder.hp)
             print_matches([args.output], info)
             wav = vocoder.mel_to_wav([m], semitones=shifts)[0].cpu().numpy()
+        if mv:
+            wav = synthesise_mv(mel, ref_sets=[[torch.from_numpy(np.ascontiguousarray(t, np.float32)).to(dev)
+                                                for t in raw_tgts]])
     if is_wav(args.output):
         inf.write_wav_to_file(wav, args.output)
     else:
         np.save(args.output, mel)
+
+
+def main(argv=None):
+    p = parser()
+    args = p.parse_args(argv)
+    check_args(p, args)
+    if args.semitones == "mv" and (args.speaker is not None or args.morph is not None):
+        try:
+            refuse_unprofiled_bank(args.bank)
+        except ValueError as e:
+            p.error(str(e))
+    config = load_config(args.config)
+    if args.pairs:
+        run_pairs(args, config)
+        raise SystemExit(0)
+    run_single(args, config)
+
+
+if __name__ == "__main__":
+    main()

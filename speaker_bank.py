@@ -22,6 +22,14 @@ utterances when -transcripts is given:
 
 The defaults of -fit_steps, -fit_lr (the config's rate), -fit_crops and -fit_speakers are not tuned.
 data_loader.frame_size 1 only.
+
+With -f0 the bank also records each speaker's pitch profile (speaker_bank.build_pitch_profiles): the mean and std of
+log2 F0 over the voiced frames of the speaker's pooled utterances, each copy-synthesised from its denormalised mel by
+the GPU Griffin-Lim vocoder (-gl_iters, -gl_momentum, -gl_init; defaults 100, 0, zero, as inference.py) and tracked by
+YIN.  The mel statistics are -a, or <data_dir>/attr.pkl for a prepared set.  inference.py -pitch_shift mv needs the
+record to match a conversion's pitch to a banked speaker, mix or morph; without -f0 the bank is unchanged:
+
+    python speaker_bank.py -c config.yaml -m model.ckpt -d data/ -set train -o bank.pt -f0 [-gl_iters 100]
 """
 import os
 import pickle
@@ -52,6 +60,10 @@ def parser():
     p.add_argument("-holdout_set", help="held-out set of the banked speakers: <data_dir>/<holdout_set>.pkl (with -d)")
     p.add_argument("-transcripts", help="directory of <id>.txt transcripts: MCD-DTW on -holdout_set")
     p.add_argument("-report", help="fit report to write (JSON)")
+    p.add_argument("-f0", action="store_true", help="also record every speaker's pitch profile (for -pitch_shift mv)")
+    p.add_argument("-gl_iters", type=int, default=None, help="Griffin-Lim iterations of -f0's copy-synthesis (100)")
+    p.add_argument("-gl_momentum", type=float, default=None, help="fast Griffin-Lim momentum in [0, 1) of -f0's (0)")
+    p.add_argument("-gl_init", default=None, choices=["zero", "pghi"], help="Griffin-Lim start phase of -f0's (zero)")
     return p
 
 
@@ -75,6 +87,15 @@ def check_args(p, args):
                     p.error(f"-wav {w[0]}: {f} is not a file")
     elif not (args.data_dir and args.set):
         p.error("-d and -set go together")
+    gl = [f"-{k}" for k in ("gl_iters", "gl_momentum", "gl_init") if getattr(args, k) is not None]
+    if gl and not args.f0:
+        p.error(f"{', '.join(gl)} set(s) the copy-synthesis of -f0")
+    if args.gl_iters is not None and args.gl_iters < 0:
+        p.error("-gl_iters must be >= 0")
+    if args.gl_momentum is not None and not 0.0 <= args.gl_momentum < 1.0:
+        p.error("-gl_momentum must lie in [0, 1)")
+    if args.f0 and not args.wav and not os.path.isfile(attr_path(args)):
+        p.error(f"-f0 needs the mel statistics: {attr_path(args)} does not exist (pass -a)")
     fit_only = [f"-{k}" for k in ("fit_lr", "holdout_set", "transcripts", "report") if getattr(args, k) is not None]
     if args.fit_steps is None:
         if fit_only:
@@ -88,6 +109,24 @@ def check_args(p, args):
         p.error("-holdout_set goes with -d (a held-out set of the prepared data)")
     if args.transcripts and not args.holdout_set:
         p.error("-transcripts needs -holdout_set (the set MCD-DTW is measured on)")
+
+
+def attr_path(args):
+    """The mel statistics: -a, or <data_dir>/attr.pkl of a prepared set."""
+    return args.attr or os.path.join(args.data_dir, "attr.pkl")
+
+
+def pitch_record(args, bank, mels):
+    """build_pitch_profiles of the bank's pooled utterances at the -gl_* settings."""
+    from adaptive_voice_conversion_b200.speaker_bank import build_pitch_profiles
+    from adaptive_voice_conversion_b200.vocoder import AudioParams
+    with open(attr_path(args), "rb") as f:
+        attr = pickle.load(f)
+    d = AudioParams()
+    hp = AudioParams(n_iter=d.n_iter if args.gl_iters is None else args.gl_iters,
+                     momentum=d.momentum if args.gl_momentum is None else args.gl_momentum,
+                     gl_init=args.gl_init or d.gl_init)
+    return build_pitch_profiles(bank, mels, attr, hp)
 
 
 def set_mels(args):
@@ -175,6 +214,11 @@ def main(argv=None):
     model.eval()
     mels, speaker_of = wav_mels(args, config, dev) if args.wav else set_mels(args)
     bank = build_bank(model, mels, speaker_of=speaker_of)
+    if args.f0:
+        bank = bank.with_pitch(pitch_record(args, bank, mels))
+        unvoiced = [s for s, n in zip(bank.speakers, bank.pitch["voiced"]) if n == 0]
+        print(f"pitch profiles: {len(bank) - len(unvoiced)} speakers voiced"
+              + (f", no voiced frame for {', '.join(unvoiced)}" if unvoiced else ""))
     if args.fit_steps is None:
         bank.save(args.output)
         print(f"bank: {len(bank)} speakers, {sum(bank.n_utts)} utterances pooled, {bank.n_skipped} skipped -> {args.output}")
