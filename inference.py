@@ -79,6 +79,7 @@ bank's profiles were synthesised with:
 """
 import os
 from argparse import ArgumentParser
+from typing import NamedTuple
 
 import numpy as np
 import torch
@@ -92,15 +93,17 @@ def is_wav(path):
     return str(path).lower().endswith(".wav")
 
 
-class BankTarget(tuple):
-    """A pairs file's ``@SPEC`` target: a code of the -bank file (SpeakerBank.code); .spec is SPEC."""
+class BankTarget(NamedTuple):
+    """A target the -bank file holds, which needs no input file: a banked speaker or mix, spec (-speaker, a pairs
+    file's ``@SPEC``; SpeakerBank.code), or a morph, keyframes (-morph's parsed (SPEC, seconds))."""
+    spec: str | None = None
+    keyframes: tuple | None = None
 
-    def __new__(cls, spec):
-        return super().__new__(cls, ("@", spec))
 
-    @property
-    def spec(self):
-        return self[1]
+def target_files(target):
+    """The input files a conversion target needs: a target is a path (one file), a tuple of paths (a reference set:
+    their pooled speaker code) or a BankTarget (none)."""
+    return () if isinstance(target, BankTarget) else (target,) if isinstance(target, str) else tuple(target)
 
 
 def target_field(field, bank=False):
@@ -135,14 +138,14 @@ def read_pairs(path, bank=False):
                 tgt = target_field(parts[1], bank)
             except ValueError as e:
                 raise err(str(e)) from None
-            for fp in [parts[0]] + ([tgt] if isinstance(tgt, str) else [] if isinstance(tgt, BankTarget) else list(tgt)):
+            for fp in (parts[0], *target_files(tgt)):
                 if not os.path.isfile(fp) or not (is_wav(fp) or fp.lower().endswith(".npy")):
                     raise err(f"{fp} is not an existing .wav or .npy file")
             stem = lambda p: os.path.splitext(os.path.basename(p))[0]  # noqa: E731
             if isinstance(tgt, BankTarget):   # a weight's '.' is not an extension: the default name gets .wav now
                 first = tgt.spec.replace(":", "-").replace(",", "+") + ".wav"
             else:
-                first = stem(tgt if isinstance(tgt, str) else tgt[0])
+                first = stem(target_files(tgt)[0])
             name = parts[2] if len(parts) == 3 else f"{stem(parts[0])}_to_{first}"
             ext = os.path.splitext(name)[1].lower()
             if os.path.basename(name) != name or ext not in ("", ".wav", ".npy"):
@@ -154,14 +157,12 @@ def read_pairs(path, bank=False):
 
 
 def check_frames(pairs, src_frames, tgt_frames, minimum):
-    """ValueError naming the line of the first pair whose source / target is shorter than (min_src, min_ref).  A
-    reference set's entry in tgt_frames lists its members' frames."""
+    """ValueError naming the line of the first pair whose source / target is shorter than (min_src, min_ref).
+    tgt_frames[i] lists the frames of the target_files of pairs[i]'s target (a one-file target's may be its count)."""
     for (n, src, tgt, _), ts, tt in zip(pairs, src_frames, tgt_frames):
         if ts < minimum[0]:
             raise ValueError(f"line {n}: source {src} has {ts} frames; the model needs at least {minimum[0]}")
-        if isinstance(tgt, BankTarget):
-            continue
-        for t, f in zip((tgt,) if isinstance(tgt, str) else tgt, (tt,) if isinstance(tgt, str) else tt):
+        for t, f in zip(target_files(tgt), [tt] if isinstance(tt, int) else tt):
             if f < minimum[1]:
                 raise ValueError(f"line {n}: target {t} has {f} frames; the model needs at least {minimum[1]}")
 
@@ -231,74 +232,95 @@ def print_matches(names, info):
 
 
 def run_pairs(args, config):
-    """The -pairs mode: every pair of the file, batched (see the module docstring)."""
-    from adaptive_voice_conversion_b200.mcd import min_frames
-    from adaptive_voice_conversion_b200.vocoder import AudioParams, Vocoder, load_wav
+    """The -pairs mode: every line of the file, refused as a whole before anything runs (see the module docstring)."""
     pairs = read_pairs(args.pairs, bank=bool(args.bank))
     if args.semitones == "match":
         refuse_bank_targets(pairs, args.pairs)
     if args.semitones == "mv" and any(isinstance(t, BankTarget) and is_wav(name) for _, _, t, name in pairs):
         refuse_unprofiled_bank(args.bank)
     os.makedirs(args.output, exist_ok=True)
+    run(args, config, pairs)
+
+
+def run(args, config, jobs):
+    """Converts jobs, [(line number or None, source, target, output name)]: the lines of a pairs file, their outputs
+    named in the -o directory, or one conversion, its output the -o path.  Every input is read once (the .wav files in
+    one Vocoder.wav_to_mel call), normalised on the device, converted, denormalised, pitch-shifted and synthesised
+    (every .wav output in one Vocoder.mel_to_wav call); see the module docstring."""
+    from adaptive_voice_conversion_b200.mcd import min_frames
+    from adaptive_voice_conversion_b200.vocoder import AudioParams, Vocoder, load_wav
     dev = local_device()
-    files = sorted({p for _, s, t, _ in pairs
-                    for p in (s,) + ((t,) if isinstance(t, str) else () if isinstance(t, BankTarget) else t)})
-    need_voc = any(is_wav(f) for f in files) or any(is_wav(name) for *_, name in pairs)
+    files = sorted({p for _, s, t, _ in jobs for p in (s, *target_files(t))})
     hp = AudioParams(n_iter=args.gl_iters, momentum=args.gl_momentum, gl_init=args.gl_init,
                      pitch_shift=0.0 if isinstance(args.semitones, str) else args.semitones)
-    vocoder = Vocoder(n_mels=config["SpeakerEncoder"]["c_in"] // config["data_loader"]["frame_size"],
-                      hp=hp) if need_voc else None
+    vocoder = None
+    if any(is_wav(f) for f in files) or any(is_wav(out) for *_, out in jobs):
+        vocoder = Vocoder(n_mels=config["SpeakerEncoder"]["c_in"] // config["data_loader"]["frame_size"], hp=hp)
     wavs = [f for f in files if is_wav(f)]
-    mels = {}
+    raw = {}
     if wavs:
-        sigs = [torch.from_numpy(load_wav(f, vocoder.hp.sr)).to(dev) for f in wavs]
-        mels.update((f, m) for f, (m, _) in zip(wavs, vocoder.wav_to_mel(sigs)))
-    mels.update((f, torch.from_numpy(np.load(f).astype(np.float32)).to(dev)) for f in files if not is_wav(f))
-    check_frames(pairs, [mels[s].shape[0] for _, s, _, _ in pairs],
-                 [mels[t].shape[0] if isinstance(t, str) else None if isinstance(t, BankTarget) else
-                  [mels[p].shape[0] for p in t] for _, _, t, _ in pairs],
-                 min_frames(config))
-    inf = Inferencer(config=config, args=args, vocoder=vocoder)
+        sigs = [torch.from_numpy(load_wav(f, hp.sr)).to(dev) for f in wavs]
+        raw.update((f, m) for f, (m, _) in zip(wavs, vocoder.wav_to_mel(sigs)))
+    raw.update((f, torch.from_numpy(np.load(f).astype(np.float32)).to(dev)) for f in files if not is_wav(f))
+    if args.pairs:
+        check_frames(jobs, [raw[s].shape[0] for _, s, _, _ in jobs],
+                     [[raw[p].shape[0] for p in target_files(t)] for _, _, t, _ in jobs], min_frames(config))
+    inf = Inferencer(config=config, args=args)
+    # the mels of every target are normalised and denormalised here, on the device, so inference_one_utterance must
+    # hand back its mels normalised
+    attr, inf.attr = inf.attr, None
     bank = load_bank(args.bank, inf.model) if args.bank else None
-    for n, _, t, _ in pairs:
-        if isinstance(t, BankTarget):
+    for n, _, t, _ in jobs:
+        if args.pairs and isinstance(t, BankTarget):
             try:
                 bank.code(t.spec)
             except ValueError as e:
                 raise ValueError(f"{args.pairs} line {n}: {e}") from None
-    raw = mels
-    if inf.attr is not None:
-        mean = torch.as_tensor(np.asarray(inf.attr["mean"], np.float32)).to(dev)
-        std = torch.as_tensor(np.asarray(inf.attr["std"], np.float32)).to(dev)
-        mels = {f: (m - mean) / std for f, m in mels.items()}
-    decs = convert_pairs(inf, pairs, mels, bank)
-    if inf.attr is not None:
+    mels = raw
+    if attr is not None:
+        mean = torch.as_tensor(np.asarray(attr["mean"], np.float32)).to(dev)
+        std = torch.as_tensor(np.asarray(attr["std"], np.float32)).to(dev)
+        mels = {f: (m - mean) / std for f, m in raw.items()}
+    fps = hp.sr / hp.hop_length
+    _, src, tgt, _ = jobs[0]
+    if isinstance(tgt, BankTarget) and tgt.keyframes is not None:
+        from adaptive_voice_conversion_b200.speaker_bank import morph_table
+        codes, weights = morph_table(bank, tgt.keyframes, mels[src].shape[0], fps)
+        decs = inf.inference_morph([mels[src]], [codes], [weights.to(dev)])
+    elif not isinstance(tgt, BankTarget) and not args.pairs:
+        # one -t file or set: unpadded, since the padded path agrees with it only within rounding
+        refs = [mels[p] for p in target_files(tgt)]
+        _, dec = inf.inference_one_utterance(mels[src], refs[0] if len(refs) == 1 else refs)
+        decs = [torch.from_numpy(dec).to(dev)]
+    else:
+        decs = convert_pairs(inf, jobs, mels, bank)
+    if attr is not None:
         decs = [d * std + mean for d in decs]
-    to_wav = [i for i, (*_, name) in enumerate(pairs) if is_wav(name)]
+    to_wav = [i for i, (*_, out) in enumerate(jobs) if is_wav(out)]
     shifts = None
     if args.semitones == "match" and to_wav:
         from adaptive_voice_conversion_b200.f0 import match_shifts
         shifts, info = match_shifts(vocoder, [decs[i].contiguous() for i in to_wav],
-                                    [[raw[p] for p in ((pairs[i][2],) if isinstance(pairs[i][2], str) else pairs[i][2])]
-                                     for i in to_wav], vocoder.hp)
-        print_matches([pairs[i][3] for i in to_wav], info)
+                                    [[raw[p] for p in target_files(jobs[i][2])] for i in to_wav], vocoder.hp)
+        print_matches([jobs[i][3] for i in to_wav], info)
     if args.semitones == "mv" and to_wav:
         from adaptive_voice_conversion_b200.f0 import mv_match
-        tgts = [pairs[i][2] for i in to_wav]
-        banked = [isinstance(t, BankTarget) for t in tgts]
+        tgts = [jobs[i][2] for i in to_wav]
+        profiles = [None if not isinstance(t, BankTarget) else bank.pitch_profile(t.spec) if t.keyframes is None else
+                    bank.morph_pitch_profile(t.keyframes, decs[i].shape[0], fps) for i, t in zip(to_wav, tgts)]
         shifts, info = mv_match(vocoder, [decs[i].contiguous() for i in to_wav], vocoder.hp,
-                                ref_sets=[None if b else [raw[p] for p in ((t,) if isinstance(t, str) else t)]
-                                          for t, b in zip(tgts, banked)],
-                                profiles=[bank.pitch_profile(t.spec) if b else None for t, b in zip(tgts, banked)])
-        print_mv([pairs[i][3] for i in to_wav], info, bank if any(banked) else None, vocoder.hp)
+                                ref_sets=[[raw[p] for p in target_files(t)] or None for t in tgts], profiles=profiles)
+        banked = any(isinstance(t, BankTarget) for t in tgts)
+        print_mv([jobs[i][3] for i in to_wav], info, bank if banked else None, vocoder.hp)
     ys = []
     if to_wav:   # a fixed shift is the vocoder's hp.pitch_shift
         ys = vocoder.mel_to_wav([decs[i].contiguous() for i in to_wav], **({} if shifts is None else {"semitones": shifts}))
+    out_dir = args.output if args.pairs else ""
     for i, y in zip(to_wav, ys):
-        inf.write_wav_to_file(y.cpu().numpy(), os.path.join(args.output, pairs[i][3]))
-    for i, (*_, name) in enumerate(pairs):
-        if not is_wav(name):
-            np.save(os.path.join(args.output, name), decs[i].cpu().numpy())
+        inf.write_wav_to_file(y.cpu().numpy(), os.path.join(out_dir, jobs[i][3]))
+    for i, (*_, out) in enumerate(jobs):
+        if not is_wav(out):
+            np.save(os.path.join(out_dir, out), decs[i].cpu().numpy())
 
 
 def load_bank(path, model):
@@ -382,74 +404,6 @@ def parser():
     return p
 
 
-def run_single(args, config):
-    """One conversion (-t, -bank -speaker or -bank -morph; see the module docstring)."""
-    targets = args.target or [None]
-    args.target = targets[0] if len(targets) == 1 else targets
-    vocoder = None
-    if any(is_wav(f) for f in (args.source, *targets, args.output)):
-        from adaptive_voice_conversion_b200.vocoder import AudioParams, Vocoder
-        vocoder = Vocoder(n_mels=config["SpeakerEncoder"]["c_in"] // config["data_loader"]["frame_size"],
-                          hp=AudioParams(n_iter=args.gl_iters, momentum=args.gl_momentum, gl_init=args.gl_init,
-                                         pitch_shift=0.0 if isinstance(args.semitones, str) else args.semitones))
-    match = args.semitones == "match" and is_wav(args.output)
-    mv = args.semitones == "mv" and is_wav(args.output)
-    inf = Inferencer(config=config, args=args, vocoder=vocoder if is_wav(args.output) and not (match or mv) else None)
-    bank = load_bank(args.bank, inf.model) if args.bank else None
-    dev = local_device()
-
-    def synthesise_mv(mel, ref_sets=None, profiles=None):
-        """The .wav of a denormalised mel shifted by mv toward its reference mels or a target profile."""
-        from adaptive_voice_conversion_b200.f0 import mv_match
-        m = torch.from_numpy(np.ascontiguousarray(mel, np.float32)).to(dev)
-        shifts, info = mv_match(vocoder, [m], vocoder.hp, ref_sets=ref_sets, profiles=profiles)
-        print_mv([args.output], info, bank if ref_sets is None else None, vocoder.hp)
-        return vocoder.mel_to_wav([m], semitones=shifts)[0].cpu().numpy()
-
-    def read(path):
-        return vocoder.get_spectrograms(path)[0] if is_wav(path) else np.load(path).astype(np.float32)
-
-    src = read(args.source)
-    src = inf.normalize(src) if inf.attr is not None else src
-    if args.morph:
-        from adaptive_voice_conversion_b200.speaker_bank import morph_table
-        from adaptive_voice_conversion_b200.vocoder import AudioParams
-        hp = vocoder.hp if vocoder is not None else AudioParams()
-        codes, weights = morph_table(bank, args.keyframes, src.shape[0], hp.sr / hp.hop_length)
-        mel = inf.inference_morph([torch.from_numpy(src).to(dev)], [codes], [weights.to(dev)])[0].cpu().numpy()
-        mel = inf.denormalize(mel) if inf.attr is not None else mel
-        wav = inf.vocoder.melspectrogram2wav(mel) if inf.vocoder is not None else None
-        if mv:   # the target profile on the output's frame grid, the morph's frame rate
-            prof = bank.morph_pitch_profile(args.keyframes, mel.shape[0], hp.sr / hp.hop_length)
-            wav = synthesise_mv(mel, profiles=[prof])
-    elif args.bank:
-        code = bank.code(args.speaker)
-        mel = inf.inference_with_codes([torch.from_numpy(src).to(dev)], code[None])[0].cpu().numpy()
-        mel = inf.denormalize(mel) if inf.attr is not None else mel
-        wav = inf.vocoder.melspectrogram2wav(mel) if inf.vocoder is not None else None
-        if mv:
-            wav = synthesise_mv(mel, profiles=[bank.pitch_profile(args.speaker)])
-    else:
-        raw_tgts = [read(t) for t in targets]
-        tgts = [inf.normalize(t) for t in raw_tgts] if inf.attr is not None else raw_tgts
-        tgt = [torch.from_numpy(t).to(dev) for t in tgts]     # several targets: one reference set
-        wav, mel = inf.inference_one_utterance(torch.from_numpy(src).to(dev), tgt[0] if len(tgt) == 1 else tgt)
-        if match:
-            from adaptive_voice_conversion_b200.f0 import match_shifts
-            m = torch.from_numpy(np.ascontiguousarray(mel, np.float32)).to(dev)
-            refs = [torch.from_numpy(np.ascontiguousarray(t, np.float32)).to(dev) for t in raw_tgts]
-            shifts, info = match_shifts(vocoder, [m], [refs], vocoder.hp)
-            print_matches([args.output], info)
-            wav = vocoder.mel_to_wav([m], semitones=shifts)[0].cpu().numpy()
-        if mv:
-            wav = synthesise_mv(mel, ref_sets=[[torch.from_numpy(np.ascontiguousarray(t, np.float32)).to(dev)
-                                                for t in raw_tgts]])
-    if is_wav(args.output):
-        inf.write_wav_to_file(wav, args.output)
-    else:
-        np.save(args.output, mel)
-
-
 def main(argv=None):
     p = parser()
     args = p.parse_args(argv)
@@ -463,7 +417,10 @@ def main(argv=None):
     if args.pairs:
         run_pairs(args, config)
         raise SystemExit(0)
-    run_single(args, config)
+    target = (BankTarget(keyframes=tuple(args.keyframes)) if args.morph is not None else
+              BankTarget(args.speaker) if args.speaker is not None else
+              args.target[0] if len(args.target) == 1 else tuple(args.target))
+    run(args, config, [(None, args.source, target, args.output)])
 
 
 if __name__ == "__main__":

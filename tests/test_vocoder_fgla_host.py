@@ -108,6 +108,10 @@ class FakeVocoder:
         self.n_mels, self.hp = n_mels, hp
         FakeVocoder.made.append(self)
 
+    def mel_to_wav(self, mels):
+        import torch
+        return [torch.zeros(8) for _ in mels]
+
 
 class FakeInferencer:
     def __init__(self, config, args, vocoder=None):

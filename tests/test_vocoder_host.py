@@ -133,3 +133,56 @@ def test_cli_npy_plumbing_is_unchanged(tmp_path, monkeypatch):
     assert x.dtype == torch.float32 and torch.equal(x, torch.from_numpy(src.astype(np.float32)))
     assert torch.equal(c, torch.from_numpy(tgt))
     assert np.array_equal(np.load(out), src.astype(np.float32)[:, :3] * 2)
+
+
+class Float64AttrInferencer:
+    """An Inferencer whose attr.pkl holds float64 statistics and whose conversions double the source."""
+    made = []
+
+    def __init__(self, config, args, vocoder=None):
+        self.vocoder, self.model = vocoder, None
+        self.attr = {"mean": np.array([0.1, -0.2, 0.3, 0.7]), "std": np.array([0.3, 1.1, 0.9, 2.5])}
+        Float64AttrInferencer.made.append(self)
+
+    def normalize(self, x):     # Inferencer's
+        return (x - self.attr["mean"]) / self.attr["std"]
+
+    def denormalize(self, x):
+        return x * self.attr["std"] + self.attr["mean"]
+
+    def inference_one_utterance(self, x, x_cond):
+        self.got = x.clone()
+        return None, (x * 2).numpy()
+
+    def inference_with_codes(self, xs, codes):
+        self.got = xs[0].clone()
+        return [xs[0] * 2]
+
+
+@pytest.mark.parametrize("target", [["-t", "t.npy"], ["-bank", "bank.pt", "-speaker", "p1"]])
+def test_cli_single_mode_casts_float64_statistics(tmp_path, monkeypatch, target):
+    """A float64 attr.pkl is cast to float32, as -pairs does: the model gets float32 mels and the .npy output is
+    float32, normalised and denormalised on the device."""
+    import torch
+    import adaptive_voice_conversion_b200.inference as I
+    import adaptive_voice_conversion_b200.speaker_bank as SB
+    import adaptive_voice_conversion_b200.utils as U
+    monkeypatch.setattr(I, "Inferencer", Float64AttrInferencer)
+    monkeypatch.setattr(U, "local_device", lambda: torch.device("cpu"))
+    monkeypatch.setattr(SB.SpeakerBank, "load", staticmethod(lambda path, model: types.SimpleNamespace(
+        code=lambda spec: torch.zeros(8))))
+    src = np.random.default_rng(0).standard_normal((10, 4)).astype(np.float32)
+    np.save(tmp_path / "s.npy", src)
+    np.save(tmp_path / "t.npy", np.ones((7, 4), np.float32))
+    monkeypatch.chdir(tmp_path)
+    monkeypatch.setattr(sys, "argv", ["inference.py", "-c", os.path.join(ROOT, "config.yaml"), "-a", "attr.pkl",
+                                      "-s", "s.npy", *target, "-o", "o.npy"])
+    Float64AttrInferencer.made.clear()
+    runpy.run_path(os.path.join(ROOT, "inference.py"), run_name="__main__")
+    inf, = Float64AttrInferencer.made
+    mean, std = (torch.tensor([0.1, -0.2, 0.3, 0.7], dtype=torch.float32),
+                 torch.tensor([0.3, 1.1, 0.9, 2.5], dtype=torch.float32))
+    x = (torch.from_numpy(src) - mean) / std
+    assert inf.got.dtype == torch.float32 and torch.equal(inf.got, x)
+    out = np.load(tmp_path / "o.npy")
+    assert out.dtype == np.float32 and np.array_equal(out, (x * 2 * std + mean).numpy())
