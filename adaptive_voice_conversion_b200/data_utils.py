@@ -14,6 +14,7 @@ import torch
 from torch.utils.data import DataLoader, Dataset
 
 from . import _lib as L
+from .engine import decoder_length
 from .utils import local_device
 
 
@@ -150,6 +151,20 @@ def device_corpus_fits(total_frames: int, n_mels: int, n_entries: int, total_mem
     section 4), and the gather kernel supports n_mels (a multiple of 4).  Total, not free, memory: the same choice on
     every run."""
     return n_mels % 4 == 0 and corpus_device_bytes(total_frames, n_mels, n_entries) <= total_memory // 2
+
+
+def check_segment_size(config: dict):
+    """Raise ValueError unless the decoder reproduces a segment of the config's segment_size (engine.decoder_length):
+    the reconstruction loss compares the decoder's output with its input frame by frame."""
+    dl = config["data_loader"]
+    seg, frame = int(dl["segment_size"]), int(dl["frame_size"])
+    if frame < 1 or seg < 1 or seg % frame != 0:
+        raise ValueError(f"segment_size {seg} is not a positive multiple of frame_size {frame}")
+    T = seg // frame
+    T_dec = decoder_length(config, T)
+    if T_dec != T:
+        raise ValueError(f"segment_size {seg}: a segment of {T} frames decodes to {T_dec} frames; the decoder reproduces "
+                         "only lengths its subsampling and upsampling map onto themselves")
 
 
 def validate_corpus(data, indexes, segment_size: int, frame_size: int, c_in: int):

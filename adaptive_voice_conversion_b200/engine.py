@@ -59,6 +59,18 @@ def conv_geometry(K: int, stride: int, Tin: int):
     return pl, pr, Tout
 
 
+def decoder_length(config: dict, T: int) -> int:
+    """Frames of the decoder's output for an input of T frames: the content encoder's subsampling convs (conv_geometry:
+    ceil(T / s) for its odd kernel), then the decoder's upsampling factors.  The reconstruction loss pairs each output
+    frame with an input frame, so training needs decoder_length(config, T) == T."""
+    ce, de = config["ContentEncoder"], config["Decoder"]
+    for s in ce["subsample"][: ce["n_conv_blocks"]]:
+        T = conv_geometry(ce["kernel_size"], s, T)[2]
+    for up in de["upsample"][: de["n_conv_blocks"]]:
+        T *= up
+    return T
+
+
 class Lengths:
     """Valid frames per sample of a padded batch at one layer: ceil(t[b] / div) * mul, with t the batch's input lengths
     (int32 [B] on the device) -- the avc_b200.h convention.  A stride-2 layer doubles div, an upsampling block

@@ -25,7 +25,7 @@ from typing import Dict, List, Sequence, Tuple
 import numpy as np
 import torch
 
-from .data_utils import DeviceSegments, corpus_device_bytes, load_corpus, validate_corpus
+from .data_utils import DeviceSegments, check_segment_size, corpus_device_bytes, load_corpus, validate_corpus
 from .utils import local_device
 
 
@@ -97,6 +97,7 @@ class HeldOut:
         if data_dir in (None, "synthetic"):
             raise ValueError("held-out evaluation needs a data directory with the test sets (-d <data_dir>)")
         dl = config["data_loader"]
+        check_segment_size(config)
         self.sets = list(sets)
         self.batch_size = int(dl["batch_size"])
         self.rank, self.world = rank, world

@@ -19,8 +19,8 @@ import numpy as np
 import torch
 import yaml
 
-from .data_utils import (DeviceSegments, PickleDataset, SyntheticSegments, corpus_device_bytes, device_corpus_fits,
-                         get_data_loader, load_corpus)
+from .data_utils import (DeviceSegments, PickleDataset, SyntheticSegments, check_segment_size, corpus_device_bytes,
+                         device_corpus_fits, get_data_loader, load_corpus)
 from .evaluate import HeldOut
 from .model import AE
 from .optim import FusedAdam
@@ -96,6 +96,7 @@ class Solver(object):
     # ---- data (solver.py:57-68)
     def get_data_loaders(self):
         dl = self.config["data_loader"]
+        check_segment_size(self.config)
         data_dir = getattr(self.args, "data_dir", "synthetic")
         if data_dir in (None, "synthetic"):
             n_mels = self.config["ContentEncoder"]["c_in"] // dl["frame_size"]

@@ -25,7 +25,7 @@ from typing import Dict, Optional
 import torch
 
 from . import _lib as L
-from .engine import A4, Engine
+from .engine import A4, Engine, decoder_length
 from .optim import FusedAdam
 
 
@@ -190,6 +190,10 @@ class FusedTrainer:
         ``losses()`` to synchronise."""
         if not x.is_cuda or x.dtype != torch.float32:
             raise L.AvcError("FusedTrainer.step: x must be a float32 CUDA tensor")
+        T, T_dec = x.shape[-1], decoder_length(self.cfg, x.shape[-1])
+        if T_dec != T:   # the loss kernels pair dec and x element by element
+            raise L.AvcError(f"FusedTrainer.step: a segment of T = {T} frames decodes to {T_dec} frames; training needs "
+                             "a length the decoder reproduces")
         x = x.contiguous()
         self.set_lambda_kl(lambda_kl)
         replay = self._graphs is not None and tuple(x.shape) == tuple(self._static.shape) and not return_outputs

@@ -221,6 +221,7 @@ def main():
     make_train_fixture(ref_model, 80, 1, 128, 1, "train_c80_b1.pt")      # BASELINE config 1
     make_train_fixture(ref_model, 80, 4, 128, 3, "train_c80_b4.pt")      # 3 Adam steps
     make_train_fixture(ref_model, 512, 2, 128, 1, "train_c512_b2.pt")    # shipped config.yaml
+    make_train_fixture(ref_model, 80, 2, 256, 2, "train_c80_b2_t256.pt")  # segment_size 256: the routes above 128 frames
     make_infer_fixture(ref_model, 80, 2, 301, 173, "infer_c80.pt")       # odd lengths, T_cond != T
     make_infer_fixture(ref_model, 80, 1, 512, 512, "infer_c80_t512.pt")  # BASELINE config 5 shape
     make_reference_forward_fixture(ref_model, "reference_forward_c80.pt")

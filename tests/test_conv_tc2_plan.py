@@ -170,12 +170,12 @@ class PlanLib:
         return f
 
 
-def cpu_engine(monkeypatch, lib, sms, c_in=80):
+def cpu_engine(monkeypatch, lib, sms, c_in=80, cfg=None, precision="tf32", stand_in=PlanLib):
     from adaptive_voice_conversion_b200 import engine as E
-    cfg = orc.default_config(c_in)
+    cfg = orc.default_config(c_in) if cfg is None else cfg
     e = object.__new__(E.Engine)      # the real constructor insists on a CUDA device
-    e.cfg, e.dev, e.lib, e.packed, e.debug = cfg, torch.device("cpu"), PlanLib(lib, sms), {}, None
-    e.precision, e.tc_status, e._packed_key = "tf32", torch.zeros(1, dtype=torch.int32), None
+    e.cfg, e.dev, e.lib, e.packed, e.debug = cfg, torch.device("cpu"), stand_in(lib, sms), {}, None
+    e.precision, e.tc_status, e._packed_key = precision, torch.zeros(1, dtype=torch.int32), None
     e._init_options()
     monkeypatch.setattr(E.Engine, "stream", property(lambda self: 0))
     monkeypatch.setattr(E.Engine, "zeros", lambda self, *shape: torch.zeros(shape))
@@ -202,10 +202,10 @@ def train_step(e, P, B, T):
 @pytest.mark.parametrize("sms", SMS)
 def test_engine_training_descriptors_all_plan(monkeypatch, lib, sms):
     """Forward blocks, stride-2 parity data gradients and folded / plain data gradients of a training step, for the
-    default segment (128 frames) and segment_size 64, 200 and 244, at B = 1, 16 and 256, with the fused fold on and off;
-    also the 512-mel config."""
+    default segment (128 frames) and segment_size 64, 200 and 232, at B = 1, 16 and 256, with the fused fold on and off;
+    also the 512-mel config.  (Training lengths are the ones the decoder reproduces: multiples of 8.)"""
     seen = set()
-    for c_in, segs in ((80, (64, 128, 200, 244)), (512, (128,))):
+    for c_in, segs in ((80, (64, 128, 200, 232)), (512, (128,))):
         e, P = cpu_engine(monkeypatch, lib, sms, c_in)
         for fold in (True, False):
             e.fold_fused = fold
@@ -214,7 +214,7 @@ def test_engine_training_descriptors_all_plan(monkeypatch, lib, sms):
                     train_step(e, P, B, T)
         assert e.lib.n > 0 and not e.lib.rejected, e.lib.rejected[:5]
         seen |= e.lib.instances
-    # the chunked folded widths are in real use (segment_size 200 / 244)
+    # the chunked folded widths are in real use (segment_size 200 / 232)
     assert any(nl != n for n, nl in seen), sorted(seen)
 
 

@@ -101,18 +101,19 @@ def oracle_state(model):
     return sd
 
 
-@pytest.mark.parametrize("sn", [False, True], ids=["plain", "sn"])
-def test_per_segment_losses_match_the_oracle(tmp_path, precision, sn):
+@pytest.mark.parametrize("sn,seg", [(False, SEG), (True, SEG), (False, 256)], ids=["plain", "sn", "plain-seg256"])
+def test_per_segment_losses_match_the_oracle(tmp_path, precision, sn, seg):
     cfg, model = make_model(sn)
+    cfg["data_loader"]["segment_size"] = seg    # (256: the conv blocks' longer-sequence routes, see test_step_routes_host.py)
     model.train()          # the evaluation is eval mode whatever the flag; it leaves the flag alone
     n = 40                 # batches of 16, 16 and 8
-    d = write_data_dir(tmp_path / "data", 80, {"in_test": n})
+    d = write_data_dir(tmp_path / "data", 80, {"in_test": n}, seg=seg)
     held = E.HeldOut(["in_test"], d, cfg, device="cuda")
     u0 = {k: v.clone() for k, v in model.named_buffers()}
     tab = held.tables(model)["in_test"].cpu()
     assert model.training and all(bits_equal(v, u0[k]) for k, v in model.named_buffers())
-    data, index = D.load_corpus(os.path.join(d, "in_test.pkl"), os.path.join(d, f"in_test_samples_{SEG}.json"))
-    pds = D.PickleDataset.from_loaded(data, index, SEG)
+    data, index = D.load_corpus(os.path.join(d, "in_test.pkl"), os.path.join(d, f"in_test_samples_{seg}.json"))
+    pds = D.PickleDataset.from_loaded(data, index, seg)
     x = D.CollateFn(1)([pds[i] for i in range(n)]).double()
     sd = oracle_state(model)
     with torch.no_grad():
@@ -126,8 +127,8 @@ def test_per_segment_losses_match_the_oracle(tmp_path, precision, sn):
     assert e_rec < tol and e_kl < tol, (e_rec, e_kl)
     res = held.evaluate(model)["in_test"]
     assert res["n"] == n
-    assert abs(res["loss_rec"] - float(rec.sum()) / (n * 80 * SEG)) < tol * res["loss_rec"]
-    assert abs(res["loss_kl"] - 0.5 * float(kl.sum()) / (n * 128 * SEG // 8)) < tol * res["loss_kl"]
+    assert abs(res["loss_rec"] - float(rec.sum()) / (n * 80 * seg)) < tol * res["loss_rec"]
+    assert abs(res["loss_kl"] - 0.5 * float(kl.sum()) / (n * 128 * seg // 8)) < tol * res["loss_kl"]
 
 
 @pytest.mark.parametrize("sn", [False, True], ids=["plain", "sn"])

@@ -70,7 +70,7 @@ def make_model(c_in):
     return m.cuda(), cfg
 
 
-@pytest.mark.parametrize("name", ["train_c80_b1.pt", "train_c80_b4.pt", "train_c512_b2.pt"])
+@pytest.mark.parametrize("name", ["train_c80_b1.pt", "train_c80_b4.pt", "train_c512_b2.pt", "train_c80_b2_t256.pt"])
 def test_forward_backward_vs_reference_fixture(golden_dir, name, precision):
     """BASELINE config 1 (single segment) and friends: AE.forward + recon/KL + grads through
     loss.backward() (the autograd path) vs the reference's own outputs."""

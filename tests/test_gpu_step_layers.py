@@ -12,7 +12,9 @@ pointer, row, residual mode or flag shows up as an error at the layer that has i
 
 - A launch that ran on the tensor cores (avc_conv_block_tc, avc_conv_wgrad_tc, avc_conv_wgrad_tc_acc; a proxy of the
   engine's library records which layer made each launch) is compared with a reference whose conv operands are rounded to
-  TF32 as the kernel rounds them.
+  TF32 as the kernel rounds them.  An FFMA launch inside a TF32 step (the weight and data gradients of layers longer
+  than the tensor-core kernels take) is compared with the captured operands as they are: dc is already TF32-rounded
+  where the engine rounded it (F_ROUND_OUT), the rest is raw fp32.
 - Every buffer the engine marks TF32-exact (A4.tf32: a consumer then skips its own rounding) must be TF32-exact.
 - ReLU ambiguity: an element whose float64 pre-activation is within TAU of its row's largest is ambiguous; the engine
   may take either branch there (per element forward, per row in the backward, at most 4 per row).
@@ -45,6 +47,14 @@ MAX_AMB_PER_ROW = 4
 # speaker encoder's in_conv at B = 37 (4736 terms per weight); at B = 8 no layer exceeds 8.0e-7.
 # ambiguous ReLU elements (|pre| < TAU of the row's largest) per training step: 79-97 at B = 8, 437 at B = 37;
 # per inference call (3 pairs): 2-221
+# Segments of other lengths (same card), worst of fwd / dc / dx / dw / grad / misc:
+#   T = 64:  fp32 2.3e-6 / 1.9e-6 / 1.2e-6 / 5.4e-7 / 3.6e-7 / 1.5e-6   tf32 3.4e-6 / 1.2e-6 / 3.2e-6 / 7.0e-7 / 5.0e-7 / 3.4e-6
+#   T = 200: fp32 2.7e-6 / 1.0e-6 / 1.7e-6 / 1.0e-6 / 3.1e-7 / 1.4e-6   tf32 2.3e-6 / 8.2e-7 / 3.9e-6 / 9.9e-7 / 4.2e-7 / 3.6e-6
+#   T = 256: fp32 2.5e-6 / 1.3e-6 / 1.5e-6 / 5.9e-7 / 4.2e-7 / 9.4e-7   tf32 2.6e-6 / 1.4e-6 / 4.0e-6 / 8.2e-7 / 3.5e-7 / 4.8e-6
+#            tf32 c512 6.1e-6 / 2.0e-6 / 4.0e-6 / 7.3e-7 / 2.7e-7 / 4.1e-6, sn 2.6e-6 / 1.6e-6 / 3.4e-6 / 7.3e-7 / 3.1e-7 / 3.6e-6
+#   T = 512 (B = 4): fp32 2.1e-6 / 1.1e-6 / 1.4e-6 / 6.7e-7 / 5.1e-7 / 1.1e-6   tf32 2.7e-6 / 1.2e-6 / 3.8e-6 / 8.1e-7 / 7.4e-7 / 4.2e-6
+# (dw at B·T = 1600-2048 terms per weight stays below 1.0e-6, in the FFMA weight gradient the TF32 step takes there too);
+# ambiguous elements per step 42-45 at T = 64, 151-207 at 200 and 256, 208-228 at 512.
 TOL = {"fp32": dict(fwd=2e-5, dc=5e-6, dx=5e-6, dw=2e-6, grad=1.5e-6, misc=5e-6),
        "tf32": dict(fwd=3.5e-5, dc=6e-6, dx=1.2e-5, dw=7.5e-6, grad=1.5e-6, misc=2e-5)}
 TC_FWD = ("avc_conv_block_tc",)
@@ -356,11 +366,21 @@ def _step(tr, x, eps):
     return tr.opt.flat_g.clone(), tr.opt.flat_p.clone(), tr.report.clone()
 
 
-TRAIN_CASES = [("c80", "fp32", 8, {}), ("c80", "tf32", 8, {}), ("c512", "fp32", 8, {}), ("c512", "tf32", 8, {}),
-               ("sn", "fp32", 8, {}), ("sn", "tf32", 8, {}), ("c80", "tf32", 37, {})] + [
-    ("c80", "tf32", 8, {k: v}) for k, v in (("AVC_FUSED_DENSE", "0"), ("AVC_FOLD_FUSED", "0"), ("AVC_NORM_BWD_FUSED", "1"),
-                                            ("AVC_WGRAD_ACC", "1"), ("AVC_WGRAD_STREAM", "0"), ("AVC_WGRAD_STREAM", "1"),
-                                            ("AVC_OVERLAP", "0"))]
+# (kind, precision, B, env, T).  The segment length decides which kernels a step runs (tests/test_step_routes_host.py
+# lists the routes of every length): at T = 128 the longest layer has 128 frames, every forward block runs fused, every
+# weight gradient on the tensor cores, every norm backward in the cached kernel.  The other lengths reach the rest: the
+# plain conv + avc_norm_apply_fwd forward (tf32 above 144 frames, fp32 above 256), the plain norm backward (above 128),
+# the FFMA weight gradient inside a TF32 step (a layer above 128 frames, or a stride-2 one above 64, or one whose length
+# is not a multiple of 8), the FFMA data gradient + avc_fold_add_fwd (a padded length above 256, the stride-2 parity
+# data gradient above 512).
+TRAIN_CASES = [("c80", "fp32", 8, {}, 128), ("c80", "tf32", 8, {}, 128), ("c512", "fp32", 8, {}, 128),
+               ("c512", "tf32", 8, {}, 128), ("sn", "fp32", 8, {}, 128), ("sn", "tf32", 8, {}, 128),
+               ("c80", "tf32", 37, {}, 128)] + [
+    ("c80", "tf32", 8, {k: v}, 128) for k, v in (("AVC_FUSED_DENSE", "0"), ("AVC_FOLD_FUSED", "0"), ("AVC_NORM_BWD_FUSED", "1"),
+                                                 ("AVC_WGRAD_ACC", "1"), ("AVC_WGRAD_STREAM", "0"), ("AVC_WGRAD_STREAM", "1"),
+                                                 ("AVC_OVERLAP", "0"))] + [
+    ("c80", p, 8, {}, T) for T in (64, 200, 256) for p in ("fp32", "tf32")] + [
+    ("c512", "tf32", 8, {}, 256), ("sn", "tf32", 8, {}, 256), ("c80", "fp32", 4, {}, 512), ("c80", "tf32", 4, {}, 512)]
 
 
 def _config(kind):
@@ -371,14 +391,14 @@ def _report(tag, chk):
     print(f"\n[{tag}] worst:", {k: f"{v:.2e} ({chk.where[k]})" for k, v in sorted(chk.worst.items())}, "ambiguous:", chk.amb)
 
 
-@pytest.mark.parametrize("kind,precision,B,env", TRAIN_CASES,
-                         ids=[f"{k}-{p}-B{b}" + "".join(f"-{n}={v}" for n, v in e.items()) for k, p, b, e in TRAIN_CASES])
-def test_training_step_layers(monkeypatch, kind, precision, B, env):
+@pytest.mark.parametrize("kind,precision,B,env,T", TRAIN_CASES,
+                         ids=[f"{k}-{p}-B{b}" + "".join(f"-{n}={v}" for n, v in e.items()) + ("" if T == 128 else f"-T{T}")
+                              for k, p, b, e, T in TRAIN_CASES])
+def test_training_step_layers(monkeypatch, kind, precision, B, env, T):
     monkeypatch.setenv("AVC_PRECISION", precision)
     for k, v in env.items():
         monkeypatch.setenv(k, v)
     cfg = _config(kind)
-    T = 128
     g = torch.Generator().manual_seed(11)
     x = torch.randn((B, cfg["SpeakerEncoder"]["c_in"], T), generator=g).cuda()
     eps = torch.randn((B, cfg["ContentEncoder"]["c_out"], T // 8), generator=g).cuda()
@@ -419,7 +439,7 @@ def test_training_step_layers(monkeypatch, kind, precision, B, env):
         ref = LR.sn_bwd(cap.sn[n][1], wbar, u1, v1, sigma)
         chk.err("grad", n + ".weight_orig", Checker._rel(tr.G[n + ".weight_orig"], ref, ref.abs().max()))
         chk.checked[n + ".weight_orig"] += 1
-    _report(f"{kind} {precision} B={B} {env}", chk)
+    _report(f"{kind} {precision} B={B} T={T} {env}", chk)
 
     names = set(tr.G)    # (with sn also name + ".weight": the gradient of W_bar, checked by its layer)
     assert {k for k, v in chk.checked.items() if v} == names, sorted(names ^ {k for k, v in chk.checked.items() if v})
@@ -431,6 +451,19 @@ def test_training_step_layers(monkeypatch, kind, precision, B, env):
     tol = TOL[precision]
     bad = {k: (v, chk.where[k]) for k, v in chk.worst.items() if not v <= tol[k]}
     assert not bad, bad
+
+
+def test_training_step_rejects_a_length_the_decoder_does_not_reproduce():
+    """244 frames decode to 248: the loss would pair misaligned frames and read past x.  The step refuses before its
+    first launch."""
+    from adaptive_voice_conversion_b200 import _lib as L
+    tr = _solver(_config("c80"), 2).trainer
+    x = torch.randn((2, 80, 244), generator=torch.Generator().manual_seed(3)).cuda()
+    torch.cuda.synchronize()
+    n0 = L.launch_count()
+    with pytest.raises(L.AvcError, match="T = 244 frames decodes to 248"):
+        tr.step(x, 1.0)
+    assert L.launch_count() == n0
 
 
 # ------------------------------------------------------------------ inference

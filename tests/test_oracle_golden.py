@@ -38,7 +38,7 @@ def test_helpers(golden_dir):
     assert rel(orc.instance_norm(x), fx["instance_norm"]) < 1e-5
 
 
-@pytest.mark.parametrize("name", ["train_c80_b1.pt", "train_c80_b4.pt", "train_c512_b2.pt"])
+@pytest.mark.parametrize("name", ["train_c80_b1.pt", "train_c80_b4.pt", "train_c512_b2.pt", "train_c80_b2_t256.pt"])
 def test_train_steps(golden_dir, name):
     fx = load(golden_dir, name)
     cfg = orc.default_config(fx["c_in"])
