@@ -13,9 +13,10 @@
 //            sample (Tout % 8 == 0), so a box never straddles samples; rows past the slice are copied from sample B,
 //            past the end of the tensor, and arrive as zeros like co past Cout.  The consumers load their A fragments
 //            from there with ld.shared and feed wgmma from registers (wgmma_tf32_rs), which takes A in any layout.
-//   B (x, by tap): a staging warpgroup loads four 16-byte A4 units (4 channels x 4 consecutive time steps), transposes
-//            the 4 x 4 block and stores four 16-byte K-major units into the no-swizzle core-matrix layout of
-//            tc_common.cuh: [8 planes][K x 32 rows][4 t], row j * 32 + ci holds xpad[ci][t * stride + j].
+//   B (x, by window): a staging thread loads the 16-byte A4 units (4 channels x 1 time step) of one (4-channel chunk,
+//            4-row plane) window once for all K taps, transposes them in registers and stores 4 K 16-byte K-major units
+//            into the no-swizzle core-matrix layout of tc_common.cuh: [8 planes][K x 32 rows][4 t], row j * 32 + ci
+//            holds xpad[ci][t * stride + j].
 // The tap shifts, the reflect padding and the stride-2 gather are all resolved while staging, so ONE wgmma per k-step
 // covers every tap.  The fp32 bit patterns are used as they are: the tensor core reads their TF32 part (truncation
 // toward zero, the operand model of tests/test_gpu_wgrad_exact.py).
@@ -43,64 +44,148 @@ struct WgTcArgs {
   int* status;
 };
 
-// 4 x 4 transpose of the staging step: unit c of the K-major side = component c of the four A4 units
-__device__ __forceinline__ float comp4(const float4& v, int c) { return c == 0 ? v.x : c == 1 ? v.y : c == 2 ? v.z : v.w; }
+// Staging windows.  Window w (0..63) of a chunk is ci chunk c4 = w % 8 and plane pl = w / 8: 4 channels at the plane's
+// 4 reduction rows t .. t + 3.  Row t + i, tap j reads input position (t + i) S + j - pad_left = t S + n - pad_left with
+// n = i S + j, so the window's K taps read 3 S + K distinct A4 units (K + 3 at stride 1, K + 6 at stride 2), and each is
+// loaded once.
+__host__ __device__ constexpr int wg_win_units(int K, int S) { return 3 * S + K; }
 
-// One staging job: four A4 units (4 channels at 4 consecutive reduction rows) -> four K-major units (4 reduction rows of
-// one channel) at operand rows row0 .. row0 + 3 of one plane.  Store k writes channel (k + rot) & 3 with rot = (c4 >> 1) & 3
-// of the job's 4-channel chunk c4: the 8 lanes of a 16-byte store phase (consecutive c4) then hit 8 different 16-byte
-// bank groups (a fixed order would put 4 of them on the same group).
-struct WgJob {
-  float4 v[4];
-  uint32_t dst;   // byte offset of operand row row0 of its plane inside the stage
-  int rot;
-};
-
-// Job e of stage chunk `ch` (rows ch * WG_ROWS .. of the CTA's slice) stages x: ci chunk e % 8, plane e / 8 % 8, tap e / 64.
-// Rows past the slice and channels past Cin are zeros.
-template <int K>
-__device__ __forceinline__ WgJob wgrad_job_load(const WgTcArgs& a, int e, int ch, int b0, int R) {
+// Loads the units of window w of chunk `ch` (rows ch * WG_ROWS .. of the CTA's slice) into u[n], n = 0 .. 3 S + K - 1.
+// Reflect padding is resolved per unit; rows past the slice and channels past Cin are zeros.
+template <int K, int S>
+__device__ __forceinline__ void wgrad_win_load(const WgTcArgs& a, float4 (&u)[wg_win_units(K, S)], int w, int ch, int b0, int R) {
   const avc_wgrad_desc& d = a.d;
-  const int T = d.Tout;
-  WgJob J;
-  const int c4 = e & 7, pl = (e >> 3) & 7, j = e >> 6;
+  const int c4 = w & 7, pl = w >> 3;
   const int r = ch * WG_ROWS + 4 * pl;
-  const int g = r / T, t = r - g * T;   // T % 8 == 0: the 4 rows lie in one sample
-  J.rot = (c4 >> 1) & 3;
-  J.dst = (uint32_t)WG_A_BYTES + (uint32_t)pl * (uint32_t)(K * WT_NT * 16) + (uint32_t)(j * WT_NT + 4 * c4) * 16u;
+  const int g = r / d.Tout, t = r - g * d.Tout;   // Tout % 8 == 0: the 4 rows lie in one sample
   const int ci = blockIdx.x * WT_NT + 4 * c4;
   const bool v = r < R && ci < d.Cin;
   const float* col = d.x + (size_t)(v ? b0 + g : 0) * d.x_bstride + (size_t)((v ? ci : 0) >> 2) * d.Tin * 4;
+  const int p0 = t * S - d.pad_left;
+  if (v && p0 >= 0 && p0 + wg_win_units(K, S) <= d.Tin) {
+    // inside the signal: one base address, the units at fixed offsets
+    const float* q = col + (size_t)p0 * 4;
 #pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    const int p = src_pos((t + i) * d.stride + j - d.pad_left, d.Tin, AVC_PAD_REFLECT, 1);
-    J.v[i] = (v && p >= 0) ? ldg4(col + (size_t)p * 4) : zero4();
+    for (int n = 0; n < wg_win_units(K, S); ++n) u[n] = ldg4(q + 4 * n);
+  } else {
+#pragma unroll
+    for (int n = 0; n < wg_win_units(K, S); ++n) {
+      const int p = src_pos(p0 + n, d.Tin, AVC_PAD_REFLECT, 1);
+      u[n] = (v && p >= 0) ? ldg4(col + (size_t)p * 4) : zero4();
+    }
   }
-  return J;
 }
 
-__device__ __forceinline__ void wgrad_job_store(uint8_t* stage, const WgJob& J) {
+__device__ __forceinline__ float comp4(const float4& v, int c) { return c == 0 ? v.x : c == 1 ? v.y : c == 2 ? v.z : v.w; }
+// component k of the result = component (k + rot) & 3 of v
+__device__ __forceinline__ float4 rot4(float4 v, int rot) {
+  if (rot & 1) v = make_float4(v.y, v.z, v.w, v.x);
+  if (rot & 2) v = make_float4(v.z, v.w, v.x, v.y);
+  return v;
+}
+
+// Transposes window w in registers and stores its 4 K K-major units: operand row j * 32 + 4 c4 + c of plane pl (tap j,
+// channel c of the chunk) holds component c of u[j], u[S + j], u[2 S + j], u[3 S + j] (rows t .. t + 3).
+// Store conflicts: a 16-byte store phase is 8 lanes, and lanes 8 h .. 8 h + 7 of a warp are the chunks c4 = 0..7 of one
+// plane at the same tap and store index k.  Store k writes channel c = (k + rot) & 3 with rot = (c4 >> 1) & 3, so its
+// 16-byte bank group (4 c4 + c) % 8 = 4 (c4 & 1) + ((k + (c4 >> 1)) & 3) differs for all 8 lanes (a fixed order would
+// put 4 of them on one group).  The units are rotated by rot once, so every store reads fixed components.
+template <int K, int S>
+__device__ __forceinline__ void wgrad_win_store(uint8_t* stage, float4 (&u)[wg_win_units(K, S)], int w) {
+  const int c4 = w & 7, pl = w >> 3, rot = (c4 >> 1) & 3;
+  uint8_t* row = stage + WG_A_BYTES + pl * (K * WT_NT * 16) + c4 * 64;
+#pragma unroll
+  for (int n = 0; n < wg_win_units(K, S); ++n) u[n] = rot4(u[n], rot);
 #pragma unroll
   for (int k = 0; k < 4; ++k) {
-    const int c = (k + J.rot) & 3;
-    *reinterpret_cast<float4*>(stage + J.dst + (uint32_t)c * 16u) = make_float4(comp4(J.v[0], c), comp4(J.v[1], c), comp4(J.v[2], c), comp4(J.v[3], c));
+    uint8_t* dst = row + ((k + rot) & 3) * 16;
+#pragma unroll
+    for (int j = 0; j < K; ++j)
+      *reinterpret_cast<float4*>(dst + j * WT_NT * 16) = make_float4(comp4(u[j], k), comp4(u[S + j], k), comp4(u[2 * S + j], k), comp4(u[3 * S + j], k));
   }
 }
 
-// Staging warpgroups per CTA.  A staging thread issues all loads of its jobs of a chunk, then stores them: the chunk's
-// global-load latency is exposed once per chunk and sets the pace (the tensor cores idle most of the time).  With two
-// staging warpgroups, each takes every other chunk, so two chunks' loads are in flight at once.  K <= 6 runs 512
-// threads; K = 7, 8 one staging warpgroup and 384 threads, because their 4 jobs per staging thread and up to 128
-// accumulators per consumer do not fit the 128 registers per thread of 512 threads.
+// Staging roles.  A staging warpgroup is two halves of 64 threads, and a half stages one chunk at a time, one window
+// per thread, so every staging thread is busy at any K.  Half h of the CTA owns the chunks ch = h (mod wg_halves).  A
+// half's loads are its latency: where two window register sets fit (wg_prefetch), a half issues the loads of its next
+// chunk before the stores of the current one, so a CTA has up to 2 wg_halves chunks' loads in flight.  K <= 6 runs two
+// staging warpgroups and 512 threads; K = 7, 8 one staging warpgroup and 384 threads, because 112-128 accumulators per
+// consumer leave too few of 512 threads' 128 registers for a window set.
 __host__ __device__ constexpr int wg_stagers(int K) { return K <= 6 ? 2 : 1; }
+__host__ __device__ constexpr int wg_halves(int K) { return 2 * wg_stagers(K); }
 __host__ __device__ constexpr int wg_threads(int K) { return 128 * (wg_stagers(K) + 2); }
 // Registers per thread after the setmaxnreg split of the launch allocation (the __launch_bounds__ cap: 128 at 512
-// threads, 168 at 384) between the staging warpgroups (at most 4 jobs, 18 registers each) and the consumers (N / 2
-// accumulators and two stages of A fragments, 32 registers).
-__host__ __device__ constexpr int wg_regs_stage(int K) { return wg_stagers(K) == 2 ? 96 : 104; }
-__host__ __device__ constexpr int wg_regs_mma(int K) { return wg_stagers(K) == 2 ? 160 : 200; }
-static_assert(2 * 128 * wg_regs_stage(1) + 256 * wg_regs_mma(1) <= 512 * 128 && 128 * wg_regs_stage(8) + 256 * wg_regs_mma(8) <= 384 * 168,
-              "setmaxnreg budget exceeds the launch allocation");
+// threads, 168 at 384) between the staging threads and the consumers (N / 2 accumulators and two stages of A
+// fragments, 32 registers).  A window set is 4 (3 S + K) registers; "2 x" = the half prefetches its next chunk:
+//   K            1..4            5        6        7        8
+//   stage / mma  128 / 128       112/144  96/160   120/192  120/192
+//   stride 1     2 x 16..28      2 x 32   1 x 36   2 x 40   1 x 44
+//   stride 2     2 x 28..40      1 x 44   1 x 48   1 x 52   1 x 56
+// Set from -Xptxas -v: K = 8 spills at 104 or 112 staging registers (stride 2) and with a stride-1 prefetch at 120;
+// K = 5 serialises its wgmmas at 136 consumer registers.
+__host__ __device__ constexpr int wg_regs_stage(int K) { return K <= 4 ? 128 : K == 5 ? 112 : K == 6 ? 96 : 120; }
+__host__ __device__ constexpr int wg_regs_mma(int K) { return K <= 4 ? 128 : K == 5 ? 144 : K == 6 ? 160 : 192; }
+// two window sets and 40 registers of addresses and loop state
+__host__ __device__ constexpr bool wg_prefetch(int K, int S) { return 2 * 4 * wg_win_units(K, S) + 40 <= wg_regs_stage(K); }
+__host__ __device__ constexpr bool wg_budget_ok(int K) {
+  return K > 8 || (wg_stagers(K) * 128 * wg_regs_stage(K) + 256 * wg_regs_mma(K) <= wg_threads(K) * (wg_stagers(K) == 2 ? 128 : 168) &&
+                   wg_budget_ok(K + 1));
+}
+static_assert(wg_budget_ok(1), "setmaxnreg budget exceeds the launch allocation");
+// The ring holds at least as many stages as there are staging halves (the parity argument in the kernel needs it)
+__host__ __device__ constexpr bool wg_ring_ok(int K) {
+  return K > 8 || ((WG_SMEM_MAX / (WG_A_BYTES + 8 * 16 * WT_NT * K) >= wg_halves(K)) && wg_ring_ok(K + 1));
+}
+static_assert(wg_ring_ok(1), "a staging half could run a whole ring ahead");
+
+// Stages chunk ch from the window registers u: waits for stage ch % nstage to be free, starts the dc copies (thread 0
+// of the half), stores the x windows and arrives on full (one arrival per warp).
+template <int K, int S>
+__device__ __forceinline__ bool wgrad_win_put(const WgTcArgs& a, const CUtensorMap* tmdc, uint8_t* smem, uint64_t* full, uint64_t* empty,
+                                              float4 (&u)[wg_win_units(K, S)], int w, int ch, int b0, int R) {
+  const avc_wgrad_desc& d = a.d;
+  const int s = ch % a.nstage;
+  const uint32_t ph = (uint32_t)(ch / a.nstage) & 1u;
+  if (ch >= a.nstage && !__all_sync(0xffffffffu, tc::mbar_wait(&empty[s], ph ^ 1u, a.status, 5))) return false;
+  uint8_t* stage = smem + (size_t)s * ((uint32_t)WG_A_BYTES + 8u * (uint32_t)(K * WT_NT * 16));
+  if (w == 0) {
+    tc::mbar_arrive_expect_tx(&full[s], (uint32_t)WG_A_BYTES);
+#pragma unroll
+    for (int p = 0; p < WG_ROWS / 4; ++p) {
+      const int r = ch * WG_ROWS + 4 * p, g = r / d.Tout;
+      tc::tensor_g2s_4d(stage + p * WG_A_PLANE, tmdc, 0, r - g * d.Tout, blockIdx.y * 32, r < R ? b0 + g : d.B, &full[s]);
+    }
+  }
+  wgrad_win_store<K, S>(stage, u, w);
+  tc::fence_proxy_async_smem();   // the generic-proxy stores, before the async proxy (wgmma) reads them
+  __syncwarp();
+  if ((w & 31) == 0) tc::mbar_arrive(&full[s]);
+  return true;
+}
+
+// The staging loop of half h at stride S.  With prefetch the two register sets alternate by chunk with static indices:
+// chunk ch + H's loads are issued before chunk ch's wait and stores.
+template <int K, int S>
+__device__ __forceinline__ void wgrad_stage_x(const WgTcArgs& a, const CUtensorMap* tmdc, uint8_t* smem, uint64_t* full, uint64_t* empty,
+                                              int h, int w, int b0, int R, int nchunk) {
+  constexpr int H = wg_halves(K), U = wg_win_units(K, S);
+  float4 ua[U];
+  if constexpr (wg_prefetch(K, S)) {
+    float4 ub[U];
+    if (h < nchunk) wgrad_win_load<K, S>(a, ua, w, h, b0, R);
+    for (int ch = h; ch < nchunk; ch += 2 * H) {
+      if (ch + H < nchunk) wgrad_win_load<K, S>(a, ub, w, ch + H, b0, R);
+      if (!wgrad_win_put<K, S>(a, tmdc, smem, full, empty, ua, w, ch, b0, R) || ch + H >= nchunk) return;
+      if (ch + 2 * H < nchunk) wgrad_win_load<K, S>(a, ua, w, ch + 2 * H, b0, R);
+      if (!wgrad_win_put<K, S>(a, tmdc, smem, full, empty, ub, w, ch + H, b0, R)) return;
+    }
+  } else {
+    for (int ch = h; ch < nchunk; ch += H) {
+      wgrad_win_load<K, S>(a, ua, w, ch, b0, R);
+      if (!wgrad_win_put<K, S>(a, tmdc, smem, full, empty, ua, w, ch, b0, R)) return;
+    }
+  }
+}
 
 // One stage of a consumer warpgroup: wait for the stage, load this thread's A fragments of its 4 k-steps into `af`
 // (a0..a3 of k-step k in af[4k..4k+3]), queue the 4 MMAs, then retire the previous stage's (wait_group 1).  The
@@ -130,8 +215,8 @@ __device__ __forceinline__ bool wgrad_mma_stage(const WgTcArgs& a, float* acc, u
   return true;
 }
 
-// Weight gradient of one (ci tile, co tile, batch slice).  mbarrier ring over the slice's row chunks: full[s] = the four
-// warps of the staging warpgroup that owns the chunk wrote the x planes of stage s, and the dc boxes of its TMA copies
+// Weight gradient of one (ci tile, co tile, batch slice).  mbarrier ring over the slice's row chunks: full[s] = the two
+// warps of the staging half that owns the chunk wrote the x planes of stage s, and the dc boxes of its TMA copies
 // landed (transaction bytes); empty[s] = both consumer warpgroups' MMAs on stage s retired.  A consumer queues the MMAs
 // of stage i, then wait_group 1 retires those of stage i - 1 and releases it; every CTA accumulates its rows in a fixed
 // order.  setmaxnreg moves registers from the staging warpgroups to the consumers (wg_regs_*).
@@ -143,7 +228,7 @@ __global__ void __launch_bounds__(wg_threads(K), 1) conv_wgrad_wgmma_kernel(cons
   extern __shared__ __align__(1024) uint8_t smem[];
   __shared__ uint64_t bar_full[WG_MAX_STAGES], bar_empty[WG_MAX_STAGES];
   const avc_wgrad_desc& d = a.d;
-  const int tid = threadIdx.x, warp = tc::warp_idx_sync(), lane = tid & 31;
+  const int tid = threadIdx.x, warp = tc::warp_idx_sync();
   const int sl = blockIdx.z, b0 = sl * a.samp_per_slice;
   const int R = max(0, min(a.samp_per_slice, d.B - b0)) * d.Tout;   // reduction rows of the slice
   const int nchunk = cdiv(R, WG_ROWS);
@@ -151,7 +236,7 @@ __global__ void __launch_bounds__(wg_threads(K), 1) conv_wgrad_wgmma_kernel(cons
 
   if (tid == 0) {
     for (int s = 0; s < a.nstage; ++s) {
-      tc::mbar_init(&bar_full[s], 5);   // four staging warps + the arrival that carries the dc copies' bytes
+      tc::mbar_init(&bar_full[s], 3);   // two staging warps + the arrival that carries the dc copies' bytes
       tc::mbar_init(&bar_empty[s], 2);
     }
     tc::fence_mbar_init();
@@ -160,38 +245,18 @@ __global__ void __launch_bounds__(wg_threads(K), 1) conv_wgrad_wgmma_kernel(cons
 
   if (warp < 4 * STAGERS) {
     // ================================================================ staging warpgroups
-    // The global loads are the latency the staging has to hide: every load of a thread's JPT jobs of a stage is issued
-    // before the first store, and before the wait for the stage to be free.  Staging warpgroup g owns the chunks
-    // ch = g (mod STAGERS).  The parity wait on empty[s] cannot alias an older phase: before chunk ch this warpgroup
-    // waited for the release of chunk ch - STAGERS - nstage, and releases come in chunk order (nstage >= 4).  Once the
-    // stage is free, thread 0 of the warpgroup starts the TMA copies of its dc planes; they land while the x stores run.
+    // Staging half h = warp / 2 owns the chunks ch = h (mod H), H = wg_halves(K); thread w = tid % 64 of the half
+    // stages window w.  The two warps of a half wait, store and arrive on their own.  The parity wait on empty[s]
+    // cannot alias an older phase: before chunk ch, each warp of the half waited for chunk ch - H, that is for the
+    // release of chunk ch - H - nstage, and releases come in chunk order.  nstage >= H (wg_ring_ok), so chunk
+    // ch - 2 nstage is released and empty[s] is at most one phase behind.  Loads issued ahead (prefetch) touch no
+    // barrier; a half's stores never run more than nstage chunks ahead of the consumers.  Once the stage is free,
+    // thread 0 of the half starts the TMA copies of its dc planes; they land while the x stores run.
     tc::setmaxnreg_dec<wg_regs_stage(K)>();
-    constexpr int NJOBS = 64 * K, JPT = (NJOBS + 127) / 128;
-    const int stid = tid & 127;
-    for (int ch = warp >> 2; ch < nchunk; ch += STAGERS) {
-      const int s = ch % a.nstage;
-      const uint32_t ph = (uint32_t)(ch / a.nstage) & 1u;
-      WgJob J[JPT];
-#pragma unroll
-      for (int q = 0; q < JPT; ++q)
-        if (stid + 128 * q < NJOBS) J[q] = wgrad_job_load<K>(a, stid + 128 * q, ch, b0, R);
-      if (ch >= a.nstage && !__all_sync(0xffffffffu, tc::mbar_wait(&bar_empty[s], ph ^ 1u, a.status, 5))) return;
-      uint8_t* stage = smem + (size_t)s * stage_bytes;
-      if (stid == 0) {
-        tc::mbar_arrive_expect_tx(&bar_full[s], (uint32_t)WG_A_BYTES);
-#pragma unroll
-        for (int p = 0; p < WG_ROWS / 4; ++p) {
-          const int r = ch * WG_ROWS + 4 * p, g = r / d.Tout;
-          tc::tensor_g2s_4d(stage + p * WG_A_PLANE, &tmdc, 0, r - g * d.Tout, blockIdx.y * 32, r < R ? b0 + g : d.B, &bar_full[s]);
-        }
-      }
-#pragma unroll
-      for (int q = 0; q < JPT; ++q)
-        if (stid + 128 * q < NJOBS) wgrad_job_store(stage, J[q]);
-      tc::fence_proxy_async_smem();   // the generic-proxy stores, before the async proxy (wgmma) reads them
-      __syncwarp();
-      if (lane == 0) tc::mbar_arrive(&bar_full[s]);
-    }
+    if (d.stride == 1)
+      wgrad_stage_x<K, 1>(a, &tmdc, smem, bar_full, bar_empty, warp >> 1, tid & 63, b0, R, nchunk);
+    else
+      wgrad_stage_x<K, 2>(a, &tmdc, smem, bar_full, bar_empty, warp >> 1, tid & 63, b0, R, nchunk);
     return;
   }
 
