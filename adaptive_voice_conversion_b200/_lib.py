@@ -250,6 +250,9 @@ class SpkIdentifyDesc(C.Structure):
                 ("target_score", _fp), ("target_rank", _fp)]
 
 
+PROBE_MAX_CLASSES = 4096   # AVC_PROBE_MAX_CLASSES
+PROBE_SUM_SCRATCH = 1024   # doubles of avc_probe_xent's scratch
+
 SN_ITERATE, SN_FIXED = 0, 1
 SN_MAX_ITEMS, SN_MAX_H, SN_MAX_W = 64, 4096, 4096
 
@@ -334,6 +337,11 @@ PROTOTYPES = {
     "avc_spk_group_mean": (_i, [C.POINTER(SpkGroupDesc), _p]),
     "avc_spk_group_mean_multi": (_i, [C.POINTER(SpkGroupDesc), _i, _p]),
     "avc_spk_identify": (_i, [C.POINTER(SpkIdentifyDesc), _p]),
+    "avc_probe_frames": (_i, [_p, _i, _i, _i, _p, _p, _p, _p]),
+    "avc_probe_moments": (_i, [_p, _i64, _i, _p, _p, _p]),
+    "avc_probe_standardize": (_i, [_p, _p, _i64, _i, _p, _p, _p, _p]),
+    "avc_probe_xent": (_i, [_p, _p, _i, _i, C.c_float, _p, _p, _p, _p, _p, _p]),
+    "avc_probe_vote": (_i, [_p, _i, _p, _i, _p, _p, _p, _p]),
     "avc_spectral_norm_scratch_floats": (_i64, [_i, _i]),
     "avc_spectral_norm": (_i, [_p, _i, _i, _i, _i, _p, _p]),
     "avc_spectral_norm_bwd": (_i, [_p, _i, _i, _i, _p, _p]),

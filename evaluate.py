@@ -4,7 +4,7 @@ data directory (adaptive_voice_conversion_b200/evaluate.py gives the definition)
     python evaluate.py -c config.yaml -m model.ckpt -d data/ [-eval_sets in_test,out_test] [-o eval.json]
                        [-mcd -transcripts VCTK-Corpus/txt [-attr data/attr.pkl] [-mcd_dims 24]] [-spk]
                        [-f0 [-gl_iters 100] [-gl_momentum 0] [-gl_init zero] [-pitch_shift match|mv]]
-                       [-max_pairs 0] [-seed 0] [-n_refs 1] [-bank bank.pt]
+                       [-max_pairs 0] [-seed 0] [-n_refs 1] [-bank bank.pt] [-probe [-probe_set train] [-probe_utts 64]]
 
 The checkpoint is loaded strictly (reference checkpoints too, and the `sn: True` layout).  Each set's losses are
 printed; -o writes them with the per-speaker means as JSON.  -mcd also measures conversion itself: the mel-cepstral
@@ -39,6 +39,10 @@ id_real the share of the set's own utterances nearest their speaker's (the encod
 pairs whose two speakers are banked (n_unbanked the others), with bank_speakers.  A bank that pooled any of the
 evaluated utterances is refused; a train bank leaves in_test leak-free and reports out_test's unseen speakers as
 unbanked.
+-probe trains speaker-classifier probes (a small MLP each) on -probe_set's speaker codes, pooled content codes, content
+code frames and pooled mels, up to -probe_utts utterances per speaker drawn with -seed, and reports their accuracy on
+each set's utterances of those speakers (adaptive_voice_conversion_b200/speaker_probe.py gives the definitions): one
+more line per set and a "probe" entry per set in -o.  The probe set must be disjoint from the evaluated sets.
 """
 import json
 import os
@@ -81,7 +85,20 @@ def main(argv=None):
                    help="references of the target speaker per conversion, their speaker codes pooled (-mcd, -spk); "
                         "-f0 as -spk")
     p.add_argument("-bank", default=None, help="speaker bank: identify conversions among its speakers (-spk)")
+    p.add_argument("-probe", action="store_true",
+                   help="also train speaker-classifier probes on the speaker code, the content code and the mel, and "
+                        "report their accuracy on each set")
+    p.add_argument("-probe_set", default="train", help="set the probes are fitted on (<probe_set>.pkl) (-probe)")
+    p.add_argument("-probe_utts", type=int, default=64, help="fit utterances drawn per speaker (-probe)")
     args = p.parse_args(argv)
+    eval_sets = [s for s in args.eval_sets.split(",") if s]
+    if args.probe:
+        if args.probe_set in eval_sets:
+            p.error(f"-probe_set {args.probe_set} is also one of -eval_sets; a probe must be scored on other utterances")
+        if not os.path.isfile(os.path.join(args.data_dir, f"{args.probe_set}.pkl")):
+            p.error(f"-probe needs {os.path.join(args.data_dir, args.probe_set + '.pkl')} (pass -probe_set)")
+        if args.probe_utts < 1:
+            p.error("-probe_utts must be >= 1")
     if args.mcd and not args.transcripts:
         p.error("-mcd needs -transcripts DIR")
     if args.bank and not args.spk:
@@ -103,7 +120,7 @@ def main(argv=None):
     model = AE(config).to(dev)
     model.load_state_dict(torch.load(args.model, map_location=dev), strict=True)
     model.eval()
-    held = HeldOut([s for s in args.eval_sets.split(",") if s], args.data_dir, config, device=dev)
+    held = HeldOut(eval_sets, args.data_dir, config, device=dev)
     res = held.evaluate(model, per_speaker=True)
     for s, r in res.items():
         print(f"{s}: n={r['n']} loss_rec={r['loss_rec']:.6f} loss_kl={r['loss_kl']:.6f} ({len(r['speakers'])} speakers)")
@@ -172,6 +189,22 @@ def main(argv=None):
                       f"mean_abs={ps['mean_abs_semitones']:.4f} n_unmatched={ps['n_unmatched']} "
                       f"n_clamped={ps['n_clamped']}{mv} (unshifted st_target="
                       + ("n/a" if not r["unshifted"]["n"] else f"{r['unshifted']['st_target']:.4f}") + ")")
+    if args.probe:
+        from adaptive_voice_conversion_b200.speaker_probe import evaluate_probe
+        with open(os.path.join(args.data_dir, f"{args.probe_set}.pkl"), "rb") as f:
+            fit_data = pickle.load(f)
+        sets = {}
+        for s in res:
+            with open(os.path.join(args.data_dir, f"{s}.pkl"), "rb") as f:
+                sets[s] = pickle.load(f)
+        probes = evaluate_probe(model, fit_data, sets, seed=args.seed, per_speaker_utts=args.probe_utts, device=dev,
+                                fit_name=args.probe_set)
+        for s, r in probes.items():
+            res[s]["probe"] = r
+            accs = " ".join(f"{k}=" + ("n/a" if r[k]["acc"] is None else f"{r[k]['acc']:.4f}")
+                            for k in ("speaker", "content", "content_frames", "mel"))
+            print(f"{s}: probe {accs} chance={r['chance']:.4f} (n={r['n']} n_unseen={r['n_unseen']} n_short={r['n_short']}, "
+                  f"{r['speakers']} speakers, fit on {args.probe_set}: {r['n_fit']} utterances)")
     if args.output:
         with open(args.output, "w") as f:
             json.dump(res, f, indent=1)

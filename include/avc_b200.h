@@ -865,6 +865,44 @@ typedef struct avc_spk_identify_desc {
 } avc_spk_identify_desc;
 int avc_spk_identify(const avc_spk_identify_desc* d, void* stream);
 
+/* ---- Speaker-classifier probes (csrc/probe.cu, speaker_probe.py).  No allocation, no synchronisation, no atomics;
+ * all arrays on the DEVICE; every float64 operation rounded on its own (no fused multiply-add); every argument is
+ * checked before any launch, so the calls can be captured in a CUDA graph and a second launch gives the same bits.
+ * The probe's linear layers are avc_linear_fwd / avc_linear_bwd, its update avc_sqnorm / avc_adam_step.
+ *
+ * avc_probe_frames: the valid frames of a padded planar batch x[B][C][T] as rows: out[row_off[b] + t][c] = x[b][c][t]
+ * for t < lengths[b] (int32 [B]); row_off (int64 [B]) places each sample.  A sample with lengths[b] outside [0, T]
+ * writes nothing.  AVC_ERR_UNSUPPORTED for B > 65535.
+ *
+ * avc_probe_moments: per dimension d of x[rows][D], in float64 adding in ascending row order:
+ *   mean[d] = (sum_r x) / rows,   std[d] = sqrt((sum_r (x - mean)^2) / rows), replaced by 1 when it is 0.
+ * avc_probe_standardize: out[r][d] = (float)((x[i][d] - mean[d]) / std[d]) with i = index[r] (int64 [rows]), or i = r
+ * when index is NULL.  The index is not checked.
+ *
+ * avc_probe_xent: for each row r < R of logits[R][S] with y = labels[r] (int32):
+ *   loss[r]       = (m + log(sum_j exp(z_j - m))) - z_y in float64, m = max_j z_j;
+ *   rank[r]       = #{j : z_j > z_y, or z_j == z_y and j < y} (0: the true class is the top decision);
+ *   dlogits[r][j] = (float)((softmax_j - [j == y]) * scale) when dlogits is not NULL;
+ *   loss_sum[0]   = the float64 sum of loss[] (two-stage, a fixed order for a given R; scratch >= 1024 doubles) when
+ *                   scratch and loss_sum are not NULL (both or neither).
+ * A row whose label lies outside [0, S) gets loss NaN, rank -1 and dlogits 0.
+ *
+ * avc_probe_vote: for each utterance u < U, over the rows [off[u], off[u+1]) of logits[][S] (off int64 [U + 1]):
+ *   scores[u][s] = sum_r (z_rs - m_r - log(sum_j exp(z_rj - m_r))) in float64, ascending r (0 without rows);
+ *   rank[u]      = #{s : scores[u][s] > scores[u][y], or equal and s < y} for y = labels[u]; -1 when y is outside
+ *                  [0, S).
+ * AVC_ERR_INVALID for null pointers or non-positive sizes; AVC_ERR_UNSUPPORTED for S > AVC_PROBE_MAX_CLASSES. */
+#define AVC_PROBE_MAX_CLASSES 4096
+int avc_probe_frames(const float* x, int B, int C, int T, const int32_t* lengths, const int64_t* row_off, float* out,
+                     void* stream);
+int avc_probe_moments(const float* x, int64_t rows, int D, double* mean, double* std, void* stream);
+int avc_probe_standardize(const float* x, const int64_t* index, int64_t rows, int D, const double* mean,
+                          const double* std, float* out, void* stream);
+int avc_probe_xent(const float* logits, const int32_t* labels, int R, int S, float scale, double* loss, float* dlogits,
+                   int32_t* rank, double* scratch, double* loss_sum, void* stream);
+int avc_probe_vote(const float* logits, int S, const int64_t* off, int U, const int32_t* labels, double* scores,
+                   int32_t* rank, void* stream);
+
 /* ---- Spectral norm of the decoder weights (csrc/spectral_norm.cu): torch.nn.utils.spectral_norm with
  * n_power_iterations=1, eps=1e-12, dim=0, for a DEVICE-resident table of n layers.  W = weight viewed as [h][w]
  * (nn.Conv1d: h = Cout, w = Cin*K; nn.Linear: [out][in]); normalize(x) = x / max(||x||, eps).
