@@ -158,6 +158,16 @@ class AudioDesc(C.Structure):
     ]
 
 
+RTISI_MAX_LOOKAHEAD = 7   # AVC_RTISI_MAX_LOOKAHEAD
+
+
+class RtisiDesc(C.Structure):
+    _fields_ = [("n_fft", C.c_int32), ("hop", C.c_int32), ("win", C.c_int32), ("lookahead", C.c_int32),
+                ("n_iter", C.c_int32), ("n_streams", C.c_int32), ("deemph", C.c_float), ("reserved", C.c_int32),
+                ("mag", _fp), ("mag_off", _fp), ("slot", _fp), ("close", _fp), ("out_off", _fp), ("y", _fp),
+                ("state", _fp), ("count", _fp)]
+
+
 class MelDesc(C.Structure):
     _fields_ = [("rows", C.c_int32), ("n_mels", C.c_int32), ("n_bins", C.c_int32), ("dir", C.c_int32),
                 ("max_db", C.c_float), ("ref_db", C.c_float), ("in_", _fp), ("mat", _fp), ("out", _fp)]
@@ -317,10 +327,13 @@ PROTOTYPES = {
     "avc_group_l1": (_i, [C.POINTER(GroupL1Desc), _p]),
     "avc_code_adam": (_i, [C.POINTER(CodeAdamDesc), _p]),
     "avc_stft": (_i, [C.POINTER(AudioDesc), _p]),
+    "avc_stft_window": (_i, [C.POINTER(AudioDesc), _p]),
     "avc_istft": (_i, [C.POINTER(AudioDesc), _p]),
     "avc_griffin_lim": (_i, [C.POINTER(AudioDesc), _p]),
     "avc_griffin_lim_from": (_i, [C.POINTER(AudioDesc), C.c_int32, C.c_float, _p]),
     "avc_pghi": (_i, [C.POINTER(AudioDesc), C.c_float, _p, _p]),
+    "avc_rtisi_state_floats": (_i64, [_i, _i]),
+    "avc_rtisi_la": (_i, [C.POINTER(RtisiDesc), _p]),
     "avc_frame_power": (_i, [C.POINTER(AudioDesc), _p, _p]),
     "avc_deemphasis": (_i, [C.POINTER(AudioDesc), C.c_float, _p]),
     "avc_yin": (_i, [C.POINTER(AudioDesc), C.c_int32, C.c_int32, C.c_int32, C.c_float, _p, _p, _p, _p]),

@@ -103,12 +103,21 @@ __device__ __forceinline__ int reflect(int i, int L) {
   return min(max(i, 0), L - 1);
 }
 
+// The same for a segment that holds samples [first, first + L) of a longer signal, which starts at 0 and ends with
+// the segment: the signal's sample i as an index into the segment.  first = 0 is reflect(i, L).
+__device__ __forceinline__ int reflect_window(int i, int first, int L) {
+  if (i < 0) i = -i;
+  if (i >= first + L) i = 2 * (first + L - 1) - i;
+  return min(max(i - first, 0), L - 1);
+}
+
 // ------------------------------------------------------------------ forward STFT
 // One frame per 128 threads: the windowed frame is read straight from the signal (reflect padding and pre-emphasis
 // applied on the fly), packed as z[n] = x[2n] + i x[2n+1], transformed, and split into the 1025 rfft bins.
 // MOMENTUM: the fast Griffin-Lim projection (X_prev set, mode PROJECT or PROJECT_FIRST).  It is its own instance so
 // that the other epilogues keep their 32 registers (4 CTAs per SM).
-template <bool MOMENTUM>
+// ORIGIN (avc_stft_window): a table entry's reserved field is its frame origin.
+template <bool MOMENTUM, bool ORIGIN>
 __global__ void __launch_bounds__(FFT_THREADS) stft_kernel(avc_audio_desc d) {
   __shared__ float2 tab[NC];
   __shared__ float2 buf[FPB][NC];
@@ -120,7 +129,13 @@ __global__ void __launch_bounds__(FFT_THREADS) stft_kernel(avc_audio_desc d) {
   if (live) g = d.segs[seg_of_frame(d.segs, d.n_seg, f)];
   const float* y = d.y + g.sample_off;
   const int L = g.n_samples, off = (NFFT - d.win) / 2;
-  const int base = (f - g.frame_off) * d.hop - NFFT / 2;
+  // frame origin o: the entry's frames are frames o, o + 1, ... of a longer signal, and its samples start at that
+  // signal's sample first (0 for origin 0, the whole signal).  Every sample a frame reads, reflected at the end or
+  // not, is at or after o hop - win/2 - 1, so with first one sample earlier its pre-emphasis neighbour is inside: a
+  // read at segment index 0 happens only when first = 0, where index 0 is the signal's sample 0.
+  const int o = ORIGIN ? g.reserved : 0;
+  const int first = ORIGIN ? max(0, o * d.hop - d.win / 2 - 2) : 0;
+  const int base = (o + f - g.frame_off) * d.hop - NFFT / 2;
   const float pe = d.preemph;
   float2* z = buf[fl];
   for (int n = t; n < NC; n += TPF) {
@@ -129,7 +144,7 @@ __global__ void __launch_bounds__(FFT_THREADS) stft_kernel(avc_audio_desc d) {
     for (int e = 0; e < 2; ++e) {
       const int q = 2 * n + e - off;
       if (live && q >= 0 && q < d.win) {
-        const int i = reflect(base + 2 * n + e, L);
+        const int i = ORIGIN ? reflect_window(base + 2 * n + e, first, L) : reflect(base + 2 * n + e, L);
         float s = __ldg(y + i);
         if (pe != 0.f && i > 0) s -= pe * __ldg(y + i - 1);
         v[e] = hann(q, d.win) * s;
@@ -669,6 +684,230 @@ __global__ void __launch_bounds__(PG_THREADS) pghi_kernel(avc_audio_desc d, floa
   }
 }
 
+// ------------------------------------------------------------------ RTISI-LA (streaming phase reconstruction)
+// One CTA per stream, RT_TPF = 128 threads per buffer frame (nb = lookahead + 1 groups).  The stream's windowed
+// inverse frames and the overlap-add numerator of its committed frames over the open samples live in shared memory
+// for the launch and in the state slot between launches.  Sample n is covered by frame F when 0 <= n - F hop + win/2
+// < win (mel_to_signal's grid); the numerator holds samples c hop - win/2 ... c hop + win/2 - 1, c the committed count.
+// Every sum runs in a fixed order (numerator, then frames in increasing order) with no atomics.
+constexpr int RT_MAX_LA = AVC_RTISI_MAX_LOOKAHEAD;
+
+// floats of one stream's state slot: frames [nb][win], magnitudes [nb][n_bins], numerator [win], de-emphasis carry
+__host__ __device__ inline int64_t rt_state_floats(int win, int lookahead) {
+  const int64_t nb = lookahead + 1;
+  return (nb * win + nb * NBIN + win + 1 + 3) / 4 * 4;
+}
+
+__host__ __device__ inline int rt_floordiv(int a, int b) { return a >= 0 ? a / b : -((-a + b - 1) / b); }
+
+struct RtSmem {  // dynamic shared-memory layout of one CTA
+  int nb, win, hop;
+  __host__ __device__ int scratch_floats() const { return max((nb - 1) * hop + win, 2 * win); }
+  __host__ __device__ size_t bytes() const {
+    return sizeof(float2) * ((size_t)NC + (size_t)nb * NC + nb) + sizeof(float) * ((size_t)nb * win + win + scratch_floats());
+  }
+};
+
+// est[i] = signal estimate at sample n0 + i, i < len: (numerator + the buffered frames c .. c + nbuf - 1 that cover it)
+// divided by the window sum-square of the frames 0 .. newest that cover it, where that exceeds FLT_MIN
+__device__ void rt_estimate(float* est, int n0, int len, const float* num, const float* fr, int c, int nbuf, int newest,
+                            int nb, int win, int hop) {
+  const int a0 = c * hop - win / 2, h = win / 2;
+  for (int i = threadIdx.x; i < len; i += blockDim.x) {
+    const int n = n0 + i;
+    const int lo = rt_floordiv(n + h - win, hop) + 1, hi = rt_floordiv(n + h, hop);
+    float acc = (n - a0 >= 0 && n - a0 < win) ? num[n - a0] : 0.f;
+    for (int F = max(lo, c); F <= min(hi, c + nbuf - 1); ++F) acc += fr[(F % nb) * win + n - F * hop + h];
+    float wss = 0.f;
+    for (int F = max(lo, 0); F <= min(hi, newest); ++F) {
+      const float w = hann(n - F * hop + h, win);
+      wss += w * w;
+    }
+    est[i] = wss > FLT_MIN ? acc / wss : acc;
+  }
+}
+
+// One frame's projection in the 128 threads of group z: STFT of the windowed estimate e[0 .. win), the magnitudes mag
+// with the estimate's phase (phase 0 where |E| = 0), iSTFT times the window into out.  Every thread of the CTA calls it.
+__device__ void rt_project(float2* z, float2* nyq, const float2* tab, int t, const float* e, const float* mag, float* out,
+                           bool live, int win) {
+  const int off = (NFFT - win) / 2;
+  for (int n = t; n < NC; n += TPF) {
+    float v[2] = {0.f, 0.f};
+#pragma unroll
+    for (int k = 0; k < 2; ++k) {
+      const int q = 2 * n + k - off;
+      if (live && q >= 0 && q < win) v[k] = hann(q, win) * e[q];
+    }
+    z[n] = make_float2(v[0], v[1]);
+  }
+  __syncthreads();
+  fft1024(z, tab, t);
+  constexpr int PER = NC / TPF + 1;  // bins per thread, the Nyquist bin with thread 0
+  float2 X[PER];
+#pragma unroll
+  for (int i = 0; i < PER; ++i) {
+    const int k = t + i * TPF;
+    X[i] = make_float2(0.f, 0.f);
+    if (k <= NC) {
+      const float2 zk = z[k & (NC - 1)], zr = z[(NC - k) & (NC - 1)];
+      const float2 xe = make_float2(0.5f * (zk.x + zr.x), 0.5f * (zk.y - zr.y));
+      const float2 xo = make_float2(0.5f * (zk.y + zr.y), -0.5f * (zk.x - zr.x));
+      const float2 w = k < NC ? tab[k] : make_float2(-1.f, 0.f);
+      const float2 wx = cmul(w, xo);
+      const float2 E = make_float2(xe.x + wx.x, xe.y + wx.y);
+      const float a = sqrtf(E.x * E.x + E.y * E.y);
+      const float m = live ? mag[k] : 0.f;
+      X[i] = a > 0.f ? make_float2(m * (E.x / a), m * (E.y / a)) : make_float2(m, 0.f);
+    }
+  }
+  __syncthreads();
+#pragma unroll
+  for (int i = 0; i < PER; ++i) {
+    const int k = t + i * TPF;
+    if (k < NC) z[k] = X[i];
+    else if (k == NC) *nyq = X[i];
+  }
+  __syncthreads();
+  float2 P[NC / TPF];
+#pragma unroll
+  for (int i = 0; i < NC / TPF; ++i) {  // istft_frames_kernel's packing
+    const int k = t + i * TPF;
+    float2 a = z[k], b = k == 0 ? *nyq : z[NC - k];
+    if (k == 0) a.y = b.y = 0.f;
+    b.y = -b.y;
+    const float2 xe = make_float2(0.5f * (a.x + b.x), 0.5f * (a.y + b.y));
+    const float2 w = tab[k];
+    const float2 xo = cmul(make_float2(0.5f * (a.x - b.x), 0.5f * (a.y - b.y)), make_float2(w.x, -w.y));
+    P[i] = make_float2(xe.x - xo.y, -(xe.y + xo.x));
+  }
+  __syncthreads();
+#pragma unroll
+  for (int i = 0; i < NC / TPF; ++i) z[t + i * TPF] = P[i];
+  __syncthreads();
+  fft1024(z, tab, t);
+  if (!live) return;
+  const float inv = 1.f / (float)NC;
+  for (int q = t; q < win; q += TPF) {
+    const int p = off + q;
+    const float2 v = z[p >> 1];
+    out[q] = ((p & 1) ? -v.y : v.x) * inv * hann(q, win);
+  }
+}
+
+__global__ void __launch_bounds__((RT_MAX_LA + 1) * TPF) rtisi_kernel(avc_rtisi_desc d, RtSmem L) {
+  extern __shared__ float4 rt_smem[];
+  const int nb = L.nb, win = L.win, hop = L.hop, h = win / 2;
+  float2* tab = reinterpret_cast<float2*>(rt_smem);
+  float2* zb = tab + NC;
+  float2* nyq = zb + (size_t)nb * NC;
+  float* fr = reinterpret_cast<float*>(nyq + nb);
+  float* num = fr + (size_t)nb * win;
+  float* est = num + win;
+  const int s = blockIdx.x, g = threadIdx.x / TPF, t = threadIdx.x % TPF;
+  const int slot = d.slot[s];
+  const int64_t stride = rt_state_floats(win, d.lookahead);
+  float* st = d.state + (int64_t)slot * stride;
+  float* st_mag = st + (int64_t)nb * win;
+  float* st_num = st_mag + (int64_t)nb * NBIN;
+  int32_t* cnt = d.count + 2 * (int64_t)slot;
+  int c = cnt[0], nbuf = cnt[1];
+  float carry = st_num[win];
+  fill_twiddles(tab);
+  for (int i = threadIdx.x; i < nb * win; i += blockDim.x) fr[i] = st[i];
+  for (int i = threadIdx.x; i < win; i += blockDim.x) num[i] = st_num[i];
+  float* y = d.y + d.out_off[s];
+  int64_t w = 0;  // samples written
+  __syncthreads();
+
+  // K Jacobi iterations over the buffered frames c .. c + nbuf - 1, the newest present frame being the last of them
+  auto iterate = [&]() {
+    for (int it = 0; it < d.n_iter; ++it) {
+      const int n0 = c * hop - h;
+      rt_estimate(est, n0, (nbuf - 1) * hop + win, num, fr, c, nbuf, c + nbuf - 1, nb, win, hop);
+      __syncthreads();
+      const int F = c + g;
+      const bool live = g < nbuf;
+      rt_project(zb + (size_t)g * NC, nyq + g, tab, t, est + g * hop, st_mag + (int64_t)(F % nb) * NBIN,
+                 fr + (size_t)(F % nb) * win, live, win);
+      __syncthreads();
+    }
+  };
+  // release samples n0 .. n0 + cnt_rel - 1 of the numerator (frames 0 .. last cover them), n >= 0 only, de-emphasised
+  auto release = [&](int n0, int len, int last) {
+    float* rel = est;
+    const int a0 = c * hop - h;
+    for (int i = threadIdx.x; i < len; i += blockDim.x) {
+      const int n = n0 + i;
+      const int lo = rt_floordiv(n + h - win, hop) + 1, hi = rt_floordiv(n + h, hop);
+      float wss = 0.f;
+      for (int F = max(lo, 0); F <= min(hi, last); ++F) {
+        const float wv = hann(n - F * hop + h, win);
+        wss += wv * wv;
+      }
+      const float acc = num[n - a0];
+      rel[i] = wss > FLT_MIN ? acc / wss : acc;
+    }
+    __syncthreads();
+    const int skip = max(0, -n0), cntw = max(0, len - skip);
+    if (threadIdx.x == 0) {
+      for (int i = skip; i < len; ++i) {
+        carry = rel[i] + d.deemph * carry;
+        rel[i] = carry;
+      }
+    }
+    __syncthreads();
+    for (int i = threadIdx.x; i < cntw; i += blockDim.x) y[w + i] = rel[skip + i];
+    w += cntw;
+    __syncthreads();
+  };
+  // commit frame c: add it to the numerator, release the hop samples it completes, shift the numerator by hop
+  auto commit = [&]() {
+    const float* f = fr + (size_t)(c % nb) * win;
+    for (int i = threadIdx.x; i < win; i += blockDim.x) num[i] += f[i];
+    __syncthreads();
+    release(c * hop - h, hop, c);
+    float* tmp = est + win;
+    for (int i = threadIdx.x; i < win; i += blockDim.x) tmp[i] = i + hop < win ? num[i + hop] : 0.f;
+    __syncthreads();
+    for (int i = threadIdx.x; i < win; i += blockDim.x) num[i] = tmp[i];
+    __syncthreads();
+    ++c;
+    --nbuf;
+  };
+
+  for (int r = d.mag_off[s]; r < d.mag_off[s + 1]; ++r) {
+    const int T = c + nbuf;  // the entering frame
+    float* m = st_mag + (int64_t)(T % nb) * NBIN;
+    for (int k = threadIdx.x; k < NBIN; k += blockDim.x) m[k] = __ldg(d.mag + (int64_t)r * NBIN + k);
+    // start phase: the estimate of the frames 0 .. T-1 over the entering frame's support
+    rt_estimate(est, T * hop - h, win, num, fr, c, nbuf, T - 1, nb, win, hop);
+    __syncthreads();
+    rt_project(zb + (size_t)g * NC, nyq + g, tab, t, est, m, fr + (size_t)(T % nb) * win, g == 0, win);
+    __syncthreads();
+    ++nbuf;
+    iterate();
+    if (nbuf == nb) commit();
+  }
+  if (d.close[s]) {
+    const int T = c + nbuf;
+    while (nbuf > 0) {
+      iterate();
+      commit();
+    }
+    // the samples after the last commit's, up to the grid's end hop (T - 1)
+    const int n0 = T * hop - h, n1 = (T - 1) * hop;
+    if (T > 0 && n1 > max(n0, 0)) release(n0, n1 - n0, T - 1);
+  }
+  for (int i = threadIdx.x; i < nb * win; i += blockDim.x) st[i] = fr[i];
+  for (int i = threadIdx.x; i < win; i += blockDim.x) st_num[i] = num[i];
+  if (threadIdx.x == 0) {
+    st_num[win] = carry;
+    cnt[0] = c;
+    cnt[1] = nbuf;
+  }
+}
+
 int check_audio(const avc_audio_desc* d, const char* who) {
   AVC_REQUIRE(d != nullptr, AVC_ERR_INVALID, "%s: null descriptor", who);
   AVC_REQUIRE(d->n_fft == NFFT, AVC_ERR_UNSUPPORTED, "%s: only n_fft = %d is supported (got %d)", who, NFFT, d->n_fft);
@@ -709,10 +948,11 @@ int launch_pghi(const avc_audio_desc& d, float tol, int8_t* parent, cudaStream_t
   return AVC_OK;
 }
 
-int launch_stft(const avc_audio_desc& d, cudaStream_t st) {
+int launch_stft(const avc_audio_desc& d, cudaStream_t st, bool origin = false) {
   if (d.n_frames == 0) return AVC_OK;
-  if (d.X_prev != nullptr) stft_kernel<true><<<cdiv(d.n_frames, FPB), FFT_THREADS, 0, st>>>(d);
-  else stft_kernel<false><<<cdiv(d.n_frames, FPB), FFT_THREADS, 0, st>>>(d);
+  if (origin) stft_kernel<false, true><<<cdiv(d.n_frames, FPB), FFT_THREADS, 0, st>>>(d);
+  else if (d.X_prev != nullptr) stft_kernel<true, false><<<cdiv(d.n_frames, FPB), FFT_THREADS, 0, st>>>(d);
+  else stft_kernel<false, false><<<cdiv(d.n_frames, FPB), FFT_THREADS, 0, st>>>(d);
   AVC_CHECK_LAUNCH("avc_stft");
   return AVC_OK;
 }
@@ -753,6 +993,21 @@ extern "C" int avc_stft(const avc_audio_desc* d, void* stream) {
     a.X_prev = nullptr;
   }
   return launch_stft(a, (cudaStream_t)stream);
+}
+
+extern "C" int avc_stft_window(const avc_audio_desc* d, void* stream) {
+  if (int rc = check_audio(d, "avc_stft_window")) return rc;
+  AVC_REQUIRE(d->y != nullptr, AVC_ERR_INVALID, "avc_stft_window: null signal");
+  AVC_REQUIRE(d->mode == AVC_STFT_MAG || d->mode == AVC_STFT_COMPLEX, AVC_ERR_INVALID,
+              "avc_stft_window: mode must be MAG or COMPLEX (got %d)", d->mode);
+  AVC_REQUIRE(d->mode != AVC_STFT_MAG || d->mag_out != nullptr || d->mag_db != nullptr, AVC_ERR_INVALID,
+              "avc_stft_window: MAG needs mag_out or mag_db");
+  AVC_REQUIRE(d->mode == AVC_STFT_MAG || d->X != nullptr, AVC_ERR_INVALID, "avc_stft_window: null X");
+  AVC_REQUIRE(d->mode != AVC_STFT_MAG || d->mag_db == nullptr || d->max_db > 0.f, AVC_ERR_INVALID,
+              "avc_stft_window: max_db must be positive");
+  avc_audio_desc a = *d;
+  a.X_prev = nullptr;
+  return launch_stft(a, (cudaStream_t)stream, true);
 }
 
 extern "C" int avc_istft(const avc_audio_desc* d, void* stream) {
@@ -835,5 +1090,35 @@ extern "C" int avc_mel_project(const avc_mel_desc* d, void* stream) {
   if (d->dir == AVC_MEL_TO_MAG) mel_gemm_kernel<AVC_MEL_TO_MAG><<<grid, 256, 0, st>>>(*d);
   else mel_gemm_kernel<AVC_MAG_TO_MEL><<<grid, 256, 0, st>>>(*d);
   AVC_CHECK_LAUNCH("avc_mel_project");
+  return AVC_OK;
+}
+
+extern "C" int64_t avc_rtisi_state_floats(int win, int lookahead) {
+  if (win <= 0 || lookahead < 0) return 0;
+  return rt_state_floats(win, lookahead);
+}
+
+extern "C" int avc_rtisi_la(const avc_rtisi_desc* d, void* stream) {
+  AVC_REQUIRE(d != nullptr, AVC_ERR_INVALID, "avc_rtisi_la: null descriptor");
+  AVC_REQUIRE(d->n_fft == NFFT, AVC_ERR_UNSUPPORTED, "avc_rtisi_la: only n_fft = %d is supported (got %d)", NFFT, d->n_fft);
+  AVC_REQUIRE(d->win > 0 && d->win <= NFFT && d->win % 2 == 0, AVC_ERR_UNSUPPORTED,
+              "avc_rtisi_la: win must be even and in (0, n_fft] (got %d)", d->win);
+  AVC_REQUIRE(d->hop > 0 && 2 * d->hop <= d->win, AVC_ERR_UNSUPPORTED, "avc_rtisi_la: hop must be in (0, win/2] (got %d)",
+              d->hop);
+  AVC_REQUIRE(d->lookahead >= 0 && d->lookahead <= RT_MAX_LA, AVC_ERR_UNSUPPORTED,
+              "avc_rtisi_la: lookahead must be in [0, %d] (got %d)", RT_MAX_LA, d->lookahead);
+  AVC_REQUIRE(d->n_iter >= 0, AVC_ERR_INVALID, "avc_rtisi_la: n_iter < 0");
+  AVC_REQUIRE(d->n_streams >= 0, AVC_ERR_INVALID, "avc_rtisi_la: n_streams < 0");
+  AVC_REQUIRE(std::isfinite(d->deemph), AVC_ERR_INVALID, "avc_rtisi_la: de-emphasis coefficient is not finite");
+  if (d->n_streams == 0) return AVC_OK;
+  AVC_REQUIRE(d->mag && d->mag_off && d->slot && d->close && d->out_off && d->y && d->state && d->count, AVC_ERR_INVALID,
+              "avc_rtisi_la: null pointer");
+  RtSmem L{d->lookahead + 1, d->win, d->hop};
+  const size_t smem = L.bytes();
+  cudaError_t e = cudaFuncSetAttribute(rtisi_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  AVC_REQUIRE(e == cudaSuccess, AVC_ERR_CUDA, "avc_rtisi_la: cudaFuncSetAttribute(%zu bytes): %s", smem,
+              cudaGetErrorString(e));
+  rtisi_kernel<<<d->n_streams, L.nb * TPF, smem, (cudaStream_t)stream>>>(*d, L);
+  AVC_CHECK_LAUNCH("avc_rtisi_la");
   return AVC_OK;
 }

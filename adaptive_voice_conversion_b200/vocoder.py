@@ -358,6 +358,9 @@ def trim(wavs, top_db: float):
     return out
 
 
+_trim = trim   # the name Vocoder.wav_to_mel's trim= keyword shadows
+
+
 def _mel_project(x, mat, direction, hp: AudioParams):
     n_out = hp.n_bins if direction == L.MEL_TO_MAG else hp.n_mels
     x = x.float().contiguous()
@@ -449,11 +452,13 @@ class Vocoder:
         self.fb_t = torch.from_numpy(np.ascontiguousarray(fb.T, np.float32)).to(self.device)    # [n_bins, n_mels]
         self.m_t = torch.from_numpy(np.ascontiguousarray(mel_to_linear_matrix(fb).T, np.float32)).to(self.device)
 
-    def wav_to_mel(self, wavs):
+    def wav_to_mel(self, wavs, *, trim: bool = True):
         """Signals at hp.sr (device tensors) -> [(mel [T, n_mels], mag [T, n_bins])], both normalised: trim (top_db),
-        pre-emphasis, |STFT|, mel projection, dB, normalisation."""
+        pre-emphasis, |STFT|, mel projection, dB, normalisation.  trim=False analyses the signals as they are (the
+        streaming analysis of streaming.py gives these frames)."""
         hp = self.hp
-        ys = _signals(trim(wavs, hp.top_db), hp, "wav_to_mel (after trimming)")
+        ys = (_signals(_trim(wavs, hp.top_db), hp, "wav_to_mel (after trimming)") if trim else
+              _signals(wavs, hp, "wav_to_mel"))
         r = _Ragged([y.numel() for y in ys], [1 + y.numel() // hp.hop_length for y in ys], self.device)
         mag = torch.empty(int(r.frame_offs[-1]), hp.n_bins, device=self.device)
         mag_db = torch.empty_like(mag)

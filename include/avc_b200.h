@@ -584,6 +584,14 @@ typedef struct avc_audio_desc {
 
 /* STFT (center, reflect padding) of every utterance: one launch. */
 int avc_stft(const avc_audio_desc* d, void* stream);
+/* avc_stft (modes MAG and COMPLEX) of windows of longer signals, for streaming analysis.  A table entry's `reserved`
+ * is its frame origin o >= 0: its frames are frames o, o + 1, ... of a signal, and its n_samples floats are that
+ * signal's samples from max(0, o hop - win/2 - 2): every sample frame o or a later one reads, reflected at the end or
+ * not, is at or after o hop - win/2 - 1, and its pre-emphasis neighbour is inside the entry.  The signal is
+ * reflect-padded at its sample 0 and at the entry's end; an entry that is a window of a signal still arriving lists
+ * only frames whose non-zero window samples lie inside it.  A frame gets avc_stft's bits for the whole signal under
+ * any origin; o = 0 for every entry is avc_stft. */
+int avc_stft_window(const avc_audio_desc* d, void* stream);
 /* iSTFT: irfft x window per frame into `frames`, then a gather overlap-add divided by the exact window sum-square
  * (where it exceeds FLT_MIN) with n_fft/2 cut from each end, into y.  X null: the spectrum is mag with zero phase.
  * Two launches. */
@@ -625,6 +633,42 @@ int avc_griffin_lim_from(const avc_audio_desc* d, int32_t start, float tol, void
 #define AVC_PGHI_RIGHT 3 /* from (f, k+1) */
 #define AVC_PGHI_SEED 4  /* largest bin of a run with no source: phi = 0 */
 int avc_pghi(const avc_audio_desc* d, float tol, int8_t* parent, void* stream);
+/* RTISI-LA: real-time iterative spectrogram inversion with look-ahead (Zhu, Beauregard & Wyse 2007) of many streams,
+ * one CTA each, on the iSTFT's window, grid and normalisation.  A stream's state slot holds its last lookahead + 1
+ * frames ("the buffer"), the overlap-add numerator of its committed frames over the samples still open and its
+ * de-emphasis carry; count holds (frames committed, frames buffered), zero with a zeroed slot for a new stream.
+ * Sample n sits at frame n / hop (mel_to_signal's grid) and frame F covers 0 <= n - F hop + win/2 < win.
+ *   A frame t entering starts from the phase of the STFT, at t, of the current estimate: the numerator plus the
+ *   buffered frames' windowed inverse frames, over the window sum-square of frames 0 .. t-1 (phase 0 where it is 0).
+ *   Then n_iter Jacobi iterations update every buffered frame at once (estimate, STFT, the frame's magnitudes with
+ *   that phase, iSTFT times the window); with lookahead + 1 frames buffered the oldest is then committed, releasing
+ *   the hop samples it completes: numerator / window sum-square of every frame covering them, de-emphasised
+ *   (y[n] = x[n] + deemph y[n-1]); samples before 0 are dropped.
+ *   close: after the new frames, the buffered ones are committed one by one, n_iter iterations each, and the samples
+ *   up to hop (T - 1) released: a stream of T frames gives hop (T - 1) samples in all.
+ * Sums run in a fixed order without atomics: a stream's bits do not depend on the other streams of a launch or on
+ * how its frames were split into launches.  A slot must appear once per launch.  AVC_ERR_UNSUPPORTED for n_fft !=
+ * 2048, an odd win or win > n_fft, hop outside (0, win/2] or lookahead outside [0, AVC_RTISI_MAX_LOOKAHEAD];
+ * AVC_ERR_INVALID for n_iter < 0, a de-emphasis that is not finite or a null pointer; both before any launch. */
+#define AVC_RTISI_MAX_LOOKAHEAD 7
+typedef struct avc_rtisi_desc {
+  int32_t n_fft, hop, win;
+  int32_t lookahead;         /* LA_v: frames after a frame that are iterated with it before it is committed */
+  int32_t n_iter;            /* K >= 0 */
+  int32_t n_streams;         /* CTAs */
+  float deemph;              /* de-emphasis coefficient of the output (0: none) */
+  int32_t reserved;
+  const float* mag;          /* [rows][n_fft/2+1] linear magnitudes of the new frames */
+  const int32_t* mag_off;    /* DEVICE [n_streams + 1]: stream s's new frames are rows mag_off[s] .. mag_off[s+1]-1 */
+  const int32_t* slot;       /* DEVICE [n_streams]: the state slot of stream s */
+  const int32_t* close;      /* DEVICE [n_streams]: non-zero commits every buffered frame after the new ones */
+  const int64_t* out_off;    /* DEVICE [n_streams]: first float of y for stream s's released samples */
+  float* y;                  /* released samples */
+  float* state;              /* DEVICE [slots][avc_rtisi_state_floats(win, lookahead)] */
+  int32_t* count;            /* DEVICE [slots][2] */
+} avc_rtisi_desc;
+int64_t avc_rtisi_state_floats(int win, int lookahead);
+int avc_rtisi_la(const avc_rtisi_desc* d, void* stream);
 /* power[frame] = mean of y^2 over frames of n_fft samples hop apart, reflect-padded by n_fft/2 (librosa's trim
  * statistic): segs frame_off / n_frames count these frames, 1 + n_samples / hop per utterance.  Any even n_fft. */
 int avc_frame_power(const avc_audio_desc* d, float* power, void* stream);

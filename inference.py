@@ -76,8 +76,17 @@ bank's profiles were synthesised with:
 
     python inference.py -c config.yaml -m model.ckpt -a attr.pkl -s src.wav -bank bank.pt -speaker p226 -o out.wav \
         -pitch_shift mv
+
+Streaming: -stream feeds -s to a StreamingConverter (adaptive_voice_conversion_b200/streaming.py) in -stream_chunk_ms
+chunks (default 20 ms) and writes the untrimmed stream it gives back; the target is -t files (their pooled code) or
+-bank -speaker SPEC.  With -pairs every line is one stream, all fed in lockstep.  -stream_hop, -stream_lookahead
+(mel frames, multiples of 8; defaults 8 and 8), -stream_gl_lookahead (default 3) and -stream_gl_iters (default 8) set
+the block schedule and RTISI-LA; -morph, a -pitch_shift other than 0 and the -gl_* options are refused with it:
+
+    python inference.py -c config.yaml -m model.ckpt -a attr.pkl -s src.wav -t tgt.wav -o out.wav -stream
 """
 import os
+import sys
 from argparse import ArgumentParser
 from typing import NamedTuple
 
@@ -401,12 +410,103 @@ def parser():
     p.add_argument("-pitch_shift", default="0", metavar="{SEMITONES,match,mv}",
                    help="transpose every .wav output by SEMITONES in [-24, 24] (formant-preserving), 'match' each "
                         "conversion's pitch level to its -t target's, or 'mv': level and range to any target's")
+    p.add_argument("-stream", action="store_true",
+                   help="convert as a live stream: feed -s in chunks to a StreamingConverter (one stream per -pairs line)")
+    p.add_argument("-stream_chunk_ms", default=20.0, type=float, help="-stream: input chunk length in milliseconds")
+    p.add_argument("-stream_window", default=None, type=int, help="-stream: frames per converted window (segment_size)")
+    p.add_argument("-stream_hop", default=8, type=int, help="-stream: frames emitted per block (multiple of 8)")
+    p.add_argument("-stream_lookahead", default=8, type=int, help="-stream: look-ahead frames of a block's window")
+    p.add_argument("-stream_gl_lookahead", default=3, type=int, help="-stream: RTISI-LA look-ahead frames (0 .. 7)")
+    p.add_argument("-stream_gl_iters", default=8, type=int, help="-stream: RTISI-LA iterations per frame step")
     return p
+
+
+def check_stream_args(p, args, argv):
+    """-stream's refusals (p.error): -morph, a pitch shift, any -gl_* option (streams are synthesised by RTISI-LA), a
+    .npy output, a chunk length that is not positive and a block schedule streaming.check_params refuses."""
+    if args.morph is not None:
+        p.error("-stream converts to one speaker code per stream: -morph is not supported while streaming")
+    if str(args.pitch_shift) not in ("0", "0.0"):
+        p.error("-pitch_shift is not supported with -stream")
+    given = [a.split("=")[0] for a in argv if a.startswith("-gl_")]
+    if given:
+        p.error(f"{given[0]}: -stream synthesises with RTISI-LA (-stream_gl_lookahead, -stream_gl_iters), not "
+                f"Griffin-Lim; -gl_* options are refused")
+    if args.stream_chunk_ms <= 0:
+        p.error("-stream_chunk_ms must be positive")
+    if not args.pairs and not is_wav(args.output):
+        p.error("-stream writes the synthesised stream: -o must be a .wav")
+    from adaptive_voice_conversion_b200.streaming import check_params
+    try:
+        check_params(stream_params(args), 128 if args.stream_window is None else args.stream_window)
+    except ValueError as e:
+        p.error(str(e))
+
+
+def stream_params(args):
+    from adaptive_voice_conversion_b200.streaming import StreamParams
+    return StreamParams(window=args.stream_window, hop=args.stream_hop, lookahead=args.stream_lookahead,
+                        gl_lookahead=args.stream_gl_lookahead, gl_iters=args.stream_gl_iters)
+
+
+def run_stream(args, config, jobs):
+    """-stream: every job's source fed to a StreamingConverter in -stream_chunk_ms chunks, all jobs in lockstep (one
+    update per chunk), and each stream's untrimmed output written.  Targets: -t files or sets (their pooled code,
+    Inferencer.embed_speakers of the trimmed, normalised reference mels) or banked speakers (SpeakerBank.code)."""
+    from adaptive_voice_conversion_b200.streaming import StreamingConverter
+    from adaptive_voice_conversion_b200.vocoder import AudioParams, Vocoder, load_wav
+    dev = local_device()
+    for n, src, t, name in jobs:
+        if not is_wav(src) or not is_wav(name) or not all(is_wav(f) for f in target_files(t)):
+            where = f"line {n}: " if n is not None else ""
+            raise ValueError(f"{where}-stream converts .wav sources to .wav outputs with .wav targets")
+    vocoder = Vocoder(n_mels=config["SpeakerEncoder"]["c_in"] // config["data_loader"]["frame_size"], hp=AudioParams())
+    hp = vocoder.hp
+    inf = Inferencer(config=config, args=args)
+    bank = load_bank(args.bank, inf.model) if args.bank else None
+    refs = sorted({f for _, _, t, _ in jobs for f in target_files(t)})
+    mel = {}
+    if refs:
+        mel = dict(zip(refs, (m for m, _ in vocoder.wav_to_mel([torch.from_numpy(load_wav(f, hp.sr)).to(dev)
+                                                                   for f in refs]))))
+        if inf.attr is not None:
+            mean = torch.as_tensor(np.asarray(inf.attr["mean"], np.float32)).to(dev)
+            std = torch.as_tensor(np.asarray(inf.attr["std"], np.float32)).to(dev)
+            mel = {f: (m - mean) / std for f, m in mel.items()}
+    conv = StreamingConverter(inf, vocoder, stream_params(args))
+    sets = {}
+    ids = []
+    for _, _, t, _ in jobs:
+        if isinstance(t, BankTarget):
+            code = bank.code(t.spec).to(dev)
+        else:
+            key = target_files(t)
+            if key not in sets:
+                sets[key] = inf.embed_speakers([[mel[f] for f in key]])[0]
+            code = sets[key]
+        ids.append(conv.open(code))
+    srcs = [load_wav(src, hp.sr) for _, src, _, _ in jobs]
+    chunk = max(1, int(round(hp.sr * args.stream_chunk_ms / 1000.0)))
+    outs = [[] for _ in jobs]
+    for k in range(0, max(len(y) for y in srcs), chunk):
+        feed = {sid: torch.from_numpy(y[k:k + chunk]) for sid, y in zip(ids, srcs) if k < len(y)}
+        for sid, y in conv.push(feed).items():
+            outs[ids.index(sid)].append(y)
+    for sid, y in conv.update({}, close=ids).items():
+        outs[ids.index(sid)].append(y)
+    print(f"streamed {len(jobs)} stream(s) in {chunk}-sample chunks; latency {conv.latency_samples} samples "
+          f"({conv.latency_samples / hp.sr * 1000:.1f} ms at {hp.sr} Hz)")
+    out_dir = args.output if args.pairs else ""
+    for (_, _, _, name), ys in zip(jobs, outs):
+        inf.write_wav_to_file(torch.cat(ys).cpu().numpy(), os.path.join(out_dir, name))
 
 
 def main(argv=None):
     p = parser()
+    argv = sys.argv[1:] if argv is None else list(argv)
     args = p.parse_args(argv)
+    if args.stream:
+        check_stream_args(p, args, argv)
     check_args(p, args)
     if args.semitones == "mv" and (args.speaker is not None or args.morph is not None):
         try:
@@ -414,6 +514,16 @@ def main(argv=None):
         except ValueError as e:
             p.error(str(e))
     config = load_config(args.config)
+    if args.stream:
+        if args.pairs:
+            jobs = read_pairs(args.pairs, bank=bool(args.bank))
+            os.makedirs(args.output, exist_ok=True)
+        else:
+            target = (BankTarget(args.speaker) if args.speaker is not None else
+                      args.target[0] if len(args.target) == 1 else tuple(args.target))
+            jobs = [(None, args.source, target, args.output)]
+        run_stream(args, config, jobs)
+        raise SystemExit(0)
     if args.pairs:
         run_pairs(args, config)
         raise SystemExit(0)
