@@ -337,6 +337,7 @@ PROTOTYPES = {
     "avc_frame_power": (_i, [C.POINTER(AudioDesc), _p, _p]),
     "avc_deemphasis": (_i, [C.POINTER(AudioDesc), C.c_float, _p]),
     "avc_yin": (_i, [C.POINTER(AudioDesc), C.c_int32, C.c_int32, C.c_int32, C.c_float, _p, _p, _p, _p]),
+    "avc_yin_window": (_i, [C.POINTER(AudioDesc), C.c_int32, C.c_int32, C.c_int32, C.c_float, _p, _p, _p, _p]),
     "avc_pitch_shift": (_i, [_p, _p, _p, C.c_int32, C.c_int32, C.c_int32, _p]),
     "avc_mel_project": (_i, [C.POINTER(MelDesc), _p]),
     "avc_resample_poly": (_i, [C.POINTER(ResampleDesc), _p]),

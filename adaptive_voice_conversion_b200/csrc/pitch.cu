@@ -38,6 +38,23 @@ __device__ __forceinline__ int reflect1(int i, int L) {
   return min(max(i, 0), L - 1);
 }
 
+// The same for an entry that holds samples [first, first + L) of a longer signal, which starts at 0 and ends with the
+// entry: the signal's sample i as an index into the entry.  first = 0 is reflect1(i, L).
+__device__ __forceinline__ int reflect1_window(int i, int first, int L) {
+  if (i < 0) i = -i;
+  if (i >= first + L) i = 2 * (first + L - 1) - i;
+  return min(max(i - first, 0), L - 1);
+}
+
+// avc_yin_window's first sample of an entry with frame origin o, span = win + tau_max: frame o's reads, reflected at
+// the end or not, start at o hop - half with half = floor(span / 2), except for the last frame of a closed signal
+// whose length L is a multiple of hop (o hop = L), whose end reflection reaches down to 2 (L - 1) - (L - half + span - 1)
+// = o hop - ceil(span / 2) - 1: one sample before its span for an even span, two for an odd one
+__host__ __device__ inline int64_t yin_first_sample(int o, int hop, int span) {
+  const int64_t v = (int64_t)o * hop - (span - span / 2) - 1;
+  return v > 0 ? v : 0;
+}
+
 __device__ __forceinline__ double warp_sum_d(double v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
@@ -49,6 +66,9 @@ __device__ __forceinline__ double warp_sum_d(double v) {
 // one fma per term; lags past tau_max are computed on the zero tail and dropped.  Warp 0 then computes the energy,
 // the prefix sums of d (a lane per chunk of consecutive lags, a fixed shuffle scan of the chunk totals), d', the lag
 // choice and the refinement.
+// ORIGIN (avc_yin_window): a table entry's reserved field is its frame origin o, and its samples start at the signal's
+// sample yin_first_sample(o).  It is its own instance, so that avc_yin's kernel keeps its code.
+template <bool ORIGIN>
 __global__ void __launch_bounds__(YIN_MAX_THREADS) yin_kernel(avc_audio_desc d, int win, int tau_min, int tau_max,
                                                               double theta, double* __restrict__ tau_out,
                                                               double* __restrict__ ap_out, double* __restrict__ en_out) {
@@ -59,15 +79,30 @@ __global__ void __launch_bounds__(YIN_MAX_THREADS) yin_kernel(avc_audio_desc d, 
   double* dp = sm + skew(n_stage) + 1;
   const avc_audio_seg g = d.segs[seg_of_frame_yin(d.segs, d.n_seg, f)];
   const int span = win + tau_max, half = span / 2, L = g.n_samples;
-  const int64_t centre = (int64_t)(f - g.frame_off) * d.hop;
-  // one reflection on each side: -half >= -(L-1) and centre + span - half - 1 <= 2 (L-1)
-  if (L < 1 || half > L - 1 || centre + (span - half - 1) > 2 * (int64_t)(L - 1)) {
-    if (t == 0) tau_out[f] = ap_out[f] = en_out[f] = __longlong_as_double(0x7ff8000000000000LL);
-    return;
-  }
   const float* y = d.y + g.sample_off;
-  const int base = (int)centre - half;
-  for (int i = t; i < n_stage; i += nt) xs[skew(i)] = i < span ? (double)__ldg(y + reflect1(base + i, L)) : 0.0;
+  if (ORIGIN) {
+    // frame F = o + f - frame_off of a signal whose samples [first, first + L) the entry holds: its end is the entry's
+    const int o = g.reserved;
+    const int64_t first = o >= 0 ? yin_first_sample(o, d.hop, span) : 0;
+    const int64_t centre = ((int64_t)o + f - g.frame_off) * d.hop, end = first + L;
+    // one reflection on each side, and every read at or after first
+    if (o < 0 || L < 1 || half > end - 1 || centre + (span - half - 1) > 2 * (end - 1) - first) {
+      if (t == 0) tau_out[f] = ap_out[f] = en_out[f] = __longlong_as_double(0x7ff8000000000000LL);
+      return;
+    }
+    const int base = (int)(centre - half);
+    for (int i = t; i < n_stage; i += nt)
+      xs[skew(i)] = i < span ? (double)__ldg(y + reflect1_window(base + i, (int)first, L)) : 0.0;
+  } else {
+    const int64_t centre = (int64_t)(f - g.frame_off) * d.hop;
+    // one reflection on each side: -half >= -(L-1) and centre + span - half - 1 <= 2 (L-1)
+    if (L < 1 || half > L - 1 || centre + (span - half - 1) > 2 * (int64_t)(L - 1)) {
+      if (t == 0) tau_out[f] = ap_out[f] = en_out[f] = __longlong_as_double(0x7ff8000000000000LL);
+      return;
+    }
+    const int base = (int)centre - half;
+    for (int i = t; i < n_stage; i += nt) xs[skew(i)] = i < span ? (double)__ldg(y + reflect1(base + i, L)) : 0.0;
+  }
   __syncthreads();
 
   const int tau0 = 1 + YIN_LAGS * t;
@@ -246,30 +281,49 @@ __global__ void __launch_bounds__(PS_THREADS) pitch_shift_kernel(const float* __
 
 using namespace avc;
 
-extern "C" int avc_yin(const avc_audio_desc* d, int32_t win, int32_t tau_min, int32_t tau_max, float threshold,
-                       double* tau, double* aperiodicity, double* energy, void* stream) {
-  AVC_REQUIRE(d != nullptr, AVC_ERR_INVALID, "avc_yin: null descriptor");
+namespace {
+// avc_yin's and avc_yin_window's argument checks and launch; `name` prefixes every message
+int yin_launch(const avc_audio_desc* d, int32_t win, int32_t tau_min, int32_t tau_max, float threshold, double* tau,
+               double* aperiodicity, double* energy, void* stream, const char* name, bool origin) {
+  AVC_REQUIRE(d != nullptr, AVC_ERR_INVALID, "%s: null descriptor", name);
   AVC_REQUIRE(d->segs != nullptr && d->n_seg > 0 && d->n_frames >= 0, AVC_ERR_INVALID,
-              "avc_yin: empty or missing utterance table (n_seg %d, n_frames %d)", d->n_seg, d->n_frames);
-  AVC_REQUIRE(d->y != nullptr, AVC_ERR_INVALID, "avc_yin: null signal y");
-  AVC_REQUIRE(d->hop > 0, AVC_ERR_INVALID, "avc_yin: hop must be positive (got %d)", d->hop);
+              "%s: empty or missing utterance table (n_seg %d, n_frames %d)", name, d->n_seg, d->n_frames);
+  AVC_REQUIRE(d->y != nullptr, AVC_ERR_INVALID, "%s: null signal y", name);
+  AVC_REQUIRE(d->hop > 0, AVC_ERR_INVALID, "%s: hop must be positive (got %d)", name, d->hop);
   AVC_REQUIRE(tau != nullptr && aperiodicity != nullptr && energy != nullptr, AVC_ERR_INVALID,
-              "avc_yin: null tau, aperiodicity or energy");
+              "%s: null tau, aperiodicity or energy", name);
   AVC_REQUIRE(tau_min >= 1 && tau_min < tau_max, AVC_ERR_INVALID,
-              "avc_yin: tau_min / tau_max must satisfy 1 <= tau_min < tau_max (got %d, %d)", tau_min, tau_max);
-  AVC_REQUIRE(win >= tau_max, AVC_ERR_INVALID, "avc_yin: win must be >= tau_max (got win %d, tau_max %d)", win, tau_max);
+              "%s: tau_min / tau_max must satisfy 1 <= tau_min < tau_max (got %d, %d)", name, tau_min, tau_max);
+  AVC_REQUIRE(win >= tau_max, AVC_ERR_INVALID, "%s: win must be >= tau_max (got win %d, tau_max %d)", name, win,
+              tau_max);
   AVC_REQUIRE((int64_t)win + tau_max <= AVC_YIN_MAX_SPAN, AVC_ERR_UNSUPPORTED,
-              "avc_yin: win + tau_max = %lld exceeds AVC_YIN_MAX_SPAN = %d", (long long)win + tau_max, AVC_YIN_MAX_SPAN);
+              "%s: win + tau_max = %lld exceeds AVC_YIN_MAX_SPAN = %d", name, (long long)win + tau_max,
+              AVC_YIN_MAX_SPAN);
   AVC_REQUIRE(std::isfinite(threshold) && threshold > 0.f && threshold <= 1.f, AVC_ERR_INVALID,
-              "avc_yin: threshold must be finite and in (0, 1] (got %g)", (double)threshold);
+              "%s: threshold must be finite and in (0, 1] (got %g)", name, (double)threshold);
   if (d->n_frames == 0) return AVC_OK;
   const int threads = 32 * cdiv(cdiv(tau_max, YIN_LAGS), 32);
   const size_t smem = sizeof(double) * (size_t)((yin_staged(win, tau_max) + (yin_staged(win, tau_max) >> 4) + 1) +
                                                  (tau_max + 1));
-  yin_kernel<<<d->n_frames, threads, smem, (cudaStream_t)stream>>>(*d, win, tau_min, tau_max, (double)threshold, tau,
-                                                                   aperiodicity, energy);
-  AVC_CHECK_LAUNCH("avc_yin");
+  if (origin)
+    yin_kernel<true><<<d->n_frames, threads, smem, (cudaStream_t)stream>>>(*d, win, tau_min, tau_max,
+                                                                           (double)threshold, tau, aperiodicity, energy);
+  else
+    yin_kernel<false><<<d->n_frames, threads, smem, (cudaStream_t)stream>>>(*d, win, tau_min, tau_max,
+                                                                            (double)threshold, tau, aperiodicity, energy);
+  AVC_CHECK_LAUNCH(name);
   return AVC_OK;
+}
+}  // namespace
+
+extern "C" int avc_yin(const avc_audio_desc* d, int32_t win, int32_t tau_min, int32_t tau_max, float threshold,
+                       double* tau, double* aperiodicity, double* energy, void* stream) {
+  return yin_launch(d, win, tau_min, tau_max, threshold, tau, aperiodicity, energy, stream, "avc_yin", false);
+}
+
+extern "C" int avc_yin_window(const avc_audio_desc* d, int32_t win, int32_t tau_min, int32_t tau_max, float threshold,
+                              double* tau, double* aperiodicity, double* energy, void* stream) {
+  return yin_launch(d, win, tau_min, tau_max, threshold, tau, aperiodicity, energy, stream, "avc_yin_window", true);
 }
 
 extern "C" int avc_pitch_shift(const float* mag, const float* ratio, float* out, int32_t rows, int32_t n_bins,

@@ -13,12 +13,19 @@ Three stages run once per update, each batched over every stream with pending in
   run as one batch (a CUDA graph per batch bucket and length), which gives each its stand-alone bits.
 * synthesis: the blocks' magnitudes go through RTISI-LA (``avc_rtisi_la``), one CTA per stream, which releases
   samples on ``mel_to_signal``'s grid as their frames are committed.
+* pitch (``PitchStage``, per stream, optional): a fixed shift passes each block's magnitudes through
+  ``avc_pitch_shift`` before RTISI-LA.  A target profile (mode, mu_t, sigma_t) synthesises the unshifted magnitudes in
+  a second RTISI-LA pool (the shadow), tracks every shadow frame whose span has been released with
+  ``avc_yin_window``, turns the new frames into shifts on the host (``PitchTracker``, causal) and shifts the buffered
+  magnitudes of those frames before they enter the output RTISI-LA.
 
-``block_schedule``, ``blend_weights`` and ``latency_samples`` state the schedule on the host.
+``block_schedule``, ``blend_weights``, ``latency_samples`` and ``tracked_latency_samples`` state the schedule on the
+host.
 """
 from __future__ import annotations
 
 import ctypes as C
+import math
 import time
 from dataclasses import dataclass
 
@@ -26,9 +33,10 @@ import numpy as np
 import torch
 
 from . import _lib as L
+from .f0 import F0Params
 from .mcd import min_frames
 from .utils import _stream
-from .vocoder import _SEG, _mel_project, _ptr
+from .vocoder import _SEG, PITCH_SHIFT_MAX, _mel_project, _ptr, _ratio
 
 
 @dataclass(frozen=True)
@@ -42,7 +50,10 @@ class StreamParams:
     gl_lookahead: int = 3
     gl_iters: int = 8
     batch_max: int = 1024     # windows per model batch
-    keep_mels: bool = False   # keep each stream's emitted mel frames for take_mels (memory grows with the stream)
+    keep_mels: bool = False   # keep each stream's emitted mel frames for take_mels, and its pitch diagnostics for
+                              # take_pitch (memory grows with the stream)
+    pitch_warmup: int = 50    # voiced frames a tracked stream sees before mv scales its range (0.625 s of voicing at
+                              # 80 frames/s); not tuned
 
 
 def check_params(p: StreamParams, window: int):
@@ -58,6 +69,8 @@ def check_params(p: StreamParams, window: int):
         raise ValueError(f"StreamParams.gl_iters must be >= 0 (got {p.gl_iters})")
     if p.batch_max < 1:
         raise ValueError("StreamParams.batch_max must be >= 1")
+    if p.pitch_warmup < 1:
+        raise ValueError(f"StreamParams.pitch_warmup must be >= 1 (got {p.pitch_warmup})")
 
 
 def min_window(config) -> int:
@@ -106,6 +119,46 @@ def latency_samples(p: StreamParams, win: int, hop_s: int, m: int) -> int:
         if (n + win // 2) // hop_s != c:
             continue
         worst = max(worst, release_sample(n, p, win, hop_s, m) - n)
+    return worst
+
+
+def yin_last_sample(t: int, hop_s: int, span: int) -> int:
+    """The last sample of a signal that YIN frame t (centred at t hop_s, span = W + tau_max samples from
+    t hop_s - floor(span / 2)) reads, with the reflection at sample 0."""
+    half = span // 2
+    return max(t * hop_s + span - half - 1, half - t * hop_s)
+
+
+def yin_ready(n: int, hop_s: int, span: int) -> int:
+    """Frames of a signal still arriving, of which samples 0 .. n - 1 are in, that can be tracked: the t with
+    yin_last_sample(t) < n (for t >= 1 that is t hop_s + span - floor(span / 2) - 1)."""
+    if n <= yin_last_sample(0, hop_s, span):
+        return 0
+    return (n - (span - span // 2)) // hop_s + 1
+
+
+def tracked_release_sample(n: int, p: StreamParams, win: int, hop_s: int, m: int, span: int) -> int:
+    """release_sample for a stream with a target profile: n's last covering frame c is committed by the output RTISI-LA
+    when frame t = c + gl_lookahead enters it, i.e. when YIN frame t has been tracked, i.e. when the shadow has released
+    sample yin_last_sample(t); the shadow releases it once it commits c' frames with c' hop - win/2 beyond it, when
+    frame c' - 1 + gl_lookahead has entered, which happens when its block is emitted."""
+    c = (n + win // 2) // hop_s
+    need = yin_last_sample(c + p.gl_lookahead, hop_s, span)
+    f = (need + win // 2) // hop_s + p.gl_lookahead
+    j = f // p.hop
+    return (block_end(j, p.hop, p.lookahead, m) - 1) * hop_s + win // 2 - 1
+
+
+def tracked_latency_samples(p: StreamParams, win: int, hop_s: int, m: int, span: int) -> int:
+    """max over output samples n >= 0 of tracked_release_sample(n) - n, found as latency_samples finds its own.  With
+    the defaults the tracking delays each frame by D = gl_lookahead + ceil((span - floor(span / 2) + win / 2) / hop) - 1
+    frames (7 at 24 kHz: 3 + 5 - 1)."""
+    worst = 0
+    for c in range(m + 4 * p.hop + 2 * p.gl_lookahead + 2 * (win // hop_s) + span // hop_s + 8):
+        n = max(0, c * hop_s - win // 2)
+        if (n + win // 2) // hop_s != c:
+            continue
+        worst = max(worst, tracked_release_sample(n, p, win, hop_s, m, span) - n)
     return worst
 
 
@@ -284,6 +337,280 @@ class Rtisi:
         return d, dict(zip(ids, torch.split(y[:outs[-1]], counts))), (mag, i32, out_off, y)
 
 
+# ------------------------------------------------------------------ pitch
+PITCH_MODES = ("match", "mv")
+
+
+def parse_pitch(pitch):
+    """None, a fixed shift (float semitones in [-24, 24]; 0 becomes None: nothing to launch) or a target profile
+    (mode, mu_t, sigma_t) with mode "match" or "mv" and finite float64 log2 F0 statistics, sigma_t >= 0.
+    ValueError otherwise."""
+    if pitch is None:
+        return None
+    if isinstance(pitch, (int, float, np.floating, np.integer)) and not isinstance(pitch, bool):
+        v = float(pitch)
+        if not np.isfinite(v) or abs(v) > PITCH_SHIFT_MAX:
+            raise ValueError(f"pitch: a fixed shift must be finite and in [-{PITCH_SHIFT_MAX:g}, {PITCH_SHIFT_MAX:g}] "
+                             f"semitones (got {pitch})")
+        return None if v == 0.0 else v
+    if isinstance(pitch, (tuple, list)) and len(pitch) == 3 and pitch[0] in PITCH_MODES:
+        try:
+            mu, sd = float(pitch[1]), float(pitch[2])
+        except (TypeError, ValueError):
+            mu = sd = float("nan")
+        if np.isfinite(mu) and np.isfinite(sd) and sd >= 0.0:
+            return (pitch[0], mu, sd)
+    raise ValueError(f"pitch: expected None, semitones or (mode in {PITCH_MODES}, log2 mean, log2 std >= 0), "
+                     f"got {pitch!r}")
+
+
+class PitchTracker:
+    """The causal shift rule of one tracked stream, in float64, fed its YIN frames in order.
+
+    Frame t is voiced when aperiodicity < theta, energy > 0 and 10 log10(energy / e_max(t)) >= -silence_db, e_max(t) the
+    largest energy of frames 0..t (``f0.voicing`` with a running floor); its l = log2(sr / tau).  (mu_c, sigma_c) are
+    Welford's running mean and (ddof 0) std of l over the voiced frames 0..t, in frame order.  On a voiced frame the
+    shift is 12 (mu_t - mu_c) for "match" and, for "mv", while fewer than `warmup` voiced frames have been seen or while
+    sigma_c = 0; after that "mv" gives 12 (mu_t + sigma_t / sigma_c (l - mu_c) - l).  Every shift is clamped to +-24.
+    An unvoiced frame holds the last voiced frame's shift, 0 before the first."""
+
+    def __init__(self, mode: str, mu_t: float, sd_t: float, warmup: int, sr: int, params: F0Params = F0Params()):
+        self.mode, self.mu_t, self.sd_t, self.warmup, self.sr = mode, float(mu_t), float(sd_t), int(warmup), sr
+        self.theta, self.floor = params.theta(), -float(params.silence_db)
+        self.emax, self.n, self.mean, self.m2, self.last = 0.0, 0, 0.0, 0.0, 0.0
+
+    def update(self, tau, ap, en):
+        """(log2 F0 (NaN where unvoiced), voiced, shift) float64 / bool / float64 arrays of the next frames."""
+        tau, ap, en = (np.asarray(v, np.float64) for v in (tau, ap, en))
+        emax = np.maximum.accumulate(np.concatenate([[self.emax], en]))[1:]
+        self.emax = float(emax[-1]) if len(emax) else self.emax
+        with np.errstate(divide="ignore", invalid="ignore"):
+            rel = np.where(emax > 0, 10.0 * np.log10(en / np.where(emax > 0, emax, 1.0)), -np.inf)
+            logf = np.where(ap < self.theta, np.log2(self.sr / tau), np.nan)
+        voiced = (ap < self.theta) & (en > 0) & (rel >= self.floor)
+        logf = np.where(voiced, logf, np.nan)
+        shift = np.empty(len(tau))
+        for i in range(len(tau)):
+            if voiced[i]:
+                l = float(logf[i])
+                self.n += 1
+                d = l - self.mean
+                self.mean += d / self.n
+                self.m2 += d * (l - self.mean)
+                sd = math.sqrt(self.m2 / self.n)
+                if self.mode == "mv" and self.n >= self.warmup and sd != 0.0:
+                    v = 12.0 * (self.mu_t + self.sd_t / sd * (l - self.mean) - l)
+                else:
+                    v = 12.0 * (self.mu_t - self.mean)
+                self.last = min(PITCH_SHIFT_MAX, max(-PITCH_SHIFT_MAX, v))
+            shift[i] = self.last
+        return logf, voiced, shift
+
+
+class _PStream:
+    __slots__ = ("ratio", "track", "pend", "frames", "n_rel", "tail", "tail_first", "tracked", "diag")
+
+    def __init__(self, ratio=None, track=None, dev=None, n_bins=0):
+        self.ratio, self.track = ratio, track
+        self.pend = torch.empty(0, n_bins, device=dev)          # unshifted magnitudes of frames not yet tracked
+        self.frames = self.n_rel = self.tail_first = self.tracked = 0
+        self.tail = torch.empty(0, device=dev)                  # shadow samples from tail_first on
+        self.diag = {k: [] for k in ("tau", "aperiodicity", "energy", "log2_f0", "voiced", "shift", "shadow")}
+
+
+class PitchStage:
+    """RTISI-LA synthesis of many streams, each with its own pitch setting (``parse_pitch``): ``open(id, pitch)``, then
+    ``run({id: linear magnitudes [n, n_bins]}, close=())`` returns {id: released samples}, one batched update.
+
+    * None: the magnitudes enter the output RTISI-LA (``rt``) as they are; an update of such streams only is one
+      avc_rtisi_la launch, as before this stage existed.
+    * a fixed shift s: they go through avc_pitch_shift with ratio float32(2^(s/12)) first.
+    * a target profile: they enter the shadow pool (``shadow``, the same look-ahead and iterations), whose output is
+      the unshifted stream's.  Every shadow frame whose span has been released is tracked by one avc_yin_window launch
+      over all streams (F0Params defaults), the YIN outputs come to the host in one copy, ``PitchTracker`` turns them
+      into shifts, and the buffered magnitudes of the newly tracked frames are shifted before they enter ``rt``.  A
+      stream keeps only the shadow samples later frames read.  At close the shadow is closed, its last frames tracked
+      with the end reflection, and the output closed, in the same update.
+    All shifted rows of an update go through one avc_pitch_shift launch.  Every step is per stream and row, so a
+    stream's bits depend neither on how its frames were split into updates nor on the other streams.
+    ``keep`` keeps each tracked stream's per-frame diagnostics and shadow samples for ``take``."""
+
+    def __init__(self, hp, lookahead: int = 3, n_iter: int = 8, device=None, warmup: int = 50, keep: bool = False,
+                 params: F0Params = F0Params()):
+        self.hp, self.params, self.warmup, self.keep = hp, params, int(warmup), keep
+        self.rt = Rtisi(hp, lookahead, n_iter, device)
+        self.shadow = Rtisi(hp, lookahead, n_iter, device)
+        self.dev = self.rt.dev
+        self.tau_min, self.tau_max = params.tau_min(hp.sr), params.tau_max(hp.sr)
+        self.span = int(params.win) + self.tau_max
+        self.streams, self.closed = {}, {}
+        self.stage_ms = None
+
+    def open(self, sid, pitch=None):
+        pitch = parse_pitch(pitch)
+        self.rt.open(sid)
+        if isinstance(pitch, float):
+            self.streams[sid] = _PStream(ratio=np.float32(_ratio(pitch)))
+        elif pitch is not None:
+            self.shadow.open(sid)
+            self.streams[sid] = _PStream(track=PitchTracker(*pitch, self.warmup, self.hp.sr, self.params),
+                                         dev=self.dev, n_bins=self.hp.n_bins)
+
+    def drop(self, sid):
+        self.rt.drop(sid)
+        self.shadow.drop(sid)
+        self.streams.pop(sid, None)
+
+    def tracked(self, sid) -> bool:
+        s = self.streams.get(sid)
+        return s is not None and s.track is not None
+
+    def first_sample(self, o: int) -> int:
+        """avc_yin_window's first sample of an entry with frame origin o."""
+        return max(0, o * self.hp.hop_length - (self.span - self.span // 2) - 1)
+
+    def take(self, sid):
+        """The diagnostics of tracked stream sid since the last call (a closed stream's once): float64 arrays tau,
+        aperiodicity, energy, log2_f0 (NaN where unvoiced), shift, a bool array voiced, and the shadow samples."""
+        if not self.keep:
+            raise ValueError("take_pitch: the converter keeps no pitch diagnostics; build it with "
+                             "StreamParams(keep_mels=True)")
+        if sid in self.closed:
+            d = self.closed.pop(sid)
+        elif self.tracked(sid):
+            d = self.streams[sid].diag
+        else:
+            raise ValueError(f"take_pitch: stream {sid!r} has no target profile")
+        out = {k: (np.concatenate(v) if v else np.zeros(0, bool if k == "voiced" else np.float64)) for k, v in d.items()
+               if k != "shadow"}
+        out["shadow"] = torch.cat(d["shadow"]) if d["shadow"] else torch.empty(0, device=self.dev)
+        for v in d.values():
+            v.clear()
+        return out
+
+    def _tick(self):
+        if self.stage_ms is None:
+            return 0.0
+        torch.cuda.synchronize(self.dev)
+        return time.perf_counter()
+
+    def _lap(self, key, t0):
+        t1 = self._tick()
+        if self.stage_ms is not None:
+            self.stage_ms[key] = self.stage_ms.get(key, 0.0) + 1e3 * (t1 - t0)
+        return t1
+
+    def run(self, mags, close=()):
+        hp = self.hp
+        close = list(close)
+        ids = list(dict.fromkeys(list(mags) + close))
+        tracked = [sid for sid in ids if self.tracked(sid)]
+        for sid in tracked:
+            s = self.streams[sid]
+            T = s.frames + (int(mags[sid].shape[0]) if sid in mags else 0)
+            if sid in close and hp.hop_length * (T - 1) < self.params.min_samples(hp.sr):
+                raise ValueError(f"stream {sid!r}: {T} frames at close; tracking its pitch needs a signal of at least "
+                                 f"{self.params.min_samples(hp.sr)} samples")
+        t0 = self._tick()
+        out = {sid: m for sid, m in mags.items() if sid not in self.streams}
+        rows, ratios, dest = [], [], []          # the rows of this update's avc_pitch_shift launch
+        for sid, m in mags.items():
+            s = self.streams.get(sid)
+            if s is not None and s.track is None and m.shape[0]:
+                rows.append(m)
+                ratios.append(np.full(int(m.shape[0]), s.ratio, np.float32))
+                dest.append(sid)
+        if tracked:
+            t0 = self._track(tracked, mags, close, rows, ratios, dest, t0)
+        if rows:
+            S = torch.cat(rows).float().contiguous()
+            ratio = torch.from_numpy(np.concatenate(ratios)).to(self.dev)
+            shifted = torch.empty_like(S)
+            L.check(L.load().avc_pitch_shift(_ptr(S), _ptr(ratio), _ptr(shifted), S.shape[0], hp.n_bins,
+                                             int(hp.ps_lifter), _stream(self.dev)), "avc_pitch_shift")
+            parts = {}
+            for sid, r in zip(dest, torch.split(shifted, [int(r.shape[0]) for r in rows])):
+                parts.setdefault(sid, []).append(r)
+            for sid, rs in parts.items():
+                out[sid] = rs[0] if len(rs) == 1 else torch.cat(rs)
+        if tracked or rows:
+            t0 = self._lap("shift", t0)
+        res = self.rt.run(out, close)
+        self._lap("rtisi", t0)
+        for sid in close:
+            s = self.streams.pop(sid, None)
+            if s is not None and s.track is not None and self.keep:
+                self.closed[sid] = s.diag
+        return res
+
+    def _track(self, tracked, mags, close, rows, ratios, dest, t0):
+        """The shadow synthesis and tracking of an update, and the host shifts; the newly tracked frames' rows are
+        appended to rows / ratios / dest."""
+        hp, hop = self.hp, self.hp.hop_length
+        shadow_in = {}
+        for sid in tracked:
+            s, m = self.streams[sid], mags.get(sid)
+            if m is not None and m.shape[0]:
+                shadow_in[sid] = m
+                s.pend = torch.cat([s.pend, m.float()])
+                s.frames += int(m.shape[0])
+        res = self.shadow.run(shadow_in, [sid for sid in tracked if sid in close])
+        t0 = self._lap("shadow", t0)
+        segs, ys, entries, soff, foff = [], [], [], 0, 0
+        for sid in tracked:
+            s = self.streams[sid]
+            y = res.get(sid)
+            if y is not None and y.numel():
+                s.tail = torch.cat([s.tail, y])
+                s.n_rel += int(y.numel())
+                if self.keep:
+                    s.diag["shadow"].append(y)
+            ready = s.frames if sid in close else min(s.frames, yin_ready(s.n_rel, hop, self.span))
+            n = ready - s.tracked
+            if n <= 0:
+                continue
+            seg = s.tail[self.first_sample(s.tracked) - s.tail_first:]
+            segs.append((soff, int(seg.numel()), foff, n, s.tracked))
+            ys.append(seg)
+            entries.append((sid, n))
+            soff += int(seg.numel())
+            foff += n
+        if not entries:
+            return t0
+        tab = np.zeros(len(segs), _SEG)
+        for k, name in enumerate(("sample_off", "n_samples", "frame_off", "n_frames", "reserved")):
+            tab[name] = [g[k] for g in segs]
+        table = torch.from_numpy(tab.view(np.uint8)).to(self.dev)
+        y = torch.cat(ys)
+        yin = torch.empty(3, foff, dtype=torch.float64, device=self.dev)
+        d = L.AudioDesc(hop=hop, n_seg=len(segs), n_frames=foff, n_samples=int(soff), segs=_ptr(table), y=_ptr(y))
+        L.check(L.load().avc_yin_window(C.byref(d), int(self.params.win), self.tau_min, self.tau_max,
+                                        C.c_float(self.params.threshold), _ptr(yin[0]), _ptr(yin[1]), _ptr(yin[2]),
+                                        _stream(self.dev)), "avc_yin_window")
+        t0 = self._lap("tracking", t0)
+        host = yin.cpu().numpy()                 # the update's one device-to-host copy
+        t0 = self._lap("tracking_copy", t0)
+        f = 0
+        for sid, n in entries:
+            s = self.streams[sid]
+            tau, ap, en = host[0, f:f + n], host[1, f:f + n], host[2, f:f + n]
+            f += n
+            logf, voiced, shift = s.track.update(tau, ap, en)
+            rows.append(s.pend[:n])
+            ratios.append(np.array([_ratio(v) for v in shift.tolist()], np.float64).astype(np.float32))
+            dest.append(sid)
+            s.pend = s.pend[n:]
+            s.tracked += n
+            keep = self.first_sample(s.tracked)
+            if keep > s.tail_first:
+                s.tail, s.tail_first = s.tail[keep - s.tail_first:], keep
+            if self.keep:
+                for k, v in (("tau", tau), ("aperiodicity", ap), ("energy", en), ("log2_f0", logf),
+                             ("voiced", voiced), ("shift", shift)):
+                    s.diag[k].append(np.array(v))
+        return t0
+
+
 # ------------------------------------------------------------------ the converter
 class _CStream:
     __slots__ = ("code", "hist", "hist_first", "block", "prev", "mels")
@@ -295,13 +622,16 @@ class _CStream:
 
 
 class StreamingConverter:
-    """Converts many live streams at once.  ``open(code)`` starts a stream converted to the speaker code ``code``
-    (float32 [c_out] on the device: a row of ``Inferencer.embed_speakers`` or ``SpeakerBank.code``) and returns its
-    id; ``push({id: pcm})`` takes float32 PCM chunks at ``hp.sr`` of any length and returns {id: new output samples}
-    (device float32), one batched update; ``close(id)`` returns the stream's last samples.  ``take_mels(id)`` hands
-    over the normalised mel frames the stream emitted so far, when the converter keeps them
-    (``StreamParams(keep_mels=True)``; off by default, since they grow with the stream).  ``latency_samples`` is the worst case, over output
-    samples n, of (index of the input sample whose arrival releases n) - n."""
+    """Converts many live streams at once.  ``open(code, pitch=None)`` starts a stream converted to the speaker code
+    ``code`` (float32 [c_out] on the device: a row of ``Inferencer.embed_speakers`` or ``SpeakerBank.code``) with a
+    pitch setting (``PitchStage``: None, a fixed shift in semitones, or a target profile ("match" | "mv", mu_t,
+    sigma_t) of log2 F0) and returns its id; ``push({id: pcm})`` takes float32 PCM chunks at ``hp.sr`` of any length
+    and returns {id: new output samples} (device float32), one batched update; ``close(id)`` returns the stream's last
+    samples.  ``take_mels(id)`` hands over the normalised mel frames the stream emitted so far and ``take_pitch(id)`` a
+    tracked stream's per-frame pitch diagnostics, when the converter keeps them (``StreamParams(keep_mels=True)``; off
+    by default, since they grow with the stream).  ``latency_samples`` is the worst case, over output samples n, of
+    (index of the input sample whose arrival releases n) - n; ``tracked_latency_samples`` the same for streams with a
+    target profile."""
 
     def __init__(self, inferencer, vocoder, params: StreamParams = StreamParams()):
         cfg = inferencer.config
@@ -320,7 +650,9 @@ class StreamingConverter:
         self.dev = vocoder.device
         self.c_out = int(cfg["SpeakerEncoder"]["c_out"])
         self.ana = StreamAnalyzer(vocoder)
-        self.rt = Rtisi(self.hp, params.gl_lookahead, params.gl_iters, self.dev)
+        self.stage = PitchStage(self.hp, params.gl_lookahead, params.gl_iters, self.dev, params.pitch_warmup,
+                                params.keep_mels)
+        self.rt = self.stage.rt
         w = blend_weights(params.hop, params.lookahead)
         self.w_new = torch.from_numpy(w).to(self.dev)[:, None]
         self.w_old = torch.from_numpy(np.float32(1) - w).to(self.dev)[:, None]
@@ -330,18 +662,23 @@ class StreamingConverter:
                               for k in ("mean", "std"))
         self.streams, self.closed = {}, {}
         self._next = 0
-        self.stage_ms = None   # a dict: each update adds its analysis / conversion / rtisi wall time (synchronised)
+        # a dict: each update adds the wall time (synchronised) of analysis, conversion and rtisi, and with pitch
+        # streams of shadow, tracking, tracking_copy (the YIN outputs' copy to the host) and shift
+        self.stage_ms = None
         self.latency_samples = latency_samples(params, self.hp.win_length, self.hp.hop_length, self.m)
+        self.tracked_latency_samples = tracked_latency_samples(params, self.hp.win_length, self.hp.hop_length, self.m,
+                                                               self.stage.span)
 
-    def open(self, code) -> int:
+    def open(self, code, pitch=None) -> int:
         if (not isinstance(code, torch.Tensor) or code.dtype != torch.float32 or tuple(code.shape) != (self.c_out,)
                 or code.device != self.dev):
             raise ValueError(f"StreamingConverter.open: code must be float32 [{self.c_out}] on {self.dev}")
+        parse_pitch(pitch)
         sid = self._next
         self._next += 1
         self.streams[sid] = _CStream(code.contiguous(), self.dev, self.n_mels)
         self.ana.open(sid)
-        self.rt.open(sid)
+        self.stage.open(sid, pitch)
         return sid
 
     def push(self, chunks):
@@ -359,6 +696,13 @@ class StreamingConverter:
         out = torch.cat(mels) if mels else torch.empty(0, self.n_mels, device=self.dev)
         mels.clear()
         return out
+
+    def take_pitch(self, sid):
+        """A stream with a target profile: its per-frame diagnostics since the last call (a closed stream's once), a
+        dict of float64 arrays tau, aperiodicity, energy (the tracker's outputs), log2_f0 (NaN where unvoiced) and
+        shift (semitones), a bool array voiced, and "shadow": the unshifted synthesis released since the last call.
+        Needs StreamParams(keep_mels=True)."""
+        return self.stage.take(sid)
 
     @torch.no_grad()
     def update(self, chunks, close=()):
@@ -420,11 +764,11 @@ class StreamingConverter:
             if keep > s.hist_first:
                 s.hist, s.hist_first = s.hist[keep - s.hist_first:], keep
         t2 = self._tick()
-        res = self.rt.run(mags, close)
         if self.stage_ms is not None:
-            t3 = self._tick()
-            for k, a, b in (("analysis", t0, t1), ("conversion", t1, t2), ("rtisi", t2, t3)):
+            for k, a, b in (("analysis", t0, t1), ("conversion", t1, t2)):
                 self.stage_ms[k] = self.stage_ms.get(k, 0.0) + 1e3 * (b - a)
+        self.stage.stage_ms = self.stage_ms
+        res = self.stage.run(mags, close)
         for sid in close:
             mels = self.streams.pop(sid).mels
             if self.p.keep_mels:

@@ -694,6 +694,18 @@ int avc_deemphasis(const avc_audio_desc* d, float coef, void* stream);
 #define AVC_YIN_MAX_SPAN 3072
 int avc_yin(const avc_audio_desc* d, int32_t win, int32_t tau_min, int32_t tau_max, float threshold, double* tau,
             double* aperiodicity, double* energy, void* stream);
+/* avc_yin over windows of longer signals, for tracking signals as they arrive.  A table entry's `reserved` is its frame
+ * origin o >= 0: its frames are frames o, o + 1, ... of a signal, and its n_samples floats are that signal's samples
+ * from max(0, o hop - ceil((win + tau_max) / 2) - 1): frame o's span, which starts at o hop - floor((win + tau_max) / 2),
+ * and the samples before it that the end reflection of a closed signal's last frame reads when the signal's length is
+ * a multiple of hop (down to o hop - ceil((win + tau_max) / 2) - 1).  The signal is
+ * reflect-padded at its sample 0 and at the entry's end; an entry that is a window of a signal still arriving lists
+ * only frames whose span lies inside it.  A frame gets avc_yin's bits for the whole signal under any origin and any
+ * split of the signal into entries; o = 0 for every entry is avc_yin.  A frame whose reads would leave the entry, or
+ * need a second reflection, and every frame of an entry with o < 0, gets NaN.  The same argument checks, codes and
+ * messages (named avc_yin_window) as avc_yin, before any launch. */
+int avc_yin_window(const avc_audio_desc* d, int32_t win, int32_t tau_min, int32_t tau_max, float threshold,
+                   double* tau, double* aperiodicity, double* energy, void* stream);
 
 /* Formant-preserving pitch shift of rows of linear magnitudes (csrc/pitch.cu), fp32.  mag and out [rows][n_bins], ratio
  * [rows] (device memory).  Per row, with N = 2 (n_bins - 1), Q = lifter and alpha = ratio[row]:

@@ -84,6 +84,17 @@ chunks (default 20 ms) and writes the untrimmed stream it gives back; the target
 the block schedule and RTISI-LA; -morph, a -pitch_shift other than 0 and the -gl_* options are refused with it:
 
     python inference.py -c config.yaml -m model.ckpt -a attr.pkl -s src.wav -t tgt.wav -o out.wav -stream
+
+-stream_pitch moves a stream's pitch as it is synthesised (streaming.PitchStage).  SEMITONES (in [-24, 24]) shifts every
+block by a fixed amount and adds no latency.  match and mv track the stream's unshifted synthesis causally and move its
+running pitch level (match) or level and range (mv) to the target's profile, at the cost of the longer
+tracked latency the run prints.  The profile of -t files and sets is tracked from the references synthesised by
+RTISI-LA at the stream's settings; a banked target (-speaker, @SPEC lines) uses the bank's pitch record (its references
+were synthesised by Griffin-Lim), so a bank without one is refused.  Unlike -pitch_shift match, -stream_pitch match
+accepts banked targets: both modes read the same profile.  A target without a voiced frame leaves its stream unshifted:
+
+    python inference.py -c config.yaml -m model.ckpt -a attr.pkl -s src.wav -bank bank.pt -speaker p225 -o out.wav \
+        -stream -stream_pitch mv
 """
 import os
 import sys
@@ -210,12 +221,12 @@ def refuse_bank_targets(pairs, path):
                              f"(@{t.spec}) has none")
 
 
-def refuse_unprofiled_bank(path):
+def refuse_unprofiled_bank(path, option="-pitch_shift mv"):
     """ValueError when the bank file at `path` has no pitch profiles (read on the host, before any model or GPU work):
-    -pitch_shift mv needs them for a banked target."""
+    `option` (-pitch_shift mv, -stream_pitch match or -stream_pitch mv) needs them for a banked target."""
     d = torch.load(path, map_location="cpu", weights_only=True)
     if not isinstance(d, dict) or d.get("pitch") is None:
-        raise ValueError(f"{path}: the bank has no pitch profiles, which -pitch_shift mv needs for a banked target; "
+        raise ValueError(f"{path}: the bank has no pitch profiles, which {option} needs for a banked target; "
                          f"rebuild it with speaker_bank.py -f0")
 
 
@@ -418,6 +429,9 @@ def parser():
     p.add_argument("-stream_lookahead", default=8, type=int, help="-stream: look-ahead frames of a block's window")
     p.add_argument("-stream_gl_lookahead", default=3, type=int, help="-stream: RTISI-LA look-ahead frames (0 .. 7)")
     p.add_argument("-stream_gl_iters", default=8, type=int, help="-stream: RTISI-LA iterations per frame step")
+    p.add_argument("-stream_pitch", default=None, metavar="{SEMITONES,match,mv}",
+                   help="-stream: shift every block by SEMITONES in [-24, 24], or track the stream and 'match' its "
+                        "pitch level, or 'mv' its level and range, to the target's profile")
     return p
 
 
@@ -427,7 +441,8 @@ def check_stream_args(p, args, argv):
     if args.morph is not None:
         p.error("-stream converts to one speaker code per stream: -morph is not supported while streaming")
     if str(args.pitch_shift) not in ("0", "0.0"):
-        p.error("-pitch_shift is not supported with -stream")
+        p.error("-pitch_shift is not supported with -stream; use -stream_pitch {SEMITONES,match,mv}")
+    stream_pitch_arg(p, args)
     given = [a.split("=")[0] for a in argv if a.startswith("-gl_")]
     if given:
         p.error(f"{given[0]}: -stream synthesises with RTISI-LA (-stream_gl_lookahead, -stream_gl_iters), not "
@@ -441,6 +456,20 @@ def check_stream_args(p, args, argv):
         check_params(stream_params(args), 128 if args.stream_window is None else args.stream_window)
     except ValueError as e:
         p.error(str(e))
+
+
+def stream_pitch_arg(p, args):
+    """args.stream_pitch becomes None, "match", "mv" or a float in [-24, 24] (p.error otherwise)."""
+    from adaptive_voice_conversion_b200.vocoder import PITCH_SHIFT_MAX
+    v = args.stream_pitch
+    if v is None or v in ("match", "mv"):
+        return
+    try:
+        args.stream_pitch = float(v)
+    except ValueError:
+        p.error(f"-stream_pitch must be a number of semitones or 'match' or 'mv' (got {v!r})")
+    if not np.isfinite(args.stream_pitch) or abs(args.stream_pitch) > PITCH_SHIFT_MAX:
+        p.error(f"-stream_pitch must be finite and in [-{PITCH_SHIFT_MAX:g}, {PITCH_SHIFT_MAX:g}] semitones (got {v})")
 
 
 def stream_params(args):
@@ -460,23 +489,29 @@ def run_stream(args, config, jobs):
         if not is_wav(src) or not is_wav(name) or not all(is_wav(f) for f in target_files(t)):
             where = f"line {n}: " if n is not None else ""
             raise ValueError(f"{where}-stream converts .wav sources to .wav outputs with .wav targets")
+    tracked = args.stream_pitch in ("match", "mv")
+    if tracked and any(isinstance(t, BankTarget) for _, _, t, _ in jobs):
+        refuse_unprofiled_bank(args.bank, f"-stream_pitch {args.stream_pitch}")
     vocoder = Vocoder(n_mels=config["SpeakerEncoder"]["c_in"] // config["data_loader"]["frame_size"], hp=AudioParams())
     hp = vocoder.hp
     inf = Inferencer(config=config, args=args)
     bank = load_bank(args.bank, inf.model) if args.bank else None
     refs = sorted({f for _, _, t, _ in jobs for f in target_files(t)})
-    mel = {}
+    raw, mel = {}, {}
     if refs:
-        mel = dict(zip(refs, (m for m, _ in vocoder.wav_to_mel([torch.from_numpy(load_wav(f, hp.sr)).to(dev)
+        raw = dict(zip(refs, (m for m, _ in vocoder.wav_to_mel([torch.from_numpy(load_wav(f, hp.sr)).to(dev)
                                                                    for f in refs]))))
+        mel = raw
         if inf.attr is not None:
             mean = torch.as_tensor(np.asarray(inf.attr["mean"], np.float32)).to(dev)
             std = torch.as_tensor(np.asarray(inf.attr["std"], np.float32)).to(dev)
-            mel = {f: (m - mean) / std for f, m in mel.items()}
-    conv = StreamingConverter(inf, vocoder, stream_params(args))
+            mel = {f: (m - mean) / std for f, m in raw.items()}
+    params = stream_params(args)
+    conv = StreamingConverter(inf, vocoder, params)
+    profiles = stream_profiles(jobs, raw, bank, vocoder, params) if tracked else None
     sets = {}
     ids = []
-    for _, _, t, _ in jobs:
+    for k, (n, _, t, name) in enumerate(jobs):
         if isinstance(t, BankTarget):
             code = bank.code(t.spec).to(dev)
         else:
@@ -484,7 +519,13 @@ def run_stream(args, config, jobs):
             if key not in sets:
                 sets[key] = inf.embed_speakers([[mel[f] for f in key]])[0]
             code = sets[key]
-        ids.append(conv.open(code))
+        pitch = args.stream_pitch
+        if tracked:
+            pr = profiles[k]
+            pitch = None if pr is None else (args.stream_pitch, pr[0], pr[1])
+            print(f"{name}: -stream_pitch {args.stream_pitch} " + ("unmatched: the target has no voiced frame, every "
+                  "shift is 0" if pr is None else f"toward log2 F0 mean {pr[0]:.4f}, std {pr[1]:.4f}"))
+        ids.append(conv.open(code, pitch))
     srcs = [load_wav(src, hp.sr) for _, src, _, _ in jobs]
     chunk = max(1, int(round(hp.sr * args.stream_chunk_ms / 1000.0)))
     outs = [[] for _ in jobs]
@@ -495,10 +536,41 @@ def run_stream(args, config, jobs):
     for sid, y in conv.update({}, close=ids).items():
         outs[ids.index(sid)].append(y)
     print(f"streamed {len(jobs)} stream(s) in {chunk}-sample chunks; latency {conv.latency_samples} samples "
-          f"({conv.latency_samples / hp.sr * 1000:.1f} ms at {hp.sr} Hz)")
+          f"({conv.latency_samples / hp.sr * 1000:.1f} ms at {hp.sr} Hz), with pitch tracking "
+          f"{conv.tracked_latency_samples} samples ({conv.tracked_latency_samples / hp.sr * 1000:.1f} ms)")
     out_dir = args.output if args.pairs else ""
     for (_, _, _, name), ys in zip(jobs, outs):
         inf.write_wav_to_file(torch.cat(ys).cpu().numpy(), os.path.join(out_dir, name))
+
+
+def stream_profiles(jobs, raw, bank, vocoder, params):
+    """The (log2 mean, log2 std) target profile of every job for -stream_pitch match / mv, or None (unmatched).  -t
+    files and sets: their denormalised mels (raw) synthesised through RTISI-LA at the converter's settings, tracked by
+    the streams' tracker (f0.yin, which gives avc_yin_window's bits, and f0.voicing) and pooled (f0.track_profile).
+    Banked targets: SpeakerBank.pitch_profile, with a note that the bank's record was synthesised by Griffin-Lim.
+    ValueError naming the file, before any synthesis, for a reference too short for the tracker."""
+    from adaptive_voice_conversion_b200.f0 import F0Params, track, track_profile
+    from adaptive_voice_conversion_b200.streaming import Rtisi
+    hp = vocoder.hp
+    refs = sorted({f for _, _, t, _ in jobs if not isinstance(t, BankTarget) for f in target_files(t)})
+    need = F0Params().min_samples(hp.sr)
+    for f in refs:
+        n = hp.hop_length * (int(raw[f].shape[0]) - 1)     # the synthesis of T frames has hop (T - 1) samples
+        if n < need:
+            raise ValueError(f"{f}: -stream_pitch tracks the pitch of the target's references; after trimming this one "
+                             f"synthesises to {n} samples, and the tracker needs at least {need}")
+    tracks = {}
+    if refs:
+        rt = Rtisi(hp, params.gl_lookahead, params.gl_iters, vocoder.device)
+        for f in refs:
+            rt.open(f)
+        sig = rt.run(dict(zip(refs, vocoder.mel_to_mag([raw[f] for f in refs]))), close=refs)
+        tracks = dict(zip(refs, track([sig[f] for f in refs], hp.sr, hp.hop_length)))
+    if any(isinstance(t, BankTarget) for _, _, t, _ in jobs):
+        print(f"note: the bank's pitch records were tracked from Griffin-Lim copy-syntheses "
+              f"({bank.pitch['griffin_lim']}), not RTISI-LA")
+    return [bank.pitch_profile(t.spec) if isinstance(t, BankTarget) else track_profile([tracks[f] for f in target_files(t)])
+            for _, _, t, _ in jobs]
 
 
 def main(argv=None):
@@ -507,12 +579,16 @@ def main(argv=None):
     args = p.parse_args(argv)
     if args.stream:
         check_stream_args(p, args, argv)
+    elif args.stream_pitch is not None:
+        p.error("-stream_pitch needs -stream (offline conversions take -pitch_shift)")
     check_args(p, args)
-    if args.semitones == "mv" and (args.speaker is not None or args.morph is not None):
-        try:
+    try:
+        if args.semitones == "mv" and (args.speaker is not None or args.morph is not None):
             refuse_unprofiled_bank(args.bank)
-        except ValueError as e:
-            p.error(str(e))
+        elif args.stream and args.stream_pitch in ("match", "mv") and args.speaker is not None:
+            refuse_unprofiled_bank(args.bank, f"-stream_pitch {args.stream_pitch}")
+    except ValueError as e:
+        p.error(str(e))
     config = load_config(args.config)
     if args.stream:
         if args.pairs:

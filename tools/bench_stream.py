@@ -2,6 +2,7 @@
 in real time.
 
     python tools/bench_stream.py [--streams 1 64 1024 4096] [--updates 20] [--config config.yaml] [-m ckpt -a attr]
+                                 [-pitch {0,SEMITONES,match,mv}]
 
 Reports, in one JSON line (and a summary on stderr):
   - per stream count S, at the default StreamParams (H = 8 frames = 100 ms per block): the mean wall time of one
@@ -13,12 +14,20 @@ Reports, in one JSON line (and a summary on stderr):
     Griffin-Lim's (avc_griffin_lim, 16 iterations on the same number of frames, median of 7);
   - with -m and -a: the frame-aligned mel L1 and cepstral distance (avc_mel_cepstrum, no DTW: the same frame grid)
     between the streamed mel and the offline conversion of the same untrimmed input.
+  - with -pitch: every stream opened with that pitch setting (a fixed shift, or match / mv toward log2 F0 mean
+    log2(200 Hz), std 0.15), the stages then include shadow, tracking, tracking_copy (the YIN outputs' one
+    device-to-host copy) and shift; the latency with tracking; the avc_yin_window kernel alone (CUDA events on tables
+    prepared beforehand, median of 7) at 64 and 1 024 streams x 8 frames; and for match / mv the output's voiced log2
+    F0 mean and std error (semitones, median over 5 synthetic glides, seeds 0-4) after warm-up, tracked offline, for
+    glides pushed as magnitudes through PitchStage toward the GPU test's target (log2(220 Hz), 0.15), the test's
+    seeds 0-2 among them.
 The model has random weights unless -m is given; the input is synthetic (harmonic tones).  The card name and power
 limit are read in the same run.  Writes nothing.
 """
 import argparse
 import dataclasses
 import json
+import math
 import os
 import subprocess
 import sys
@@ -45,6 +54,42 @@ def harmonic(n, sr, seed):
     return torch.from_numpy(h(n, sr, seed=seed).astype(np.float32))
 
 
+def yin_window_ms(n_streams, hp, dev, frames=8, origin=40):
+    """avc_yin_window alone: n_streams entries of `frames` frames each at a steady-state origin, the table and buffers
+    prepared beforehand, CUDA events around the C call (median of 7 after a warm-up)."""
+    import ctypes as C
+    from adaptive_voice_conversion_b200 import _lib as L
+    from adaptive_voice_conversion_b200.f0 import F0Params
+    from adaptive_voice_conversion_b200.streaming import yin_last_sample
+    from adaptive_voice_conversion_b200.utils import _stream
+    from adaptive_voice_conversion_b200.vocoder import _SEG, _ptr
+    fp = F0Params()
+    span = fp.win + fp.tau_max(hp.sr)
+    first = max(0, origin * hp.hop_length - span // 2 - 1)
+    n = yin_last_sample(origin + frames - 1, hp.hop_length, span) + 1 - first
+    y = torch.randn(n_streams * n, device=dev)
+    tab = np.zeros(n_streams, _SEG)
+    for k in range(n_streams):
+        tab[k] = (k * n, n, k * frames, frames, origin)
+    table = torch.from_numpy(tab.view(np.uint8)).to(dev)
+    out = torch.empty(3, n_streams * frames, dtype=torch.float64, device=dev)
+    d = L.AudioDesc(hop=hp.hop_length, n_seg=n_streams, n_frames=n_streams * frames, n_samples=int(y.numel()),
+                    segs=_ptr(table), y=_ptr(y))
+    ev = [torch.cuda.Event(enable_timing=True) for _ in range(2)]
+    times = []
+    for i in range(8):
+        torch.cuda.synchronize()
+        ev[0].record()
+        L.check(L.load().avc_yin_window(C.byref(d), fp.win, fp.tau_min(hp.sr), fp.tau_max(hp.sr),
+                                        C.c_float(fp.threshold), _ptr(out[0]), _ptr(out[1]), _ptr(out[2]),
+                                        _stream(dev)), "avc_yin_window")
+        ev[1].record()
+        torch.cuda.synchronize()
+        if i:
+            times.append(ev[0].elapsed_time(ev[1]))
+    return sorted(times)[len(times) // 2]
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--streams", type=int, nargs="+", default=[1, 64, 1024, 4096])
@@ -53,7 +98,10 @@ def main():
     ap.add_argument("-m", "--model")
     ap.add_argument("-a", "--attr")
     ap.add_argument("--quality-seconds", type=float, default=6.0)
+    ap.add_argument("-pitch", "--pitch", default="0", help="pitch setting of every stream: 0, SEMITONES, match or mv")
     args = ap.parse_args()
+    target = (math.log2(200.0), 0.15)
+    pitch = (args.pitch, *target) if args.pitch in ("match", "mv") else (float(args.pitch) or None)
     if not torch.cuda.is_available():
         raise SystemExit("bench_stream.py needs a CUDA device")
     from adaptive_voice_conversion_b200.config import load_config
@@ -71,11 +119,14 @@ def main():
     block = p.hop * hp.hop_length
     budget_ms = 1e3 * block / hp.sr
     c_out = cfg["SpeakerEncoder"]["c_out"]
-    res = {"card": card(), "params": p.__dict__, "block_ms": budget_ms, "n_mels": hp.n_mels, "stages": {}}
+    res = {"card": card(), "params": p.__dict__, "block_ms": budget_ms, "n_mels": hp.n_mels, "pitch": args.pitch,
+           "stages": {}}
     rt_ms = None
     for S in args.streams:
         conv = StreamingConverter(inf, voc, p)
-        ids = [conv.open(torch.randn(c_out, generator=torch.Generator().manual_seed(i)).to(dev)) for i in range(S)]
+        ids = [conv.open(torch.randn(c_out, generator=torch.Generator().manual_seed(i)).to(dev), pitch)
+               for i in range(S)]
+        res["latency_samples"], res["tracked_latency_samples"] = conv.latency_samples, conv.tracked_latency_samples
         sig = harmonic(block * (args.updates + 40), hp.sr, seed=S).to(dev)
         # start-up (the first block needs m frames, start-up windows of every length) and graph captures
         pos = 0
@@ -90,8 +141,8 @@ def main():
         st = {k: v / args.updates for k, v in conv.stage_ms.items()}
         st["update"] = sum(st.values())
         res["stages"][S] = st
-        print(f"S={S:5d}: update {st['update']:.2f} ms (analysis {st['analysis']:.2f}, conversion "
-              f"{st['conversion']:.2f}, rtisi {st['rtisi']:.2f}); block {budget_ms:.0f} ms", file=sys.stderr)
+        parts = ", ".join(f"{k} {v:.2f}" for k, v in st.items() if k != "update")
+        print(f"S={S:5d}: update {st['update']:.2f} ms ({parts}); block {budget_ms:.0f} ms", file=sys.stderr)
         if S == max(args.streams):
             # the avc_rtisi_la kernel alone: one steady-state update's tables and buffers prepared once, then the C
             # call timed by CUDA events, each launch from a copy of the same state (the copy outside the events)
@@ -137,6 +188,17 @@ def main():
         torch.cuda.empty_cache()
     fits = [S for S, st in res["stages"].items() if st["update"] <= budget_ms]
     res["max_realtime_streams_measured"] = max(fits) if fits else 0
+    if args.pitch in ("match", "mv"):
+        res["yin_window_kernel"] = {n: yin_window_ms(n, hp, dev) for n in (64, 1024)}
+        for n, ms in res["yin_window_kernel"].items():
+            print(f"avc_yin_window kernel, {n} streams x 8 frames: {ms:.3f} ms", file=sys.stderr)
+        from test_gpu_stream_pitch import GLIDE_TARGET, glide_errors
+        errs = [glide_errors((args.pitch, *GLIDE_TARGET), seed, warmup=p.pitch_warmup) for seed in range(5)]
+        res["glide"] = {"mean_error_st": float(np.median([e[0] for e in errs])),
+                        "std_error_st": float(np.median([e[1] for e in errs])),
+                        "per_glide": [[float(a), float(b), int(c)] for a, b, c in errs]}
+        print(f"glide after warm-up: median error of the voiced mean {res['glide']['mean_error_st']:.3f} st, of the "
+              f"std {res['glide']['std_error_st']:.3f} st", file=sys.stderr)
     if args.model and args.attr:
         from adaptive_voice_conversion_b200.mcd import mel_cepstrum
         conv = StreamingConverter(inf, voc, dataclasses.replace(p, keep_mels=True))
@@ -157,7 +219,8 @@ def main():
                           "cepstral_distance": float((cs[:, 1:] - co[:, 1:]).pow(2).sum(1).sqrt().mean()),
                           "frames": int(mel.shape[0])}
         print(f"quality vs offline: {res['quality']}", file=sys.stderr)
-    print(f"card: {res['card']}; largest measured S in real time: {res['max_realtime_streams_measured']}", file=sys.stderr)
+    print(f"card: {res['card']}; largest measured S in real time: {res['max_realtime_streams_measured']}; latency "
+          f"{res.get('latency_samples')} samples, tracked {res.get('tracked_latency_samples')}", file=sys.stderr)
     print(json.dumps(res))
 
 
