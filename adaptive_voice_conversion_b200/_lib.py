@@ -281,7 +281,6 @@ PROTOTYPES = {
     "avc_conv_block_tc_plan": (_i, [C.POINTER(ConvDesc), _i, C.POINTER(TcPlan)]),
     "avc_pack_conv_weight_tc": (_i, [_p, _p, _i, _i, _i, _i, _p]),
     "avc_tc_packed_floats": (_i64, [_i, _i, _i]),
-    "avc_tc2_set_debug": (None, [_p]),
     "avc_pack_conv_weights_batch": (_i, [_p, _i, _i64, _p]),
     "avc_norm_apply_fwd": (_i, [C.POINTER(ConvDesc), _p]),
     "avc_norm_bwd": (_i, [C.POINTER(ConvDesc), _p]),
@@ -361,7 +360,6 @@ PROTOTYPES = {
     "avc_spectral_norm_bwd": (_i, [_p, _i, _i, _i, _p, _p]),
     "avc_tc_probe_gemm": (_i, [_p, _i, _p, _i, C.POINTER(C.c_uint32), _i, _i, _i, _i, _i, _p, _p, _p]),
     "avc_tc_probe_set_ld_shift": (None, [_i]),
-    "avc_probe_store": (_i, [_p, C.c_longlong, _i, _i, _p, _p]),
     "avc_last_error": (C.c_char_p, []),
     "avc_build_info": (C.c_char_p, []),
     "avc_launch_count": (_i64, []),

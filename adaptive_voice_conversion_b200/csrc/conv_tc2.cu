@@ -62,7 +62,6 @@ struct Tc2Args {
   uint32_t off_tile, off_par, off_stat;  // byte offsets inside dynamic shared memory
   int patch;    // 1: the patch warps sit between the bulk copy and the MMAs (halo rows and/or TF32 rounding)
   int* status;
-  long long* dbg;
 };
 
 __device__ __forceinline__ float t2_round_tf32(float x) {
@@ -271,8 +270,6 @@ __global__ void __launch_bounds__(T2_THREADS, 1) conv_block_tc2_kernel(const Tc2
     tc::fence_mbar_init();
   }
   __syncthreads();
-  // CTA start time goes out at once: a value live across the register split would be spilled
-  if (a.dbg && tid == 0) a.dbg[(size_t)blockIdx.x * 16] = clock64();
 
   if (warp < 4) {
     tc::setmaxnreg_dec<T2_REGS_PRODUCER>();   // all four warps, also patch warps that idle (a.patch == 0)
@@ -282,16 +279,13 @@ __global__ void __launch_bounds__(T2_THREADS, 1) conv_block_tc2_kernel(const Tc2
       uint32_t ph = 0;
       bool ok = true;
       bool first_round = true;
-      long long dbg0 = 0;
       for (int tile = blockIdx.x; tile < a.ntiles && ok; tile += gridDim.x) {
         const TileCoord c = t2_decode(a, tile);
         const float* wsrc = d.w_tc + (size_t)c.mtile * a.nslab * ((size_t)K * (T2_WTAP_BYTES / 4));
         const int tstart = c.t0 * S - d.pad_left;   // first input position of the staged rows (may be negative)
         for (int ii = 0; ii < a.nst * a.nchunk; ++ii) {   // every column chunk streams the same stages again
           const int i = ii % a.nst;
-          const long long w0 = a.dbg ? clock64() : 0;
           if (!first_round) ok = __all_sync(0xffffffffu, tc::mbar_wait(&bar_empty[s], ph ^ 1u, a.status, 2));
-          if (a.dbg) dbg0 += clock64() - w0;
           if (!ok) break;
           uint8_t* sw = smem + (size_t)s * a.stage_bytes;
           const int h0 = i * a.hs, nh = min(a.hs, a.nhalf - h0);   // half-slabs [h0, h0 + nh) of the tile
@@ -312,7 +306,6 @@ __global__ void __launch_bounds__(T2_THREADS, 1) conv_block_tc2_kernel(const Tc2
           if (++s == a.nstage) { s = 0; ph ^= 1u; first_round = false; }
         }
       }
-      if (a.dbg && lane == 0) a.dbg[(size_t)blockIdx.x * 16 + 2] = dbg0;
     } else {
       // ================================================================ patch warps (3 warps, ROUND ROBIN over the stages)
       // (a) reflect padding: the copy engine delivered zeros for the rows outside the sample; they are overwritten
@@ -336,7 +329,6 @@ __global__ void __launch_bounds__(T2_THREADS, 1) conv_block_tc2_kernel(const Tc2
       int s = 0;
       uint32_t ph = 0;
       bool ok = true;
-      long long dbg0 = 0, dbg1 = 0;
       for (int tile = blockIdx.x; a.patch && pw < npw && tile < a.ntiles && ok; tile += gridDim.x) {
         const TileCoord c = t2_decode(a, tile);
         const int pbeg = c.t0 * S - d.pad_left;
@@ -370,10 +362,7 @@ __global__ void __launch_bounds__(T2_THREADS, 1) conv_block_tc2_kernel(const Tc2
         for (int ii = 0; ii < a.nst * a.nchunk && ok; ++ii) {
           const int i = ii % a.nst;
           if (s % npw == pw) {
-            const long long w0 = a.dbg ? clock64() : 0;
             ok = tc::mbar_wait(&bar_fullx[s], ph, a.status, 4);
-            const long long w1 = a.dbg ? clock64() : 0;
-            dbg0 += w1 - w0;
             if (!ok) break;
             float4* sx = reinterpret_cast<float4*>(smem + (size_t)s * a.stage_bytes + a.w_bytes);
             bool wrote = false;
@@ -420,14 +409,9 @@ __global__ void __launch_bounds__(T2_THREADS, 1) conv_block_tc2_kernel(const Tc2
             if (wrote) tc::fence_proxy_async_smem();   // only writers pay for the proxy fence
             __syncwarp();
             if (lane == 0) tc::mbar_arrive(&bar_ready[s]);
-            if (a.dbg) dbg1 += clock64() - w1;
           }
           if (++s == a.nstage) { s = 0; ph ^= 1u; }
         }
-      }
-      if (a.dbg && tid == 32) {
-        long long* o = a.dbg + (size_t)blockIdx.x * 16;
-        o[3] = dbg0; o[4] = dbg1;
       }
     }
   } else {
@@ -460,11 +444,8 @@ __global__ void __launch_bounds__(T2_THREADS, 1) conv_block_tc2_kernel(const Tc2
     const bool rnd_out = (d.flags & AVC_F_ROUND_OUT) != 0;
     bool ok = true;
     int tl = 0;
-    long long dbg0 = 0, dbg1 = 0, dbg2 = 0, dbg3 = 0, dbg4 = 0, dbg5 = 0;
     for (int tile = blockIdx.x; tile < a.ntiles; tile += gridDim.x, ++tl) {
       const TileCoord c = t2_decode(a, tile);
-      long long e3b = 0;
-      const long long e0 = a.dbg ? clock64() : 0;
       // ---------------- main loop, then pass 0: accumulators (+bias) -> staged A4 tile
       for (int ch = 0; ch < a.nchunk; ++ch) {
         const int col0 = ch * N;
@@ -473,7 +454,6 @@ __global__ void __launch_bounds__(T2_THREADS, 1) conv_block_tc2_kernel(const Tc2
                              : t2_tile<N>(a, c, smem0, bar_full, bar_fullx, bar_ready, bar_empty, s, ph, stile, wg, wt, col0);
         ok = ok && mok;
       }
-      const long long e1 = a.dbg ? clock64() : 0;
       const int co = c.mtile * 128 + col_l;
       const bool co_ok = co < d.Cout;
       t2_bar_sync(2, 256);
@@ -492,7 +472,6 @@ __global__ void __launch_bounds__(T2_THREADS, 1) conv_block_tc2_kernel(const Tc2
           stat[(1 * a.G + g) * 128 + r] = make_float2(0.f, 0.f);
         }
       }
-      const long long e2 = a.dbg ? clock64() : 0;
       t2_bar_sync(2, 256);
       // ---------------- per (sample, channel) parameters: mean, scale = rstd*gamma, shift = beta
       for (int g = half; g < c.nsamp && !fold; g += 2) {
@@ -525,7 +504,6 @@ __global__ void __launch_bounds__(T2_THREADS, 1) conv_block_tc2_kernel(const Tc2
         par[(2 * a.G + g) * 128 + col_l] = beta;
       }
       t2_bar_sync(2, 256);
-      const long long e3 = a.dbg ? clock64() : 0;
       // ---------------- pass B: staged tile -> c / out, thread = one 16-byte A4 unit, lanes along time
       if (ok) {
         const int nq = min(32, (d.Cout - c.mtile * 128) >> 2);  // valid 4-row chunks of this tile
@@ -710,7 +688,6 @@ __global__ void __launch_bounds__(T2_THREADS, 1) conv_block_tc2_kernel(const Tc2
               }
             }
           }
-          if (a.dbg) e3b = clock64();
         } else {
           if (d.save_c) {  // raw conv (+bias) rows in conv layout, kept for the backward pass
             for (RowIter ri = t2_rows(ewarp, lane, c.tw, nq); ri.row < c.nsamp * nq; t2_next(ri)) {
@@ -721,7 +698,6 @@ __global__ void __launch_bounds__(T2_THREADS, 1) conv_block_tc2_kernel(const Tc2
             }
             __syncwarp();
           }
-          if (a.dbg) e3b = clock64();
           const int nqo = shuf ? nq >> 1 : nq;       // output chunks of this tile
           const int two = shuf ? c.tw * 2 : c.tw;    // output time steps of this tile
           const int to0 = shuf ? c.t0 * 2 : c.t0;    // first output time step of this tile
@@ -787,22 +763,11 @@ __global__ void __launch_bounds__(T2_THREADS, 1) conv_block_tc2_kernel(const Tc2
           }
         }
       }
-      const long long e3c = a.dbg ? clock64() : 0;
       t2_bar_sync(2, 256);  // the staged tile and the parameter arrays are reused by the next tile
-      if (a.dbg) {
-        const long long e4 = clock64();
-        if (e3b == 0) e3b = e3;
-        dbg0 += e1 - e0; dbg1 += e2 - e1; dbg2 += e3 - e2; dbg3 += e3b - e3; dbg4 += e3c - e3b; dbg5 += e4 - e3c;
-      }
     }
     if (nbw && d.dbias && etid < 128 && etid < d.Cout && tl > 0) atomicAdd(d.dbias + etid, dbacc[etid]);   // mtiles == 1 (plan)
-    if (a.dbg && etid == 0) {
-      long long* o = a.dbg + (size_t)blockIdx.x * 16;
-      o[8] = dbg0; o[9] = dbg1; o[10] = dbg2; o[11] = dbg3; o[12] = tl; o[13] = dbg4; o[14] = dbg5;
-    }
   }
   __syncthreads();
-  if (a.dbg && tid == 0) a.dbg[(size_t)blockIdx.x * 16 + 1] = clock64();
 }
 
 // ------------------------------------------------------------------ host side: tile plan
@@ -916,8 +881,6 @@ int t2_plan(const avc_conv_desc* d, int sms, Tc2Args& a) {
 // dynamic shared memory of a plan: the stages, the staged epilogue tile, the parameter and statistics arrays
 static uint32_t t2_smem_bytes(const Tc2Args& a) { return a.off_stat + 2u * (uint32_t)a.G * 128u * 8u; }
 
-static long long* g_tc2_dbg = nullptr;
-
 template <int N, int NL>
 static int t2_launch(const Tc2Args& a, const CUtensorMap& tmx, const CUtensorMap& tmw, int grid, int smem, cudaStream_t stream) {
   auto kern = conv_block_tc2_kernel<N, NL>;
@@ -973,7 +936,6 @@ int conv_block_tc2_launch(const avc_conv_desc* d, int* status, void* stream) {
   const int rc = t2_plan(d, t2_num_sms(), a);
   if (rc != AVC_OK) return rc;
   a.status = status;
-  a.dbg = g_tc2_dbg;
   CUtensorMap tmx, tmw;
   {
     PFN_tmap_encode enc = tmap_encode_fn();
@@ -1028,5 +990,3 @@ int conv_block_tc2_plan(const avc_conv_desc* d, int num_sms, avc_tc_plan* out) {
 }
 
 }  // namespace avc
-
-extern "C" void avc_tc2_set_debug(void* dev_buffer) { avc::g_tc2_dbg = (long long*)dev_buffer; }

@@ -61,50 +61,9 @@ __global__ void __launch_bounds__(256) tc_probe_kernel(const ProbeArgs a) {
   }
 }
 
-// Store-path probe: every CTA writes `bytes` to its own region of `dst`; mode 0 = coalesced STG.128 from registers,
-// mode 1 = 2 KB bulk (TMA) stores from shared memory, mode 2 = both at once (half the bytes each).  cycles[cta] =
-// clock64 span of the CTA.  Answers "how many bytes per clock can one SM push to L2".
-__global__ void __launch_bounds__(256) store_probe_kernel(float* dst, long long bytes, int mode, long long* cycles) {
-  extern __shared__ __align__(1024) uint8_t smem[];
-  const int tid = threadIdx.x;
-  float4* sm4 = reinterpret_cast<float4*>(smem);
-  for (int i = tid; i < 4096; i += 256) sm4[i] = make_float4((float)i, 1.f, 2.f, 3.f);   // 64 KB
-  tc::fence_proxy_async_smem();
-  __syncthreads();
-  float* base = dst + (size_t)blockIdx.x * (bytes / 4);
-  const long long n16 = bytes / 16;
-  const long long t0 = clock64();
-  if (mode == 0 || mode == 2) {
-    const long long lim = mode == 2 ? n16 / 2 : n16;
-    const float4 v = make_float4((float)tid, 1.f, 2.f, 3.f);
-    for (long long i = tid; i < lim; i += 256) st4(base + i * 4, v);
-  }
-  if (mode == 1 || mode == 2) {
-    const long long first = mode == 2 ? n16 / 2 : 0;
-    const long long rows = (n16 - first) / 128;   // 2 KB rows
-    if ((tid & 31) == 0) {
-      for (long long r = tid >> 5; r < rows; r += 8) tc::bulk_s2g(base + (first + r * 128) * 4, smem + (size_t)(r & 31) * 2048, 2048u);
-      tc::bulk_commit();
-      tc::bulk_wait_all();
-    }
-  }
-  __syncthreads();
-  if (tid == 0) cycles[blockIdx.x] = clock64() - t0;
-}
-
 }  // namespace avc
 
 using namespace avc;
-
-extern "C" int avc_probe_store(float* dst, long long bytes_per_cta, int ctas, int mode, long long* cycles, void* stream) {
-  AVC_REQUIRE(dst && cycles && bytes_per_cta > 0 && bytes_per_cta % 4096 == 0 && ctas > 0 && mode >= 0 && mode <= 2, AVC_ERR_INVALID,
-              "avc_probe_store: bad argument");
-  cudaError_t e = cudaFuncSetAttribute(store_probe_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024);
-  if (e != cudaSuccess) { set_error("avc_probe_store: %s", cudaGetErrorString(e)); return AVC_ERR_CUDA; }
-  store_probe_kernel<<<ctas, 256, 64 * 1024, (cudaStream_t)stream>>>(dst, bytes_per_cta, mode, cycles);
-  AVC_CHECK_LAUNCH("store_probe");
-  return AVC_OK;
-}
 
 static int g_probe_ld_shift = 0;
 extern "C" void avc_tc_probe_set_ld_shift(int shift) { g_probe_ld_shift = shift < 0 ? 0 : shift; }

@@ -134,7 +134,9 @@ class Engine:
             raise L.AvcError("adaptive_voice_conversion_b200 runs on CUDA (sm_90a) only; there is no CPU path")
         self.lib = L.load()
         self.packed: Dict[str, Dict[str, torch.Tensor]] = {}
-        self.debug = None  # optional callback(name, stage, obj) for tools/diag_*.py
+        # optional callback(name, "dc", dc), called right behind the launch that wrote each block's gradient w.r.t. its
+        # raw conv output: the layer-by-layer tests (tests/test_gpu_step_layers.py) capture dc through it
+        self.debug = None
         # "tf32": conv blocks / data gradients on the tensor cores (TF32 inputs rounded
         # to nearest, fp32 accumulate); "fp32": the exact FFMA kernels.  AVC_PRECISION overrides.
         self.precision = os.environ.get("AVC_PRECISION", "tf32")
@@ -176,7 +178,7 @@ class Engine:
         # the data-gradient conv of a block also runs the upstream block's norm backward (AVC_F_NORMBWD); off = one
         # avc_norm_bwd launch per block
         self.norm_bwd_fused = os.environ.get("AVC_NORM_BWD_FUSED", "1" if L.DEFAULT_NORM_BWD_FUSED else "0") == "1"
-        # diagnostic (tools/diag_tf32.py, tests/test_gpu_tf32_accuracy.py): forward conv blocks on the exact-fp32 FFMA
+        # diagnostic (tests/test_gpu_tf32_accuracy.py): forward conv blocks on the exact-fp32 FFMA
         # kernels while the backward stays on the tensor cores -- separates "TF32 forward flips ReLU masks" from
         # "TF32 backward kernels are inaccurate" in the gradient-parity numbers
         self.fwd_fp32 = os.environ.get("AVC_FWD_FP32", "0") == "1"
@@ -717,8 +719,6 @@ class Engine:
             wd.x, wd.x_bstride, wd.dc, wd.dc_bstride = xin.ptr, xin.bstride, dc.ptr, dc.bstride
             wd.dw = G[name + ".weight"].data_ptr()
             self.wgrad(wd, name, keep=(xin.t, dc.t))
-            if self.debug:
-                self.debug(name, "dw", G[name + ".weight"])
         if not need_dx:
             return None
         # data gradient: full transposed conv (zero pad) then fold the reflect halo back
@@ -778,8 +778,6 @@ class Engine:
                         self.debug(up["name"], "dc", dc_up)
                     return dx if fuse_up.get("need_dx", True) else None
                 self._ck(self.lib.avc_conv_block_tc(C.byref(d), self.tc_status.data_ptr(), st), f"conv_dgrad_tc_fold[{name}]")
-                if self.debug:
-                    self.debug(name, "dx", dx)
                 return dx
             self._ck(self.lib.avc_conv_block_tc(C.byref(d), self.tc_status.data_ptr(), st), f"conv_dgrad_tc[{name}]")
         else:
@@ -795,9 +793,6 @@ class Engine:
             f.dres, f.dres_bstride, f.res_mode, f.res_T = dres.ptr, dres.bstride, dres_mode, dres.T
         f.dx, f.dx_bstride = dx.ptr, dx.bstride
         self._ck(self.lib.avc_fold_add_fwd(C.byref(f), st), f"fold_add[{name}]")
-        if self.debug:
-            self.debug(name, "dxp", dxp)
-            self.debug(name, "dx", dx)
         return dx
 
     # ------------------------------------------------------------------ linear layers

@@ -161,11 +161,6 @@ int avc_conv_block_tc_plan(const avc_conv_desc* d, int num_sms, avc_tc_plan* out
  * and ci_total input channels (FWD: Cout, Cin; DGRAD: Cin, Cout). */
 int avc_pack_conv_weight_tc(const float* w, float* packed, int Cout, int Cin, int K, int mode, void* stream);
 int64_t avc_tc_packed_floats(int co_total, int ci_total, int K);
-/* Diagnostics: device buffer of 16 int64 per CTA receiving phase counters of subsequent avc_conv_block_tc launches
- * (null disables): [0] start [1] end clock; wait / work cycle sums of the roles:
- * [2] producer wait-empty, [3] patch wait-full [4] patch work, [5] MMA wait-ready [6] wait-accumulator [7] issue,
- * [8] epilogue wait-accumulator [9] accumulator pass [10] parameters [11] c rows [13] out rows [14] end barrier, [12] tiles done. */
-void avc_tc2_set_debug(void* dev_buffer);
 /* Every re-pack of a model in one launch: a DEVICE-resident table of items (null destinations
  * are skipped); max_elems = the largest destination element count in the table. */
 typedef struct avc_pack_item {
@@ -1003,9 +998,6 @@ int avc_tc_probe_gemm(const float* a_img, int a_bytes, const float* b_img, int b
 /* Read-back variant of the self-test: only columns >= `shift` are written (columns below `shift` are left
  * untouched in D). */
 void avc_tc_probe_set_ld_shift(int shift);
-/* Store-path probe (diagnostic): `ctas` CTAs of 256 threads each write bytes_per_cta (multiple of 4096) to their own
- * region of dst; mode 0 = STG.128, 1 = 2 KB bulk (TMA) stores from shared memory, 2 = half each; cycles[cta] = span. */
-int avc_probe_store(float* dst, long long bytes_per_cta, int ctas, int mode, long long* cycles, void* stream);
 
 const char* avc_last_error(void);
 /* "sm_90a" build tag, number of kernels launched so far by this process (for bench.py's

@@ -8,7 +8,7 @@ that hold whatever the batch size and need no CPU-sized oracle run --
 Both arithmetic modes.  In tf32 mode activations that feed a tensor-core conv are ROUNDED to a 10-bit mantissa:
 rounding is discontinuous, so a 1e-7 difference in an InstanceNorm sum (another summation order for another
 tile shape) is amplified layer by layer up to the TF32 noise floor (~5e-4) -- exactly as far as either result is
-from the fp32 reference.  Measured in round 2 (tools/diag_batchdep.py): every kernel is bit-identical or 1e-7
+from the fp32 reference.  Measured in round 2: every kernel is bit-identical or 1e-7
 apart per sample across batch sizes, the 14-layer content encoder 5e-4.  Tolerances below reflect that.
 """
 import os
