@@ -131,9 +131,19 @@ def morph_weights(keyframes: Sequence[tuple], n_frames: int, frames_per_second: 
         for n, w in parts:
             V[i, names.index(n)] = w / total
     ts = np.arange(int(n_frames), dtype=np.float64) / float(frames_per_second)
+    return names, interpolate_keyframes(times, V, ts).T.astype(np.float32)
+
+
+def interpolate_keyframes(times, vectors, at) -> np.ndarray:
+    """float64 [len(at), K]: the keyframe vectors (float64 [n_keyframes, K] at non-decreasing times) at the times `at`,
+    interpolated linearly between consecutive keyframes, the first one held before it and the last one after it; at
+    two keyframes of the same time the later one takes over there (a hard cut).  The one statement of that rule, shared
+    by morph_weights (times in seconds) and streaming.TargetSchedule (times in frames)."""
+    V = np.asarray(vectors, dtype=np.float64)
+    ts = np.asarray(at, dtype=np.float64)
     tk = np.asarray(times, dtype=np.float64)
     i = np.searchsorted(tk, ts, side="right") - 1                 # last keyframe at or before the frame
-    out = np.empty((int(n_frames), len(names)), dtype=np.float64)
+    out = np.empty((len(ts), V.shape[1]), dtype=np.float64)
     before, after = i < 0, i >= len(tk) - 1
     out[before] = V[0]
     out[after & ~before] = V[-1]
@@ -142,7 +152,7 @@ def morph_weights(keyframes: Sequence[tuple], n_frames: int, frames_per_second: 
         j = i[mid]
         a = ((ts[mid] - tk[j]) / (tk[j + 1] - tk[j]))[:, None]
         out[mid] = (1 - a) * V[j] + a * V[j + 1]
-    return names, out.T.astype(np.float32)
+    return out
 
 
 def morph_table(bank: "SpeakerBank", keyframes: Sequence[tuple], n_frames: int, frames_per_second: float):

@@ -19,6 +19,11 @@ Three stages run once per update, each batched over every stream with pending in
   ``avc_yin_window``, turns the new frames into shifts on the host (``PitchTracker``, causal) and shifts the buffered
   magnitudes of those frames before they enter the output RTISI-LA.
 
+A stream's target voice follows its ``TargetSchedule``: anchor codes and keyframes of weights over them at mel frames.
+``StreamingConverter.retarget`` cuts or glides to another code from a frame no converted window has reached.  A window
+whose weights are one anchor at weight 1 on every frame converts as above; any other (a morph window) converts through
+``AE.inference_morph`` with the schedule's per-frame weights, and the pitch targets follow the same weights.
+
 ``block_schedule``, ``blend_weights``, ``latency_samples`` and ``tracked_latency_samples`` state the schedule on the
 host.
 """
@@ -35,6 +40,7 @@ import torch
 from . import _lib as L
 from .f0 import F0Params
 from .mcd import min_frames
+from .speaker_bank import interpolate_keyframes
 from .utils import _stream
 from .vocoder import _SEG, PITCH_SHIFT_MAX, _mel_project, _ptr, _ratio
 
@@ -379,8 +385,10 @@ class PitchTracker:
         self.theta, self.floor = params.theta(), -float(params.silence_db)
         self.emax, self.n, self.mean, self.m2, self.last = 0.0, 0, 0.0, 0.0, 0.0
 
-    def update(self, tau, ap, en):
-        """(log2 F0 (NaN where unvoiced), voiced, shift) float64 / bool / float64 arrays of the next frames."""
+    def update(self, tau, ap, en, mu_t=None, sd_t=None):
+        """(log2 F0 (NaN where unvoiced), voiced, shift) float64 / bool / float64 arrays of the next frames.  mu_t and
+        sd_t, when given, are float64 per-frame targets of these frames (TargetSchedule.profile) in place of the
+        constant ones; equal targets on every frame give the constant targets' bits."""
         tau, ap, en = (np.asarray(v, np.float64) for v in (tau, ap, en))
         emax = np.maximum.accumulate(np.concatenate([[self.emax], en]))[1:]
         self.emax = float(emax[-1]) if len(emax) else self.emax
@@ -398,20 +406,195 @@ class PitchTracker:
                 self.mean += d / self.n
                 self.m2 += d * (l - self.mean)
                 sd = math.sqrt(self.m2 / self.n)
+                mu = self.mu_t if mu_t is None else float(mu_t[i])
+                sdt = self.sd_t if sd_t is None else float(sd_t[i])
                 if self.mode == "mv" and self.n >= self.warmup and sd != 0.0:
-                    v = 12.0 * (self.mu_t + self.sd_t / sd * (l - self.mean) - l)
+                    v = 12.0 * (mu + sdt / sd * (l - self.mean) - l)
                 else:
-                    v = 12.0 * (self.mu_t - self.mean)
+                    v = 12.0 * (mu - self.mean)
                 self.last = min(PITCH_SHIFT_MAX, max(-PITCH_SHIFT_MAX, v))
             shift[i] = self.last
         return logf, voiced, shift
 
 
-class _PStream:
-    __slots__ = ("ratio", "track", "pend", "frames", "n_rel", "tail", "tail_first", "tracked", "diag")
+# ------------------------------------------------------------------ target schedule
+class _Keep:
+    def __repr__(self):
+        return "KEEP"
 
-    def __init__(self, ratio=None, track=None, dev=None, n_bins=0):
-        self.ratio, self.track = ratio, track
+
+KEEP = _Keep()    # retarget's pitch: the new anchor takes the pitch target the schedule has at `at`
+
+
+def pitch_kind(pitch):
+    """The kind of a parsed pitch setting: None, "shift" or the profile's mode."""
+    return None if pitch is None else "shift" if isinstance(pitch, float) else pitch[0]
+
+
+class TargetSchedule:
+    """The target voice of one stream over its mel frames: anchor codes in order of first use, each with a pitch
+    target of the stream's kind (None; semitones for a fixed shift; (mu, sigma) of log2 F0 for a profile), and
+    keyframes (frame, float64 weights over the anchors) at non-decreasing frames.
+
+    The weights of frame t follow speaker_bank.morph_weights' rule (interpolate_keyframes) with times in frames: the
+    first keyframe held before it and the last after it, linear in between, the later of two keyframes on one frame
+    winning (a hard cut); float64, rounded once to float32 (``weights``).  Pitch targets are the weighted sums of the
+    anchors' in float64 with the float32 weights: a shift sum_k w_k s_k, a profile's mu and sigma as
+    SpeakerBank.morph_pitch_profile gives them.  Anchors are de-duplicated by bitwise equality of their codes (and
+    of the pitch target, when one is given).  ``prune`` drops what no frame from a given one on can read."""
+
+    def __init__(self, code, pitch=None):
+        self.kind = pitch_kind(pitch)
+        self.codes = [code]
+        self.pitch = [None if pitch is None else pitch if isinstance(pitch, float) else (float(pitch[1]),
+                                                                                         float(pitch[2]))]
+        self.frames = [0]
+        self.V = np.ones((1, 1))       # float64 [keyframes, anchors]
+
+    def mix(self, f0: int, f1: int) -> np.ndarray:
+        """float64 [f1 - f0, K]: the weights of frames f0 .. f1 - 1 before rounding."""
+        return interpolate_keyframes(self.frames, self.V, np.arange(f0, f1))
+
+    def weights(self, f0: int, f1: int) -> np.ndarray:
+        """float32 [K, f1 - f0]: the weights of frames f0 .. f1 - 1."""
+        if self.V.shape == (1, 1):
+            return np.ones((1, f1 - f0), np.float32)
+        return self.mix(f0, f1).T.astype(np.float32)
+
+    def window(self, f0: int, f1: int):
+        """(k, None) when frames f0 .. f1 - 1 all have anchor k alone at weight 1 (a plain window), otherwise
+        (anchors of non-zero weight in schedule order, their float32 weights [K, f1 - f0])."""
+        if self.V.shape == (1, 1):
+            return 0, None
+        w = self.weights(f0, f1)
+        nz = np.flatnonzero(w.any(1))
+        if len(nz) == 1 and (w[nz[0]] == 1).all():
+            return int(nz[0]), None
+        return nz.tolist(), w[nz]
+
+    def shift(self, f0: int, n: int) -> np.ndarray:
+        """float64 [n]: the fixed-shift target (semitones) of frames f0 .. f0 + n - 1."""
+        if len(self.codes) == 1:
+            return np.full(n, self.pitch[0])
+        w = self.weights(f0, f0 + n).astype(np.float64)
+        s = np.zeros(n)
+        for wk, sk in zip(w, self.pitch):
+            s = s + wk * sk
+        return s
+
+    def profile(self, f0: int, n: int):
+        """(mu, sigma) float64 [n]: the profile target of frames f0 .. f0 + n - 1."""
+        if len(self.codes) == 1:
+            return np.full(n, self.pitch[0][0]), np.full(n, self.pitch[0][1])
+        w = self.weights(f0, f0 + n).astype(np.float64)
+        mu, sd, wsum = np.zeros(n), np.zeros(n), np.zeros(n)
+        for wk, (m, s) in zip(w, self.pitch):
+            if not wk.any():
+                continue
+            mu, sd, wsum = mu + wk * m, sd + wk * s, wsum + wk
+        return mu / wsum, sd / wsum
+
+    def pitch_value(self, pitch, at: int):
+        """retarget's pitch as an anchor's pitch target: KEEP gives the schedule's at frame `at`; otherwise it must be
+        of the stream's kind (None; a number of semitones, 0 included; a profile of the stream's mode).  ValueError
+        otherwise."""
+        if pitch is KEEP:
+            if self.kind is None:
+                return None
+            if self.kind == "shift":
+                return float(self.shift(at, 1)[0])
+            mu, sd = self.profile(at, 1)
+            return float(mu[0]), float(sd[0])
+        if self.kind == "shift":
+            ok = isinstance(pitch, (int, float, np.floating, np.integer)) and not isinstance(pitch, bool)
+            v = parse_pitch(pitch) if ok else "bad"
+            if ok and v is None:
+                return 0.0
+            if isinstance(v, float):
+                return v
+        else:
+            try:
+                v = parse_pitch(pitch)
+            except ValueError:
+                v = "bad"
+            if v != "bad" and pitch_kind(v) == self.kind:
+                return None if v is None else (v[1], v[2])
+        want = {None: "None", "shift": "a number of semitones"}.get(self.kind, f"a ({self.kind!r}, mu, sigma) profile")
+        raise ValueError(f"retarget: the stream's pitch setting takes {want} or KEEP (its kind cannot change), got "
+                         f"{pitch!r}")
+
+    def retarget(self, code, at: int, ramp: int, pitch=KEEP, first: int = 0, lo: int = 0, window: int = 0,
+                 max_k: int = L.MORPH_MAX_K):
+        """Moves the schedule from its mix at frame `at` to code (one-hot) over `ramp` frames: drops the keyframes
+        after `at`, then adds (at, mix at `at`) and (at + ramp, one-hot).  pitch: the anchor's pitch target
+        (pitch_value).  ValueError, the schedule unchanged, for at < first (a frame already converted), a negative
+        ramp, or when a window of `window` frames starting at or after frame lo would need more than max_k anchors of
+        non-zero weight."""
+        if at < first:
+            raise ValueError(f"retarget: frame {at} is before the end of the stream's last converted window ({first})")
+        if ramp < 0:
+            raise ValueError(f"retarget: ramp must be >= 0 frames (got {ramp})")
+        v = self.mix(at, at + 1)[0]
+        k = next((i for i, c in enumerate(self.codes) if (c is code or torch.equal(c, code))
+                  and (pitch is KEEP or self.pitch[i] == pitch)), None)
+        if k is None and pitch is KEEP:
+            pitch = self.pitch_value(KEEP, at)
+        codes, pitches, V = list(self.codes), list(self.pitch), self.V
+        if k is None:
+            codes.append(code)
+            pitches.append(pitch)
+            V = np.concatenate([V, np.zeros((V.shape[0], 1))], 1)
+            v = np.concatenate([v, [0.0]])
+            k = len(codes) - 1
+        keep = sum(1 for f in self.frames if f <= at)
+        onehot = np.zeros(len(codes))
+        onehot[k] = 1.0
+        frames = self.frames[:keep] + [at, at + ramp]
+        V = np.concatenate([V[:keep], v[None], onehot[None]])
+        need = live_anchors(frames, V, lo, window)
+        if need > max_k:
+            raise ValueError(f"retarget: a window would need {need} anchors of non-zero weight; at most {max_k} are "
+                             f"supported")
+        self.codes, self.pitch, self.frames, self.V = codes, pitches, frames, V
+
+    def prune(self, lo: int):
+        """Drops the keyframes and anchors no frame from lo on reads: every keyframe before the last one at or before
+        lo, then every anchor of zero weight in all the keyframes left (the others keep their order)."""
+        i = max(0, sum(1 for f in self.frames if f <= lo) - 1)
+        if i:
+            self.frames, self.V = self.frames[i:], self.V[i:]
+        live = np.flatnonzero(self.V.any(0))
+        if len(live) < len(self.codes):
+            self.codes = [self.codes[k] for k in live]
+            self.pitch = [self.pitch[k] for k in live]
+            self.V = self.V[:, live]
+
+
+def live_anchors(frames, V, lo: int, window: int) -> int:
+    """The most anchors of non-zero weight any window of `window` frames from frame lo on can need (counting, on each
+    span between consecutive keyframes, the anchors of either end)."""
+    segs = []   # (first frame, end frame, anchors)
+    nz = [set(np.flatnonzero(r).tolist()) for r in V]
+    for i in range(len(frames)):
+        end = frames[i + 1] if i + 1 < len(frames) else math.inf
+        if end > frames[i] or i + 1 == len(frames):
+            segs.append((frames[i], end, nz[i] | (nz[i + 1] if i + 1 < len(frames) else set())))
+    segs.insert(0, (-math.inf, frames[0], nz[0]))
+    worst = 0
+    for a in {lo} | {max(lo, s[1] - 1) for s in segs if s[1] != math.inf}:
+        used = set()
+        for s0, s1, ks in segs:
+            if s0 < a + max(1, window) and s1 > a:
+                used |= ks
+        worst = max(worst, len(used))
+    return worst
+
+
+class _PStream:
+    __slots__ = ("ratio", "track", "pend", "frames", "n_rel", "tail", "tail_first", "tracked", "diag", "sched")
+
+    def __init__(self, ratio=None, track=None, dev=None, n_bins=0, sched=None):
+        self.ratio, self.track, self.sched = ratio, track, sched
         self.pend = torch.empty(0, n_bins, device=dev)          # unshifted magnitudes of frames not yet tracked
         self.frames = self.n_rel = self.tail_first = self.tracked = 0
         self.tail = torch.empty(0, device=dev)                  # shadow samples from tail_first on
@@ -446,15 +629,24 @@ class PitchStage:
         self.streams, self.closed = {}, {}
         self.stage_ms = None
 
-    def open(self, sid, pitch=None):
+    def open(self, sid, pitch=None, schedule: TargetSchedule = None):
+        """schedule, when given, holds the stream's per-frame pitch targets (TargetSchedule.shift / .profile) in place
+        of pitch's constant one; pitch still sets the kind."""
         pitch = parse_pitch(pitch)
         self.rt.open(sid)
         if isinstance(pitch, float):
-            self.streams[sid] = _PStream(ratio=np.float32(_ratio(pitch)))
+            self.streams[sid] = _PStream(ratio=np.float32(_ratio(pitch)), sched=schedule)
         elif pitch is not None:
             self.shadow.open(sid)
             self.streams[sid] = _PStream(track=PitchTracker(*pitch, self.warmup, self.hp.sr, self.params),
-                                         dev=self.dev, n_bins=self.hp.n_bins)
+                                         dev=self.dev, n_bins=self.hp.n_bins, sched=schedule)
+
+    def next_frame(self, sid):
+        """The first frame of stream sid whose pitch target the stage has not read yet; None when it reads none."""
+        s = self.streams.get(sid)
+        if s is None:
+            return None
+        return s.frames if s.track is None else s.tracked
 
     def drop(self, sid):
         self.rt.drop(sid)
@@ -517,9 +709,17 @@ class PitchStage:
         for sid, m in mags.items():
             s = self.streams.get(sid)
             if s is not None and s.track is None and m.shape[0]:
+                n = int(m.shape[0])
                 rows.append(m)
-                ratios.append(np.full(int(m.shape[0]), s.ratio, np.float32))
+                if s.sched is None:
+                    ratios.append(np.full(n, s.ratio, np.float32))
+                elif len(s.sched.codes) == 1:     # one anchor: weight 1 on every frame, its own shift
+                    ratios.append(np.full(n, np.float32(_ratio(s.sched.pitch[0])), np.float32))
+                else:
+                    ratios.append(np.array([_ratio(v) for v in s.sched.shift(s.frames, n).tolist()],
+                                           np.float64).astype(np.float32))
                 dest.append(sid)
+                s.frames += n
         if tracked:
             t0 = self._track(tracked, mags, close, rows, ratios, dest, t0)
         if rows:
@@ -595,7 +795,8 @@ class PitchStage:
             s = self.streams[sid]
             tau, ap, en = host[0, f:f + n], host[1, f:f + n], host[2, f:f + n]
             f += n
-            logf, voiced, shift = s.track.update(tau, ap, en)
+            targets = () if s.sched is None else s.sched.profile(s.tracked, n)
+            logf, voiced, shift = s.track.update(tau, ap, en, *targets)
             rows.append(s.pend[:n])
             ratios.append(np.array([_ratio(v) for v in shift.tolist()], np.float64).astype(np.float32))
             dest.append(sid)
@@ -613,12 +814,12 @@ class PitchStage:
 
 # ------------------------------------------------------------------ the converter
 class _CStream:
-    __slots__ = ("code", "hist", "hist_first", "block", "prev", "mels")
+    __slots__ = ("sched", "hist", "hist_first", "block", "prev", "mels", "e_last")
 
-    def __init__(self, code, dev, n_mels):
-        self.code = code
+    def __init__(self, sched, dev, n_mels):
+        self.sched = sched
         self.hist = torch.empty(0, n_mels, device=dev)
-        self.hist_first, self.block, self.prev, self.mels = 0, 0, None, []
+        self.hist_first, self.block, self.prev, self.mels, self.e_last = 0, 0, None, [], 0
 
 
 class StreamingConverter:
@@ -627,7 +828,8 @@ class StreamingConverter:
     pitch setting (``PitchStage``: None, a fixed shift in semitones, or a target profile ("match" | "mv", mu_t,
     sigma_t) of log2 F0) and returns its id; ``push({id: pcm})`` takes float32 PCM chunks at ``hp.sr`` of any length
     and returns {id: new output samples} (device float32), one batched update; ``close(id)`` returns the stream's last
-    samples.  ``take_mels(id)`` hands over the normalised mel frames the stream emitted so far and ``take_pitch(id)`` a
+    samples; ``retarget(id, code, at, ramp, pitch)`` moves a live stream to another code (``TargetSchedule``).
+    ``take_mels(id)`` hands over the normalised mel frames the stream emitted so far and ``take_pitch(id)`` a
     tracked stream's per-frame pitch diagnostics, when the converter keeps them (``StreamParams(keep_mels=True)``; off
     by default, since they grow with the stream).  ``latency_samples`` is the worst case, over output samples n, of
     (index of the input sample whose arrival releases n) - n; ``tracked_latency_samples`` the same for streams with a
@@ -669,17 +871,55 @@ class StreamingConverter:
         self.tracked_latency_samples = tracked_latency_samples(params, self.hp.win_length, self.hp.hop_length, self.m,
                                                                self.stage.span)
 
-    def open(self, code, pitch=None) -> int:
+    def _check_code(self, code, what):
         if (not isinstance(code, torch.Tensor) or code.dtype != torch.float32 or tuple(code.shape) != (self.c_out,)
                 or code.device != self.dev):
-            raise ValueError(f"StreamingConverter.open: code must be float32 [{self.c_out}] on {self.dev}")
-        parse_pitch(pitch)
+            raise ValueError(f"StreamingConverter.{what}: code must be float32 [{self.c_out}] on {self.dev}")
+
+    def open(self, code, pitch=None) -> int:
+        self._check_code(code, "open")
+        pitch = parse_pitch(pitch)
         sid = self._next
         self._next += 1
-        self.streams[sid] = _CStream(code.contiguous(), self.dev, self.n_mels)
+        sched = TargetSchedule(code.contiguous(), pitch)
+        self.streams[sid] = _CStream(sched, self.dev, self.n_mels)
         self.ana.open(sid)
-        self.stage.open(sid, pitch)
+        self.stage.open(sid, pitch, sched)
         return sid
+
+    def retarget(self, sid, code, at=None, ramp: int = 0, pitch=KEEP) -> int:
+        """Moves stream sid from its current mix to `code` (float32 [c_out] on the device, one-hot) over `ramp` mel
+        frames from frame `at` (TargetSchedule.retarget), and returns the `at` used.  `at` must not precede the end of
+        the stream's last converted window, so that no converted frame changes; None: ceil(n_in / hop_length), the
+        first frame centred at or after the next input sample.  pitch: the new anchor's pitch target, of the kind the
+        stream was opened with (None; semitones; (mode, mu, sigma) of its mode), or KEEP: the target the schedule has
+        at `at`.  Retargets issued ahead of time, in order, compose; one issued during a ramp starts from the mix that
+        ramp has reached, so its anchors keep a non-zero weight (decaying along a chain of interrupted ramps) and
+        count toward MORPH_MAX_K until that weight underflows.  The decoder's windows reach up to H + LA frames past
+        the block they emit, so a block's voice starts to move that much before `at`.  KeyError for an unknown or closed stream; ValueError, the
+        schedule unchanged, for an earlier `at`, a pitch of another kind, or a window that would need more than
+        MORPH_MAX_K anchors."""
+        if sid not in self.streams:
+            raise KeyError(f"unknown stream {sid!r}")
+        self._check_code(code, "retarget")
+        s = self.streams[sid]
+        nxt = -(-self.ana.streams[sid].n_in // self.hp.hop_length)
+        if at is None:
+            # a window is converted only once all its frames are analysed, which needs input past its last centre
+            assert nxt >= s.e_last, (nxt, s.e_last)
+            at = nxt
+        at, ramp = int(at), int(ramp)
+        value = pitch if pitch is KEEP else s.sched.pitch_value(pitch, at)
+        lo = max(0, self.ana.streams[sid].frames - self.window)
+        s.sched.retarget(code.contiguous(), at, ramp, value, first=s.e_last, lo=lo, window=self.window)
+        s.sched.prune(self._read_from(sid))
+        return at
+
+    def _read_from(self, sid) -> int:
+        """The first frame of stream sid whose weights a later window or the pitch stage can still read."""
+        lo = max(0, self.ana.streams[sid].frames - self.window)
+        f = self.stage.next_frame(sid)
+        return lo if f is None else min(lo, f)
 
     def push(self, chunks):
         return self.update(chunks)
@@ -731,6 +971,7 @@ class StreamingConverter:
                 b0, b1, w0, w1 = block_schedule(s.block, W, H, LA, self.m)
                 wins.append((sid, b0, b1, w0, w1))
                 s.block += 1
+                s.e_last = w1
             if sid in close and s.block * H < F:
                 w0, w1 = close_window(F, W)
                 wins.append((sid, s.block * H, F, w0, w1))
@@ -769,6 +1010,9 @@ class StreamingConverter:
                 self.stage_ms[k] = self.stage_ms.get(k, 0.0) + 1e3 * (b - a)
         self.stage.stage_ms = self.stage_ms
         res = self.stage.run(mags, close)
+        for sid in chunks:
+            if sid not in close:
+                self.streams[sid].sched.prune(self._read_from(sid))
         for sid in close:
             mels = self.streams.pop(sid).mels
             if self.p.keep_mels:
@@ -783,16 +1027,23 @@ class StreamingConverter:
         return time.perf_counter()
 
     def _convert(self, wins, final):
-        """Converted mels [window frames, n_mels] of every window, grouped by length into batches."""
+        """Converted mels [window frames, n_mels] of every window, grouped into batches: plain windows by length, morph
+        windows by length and anchor count K rounded up to a power of two (the padding anchors have zero weight)."""
         out = [None] * len(wins)
-        groups = {}
+        groups, morph = {}, {}
         for k, (sid, _, _, w0, w1) in enumerate(wins):
-            groups.setdefault((w1 - w0, sid in final), []).append(k)
-        for (Lw, last), idx in groups.items():
-            for f in range(0, len(idx), self.p.batch_max):
-                part = idx[f:f + self.p.batch_max]
-                xs = [self._slice(wins[k]) for k in part]
-                codes = [self.streams[wins[k][0]].code for k in part]
+            sched = self.streams[sid].sched
+            a, w = sched.window(w0, w1)
+            if w is None:
+                groups.setdefault((w1 - w0, sid in final), []).append((k, sched.codes[a]))
+            else:
+                Kp = 1 << (len(a) - 1).bit_length()
+                morph.setdefault((w1 - w0, sid in final, Kp), []).append((k, [sched.codes[i] for i in a], w))
+        for (Lw, last), items in groups.items():
+            for f in range(0, len(items), self.p.batch_max):
+                part = items[f:f + self.p.batch_max]
+                xs = [self._slice(wins[k]) for k, _ in part]
+                codes = [c for _, c in part]
                 if last:   # a close window has any length: eager, the exact batch
                     dec = self.inf.model.inference_from_embeddings(torch.stack(xs), torch.stack(codes))
                 else:
@@ -802,7 +1053,29 @@ class StreamingConverter:
                     xb.copy_(torch.stack([xs[r] for r in rows]))
                     eb.copy_(torch.stack([codes[r] for r in rows]))
                     dec = run()
-                for j, k in enumerate(part):
+                for j, (k, _) in enumerate(part):
+                    out[k] = dec[j, :, :Lw].transpose(0, 1)
+        for (Lw, last, Kp), items in morph.items():
+            for f in range(0, len(items), self.p.batch_max):
+                part = items[f:f + self.p.batch_max]
+                B = len(part) if last else min(self.p.batch_max, 1 << (len(part) - 1).bit_length())
+                rows = list(range(len(part))) + [0] * (B - len(part))
+                zero = torch.zeros(self.c_out, device=self.dev)
+                x = torch.stack([self._slice(wins[part[r][0]]) for r in rows])
+                cb = torch.stack([c for r in rows for c in part[r][1] + [zero] * (Kp - len(part[r][1]))])
+                wh = np.zeros((B, Kp, Lw), np.float32)          # the batch's weights, built on the host
+                for j, r in enumerate(rows):
+                    wh[j, :part[r][2].shape[0]] = part[r][2]
+                if last:   # eager, the exact batch
+                    dec = self.inf.model.inference_morph(x, cb.view(B, Kp, self.c_out), torch.from_numpy(wh).to(self.dev))
+                else:
+                    xb, cbuf, wb, lx, run = self.inf._morph_slot(B, self.n_mels, Lw, Kp, self.dev)
+                    xb.copy_(x)
+                    cbuf.copy_(cb.view(B, Kp, self.c_out))
+                    wb.copy_(torch.from_numpy(wh))                  # one upload per batch
+                    lx.fill_(Lw)                                    # the slot is shared with Inferencer.inference_morph
+                    dec = run()
+                for j, (k, _, _) in enumerate(part):
                     out[k] = dec[j, :, :Lw].transpose(0, 1)
         if wins:
             self.inf.model.engine(self.dev).check_tc_status()

@@ -81,7 +81,8 @@ Streaming: -stream feeds -s to a StreamingConverter (adaptive_voice_conversion_b
 chunks (default 20 ms) and writes the untrimmed stream it gives back; the target is -t files (their pooled code) or
 -bank -speaker SPEC.  With -pairs every line is one stream, all fed in lockstep.  -stream_hop, -stream_lookahead
 (mel frames, multiples of 8; defaults 8 and 8), -stream_gl_lookahead (default 3) and -stream_gl_iters (default 8) set
-the block schedule and RTISI-LA; -morph, a -pitch_shift other than 0 and the -gl_* options are refused with it:
+the block schedule and RTISI-LA; -morph (use -stream_morph), a -pitch_shift other than 0 (use -stream_pitch) and the
+-gl_* options are refused with it:
 
     python inference.py -c config.yaml -m model.ckpt -a attr.pkl -s src.wav -t tgt.wav -o out.wav -stream
 
@@ -95,7 +96,22 @@ accepts banked targets: both modes read the same profile.  A target without a vo
 
     python inference.py -c config.yaml -m model.ckpt -a attr.pkl -s src.wav -bank bank.pt -speaker p225 -o out.wav \
         -stream -stream_pitch mv
+
+-stream_morph SPEC@SECONDS [SPEC@SECONDS ...] is -morph's streaming counterpart: it needs -stream and -bank and
+excludes -t, -speaker and -pairs.  Keyframe k lies at mel frame floor(seconds sr / hop + 0.5); the stream opens with
+the first keyframe's code, and each later keyframe k becomes StreamingConverter.retarget(code_k, at=frame_{k-1},
+ramp=frame_k - frame_{k-1}) before the first chunk, so ``A@0 A@4 B@4.3`` glides from A to B over 0.3 s from 4 s, as
+-morph does.  A mix keyframe is one anchor, its mixed code (SpeakerBank.code), where -morph mixes the decoder's AdaIN
+rows; the two agree up to rounding.  The decoder's windows reach H + LA frames (16, 0.2 s, with the defaults) past
+the block they emit, so a block's voice starts to move up to that much before a keyframe's time.  With -stream_pitch
+match or mv each keyframe's target profile is the bank's (SpeakerBank.pitch_profile) and the stream's target follows
+the same weights; a bank without a pitch record is refused, and when some keyframe has no voiced frame the stream is
+left unshifted, which the run prints:
+
+    python inference.py -c config.yaml -m model.ckpt -a attr.pkl -s src.wav -bank bank.pt -o out.wav -stream \
+        -stream_morph p225@0 p225@4.0 p226@4.3 -stream_pitch mv
 """
+import math
 import os
 import sys
 from argparse import ArgumentParser
@@ -370,23 +386,43 @@ def pitch_shift_arg(p, args):
         p.error("-pitch_shift shifts the synthesis: a .npy output is a mel and is not synthesised")
 
 
+def parse_keyframes(p, option, given):
+    """[(SPEC, seconds)] of -morph's or -stream_morph's keyframes; p.error for one that does not parse or times that
+    decrease."""
+    from adaptive_voice_conversion_b200.speaker_bank import parse_keyframe
+    try:
+        keyframes = [parse_keyframe(k) for k in given]
+    except ValueError as e:
+        p.error(str(e))
+    times = [t for _, t in keyframes]
+    if any(b < a for a, b in zip(times, times[1:])):
+        p.error(f"{option}: keyframe times must not decrease, got {times}")
+    return keyframes
+
+
+def keyframe_frame(seconds, sr, hop):
+    """The mel frame of a -stream_morph keyframe time: floor(seconds sr / hop + 0.5)."""
+    return int(math.floor(seconds * sr / hop + 0.5))
+
+
 def check_args(p, args):
-    """Argument errors (p.error): -t, or -bank with -speaker, for one conversion; -speaker needs -bank; -morph needs
-    -bank, excludes -t, -speaker and -pairs, and its keyframes must parse; -pitch_shift as pitch_shift_arg."""
+    """Argument errors (p.error): -t, or -bank with -speaker, for one conversion; -speaker needs -bank; -morph and
+    -stream_morph need -bank, exclude -t, -speaker and -pairs, and their keyframes must parse; -pitch_shift as
+    pitch_shift_arg."""
     pitch_shift_arg(p, args)
+    if args.stream_morph is not None:
+        if not args.bank:
+            p.error("-stream_morph needs -bank")
+        if args.target is not None or args.speaker is not None or args.pairs:
+            p.error("-stream_morph streams one source through banked speakers: it excludes -t, -speaker and -pairs")
+        args.keyframes = parse_keyframes(p, "-stream_morph", args.stream_morph)
+        return
     if args.morph is not None:
         if not args.bank:
             p.error("-morph needs -bank")
         if args.target is not None or args.speaker is not None or args.pairs:
             p.error("-morph converts one source with banked speakers: it excludes -t, -speaker and -pairs")
-        from adaptive_voice_conversion_b200.speaker_bank import parse_keyframe
-        try:
-            args.keyframes = [parse_keyframe(k) for k in args.morph]
-        except ValueError as e:
-            p.error(str(e))
-        times = [t for _, t in args.keyframes]
-        if any(b < a for a, b in zip(times, times[1:])):
-            p.error(f"-morph: keyframe times must not decrease, got {times}")
+        args.keyframes = parse_keyframes(p, "-morph", args.morph)
         return
     if args.speaker is not None and not args.bank:
         p.error("-speaker needs -bank")
@@ -432,6 +468,10 @@ def parser():
     p.add_argument("-stream_pitch", default=None, metavar="{SEMITONES,match,mv}",
                    help="-stream: shift every block by SEMITONES in [-24, 24], or track the stream and 'match' its "
                         "pitch level, or 'mv' its level and range, to the target's profile")
+    p.add_argument("-stream_morph", nargs="+", metavar="SPEC@SECONDS",
+                   help="-stream: banked speakers or mixes at keyframe times, glided between while streaming (needs "
+                        "-bank; excludes -t, -speaker and -pairs).  A mix keyframe is one anchor, its mixed code; "
+                        "offline -morph mixes the AdaIN rows instead, and the two agree up to rounding")
     return p
 
 
@@ -439,7 +479,7 @@ def check_stream_args(p, args, argv):
     """-stream's refusals (p.error): -morph, a pitch shift, any -gl_* option (streams are synthesised by RTISI-LA), a
     .npy output, a chunk length that is not positive and a block schedule streaming.check_params refuses."""
     if args.morph is not None:
-        p.error("-stream converts to one speaker code per stream: -morph is not supported while streaming")
+        p.error("-morph is not supported with -stream; use -stream_morph SPEC@SECONDS [SPEC@SECONDS ...]")
     if str(args.pitch_shift) not in ("0", "0.0"):
         p.error("-pitch_shift is not supported with -stream; use -stream_pitch {SEMITONES,match,mv}")
     stream_pitch_arg(p, args)
@@ -512,7 +552,9 @@ def run_stream(args, config, jobs):
     sets = {}
     ids = []
     for k, (n, _, t, name) in enumerate(jobs):
-        if isinstance(t, BankTarget):
+        if isinstance(t, BankTarget) and t.keyframes is not None:
+            code = bank.code(t.keyframes[0][0]).to(dev)
+        elif isinstance(t, BankTarget):
             code = bank.code(t.spec).to(dev)
         else:
             key = target_files(t)
@@ -520,12 +562,22 @@ def run_stream(args, config, jobs):
                 sets[key] = inf.embed_speakers([[mel[f] for f in key]])[0]
             code = sets[key]
         pitch = args.stream_pitch
+        morph = isinstance(t, BankTarget) and t.keyframes is not None
         if tracked:
             pr = profiles[k]
-            pitch = None if pr is None else (args.stream_pitch, pr[0], pr[1])
-            print(f"{name}: -stream_pitch {args.stream_pitch} " + ("unmatched: the target has no voiced frame, every "
-                  "shift is 0" if pr is None else f"toward log2 F0 mean {pr[0]:.4f}, std {pr[1]:.4f}"))
-        ids.append(conv.open(code, pitch))
+            if morph:   # a profile per keyframe; unmatched when any keyframe has none
+                pitch = None if any(x is None for x in pr) else [(args.stream_pitch, *x) for x in pr]
+            else:
+                pitch = None if pr is None else (args.stream_pitch, pr[0], pr[1])
+            head = pr[0] if morph and pitch is not None else pr
+            print(f"{name}: -stream_pitch {args.stream_pitch} " + (
+                ("unmatched: a keyframe's target has no voiced frame, the stream is left unshifted" if morph else
+                 "unmatched: the target has no voiced frame, every shift is 0") if pitch is None else
+                f"toward log2 F0 mean {head[0]:.4f}, std {head[1]:.4f}" + (" at the first keyframe" if morph else "")))
+        if morph:
+            ids.append(open_morph(conv, code, bank, t.keyframes, pitch, hp, dev))
+        else:
+            ids.append(conv.open(code, pitch))
     srcs = [load_wav(src, hp.sr) for _, src, _, _ in jobs]
     chunk = max(1, int(round(hp.sr * args.stream_chunk_ms / 1000.0)))
     outs = [[] for _ in jobs]
@@ -541,6 +593,19 @@ def run_stream(args, config, jobs):
     out_dir = args.output if args.pairs else ""
     for (_, _, _, name), ys in zip(jobs, outs):
         inf.write_wav_to_file(torch.cat(ys).cpu().numpy(), os.path.join(out_dir, name))
+
+
+def open_morph(conv, code, bank, keyframes, pitch, hp, dev):
+    """A stream of -stream_morph: opened with code, the first keyframe's, then keyframe k >= 1 becomes a retarget to
+    its code at keyframe k - 1's frame over the frames between them (keyframe_frame), before any input.  pitch: None,
+    a fixed shift (every anchor's) or one (mode, mu, sigma) profile per keyframe."""
+    frames = [keyframe_frame(sec, hp.sr, hp.hop_length) for _, sec in keyframes]
+    per = pitch if isinstance(pitch, list) else [pitch] * len(keyframes)
+    sid = conv.open(code, per[0])
+    for k in range(1, len(keyframes)):
+        conv.retarget(sid, bank.code(keyframes[k][0]).to(dev), at=frames[k - 1], ramp=frames[k] - frames[k - 1],
+                      pitch=per[k])
+    return sid
 
 
 def stream_profiles(jobs, raw, bank, vocoder, params):
@@ -569,8 +634,9 @@ def stream_profiles(jobs, raw, bank, vocoder, params):
     if any(isinstance(t, BankTarget) for _, _, t, _ in jobs):
         print(f"note: the bank's pitch records were tracked from Griffin-Lim copy-syntheses "
               f"({bank.pitch['griffin_lim']}), not RTISI-LA")
-    return [bank.pitch_profile(t.spec) if isinstance(t, BankTarget) else track_profile([tracks[f] for f in target_files(t)])
-            for _, _, t, _ in jobs]
+    return [([bank.pitch_profile(spec) for spec, _ in t.keyframes] if t.keyframes is not None else
+             bank.pitch_profile(t.spec)) if isinstance(t, BankTarget) else
+            track_profile([tracks[f] for f in target_files(t)]) for _, _, t, _ in jobs]
 
 
 def main(argv=None):
@@ -581,11 +647,14 @@ def main(argv=None):
         check_stream_args(p, args, argv)
     elif args.stream_pitch is not None:
         p.error("-stream_pitch needs -stream (offline conversions take -pitch_shift)")
+    elif args.stream_morph is not None:
+        p.error("-stream_morph needs -stream (offline conversions take -morph)")
     check_args(p, args)
     try:
         if args.semitones == "mv" and (args.speaker is not None or args.morph is not None):
             refuse_unprofiled_bank(args.bank)
-        elif args.stream and args.stream_pitch in ("match", "mv") and args.speaker is not None:
+        elif args.stream and args.stream_pitch in ("match", "mv") and (args.speaker is not None
+                                                                       or args.stream_morph is not None):
             refuse_unprofiled_bank(args.bank, f"-stream_pitch {args.stream_pitch}")
     except ValueError as e:
         p.error(str(e))
@@ -595,7 +664,8 @@ def main(argv=None):
             jobs = read_pairs(args.pairs, bank=bool(args.bank))
             os.makedirs(args.output, exist_ok=True)
         else:
-            target = (BankTarget(args.speaker) if args.speaker is not None else
+            target = (BankTarget(keyframes=tuple(args.keyframes)) if args.stream_morph is not None else
+                      BankTarget(args.speaker) if args.speaker is not None else
                       args.target[0] if len(args.target) == 1 else tuple(args.target))
             jobs = [(None, args.source, target, args.output)]
         run_stream(args, config, jobs)

@@ -2,7 +2,7 @@
 in real time.
 
     python tools/bench_stream.py [--streams 1 64 1024 4096] [--updates 20] [--config config.yaml] [-m ckpt -a attr]
-                                 [-pitch {0,SEMITONES,match,mv}]
+                                 [-pitch {0,SEMITONES,match,mv}] [-retarget]
 
 Reports, in one JSON line (and a summary on stderr):
   - per stream count S, at the default StreamParams (H = 8 frames = 100 ms per block): the mean wall time of one
@@ -20,7 +20,11 @@ Reports, in one JSON line (and a summary on stderr):
     prepared beforehand, median of 7) at 64 and 1 024 streams x 8 frames; and for match / mv the output's voiced log2
     F0 mean and std error (semitones, median over 5 synthetic glides, seeds 0-4) after warm-up, tracked offline, for
     glides pushed as magnitudes through PitchStage toward the GPU test's target (log2(220 Hz), 0.15), the test's
-    seeds 0-2 among them.
+    seeds 0-2 among them;
+  - with -retarget: before every update (start-up and timed alike) each stream is retargeted (at=None) to the next of
+    four codes over a ramp of H frames, so every window of every stream in steady state is a morph window (up to
+    four anchors, K = 4) and every frame lies in a ramp: the worst case.  The host time of the retarget calls is the
+    stage "retarget".
 The model has random weights unless -m is given; the input is synthetic (harmonic tones).  The card name and power
 limit are read in the same run.  Writes nothing.
 """
@@ -99,6 +103,8 @@ def main():
     ap.add_argument("-a", "--attr")
     ap.add_argument("--quality-seconds", type=float, default=6.0)
     ap.add_argument("-pitch", "--pitch", default="0", help="pitch setting of every stream: 0, SEMITONES, match or mv")
+    ap.add_argument("-retarget", "--retarget", action="store_true",
+                    help="retarget every stream before every update (a ramp of H frames through four codes)")
     args = ap.parse_args()
     target = (math.log2(200.0), 0.15)
     pitch = (args.pitch, *target) if args.pitch in ("match", "mv") else (float(args.pitch) or None)
@@ -120,7 +126,20 @@ def main():
     budget_ms = 1e3 * block / hp.sr
     c_out = cfg["SpeakerEncoder"]["c_out"]
     res = {"card": card(), "params": p.__dict__, "block_ms": budget_ms, "n_mels": hp.n_mels, "pitch": args.pitch,
-           "stages": {}}
+           "retarget": args.retarget, "stages": {}}
+    import time
+    from adaptive_voice_conversion_b200.streaming import KEEP
+    pool = [torch.randn(c_out, generator=torch.Generator().manual_seed(10 ** 6 + k)).to(dev) for k in range(4)]
+
+    def push(conv, ids, chunk, k):
+        """One update, after retargeting every stream with -retarget (its host time added to stage "retarget")."""
+        if args.retarget:
+            t0 = time.perf_counter()
+            for i, sid in enumerate(ids):
+                conv.retarget(sid, pool[(k + i) % len(pool)], ramp=p.hop, pitch=KEEP)
+            if conv.stage_ms is not None:
+                conv.stage_ms["retarget"] = conv.stage_ms.get("retarget", 0.0) + 1e3 * (time.perf_counter() - t0)
+        conv.push({sid: chunk for sid in ids})
     rt_ms = None
     for S in args.streams:
         conv = StreamingConverter(inf, voc, p)
@@ -130,13 +149,13 @@ def main():
         sig = harmonic(block * (args.updates + 40), hp.sr, seed=S).to(dev)
         # start-up (the first block needs m frames, start-up windows of every length) and graph captures
         pos = 0
-        for _ in range(20):
-            conv.push({sid: sig[pos:pos + block] for sid in ids})
+        for k in range(20):
+            push(conv, ids, sig[pos:pos + block], k)
             pos += block
         conv.stage_ms = {}
         torch.cuda.synchronize()
-        for _ in range(args.updates):
-            conv.push({sid: sig[pos:pos + block] for sid in ids})
+        for k in range(20, 20 + args.updates):
+            push(conv, ids, sig[pos:pos + block], k)
             pos += block
         st = {k: v / args.updates for k, v in conv.stage_ms.items()}
         st["update"] = sum(st.values())
