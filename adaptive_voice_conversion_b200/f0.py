@@ -55,7 +55,7 @@ import torch
 from . import _lib as L
 from .evaluate import speaker_of
 from .utils import _stream, eval_mode, upload_mels
-from .vocoder import PITCH_SHIFT_MAX, AudioParams, Vocoder, _Ragged
+from .vocoder import PITCH_SHIFT_MAX, AudioParams, Vocoder, _Ragged, _ptr
 
 METRICS = ("vuv_agree", "f0_corr", "st_target", "st_source", "f0_success", "st_target_source")
 
@@ -102,17 +102,22 @@ def yin(wavs, sr: int, hop: int, params: F0Params = F0Params()):
         if y.numel() < need:
             raise ValueError(f"yin: signal {i} has {y.numel()} samples; W = {params.win} and tau_max = "
                              f"{params.tau_max(sr)} need at least {need}")
-    dev = ys[0].device
-    r = _Ragged([y.numel() for y in ys], [1 + y.numel() // hop for y in ys], dev)
-    n = int(r.frame_offs[-1])
-    out = torch.empty(3, n, dtype=torch.float64, device=dev)
-    d = L.AudioDesc(hop=int(hop), n_seg=len(ys), n_frames=n, n_samples=int(r.sample_offs[-1]))
-    d.segs, y = C.c_void_p(r.table.data_ptr()), torch.cat(ys)
-    d.y = C.c_void_p(y.data_ptr())
-    L.check(L.load().avc_yin(C.byref(d), int(params.win), params.tau_min(sr), params.tau_max(sr),
-                             C.c_float(params.threshold), out[0].data_ptr(), out[1].data_ptr(), out[2].data_ptr(),
-                             _stream(dev)), "avc_yin")
+    r = _Ragged([y.numel() for y in ys], [1 + y.numel() // hop for y in ys], ys[0].device)
+    out = _yin_launch(r, torch.cat(ys), hop, sr, params)
     return list(zip(*[r.split_frames(o) for o in out]))
+
+
+def _yin_launch(r: _Ragged, y, hop: int, sr: int, params: F0Params, window: bool = False):
+    """float64 [3, frames of r] (tau, aperiodicity, energy) of the entries of r in the signal y, in one avc_yin launch,
+    or with window one avc_yin_window launch (each entry from r's frame origin on)."""
+    out = torch.empty(3, int(r.frame_offs[-1]), dtype=torch.float64, device=y.device)
+    d = L.AudioDesc(hop=int(hop), n_seg=len(r.n_samples), n_frames=out.shape[1], n_samples=int(r.sample_offs[-1]),
+                    segs=_ptr(r.table), y=_ptr(y))
+    name = "avc_yin_window" if window else "avc_yin"
+    L.check(getattr(L.load(), name)(C.byref(d), int(params.win), params.tau_min(sr), params.tau_max(sr),
+                                    C.c_float(params.threshold), _ptr(out[0]), _ptr(out[1]), _ptr(out[2]),
+                                    _stream(y.device)), name)
+    return out
 
 
 def voicing(tau: np.ndarray, aperiodicity: np.ndarray, energy: np.ndarray, sr: int, params: F0Params = F0Params()):

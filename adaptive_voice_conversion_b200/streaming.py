@@ -38,11 +38,11 @@ import numpy as np
 import torch
 
 from . import _lib as L
-from .f0 import F0Params
+from .f0 import F0Params, _yin_launch
 from .mcd import min_frames
 from .speaker_bank import interpolate_keyframes
 from .utils import _stream
-from .vocoder import _SEG, PITCH_SHIFT_MAX, _mel_project, _ptr, _ratio
+from .vocoder import PITCH_SHIFT_MAX, _mel_project, _ptr, _Ragged, _shift_rows
 
 
 @dataclass(frozen=True)
@@ -115,17 +115,22 @@ def release_sample(n: int, p: StreamParams, win: int, hop_s: int, m: int) -> int
     return (block_end(j, p.hop, p.lookahead, m) - 1) * hop_s + win // 2 - 1
 
 
+def _worst_latency(release, frames: int, win: int, hop_s: int) -> int:
+    """max of release(n) - n over the smallest output sample n each frame c < frames is the last covering frame of."""
+    worst = 0
+    for c in range(frames):
+        n = max(0, c * hop_s - win // 2)
+        if (n + win // 2) // hop_s == c:
+            worst = max(worst, release(n) - n)
+    return worst
+
+
 def latency_samples(p: StreamParams, win: int, hop_s: int, m: int) -> int:
     """max over output samples n >= 0 of release_sample(n) - n.  For a frame c the smallest n it is the last
     frame of is the worst; past the start-up windows the schedule repeats every block, so a few blocks beyond m
     cover every case.  Without start-up effects this is (H + LA + LA_v - 1) hop + win - 1."""
-    worst = 0
-    for c in range(m + 4 * p.hop + p.gl_lookahead + 2 * (win // hop_s) + 8):
-        n = max(0, c * hop_s - win // 2)
-        if (n + win // 2) // hop_s != c:
-            continue
-        worst = max(worst, release_sample(n, p, win, hop_s, m) - n)
-    return worst
+    return _worst_latency(lambda n: release_sample(n, p, win, hop_s, m),
+                          m + 4 * p.hop + p.gl_lookahead + 2 * (win // hop_s) + 8, win, hop_s)
 
 
 def yin_last_sample(t: int, hop_s: int, span: int) -> int:
@@ -146,35 +151,45 @@ def yin_ready(n: int, hop_s: int, span: int) -> int:
 def tracked_release_sample(n: int, p: StreamParams, win: int, hop_s: int, m: int, span: int) -> int:
     """release_sample for a stream with a target profile: n's last covering frame c is committed by the output RTISI-LA
     when frame t = c + gl_lookahead enters it, i.e. when YIN frame t has been tracked, i.e. when the shadow has released
-    sample yin_last_sample(t); the shadow releases it once it commits c' frames with c' hop - win/2 beyond it, when
-    frame c' - 1 + gl_lookahead has entered, which happens when its block is emitted."""
-    c = (n + win // 2) // hop_s
-    need = yin_last_sample(c + p.gl_lookahead, hop_s, span)
-    f = (need + win // 2) // hop_s + p.gl_lookahead
-    j = f // p.hop
-    return (block_end(j, p.hop, p.lookahead, m) - 1) * hop_s + win // 2 - 1
+    sample yin_last_sample(t); the shadow is synthesised on the output's schedule, so that is its release_sample."""
+    return release_sample(yin_last_sample((n + win // 2) // hop_s + p.gl_lookahead, hop_s, span), p, win, hop_s, m)
 
 
 def tracked_latency_samples(p: StreamParams, win: int, hop_s: int, m: int, span: int) -> int:
     """max over output samples n >= 0 of tracked_release_sample(n) - n, found as latency_samples finds its own.  With
     the defaults the tracking delays each frame by D = gl_lookahead + ceil((span - floor(span / 2) + win / 2) / hop) - 1
     frames (7 at 24 kHz: 3 + 5 - 1)."""
-    worst = 0
-    for c in range(m + 4 * p.hop + 2 * p.gl_lookahead + 2 * (win // hop_s) + span // hop_s + 8):
-        n = max(0, c * hop_s - win // 2)
-        if (n + win // 2) // hop_s != c:
-            continue
-        worst = max(worst, tracked_release_sample(n, p, win, hop_s, m, span) - n)
-    return worst
+    return _worst_latency(lambda n: tracked_release_sample(n, p, win, hop_s, m, span),
+                          m + 4 * p.hop + 2 * p.gl_lookahead + 2 * (win // hop_s) + span // hop_s + 8, win, hop_s)
+
+
+class _Tail:
+    """The rows of a growing sequence from absolute index ``first`` on: what later work still reads of it."""
+    __slots__ = ("x", "first")
+
+    def __init__(self, x):
+        self.x, self.first = x, 0
+
+    def append(self, y):
+        self.x = torch.cat([self.x, y])
+
+    def view(self, a: int, b: int | None = None):
+        """Rows a .. b - 1 (to the end without b), by absolute index."""
+        return self.x[a - self.first:None if b is None else b - self.first]
+
+    def trim(self, a: int):
+        """Drops the rows before absolute index a."""
+        if a > self.first:
+            self.x, self.first = self.x[a - self.first:], a
 
 
 # ------------------------------------------------------------------ analysis
 class _AStream:
-    __slots__ = ("n_in", "frames", "tail", "tail_first", "closed")
+    __slots__ = ("n_in", "frames", "tail", "closed")
 
     def __init__(self, dev):
-        self.n_in, self.frames, self.tail_first, self.closed = 0, 0, 0, False
-        self.tail = torch.empty(0, device=dev)
+        self.n_in, self.frames, self.closed = 0, 0, False
+        self.tail = _Tail(torch.empty(0, device=dev))
 
 
 class StreamAnalyzer:
@@ -212,7 +227,7 @@ class StreamAnalyzer:
                 raise ValueError(f"stream {sid!r} is closed")
             x = torch.as_tensor(x).to(device=self.dev, dtype=torch.float32).reshape(-1)
             if x.numel():
-                s.tail = torch.cat([s.tail, x])
+                s.tail.append(x)
                 s.n_in += x.numel()
         for sid in close:
             s = self.streams[sid]
@@ -220,38 +235,27 @@ class StreamAnalyzer:
                 raise ValueError(f"stream {sid!r} has {s.n_in} samples; an STFT with n_fft={hp.n_fft} needs at least "
                                  f"{hp.min_samples}")
             s.closed = True
-        segs, ys, ids, counts = [], [], [], []
-        soff = foff = 0
+        ys, ids, counts, origins = [], [], [], []
         for sid in dict.fromkeys(list(chunks) + list(close)):
             s = self.streams[sid]
             n = self.ready(s) - s.frames
             if n <= 0:
                 continue
-            first = self.first_sample(s.frames)
-            y = s.tail[first - s.tail_first:]
-            segs.append((soff, y.numel(), foff, n, s.frames))
-            ys.append(y)
+            ys.append(s.tail.view(self.first_sample(s.frames)))
             ids.append(sid)
             counts.append(n)
-            soff += y.numel()
-            foff += n
+            origins.append(s.frames)
             s.frames += n
-            keep = self.first_sample(s.frames)
-            s.tail, s.tail_first = s.tail[keep - s.tail_first:], keep
+            s.tail.trim(self.first_sample(s.frames))
         if not ids:
             return {}
-        tab = np.zeros(len(segs), _SEG)
-        for k, name in enumerate(("sample_off", "n_samples", "frame_off", "n_frames", "reserved")):
-            tab[name] = [g[k] for g in segs]
-        table = torch.from_numpy(tab.view(np.uint8)).to(self.dev)
-        mag = torch.empty(foff, hp.n_bins, device=self.dev)
+        r = _Ragged([y.numel() for y in ys], counts, self.dev, origins)
+        mag = torch.empty(sum(counts), hp.n_bins, device=self.dev)
         y = torch.cat(ys)
-        d = L.AudioDesc(n_fft=hp.n_fft, hop=hp.hop_length, win=hp.win_length, n_seg=len(segs), n_frames=foff,
-                        n_samples=int(soff), mode=L.STFT_MAG, preemph=hp.preemphasis, max_db=hp.max_db,
-                        ref_db=hp.ref_db, segs=_ptr(table), y=_ptr(y), mag_out=_ptr(mag))
+        d = r.desc(hp, mode=L.STFT_MAG, preemph=hp.preemphasis, y=y, mag_out=mag)
         L.check(L.load().avc_stft_window(C.byref(d), _stream(self.dev)), "avc_stft_window")
         mel = _mel_project(mag, self.voc.fb_t, L.MAG_TO_MEL, hp)
-        return dict(zip(ids, torch.split(mel, counts)))
+        return dict(zip(ids, r.split_frames(mel)))
 
 
 # ------------------------------------------------------------------ RTISI-LA
@@ -590,14 +594,30 @@ def live_anchors(frames, V, lo: int, window: int) -> int:
     return worst
 
 
-class _PStream:
-    __slots__ = ("ratio", "track", "pend", "frames", "n_rel", "tail", "tail_first", "tracked", "diag", "sched")
+class _Clock:
+    """Wall time per stage, each stage ended by a device synchronise: ``ms`` None is off, a dict accumulates
+    milliseconds per stage."""
 
-    def __init__(self, ratio=None, track=None, dev=None, n_bins=0, sched=None):
-        self.ratio, self.track, self.sched = ratio, track, sched
+    def __init__(self, dev):
+        self.dev, self.ms, self.t = dev, None, 0.0
+
+    def lap(self, key=None):
+        """Ends stage `key` (None: the time since the last lap belongs to no stage) and starts the next."""
+        if self.ms is not None:
+            torch.cuda.synchronize(self.dev)
+            t, self.t = self.t, time.perf_counter()
+            if key is not None:
+                self.ms[key] = self.ms.get(key, 0.0) + 1e3 * (self.t - t)
+
+
+class _PStream:
+    __slots__ = ("sched", "track", "pend", "frames", "n_rel", "tail", "tracked", "diag")
+
+    def __init__(self, sched, track=None, dev=None, n_bins=0):
+        self.sched, self.track = sched, track
         self.pend = torch.empty(0, n_bins, device=dev)          # unshifted magnitudes of frames not yet tracked
-        self.frames = self.n_rel = self.tail_first = self.tracked = 0
-        self.tail = torch.empty(0, device=dev)                  # shadow samples from tail_first on
+        self.frames = self.n_rel = self.tracked = 0
+        self.tail = _Tail(torch.empty(0, device=dev))           # shadow samples
         self.diag = {k: [] for k in ("tau", "aperiodicity", "energy", "log2_f0", "voiced", "shift", "shadow")}
 
 
@@ -624,22 +644,25 @@ class PitchStage:
         self.rt = Rtisi(hp, lookahead, n_iter, device)
         self.shadow = Rtisi(hp, lookahead, n_iter, device)
         self.dev = self.rt.dev
-        self.tau_min, self.tau_max = params.tau_min(hp.sr), params.tau_max(hp.sr)
-        self.span = int(params.win) + self.tau_max
+        self.span = int(params.win) + params.tau_max(hp.sr)
         self.streams, self.closed = {}, {}
-        self.stage_ms = None
+        self.clock = _Clock(self.dev)
 
     def open(self, sid, pitch=None, schedule: TargetSchedule = None):
-        """schedule, when given, holds the stream's per-frame pitch targets (TargetSchedule.shift / .profile) in place
-        of pitch's constant one; pitch still sets the kind."""
+        """schedule, when given, holds the stream's per-frame pitch targets (TargetSchedule.shift / .profile);
+        otherwise they are pitch's constant one.  pitch sets the kind."""
         pitch = parse_pitch(pitch)
         self.rt.open(sid)
+        if pitch is None:
+            return
+        if schedule is None:    # the stage never retargets, so the schedule's code is never read
+            schedule = TargetSchedule(None, pitch)
         if isinstance(pitch, float):
-            self.streams[sid] = _PStream(ratio=np.float32(_ratio(pitch)), sched=schedule)
-        elif pitch is not None:
+            self.streams[sid] = _PStream(schedule)
+        else:
             self.shadow.open(sid)
-            self.streams[sid] = _PStream(track=PitchTracker(*pitch, self.warmup, self.hp.sr, self.params),
-                                         dev=self.dev, n_bins=self.hp.n_bins, sched=schedule)
+            self.streams[sid] = _PStream(schedule, PitchTracker(*pitch, self.warmup, self.hp.sr, self.params),
+                                         self.dev, self.hp.n_bins)
 
     def next_frame(self, sid):
         """The first frame of stream sid whose pitch target the stage has not read yet; None when it reads none."""
@@ -680,18 +703,6 @@ class PitchStage:
             v.clear()
         return out
 
-    def _tick(self):
-        if self.stage_ms is None:
-            return 0.0
-        torch.cuda.synchronize(self.dev)
-        return time.perf_counter()
-
-    def _lap(self, key, t0):
-        t1 = self._tick()
-        if self.stage_ms is not None:
-            self.stage_ms[key] = self.stage_ms.get(key, 0.0) + 1e3 * (t1 - t0)
-        return t1
-
     def run(self, mags, close=()):
         hp = self.hp
         close = list(close)
@@ -703,50 +714,35 @@ class PitchStage:
             if sid in close and hp.hop_length * (T - 1) < self.params.min_samples(hp.sr):
                 raise ValueError(f"stream {sid!r}: {T} frames at close; tracking its pitch needs a signal of at least "
                                  f"{self.params.min_samples(hp.sr)} samples")
-        t0 = self._tick()
+        self.clock.lap()
         out = {sid: m for sid, m in mags.items() if sid not in self.streams}
-        rows, ratios, dest = [], [], []          # the rows of this update's avc_pitch_shift launch
+        rows, semis, dest = [], [], []           # the rows of this update's avc_pitch_shift launch
         for sid, m in mags.items():
             s = self.streams.get(sid)
             if s is not None and s.track is None and m.shape[0]:
                 n = int(m.shape[0])
                 rows.append(m)
-                if s.sched is None:
-                    ratios.append(np.full(n, s.ratio, np.float32))
-                elif len(s.sched.codes) == 1:     # one anchor: weight 1 on every frame, its own shift
-                    ratios.append(np.full(n, np.float32(_ratio(s.sched.pitch[0])), np.float32))
-                else:
-                    ratios.append(np.array([_ratio(v) for v in s.sched.shift(s.frames, n).tolist()],
-                                           np.float64).astype(np.float32))
+                semis.append(s.sched.shift(s.frames, n))
                 dest.append(sid)
                 s.frames += n
         if tracked:
-            t0 = self._track(tracked, mags, close, rows, ratios, dest, t0)
+            self._track(tracked, mags, close, rows, semis, dest)
         if rows:
-            S = torch.cat(rows).float().contiguous()
-            ratio = torch.from_numpy(np.concatenate(ratios)).to(self.dev)
-            shifted = torch.empty_like(S)
-            L.check(L.load().avc_pitch_shift(_ptr(S), _ptr(ratio), _ptr(shifted), S.shape[0], hp.n_bins,
-                                             int(hp.ps_lifter), _stream(self.dev)), "avc_pitch_shift")
-            parts = {}
-            for sid, r in zip(dest, torch.split(shifted, [int(r.shape[0]) for r in rows])):
-                parts.setdefault(sid, []).append(r)
-            for sid, rs in parts.items():
-                out[sid] = rs[0] if len(rs) == 1 else torch.cat(rs)
+            out.update(zip(dest, _shift_rows(rows, semis, hp)))
         if tracked or rows:
-            t0 = self._lap("shift", t0)
+            self.clock.lap("shift")
         res = self.rt.run(out, close)
-        self._lap("rtisi", t0)
+        self.clock.lap("rtisi")
         for sid in close:
             s = self.streams.pop(sid, None)
             if s is not None and s.track is not None and self.keep:
                 self.closed[sid] = s.diag
         return res
 
-    def _track(self, tracked, mags, close, rows, ratios, dest, t0):
+    def _track(self, tracked, mags, close, rows, semis, dest):
         """The shadow synthesis and tracking of an update, and the host shifts; the newly tracked frames' rows are
-        appended to rows / ratios / dest."""
-        hp, hop = self.hp, self.hp.hop_length
+        appended to rows / semis / dest."""
+        hop = self.hp.hop_length
         shadow_in = {}
         for sid in tracked:
             s, m = self.streams[sid], mags.get(sid)
@@ -755,71 +751,49 @@ class PitchStage:
                 s.pend = torch.cat([s.pend, m.float()])
                 s.frames += int(m.shape[0])
         res = self.shadow.run(shadow_in, [sid for sid in tracked if sid in close])
-        t0 = self._lap("shadow", t0)
-        segs, ys, entries, soff, foff = [], [], [], 0, 0
+        self.clock.lap("shadow")
+        ys, entries = [], []
         for sid in tracked:
             s = self.streams[sid]
             y = res.get(sid)
             if y is not None and y.numel():
-                s.tail = torch.cat([s.tail, y])
+                s.tail.append(y)
                 s.n_rel += int(y.numel())
                 if self.keep:
                     s.diag["shadow"].append(y)
             ready = s.frames if sid in close else min(s.frames, yin_ready(s.n_rel, hop, self.span))
-            n = ready - s.tracked
-            if n <= 0:
-                continue
-            seg = s.tail[self.first_sample(s.tracked) - s.tail_first:]
-            segs.append((soff, int(seg.numel()), foff, n, s.tracked))
-            ys.append(seg)
-            entries.append((sid, n))
-            soff += int(seg.numel())
-            foff += n
+            if ready > s.tracked:
+                ys.append(s.tail.view(self.first_sample(s.tracked)))
+                entries.append((sid, s, ready - s.tracked))
         if not entries:
-            return t0
-        tab = np.zeros(len(segs), _SEG)
-        for k, name in enumerate(("sample_off", "n_samples", "frame_off", "n_frames", "reserved")):
-            tab[name] = [g[k] for g in segs]
-        table = torch.from_numpy(tab.view(np.uint8)).to(self.dev)
-        y = torch.cat(ys)
-        yin = torch.empty(3, foff, dtype=torch.float64, device=self.dev)
-        d = L.AudioDesc(hop=hop, n_seg=len(segs), n_frames=foff, n_samples=int(soff), segs=_ptr(table), y=_ptr(y))
-        L.check(L.load().avc_yin_window(C.byref(d), int(self.params.win), self.tau_min, self.tau_max,
-                                        C.c_float(self.params.threshold), _ptr(yin[0]), _ptr(yin[1]), _ptr(yin[2]),
-                                        _stream(self.dev)), "avc_yin_window")
-        t0 = self._lap("tracking", t0)
+            return
+        r = _Ragged([y.numel() for y in ys], [n for _, _, n in entries], self.dev, [s.tracked for _, s, _ in entries])
+        yin = _yin_launch(r, torch.cat(ys), hop, self.hp.sr, self.params, window=True)
+        self.clock.lap("tracking")
         host = yin.cpu().numpy()                 # the update's one device-to-host copy
-        t0 = self._lap("tracking_copy", t0)
-        f = 0
-        for sid, n in entries:
-            s = self.streams[sid]
-            tau, ap, en = host[0, f:f + n], host[1, f:f + n], host[2, f:f + n]
-            f += n
-            targets = () if s.sched is None else s.sched.profile(s.tracked, n)
-            logf, voiced, shift = s.track.update(tau, ap, en, *targets)
+        self.clock.lap("tracking_copy")
+        for (sid, s, n), (tau, ap, en) in zip(entries, np.split(host, r.frame_offs[1:-1], axis=1)):
+            logf, voiced, shift = s.track.update(tau, ap, en, *s.sched.profile(s.tracked, n))
             rows.append(s.pend[:n])
-            ratios.append(np.array([_ratio(v) for v in shift.tolist()], np.float64).astype(np.float32))
+            semis.append(shift)
             dest.append(sid)
             s.pend = s.pend[n:]
             s.tracked += n
-            keep = self.first_sample(s.tracked)
-            if keep > s.tail_first:
-                s.tail, s.tail_first = s.tail[keep - s.tail_first:], keep
+            s.tail.trim(self.first_sample(s.tracked))
             if self.keep:
                 for k, v in (("tau", tau), ("aperiodicity", ap), ("energy", en), ("log2_f0", logf),
                              ("voiced", voiced), ("shift", shift)):
                     s.diag[k].append(np.array(v))
-        return t0
 
 
 # ------------------------------------------------------------------ the converter
 class _CStream:
-    __slots__ = ("sched", "hist", "hist_first", "block", "prev", "mels", "e_last")
+    __slots__ = ("sched", "hist", "block", "prev", "mels", "e_last")
 
     def __init__(self, sched, dev, n_mels):
         self.sched = sched
-        self.hist = torch.empty(0, n_mels, device=dev)
-        self.hist_first, self.block, self.prev, self.mels, self.e_last = 0, 0, None, [], 0
+        self.hist = _Tail(torch.empty(0, n_mels, device=dev))
+        self.block, self.prev, self.mels, self.e_last = 0, None, [], 0
 
 
 class StreamingConverter:
@@ -864,12 +838,21 @@ class StreamingConverter:
                               for k in ("mean", "std"))
         self.streams, self.closed = {}, {}
         self._next = 0
-        # a dict: each update adds the wall time (synchronised) of analysis, conversion and rtisi, and with pitch
-        # streams of shadow, tracking, tracking_copy (the YIN outputs' copy to the host) and shift
-        self.stage_ms = None
+        self.clock = self.stage.clock
         self.latency_samples = latency_samples(params, self.hp.win_length, self.hp.hop_length, self.m)
         self.tracked_latency_samples = tracked_latency_samples(params, self.hp.win_length, self.hp.hop_length, self.m,
                                                                self.stage.span)
+
+    @property
+    def stage_ms(self):
+        """None (off, the default) or a dict: each update adds the wall time (synchronised) of analysis, conversion
+        and rtisi, and with pitch streams of shadow, tracking, tracking_copy (the YIN outputs' copy to the host) and
+        shift."""
+        return self.clock.ms
+
+    @stage_ms.setter
+    def stage_ms(self, ms):
+        self.clock.ms = ms
 
     def _check_code(self, code, what):
         if (not isinstance(code, torch.Tensor) or code.dtype != torch.float32 or tuple(code.shape) != (self.c_out,)
@@ -956,13 +939,12 @@ class StreamingConverter:
             T = 1 + (a.n_in + (torch.as_tensor(chunks[sid]).numel() if sid in chunks else 0)) // self.hp.hop_length
             if T < self.m:
                 raise ValueError(f"stream {sid!r} has {T} frames at close; the model needs at least {self.m}")
-        t0 = self._tick()
+        self.clock.lap()
         new = self.ana.push(chunks, close)
         for sid, mel in new.items():
-            s = self.streams[sid]
             if self.norm is not None:
                 mel = (mel - self.norm[0]) / self.norm[1]
-            s.hist = torch.cat([s.hist, mel])
+            self.streams[sid].hist.append(mel)
         # the windows of every ready block, and of each closing stream's last one
         wins = []     # (sid, block start, block end, window start, window end)
         for sid in dict.fromkeys(list(chunks) + list(close)):
@@ -976,7 +958,7 @@ class StreamingConverter:
                 w0, w1 = close_window(F, W)
                 wins.append((sid, s.block * H, F, w0, w1))
                 s.block = -(-F // H)
-        t1 = self._tick()
+        self.clock.lap("analysis")
         outs = self._convert(wins, final=set(close))
         blocks = {}
         for (sid, b0, b1, w0, w1), dec in zip(wins, outs):
@@ -1000,15 +982,8 @@ class StreamingConverter:
             mags = dict(zip(ids, torch.split(self.voc.mel_to_mag([mel])[0], [c.shape[0] for c in cat])))
         # history no longer needed: the next window, or the last one at close, starts at or after frame F - W
         for sid in chunks:
-            s = self.streams[sid]
-            keep = max(0, self.ana.streams[sid].frames - W)
-            if keep > s.hist_first:
-                s.hist, s.hist_first = s.hist[keep - s.hist_first:], keep
-        t2 = self._tick()
-        if self.stage_ms is not None:
-            for k, a, b in (("analysis", t0, t1), ("conversion", t1, t2)):
-                self.stage_ms[k] = self.stage_ms.get(k, 0.0) + 1e3 * (b - a)
-        self.stage.stage_ms = self.stage_ms
+            self.streams[sid].hist.trim(max(0, self.ana.streams[sid].frames - W))
+        self.clock.lap("conversion")
         res = self.stage.run(mags, close)
         for sid in chunks:
             if sid not in close:
@@ -1020,60 +995,44 @@ class StreamingConverter:
             self.ana.drop(sid)
         return {sid: res.get(sid, torch.empty(0, device=self.dev)) for sid in dict.fromkeys(list(chunks) + list(close))}
 
-    def _tick(self):
-        if self.stage_ms is None:
-            return 0.0
-        torch.cuda.synchronize(self.dev)
-        return time.perf_counter()
-
     def _convert(self, wins, final):
         """Converted mels [window frames, n_mels] of every window, grouped into batches: plain windows by length, morph
         windows by length and anchor count K rounded up to a power of two (the padding anchors have zero weight)."""
         out = [None] * len(wins)
-        groups, morph = {}, {}
+        groups = {}    # (length, close window, K rounded up; None for plain windows): [(window, codes, weights)]
         for k, (sid, _, _, w0, w1) in enumerate(wins):
             sched = self.streams[sid].sched
             a, w = sched.window(w0, w1)
-            if w is None:
-                groups.setdefault((w1 - w0, sid in final), []).append((k, sched.codes[a]))
-            else:
-                Kp = 1 << (len(a) - 1).bit_length()
-                morph.setdefault((w1 - w0, sid in final, Kp), []).append((k, [sched.codes[i] for i in a], w))
-        for (Lw, last), items in groups.items():
+            Kp = None if w is None else 1 << (len(a) - 1).bit_length()
+            codes = [sched.codes[a]] if w is None else [sched.codes[i] for i in a]
+            groups.setdefault((w1 - w0, sid in final, Kp), []).append((k, codes, w))
+        for (Lw, last, Kp), items in sorted(groups.items(), key=lambda g: g[0][2] is not None):   # plain ones first
             for f in range(0, len(items), self.p.batch_max):
                 part = items[f:f + self.p.batch_max]
-                xs = [self._slice(wins[k]) for k, _ in part]
-                codes = [c for _, c in part]
-                if last:   # a close window has any length: eager, the exact batch
-                    dec = self.inf.model.inference_from_embeddings(torch.stack(xs), torch.stack(codes))
-                else:
-                    Bp = min(self.p.batch_max, 1 << (len(part) - 1).bit_length())
-                    xb, eb, run = self._slot(Bp, Lw)
-                    rows = list(range(len(part))) + [0] * (Bp - len(part))
-                    xb.copy_(torch.stack([xs[r] for r in rows]))
-                    eb.copy_(torch.stack([codes[r] for r in rows]))
-                    dec = run()
-                for j, (k, _) in enumerate(part):
-                    out[k] = dec[j, :, :Lw].transpose(0, 1)
-        for (Lw, last, Kp), items in morph.items():
-            for f in range(0, len(items), self.p.batch_max):
-                part = items[f:f + self.p.batch_max]
+                # a close window has any length: eager, the exact batch; otherwise padded by repeating row 0
                 B = len(part) if last else min(self.p.batch_max, 1 << (len(part) - 1).bit_length())
-                rows = list(range(len(part))) + [0] * (B - len(part))
-                zero = torch.zeros(self.c_out, device=self.dev)
-                x = torch.stack([self._slice(wins[part[r][0]]) for r in rows])
-                cb = torch.stack([c for r in rows for c in part[r][1] + [zero] * (Kp - len(part[r][1]))])
-                wh = np.zeros((B, Kp, Lw), np.float32)          # the batch's weights, built on the host
-                for j, r in enumerate(rows):
-                    wh[j, :part[r][2].shape[0]] = part[r][2]
-                if last:   # eager, the exact batch
-                    dec = self.inf.model.inference_morph(x, cb.view(B, Kp, self.c_out), torch.from_numpy(wh).to(self.dev))
+                rows = part + [part[0]] * (B - len(part))
+                x = torch.stack([self._slice(wins[k]) for k, _, _ in rows])
+                if Kp is None:
+                    ins = (x, torch.stack([c[0] for _, c, _ in rows]))
                 else:
-                    xb, cbuf, wb, lx, run = self.inf._morph_slot(B, self.n_mels, Lw, Kp, self.dev)
-                    xb.copy_(x)
-                    cbuf.copy_(cb.view(B, Kp, self.c_out))
-                    wb.copy_(torch.from_numpy(wh))                  # one upload per batch
-                    lx.fill_(Lw)                                    # the slot is shared with Inferencer.inference_morph
+                    zero = torch.zeros(self.c_out, device=self.dev)
+                    cb = torch.stack([c for _, cs, _ in rows for c in cs + [zero] * (Kp - len(cs))])
+                    wh = np.zeros((B, Kp, Lw), np.float32)          # the batch's weights, built on the host
+                    for j, (_, _, w) in enumerate(rows):
+                        wh[j, :w.shape[0]] = w
+                    ins = (x, cb.view(B, Kp, self.c_out), torch.from_numpy(wh))
+                model = self.inf.model
+                if last:
+                    dec = (model.inference_from_embeddings if Kp is None else model.inference_morph)(
+                        *(t.to(self.dev) for t in ins))
+                else:
+                    *bufs, run = (self._slot(B, Lw) if Kp is None else
+                                  self.inf._morph_slot(B, self.n_mels, Lw, Kp, self.dev))
+                    for b, t in zip(bufs, ins):                      # a morph batch's weights: one upload
+                        b.copy_(t)
+                    if Kp is not None:
+                        bufs[3].fill_(Lw)                           # the slot is shared with Inferencer.inference_morph
                     dec = run()
                 for j, (k, _, _) in enumerate(part):
                     out[k] = dec[j, :, :Lw].transpose(0, 1)
@@ -1083,8 +1042,7 @@ class StreamingConverter:
 
     def _slice(self, win):
         sid, _, _, w0, w1 = win
-        s = self.streams[sid]
-        return s.hist[w0 - s.hist_first:w1 - s.hist_first].transpose(0, 1)
+        return self.streams[sid].hist.view(w0, w1).transpose(0, 1)
 
     def _slot(self, B, T):
         inf = self.inf

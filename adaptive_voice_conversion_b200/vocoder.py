@@ -139,9 +139,10 @@ def _ptr(t):
 
 
 class _Ragged:
-    """Utterances laid end to end: the device table of per-utterance sample and frame offsets."""
+    """Utterances laid end to end: the device table of per-utterance sample and frame offsets, and with origins each
+    entry's frame origin (``reserved``: the absolute index of its first frame, for the windowed kernels)."""
 
-    def __init__(self, n_samples, n_frames, dev):
+    def __init__(self, n_samples, n_frames, dev, origins=None):
         self.n_samples, self.n_frames = [int(n) for n in n_samples], [int(n) for n in n_frames]
         self.sample_offs = np.concatenate([[0], np.cumsum(self.n_samples)]).astype(np.int64)
         self.frame_offs = np.concatenate([[0], np.cumsum(self.n_frames)]).astype(np.int64)
@@ -150,6 +151,8 @@ class _Ragged:
         tab = np.zeros(len(self.n_samples), _SEG)
         tab["sample_off"], tab["n_samples"] = self.sample_offs[:-1], self.n_samples
         tab["frame_off"], tab["n_frames"] = self.frame_offs[:-1], self.n_frames
+        if origins is not None:
+            tab["reserved"] = origins
         self.table = torch.from_numpy(tab.view(np.uint8)).to(dev)
 
     def desc(self, hp: AudioParams, **kw) -> L.AudioDesc:
@@ -424,14 +427,19 @@ def pitch_shift(mags, semitones, hp: AudioParams = AudioParams()):
     equal values gives the bits of that value as a float."""
     if not mags:
         raise ValueError("pitch_shift: empty batch")
+    return _shift_rows(mags, _semitones(semitones, len(mags), "pitch_shift", [int(m.shape[0]) for m in mags]), hp)
+
+
+def _shift_rows(mags, semitones, hp: AudioParams):
+    """The avc_pitch_shift launch of pitch_shift, on shifts it does not check: semitones[i] is a float or a float64
+    array of one value per frame of mags[i]."""
     lens = [int(m.shape[0]) for m in mags]
-    s = _semitones(semitones, len(mags), "pitch_shift", lens)
     dev = mags[0].device
     S = torch.cat([m.float() for m in mags]).contiguous()
     if S.dim() != 2 or S.shape[1] != hp.n_bins:
         raise ValueError(f"pitch_shift: magnitudes have shape {tuple(S.shape)}, n_fft={hp.n_fft} gives {hp.n_bins} bins")
     ratio = np.concatenate([np.full(T, _ratio(v), np.float64) if isinstance(v, float) else
-                            np.array([_ratio(x) for x in v.tolist()], np.float64) for v, T in zip(s, lens)])
+                            np.array([_ratio(x) for x in v.tolist()], np.float64) for v, T in zip(semitones, lens)])
     ratio = torch.from_numpy(ratio.astype(np.float32)).to(dev)
     out = torch.empty_like(S)
     L.check(L.load().avc_pitch_shift(_ptr(S), _ptr(ratio), _ptr(out), S.shape[0], hp.n_bins, int(hp.ps_lifter),
