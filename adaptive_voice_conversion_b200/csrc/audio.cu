@@ -104,11 +104,13 @@ __device__ __forceinline__ int reflect(int i, int L) {
 }
 
 // The same for a segment that holds samples [first, first + L) of a longer signal, which starts at 0 and ends with
-// the segment: the signal's sample i as an index into the segment.  first = 0 is reflect(i, L).
-__device__ __forceinline__ int reflect_window(int i, int first, int L) {
-  if (i < 0) i = -i;
-  if (i >= first + L) i = 2 * (first + L - 1) - i;
-  return min(max(i - first, 0), L - 1);
+// the segment: the signal's sample first + p as an index into the segment.  Positions are relative to first, so they
+// stay small however long the signal is; the reflection at the signal's sample 0 applies only when first = 0 (at_0),
+// which is then reflect(p, L).
+__device__ __forceinline__ int reflect_window(int p, bool at_0, int L) {
+  if (at_0 && p < 0) p = -p;
+  if (p >= L) p = 2 * (L - 1) - p;
+  return min(max(p, 0), L - 1);
 }
 
 // ------------------------------------------------------------------ forward STFT
@@ -133,9 +135,11 @@ __global__ void __launch_bounds__(FFT_THREADS) stft_kernel(avc_audio_desc d) {
   // signal's sample first (0 for origin 0, the whole signal).  Every sample a frame reads, reflected at the end or
   // not, is at or after o hop - win/2 - 1, so with first one sample earlier its pre-emphasis neighbour is inside: a
   // read at segment index 0 happens only when first = 0, where index 0 is the signal's sample 0.
+  // With an origin, base is relative to first (64-bit products: o hop passes 2^31 after a day of a live stream).
   const int o = ORIGIN ? g.reserved : 0;
-  const int first = ORIGIN ? max(0, o * d.hop - d.win / 2 - 2) : 0;
-  const int base = (o + f - g.frame_off) * d.hop - NFFT / 2;
+  const int64_t first = ORIGIN ? max((int64_t)0, (int64_t)o * d.hop - d.win / 2 - 2) : 0;
+  const int base = ORIGIN ? (int)(((int64_t)o + (f - g.frame_off)) * d.hop - NFFT / 2 - first)
+                          : (f - g.frame_off) * d.hop - NFFT / 2;
   const float pe = d.preemph;
   float2* z = buf[fl];
   for (int n = t; n < NC; n += TPF) {
@@ -144,7 +148,7 @@ __global__ void __launch_bounds__(FFT_THREADS) stft_kernel(avc_audio_desc d) {
     for (int e = 0; e < 2; ++e) {
       const int q = 2 * n + e - off;
       if (live && q >= 0 && q < d.win) {
-        const int i = ORIGIN ? reflect_window(base + 2 * n + e, first, L) : reflect(base + 2 * n + e, L);
+        const int i = ORIGIN ? reflect_window(base + 2 * n + e, first == 0, L) : reflect(base + 2 * n + e, L);
         float s = __ldg(y + i);
         if (pe != 0.f && i > 0) s -= pe * __ldg(y + i - 1);
         v[e] = hann(q, d.win) * s;
@@ -708,19 +712,21 @@ struct RtSmem {  // dynamic shared-memory layout of one CTA
   }
 };
 
-// est[i] = signal estimate at sample n0 + i, i < len: (numerator + the buffered frames c .. c + nbuf - 1 that cover it)
-// divided by the window sum-square of the frames 0 .. newest that cover it, where that exceeds FLT_MIN
-__device__ void rt_estimate(float* est, int n0, int len, const float* num, const float* fr, int c, int nbuf, int newest,
+// est[i] = signal estimate at sample c hop + r0 + i, i < len: (numerator + the buffered frames c .. c + nbuf - 1 that
+// cover it) divided by the window sum-square of the frames 0 .. newest (<= c + nbuf - 1) that cover it, where that
+// exceeds FLT_MIN.  Sample positions are relative to c hop, so they stay small however long the stream is; frames
+// are absolute, and the covering range is capped at c + nbuf so that it stays below 2^31 with the stream's frames.
+__device__ void rt_estimate(float* est, int r0, int len, const float* num, const float* fr, int c, int nbuf, int newest,
                             int nb, int win, int hop) {
-  const int a0 = c * hop - win / 2, h = win / 2;
+  const int h = win / 2;
   for (int i = threadIdx.x; i < len; i += blockDim.x) {
-    const int n = n0 + i;
-    const int lo = rt_floordiv(n + h - win, hop) + 1, hi = rt_floordiv(n + h, hop);
-    float acc = (n - a0 >= 0 && n - a0 < win) ? num[n - a0] : 0.f;
-    for (int F = max(lo, c); F <= min(hi, c + nbuf - 1); ++F) acc += fr[(F % nb) * win + n - F * hop + h];
+    const int r = r0 + i;
+    const int lo = c + rt_floordiv(r + h - win, hop) + 1, hi = c + min(rt_floordiv(r + h, hop), nbuf);
+    float acc = (r + h >= 0 && r + h < win) ? num[r + h] : 0.f;
+    for (int F = max(lo, c); F <= min(hi, c + nbuf - 1); ++F) acc += fr[(F % nb) * win + r - (F - c) * hop + h];
     float wss = 0.f;
     for (int F = max(lo, 0); F <= min(hi, newest); ++F) {
-      const float w = hann(n - F * hop + h, win);
+      const float w = hann(r - (F - c) * hop + h, win);
       wss += w * w;
     }
     est[i] = wss > FLT_MIN ? acc / wss : acc;
@@ -823,8 +829,7 @@ __global__ void __launch_bounds__((RT_MAX_LA + 1) * TPF) rtisi_kernel(avc_rtisi_
   // K Jacobi iterations over the buffered frames c .. c + nbuf - 1, the newest present frame being the last of them
   auto iterate = [&]() {
     for (int it = 0; it < d.n_iter; ++it) {
-      const int n0 = c * hop - h;
-      rt_estimate(est, n0, (nbuf - 1) * hop + win, num, fr, c, nbuf, c + nbuf - 1, nb, win, hop);
+      rt_estimate(est, -h, (nbuf - 1) * hop + win, num, fr, c, nbuf, c + nbuf - 1, nb, win, hop);
       __syncthreads();
       const int F = c + g;
       const bool live = g < nbuf;
@@ -833,23 +838,24 @@ __global__ void __launch_bounds__((RT_MAX_LA + 1) * TPF) rtisi_kernel(avc_rtisi_
       __syncthreads();
     }
   };
-  // release samples n0 .. n0 + cnt_rel - 1 of the numerator (frames 0 .. last cover them), n >= 0 only, de-emphasised
-  auto release = [&](int n0, int len, int last) {
+  // release samples c hop + r0 .. c hop + r0 + len - 1 of the numerator (frames 0 .. last <= c cover them), n >= 0
+  // only, de-emphasised; positions relative to c hop as in rt_estimate, only the test n >= 0 forms c hop (in 64 bits)
+  auto release = [&](int r0, int len, int last) {
     float* rel = est;
-    const int a0 = c * hop - h;
     for (int i = threadIdx.x; i < len; i += blockDim.x) {
-      const int n = n0 + i;
-      const int lo = rt_floordiv(n + h - win, hop) + 1, hi = rt_floordiv(n + h, hop);
+      const int r = r0 + i;
+      const int lo = c + rt_floordiv(r + h - win, hop) + 1, hi = c + min(rt_floordiv(r + h, hop), 1);
       float wss = 0.f;
       for (int F = max(lo, 0); F <= min(hi, last); ++F) {
-        const float wv = hann(n - F * hop + h, win);
+        const float wv = hann(r - (F - c) * hop + h, win);
         wss += wv * wv;
       }
-      const float acc = num[n - a0];
+      const float acc = num[r + h];
       rel[i] = wss > FLT_MIN ? acc / wss : acc;
     }
     __syncthreads();
-    const int skip = max(0, -n0), cntw = max(0, len - skip);
+    const int64_t n0 = (int64_t)c * hop + r0;
+    const int skip = n0 < 0 ? (int)min(-n0, (int64_t)len) : 0, cntw = len - skip;
     if (threadIdx.x == 0) {
       for (int i = skip; i < len; ++i) {
         carry = rel[i] + d.deemph * carry;
@@ -866,7 +872,7 @@ __global__ void __launch_bounds__((RT_MAX_LA + 1) * TPF) rtisi_kernel(avc_rtisi_
     const float* f = fr + (size_t)(c % nb) * win;
     for (int i = threadIdx.x; i < win; i += blockDim.x) num[i] += f[i];
     __syncthreads();
-    release(c * hop - h, hop, c);
+    release(-h, hop, c);
     float* tmp = est + win;
     for (int i = threadIdx.x; i < win; i += blockDim.x) tmp[i] = i + hop < win ? num[i + hop] : 0.f;
     __syncthreads();
@@ -881,7 +887,7 @@ __global__ void __launch_bounds__((RT_MAX_LA + 1) * TPF) rtisi_kernel(avc_rtisi_
     float* m = st_mag + (int64_t)(T % nb) * NBIN;
     for (int k = threadIdx.x; k < NBIN; k += blockDim.x) m[k] = __ldg(d.mag + (int64_t)r * NBIN + k);
     // start phase: the estimate of the frames 0 .. T-1 over the entering frame's support
-    rt_estimate(est, T * hop - h, win, num, fr, c, nbuf, T - 1, nb, win, hop);
+    rt_estimate(est, nbuf * hop - h, win, num, fr, c, nbuf, T - 1, nb, win, hop);
     __syncthreads();
     rt_project(zb + (size_t)g * NC, nyq + g, tab, t, est, m, fr + (size_t)(T % nb) * win, g == 0, win);
     __syncthreads();
@@ -895,9 +901,9 @@ __global__ void __launch_bounds__((RT_MAX_LA + 1) * TPF) rtisi_kernel(avc_rtisi_
       iterate();
       commit();
     }
-    // the samples after the last commit's, up to the grid's end hop (T - 1)
-    const int n0 = T * hop - h, n1 = (T - 1) * hop;
-    if (T > 0 && n1 > max(n0, 0)) release(n0, n1 - n0, T - 1);
+    // the samples after the last commit's, T hop - win/2 .. hop (T - 1) - 1 (c = T now), where the grid ends: there are
+    // some when hop < win/2 and T > 1 (for T = 1 they are all before sample 0)
+    if (T > 1 && h > hop) release(-h, h - hop, T - 1);
   }
   for (int i = threadIdx.x; i < nb * win; i += blockDim.x) st[i] = fr[i];
   for (int i = threadIdx.x; i < win; i += blockDim.x) st_num[i] = num[i];

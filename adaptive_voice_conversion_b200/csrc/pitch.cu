@@ -39,11 +39,13 @@ __device__ __forceinline__ int reflect1(int i, int L) {
 }
 
 // The same for an entry that holds samples [first, first + L) of a longer signal, which starts at 0 and ends with the
-// entry: the signal's sample i as an index into the entry.  first = 0 is reflect1(i, L).
-__device__ __forceinline__ int reflect1_window(int i, int first, int L) {
-  if (i < 0) i = -i;
-  if (i >= first + L) i = 2 * (first + L - 1) - i;
-  return min(max(i - first, 0), L - 1);
+// entry: the signal's sample first + p as an index into the entry.  Positions are relative to first, so they stay small
+// however long the signal is; the reflection at the signal's sample 0 applies only when first = 0 (at_0), which is
+// then reflect1(p, L).
+__device__ __forceinline__ int reflect1_window(int p, bool at_0, int L) {
+  if (at_0 && p < 0) p = -p;
+  if (p >= L) p = 2 * (L - 1) - p;
+  return min(max(p, 0), L - 1);
 }
 
 // avc_yin_window's first sample of an entry with frame origin o, span = win + tau_max: frame o's reads, reflected at
@@ -90,9 +92,9 @@ __global__ void __launch_bounds__(YIN_MAX_THREADS) yin_kernel(avc_audio_desc d, 
       if (t == 0) tau_out[f] = ap_out[f] = en_out[f] = __longlong_as_double(0x7ff8000000000000LL);
       return;
     }
-    const int base = (int)(centre - half);
+    const int base = (int)(centre - half - first);   // relative to first
     for (int i = t; i < n_stage; i += nt)
-      xs[skew(i)] = i < span ? (double)__ldg(y + reflect1_window(base + i, (int)first, L)) : 0.0;
+      xs[skew(i)] = i < span ? (double)__ldg(y + reflect1_window(base + i, first == 0, L)) : 0.0;
   } else {
     const int64_t centre = (int64_t)(f - g.frame_off) * d.hop;
     // one reflection on each side: -half >= -(L-1) and centre + span - half - 1 <= 2 (L-1)

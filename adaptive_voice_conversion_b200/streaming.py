@@ -259,6 +259,9 @@ class StreamAnalyzer:
 
 
 # ------------------------------------------------------------------ RTISI-LA
+RTISI_MAX_FRAMES = 2 ** 31 - 1   # frames of one stream (int32 counts): about 310 days at hop 300 and 24 kHz
+
+
 class Rtisi:
     """RTISI-LA state of many streams in a pool of slots, and one avc_rtisi_la launch per update.
     ``run({id: mags [n, n_bins]}, close=())`` returns {id: released samples}."""
@@ -314,6 +317,11 @@ class Rtisi:
         ids = list(dict.fromkeys(list(mags) + list(close)))
         if not ids:
             return None
+        for sid in ids:   # avc_rtisi_la's frame counts are int32: refuse before any state changes
+            c, nb = self.host[sid]
+            m = mags.get(sid)
+            if c + nb + (0 if m is None else int(m.shape[0])) > RTISI_MAX_FRAMES:
+                raise ValueError(f"stream {sid!r} would pass {RTISI_MAX_FRAMES} frames, the RTISI-LA limit")
         rows, offs, slots, closes, outs, counts = [], [0], [], [], [0], []
         for sid in ids:
             c, nb = self.host[sid]

@@ -585,7 +585,9 @@ int avc_stft(const avc_audio_desc* d, void* stream);
  * not, is at or after o hop - win/2 - 1, and its pre-emphasis neighbour is inside the entry.  The signal is
  * reflect-padded at its sample 0 and at the entry's end; an entry that is a window of a signal still arriving lists
  * only frames whose non-zero window samples lie inside it.  A frame gets avc_stft's bits for the whole signal under
- * any origin; o = 0 for every entry is avc_stft. */
+ * any origin; o = 0 for every entry is avc_stft.  Sample positions are 64-bit or relative to the entry's first
+ * sample, so they may pass 2^31; the limit is the int32 origin and frame counts: a stream of at most 2^31 - 1 frames
+ * (about 310 days at hop 300 and 24 kHz). */
 int avc_stft_window(const avc_audio_desc* d, void* stream);
 /* iSTFT: irfft x window per frame into `frames`, then a gather overlap-add divided by the exact window sum-square
  * (where it exceeds FLT_MIN) with n_fft/2 cut from each end, into y.  X null: the spectrum is mag with zero phase.
@@ -644,7 +646,10 @@ int avc_pghi(const avc_audio_desc* d, float tol, int8_t* parent, void* stream);
  * Sums run in a fixed order without atomics: a stream's bits do not depend on the other streams of a launch or on
  * how its frames were split into launches.  A slot must appear once per launch.  AVC_ERR_UNSUPPORTED for n_fft !=
  * 2048, an odd win or win > n_fft, hop outside (0, win/2] or lookahead outside [0, AVC_RTISI_MAX_LOOKAHEAD];
- * AVC_ERR_INVALID for n_iter < 0, a de-emphasis that is not finite or a null pointer; both before any launch. */
+ * AVC_ERR_INVALID for n_iter < 0, a de-emphasis that is not finite or a null pointer; both before any launch.
+ * Length: sample positions are kept relative to sample c hop (c the committed count), so a stream may pass 2^31
+ * samples; its frame counts are int32, so a stream is limited to 2^31 - 1 frames (about 310 days at hop 300 and
+ * 24 kHz), which streaming.Rtisi refuses to pass. */
 #define AVC_RTISI_MAX_LOOKAHEAD 7
 typedef struct avc_rtisi_desc {
   int32_t n_fft, hop, win;
@@ -698,7 +703,8 @@ int avc_yin(const avc_audio_desc* d, int32_t win, int32_t tau_min, int32_t tau_m
  * only frames whose span lies inside it.  A frame gets avc_yin's bits for the whole signal under any origin and any
  * split of the signal into entries; o = 0 for every entry is avc_yin.  A frame whose reads would leave the entry, or
  * need a second reflection, and every frame of an entry with o < 0, gets NaN.  The same argument checks, codes and
- * messages (named avc_yin_window) as avc_yin, before any launch. */
+ * messages (named avc_yin_window) as avc_yin, before any launch.  As for avc_stft_window, positions may pass 2^31
+ * samples; origins and frame counts are int32. */
 int avc_yin_window(const avc_audio_desc* d, int32_t win, int32_t tau_min, int32_t tau_max, float threshold,
                    double* tau, double* aperiodicity, double* energy, void* stream);
 

@@ -40,20 +40,35 @@ def _covering(n, win, hop):
     return (n + h - win) // hop + 1, (n + h) // hop
 
 
+def _wss(n, lo_frame, hi_frame, win, hop):
+    """Window sum-square at samples n (an array) of the frames lo_frame .. hi_frame that cover each, added in
+    increasing frame order (the kernel's)."""
+    w2 = hann(win) ** 2
+    out = np.zeros(len(n))
+    if len(n) == 0:
+        return out
+    h = win // 2
+    first, last = _covering(int(n[0]), win, hop)[0], _covering(int(n[-1]), win, hop)[1]
+    for F in range(max(lo_frame, first), min(hi_frame, last) + 1):
+        q = n - F * hop + h
+        m = (q >= 0) & (q < win)
+        out[m] += w2[q[m]]
+    return out
+
+
 def estimate(st, n0, length, newest):
     win, hop, h = st.win, st.hop, st.win // 2
-    w2 = hann(win) ** 2
     a0 = st.c * hop - h
+    n = n0 + np.arange(length, dtype=np.int64)
     out = np.zeros(length)
-    for i in range(length):
-        n = n0 + i
-        lo, hi = _covering(n, win, hop)
-        acc = st.num[n - a0] if 0 <= n - a0 < win else 0.0
-        for F in range(max(lo, st.c), min(hi, st.c + st.nbuf - 1) + 1):
-            acc += st.fr[F][n - F * hop + h]
-        wss = sum(w2[n - F * hop + h] for F in range(max(lo, 0), min(hi, newest) + 1))
-        out[i] = acc / wss if wss > np.finfo(np.float32).tiny else acc
-    return out
+    m = (n - a0 >= 0) & (n - a0 < win)
+    out[m] = st.num[(n - a0)[m]]
+    for F in range(st.c, st.c + st.nbuf):
+        q = n - F * hop + h
+        m = (q >= 0) & (q < win)
+        out[m] += st.fr[F][q[m]]
+    wss = _wss(n, 0, newest, win, hop)
+    return np.where(wss > np.finfo(np.float32).tiny, out / np.where(wss > 0, wss, 1.0), out)
 
 
 def project(e, mag, win):
@@ -81,16 +96,14 @@ def _iterate(st, n_iter):
 
 def _release(st, n0, length, last, deemph, out):
     win, hop, h = st.win, st.hop, st.win // 2
-    w2 = hann(win) ** 2
     a0 = st.c * hop - h
-    for i in range(length):
-        n = n0 + i
-        lo, hi = _covering(n, win, hop)
-        wss = sum(w2[n - F * hop + h] for F in range(max(lo, 0), min(hi, last) + 1))
-        x = st.num[n - a0] / wss if wss > np.finfo(np.float32).tiny else st.num[n - a0]
-        if n >= 0:
-            st.carry = x + deemph * st.carry
-            out.append(st.carry)
+    n = n0 + np.arange(length, dtype=np.int64)
+    wss = _wss(n, 0, last, win, hop)
+    num = st.num[n - a0]
+    x = np.where(wss > np.finfo(np.float32).tiny, num / np.where(wss > 0, wss, 1.0), num)
+    for v in x[n >= 0]:       # the de-emphasis recurrence, in sample order
+        st.carry = v + deemph * st.carry
+        out.append(st.carry)
 
 
 def _commit(st, deemph, out):

@@ -173,3 +173,71 @@ def test_cli_stream_refusals(extra, msg):
 def test_cli_stream_needs_wav_output():
     r = _cli("-c", "config.yaml", "-s", "s.wav", "-t", "t.wav", "-o", "o.npy", "-stream")
     assert r.returncode == 2 and "-stream" in r.stderr, r.stderr
+
+
+def _direct_estimate(st, n0, length, newest):
+    """The estimate sample by sample, as the kernel's thread for sample n sums it."""
+    win, hop, h = st.win, st.hop, st.win // 2
+    w2 = R.hann(win) ** 2
+    out = np.zeros(length)
+    for i in range(length):
+        n = n0 + i
+        lo, hi = (n + h - win) // hop + 1, (n + h) // hop
+        acc = st.num[n - st.c * hop + h] if 0 <= n - st.c * hop + h < win else 0.0
+        for F in range(max(lo, st.c), min(hi, st.c + st.nbuf - 1) + 1):
+            acc += st.fr[F][n - F * hop + h]
+        wss = sum(w2[n - F * hop + h] for F in range(max(lo, 0), min(hi, newest) + 1))
+        out[i] = acc / wss if wss > np.finfo(np.float32).tiny else acc
+    return out
+
+
+def _direct_release(st, n0, length, last, deemph):
+    win, hop, h = st.win, st.hop, st.win // 2
+    w2 = R.hann(win) ** 2
+    out, carry = [], st.carry
+    for i in range(length):
+        n = n0 + i
+        lo, hi = (n + h - win) // hop + 1, (n + h) // hop
+        wss = sum(w2[n - F * hop + h] for F in range(max(lo, 0), min(hi, last) + 1))
+        x = st.num[n - st.c * hop + h]
+        x = x / wss if wss > np.finfo(np.float32).tiny else x
+        if n >= 0:
+            carry = x + deemph * carry
+            out.append(carry)
+    return np.asarray(out), carry
+
+
+@pytest.mark.parametrize("win,hop", [(1200, 300), (2046, 1023), (64, 1)])
+def test_rtisi_ref_vectorised_matches_direct_sums(win, hop):
+    """The restatement's numpy estimate and release against per-sample sums written out here, on random states at
+    the start of a stream (frames before 0 and samples before 0), far into one and past 2^31 samples."""
+    rng = np.random.default_rng(win + hop)
+    for la in (0, 3, 7):
+        for c in (0, 1, 2, 5, 40, 2 ** 31 // hop + 3):
+            for nbuf in sorted({0, 1, la, la + 1}):
+                st = R.State(win, hop, la)
+                st.c, st.nbuf, st.carry = c, nbuf, float(rng.standard_normal())
+                st.num = rng.standard_normal(win)
+                st.fr = {F: rng.standard_normal(win) for F in range(c, c + nbuf)}
+                h = win // 2
+                for n0, length, newest in [(c * hop - h, max(nbuf - 1, 0) * hop + win, c + nbuf - 1),
+                                           ((c + nbuf) * hop - h, win, c + nbuf - 1)]:
+                    got, want = R.estimate(st, n0, length, newest), _direct_estimate(st, n0, length, newest)
+                    assert np.allclose(got, want, rtol=1e-12, atol=1e-12 * np.abs(want).max()), (la, c, nbuf, n0)
+                for n0, length, last in [(c * hop - h, hop, c), (c * hop - h, max(0, h - hop), c - 1)]:
+                    want, carry = _direct_release(st, n0, length, last, 0.97)
+                    s2 = st.copy()
+                    out = []
+                    R._release(s2, n0, length, last, 0.97, out)
+                    assert len(out) == len(want) and np.allclose(out, want, rtol=1e-12, atol=1e-12), (la, c, nbuf, n0)
+                    assert s2.carry == carry or abs(s2.carry - carry) <= 1e-12 * abs(carry), (s2.carry, carry)
+
+
+def test_rtisi_refuses_past_int32_frames():
+    """avc_rtisi_la's frame counts are int32: an update that would take a stream past 2^31 - 1 frames is refused before
+    any count moves (no device is touched: the check precedes the launch's tables)."""
+    rt = S.Rtisi.__new__(S.Rtisi)
+    rt.hp, rt.la, rt.host = None, 3, {"a": [S.RTISI_MAX_FRAMES - 5, 3]}
+    with pytest.raises(ValueError, match="RTISI-LA limit"):
+        rt.prepare({"a": np.zeros((3, 1025), np.float32)})
+    assert rt.host["a"] == [S.RTISI_MAX_FRAMES - 5, 3]
