@@ -168,6 +168,12 @@ class RtisiDesc(C.Structure):
                 ("state", _fp), ("count", _fp)]
 
 
+class PghiStreamDesc(C.Structure):
+    _fields_ = [("n_fft", C.c_int32), ("hop", C.c_int32), ("win", C.c_int32), ("n_streams", C.c_int32),
+                ("mag", _fp), ("mag_off", _fp), ("slot", _fp), ("close", _fp), ("out_off", _fp), ("mag_out", _fp),
+                ("X", _fp), ("state", _fp)]
+
+
 class MelDesc(C.Structure):
     _fields_ = [("rows", C.c_int32), ("n_mels", C.c_int32), ("n_bins", C.c_int32), ("dir", C.c_int32),
                 ("max_db", C.c_float), ("ref_db", C.c_float), ("in_", _fp), ("mat", _fp), ("out", _fp)]
@@ -333,6 +339,9 @@ PROTOTYPES = {
     "avc_pghi": (_i, [C.POINTER(AudioDesc), C.c_float, _p, _p]),
     "avc_rtisi_state_floats": (_i64, [_i, _i]),
     "avc_rtisi_la": (_i, [C.POINTER(RtisiDesc), _p]),
+    "avc_rtisi_la_from": (_i, [C.POINTER(RtisiDesc), _p, _p]),
+    "avc_pghi_stream_state_floats": (_i64, [_i]),
+    "avc_pghi_stream": (_i, [C.POINTER(PghiStreamDesc), C.c_float, _p, _p]),
     "avc_frame_power": (_i, [C.POINTER(AudioDesc), _p, _p]),
     "avc_deemphasis": (_i, [C.POINTER(AudioDesc), C.c_float, _p]),
     "avc_yin": (_i, [C.POINTER(AudioDesc), C.c_int32, C.c_int32, C.c_int32, C.c_float, _p, _p, _p, _p]),

@@ -4,7 +4,9 @@
 // utterance the bits it gets alone.
 #include <float.h>
 
+#include <climits>
 #include <cmath>
+#include <type_traits>
 
 #include "common.cuh"
 
@@ -480,28 +482,77 @@ __device__ __forceinline__ double diff_bins(const double* l, int k) {
   return k == 0 ? l[1] - l[0] : k == NC ? l[NC] - l[NC - 1] : 0.5 * (l[k + 1] - l[k - 1]);
 }
 
-__global__ void __launch_bounds__(PG_THREADS) pghi_kernel(avc_audio_desc d, float tol, int8_t* parent) {
+// The streaming instance (avc_pghi_stream) runs one stream per CTA, its frames in order across launches.  Frame f is
+// integrated once frame f+1 has arrived, or at close, at the threshold tol s_max(f), s_max(f) the largest magnitude of
+// frames 0 .. f+1 (0 .. f for the last): the three ln-magnitude rows a frame reads are taken again at its threshold, so
+// its bits depend only on the stream's magnitudes, not on how they were split into launches.  The state slot holds
+// the magnitudes of the last two frames received (slot frame % 2), the phases of the last frame integrated (float64),
+// s_max and the count of frames received.  The CTA's entry is an utterance-table entry: frame_off places the first
+// frame the launch completes, f_lo, at the stream's out_off row, and n_frames is the stream's length at close (INT_MAX
+// before: no frame the launch completes is the last).
+constexpr int PS_PHI = 2 * NBIN;                // float offset of the phases (even: 8-byte aligned)
+constexpr int PS_SMAX = PS_PHI + 2 * NBIN;
+constexpr int PS_COUNT = PS_SMAX + 1;
+constexpr int PS_FLOATS = (PS_COUNT + 1 + 3) / 4 * 4;
+
+__device__ __forceinline__ int32_t ps_count(const avc_pghi_stream_desc& d) {
+  return *reinterpret_cast<const int32_t*>(d.state + (int64_t)d.slot[blockIdx.x] * PS_FLOATS + PS_COUNT);
+}
+// frames f_lo .. f_hi - 1 that a launch completes, of a stream that had n0 frames and has n1
+__device__ __forceinline__ int ps_lo(int n0) { return max(0, n0 - 1); }
+__device__ __forceinline__ int ps_hi(int n1, bool close) { return close ? n1 : max(0, n1 - 1); }
+
+__device__ __forceinline__ avc_audio_seg pghi_entry(const avc_audio_desc& d) { return d.segs[blockIdx.x]; }
+__device__ __forceinline__ avc_audio_seg pghi_entry(const avc_pghi_stream_desc& d) {
+  const int s = blockIdx.x, n0 = ps_count(d), n1 = n0 + (d.mag_off[s + 1] - d.mag_off[s]);
+  avc_audio_seg g = {};
+  g.frame_off = d.out_off[s] - ps_lo(n0);
+  g.n_frames = d.close[s] ? n1 : INT_MAX;
+  return g;
+}
+
+// The streaming instance may use more than 128 registers (at least one CTA per SM); the offline one keeps its bounds.
+template <class Desc>
+__global__ void __launch_bounds__(PG_THREADS, (std::is_same<Desc, avc_pghi_stream_desc>::value ? 1 : 0))
+    pghi_kernel(Desc d, float tol, int8_t* parent) {
+  constexpr bool STREAM = std::is_same<Desc, avc_pghi_stream_desc>::value;
   __shared__ double lrow[3][NBIN];  // ln max(s, tol s_max) of frames f-1, f, f+1 (slot = frame % 3)
   __shared__ float srow[3][NBIN];
   __shared__ Pair sh[PG_WARPS];
   __shared__ float red[PG_WARPS];
-  const avc_audio_seg g = d.segs[blockIdx.x];
+  const avc_audio_seg g = pghi_entry(d);
   const int nF = g.n_frames, t = threadIdx.x, k0 = t * PG_PER;
   if (nF <= 0) return;
   const float* mag = d.mag + (int64_t)g.frame_off * NBIN;
   float2* X = reinterpret_cast<float2*>(d.X) + (int64_t)g.frame_off * NBIN;
   int8_t* par = parent ? parent + (int64_t)g.frame_off * NBIN : nullptr;
 
-  // s_max of the utterance (fmaxf is exact, so the order does not matter)
+  // streaming: the stream's state, its frames n0 .. n1 - 1 arriving, frames f_lo .. f_hi - 1 completed
+  float* st = nullptr;
+  int n0 = 0, n1 = 0, f_lo = 0, f_hi = nF, r0 = 0;
+  if constexpr (STREAM) {
+    st = d.state + (int64_t)d.slot[blockIdx.x] * PS_FLOATS;
+    r0 = d.mag_off[blockIdx.x];
+    n0 = ps_count(d);
+    n1 = n0 + (d.mag_off[blockIdx.x + 1] - r0);
+    f_lo = ps_lo(n0);
+    f_hi = ps_hi(n1, d.close[blockIdx.x] != 0);
+  }
+
+  // s_max of the utterance (fmaxf is exact, so the order does not matter); streaming: of the frames so far
   float m = 0.f;
-  for (int64_t i = t; i < (int64_t)nF * NBIN; i += PG_THREADS) m = fmaxf(m, __ldg(mag + i));
+  if constexpr (STREAM) {
+    m = st[PS_SMAX];
+  } else {
+    for (int64_t i = t; i < (int64_t)nF * NBIN; i += PG_THREADS) m = fmaxf(m, __ldg(mag + i));
 #pragma unroll
-  for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
-  if ((t & 31) == 0) red[t >> 5] = m;
-  __syncthreads();
-  m = red[0];
-  for (int w = 1; w < PG_WARPS; ++w) m = fmaxf(m, red[w]);
-  const double thr = (double)tol * (double)m;
+    for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+    if ((t & 31) == 0) red[t >> 5] = m;
+    __syncthreads();
+    m = red[0];
+    for (int w = 1; w < PG_WARPS; ++w) m = fmaxf(m, red[w]);
+  }
+  double thr = (double)tol * (double)m;
   const double lambda = 0.25645 * (double)d.win * (double)d.win;
   const double a_t = (double)d.hop * (double)NFFT / lambda, b_t = (double)d.hop * 2.0 * M_PI / (double)NFFT;
   const double a_f = -lambda / ((double)NFFT * (double)d.hop);
@@ -525,18 +576,59 @@ __global__ void __launch_bounds__(PG_THREADS) pghi_kernel(avc_audio_desc d, floa
       }
     }
   };
-  fetch(0);
-  store(0);
-  fetch(1);
-  store(1);
-  fetch(2);
+  // streaming: frames up to `last` (< n1) into srow, s_max updated with the new ones
+  int got = n0;
+  auto receive = [&](int last) {
+    if constexpr (STREAM) {
+      for (; got <= last; ++got) {
+        float mx = 0.f;
+        for (int k = t; k < NBIN; k += PG_THREADS) {
+          const float v = __ldg(d.mag + (int64_t)(r0 + got - n0) * NBIN + k);
+          srow[got % 3][k] = v;
+          mx = fmaxf(mx, v);
+        }
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+        if ((t & 31) == 0) red[t >> 5] = mx;
+        __syncthreads();
+        for (int w = 0; w < PG_WARPS; ++w) m = fmaxf(m, red[w]);
+        __syncthreads();
+      }
+    }
+  };
+  if constexpr (STREAM) {
+    for (int k = t; k < NBIN; k += PG_THREADS) {
+      if (n0 >= 1) srow[(n0 - 1) % 3][k] = st[((n0 - 1) & 1) * NBIN + k];
+      if (n0 >= 2) srow[(n0 - 2) % 3][k] = st[((n0 - 2) & 1) * NBIN + k];
+    }
+  } else {
+    fetch(0);
+    store(0);
+    fetch(1);
+    store(1);
+    fetch(2);
+  }
   __syncthreads();
 
   double phi_prev[PG_PER];
 #pragma unroll
   for (int j = 0; j < PG_PER; ++j) phi_prev[j] = 0.0;
+  if constexpr (STREAM) {
+    const double* st_phi = reinterpret_cast<const double*>(st + PS_PHI);
+#pragma unroll
+    for (int j = 0; j < PG_PER; ++j) phi_prev[j] = k0 + j < NBIN ? st_phi[k0 + j] : 0.0;
+  }
 
-  for (int f = 0; f < nF; ++f) {
+  for (int f = f_lo; f < f_hi; ++f) {
+    if constexpr (STREAM) {  // frame f+1 in, then rows f-1 .. f+1 in ln at this frame's threshold
+      receive(min(f + 1, n1 - 1));
+      thr = (double)tol * (double)m;
+      for (int k = t; k < NBIN; k += PG_THREADS) {
+        for (int i = max(f - 1, 0); i <= min(f + 1, n1 - 1); ++i) lrow[i % 3][k] = log(fmax((double)srow[i % 3][k], thr));
+        d.mag_out[((int64_t)g.frame_off + f) * NBIN + k] = srow[f % 3][k];
+      }
+      __syncthreads();
+    }
     const double* lm = lrow[(f + 2) % 3];
     const double* l0 = lrow[f % 3];
     const double* lp = lrow[(f + 1) % 3];
@@ -682,9 +774,26 @@ __global__ void __launch_bounds__(PG_THREADS) pghi_kernel(avc_audio_desc d, floa
       }
     }
     // frame f-1's slot takes frame f+2 (every read of it this frame is behind the scans' barriers)
-    store(f + 2);
-    fetch(f + 3);
+    if constexpr (!STREAM) {
+      store(f + 2);
+      fetch(f + 3);
+    }
     __syncthreads();
+  }
+  if constexpr (STREAM) {  // the frames that complete none, then the state
+    receive(n1 - 1);
+    for (int k = t; k < NBIN; k += PG_THREADS) {
+      if (n1 >= 1) st[((n1 - 1) & 1) * NBIN + k] = srow[(n1 - 1) % 3][k];
+      if (n1 >= 2) st[((n1 - 2) & 1) * NBIN + k] = srow[(n1 - 2) % 3][k];
+    }
+    double* st_phi = reinterpret_cast<double*>(st + PS_PHI);
+#pragma unroll
+    for (int j = 0; j < PG_PER; ++j)
+      if (k0 + j < NBIN) st_phi[k0 + j] = phi_prev[j];
+    if (t == 0) {
+      st[PS_SMAX] = m;
+      *reinterpret_cast<int32_t*>(st + PS_COUNT) = n1;
+    }
   }
 }
 
@@ -735,36 +844,46 @@ __device__ void rt_estimate(float* est, int r0, int len, const float* num, const
 
 // One frame's projection in the 128 threads of group z: STFT of the windowed estimate e[0 .. win), the magnitudes mag
 // with the estimate's phase (phase 0 where |E| = 0), iSTFT times the window into out.  Every thread of the CTA calls it.
+// FROM: the spectrum is Xr (n_fft/2 + 1 complex bins) as given, with no STFT (e and mag are not read).
+template <bool FROM = false>
 __device__ void rt_project(float2* z, float2* nyq, const float2* tab, int t, const float* e, const float* mag, float* out,
-                           bool live, int win) {
+                           bool live, int win, const float2* Xr = nullptr) {
   const int off = (NFFT - win) / 2;
-  for (int n = t; n < NC; n += TPF) {
-    float v[2] = {0.f, 0.f};
-#pragma unroll
-    for (int k = 0; k < 2; ++k) {
-      const int q = 2 * n + k - off;
-      if (live && q >= 0 && q < win) v[k] = hann(q, win) * e[q];
-    }
-    z[n] = make_float2(v[0], v[1]);
-  }
-  __syncthreads();
-  fft1024(z, tab, t);
   constexpr int PER = NC / TPF + 1;  // bins per thread, the Nyquist bin with thread 0
   float2 X[PER];
+  if constexpr (FROM) {
 #pragma unroll
-  for (int i = 0; i < PER; ++i) {
-    const int k = t + i * TPF;
-    X[i] = make_float2(0.f, 0.f);
-    if (k <= NC) {
-      const float2 zk = z[k & (NC - 1)], zr = z[(NC - k) & (NC - 1)];
-      const float2 xe = make_float2(0.5f * (zk.x + zr.x), 0.5f * (zk.y - zr.y));
-      const float2 xo = make_float2(0.5f * (zk.y + zr.y), -0.5f * (zk.x - zr.x));
-      const float2 w = k < NC ? tab[k] : make_float2(-1.f, 0.f);
-      const float2 wx = cmul(w, xo);
-      const float2 E = make_float2(xe.x + wx.x, xe.y + wx.y);
-      const float a = sqrtf(E.x * E.x + E.y * E.y);
-      const float m = live ? mag[k] : 0.f;
-      X[i] = a > 0.f ? make_float2(m * (E.x / a), m * (E.y / a)) : make_float2(m, 0.f);
+    for (int i = 0; i < PER; ++i) {
+      const int k = t + i * TPF;
+      X[i] = live && k <= NC ? Xr[k] : make_float2(0.f, 0.f);
+    }
+  } else {
+    for (int n = t; n < NC; n += TPF) {
+      float v[2] = {0.f, 0.f};
+#pragma unroll
+      for (int k = 0; k < 2; ++k) {
+        const int q = 2 * n + k - off;
+        if (live && q >= 0 && q < win) v[k] = hann(q, win) * e[q];
+      }
+      z[n] = make_float2(v[0], v[1]);
+    }
+    __syncthreads();
+    fft1024(z, tab, t);
+#pragma unroll
+    for (int i = 0; i < PER; ++i) {
+      const int k = t + i * TPF;
+      X[i] = make_float2(0.f, 0.f);
+      if (k <= NC) {
+        const float2 zk = z[k & (NC - 1)], zr = z[(NC - k) & (NC - 1)];
+        const float2 xe = make_float2(0.5f * (zk.x + zr.x), 0.5f * (zk.y - zr.y));
+        const float2 xo = make_float2(0.5f * (zk.y + zr.y), -0.5f * (zk.x - zr.x));
+        const float2 w = k < NC ? tab[k] : make_float2(-1.f, 0.f);
+        const float2 wx = cmul(w, xo);
+        const float2 E = make_float2(xe.x + wx.x, xe.y + wx.y);
+        const float a = sqrtf(E.x * E.x + E.y * E.y);
+        const float m = live ? mag[k] : 0.f;
+        X[i] = a > 0.f ? make_float2(m * (E.x / a), m * (E.y / a)) : make_float2(m, 0.f);
+      }
     }
   }
   __syncthreads();
@@ -801,7 +920,10 @@ __device__ void rt_project(float2* z, float2* nyq, const float2* tab, int t, con
   }
 }
 
-__global__ void __launch_bounds__((RT_MAX_LA + 1) * TPF) rtisi_kernel(avc_rtisi_desc d, RtSmem L) {
+// FROM (avc_rtisi_la_from): an entering row r starts from the caller's spectrum X row r (n_fft/2 + 1 complex bins)
+// instead of the estimate's phase, which skips the entry STFT.
+template <bool FROM>
+__global__ void __launch_bounds__((RT_MAX_LA + 1) * TPF) rtisi_kernel(avc_rtisi_desc d, RtSmem L, const float2* X) {
   extern __shared__ float4 rt_smem[];
   const int nb = L.nb, win = L.win, hop = L.hop, h = win / 2;
   float2* tab = reinterpret_cast<float2*>(rt_smem);
@@ -886,10 +1008,15 @@ __global__ void __launch_bounds__((RT_MAX_LA + 1) * TPF) rtisi_kernel(avc_rtisi_
     const int T = c + nbuf;  // the entering frame
     float* m = st_mag + (int64_t)(T % nb) * NBIN;
     for (int k = threadIdx.x; k < NBIN; k += blockDim.x) m[k] = __ldg(d.mag + (int64_t)r * NBIN + k);
-    // start phase: the estimate of the frames 0 .. T-1 over the entering frame's support
-    rt_estimate(est, nbuf * hop - h, win, num, fr, c, nbuf, T - 1, nb, win, hop);
-    __syncthreads();
-    rt_project(zb + (size_t)g * NC, nyq + g, tab, t, est, m, fr + (size_t)(T % nb) * win, g == 0, win);
+    if (FROM) {  // start: X row r as given
+      rt_project<true>(zb + (size_t)g * NC, nyq + g, tab, t, nullptr, nullptr, fr + (size_t)(T % nb) * win, g == 0, win,
+                       X + (int64_t)r * NBIN);
+    } else {
+      // start phase: the estimate of the frames 0 .. T-1 over the entering frame's support
+      rt_estimate(est, nbuf * hop - h, win, num, fr, c, nbuf, T - 1, nb, win, hop);
+      __syncthreads();
+      rt_project(zb + (size_t)g * NC, nyq + g, tab, t, est, m, fr + (size_t)(T % nb) * win, g == 0, win);
+    }
     __syncthreads();
     ++nbuf;
     iterate();
@@ -1104,27 +1231,59 @@ extern "C" int64_t avc_rtisi_state_floats(int win, int lookahead) {
   return rt_state_floats(win, lookahead);
 }
 
-extern "C" int avc_rtisi_la(const avc_rtisi_desc* d, void* stream) {
-  AVC_REQUIRE(d != nullptr, AVC_ERR_INVALID, "avc_rtisi_la: null descriptor");
-  AVC_REQUIRE(d->n_fft == NFFT, AVC_ERR_UNSUPPORTED, "avc_rtisi_la: only n_fft = %d is supported (got %d)", NFFT, d->n_fft);
+// avc_rtisi_la's checks (who names the entry point), then the launch of its FROM or estimate instance
+static int rtisi_launch(const avc_rtisi_desc* d, const float2* X, const char* who, cudaStream_t stream) {
+  AVC_REQUIRE(d != nullptr, AVC_ERR_INVALID, "%s: null descriptor", who);
+  AVC_REQUIRE(d->n_fft == NFFT, AVC_ERR_UNSUPPORTED, "%s: only n_fft = %d is supported (got %d)", who, NFFT, d->n_fft);
   AVC_REQUIRE(d->win > 0 && d->win <= NFFT && d->win % 2 == 0, AVC_ERR_UNSUPPORTED,
-              "avc_rtisi_la: win must be even and in (0, n_fft] (got %d)", d->win);
-  AVC_REQUIRE(d->hop > 0 && 2 * d->hop <= d->win, AVC_ERR_UNSUPPORTED, "avc_rtisi_la: hop must be in (0, win/2] (got %d)",
+              "%s: win must be even and in (0, n_fft] (got %d)", who, d->win);
+  AVC_REQUIRE(d->hop > 0 && 2 * d->hop <= d->win, AVC_ERR_UNSUPPORTED, "%s: hop must be in (0, win/2] (got %d)", who,
               d->hop);
   AVC_REQUIRE(d->lookahead >= 0 && d->lookahead <= RT_MAX_LA, AVC_ERR_UNSUPPORTED,
-              "avc_rtisi_la: lookahead must be in [0, %d] (got %d)", RT_MAX_LA, d->lookahead);
-  AVC_REQUIRE(d->n_iter >= 0, AVC_ERR_INVALID, "avc_rtisi_la: n_iter < 0");
-  AVC_REQUIRE(d->n_streams >= 0, AVC_ERR_INVALID, "avc_rtisi_la: n_streams < 0");
-  AVC_REQUIRE(std::isfinite(d->deemph), AVC_ERR_INVALID, "avc_rtisi_la: de-emphasis coefficient is not finite");
+              "%s: lookahead must be in [0, %d] (got %d)", who, RT_MAX_LA, d->lookahead);
+  AVC_REQUIRE(d->n_iter >= 0, AVC_ERR_INVALID, "%s: n_iter < 0", who);
+  AVC_REQUIRE(d->n_streams >= 0, AVC_ERR_INVALID, "%s: n_streams < 0", who);
+  AVC_REQUIRE(std::isfinite(d->deemph), AVC_ERR_INVALID, "%s: de-emphasis coefficient is not finite", who);
   if (d->n_streams == 0) return AVC_OK;
   AVC_REQUIRE(d->mag && d->mag_off && d->slot && d->close && d->out_off && d->y && d->state && d->count, AVC_ERR_INVALID,
-              "avc_rtisi_la: null pointer");
+              "%s: null pointer", who);
+  const bool from = X != nullptr;
+  auto kernel = from ? rtisi_kernel<true> : rtisi_kernel<false>;
   RtSmem L{d->lookahead + 1, d->win, d->hop};
   const size_t smem = L.bytes();
-  cudaError_t e = cudaFuncSetAttribute(rtisi_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  AVC_REQUIRE(e == cudaSuccess, AVC_ERR_CUDA, "avc_rtisi_la: cudaFuncSetAttribute(%zu bytes): %s", smem,
+  cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  AVC_REQUIRE(e == cudaSuccess, AVC_ERR_CUDA, "%s: cudaFuncSetAttribute(%zu bytes): %s", who, smem,
               cudaGetErrorString(e));
-  rtisi_kernel<<<d->n_streams, L.nb * TPF, smem, (cudaStream_t)stream>>>(*d, L);
-  AVC_CHECK_LAUNCH("avc_rtisi_la");
+  kernel<<<d->n_streams, L.nb * TPF, smem, stream>>>(*d, L, X);
+  AVC_CHECK_LAUNCH(who);
+  return AVC_OK;
+}
+
+extern "C" int avc_rtisi_la(const avc_rtisi_desc* d, void* stream) {
+  return rtisi_launch(d, nullptr, "avc_rtisi_la", (cudaStream_t)stream);
+}
+
+extern "C" int avc_rtisi_la_from(const avc_rtisi_desc* d, const float* X, void* stream) {
+  AVC_REQUIRE(X != nullptr, AVC_ERR_INVALID, "avc_rtisi_la_from: null X");
+  return rtisi_launch(d, reinterpret_cast<const float2*>(X), "avc_rtisi_la_from", (cudaStream_t)stream);
+}
+
+extern "C" int64_t avc_pghi_stream_state_floats(int n_fft) { return n_fft == NFFT ? PS_FLOATS : 0; }
+
+extern "C" int avc_pghi_stream(const avc_pghi_stream_desc* d, float tol, int8_t* parent, void* stream) {
+  AVC_REQUIRE(d != nullptr, AVC_ERR_INVALID, "avc_pghi_stream: null descriptor");
+  AVC_REQUIRE(d->n_fft == NFFT, AVC_ERR_UNSUPPORTED, "avc_pghi_stream: only n_fft = %d is supported (got %d)", NFFT,
+              d->n_fft);
+  AVC_REQUIRE(d->win > 0 && d->win <= NFFT && d->win % 2 == 0, AVC_ERR_UNSUPPORTED,
+              "avc_pghi_stream: win must be even and in (0, n_fft] (got %d)", d->win);
+  AVC_REQUIRE(d->hop > 0 && 2 * d->hop <= d->win, AVC_ERR_UNSUPPORTED,
+              "avc_pghi_stream: hop must be in (0, win/2] (got %d)", d->hop);
+  AVC_REQUIRE(d->n_streams >= 0, AVC_ERR_INVALID, "avc_pghi_stream: n_streams < 0");
+  if (int rc = check_tol(tol, "avc_pghi_stream")) return rc;
+  if (d->n_streams == 0) return AVC_OK;
+  AVC_REQUIRE(d->mag && d->mag_off && d->slot && d->close && d->out_off && d->mag_out && d->X && d->state,
+              AVC_ERR_INVALID, "avc_pghi_stream: null pointer");
+  pghi_kernel<<<d->n_streams, PG_THREADS, 0, (cudaStream_t)stream>>>(*d, tol, parent);
+  AVC_CHECK_LAUNCH("avc_pghi_stream");
   return AVC_OK;
 }

@@ -12,7 +12,8 @@ Three stages run once per update, each batched over every stream with pending in
   first X = min(LA, H) frames are blended linearly with the previous window's look-ahead rows.  Windows of one length
   run as one batch (a CUDA graph per batch bucket and length), which gives each its stand-alone bits.
 * synthesis: the blocks' magnitudes go through RTISI-LA (``avc_rtisi_la``), one CTA per stream, which releases
-  samples on ``mel_to_signal``'s grid as their frames are committed.
+  samples on ``mel_to_signal``'s grid as their frames are committed.  With ``StreamParams(gl_init="pghi")`` each frame
+  enters from a streamed PGHI phase (``avc_pghi_stream``, then ``avc_rtisi_la_from``), a frame later.
 * pitch (``PitchStage``, per stream, optional): a fixed shift passes each block's magnitudes through
   ``avc_pitch_shift`` before RTISI-LA.  A target profile (mode, mu_t, sigma_t) synthesises the unshifted magnitudes in
   a second RTISI-LA pool (the shadow), tracks every shadow frame whose span has been released with
@@ -55,6 +56,8 @@ class StreamParams:
     lookahead: int = 8
     gl_lookahead: int = 3
     gl_iters: int = 8
+    gl_init: str = "estimate"  # RTISI-LA's start phase of each entering frame: "estimate" (the current estimate's) or
+                               # "pghi" (streamed PGHI, Rtisi; one more frame of latency)
     batch_max: int = 1024     # windows per model batch
     keep_mels: bool = False   # keep each stream's emitted mel frames for take_mels, and its pitch diagnostics for
                               # take_pitch (memory grows with the stream)
@@ -73,6 +76,8 @@ def check_params(p: StreamParams, window: int):
         raise ValueError(f"StreamParams.gl_lookahead must be in [0, {L.RTISI_MAX_LOOKAHEAD}] (got {p.gl_lookahead})")
     if p.gl_iters < 0:
         raise ValueError(f"StreamParams.gl_iters must be >= 0 (got {p.gl_iters})")
+    if p.gl_init not in RTISI_INITS:
+        raise ValueError(f"StreamParams.gl_init must be one of {RTISI_INITS} (got {p.gl_init!r})")
     if p.batch_max < 1:
         raise ValueError("StreamParams.batch_max must be >= 1")
     if p.pitch_warmup < 1:
@@ -106,12 +111,17 @@ def blend_weights(hop: int, lookahead: int) -> np.ndarray:
     return (np.arange(1, X + 1, dtype=np.float32) / np.float32(X + 1)).astype(np.float32)
 
 
+def init_delay(p: StreamParams) -> int:
+    """Frames a frame waits before it enters RTISI-LA: 1 with the PGHI start (frame f's phase needs frame f+1), else 0."""
+    return 1 if p.gl_init == "pghi" else 0
+
+
 def release_sample(n: int, p: StreamParams, win: int, hop_s: int, m: int) -> int:
     """Index of the input sample whose arrival releases output sample n (before close): n's last covering frame c is
-    committed when frame c + gl_lookahead enters RTISI-LA, i.e. when its block j is emitted, at the arrival of the
-    sample that completes frame e_j - 1."""
+    committed when frame c + gl_lookahead enters RTISI-LA, i.e. (with init_delay) when frame c + gl_lookahead +
+    init_delay is emitted in its block j, at the arrival of the sample that completes frame e_j - 1."""
     c = (n + win // 2) // hop_s
-    j = (c + p.gl_lookahead) // p.hop
+    j = (c + p.gl_lookahead + init_delay(p)) // p.hop
     return (block_end(j, p.hop, p.lookahead, m) - 1) * hop_s + win // 2 - 1
 
 
@@ -130,7 +140,7 @@ def latency_samples(p: StreamParams, win: int, hop_s: int, m: int) -> int:
     frame of is the worst; past the start-up windows the schedule repeats every block, so a few blocks beyond m
     cover every case.  Without start-up effects this is (H + LA + LA_v - 1) hop + win - 1."""
     return _worst_latency(lambda n: release_sample(n, p, win, hop_s, m),
-                          m + 4 * p.hop + p.gl_lookahead + 2 * (win // hop_s) + 8, win, hop_s)
+                          m + 4 * p.hop + p.gl_lookahead + init_delay(p) + 2 * (win // hop_s) + 8, win, hop_s)
 
 
 def yin_last_sample(t: int, hop_s: int, span: int) -> int:
@@ -150,9 +160,11 @@ def yin_ready(n: int, hop_s: int, span: int) -> int:
 
 def tracked_release_sample(n: int, p: StreamParams, win: int, hop_s: int, m: int, span: int) -> int:
     """release_sample for a stream with a target profile: n's last covering frame c is committed by the output RTISI-LA
-    when frame t = c + gl_lookahead enters it, i.e. when YIN frame t has been tracked, i.e. when the shadow has released
-    sample yin_last_sample(t); the shadow is synthesised on the output's schedule, so that is its release_sample."""
-    return release_sample(yin_last_sample((n + win // 2) // hop_s + p.gl_lookahead, hop_s, span), p, win, hop_s, m)
+    when frame c + gl_lookahead enters it, which needs frame t = c + gl_lookahead + init_delay shifted, i.e. YIN frame t
+    tracked, i.e. the shadow's release of sample yin_last_sample(t); the shadow is synthesised on the output's schedule
+    and start, so that is its release_sample."""
+    t = (n + win // 2) // hop_s + p.gl_lookahead + init_delay(p)
+    return release_sample(yin_last_sample(t, hop_s, span), p, win, hop_s, m)
 
 
 def tracked_latency_samples(p: StreamParams, win: int, hop_s: int, m: int, span: int) -> int:
@@ -160,7 +172,8 @@ def tracked_latency_samples(p: StreamParams, win: int, hop_s: int, m: int, span:
     the defaults the tracking delays each frame by D = gl_lookahead + ceil((span - floor(span / 2) + win / 2) / hop) - 1
     frames (7 at 24 kHz: 3 + 5 - 1)."""
     return _worst_latency(lambda n: tracked_release_sample(n, p, win, hop_s, m, span),
-                          m + 4 * p.hop + 2 * p.gl_lookahead + 2 * (win // hop_s) + span // hop_s + 8, win, hop_s)
+                          m + 4 * p.hop + 2 * (p.gl_lookahead + init_delay(p)) + 2 * (win // hop_s) + span // hop_s + 8,
+                          win, hop_s)
 
 
 class _Tail:
@@ -262,17 +275,32 @@ class StreamAnalyzer:
 RTISI_MAX_FRAMES = 2 ** 31 - 1   # frames of one stream (int32 counts): about 310 days at hop 300 and 24 kHz
 
 
+RTISI_INITS = ("estimate", "pghi")
+
+
 class Rtisi:
     """RTISI-LA state of many streams in a pool of slots, and one avc_rtisi_la launch per update.
-    ``run({id: mags [n, n_bins]}, close=())`` returns {id: released samples}."""
+    ``run({id: mags [n, n_bins]}, close=())`` returns {id: released samples}.
 
-    def __init__(self, hp, lookahead: int = 3, n_iter: int = 8, device=None):
-        self.hp, self.la, self.n_iter = hp, int(lookahead), int(n_iter)
+    ``init`` is the start phase of each entering frame: "estimate" (the phase of the current estimate's STFT) or
+    "pghi", the stream's own streamed PGHI phase (``avc_pghi_stream``, tolerance ``hp.pghi_tol``), which holds each
+    frame until the next one has arrived (or the stream closes): an update is then one avc_pghi_stream launch and one
+    avc_rtisi_la_from launch on the same tables, and the PGHI state pool sits beside the slot pool."""
+    init = "estimate"
+
+    def __init__(self, hp, lookahead: int = 3, n_iter: int = 8, device=None, init: str = "estimate"):
+        if init not in RTISI_INITS:
+            raise ValueError(f"Rtisi: init must be one of {RTISI_INITS} (got {init!r})")
+        self.hp, self.la, self.n_iter, self.init = hp, int(lookahead), int(n_iter), init
         self.dev = torch.device(device) if device is not None else torch.device("cuda")
         self.stride = int(L.load().avc_rtisi_state_floats(hp.win_length, self.la))
         self.state = torch.zeros(0, self.stride, device=self.dev)
         self.count = torch.zeros(0, 2, dtype=torch.int32, device=self.dev)
-        self.free, self.slot, self.host = [], {}, {}
+        self.pstate = None
+        if init == "pghi":
+            self.pstride = int(L.load().avc_pghi_stream_state_floats(hp.n_fft))
+            self.pstate = torch.zeros(0, self.pstride, device=self.dev)
+        self.free, self.slot, self.host, self.held = [], {}, {}, {}
 
     def open(self, sid):
         if not self.free:
@@ -283,16 +311,24 @@ class Rtisi:
             state[:old].copy_(self.state)
             count[:old].copy_(self.count)
             self.state, self.count = state, count
+            if self.pstate is not None:
+                pstate = torch.zeros(n, self.pstride, device=self.dev)
+                pstate[:old].copy_(self.pstate)
+                self.pstate = pstate
             self.free = list(range(n - 1, old - 1, -1))
         k = self.free.pop()
         self.state[k].zero_()
         self.count[k].zero_()
+        if self.pstate is not None:
+            self.pstate[k].zero_()
+            self.held[sid] = 0
         self.slot[sid], self.host[sid] = k, [0, 0]
 
     def drop(self, sid):
         if sid in self.slot:
             self.free.append(self.slot.pop(sid))
             self.host.pop(sid)
+            self.held.pop(sid, None)
 
     def released(self, c: int) -> int:
         return max(0, c * self.hp.hop_length - self.hp.win_length // 2)
@@ -308,27 +344,43 @@ class Rtisi:
         return res
 
     def launch(self, desc):
-        """The avc_rtisi_la launch of a prepared update (its tables and buffers are kept alive by prepare's result)."""
-        L.check(L.load().avc_rtisi_la(C.byref(desc), _stream(self.dev)), "avc_rtisi_la")
+        """The launches of a prepared update (its tables and buffers are kept alive by prepare's result): avc_rtisi_la,
+        or with init "pghi" avc_pghi_stream then avc_rtisi_la_from."""
+        lib, st = L.load(), _stream(self.dev)
+        if self.init == "pghi":
+            pd, rd = desc
+            L.check(lib.avc_pghi_stream(C.byref(pd), C.c_float(self.hp.pghi_tol), None, st), "avc_pghi_stream")
+            L.check(lib.avc_rtisi_la_from(C.byref(rd), pd.X, st), "avc_rtisi_la_from")
+        else:
+            L.check(lib.avc_rtisi_la(C.byref(desc), st), "avc_rtisi_la")
 
     def prepare(self, mags, close=()):
-        """(descriptor, {id: output view}, buffers) of one update, the host's counts advanced; None when empty."""
-        hp = self.hp
+        """(descriptor, {id: output view}, buffers) of one update, the host's counts advanced; None when empty.  With
+        init "pghi" the descriptor is the pair (avc_pghi_stream's, avc_rtisi_la_from's), and the frames entering
+        RTISI-LA are the ones PGHI completes: each but the newest, all of them at close."""
+        hp, pghi = self.hp, self.init == "pghi"
         ids = list(dict.fromkeys(list(mags) + list(close)))
         if not ids:
             return None
         for sid in ids:   # avc_rtisi_la's frame counts are int32: refuse before any state changes
             c, nb = self.host[sid]
             m = mags.get(sid)
-            if c + nb + (0 if m is None else int(m.shape[0])) > RTISI_MAX_FRAMES:
+            # (avc_pghi_stream forms frame f + 2 for its last frame f: one frame fewer)
+            if c + nb + (self.held[sid] if pghi else 0) + (0 if m is None else int(m.shape[0])) > RTISI_MAX_FRAMES - pghi:
                 raise ValueError(f"stream {sid!r} would pass {RTISI_MAX_FRAMES} frames, the RTISI-LA limit")
-        rows, offs, slots, closes, outs, counts = [], [0], [], [], [0], []
+        rows, offs, slots, closes, outs, counts, ents = [], [0], [], [], [0], [], [0]
         for sid in ids:
             c, nb = self.host[sid]
             m = mags.get(sid)
             p = 0 if m is None else int(m.shape[0])
             if m is not None and p:
                 rows.append(m)
+            offs.append(offs[-1] + p)
+            if pghi:   # the newest frame waits for the next one, or for close
+                h = self.held[sid] + p
+                self.held[sid] = 0 if sid in close else min(h, 1)
+                p = h - self.held[sid]
+                ents.append(ents[-1] + p)
             if sid in close:
                 T = c + nb + p
                 n_out = max(0, (T - 1) * hp.hop_length) - self.released(c)
@@ -338,21 +390,31 @@ class Rtisi:
                 c2 = c + nb + p - nb2
                 n_out = self.released(c2) - self.released(c)
                 self.host[sid] = [c2, nb2]
-            offs.append(offs[-1] + p)
             slots.append(self.slot[sid])
             closes.append(1 if sid in close else 0)
             counts.append(n_out)
             outs.append(outs[-1] + n_out)
         mag = torch.cat(rows).float().contiguous() if rows else torch.zeros(1, hp.n_bins, device=self.dev)
         n = len(ids)
-        i32 = torch.tensor(offs + slots + closes, dtype=torch.int32).to(self.dev)
+        i32 = torch.tensor(offs + slots + closes + (ents if pghi else []), dtype=torch.int32).to(self.dev)
         out_off = torch.tensor(outs[:-1], dtype=torch.int64).to(self.dev)
         y = torch.empty(max(1, outs[-1]), device=self.dev)
+        keep = (mag, i32, out_off, y)
+        rmag, roff = mag, i32[:n + 1]
+        if pghi:
+            rmag = torch.empty(max(1, ents[-1]), hp.n_bins, device=self.dev)
+            X = torch.empty(max(1, ents[-1]), hp.n_bins, 2, device=self.dev)
+            roff = i32[3 * n + 1:]
+            pd = L.PghiStreamDesc(n_fft=hp.n_fft, hop=hp.hop_length, win=hp.win_length, n_streams=n, mag=_ptr(mag),
+                                  mag_off=_ptr(i32[:n + 1]), slot=_ptr(i32[n + 1:2 * n + 1]),
+                                  close=_ptr(i32[2 * n + 1:3 * n + 1]), out_off=_ptr(roff), mag_out=_ptr(rmag),
+                                  X=_ptr(X), state=_ptr(self.pstate))
+            keep += (rmag, X)
         d = L.RtisiDesc(n_fft=hp.n_fft, hop=hp.hop_length, win=hp.win_length, lookahead=self.la, n_iter=self.n_iter,
-                        n_streams=n, deemph=hp.preemphasis, mag=_ptr(mag), mag_off=_ptr(i32[:n + 1]),
-                        slot=_ptr(i32[n + 1:2 * n + 1]), close=_ptr(i32[2 * n + 1:]), out_off=_ptr(out_off),
+                        n_streams=n, deemph=hp.preemphasis, mag=_ptr(rmag), mag_off=_ptr(roff),
+                        slot=_ptr(i32[n + 1:2 * n + 1]), close=_ptr(i32[2 * n + 1:3 * n + 1]), out_off=_ptr(out_off),
                         y=_ptr(y), state=_ptr(self.state), count=_ptr(self.count))
-        return d, dict(zip(ids, torch.split(y[:outs[-1]], counts))), (mag, i32, out_off, y)
+        return (pd, d) if pghi else d, dict(zip(ids, torch.split(y[:outs[-1]], counts))), keep
 
 
 # ------------------------------------------------------------------ pitch
@@ -647,10 +709,11 @@ class PitchStage:
     ``keep`` keeps each tracked stream's per-frame diagnostics and shadow samples for ``take``."""
 
     def __init__(self, hp, lookahead: int = 3, n_iter: int = 8, device=None, warmup: int = 50, keep: bool = False,
-                 params: F0Params = F0Params()):
+                 params: F0Params = F0Params(), init: str = "estimate"):
         self.hp, self.params, self.warmup, self.keep = hp, params, int(warmup), keep
-        self.rt = Rtisi(hp, lookahead, n_iter, device)
-        self.shadow = Rtisi(hp, lookahead, n_iter, device)
+        # the shadow starts its frames as the output does, so that it is the unshifted stream bit for bit
+        self.rt = Rtisi(hp, lookahead, n_iter, device, init)
+        self.shadow = Rtisi(hp, lookahead, n_iter, device, init)
         self.dev = self.rt.dev
         self.span = int(params.win) + params.tau_max(hp.sr)
         self.streams, self.closed = {}, {}
@@ -835,7 +898,7 @@ class StreamingConverter:
         self.c_out = int(cfg["SpeakerEncoder"]["c_out"])
         self.ana = StreamAnalyzer(vocoder)
         self.stage = PitchStage(self.hp, params.gl_lookahead, params.gl_iters, self.dev, params.pitch_warmup,
-                                params.keep_mels)
+                                params.keep_mels, init=params.gl_init)
         self.rt = self.stage.rt
         w = blend_weights(params.hop, params.lookahead)
         self.w_new = torch.from_numpy(w).to(self.dev)[:, None]

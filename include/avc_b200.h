@@ -669,6 +669,43 @@ typedef struct avc_rtisi_desc {
 } avc_rtisi_desc;
 int64_t avc_rtisi_state_floats(int win, int lookahead);
 int avc_rtisi_la(const avc_rtisi_desc* d, void* stream);
+/* avc_rtisi_la with each entering row r started from X row r ([rows][n_fft/2+1] complex, the rows of d->mag) instead
+ * of the phase of the current estimate: its windowed inverse frame is window x irfft(X row r) (imaginary parts of the
+ * DC and Nyquist bins ignored), and the entry's STFT is skipped.  The iterations, commits, release and de-emphasis are
+ * avc_rtisi_la's, and so are the state slot, counts, checks and length limits; AVC_ERR_INVALID also for a null X.
+ * The start is an argument rather than a field of avc_rtisi_desc for the reason avc_griffin_lim_from gives. */
+int avc_rtisi_la_from(const avc_rtisi_desc* d, const float* X, void* stream);
+/* Streamed PGHI start spectra for avc_rtisi_la_from (RTPGHI with one frame of delay, Prusa & Holighaus 2017): one CTA
+ * per stream, the stream's frames in order across launches.  Frame f is avc_pghi's frame step with threshold
+ * tol s_max(f), s_max(f) the largest magnitude of frames 0 .. min(f+1, T-1), used for l of frames f-1, f and f+1 and for
+ * the significance of frames f-1 and f; it runs once frame f+1 has arrived, or at close for the last frame (one-sided
+ * difference over frames, as offline).  phi(f-1) is the stream's own PGHI phase.  When a stream's largest magnitude
+ * lies in frame 0 or 1, every frame gets avc_pghi's phases and parents for the whole stream.
+ * Table layout as avc_rtisi_la: stream s's new rows are mag rows mag_off[s] .. mag_off[s+1]-1, in slot slot[s], closed
+ * after them when close[s] is non-zero.  Each frame completed in the launch is written, in frame order, to rows
+ * out_off[s] .. out_off[s+1]-1 of mag_out (its magnitudes), X (mag e^{i phi}) and parent (nullable, AVC_PGHI_* as
+ * avc_pghi); out_off[s+1] - out_off[s] must be that count: (frames received after the launch, less 1 unless closed)
+ * less (frames received before, less 1), at least 0.  A zeroed slot starts a stream; the slot holds the magnitudes of
+ * the last two frames, phi of the last frame completed (float64), s_max and the frame count.  No atomics and fixed
+ * scan orders: a stream's bits depend neither on the other streams nor on how its frames were split into launches.  A
+ * slot must appear once per launch.  AVC_ERR_UNSUPPORTED for n_fft != 2048, an odd win or win > n_fft, or hop outside
+ * (0, win/2]; AVC_ERR_INVALID for tol not finite or not in (0, 1), n_streams < 0 or a null pointer; both before any
+ * launch.  Frame counts are int32: at most 2^31 - 1 frames per stream. */
+typedef struct avc_pghi_stream_desc {
+  int32_t n_fft, hop, win;
+  int32_t n_streams;         /* CTAs */
+  const float* mag;          /* [rows][n_fft/2+1] linear magnitudes of the new frames */
+  const int32_t* mag_off;    /* DEVICE [n_streams + 1] */
+  const int32_t* slot;       /* DEVICE [n_streams] */
+  const int32_t* close;      /* DEVICE [n_streams] */
+  const int32_t* out_off;    /* DEVICE [n_streams + 1]: rows of the completed frames */
+  float* mag_out;            /* [out rows][n_fft/2+1] */
+  float* X;                  /* [out rows][n_fft/2+1] complex (re, im) */
+  float* state;              /* DEVICE [slots][avc_pghi_stream_state_floats(n_fft)] */
+} avc_pghi_stream_desc;
+/* floats of one stream's avc_pghi_stream state slot; 0 for an unsupported n_fft */
+int64_t avc_pghi_stream_state_floats(int n_fft);
+int avc_pghi_stream(const avc_pghi_stream_desc* d, float tol, int8_t* parent, void* stream);
 /* power[frame] = mean of y^2 over frames of n_fft samples hop apart, reflect-padded by n_fft/2 (librosa's trim
  * statistic): segs frame_off / n_frames count these frames, 1 + n_samples / hop per utterance.  Any even n_fft. */
 int avc_frame_power(const avc_audio_desc* d, float* power, void* stream);

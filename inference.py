@@ -81,8 +81,9 @@ Streaming: -stream feeds -s to a StreamingConverter (adaptive_voice_conversion_b
 chunks (default 20 ms) and writes the untrimmed stream it gives back; the target is -t files (their pooled code) or
 -bank -speaker SPEC.  With -pairs every line is one stream, all fed in lockstep.  -stream_hop, -stream_lookahead
 (mel frames, multiples of 8; defaults 8 and 8), -stream_gl_lookahead (default 3) and -stream_gl_iters (default 8) set
-the block schedule and RTISI-LA; -morph (use -stream_morph), a -pitch_shift other than 0 (use -stream_pitch) and the
--gl_* options are refused with it:
+the block schedule and RTISI-LA, and -stream_gl_init pghi starts each RTISI-LA frame from a streamed phase-gradient
+(PGHI) estimate instead of the current estimate's phase (-stream_gl_init estimate, the default), one frame later;
+-morph (use -stream_morph), a -pitch_shift other than 0 (use -stream_pitch) and the -gl_* options are refused with it:
 
     python inference.py -c config.yaml -m model.ckpt -a attr.pkl -s src.wav -t tgt.wav -o out.wav -stream
 
@@ -465,6 +466,9 @@ def parser():
     p.add_argument("-stream_lookahead", default=8, type=int, help="-stream: look-ahead frames of a block's window")
     p.add_argument("-stream_gl_lookahead", default=3, type=int, help="-stream: RTISI-LA look-ahead frames (0 .. 7)")
     p.add_argument("-stream_gl_iters", default=8, type=int, help="-stream: RTISI-LA iterations per frame step")
+    p.add_argument("-stream_gl_init", default=None, choices=["estimate", "pghi"],
+                   help="-stream: RTISI-LA's start phase of each frame: the current estimate's (default) or a streamed "
+                        "phase-gradient (PGHI) estimate, one frame later")
     p.add_argument("-stream_pitch", default=None, metavar="{SEMITONES,match,mv}",
                    help="-stream: shift every block by SEMITONES in [-24, 24], or track the stream and 'match' its "
                         "pitch level, or 'mv' its level and range, to the target's profile")
@@ -515,7 +519,8 @@ def stream_pitch_arg(p, args):
 def stream_params(args):
     from adaptive_voice_conversion_b200.streaming import StreamParams
     return StreamParams(window=args.stream_window, hop=args.stream_hop, lookahead=args.stream_lookahead,
-                        gl_lookahead=args.stream_gl_lookahead, gl_iters=args.stream_gl_iters)
+                        gl_lookahead=args.stream_gl_lookahead, gl_iters=args.stream_gl_iters,
+                        gl_init=args.stream_gl_init or "estimate")
 
 
 def run_stream(args, config, jobs):
@@ -626,7 +631,7 @@ def stream_profiles(jobs, raw, bank, vocoder, params):
                              f"synthesises to {n} samples, and the tracker needs at least {need}")
     tracks = {}
     if refs:
-        rt = Rtisi(hp, params.gl_lookahead, params.gl_iters, vocoder.device)
+        rt = Rtisi(hp, params.gl_lookahead, params.gl_iters, vocoder.device, params.gl_init)
         for f in refs:
             rt.open(f)
         sig = rt.run(dict(zip(refs, vocoder.mel_to_mag([raw[f] for f in refs]))), close=refs)
@@ -649,6 +654,8 @@ def main(argv=None):
         p.error("-stream_pitch needs -stream (offline conversions take -pitch_shift)")
     elif args.stream_morph is not None:
         p.error("-stream_morph needs -stream (offline conversions take -morph)")
+    elif args.stream_gl_init is not None:
+        p.error("-stream_gl_init needs -stream (offline conversions take -gl_init)")
     check_args(p, args)
     try:
         if args.semitones == "mv" and (args.speaker is not None or args.morph is not None):

@@ -29,6 +29,7 @@ The model has random weights unless -m is given; the input is synthetic (harmoni
 limit are read in the same run.  Writes nothing.
 """
 import argparse
+import ctypes as C
 import dataclasses
 import json
 import math
@@ -43,6 +44,8 @@ sys.path.insert(0, os.path.join(ROOT, "tests"))
 
 import numpy as np  # noqa: E402
 import torch  # noqa: E402
+
+from adaptive_voice_conversion_b200 import _lib as L  # noqa: E402
 
 
 def card():
@@ -105,6 +108,8 @@ def main():
     ap.add_argument("-pitch", "--pitch", default="0", help="pitch setting of every stream: 0, SEMITONES, match or mv")
     ap.add_argument("-retarget", "--retarget", action="store_true",
                     help="retarget every stream before every update (a ramp of H frames through four codes)")
+    ap.add_argument("-stream_gl_init", "--stream-gl-init", default="estimate", choices=["estimate", "pghi"],
+                    help="RTISI-LA's start phase (StreamParams.gl_init); pghi also times avc_pghi_stream alone")
     args = ap.parse_args()
     target = (math.log2(200.0), 0.15)
     pitch = (args.pitch, *target) if args.pitch in ("match", "mv") else (float(args.pitch) or None)
@@ -121,7 +126,7 @@ def main():
     dev = torch.device("cuda:0")
     voc = Vocoder(n_mels=cfg["SpeakerEncoder"]["c_in"], device=dev)
     hp = voc.hp
-    p = StreamParams()
+    p = StreamParams(gl_init=args.stream_gl_init)
     block = p.hop * hp.hop_length
     budget_ms = 1e3 * block / hp.sr
     c_out = cfg["SpeakerEncoder"]["c_out"]
@@ -167,20 +172,37 @@ def main():
             # call timed by CUDA events, each launch from a copy of the same state (the copy outside the events)
             conv.stage_ms = None
             mags = {sid: voc.mel_to_mag([torch.rand(p.hop, hp.n_mels, device=dev)])[0] for sid in ids}
+            pghi = p.gl_init == "pghi"
             state0, count0 = conv.rt.state.clone(), conv.rt.count.clone()
+            pstate0 = conv.rt.pstate.clone() if pghi else None
             desc, _, keep = conv.rt.prepare(mags)
-            ev = [torch.cuda.Event(enable_timing=True) for _ in range(2)]
-            times = []
+            ev = [torch.cuda.Event(enable_timing=True) for _ in range(3)]
+            times, ptimes = [], []
+            lib = L.load()
             for _ in range(7):
                 conv.rt.state.copy_(state0)
                 conv.rt.count.copy_(count0)
+                if pghi:
+                    conv.rt.pstate.copy_(pstate0)
                 torch.cuda.synchronize()
                 ev[0].record()
-                conv.rt.launch(desc)
+                if pghi:   # the two launches of Rtisi.launch, with an event between them
+                    L.check(lib.avc_pghi_stream(C.byref(desc[0]), C.c_float(hp.pghi_tol), None, None), "avc_pghi_stream")
+                    ev[2].record()
+                    L.check(lib.avc_rtisi_la_from(C.byref(desc[1]), desc[0].X, None), "avc_rtisi_la_from")
+                else:
+                    conv.rt.launch(desc)
                 ev[1].record()
                 torch.cuda.synchronize()
                 times.append(ev[0].elapsed_time(ev[1]))
+                if pghi:
+                    ptimes.append(ev[0].elapsed_time(ev[2]))
             rt_ms = sorted(times)[len(times) // 2]
+            if pghi:
+                pg_ms = sorted(ptimes)[len(ptimes) // 2]
+                res["pghi_stream_kernel"] = {"streams": S, "ms": pg_ms}
+                print(f"avc_pghi_stream kernel alone, {S} streams x {p.hop} frames: {pg_ms:.3f} ms (of {rt_ms:.3f} ms "
+                      f"with avc_rtisi_la_from)", file=sys.stderr)
             del keep
             ffts = S * p.hop * (1 + p.gl_iters * (p.gl_lookahead + 1)) * 2
             # offline Griffin-Lim on the same number of frames: 2 FFTs per frame per iteration
