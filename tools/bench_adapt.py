@@ -15,11 +15,10 @@ import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "tools"))
 
 import torch  # noqa: E402
 
-from bench_padded import card  # noqa: E402
+from _harness import card, events_ms  # noqa: E402
 
 
 def trainers(n_mels, B, graph):
@@ -49,14 +48,9 @@ def trainers(n_mels, B, graph):
 
 
 def time_steps(t, x, lam, n):
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(n):
-        t.step(x, lam)
-    e1.record()
-    torch.cuda.synchronize()
+    ms = events_ms(lambda: t.step(x, lam), n, 0)
     t.losses()      # raises on a tensor-core pipeline time-out
-    return e0.elapsed_time(e1) / n
+    return ms
 
 
 def bench(n_mels, B, steps, reps):

@@ -19,24 +19,11 @@ import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "tools"))
 
 import numpy as np  # noqa: E402
 import torch  # noqa: E402
 
-from bench_padded import card, timed  # noqa: E402
-
-
-def events(launch, iters):
-    for _ in range(min(iters, 10)):
-        launch()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(iters):
-        launch()
-    e1.record()
-    torch.cuda.synchronize()
-    return e0.elapsed_time(e1) * 1e3 / iters
+from _harness import card, events_ms, median_wall_s  # noqa: E402
 
 
 def pooling(n_spk, n_utts, iters=200):
@@ -50,17 +37,22 @@ def pooling(n_spk, n_utts, iters=200):
     lt = torch.tensor(lens, dtype=torch.int32, device="cuda")
     sums = torch.empty(B, Cc, device="cuda")
     counts = torch.empty(B, dtype=torch.int32, device="cuda")
-    us_sum = events(lambda: L.check(lib.avc_time_sum_varlen(x.data_ptr(), x[0].numel(), sums.data_ptr(), counts.data_ptr(),
-                                                             B, Cc, T, lt.data_ptr(), div, 1, None), "avc_time_sum_varlen"),
-                    iters)
+
+    def time_sum():
+        L.check(lib.avc_time_sum_varlen(x.data_ptr(), x[0].numel(), sums.data_ptr(), counts.data_ptr(), B, Cc, T,
+                                        lt.data_ptr(), div, 1, None), "avc_time_sum_varlen")
+    us_sum = 1e3 * events_ms(time_sum, iters, min(iters, 10))
     frames = int(sum(-(-int(v) // div) for v in lens))
     N = n_spk * n_utts
     tab = torch.randn(N, Cc, device="cuda")
     cnt = torch.tensor(rng.integers(13, 76, N), dtype=torch.int32, device="cuda")
     offs = torch.arange(0, N + 1, n_utts, dtype=torch.int64, device="cuda")
     out = torch.empty(n_spk, Cc, device="cuda")
-    us_pool = events(lambda: L.check(lib.avc_pooled_group_mean(tab.data_ptr(), cnt.data_ptr(), N, Cc, offs.data_ptr(), n_spk,
-                                                               out.data_ptr(), None), "avc_pooled_group_mean"), iters)
+
+    def group_mean():
+        L.check(lib.avc_pooled_group_mean(tab.data_ptr(), cnt.data_ptr(), N, Cc, offs.data_ptr(), n_spk, out.data_ptr(),
+                                          None), "avc_pooled_group_mean")
+    us_pool = 1e3 * events_ms(group_mean, iters, min(iters, 10))
     return {"time_sum_varlen": {"utterances": B, "channels": Cc, "valid_frames": frames, "us_per_launch": us_sum,
                                 "read_GB_per_s": (frames * Cc * 4 + B * 4) / (us_sum * 1e-6) / 1e9},
             "pooled_group_mean": {"groups": n_spk, "rows": N, "channels": Cc, "us_per_launch": us_pool,
@@ -83,7 +75,8 @@ def identify(m, s, d, iters=5):
                              best=best.data_ptr(), best_score=bs.data_ptr(), target_score=ts.data_ptr(),
                              target_rank=rank.data_ptr())
     S.identify(q[:4], bank)    # the Python path once
-    us = events(lambda: L.check(lib.avc_spk_identify(C.byref(desc), None), "avc_spk_identify"), iters)
+    us = 1e3 * events_ms(lambda: L.check(lib.avc_spk_identify(C.byref(desc), None), "avc_spk_identify"), iters,
+                         min(iters, 10))
     fma = 2 * m * s * d
     return {"m": m, "s": s, "dims": d, "ms_per_launch": us / 1e3, "fp64_fma_per_s": fma / (us * 1e-6)}
 
@@ -101,8 +94,8 @@ def build(n_mels, n_spk, n_utts, reps=3):
     mels = {f"p{s:03d}_{k:03d}": torch.randn(int(rng.integers(100, 601)), n_mels, device="cuda")
             for s in range(n_spk) for k in range(n_utts)}
     frames = sum(int(v.shape[0]) for v in mels.values())
-    build_bank(model, mels)
-    ts = [timed(lambda: build_bank(model, mels)) for _ in range(reps)]
+    ts = []
+    median_wall_s(lambda: build_bank(model, mels), reps, samples=ts)
     t = min(ts)
     return {"c_in": n_mels, "speakers": n_spk, "utterances": len(mels), "input_frames": frames, "seconds": ts,
             "utterances_per_s": len(mels) / t, "input_frames_per_s": frames / t}

@@ -18,11 +18,11 @@ nothing outside the temporary directory.
 import argparse
 import contextlib
 import io
+import itertools
 import json
 import os
 import pickle
 import statistics
-import subprocess
 import sys
 import tempfile
 import types
@@ -33,14 +33,10 @@ sys.path.insert(0, ROOT)
 import numpy as np  # noqa: E402
 import torch  # noqa: E402
 
+from _harness import card, events_ms  # noqa: E402
+
 HBM_BPS = 3.35e12
 SEG = 128
-
-
-def card():
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                       capture_output=True, text=True).stdout.strip().splitlines()
-    return q[torch.cuda.current_device()] if q else torch.cuda.get_device_name()
 
 
 def write_corpus(path, n_utt, n_mels, seed=0):
@@ -73,14 +69,12 @@ def gather_time(ds, launches):
     next(ds)                                   # loads epoch 0's order
     B = ds.sampler.batch_size
     xs = [ds.gather(0, B) for _ in range(3)]
-    torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for i in range(launches):
+    n = itertools.count()
+
+    def launch():
+        i = next(n)
         xs[i % 3] = ds.gather((i * B) % max(1, ds.sampler.n - B), B)
-    e1.record()
-    torch.cuda.synchronize()
-    us = e0.elapsed_time(e1) * 1e3 / launches
+    us = 1e3 * events_ms(launch, launches, 0, sync=True)
     nbytes = 2 * B * ds.c_in * ds.T * 4 + B * 12      # batch read + written; order and starts entries
     return {"us_per_launch": us, "bytes_per_launch": nbytes, "achieved_TBps": nbytes / us / 1e6,
             "share_of_3.35TBps": nbytes / us / 1e6 / (HBM_BPS / 1e12)}
@@ -127,15 +121,9 @@ def run_config(n_mels, batch, a):
         names = list(arms)
         for w in range(a.windows):
             for name in names[w % 3:] + names[:w % 3]:    # rotated: no arm always follows the same one
-                s = arms[name]
-                torch.cuda.synchronize()
-                e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-                e0.record()
-                meta = s.run_steps(K, lambda_of=lambda it: 1.0)
-                e1.record()
-                torch.cuda.synchronize()
-                assert all(np.isfinite(v) for v in meta.values()), (name, meta)
-                wins[name].append(e0.elapsed_time(e1))
+                s, metas = arms[name], []
+                wins[name].append(events_ms(lambda: metas.append(s.run_steps(K, lambda_of=lambda it: 1.0)), 1, 0))
+                assert all(np.isfinite(v) for v in metas[0].values()), (name, metas[0])
         res["run_steps"] = {k: {"seg_per_s": batch * K / (statistics.median(v) * 1e-3), "ms_per_step": statistics.median(v) / K,
                                 "window_ms": v} for k, v in wins.items()}
         syn_rate = res["run_steps"]["synthetic"]["seg_per_s"]

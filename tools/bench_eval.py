@@ -17,34 +17,24 @@ from __future__ import annotations
 import argparse
 import contextlib
 import io
+import itertools
 import json
 import os
 import pickle
-import statistics
-import subprocess
 import sys
 import tempfile
-import time
 import types
 
 import numpy as np
 import torch
+
+from _harness import card, events_ms, median_wall_s
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 HBM_BYTES_PER_S = 3.35e12
 SEG = 128
-
-
-def card():
-    name = torch.cuda.get_device_name()
-    try:
-        q = subprocess.run(["nvidia-smi", "--query-gpu=power.limit,clocks.max.sm", "--format=csv,noheader"],
-                           capture_output=True, text=True, timeout=30).stdout.strip().splitlines()[0]
-    except Exception as e:   # noqa: BLE001
-        q = f"unavailable ({e})"
-    return {"name": name, "power_limit_and_max_sm_clock": q}
 
 
 def write_set(root, name, n_mels, n_entries, seed, n_speakers=20, utts_per_speaker=10):
@@ -83,13 +73,8 @@ def kernel_time(c_in, B, reps=200, rotate_bytes=256 << 20):
     lib, st = L.load(), torch.cuda.current_stream().cuda_stream
     for d in descs:
         L.check(lib.avc_eval_losses(d, st))
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for i in range(reps):
-        lib.avc_eval_losses(descs[i % len(descs)], st)
-    e1.record()
-    torch.cuda.synchronize()
-    us = e0.elapsed_time(e1) * 1e3 / reps
+    n = itertools.count()
+    us = 1e3 * events_ms(lambda: lib.avc_eval_losses(descs[next(n) % len(descs)], st), reps, 0)
     return {"us": round(us, 2), "bytes": nbytes, "input_sets_rotated": len(descs), "GB_per_s": round(nbytes / us / 1e3, 1),
             "share_of_3.35TB_per_s": round(nbytes / (us * 1e-6) / HBM_BYTES_PER_S, 3)}
 
@@ -113,27 +98,16 @@ def bench(root, c_in, B, n_entries):
         s = Solver(cfg, args)
         s.run_steps(8)                      # capture and warm the training graph
         s.evaluate()                        # warm-up: loads the set, allocator, packs
-    torch.cuda.synchronize()
-    times = []
-    for _ in range(3):
-        t0 = time.perf_counter()
-        res = s.evaluate()
-        torch.cuda.synchronize()
-        times.append(time.perf_counter() - t0)
-    eval_s = statistics.median(times)
+    times, results = [], []
+    eval_s = median_wall_s(lambda: results.append(s.evaluate()), 3, warmup=0, samples=times)
+    res = results[-1]
     n_steps, windows = 40, []
-    for _ in range(3):
-        torch.cuda.synchronize()
-        t0 = time.perf_counter()
-        s.run_steps(n_steps)
-        torch.cuda.synchronize()
-        windows.append((time.perf_counter() - t0) / n_steps)
-    step_s = statistics.median(windows)
+    step_s = median_wall_s(lambda: s.run_steps(n_steps), 3, warmup=0, samples=windows) / n_steps
     s.save_model(s.iteration - 1)          # <d>/model.ckpt for `python evaluate.py`
     return {"c_in": c_in, "batch": B, "entries": n_entries, "batches": -(-n_entries // B),
             "evaluate_s_median_of_3": round(eval_s, 4), "evaluate_s_all": [round(t, 4) for t in times],
             "segments_per_s": round(n_entries / eval_s), "train_step_ms": round(step_s * 1e3, 3),
-            "train_step_ms_windows": [round(w * 1e3, 3) for w in windows],
+            "train_step_ms_windows": [round(w * 1e3 / n_steps, 3) for w in windows],
             "evaluate_in_train_steps": round(eval_s / step_s, 1), "kernel": kernel_time(c_in, B),
             "in_test": res["in_test"]}
 

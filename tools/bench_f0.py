@@ -18,42 +18,18 @@ from __future__ import annotations
 import argparse
 import json
 import os
-import statistics
-import subprocess
 import sys
 
 import numpy as np
 import torch
+
+from _harness import card, median_events_s
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 
 FP64_PEAK = 34e12   # H100 SXM data sheet, FP64 without tensor cores
-
-
-def card():
-    name = torch.cuda.get_device_name()
-    try:
-        q = subprocess.run(["nvidia-smi", "--query-gpu=power.limit,clocks.max.sm", "--format=csv,noheader"],
-                           capture_output=True, text=True, timeout=30).stdout.strip().splitlines()[0]
-    except Exception as e:   # noqa: BLE001
-        q = f"unavailable ({e})"
-    return {"name": name, "power_limit_and_max_sm_clock": q}
-
-
-def timed(fn, reps=5):
-    fn()
-    torch.cuda.synchronize()
-    ts = []
-    for _ in range(reps):
-        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        a.record()
-        fn()
-        b.record()
-        b.synchronize()
-        ts.append(a.elapsed_time(b) / 1e3)
-    return statistics.median(ts)
 
 
 def tracker(n_signals, n_frames):
@@ -65,7 +41,7 @@ def tracker(n_signals, n_frames):
     sigs = [torch.from_numpy(harmonic(float(rng.uniform(60, 400)), (n_frames - 1) * hop / sr, phase_seed=i)).cuda()
             for i in range(n_signals)]
     frames = sum(1 + s.numel() // hop for s in sigs)
-    t = timed(lambda: F.yin(sigs, sr, hop, p))
+    t = median_events_s(lambda: F.yin(sigs, sr, hop, p), 5)
     ops = 3.0 * frames * p.tau_max(sr) * p.win
     return {"signals": n_signals, "frames": frames, "seconds_per_call": t, "frames_per_second": frames / t,
             "fp64_flops": ops / t, "fp64_share_of_datasheet": ops / t / FP64_PEAK}

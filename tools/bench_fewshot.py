@@ -19,12 +19,11 @@ import types
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "tools"))
 
 import numpy as np  # noqa: E402
 import torch  # noqa: E402
 
-from bench_padded import card, timed  # noqa: E402
+from _harness import card, events_ms, median_wall_s  # noqa: E402
 
 
 def kernel(iters=200):
@@ -43,15 +42,7 @@ def kernel(iters=200):
     def launch():
         L.check(lib.avc_time_mean_grouped_fwd(x.data_ptr(), x[0].numel(), out.data_ptr(), B, Cc, T, lt.data_ptr(), div, 1,
                                               offs.data_ptr(), len(sizes), None), "avc_time_mean_grouped_fwd")
-    for _ in range(10):
-        launch()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(iters):
-        launch()
-    e1.record()
-    torch.cuda.synchronize()
-    us = e0.elapsed_time(e1) * 1e3 / iters
+    us = 1e3 * events_ms(launch, iters, 10)
     frames = int(sum(-(-int(v) // div) for v in lens))
     nbytes = frames * Cc * 4 + B * 4 + len(sizes) * Cc * 4
     return {"groups": len(sizes), "members": B, "channels": Cc, "valid_frames": frames, "us_per_launch": us,
@@ -74,9 +65,9 @@ def embedding(inf, n_mels, n_sets, ks, reps):
     out = []
     for k in ks:
         sets = [[torch.randn((int(t), n_mels), generator=g).cuda() for t in rng.integers(100, 601, k)] for _ in range(n_sets)]
-        inf.embed_speakers(sets)
-        t = [timed(lambda: inf.embed_speakers(sets)) for _ in range(reps)]
-        out.append({"K": k, "sets": n_sets, "sets_per_s": n_sets / statistics.median(t), "s": t})
+        t = []
+        med = median_wall_s(lambda: inf.embed_speakers(sets), reps, samples=t)
+        out.append({"K": k, "sets": n_sets, "sets_per_s": n_sets / med, "s": t})
     return out
 
 
@@ -91,8 +82,8 @@ def conversion(inf, n_mels, n_pairs, reps, k=4):
     caps = inf.padded_captures
     t1, tk = [], []
     for _ in range(reps):
-        t1.append(timed(lambda: inf.inference_padded(xs, cs)))
-        tk.append(timed(lambda: inf.inference_padded(xs, sets)))
+        t1.append(median_wall_s(lambda: inf.inference_padded(xs, cs), 1, warmup=0))
+        tk.append(median_wall_s(lambda: inf.inference_padded(xs, sets), 1, warmup=0))
     return {"pairs": n_pairs, "K": k, "single_pairs_per_s": n_pairs / statistics.median(t1),
             "sets_pairs_per_s": n_pairs / statistics.median(tk), "single_s": t1, "sets_s": tk,
             "captures_in_timed_calls": inf.padded_captures - caps}

@@ -17,12 +17,11 @@ import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "tools"))
 
 import numpy as np  # noqa: E402
 import torch  # noqa: E402
 
-from bench_padded import card  # noqa: E402
+from _harness import card, events_ms  # noqa: E402
 
 
 def model_of(cfg):
@@ -67,13 +66,7 @@ def bench(n_mels, S, m, steps, reps, fit_steps):
     ms = {"fit": [], "adapt": []}
     for _ in range(reps):
         for key, fn in (("fit", fit_step), ("adapt", ad_step)):
-            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            e0.record()
-            for _ in range(steps):
-                fn()
-            e1.record()
-            torch.cuda.synchronize()
-            ms[key].append(e0.elapsed_time(e1) / steps)
+            ms[key].append(events_ms(fn, steps, 0))
     fit.eng.check_tc_status()
     ad.losses()     # raises on a tensor-core pipeline time-out
     best = {key: min(v) for key, v in ms.items()}

@@ -22,8 +22,6 @@ import io
 import json
 import os
 import pickle
-import statistics
-import subprocess
 import sys
 import tempfile
 import time
@@ -31,33 +29,11 @@ import time
 import numpy as np
 import torch
 
+from _harness import card, median_events_s
+
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests"))
-
-
-def card():
-    name = torch.cuda.get_device_name()
-    try:
-        q = subprocess.run(["nvidia-smi", "--query-gpu=power.limit,clocks.max.sm", "--format=csv,noheader"],
-                           capture_output=True, text=True, timeout=30).stdout.strip().splitlines()[0]
-    except Exception as e:   # noqa: BLE001
-        q = f"unavailable ({e})"
-    return {"name": name, "power_limit_and_max_sm_clock": q}
-
-
-def timed(fn, reps=3):
-    fn()
-    torch.cuda.synchronize()
-    ts = []
-    for _ in range(reps):
-        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        a.record()
-        fn()
-        b.record()
-        b.synchronize()
-        ts.append(a.elapsed_time(b) / 1e3)
-    return statistics.median(ts)
 
 
 def kernels(n_pairs, dims, n_mels, host_pairs):
@@ -70,11 +46,11 @@ def kernels(n_pairs, dims, n_mels, host_pairs):
     g = torch.Generator(device="cuda").manual_seed(0)
     mels = torch.randn((sum(lengths), n_mels), generator=g, device="cuda")
     parts = list(torch.split(mels, lengths))
-    t_cep = timed(lambda: M.mel_cepstrum(parts, attr, dims=dims))
+    t_cep = median_events_s(lambda: M.mel_cepstrum(parts, attr, dims=dims), 3)
     ceps = M.mel_cepstrum(parts, attr, dims=dims)
     del mels, parts
     xs, ys = ceps[:n_pairs], ceps[n_pairs:]
-    t_dtw = timed(lambda: M.dtw(xs, ys))
+    t_dtw = median_events_s(lambda: M.dtw(xs, ys), 3)
     rows = sum(lengths)
     cells = int((tx * ty).sum())
     sub = range(host_pairs)

@@ -16,11 +16,10 @@ import types
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "tools"))
 
 import torch  # noqa: E402
 
-from bench_padded import card, timed  # noqa: E402
+from _harness import card, median_wall_s  # noqa: E402
 
 
 def run(n_mels, n_src, frames, ks, reps):
@@ -46,9 +45,9 @@ def run(n_mels, n_src, frames, ks, reps):
         morphs[K]()
     best = {"codes": float("inf"), **{K: float("inf") for K in ks}}
     for _ in range(reps):
-        best["codes"] = min(best["codes"], timed(plain))
+        best["codes"] = min(best["codes"], median_wall_s(plain, 1, warmup=0))
         for K in ks:
-            best[K] = min(best[K], timed(morphs[K]))
+            best[K] = min(best[K], median_wall_s(morphs[K], 1, warmup=0))
     out["inference_with_codes_ms"] = best["codes"] * 1e3
     for K in ks:
         out[f"inference_morph_K{K}_ms"] = best[K] * 1e3

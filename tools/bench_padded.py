@@ -25,23 +25,7 @@ sys.path.insert(0, ROOT)
 import numpy as np  # noqa: E402
 import torch  # noqa: E402
 
-
-def card():
-    name = torch.cuda.get_device_name()
-    try:
-        q = subprocess.run(["nvidia-smi", "--query-gpu=power.limit,clocks.max.sm", "--format=csv,noheader"],
-                           capture_output=True, text=True, timeout=30).stdout.strip().splitlines()[0]
-    except Exception as e:   # noqa: BLE001
-        q = f"unavailable ({e})"
-    return {"name": name, "power_limit_and_max_sm_clock": q}
-
-
-def timed(fn):
-    torch.cuda.synchronize()
-    t0 = time.perf_counter()
-    fn()
-    torch.cuda.synchronize()
-    return time.perf_counter() - t0
+from _harness import card, median_wall_s  # noqa: E402
 
 
 def conversion(n_mels, n_pairs, reps):
@@ -62,8 +46,8 @@ def conversion(n_mels, n_pairs, reps):
     caps = inf.padded_captures
     t_r, t_p = [], []
     for _ in range(reps):
-        t_r.append(timed(lambda: inf.inference_ragged(xs, cs)))
-        t_p.append(timed(lambda: inf.inference_padded(xs, cs)))
+        t_r.append(median_wall_s(lambda: inf.inference_ragged(xs, cs), 1, warmup=0))
+        t_p.append(median_wall_s(lambda: inf.inference_padded(xs, cs), 1, warmup=0))
     plan = padded_batches(src, ref)
     pad_src = sum(B * T for _, T, _, B in plan) / sum(src)
     pad_ref = sum(B * Tc for _, _, Tc, B in plan) / sum(ref)

@@ -28,11 +28,11 @@ import types
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "tools"))
 
 import torch  # noqa: E402
 
-from bench_vocoder import card, convergence_table, event_time, fewest_iterations, timed, utterances  # noqa: E402
+from _harness import card, events_ms, median_wall_s  # noqa: E402
+from bench_vocoder import convergence_table, fewest_iterations, utterances  # noqa: E402
 
 INITS = ("zero", "pghi")
 
@@ -44,8 +44,8 @@ def pghi_time(V, mags, hp, windows, reps=5):
     X = torch.empty(S.shape[0], hp.n_bins, 2, device=S.device)
     d = r.desc(hp, mag=S, X=X)
     tol = C.c_float(hp.pghi_tol)
-    return statistics.median(event_time(lambda: V._call("avc_pghi", d, S.device, tol, None), reps)
-                             for _ in range(windows))
+    return statistics.median(events_ms(lambda: V._call("avc_pghi", d, S.device, tol, None), reps, 1, sync=True)
+                             for _ in range(windows)) / 1e3
 
 
 def tables(V, mags, hp, iters, momenta):
@@ -82,7 +82,7 @@ def main():
     wavs = utterances(a.utts, n_samples)
     res = {"card": card(), "utts": a.utts, "frames": a.frames, "long_frames": a.long, "momentum": a.momentum,
            "pghi_tol": hp0.pghi_tol, "signals": "synthetic (vibrato tones with harmonics and a noise floor)"}
-    print(f"card (name, power limit, max SM clock): {res['card']}", file=sys.stderr)
+    print(f"card: {res['card']}", file=sys.stderr)
     iters = sorted(set(a.sc_iters) | {100})
     momenta = (0.0, a.momentum)
     consistent = [A for A, _ in V.magnitude(wavs, hp0)]
@@ -111,13 +111,14 @@ def main():
             tgt = src[1:] + src[:1]
             return voc.mel_to_wav(inf.inference_ragged(src, tgt), n_iter, momentum, init)
 
-        t_plain, _ = timed(convert, a.windows, 1)
+        t_plain = median_wall_s(convert, a.windows)
         out["conversion_zero_100"] = {"utt_per_s": a.utts / t_plain, "audio_s_per_s": audio_s / t_plain}
         for m in momenta:
             n_fast = fewest_pghi_iterations(table, m)
             rec = {"fewest_pghi_grid_iters_at_or_below_zero_100": n_fast}
             if n_fast is not None:
-                t_fast, w_fast = timed(lambda: convert(n_fast, m, "pghi"), a.windows, 1)
+                w_fast = []
+                t_fast = median_wall_s(lambda: convert(n_fast, m, "pghi"), a.windows, samples=w_fast)
                 rec["conversion"] = {"n_iter": n_fast, "utt_per_s": a.utts / t_fast, "audio_s_per_s": audio_s / t_fast,
                                      "windows_s": w_fast}
             out[f"momentum_{m}"] = rec

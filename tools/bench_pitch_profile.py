@@ -22,41 +22,19 @@ from __future__ import annotations
 import argparse
 import json
 import os
-import statistics
-import subprocess
 import sys
 import time
 
 import numpy as np
 import torch
 
+from _harness import card, median_wall_s
+
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 
 SR, HOP = 24000, 300
-
-
-def card():
-    name = torch.cuda.get_device_name()
-    try:
-        q = subprocess.run(["nvidia-smi", "--query-gpu=power.limit,clocks.max.sm", "--format=csv,noheader"],
-                           capture_output=True, text=True, timeout=30).stdout.strip().splitlines()[0]
-    except Exception as e:   # noqa: BLE001
-        q = f"unavailable ({e})"
-    return {"name": name, "power_limit_and_max_sm_clock": q}
-
-
-def wall(fn, reps=3):
-    fn()
-    torch.cuda.synchronize()
-    ts = []
-    for _ in range(reps):
-        t0 = time.perf_counter()
-        fn()
-        torch.cuda.synchronize()
-        ts.append(time.perf_counter() - t0)
-    return statistics.median(ts)
 
 
 def dev(a):
@@ -116,8 +94,9 @@ def wav_to_wav(n_convs, frames):
     def mv_bank():
         s, _ = F.mv_match(voc, convs, hp, profiles=[prof] * n_convs)
         voc.mel_to_wav(convs, semitones=s)
-    res = {"convs": n_convs, "frames": frames, "unshifted_s": wall(lambda: voc.mel_to_wav(convs)),
-           "match_s": wall(match), "mv_refs_s": wall(mv_refs), "mv_bank_s": wall(mv_bank)}
+    res = {"convs": n_convs, "frames": frames, "unshifted_s": median_wall_s(lambda: voc.mel_to_wav(convs), 3),
+           "match_s": median_wall_s(match, 3), "mv_refs_s": median_wall_s(mv_refs, 3),
+           "mv_bank_s": median_wall_s(mv_bank, 3)}
     tracks = F.track_chunks(F.synthesize(voc, convs, hp), SR, HOP, F.F0Params())
     t0 = time.perf_counter()
     F.mv_shifts(tracks, [prof] * n_convs)

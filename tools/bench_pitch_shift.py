@@ -20,13 +20,12 @@ from __future__ import annotations
 import argparse
 import json
 import os
-import statistics
-import subprocess
 import sys
-import time
 
 import numpy as np
 import torch
+
+from _harness import card, median_events_s, median_wall_s
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
@@ -35,42 +34,6 @@ sys.path.insert(0, os.path.join(ROOT, "tests"))
 HBM_PEAK = 3.35e12    # H100 SXM data sheet, bytes/s
 FP32_PEAK = 67e12     # H100 SXM data sheet, FP32 FLOP/s without tensor cores
 SHIFTS = (-12.0, -7.0, -3.0, 4.0, 7.0, 12.0)
-
-
-def card():
-    name = torch.cuda.get_device_name()
-    try:
-        q = subprocess.run(["nvidia-smi", "--query-gpu=power.limit,clocks.max.sm", "--format=csv,noheader"],
-                           capture_output=True, text=True, timeout=30).stdout.strip().splitlines()[0]
-    except Exception as e:   # noqa: BLE001
-        q = f"unavailable ({e})"
-    return {"name": name, "power_limit_and_max_sm_clock": q}
-
-
-def timed(fn, reps=5):
-    fn()
-    torch.cuda.synchronize()
-    ts = []
-    for _ in range(reps):
-        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        a.record()
-        fn()
-        b.record()
-        b.synchronize()
-        ts.append(a.elapsed_time(b) / 1e3)
-    return statistics.median(ts)
-
-
-def wall(fn, reps=3):
-    fn()
-    torch.cuda.synchronize()
-    ts = []
-    for _ in range(reps):
-        t0 = time.perf_counter()
-        fn()
-        torch.cuda.synchronize()
-        ts.append(time.perf_counter() - t0)
-    return statistics.median(ts)
 
 
 def dev(a):
@@ -100,7 +63,7 @@ def kernel(n_signals, n_frames):
     def call():
         L.check(lib.avc_pitch_shift(S.data_ptr(), ratio.data_ptr(), out.data_ptr(), rows, 1025, lifter,
                                     torch.cuda.current_stream().cuda_stream), "avc_pitch_shift")
-    t = timed(call)
+    t = median_events_s(call, 5)
     bytes_ = 2 * 4100 * rows
     flops = 2 * 2 * lifter * 1025 * rows
     t_hbm, t_fp32 = bytes_ / HBM_PEAK, flops / FP32_PEAK
@@ -125,9 +88,9 @@ def wav_to_wav(n_utts):
             shifts, _ = F.match_shifts(voc, convs, [[r] for r in refs], voc.hp)
             return voc.mel_to_wav(convs, semitones=shifts)
         r = {"utterances": n_utts, "frames": int(sum(m.shape[0] for m in convs)),
-             "shift_0_s": wall(lambda: voc.mel_to_wav(convs)),
-             "shift_+4_s": wall(lambda: voc.mel_to_wav(convs, semitones=4.0)),
-             "match_s": wall(match)}
+             "shift_0_s": median_wall_s(lambda: voc.mel_to_wav(convs), 3),
+             "shift_+4_s": median_wall_s(lambda: voc.mel_to_wav(convs, semitones=4.0), 3),
+             "match_s": median_wall_s(match, 3)}
         r["match_over_shift_0"] = r["match_s"] / r["shift_0_s"]
         r["fixed_over_shift_0"] = r["shift_+4_s"] / r["shift_0_s"]
         out[label] = r

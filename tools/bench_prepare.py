@@ -21,7 +21,6 @@ import functools
 import json
 import os
 import shutil
-import subprocess
 import sys
 import tempfile
 import time
@@ -34,6 +33,7 @@ from scipy.io import wavfile
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from adaptive_voice_conversion_b200 import prepare as P   # noqa: E402
 from adaptive_voice_conversion_b200 import vocoder as V   # noqa: E402
+from _harness import card   # noqa: E402
 
 HBM_BYTES_PER_S = 3.35e12   # H100 SXM data sheet
 
@@ -107,12 +107,6 @@ def write_libri_corpus(root, n_utts, n_speakers, seed):
         wavfile.write(os.path.join(d, f"{spk}_{ch}_{k:06d}_{k + 1:06d}.wav"), 24000, pcm)
         n_in.append(pcm.size)
     return libri, np.array(n_in, np.int64)
-
-
-def card():
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm,clocks.sm", "--format=csv,noheader",
-                        "-i", str(torch.cuda.current_device())], capture_output=True, text=True).stdout.strip()
-    return q or torch.cuda.get_device_name()
 
 
 def main():

@@ -21,36 +21,14 @@ import ctypes as C
 import json
 import os
 import sys
-import time
 
 import numpy as np
 import torch
 
+from _harness import card, events_ms, median_wall_s
+
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "tools"))
-
-from bench_mcd import card  # noqa: E402
-
-
-def host_timed(fn):
-    torch.cuda.synchronize()
-    t = time.perf_counter()
-    out = fn()
-    torch.cuda.synchronize()
-    return out, time.perf_counter() - t
-
-
-def event_ms(fn, reps=200):
-    for _ in range(5):
-        fn()
-    a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    a.record()
-    for _ in range(reps):
-        fn()
-    b.record()
-    b.synchronize()
-    return a.elapsed_time(b) / reps
 
 
 def step_split(D, S, Bt, H=256):
@@ -81,11 +59,12 @@ def step_split(D, S, Bt, H=256):
         L.check(lib.avc_adam_step(flat.data_ptr(), grad.data_ptr(), m.data_ptr(), v.data_ptr(), vmax.data_ptr(), n,
                                   hp.data_ptr(), sq.data_ptr(), step.data_ptr(), st))
     net.forward(Pv, x, Bt)
-    out = {"linear_fwd": event_ms(lambda: net.forward(Pv, x, Bt)),
-           "xent": event_ms(lambda: P.xent(net.z, lab, 1.0 / Bt, dlogits=net.dz, loss_sum=tot, scratch=scratch)),
-           "fill_zero": event_ms(zero),
-           "linear_bwd": event_ms(lambda: net.backward(Pv, Gv, x, Bt)),
-           "sqnorm_adam": event_ms(update)}
+    out = {"linear_fwd": events_ms(lambda: net.forward(Pv, x, Bt), 200, 5),
+           "xent": events_ms(lambda: P.xent(net.z, lab, 1.0 / Bt, dlogits=net.dz, loss_sum=tot, scratch=scratch),
+                             200, 5),
+           "fill_zero": events_ms(zero, 200, 5),
+           "linear_bwd": events_ms(lambda: net.backward(Pv, Gv, x, Bt), 200, 5),
+           "sqnorm_adam": events_ms(update, 200, 5)}
     out["step"] = sum(out.values())
     flops = 2 * Bt * (D * H + H * H + H * S) * 3        # forward, data and weight gradients
     out["linear_tflops"] = flops / ((out["linear_fwd"] + out["linear_bwd"]) * 1e-3) / 1e12
@@ -103,15 +82,20 @@ def run(c_in, n_spk, n_utts, frames, seed=0):
     mels = [torch.randn(int(T), c_in, device="cuda") for T in lens]
     labels = np.repeat(np.arange(n_spk), n_utts)
     P.features(model, mels[:8])                          # warm-up
-    feats, t_feat = host_timed(lambda: P.features(model, mels))
+    feats = {}
+    t_feat = median_wall_s(lambda: feats.update(P.features(model, mels)), 1, warmup=0)
     res = {"c_in": c_in, "utterances": len(mels), "mel_frames": int(lens.sum()),
            "latent_frames": int(feats["offsets"][-1]), "features_s": t_feat, "probes": {}}
     frame_lab = np.repeat(labels, np.diff(feats["offsets"]))
     for k in P.REPRESENTATIONS:
         fr = k == "content_frames"
         lab = frame_lab if fr else labels
-        probe, t_fit = host_timed(lambda: P.fit_probe(feats[k], lab, seed=seed, n_classes=n_spk, frames=fr))
-        sc, t_score = host_timed(lambda: P.score_probe(probe, feats[k], lab))
+        fitted, scored = [], []
+        t_fit = median_wall_s(lambda: fitted.append(P.fit_probe(feats[k], lab, seed=seed, n_classes=n_spk, frames=fr)),
+                              1, warmup=0)
+        probe = fitted[0]
+        t_score = median_wall_s(lambda: scored.append(P.score_probe(probe, feats[k], lab)), 1, warmup=0)
+        sc = scored[0]
         res["probes"][k] = {"rows": int(feats[k].shape[0]), "dims": int(feats[k].shape[1]), "fit_s": t_fit,
                             "score_s": t_score, "fit_acc": float((sc["rank"] == 0).mean()),
                             "last_loss": probe.losses[-1]}

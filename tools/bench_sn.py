@@ -16,13 +16,13 @@ import contextlib
 import io
 import json
 import os
-import subprocess
 import sys
 import tempfile
-import time
 import types
 
 import torch
+
+from _harness import card, graph_us, median_wall_s
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
@@ -36,35 +36,6 @@ def config(c_in, sn, batch=None):
     if batch is not None:
         cfg["data_loader"]["batch_size"] = batch
     return cfg
-
-
-def card():
-    name = torch.cuda.get_device_name()
-    try:
-        q = subprocess.run(["nvidia-smi", "--query-gpu=power.limit,clocks.max.sm", "--format=csv,noheader"],
-                           capture_output=True, text=True, timeout=30).stdout.strip().splitlines()[0]
-    except Exception as e:   # noqa: BLE001
-        q = f"unavailable ({e})"
-    return {"name": name, "power_limit_and_max_sm_clock": q}
-
-
-def graph_time_us(fn, reps=50, replays=20):
-    """Device time of one fn() call: reps calls in one CUDA graph, timed over replays with events."""
-    fn()
-    torch.cuda.synchronize()
-    g = torch.cuda.CUDAGraph()
-    with torch.cuda.graph(g):
-        for _ in range(reps):
-            fn()
-    g.replay()
-    torch.cuda.synchronize()
-    a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    a.record()
-    for _ in range(replays):
-        g.replay()
-    b.record()
-    torch.cuda.synchronize()
-    return 1000.0 * a.elapsed_time(b) / (replays * reps)
 
 
 def kernel_times(c_in):
@@ -81,9 +52,9 @@ def kernel_times(c_in):
     floats = sum(P[n + ".weight_orig"].numel() for n in names)
     with torch.no_grad():
         out = {"layers": len(names), "weight_MB": round(4 * floats / 1e6, 2),
-               "iterate_us": graph_time_us(lambda: eng.spectral_norm(P, True)),
-               "fixed_us": graph_time_us(lambda: eng.spectral_norm(P, False)),
-               "bwd_us": graph_time_us(lambda: eng.spectral_norm_bwd(P, G))}
+               "iterate_us": graph_us(lambda: eng.spectral_norm(P, True), 50, 20),
+               "fixed_us": graph_us(lambda: eng.spectral_norm(P, False), 50, 20),
+               "bwd_us": graph_us(lambda: eng.spectral_norm_bwd(P, G), 50, 20)}
     return out
 
 
@@ -104,11 +75,7 @@ def step_times(c_in, batch, steps, windows):
     ms = {False: [], True: []}
     for _ in range(windows):
         for sn in (False, True):
-            torch.cuda.synchronize()
-            t0 = time.perf_counter()
-            solvers[sn].run_steps(steps)
-            torch.cuda.synchronize()
-            ms[sn].append(1000.0 * (time.perf_counter() - t0) / steps)
+            ms[sn].append(1000.0 * median_wall_s(lambda: solvers[sn].run_steps(steps), 1, warmup=0) / steps)
     med = {sn: sorted(v)[len(v) // 2] for sn, v in ms.items()}
     return {"c_in": c_in, "batch": batch, "steps_per_window": steps, "sn_false_ms": ms[False], "sn_true_ms": ms[True],
             "median_sn_false_ms": med[False], "median_sn_true_ms": med[True],

@@ -30,11 +30,10 @@ import time
 import numpy as np
 import torch
 
+from _harness import card, median_events_s
+
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "tools"))
-
-from bench_mcd import card, timed  # noqa: E402
 
 FP64_PEAK = 33.5e12      # H100 SXM data sheet, FP64 (non-tensor), FMA counted as two
 HBM_PEAK = 3.35e12
@@ -64,7 +63,7 @@ def eer_kernel(n, d):
     V = torch.from_numpy((centres[labels] + rng.standard_normal((n, d))).astype(np.float32)).cuda()
     ws = S.eer_workspace(n, "cuda")
     res = S.eer(V, labels, ws)
-    t = timed(lambda: S.eer(V, labels, ws))
+    t = median_events_s(lambda: S.eer(V, labels, ws), 3)
     k = kernel_times(lambda: S.eer(V, labels, ws))
     pick = lambda name: sum(v for kk, v in k.items() if name in kk)
     trials = n * (n - 1) // 2
@@ -87,13 +86,13 @@ def pooling():
     rng = np.random.default_rng(0)
     lens = rng.integers(100, 601, 64)
     x = torch.randn(64, 512, 640, device="cuda")
-    t = timed(lambda: S.time_stats(x, lens), reps=5)
+    t = median_events_s(lambda: S.time_stats(x, lens), 5)
     lx = torch.from_numpy(lens.astype(np.int32)).cuda()
     from adaptive_voice_conversion_b200 import _lib as L
     out = torch.empty(64, 1024, device="cuda")
     launch = lambda: L.load().avc_time_stats_varlen(x.data_ptr(), out.data_ptr(), 64, 512, 640, lx.data_ptr(),
                                                     torch.cuda.current_stream().cuda_stream)
-    t_k = timed(launch, reps=5)
+    t_k = median_events_s(launch, 5)
     read = 2 * int(lens.sum()) * 512 * 4
     return {"batch": 64, "channels": 512, "extent": 640, "wrapper_s": t, "kernel_s": t_k,
             "bytes_read_per_s": read / t_k}

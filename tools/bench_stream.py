@@ -34,7 +34,6 @@ import dataclasses
 import json
 import math
 import os
-import subprocess
 import sys
 import types
 
@@ -45,15 +44,8 @@ sys.path.insert(0, os.path.join(ROOT, "tests"))
 import numpy as np  # noqa: E402
 import torch  # noqa: E402
 
+from _harness import card, median_events_s  # noqa: E402
 from adaptive_voice_conversion_b200 import _lib as L  # noqa: E402
-
-
-def card():
-    try:
-        return subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                              capture_output=True, text=True, timeout=30).stdout.strip().splitlines()[0]
-    except Exception as e:   # noqa: BLE001
-        return f"unknown ({e})"
 
 
 def harmonic(n, sr, seed):
@@ -82,19 +74,12 @@ def yin_window_ms(n_streams, hp, dev, frames=8, origin=40):
     out = torch.empty(3, n_streams * frames, dtype=torch.float64, device=dev)
     d = L.AudioDesc(hop=hp.hop_length, n_seg=n_streams, n_frames=n_streams * frames, n_samples=int(y.numel()),
                     segs=_ptr(table), y=_ptr(y))
-    ev = [torch.cuda.Event(enable_timing=True) for _ in range(2)]
-    times = []
-    for i in range(8):
-        torch.cuda.synchronize()
-        ev[0].record()
+
+    def launch():
         L.check(L.load().avc_yin_window(C.byref(d), fp.win, fp.tau_min(hp.sr), fp.tau_max(hp.sr),
                                         C.c_float(fp.threshold), _ptr(out[0]), _ptr(out[1]), _ptr(out[2]),
                                         _stream(dev)), "avc_yin_window")
-        ev[1].record()
-        torch.cuda.synchronize()
-        if i:
-            times.append(ev[0].elapsed_time(ev[1]))
-    return sorted(times)[len(times) // 2]
+    return 1e3 * median_events_s(launch, 7)
 
 
 def main():
@@ -210,16 +195,7 @@ def main():
             n_iter = 16
             utts = [torch.rand(max(8, frames // 64), hp.n_bins, device=dev) for _ in range(64)]
             gl = GriffinLim(utts, hp, n_iter=n_iter)
-            gl.run()
-            times = []
-            for _ in range(7):
-                torch.cuda.synchronize()
-                ev[0].record()
-                gl.run()
-                ev[1].record()
-                torch.cuda.synchronize()
-                times.append(ev[0].elapsed_time(ev[1]))
-            gl_ms = sorted(times)[len(times) // 2]
+            gl_ms = 1e3 * median_events_s(gl.run, 7)
             gl_ffts = sum(u.shape[0] for u in utts) * (2 * n_iter + 1)
             res["rtisi_kernel"] = {"streams": S, "ms": rt_ms, "fft_per_s": ffts / (rt_ms * 1e-3),
                                    "gl_ms": gl_ms, "gl_fft_per_s": gl_ffts / (gl_ms * 1e-3)}

@@ -24,7 +24,6 @@ import argparse
 import json
 import os
 import statistics
-import subprocess
 import sys
 import time
 import types
@@ -35,13 +34,9 @@ sys.path.insert(0, ROOT)
 import numpy as np  # noqa: E402
 import torch  # noqa: E402
 
+from _harness import card, events_ms, median_wall_s  # noqa: E402
+
 HBM_BPS = 3.35e12
-
-
-def card():
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                       capture_output=True, text=True).stdout.strip().splitlines()
-    return q[torch.cuda.current_device()] if q else torch.cuda.get_device_name()
 
 
 def utterances(n_utt, n_samples, seed=0):
@@ -57,19 +52,6 @@ def utterances(n_utt, n_samples, seed=0):
     return out
 
 
-def timed(fn, windows, reps):
-    fn()
-    torch.cuda.synchronize()
-    ts = []
-    for _ in range(windows):
-        t0 = time.perf_counter()
-        for _ in range(reps):
-            fn()
-        torch.cuda.synchronize()
-        ts.append((time.perf_counter() - t0) / reps)
-    return statistics.median(ts), ts
-
-
 def gl_bytes_per_iteration(F, n_samples, win, bins, momentum=False):
     """Least HBM traffic of one iteration: iSTFT frames read X and write the windowed frames, the overlap-add reads
     them and writes the signal, the projecting STFT reads the signal and S and writes the next X; with momentum it
@@ -78,21 +60,9 @@ def gl_bytes_per_iteration(F, n_samples, win, bins, momentum=False):
             + (2 * F * bins * 8 if momentum else 0))
 
 
-def event_time(fn, reps):
-    fn()
-    torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(reps):
-        fn()
-    e1.record()
-    torch.cuda.synchronize()
-    return e0.elapsed_time(e1) / 1e3 / reps
-
-
 def gl_kernel_time(V, mags, hp, n_iter, momentum=0.0, reps=5):
     plan = V.GriffinLim(mags, hp, n_iter, momentum)
-    return event_time(plan.run, reps)
+    return events_ms(plan.run, reps, 1, sync=True) / 1e3
 
 
 def spectral_convergence(V, mags, ys):
@@ -124,8 +94,8 @@ def gl_stage_times(V, L, mags, hp, reps=20):
     d_istft = L.AudioDesc.from_buffer_copy(plan.desc)
     d_stft = L.AudioDesc.from_buffer_copy(plan.desc)
     d_stft.mode = L.STFT_PROJECT
-    t_istft = event_time(lambda: V._call("avc_istft", d_istft, plan.dev), reps)
-    t_stft = event_time(lambda: V._call("avc_stft", d_stft, plan.dev), reps)
+    t_istft = events_ms(lambda: V._call("avc_istft", d_istft, plan.dev), reps, 1, sync=True) / 1e3
+    t_stft = events_ms(lambda: V._call("avc_stft", d_stft, plan.dev), reps, 1, sync=True) / 1e3
     return t_istft, t_stft
 
 
@@ -155,7 +125,7 @@ def main():
     wavs = utterances(a.utts, n_samples)
     res = {"card": card(), "utts": a.utts, "frames": a.frames, "audio_seconds": round(audio_s, 3), "n_iter": hp0.n_iter,
            "momentum": a.momentum, "signals": "synthetic (vibrato tones with harmonics and a noise floor)"}
-    print(f"card (name, power limit, max SM clock): {res['card']}", file=sys.stderr)
+    print(f"card: {res['card']}", file=sys.stderr)
     iters = sorted(set(a.sc_iters) | {100})
     momenta = (0.0, a.momentum)
     consistent = [A for A, _ in V.magnitude(wavs, hp0)]
@@ -177,9 +147,10 @@ def main():
             tgt = src[1:] + src[:1]
             return voc.mel_to_wav(inf.inference_ragged(src, tgt), n_iter, momentum)
 
-        t_ana, w_ana = timed(lambda: voc.wav_to_mel(wavs), a.windows, a.reps)
-        t_syn, w_syn = timed(lambda: voc.mel_to_wav(mels), a.windows, a.reps)
-        t_cnv, w_cnv = timed(convert, a.windows, 1)
+        w_ana, w_syn, w_cnv = [], [], []
+        t_ana = median_wall_s(lambda: voc.wav_to_mel(wavs), a.windows, a.reps, samples=w_ana)
+        t_syn = median_wall_s(lambda: voc.mel_to_wav(mels), a.windows, a.reps, samples=w_syn)
+        t_cnv = median_wall_s(convert, a.windows, samples=w_cnv)
         mags = voc.mel_to_mag(mels)
         t100 = gl_kernel_time(V, mags, hp, hp.n_iter)
         t0 = gl_kernel_time(V, mags, hp, 0)
@@ -197,7 +168,8 @@ def main():
                 "gl_iteration_TBps": nbytes_m / per_it_m / 1e12, "gl_iteration_vs_plain": per_it_m / per_it,
                 "sc_mel_pseudo_inverse": sc_mel, "fewest_iters_at_or_below_plain_100": n_fast}
         if n_fast is not None:
-            t_fast, w_fast = timed(lambda: convert(n_fast, a.momentum), a.windows, 1)
+            w_fast = []
+            t_fast = median_wall_s(lambda: convert(n_fast, a.momentum), a.windows, samples=w_fast)
             fast["conversion"] = {"n_iter": n_fast, "utt_per_s": a.utts / t_fast, "audio_s_per_s": audio_s / t_fast,
                                   "windows_s": w_fast}
         res[f"mels{n_mels}"] = {

@@ -12,13 +12,15 @@ SM clock are printed with the table.
 """
 import argparse
 import ctypes as C
+import itertools
 import json
 import os
-import subprocess
 import sys
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch  # noqa: E402
+
+from _harness import card, graph_us  # noqa: E402
 
 TF32_PEAK = 495.0     # TFLOP/s, H100 SXM data sheet, dense, 700 W
 L2_BYTES = 50 << 20
@@ -107,38 +109,16 @@ def time_descriptor(e, d, dev, reps):
         q = L.WgradDesc.from_buffer_copy(d)
         q.x, q.dc, q.dw = xs[i].data_ptr(), dcs[i].data_ptr(), dw.data_ptr()
         descs.append(q)
-    side = torch.cuda.Stream(dev)
+    n = itertools.count()
 
-    def launch(i, stream):
-        e._ck(lib.avc_conv_wgrad_tc(C.byref(descs[i % nset]), scratch.data_ptr(), e.tc_status.data_ptr(), stream), "avc_conv_wgrad_tc")
-
-    with torch.cuda.stream(side):
-        for i in range(3):
-            launch(i, side.cuda_stream)
-        side.synchronize()
-        g = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(g, stream=side):
-            for i in range(reps):
-                launch(i, side.cuda_stream)
-        g.replay()
-        side.synchronize()
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record(side)
-        for _ in range(5):
-            g.replay()
-        e1.record(side)
-        side.synchronize()
+    def launch():
+        e._ck(lib.avc_conv_wgrad_tc(C.byref(descs[next(n) % nset]), scratch.data_ptr(), e.tc_status.data_ptr(),
+                                    torch.cuda.current_stream().cuda_stream), "avc_conv_wgrad_tc")
+    launch()
+    launch()
+    us = graph_us(launch, reps, 5)
     e.check_tc_status()
-    return e0.elapsed_time(e1) * 1e3 / (5 * reps)
-
-
-def card():
-    q = "name,power.limit,clocks.sm,clocks.max.sm"
-    try:
-        out = subprocess.run(["nvidia-smi", f"--query-gpu={q}", "--format=csv,noheader"], capture_output=True, text=True, timeout=30).stdout
-        return out.strip().splitlines()[0]
-    except Exception as ex:   # the table is still valid without it; say so
-        return f"{torch.cuda.get_device_name(0)} (nvidia-smi unavailable: {ex})"
+    return us
 
 
 def main():
@@ -150,8 +130,8 @@ def main():
     ap.add_argument("--json", default=None)
     args = ap.parse_args()
     dev = torch.device("cuda", 0)
-    result = {"card (name, power limit, SM clock, max SM clock)": card(), "configs": {}}
-    print(f"card: {result['card (name, power limit, SM clock, max SM clock)']}")
+    result = {"card": card(dev), "configs": {}}
+    print(f"card: {result['card']}")
     for c_in in args.c_in:
         e, launches = step_descriptors(c_in, args.batch, args.seg, dev)
         count, first = {}, {}
