@@ -210,7 +210,7 @@ class CodeAdamDesc(C.Structure):
 
 
 PCM_S16, PCM_F32 = 0, 1
-RESAMPLE_TILE, RESAMPLE_MAX_TAPS, RESAMPLE_MAX_PHASE_TAPS = 512, 8192, 96
+RESAMPLE_TILE, RESAMPLE_MAX_TAPS, RESAMPLE_MAX_PHASE_TAPS = 512, 32768, 256
 
 
 class ResampleSeg(C.Structure):

@@ -8,6 +8,7 @@ namespace {
 
 constexpr int RS_TILE = AVC_RESAMPLE_TILE;
 constexpr int RS_THREADS = 256;
+constexpr size_t RS_SMEM = 48 * 1024;   // shared memory of one CTA without an opt-in
 constexpr int MOM_THREADS = 128;
 
 // the channel mean of sample k of an utterance
@@ -36,11 +37,14 @@ int window_floats(const avc_resample_desc& d) {
   return (int)(((int64_t)(RS_TILE - 1) * d.down) / d.up) + d.n_taps + 1;
 }
 
-// One CTA per tile of RS_TILE outputs of one utterance: the tap table and the tile's input window (converted to float,
-// channels averaged, zero outside the utterance) are staged in shared memory; each output is then one fixed-order dot
-// product of its phase's taps with the window, newest sample first.
+// One CTA per tile of RS_TILE outputs of one utterance: the tile's input window (converted to float, channels
+// averaged, zero outside the utterance) is staged in shared memory, and so is the tap table when both fit RS_SMEM
+// (staged); a larger table is read through L1 instead.  Each output is then one fixed-order dot product of its
+// phase's taps with the window, newest sample first: the same sum, in the same order, either way.  `staged` is one
+// value for the whole launch, so the branch on it sits outside the tap loop.  Tile bounds are int64: the last tile of
+// an utterance of n_out >= 2^31 - RS_TILE + 1 outputs ends past INT_MAX.
 template <int FMT>
-__global__ void __launch_bounds__(RS_THREADS) resample_poly_kernel(const avc_resample_desc d) {
+__global__ void __launch_bounds__(RS_THREADS) resample_poly_kernel(const avc_resample_desc d, const bool staged) {
   extern __shared__ float sm[];
   int lo = 0, hi = d.n_seg - 1;
   while (lo < hi) {
@@ -48,33 +52,38 @@ __global__ void __launch_bounds__(RS_THREADS) resample_poly_kernel(const avc_res
     if (__ldg(&d.segs[mid].tile0) <= (int)blockIdx.x) lo = mid; else hi = mid - 1;
   }
   const avc_resample_seg g = d.segs[lo];
-  const int m0 = ((int)blockIdx.x - g.tile0) * RS_TILE;
-  const int m1 = min(g.n_out, m0 + RS_TILE);
-  float* out = d.out + g.out_off;
+  const int64_t m0 = (int64_t)((int)blockIdx.x - g.tile0) * RS_TILE;
+  const int64_t m1 = min((int64_t)g.n_out, m0 + RS_TILE);
+  const int n = (int)(m1 - m0);   // outputs of this tile, <= RS_TILE
+  float* out = d.out + g.out_off + m0;
   if (d.up == 1 && d.down == 1) {
-    for (int m = m0 + threadIdx.x; m < m1; m += RS_THREADS) out[m] = pcm_mono<FMT>(d.pcm, g.in_off + (int64_t)m * g.channels, g.channels);
+    for (int j = threadIdx.x; j < n; j += RS_THREADS) out[j] = pcm_mono<FMT>(d.pcm, g.in_off + (m0 + j) * g.channels, g.channels);
     return;
   }
-  const int ntab = d.up * d.n_taps;
-  float* tab = sm;
+  const int ntab = staged ? d.up * d.n_taps : 0;
   float* win = sm + ntab;
   const int64_t kw0 = window_first(m0, d);
-  const int nw = (int)(((int64_t)(m1 - 1) * d.down + d.half_len) / d.up - kw0) + 1;
-  for (int i = threadIdx.x; i < ntab; i += RS_THREADS) tab[i] = __ldg(d.taps + i);
+  const int nw = (int)(((m1 - 1) * d.down + d.half_len) / d.up - kw0) + 1;
+  for (int i = threadIdx.x; i < ntab; i += RS_THREADS) sm[i] = __ldg(d.taps + i);
   for (int w = threadIdx.x; w < nw; w += RS_THREADS) {
     const int64_t k = kw0 + w;
     win[w] = (k >= 0 && k < g.n_in) ? pcm_mono<FMT>(d.pcm, g.in_off + k * g.channels, g.channels) : 0.f;
   }
   __syncthreads();
-  for (int m = m0 + threadIdx.x; m < m1; m += RS_THREADS) {
-    const int64_t p = (int64_t)m * d.down + d.half_len;
+  for (int j = threadIdx.x; j < n; j += RS_THREADS) {
+    const int64_t p = (m0 + j) * d.down + d.half_len;
     const int r = (int)(p % d.up);
     const int cnt = (2 * d.half_len - r) / d.up + 1;
-    const float* t = tab + r * d.n_taps;
     const float* x = win + (p / d.up - kw0);
     float acc = 0.f;
-    for (int i = 0; i < cnt; ++i) acc = fmaf(x[-i], t[i], acc);
-    out[m] = acc;
+    if (staged) {
+      const float* t = sm + r * d.n_taps;
+      for (int i = 0; i < cnt; ++i) acc = fmaf(x[-i], t[i], acc);
+    } else {
+      const float* t = d.taps + (int64_t)r * d.n_taps;
+      for (int i = 0; i < cnt; ++i) acc = fmaf(x[-i], __ldg(t + i), acc);
+    }
+    out[j] = acc;
   }
 }
 
@@ -147,12 +156,17 @@ extern "C" int avc_resample_poly(const avc_resample_desc* d, void* stream) {
                 d->up, d->down, d->n_taps, (long long)d->up * d->n_taps, AVC_RESAMPLE_MAX_PHASE_TAPS, AVC_RESAMPLE_MAX_TAPS);
   }
   if (d->n_tiles == 0) return AVC_OK;
-  const size_t smem = identity ? 0 : sizeof(float) * ((size_t)d->up * d->n_taps + window_floats(*d));
-  AVC_REQUIRE(smem <= 48 * 1024, AVC_ERR_UNSUPPORTED, "avc_resample_poly: up %d / down %d needs %zu bytes of shared memory",
+  // the window is at most 511 down/up + n_taps + 1 floats, under 6 800 within the limits above; the table joins it in
+  // shared memory when both fit
+  const size_t win_bytes = identity ? 0 : sizeof(float) * window_floats(*d);
+  const size_t tab_bytes = identity ? 0 : sizeof(float) * d->up * d->n_taps;
+  const bool staged = win_bytes + tab_bytes <= RS_SMEM;
+  const size_t smem = win_bytes + (staged ? tab_bytes : 0);
+  AVC_REQUIRE(smem <= RS_SMEM, AVC_ERR_UNSUPPORTED, "avc_resample_poly: up %d / down %d needs %zu bytes of shared memory",
               d->up, d->down, smem);
   cudaStream_t st = (cudaStream_t)stream;
-  if (d->format == AVC_PCM_S16) resample_poly_kernel<AVC_PCM_S16><<<d->n_tiles, RS_THREADS, smem, st>>>(*d);
-  else resample_poly_kernel<AVC_PCM_F32><<<d->n_tiles, RS_THREADS, smem, st>>>(*d);
+  if (d->format == AVC_PCM_S16) resample_poly_kernel<AVC_PCM_S16><<<d->n_tiles, RS_THREADS, smem, st>>>(*d, staged);
+  else resample_poly_kernel<AVC_PCM_F32><<<d->n_tiles, RS_THREADS, smem, st>>>(*d, staged);
   AVC_CHECK_LAUNCH("avc_resample_poly");
   return AVC_OK;
 }

@@ -153,6 +153,28 @@ def resample_taps(up, down):
     return half, np.ascontiguousarray(padded.reshape(n_taps, up).T)
 
 
+def resample_supported(up, down):
+    """Whether avc_resample_poly takes the pair: up = down = 1, or a tap table within RESAMPLE_MAX_PHASE_TAPS taps per
+    phase and RESAMPLE_MAX_TAPS in all (resample_taps' shape, without designing the filter)."""
+    if (up, down) == (1, 1):
+        return True
+    n_taps = -(-(20 * max(up, down) + 1) // up)
+    return n_taps <= L.RESAMPLE_MAX_PHASE_TAPS and up * n_taps <= L.RESAMPLE_MAX_TAPS
+
+
+def check_rates(sets, sample_rate):
+    """Reads every header of every set ({name: paths}) and raises ValueError naming the first file whose rate the
+    resampler cannot take to sample_rate, so that a run stops before it analyses or writes any set."""
+    for paths in sets.values():
+        for p in paths:
+            rate = int(_header(p)[0])
+            if not resample_supported(*rate_pair(rate, sample_rate)):
+                up, down = rate_pair(rate, sample_rate)
+                raise ValueError(f"{p}: a file at {rate} Hz cannot be resampled to --sample_rate {sample_rate} (up {up} / "
+                                 f"down {down} needs more than {L.RESAMPLE_MAX_PHASE_TAPS} taps per phase or "
+                                 f"{L.RESAMPLE_MAX_TAPS} in all)")
+
+
 def n_resampled(n, up, down):
     return -(-n * up // down)
 
@@ -368,7 +390,11 @@ def _load(path):
 def _features(sets, out_dir, cache, n_mels, sample_rate, n_utts_attr, chunk_seconds, device, timer, log):
     """Stage 0's features: each set of `sets` ({name: paths in processing order}, "train" first) analysed in that
     order; attr.pkl over the first n_utts_attr analysed training utterances; every set normalised by it and pickled
-    (and kept in `cache`); the skipped files in skipped_files.txt."""
+    (and kept in `cache`); the skipped files in skipped_files.txt.  Every file's rate is checked first (check_rates):
+    the sets run one after another, and a file the resampler refuses would otherwise end the run only when its set's
+    turn comes, after the training set has been processed."""
+    with timer.host("headers"):
+        check_rates(sets, sample_rate)
     prep = Preparer(n_mels, sample_rate, device, timer)
     chunk = max(1, int(chunk_seconds * sample_rate))
     skipped, mean = [], None

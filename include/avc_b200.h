@@ -790,12 +790,14 @@ int avc_mel_project(const avc_mel_desc* d, void* stream);
  * up = down = 1: y = x (conversion and channel mix only; taps may be null).
  * AVC_ERR_INVALID for null pointers, n_seg < 1, n_tiles < 0, up/down < 1, an unknown format, or a tap table whose shape
  * is not the one above; AVC_ERR_UNSUPPORTED for tables of more than AVC_RESAMPLE_MAX_TAPS floats or
- * AVC_RESAMPLE_MAX_PHASE_TAPS taps per phase.  The kernel trusts the utterance table (offsets inside the buffers). */
+ * AVC_RESAMPLE_MAX_PHASE_TAPS taps per phase.  Within them every pair of the file rates 8, 11.025, 12, 16, 22.05, 24, 32,
+ * 44.1, 48, 88.2, 96, 176.4 and 192 kHz to the targets 16, 22.05, 24, 44.1 and 48 kHz is taken (at most 25 725 floats
+ * and 241 taps per phase).  The kernel trusts the utterance table (offsets inside the buffers). */
 #define AVC_PCM_S16 0 /* int16, scaled by 1/32768 */
 #define AVC_PCM_F32 1 /* float32 as is */
-#define AVC_RESAMPLE_TILE 512          /* output samples per CTA */
-#define AVC_RESAMPLE_MAX_TAPS 8192     /* up * n_taps */
-#define AVC_RESAMPLE_MAX_PHASE_TAPS 96 /* n_taps */
+#define AVC_RESAMPLE_TILE 512            /* output samples per CTA */
+#define AVC_RESAMPLE_MAX_TAPS 32768      /* up * n_taps */
+#define AVC_RESAMPLE_MAX_PHASE_TAPS 256  /* n_taps */
 typedef struct avc_resample_seg {
   int64_t in_off;    /* first PCM element of the utterance (element = one channel's sample) */
   int64_t out_off;   /* first output sample */

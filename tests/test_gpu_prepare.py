@@ -86,7 +86,7 @@ def test_resampler_matches_resample_poly_and_is_batch_invariant():
         assert np.array_equal(bits(alone), bits(got[i])), items[i][0]
 
 
-def test_resampler_rejects_invalid_arguments():
+def test_resampler_rejects_invalid_arguments_and_tables_past_its_limits():
     lib = L.load()
     prep = P.Preparer(N_MELS, SR)
     half, n_taps, taps = prep.taps(1, 2)
@@ -100,8 +100,8 @@ def test_resampler_rejects_invalid_arguments():
                ({"n_seg": 0}, "empty table"), ({"n_tiles": -1}, "empty table"), ({"format": 7}, "unknown format"),
                ({"up": 0}, "must be >= 1"), ({"down": -2}, "must be >= 1"), ({"taps": None}, "null tap table"),
                ({"half_len": half + 1}, "tap table"), ({"n_taps": n_taps - 1}, "tap table")]
-    unsupported = [({"up": 1, "down": 5, "half_len": 50, "n_taps": 101}, "taps per phase"),
-                   ({"up": 441, "down": 80, "half_len": 4410, "n_taps": 21}, "taps per phase")]
+    unsupported = [({"up": 5, "down": 64, "half_len": 640, "n_taps": 257}, "taps per phase"),
+                   ({"up": 331, "down": 1638, "half_len": 16380, "n_taps": 99}, "taps per phase")]
     n0 = L.launch_count()
     for cases, code in ((invalid, L.ERR_INVALID), (unsupported, L.ERR_UNSUPPORTED)):
         for patch, msg in cases:

@@ -17,8 +17,9 @@ from adaptive_voice_conversion_b200 import _lib as L
 from adaptive_voice_conversion_b200 import prepare as P
 from conftest import ROOT
 
-# the rates a user meets, each to 24 kHz
-RATES = [8000, 11025, 16000, 22050, 24000, 32000, 44100, 48000, 88200, 96000]
+# the file rates a user meets, each to every target rate --sample_rate is meant for
+RATES = [8000, 11025, 12000, 16000, 22050, 24000, 32000, 44100, 48000, 88200, 96000, 176400, 192000]
+TARGETS = [16000, 22050, 24000, 44100, 48000]
 
 
 def write_tree(root, speakers):
@@ -126,15 +127,49 @@ def test_index_sampling_of_a_set_without_long_utterances_raises():
 
 # ------------------------------------------------------------------ resampler
 def pairs():
-    return sorted({P.rate_pair(r, 24000) for r in RATES} - {(1, 1)})
+    return sorted({P.rate_pair(r, sr) for r in RATES for sr in TARGETS} - {(1, 1)})
 
 
 def test_supported_rates_fit_the_kernel_limits():
     for up, down in pairs():
         half, tab = P.resample_taps(up, down)
         assert tab.shape[1] <= L.RESAMPLE_MAX_PHASE_TAPS and tab.size <= L.RESAMPLE_MAX_TAPS, (up, down, tab.shape)
-    assert max(P.resample_taps(*p)[1].size for p in pairs()) == 6720
-    assert max(P.resample_taps(*p)[1].shape[1] for p in pairs()) == 81
+        assert P.resample_supported(up, down)
+    assert max(P.resample_taps(*p)[1].size for p in pairs()) == 25725          # 192 kHz -> 22.05 kHz
+    assert max(P.resample_taps(*p)[1].shape[1] for p in pairs()) == 241        # 192 kHz -> 16 kHz
+
+
+# (up, down) whose tap table is exactly at a limit, and one past it
+LIMIT_PAIRS = {(4, 51): (256, 1024), (128, 1633): (256, 32768), (5, 64): (257, 1285), (331, 1638): (99, 32769)}
+
+
+@pytest.mark.parametrize("up, down", sorted(LIMIT_PAIRS))
+def test_limit_pairs_have_the_tables_they_are_meant_to(up, down):
+    half, tab = P.resample_taps(up, down)
+    assert tab.shape[1::-1] == LIMIT_PAIRS[(up, down)][:1] + (up,) and tab.size == LIMIT_PAIRS[(up, down)][1]
+    fits = tab.shape[1] <= L.RESAMPLE_MAX_PHASE_TAPS and tab.size <= L.RESAMPLE_MAX_TAPS
+    assert P.resample_supported(up, down) == fits == ((up, down) in ((4, 51), (128, 1633)))
+
+
+def test_a_refused_rate_stops_the_run_before_any_set_is_analysed(tmp_path):
+    """44 056 Hz to 16 kHz is up 2000 / down 5507: 56 taps per phase, 112 000 in all.  The file is in out_test, the
+    last set processed; the run must name it before it analyses the training set."""
+    from scipy.io import wavfile
+    wav = tmp_path / "wav"
+    for spk in ("225", "226", "227"):
+        os.makedirs(wav / f"p{spk}")
+        for i in range(3):
+            wavfile.write(str(wav / f"p{spk}" / f"p{spk}_{i + 1:03d}.wav"), 48000, np.zeros(4800, np.int16))
+    info = tmp_path / "speaker-info.txt"
+    info.write_text("ID  AGE\n225  23\n226  22\n227  21\n")
+    out = tmp_path / "out"
+    train, _, out_test = P.split_files(["225", "226", "227"], P.read_filenames(str(wav)), 1, 0.34, 0)
+    bad = sorted(out_test)[-1]
+    wavfile.write(bad, 44056, np.zeros(4800, np.int16))
+    with pytest.raises(ValueError, match=re.escape(bad) + ".*44056 Hz.*--sample_rate 16000"):
+        P.run(str(wav), str(info), str(out), n_out_speakers=1, test_prop=0.34, sample_rate=16000, log=lambda *a: None)
+    assert not [f for f in os.listdir(out) if f.endswith(".pkl")]
+    assert not P.resample_supported(*P.rate_pair(44056, 16000))
 
 
 @pytest.mark.parametrize("up, down", pairs())

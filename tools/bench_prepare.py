@@ -13,6 +13,9 @@ are CUDA events around their launches, summed over chunks.  End to end is one ru
 run less the timed stages 1-3 (reduce, index sampling).  "headers" is the first pass over the files (their lengths,
 for the chunk planner); "decode" is the full read of each chunk's files.  avc_resample_poly's traffic is 2 bytes read
 per input sample and 4 written per output sample (plus its tap table and the staged windows' overlap, not counted).
+"resample_pairs" times avc_resample_poly alone on 10 minutes of 3 s int16 files at 48 kHz -> 24 kHz, whose tap table
+is staged in shared memory, and at 11.025 kHz -> 48 kHz, whose table (13 440 floats) does not fit beside the window and
+is read through L1: the median of 7 calls of Preparer.resample's launches, CUDA events.
 The card's name, power limit and clock are read in the same run.
 """
 import argparse
@@ -109,6 +112,33 @@ def write_libri_corpus(root, n_utts, n_speakers, seed):
     return libri, np.array(n_in, np.int64)
 
 
+RESAMPLE_PAIRS = [(48000, 24000), (11025, 48000)]
+
+
+def resample_pairs(seed, seconds=600.0, reps=7):
+    """{"<rate>-><target>": ms, traffic and whether the tap table is staged} of avc_resample_poly per RESAMPLE_PAIRS."""
+    out = {}
+    for rate, sr in RESAMPLE_PAIRS:
+        rng = np.random.default_rng(seed)
+        items = [(rate, synth_pcm(rng, rate)[:3 * rate]) for _ in range(int(seconds // 3))]
+        prep = P.Preparer(80, sr)
+        prep.resample(items)
+        ts = []
+        for _ in range(reps):
+            prep.timer = Timer()
+            prep.resample(items)
+            ts.append(prep.timer.device_s()["resample"])
+        up, down = P.rate_pair(rate, sr)
+        half, tab = P.resample_taps(up, down)
+        window = 511 * down // up + tab.shape[1] + 1
+        n_in = sum(a.size for _, a in items)
+        n_bytes = 2 * n_in + 4 * sum(P.n_resampled(a.size, up, down) for _, a in items)
+        t = float(np.median(ts))
+        out[f"{rate}->{sr}"] = {"up_down": [up, down], "taps": int(tab.size), "staged_taps": 4 * (tab.size + window) <= 48 * 1024,
+                                "ms": round(1e3 * t, 3), "GB_per_s": round(n_bytes / t / 1e9, 1)}
+    return out
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--corpus", choices=("vctk", "libri"), default="vctk")
@@ -174,6 +204,7 @@ def main():
             voc.get_spectrograms(p)
         t_base = time.perf_counter() - t0
 
+        pairs = resample_pairs(a.seed)
         res = {
             "card": card(),
             "corpus": a.corpus, "files": a.utts, "audio_hours": round(float(audio_s) / 3600, 3), "n_mels": a.n_mels,
@@ -182,6 +213,7 @@ def main():
             "device_s": {k: round(v, 4) for k, v in dev.items()},
             "resample": {"bytes": rs_bytes, "GB_per_s": round(rs_bytes / dev["resample"] / 1e9, 1),
                          "share_of_3.35TB_per_s": round(rs_bytes / dev["resample"] / HBM_BYTES_PER_S, 3)},
+            "resample_pairs": pairs,
             "stage0_s": round(t_features, 2),
             "stage0_without_pickling_s": round(t_no_pickle, 2),
             "stages1_3_s": round(t_index, 2),
